@@ -1,6 +1,7 @@
 """STA image-pairs/s benchmark (BASELINE.json metric) -- contract: see the task statement / DESIGN.md.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--pairs P] [--height H] [--width W]
+                    [--dump-outputs DIR]
 
 * b200 arm (default): one process per GPU (torchrun sets RANK/LOCAL_RANK/WORLD_SIZE).  Rank 0 initialises the
   weights, one NCCL broadcast of the packed weight arena, then every rank runs `--pairs` synthetic
@@ -9,8 +10,12 @@
   `e2e`     = the same metric through the host-buffer C-ABI call sta_forward_pairs_host: pinned-host ->
               device copies of both image batches and device -> host copies of all four outputs are
               inside the timed region.
-  `roofline`= tensor-pipe roofline of the dominant kernel family (tcgen05 GEMM / implicit-GEMM conv),
+  `roofline`= tensor-pipe roofline of the dominant kernel family (wgmma GEMM / implicit-GEMM conv),
               timed live with CUDA events on the launch stream (sta_profile).
+  `--dump-outputs DIR` writes what the last timed step returned on rank 0 -- with --gpus N > 1 that is rank 0's own
+              pair shard only -- as DIR/<view>_<output>.npy, float32: the
+              pose outputs whole, the dense maps as a fixed seeded sample (DUMP_SAMPLE elements each), so that two
+              builds can be compared output for output on identical inputs (seeded images and weights).
   `cpu_baseline` = the oracle (PyTorch fp32 CPU port of the reference, oracle/sta_oracle.py) timed on the
               host cores on a bounded sample (rank 0, N=1 only).
 * reference arm (`--impl reference`): the reference's own CPU implementation of the path = the oracle
@@ -44,14 +49,14 @@ def make_config(P, world, H, W, total=None):
                 "pairs_per_gpu": max(b - a for a, b in shards), "global_pairs": total, "height": H, "width": W,
                 "parallelism": "contiguous pair shard per rank (vista_slam_b200/dist.py::pair_shard), 1 NCCL weight broadcast, "
                                "no data-path collective",
-                "l2_policy": "no explicit flush: weights (0.88 GB) + activations exceed the 126 MB L2",
+                "l2_policy": "no explicit flush: weights (0.88 GB) + activations exceed the 50 MB L2",
                 "gflop_per_pair": flops_per_pair(H, W) / 1e9}
     return {"workload": "cfg-2: %d synthetic %dx%d bf16 pairs per GPU per step, STA forward only "
                         "(2 enc + symmetric dec + 2 DPT + 2 pose heads per pair), random-init weights" % (P, W, H),
             "pairs_per_gpu": P, "global_pairs": P * world, "height": H, "width": W,
             "parallelism": "pair shard per rank, 1 NCCL weight broadcast, no data-path collective",
             "l2_policy": "no explicit flush: per-step working set (0.88 GB weights + >2 GB activations) "
-                         "exceeds the 126 MB L2",
+                         "exceeds the 50 MB L2",
             "gflop_per_pair": flops_per_pair(H, W) / 1e9}
 
 
@@ -61,7 +66,8 @@ def load_peaks():
         d = json.load(open(p))
         return {"bf16_burst": d.get("bf16_tflops"), "bf16_sustained": d.get("bf16_tflops_sustained"),
                 "hbm_gbs": d.get("hbm_gbs"), "source": "measured (MEASURED_PEAKS.json)"}
-    return {"bf16_burst": 1590.0, "bf16_sustained": 1400.0, "hbm_gbs": 6650.0, "source": "fallback (B200_PROFILING.md)"}
+    # NVIDIA H100 SXM data sheet (700 W card): dense BF16 989 TFLOP/s, HBM3 3.35 TB/s -- not a measured rate
+    return {"bf16_burst": 989.0, "bf16_sustained": None, "hbm_gbs": 3350.0, "source": "H100 SXM data sheet (dense BF16)"}
 
 
 class ClockSampler:
@@ -132,35 +138,26 @@ class ClockSampler:
                 "samples": len(sm)}
 
 
-def ncu_traffic():
-    """DRAM bytes per launch of the dominant kernel family from the newest committed `ncu --set full` summary
-    (profiles/r*_ncu_gemm_full_summary.txt, written by tools/ncu_summary.py from the capture recipe tools/profile.sh):
-    mean of dram__bytes_read.sum + dram__bytes_write.sum over the captured gemm_tc_kernel launches.  It is parsed at run
-    time from the committed evidence -- this run does not (and must not) execute under a profiler; None if absent."""
-    import ast
-    import glob
-    files = sorted(glob.glob(os.path.join(ROOT, "profiles", "r*_ncu_gemm_full_summary.txt")))
-    if not files:
-        return None, None
-    vals = []
-    for ln in open(files[-1]):
-        ln = ln.strip()
-        if not ln.startswith("{"):
-            continue
-        try:
-            d = ast.literal_eval(ln)
-        except Exception:
-            continue
-        if "gemm_tc_kernel" not in d.get("kernel", ""):
-            continue
+DUMP_SAMPLE = 1 << 20  # elements kept of each dense output by --dump-outputs
 
-        def mb(key):
-            v, unit = d[key].split()[:2]
-            return float(v) * {"byte": 1.0, "Kbyte": 1e3, "Mbyte": 1e6, "Gbyte": 1e9}[unit]
-        vals.append(mb("dram__bytes_read.sum") + mb("dram__bytes_write.sum"))
-    if not vals:
-        return None, None
-    return sum(vals) / len(vals), os.path.relpath(files[-1], ROOT) + " (%d launches)" % len(vals)
+
+def dump_outputs(out_dir, views):
+    """Write the outputs of one forward_pairs call ((view1, view2) dicts of tensors) as float32 .npy files.  Outputs with
+    more than DUMP_SAMPLE elements are sampled at DUMP_SAMPLE flat indices drawn once from a fixed seed (sorted), so the
+    files of two runs with the same arguments line up element for element; at most ~4 MB per file, ~17 MB in all at cfg-2."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    written = {}
+    for v, d in enumerate(views):
+        for key in sorted(d):
+            a = d[key].detach().float().cpu().numpy().reshape(-1)
+            if a.size > DUMP_SAMPLE:
+                idx = np.sort(np.random.default_rng(20240917).choice(a.size, DUMP_SAMPLE, replace=False))
+                a = a[idx]
+            name = "view%d_%s" % (v + 1, key)
+            np.save(os.path.join(out_dir, name + ".npy"), np.ascontiguousarray(a, dtype=np.float32))
+            written[name] = int(a.size)
+    return written
 
 
 def cpu_port_baseline(H, W, budget_s=45.0):
@@ -298,6 +295,7 @@ def run_b200_arm(args, rank, local_rank, world):
     global_pairs = total if total is not None else world * P
     value = global_pairs / (ms_step / 1e3)
     ok = bool(torch.isfinite(out[0]["pts3d_pred"]).all()) and bool(torch.isfinite(out[1]["relative_pose"]).all())
+    dumped = dump_outputs(args.dump_outputs, out) if (args.dump_outputs and rank == 0) else None
 
     # ---------------- end-to-end through the host-buffer C-ABI call (`e2e`) ----------------
     hout = {"pts3d": torch.empty(2, P, H, W, 3).pin_memory(), "conf": torch.empty(2, P, H, W).pin_memory(),
@@ -334,15 +332,10 @@ def run_b200_arm(args, rank, local_rank, world):
     gemm_launches = (cnt4[0] + cnt4[1]) // prof_steps
     achieved = P * gemm_flops_pair / (gemm_ms / 1e3) / 1e12
     peak = peaks["bf16_sustained"] or peaks["bf16_burst"]
-    traffic, traffic_src = ncu_traffic()
     roofline = {
-        "bound": "tensor", "kernel": "gemm_tc_kernel (tcgen05 GEMM + implicit-GEMM 3x3 conv family)",
+        "bound": "tensor", "kernel": "gemm_wg_kernel (wgmma GEMM + implicit-GEMM 3x3 conv family)",
         "achieved": achieved, "peak": peak, "unit": "TFLOP/s", "frac": achieved / peak,
-        # DRAM bytes per launch from the committed `ncu --set full` capture of this kernel family (parsed at run time;
-        # the family is tensor-bound, so this is context: traffic <= operand + output bytes means no re-reads)
-        "traffic": traffic, "traffic_unit": "bytes per launch (ncu dram__bytes_read.sum + dram__bytes_write.sum)",
-        "traffic_source": traffic_src,
-        "peak_source": peaks["source"] + ", sustained cuBLAS bf16 (kernel timed inside a long step)",
+        "peak_source": peaks["source"],
         "launches_per_step": int(gemm_launches), "avg_launch_ms": gemm_ms / max(1, gemm_launches),
         "algorithmic_gflop_per_launch_avg": P * gemm_flops_pair / max(1, gemm_launches) / 1e9,
         "family_ms_per_step": {"gemm_linear": ms4[0] / prof_steps, "gemm_conv3x3": ms4[1] / prof_steps,
@@ -371,6 +364,8 @@ def run_b200_arm(args, rank, local_rank, world):
                                       "exposed_copy_ms": max(0.0, e2e_ms - ms_step)},
             "gpu_launches": int(launches), "roofline": roofline, "cpu_baseline": cpu_baseline, "outputs_finite": ok,
         }
+        if dumped is not None:
+            line["dumped_outputs"] = {"dir": args.dump_outputs, "elements": dumped}
         print(json.dumps(line), flush=True)
     if world > 1:
         dist.destroy_process_group()
@@ -388,6 +383,9 @@ def main():
     ap.add_argument("--total-pairs", type=int, default=None,
                     help="cfg-5: global batch split contiguously over the ranks (strong scaling); overrides --pairs")
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the outputs of the last timed step as DIR/<name>.npy (float32, dense maps sampled); "
+                         "with --gpus N > 1, rank 0's pair shard only")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))

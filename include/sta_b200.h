@@ -1,5 +1,5 @@
 /*
- * sta_b200.h -- C ABI of libsta_b200.so, the B200 (sm_100a) implementation of the
+ * sta_b200.h -- C ABI of libsta_b200.so, the H100 (sm_90a) implementation of the
  * ViSTA-SLAM "Symmetric Two-view Association" (STA) frontend forward pass.
  *
  * The library is the drop-in boundary underneath the reference's Python module
@@ -36,7 +36,7 @@ int sta_create(StaModel** out);
 /* Same with an explicit operand precision.  STA_PRECISION_BF16 (what sta_create uses, and what every benchmark
  * number is measured with): bf16 tensor-core operands, fp32 accumulation.  STA_PRECISION_X3: split-precision PARITY
  * mode -- every bf16 activation is carried as (hi | lo | hi) and every bf16 weight as (hi | hi | lo), so the same
- * tcgen05 kernels compute a_hi w_hi + a_lo w_hi + a_hi w_lo over K' = 3K (about 17 significant operand bits),
+ * wgmma kernels compute a_hi w_hi + a_lo w_hi + a_hi w_lo over K' = 3K (about 17 significant operand bits),
  * and attention runs in fp32 on the CUDA cores.  It exists to check the kernels against the fp32 reference at
  * north_star's tolerance (pointmaps 1e-3, pose 1e-4); ~3x the weight memory, several times slower. */
 enum { STA_PRECISION_BF16 = 0, STA_PRECISION_X3 = 1 };
@@ -107,7 +107,7 @@ int64_t sta_launch_count(StaModel* m);
 int64_t sta_device_bytes(StaModel* m);
 
 /* Per-kernel-family device timing with CUDA events on the launch stream (adds two event records per
- * launch while enabled).  Families: 0 = tcgen05 GEMM (linear), 1 = tcgen05 GEMM (implicit 3x3 conv),
+ * launch while enabled).  Families: 0 = wgmma GEMM (linear), 1 = wgmma GEMM (implicit 3x3 conv),
  * 2 = attention, 3 = LayerNorm.  sta_profile_read synchronises, returns the accumulated milliseconds,
  * launch counts and executed FLOPs per family since the last read, and resets the counters. */
 int sta_profile(StaModel* m, int enable);

@@ -14,7 +14,7 @@ Every function cites the reference file:line it restates.  Two arithmetic modes:
   * emulate_bf16=False : pure fp32 -- the reference's CPU semantics (its CUDA path adds TF32).
   * emulate_bf16=True  : GEMM/conv operands and the activations the CUDA path stores as bf16 are
     rounded to bf16 (fp32 accumulate, fp32 residual stream / LayerNorm / softmax), i.e. the same
-    operand precision as the B200 kernels, so that parity can be checked below bf16's noise floor.
+    operand precision as the CUDA kernels, so that parity can be checked below bf16's noise floor.
 """
 import math
 

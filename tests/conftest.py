@@ -11,7 +11,7 @@ GOLDEN_DIR = os.path.join(ROOT, "tests", "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run with -m gpu on the GPU box)")
+    config.addinivalue_line("markers", "gpu: needs an H100 (sm_90a) GPU")
     import torch
     from oracle.sta_oracle import usable_cpus
     torch.set_num_threads(usable_cpus())  # the oracle runs on the host: do not oversubscribe a cgroup-limited box

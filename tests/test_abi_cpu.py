@@ -82,3 +82,20 @@ def test_product_never_imports_the_oracle():
                 # oracle/<file> as the checker of a kernel
                 assert "import oracle" not in src and "from oracle" not in src, (dp, f)
                 assert "oracle" not in src.replace("oracle/", "").lower(), (dp, f)
+
+
+def test_library_built_with_other_nvcc_flags_is_stale(tmp_path, monkeypatch):
+    """A library whose recorded nvcc flags differ from the current ones (e.g. another GPU architecture) is rebuilt,
+    however new it is."""
+    from vista_slam_b200 import build as b
+    lib = tmp_path / "libsta_b200.so"
+    lib.write_bytes(b"")
+    stamp = tmp_path / "nvcc_flags.txt"
+    monkeypatch.setattr(b, "LIB", str(lib))
+    monkeypatch.setattr(b, "STAMP", str(stamp))
+    monkeypatch.setattr(b, "CSRC", str(tmp_path))  # no sources here: only the flags decide
+    assert b._stale()  # no record of the flags
+    stamp.write_text(" ".join(b.NVCC_FLAGS))
+    assert not b._stale()
+    stamp.write_text(" ".join(b.NVCC_FLAGS).replace("sm_90a", "sm_100a"))
+    assert b._stale()

@@ -1,5 +1,5 @@
 """CPU: host-side pieces of bench.py that decide what the JSON line says -- the clock sampler's in-region window, the
-run-time parse of the committed ncu summary (`roofline.traffic`), the measured-peak lookup and the workload description."""
+output dump (--dump-outputs) and the workload description."""
 import importlib.util
 import os
 
@@ -51,10 +51,22 @@ def test_clock_sampler_without_in_region_samples_falls_back_to_the_latest_one():
     assert s2.stop()["sm_mhz"] is None
 
 
-def test_roofline_traffic_is_parsed_from_the_newest_committed_ncu_summary():
-    traffic, src = bench.ncu_traffic()
-    assert src is not None and src.startswith("profiles/r02_ncu_gemm_full_summary.txt")
-    assert 5e7 < traffic < 1e9  # bytes per launch: operands + outputs of one trunk GEMM
+def test_dump_outputs_is_deterministic_float32_and_bounded(tmp_path):
+    import numpy as np
+    import torch
+    g = torch.Generator().manual_seed(0)
+    views = tuple({"pts3d_pred": torch.randn(2, 600, 1000, 3, generator=g), "relative_pose": torch.randn(2, 4, 4, generator=g)}
+                  for _ in range(2))
+    a = bench.dump_outputs(str(tmp_path / "a"), views)
+    b = bench.dump_outputs(str(tmp_path / "b"), views)
+    assert a == b and a["view1_pts3d_pred"] == bench.DUMP_SAMPLE and a["view2_relative_pose"] == 32
+    total = 0
+    for name in a:
+        x, y = np.load(tmp_path / "a" / (name + ".npy")), np.load(tmp_path / "b" / (name + ".npy"))
+        assert x.dtype == np.float32 and np.array_equal(x, y)
+        total += x.nbytes
+    assert total <= 64 << 20
+    assert np.array_equal(np.load(tmp_path / "a" / "view2_relative_pose.npy"), views[1]["relative_pose"].numpy().reshape(-1))
 
 
 def test_workload_description_names_the_baseline_config():

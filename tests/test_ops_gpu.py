@@ -50,7 +50,7 @@ def test_bandwidth_kernels(capsys):
 
 
 def test_split_precision_mode_of_the_tensor_core_kernels(capsys):
-    """x3 parity mode at op level: the same tcgen05 GEMM / implicit-conv kernels with (hi | lo | hi) x (hi | hi | lo) operands
+    """x3 parity mode at op level: the same wgmma GEMM / implicit-conv kernels with (hi | lo | hi) x (hi | hi | lo) operands
     against fp64 references, 1e-4 max-normalised (100x below the bf16 floor)."""
     assert len(_collect(bu.group_x3, capsys)) == 13
 
@@ -92,13 +92,13 @@ def test_error_reporting_through_the_abi():
     assert rc != 0 and b"multiple of 32" in lib().sta_last_error()
 
 
+# env0 / env3 / env4 keep the ids of the routes they continue (no halo tile; the query-tile-pair and one-query-tile
+# attention kernels, now 128- and 64-row tiles); the epilogue route is new on this list
 @pytest.mark.parametrize("env,group", [
-    ({"STA_CONV_HALO": "0"}, "conv"),        # one TMA box per filter tap instead of the halo-staged tile
-    ({"STA_CONV_EW16": "0"}, "conv"),        # 8 epilogue warps for the skip-tensor convolutions
-    ({"STA_GEMM_TAIL": "0"}, "gemm_epi"),    # full tiles in the last (partial) wave instead of half tiles
-    ({"STA_ATTN_FEAT": "144"}, "attention"),  # query-tile-pair kernel for every shape
-    ({"STA_ATTN_FEAT": "192"}, "attention"),  # one-query-tile-per-CTA kernel for every shape
-    ({"STA_ATTN_FEAT": "16"}, "attention"),   # scalar FFMA / FADD softmax (A/B reference of the packed fp32 form)
+    pytest.param({"STA_CONV_HALO": "0"}, "conv", id="env0-conv"),           # one TMA box per filter tap, no halo tile
+    pytest.param({"STA_ATTN_QROWS": "128"}, "attention", id="env3-attention"),  # 128-row query tiles for every shape
+    pytest.param({"STA_ATTN_QROWS": "64"}, "attention", id="env4-attention"),   # 64-row query tiles for every shape
+    pytest.param({"STA_GEMM_TMA_EPI": "0"}, "gemm_epi", id="no_tma_epilogue-gemm_epi"),  # per-warp coalesced stores
 ])
 def test_alternate_kernel_routes(env, group):
     """The launchers pick one kernel variant per shape; the variants they do NOT pick by default (kept for same-box A/B

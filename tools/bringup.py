@@ -169,7 +169,7 @@ def group_gemm_epi():
     refr = refs.clone()
     refr[:, :768] = rope_ref(refs[:, :768].reshape(Ms, 12, 64), poss).reshape(Ms, 768)
     report("small M196 rope", outs, refr, 1e-2)
-    # the same epilogues on a problem wide enough for the 256-wide CTA-pair tiles (TMA-store epilogue, BN = 256)
+    # the same epilogues on a problem wide enough to fill every SM with 128 x 128 tiles (TMA-store epilogue)
     Mw, Kw = 5000, 256
     Aw = torch.randn(Mw, Kw, device=dev).bfloat16()
     Ww = (torch.randn(1024, Kw, device=dev) / math.sqrt(Kw)).bfloat16()
@@ -187,7 +187,7 @@ def group_gemm_epi():
     xw0 = xw.clone()
     run_gemm(gemm_desc(epi=EPI_F32, A=Aw, lda=Kw, W=Ww, ldw=Kw, M=Mw, N=1024, K=Kw, bias=bl, out=xw, ldo=1024, resid=xw))
     report("wide M5000 f32 in place (reduce-add)", xw, xw0 + refw, 2e-3)
-    # wave-quantisation tail: 24576 x 1024 = 384 tile pairs on 74 CTA pairs -> the last 14 run as 28 half tiles (256 x 128)
+    # a full-size in-place fp32 layer: 24576 x 1024 = 1536 tiles, many waves of the persistent grid
     Mt, Kt = 24576, 256
     At = torch.randn(Mt, Kt, device=dev).bfloat16()
     Wt = (torch.randn(1024, Kt, device=dev) / math.sqrt(Kt)).bfloat16()
@@ -195,7 +195,7 @@ def group_gemm_epi():
     xt = torch.randn(Mt, 1024, device=dev)
     xt0 = xt.clone()
     run_gemm(gemm_desc(epi=EPI_F32, A=At, lda=Kt, W=Wt, ldw=Kt, M=Mt, N=1024, K=Kt, bias=bt, out=xt, ldo=1024, resid=xt))
-    report("M24576 N1024 f32 in place (half-tile tail wave)", xt, xt0 + At.float() @ Wt.float().t() + bt, 2e-3)
+    report("M24576 N1024 f32 in place (many waves)", xt, xt0 + At.float() @ Wt.float().t() + bt, 2e-3)
     # PIXSHUF: tokens (2 img, 5x7 grid), Cin 128, cout 64, k 2
     nimg, h, w, cin, cout, k = 2, 5, 7, 128, 64, 2
     At = torch.randn(nimg * h * w, cin, device=dev).bfloat16()
@@ -386,7 +386,7 @@ def merge3(o, N, name):
 
 
 def group_x3():
-    """Split-precision parity mode of the SAME tcgen05 kernels (operands expanded along K, two-pass / three-store
+    """Split-precision parity mode of the SAME wgmma kernels (operands expanded along K, two-pass / three-store
     epilogues), against fp64 references on the un-rounded fp32 operands.  Bounds 1e-4 max-normalised: two orders of
     magnitude below the bf16 operand noise floor, so an indexing / epilogue error of any size cannot hide."""
     import ctypes
@@ -396,8 +396,7 @@ def group_x3():
     torch.manual_seed(7)
     dev = "cuda"
     TOL = 1e-4
-    # small-problem route (128-wide single-CTA tiles, TMA epilogue) / 256-wide CTA pairs (TMA epilogue) / N % 256 != 0
-    # (128-wide tiles, staging epilogue)
+    # small problem / many tiles / N % 256 != 0
     for (M, N, K) in [(777, 512, 256), (4096, 768, 768), (300, 384, 192)]:
         A = torch.randn(M, K, device=dev)
         W = torch.randn(N, K, device=dev) / math.sqrt(K)
@@ -406,7 +405,7 @@ def group_x3():
         A3, W3 = split_act(A), split_w(W)
         for epi, nm, fn in ((EPI_BF16, "bf16", lambda t: t), (EPI_GELU, "gelu", lambda t: F.gelu(t))):
             if epi == EPI_GELU and N % 256 != 0:
-                continue  # the model has no GELU layer with N % 256 != 0 (no such kernel instance)
+                continue  # the model has no GELU layer with N % 256 != 0
             out = torch.full((M, 3 * N), float("nan"), device=dev, dtype=torch.bfloat16)
             run_gemm(gemm_desc(epi=epi, A=A3, lda=3 * K, W=W3, ldw=3 * K, M=M, N=N, K=3 * K, bias=bias, out=out, ldo=3 * N,
                                split_precision=1))

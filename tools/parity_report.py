@@ -7,8 +7,8 @@ same seeded inputs go through `forward_pairs` on the GPU.  Per output the report
   max-normalised error  max|a-b| / max|b|      and      median-normalised error  median|a-b| / max|b|
 of (1) cuda vs fp32 reference golden, (2) cuda vs the oracle in bf16-operand emulation, (3) emulation oracle vs the
 fp32 golden -- so that |cuda - fp32| can be compared with the noise floor |emu - fp32| of the same operand precision.
-The cfg-2 case is also run as pair 0 of a 16-pair batch (the production tile routes: 256-wide CTA pairs, 7 attention
-tiles) next to the single-pair call (small-problem route).
+The cfg-2 case is also run as pair 0 of a 16-pair batch (the production tile routes: full GEMM grids, 128-row attention
+tiles) next to the single-pair call (small-problem routes).
 """
 import json
 import os

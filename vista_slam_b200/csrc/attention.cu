@@ -1,4 +1,4 @@
-// Flash-attention forward (head_dim 64, non-causal) on tcgen05 for sm_100a.
+// Flash-attention forward (head_dim 64, non-causal) on wgmma for sm_90a.
 //
 // Replaces, for one (sample, head, 128-query tile) per CTA:
 //   * xformers memory_efficient_attention at vista_slam/sta_model/blocks/sta_blocks.py:143
@@ -9,22 +9,15 @@
 // Q, K, V are read straight out of the projection GEMM outputs with 3-D TMA tensor maps
 // (64 head columns x tokens x samples); nothing is re-laid-out.
 //
-// Pipeline (persistent; a CTA walks work items = (pair of 128-query tiles, head, sample); 384 threads,
-// setmaxnreg moves registers from the TMA/MMA warpgroup to the two softmax warpgroups):
-//   warp 0      TMA producer: the two Q tiles of the item (double buffered across items), K tiles and V tiles
-//               of 128 keys (3 stages each) -- K/V are shared by the two query tiles
-//   warp 1      MMA issuer (one elected thread), per key tile n and query tile t in {A, B}:
-//               S_t = Q_t K_n^T (128x128x64, fp32 in TMEM), O_t += P_t V_n (128x64x128 accumulating in TMEM,
-//               V consumed MN-major exactly as TMA wrote it)
-//   warps 4..7  softmax group A (query tile 2i), warps 8..11 group B (query tile 2i+1): one thread per query
-//               row.  The 128 scores of the row are read from TMEM ONCE into registers, which frees the S
-//               buffer at once (the next Q K^T overlaps the softmax); P = exp2(S*c - m) goes to a
-//               128B-swizzled K-major bf16 smem tile.  O stays in TMEM: the running maximum used for the
-//               exponentials is only raised when the true maximum exceeds it by more than 2^8 (exact after
-//               the final division by l, P <= 256 in between), so O has to be rescaled in place
-//               (tcgen05.ld / st) only on the rare tiles where that happens.
-// The two groups are independent streams sharing K/V; group B starts half a period late so that one group's
-// exp2 (MUFU-bound) phase overlaps the other's load / max / store phases.
+// Pipeline (128 + 128 * CWG threads):
+//   warp 0        TMA producer: the Q tile, then K and V tiles of 128 keys (3 stages, separate full barriers so that
+//                 Q K^T starts before V has landed)
+//   warps 4..     CWG consumer warpgroups (1 or 2), 64 query rows each: S = Q K^T (wgmma m64n128k16, fp32 in registers),
+//                 online softmax in registers (exp2 with the scale folded in, running maximum per row), P rounded to bf16
+//                 and kept in registers as the A operand of O += P V (wgmma m64n64k16, V consumed MN-major exactly as TMA
+//                 wrote it).  The final O / l is stored straight from the accumulator registers.
+// Two warpgroups per CTA share every K / V tile (half the K / V traffic); one warpgroup per CTA doubles the CTA count
+// for problems that would not fill the GPU with 128-row tiles (launch_attention chooses).
 #include "common.cuh"
 #include "host_util.h"
 
@@ -37,925 +30,182 @@ namespace sta {
 
 namespace {
 
-constexpr int ATT_THREADS = 384;  // warpgroup 0: TMA / MMA / 2 idle warps; warpgroups 1, 2: softmax groups A, B
+// CWG consumer warpgroups of 64 query rows each (query tile = 64 * CWG rows); warp 0 is the TMA producer (warps 1-3 idle)
+template <int CWG>
+constexpr int att_threads() { return 128 + 128 * CWG; }
 constexpr int KV_STAGES = 3;
 constexpr uint32_t TILE_BYTES = 128 * 64 * 2;  // 16 KB: [128 rows][64 bf16]
-// Q [group][2 buffers] | K x3 | V x3 | P [group] (two 64-key sub-tiles each) | barriers
-constexpr uint32_t ATT_OFF_K = 4 * TILE_BYTES;
+// Q (up to 128 rows) | K x3 | V x3 | barriers
+constexpr uint32_t ATT_OFF_K = TILE_BYTES;
 constexpr uint32_t ATT_OFF_V = ATT_OFF_K + KV_STAGES * TILE_BYTES;
-constexpr uint32_t ATT_OFF_P = ATT_OFF_V + KV_STAGES * TILE_BYTES;
-constexpr uint32_t ATT_OFF_ONES = ATT_OFF_P + 4 * TILE_BYTES;  // 16 rows x 128 B of bf16 1.0 (B operand of the row-sum MMA)
-constexpr uint32_t ONES_BYTES = 16 * 128;
-constexpr uint32_t ATT_OFF_BAR = ATT_OFF_ONES + ONES_BYTES;
+constexpr uint32_t ATT_OFF_BAR = ATT_OFF_V + KV_STAGES * TILE_BYTES;
 constexpr uint32_t ATT_SMEM = ATT_OFF_BAR + 256;
-static_assert(ATT_SMEM <= 227 * 1024, "attention shared memory");
-// Feature bits (template parameter; STA_ATTN_FEAT selects an instance for A/B timing, tools/attn_ab.py):
-//   AF_SKIP  warps whose 32 query rows are all >= nq (ragged last query tile / dead second tile: the decoder's 769 rows are
-//            6 x 128 + 1) only keep the barrier protocol going -- no TMEM traffic, no math;
-//   AF_ONES  row sum l from the tensor core: one extra N = 16 MMA per key step multiplies P by a tile of ones, so l
-//            accumulates in TMEM next to O (and is the sum of exactly the bf16 P values that multiply V).
-//   AF_PTMEM P stays in tensor memory: the softmax threads write the bf16 probabilities with tcgen05.st into 64 TMEM columns
-//            per query tile and the P V MMAs take their A operand from there (tcgen05.mma with a TMEM A operand), so an
-//            N = 64 MMA no longer has to stream a 4 KB slice of P out of shared memory (it is shared-memory-bandwidth
-//            bound otherwise: ~64 clk instead of 32), and the softmax needs no st.shared / fence.proxy.async.
-//            TMEM: S 2 x 128 | O 2 x 64 | P 2 x 64 = 512 columns (hence exclusive with AF_ONES).
-//   AF_EMU   2 of every 8 exponentials on the FMA pipe (ex2_fma, degree-3 polynomial) instead of the 16-lane/clk MUFU.
-//   AF_1Q    one query tile per CTA, two CTAs per SM (attention_1q_kernel below; implies P in tensor memory).
-//   AF_X2    scale-subtract and row sums with the packed fp32 instructions FFMA2 / FADD2 (common.cuh::f32x2_*).
-enum AttnFeat : int { AF_SKIP = 1, AF_ONES = 8, AF_PTMEM = 16, AF_EMU = 32, AF_1Q = 64, AF_X2 = 128 };
-constexpr float kRescaleThreshold = 8.0f;  // log2 units
 
 struct AttnParams {
-  int nq, nk, batch, heads, qpairs, kv_batch_shift;
-  int nitems;
-  int pingpong;  // enforce alternating exp2 phases of the two softmax groups
+  int nq, nk, batch, heads, qtiles, kv_batch_shift;
   int q_row0;  // first query row handled by the tiled kernel (1 when row 0 goes to attention_row0_kernel)
   float scale_log2;
   __nv_bfloat16* out;
   long long ldo;
-  long long* dbg;  // clock64 stamps of CTA 0 (only in builds with -DSTA_ATTN_TRACE_BUILD; tools/attn_trace.py), else unused
 };
-#ifdef STA_ATTN_TRACE_BUILD
-#define ATTN_STAMP(cond, idx) do { if ((cond) && p.dbg) p.dbg[(idx)] = clock64(); } while (0)
-#else
-#define ATTN_STAMP(cond, idx) do { } while (0)
-#endif
 
-template <int FEAT>
-__global__ void __launch_bounds__(ATT_THREADS, 1)
+// One CTA per (64 * CWG-query tile, head, sample); the tile index is fastest, so neighbouring CTAs share one
+// (sample, head)'s K / V tiles in L2.
+template <int CWG>
+__global__ void __launch_bounds__(att_threads<CWG>(), 1)
 attention_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
-                     const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmO,
-                     const AttnParams p, int q_col0, int k_col0, int v_col0) {
+                     const __grid_constant__ CUtensorMap tmV, const AttnParams p, int q_col0, int k_col0, int v_col0) {
   extern __shared__ __align__(1024) uint8_t smem[];
-  uint8_t* sQ = smem;  // group t, buffer b at sQ + (2 * t + b) * TILE_BYTES
+  uint8_t* sQ = smem;
   uint8_t* sK = smem + ATT_OFF_K;
   uint8_t* sV = smem + ATT_OFF_V;
-  uint8_t* sP = smem + ATT_OFF_P;  // group t at sP + t * 2 * TILE_BYTES
-  [[maybe_unused]] uint8_t* sOnes = smem + ATT_OFF_ONES;
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + ATT_OFF_BAR);
-  uint64_t* q_full = bars + 0;    // [2 groups][2 buffers]
-  uint64_t* q_empty = bars + 4;   // [2][2]
-  uint64_t* k_full = bars + 8;    // [3]
-  uint64_t* k_empty = bars + 11;  // [3]
-  uint64_t* v_full = bars + 14;   // [3]
-  uint64_t* v_empty = bars + 17;  // [3]
-  uint64_t* s_full = bars + 20;   // [2]  MMA -> softmax group t: S_t ready
-  uint64_t* s_free = bars + 22;   // [2]  softmax group t -> MMA: S_t is in registers, buffer reusable
-  uint64_t* p_full = bars + 24;   // [2]  softmax group t -> MMA: P_t written (and O_t rescaled if needed)
-  uint64_t* o_full = bars + 26;   // [2]  MMA -> softmax group t: O_t += P_t V done (P_t consumed)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 28);
+  uint64_t* q_full = bars;
+  uint64_t* k_full = bars + 1;
+  uint64_t* v_full = k_full + KV_STAGES;
+  uint64_t* kv_empty = v_full + KV_STAGES;
 
+  const int item = blockIdx.x;
+  const int qt = item % p.qtiles;
+  const int head = (item / p.qtiles) % p.heads;
+  const int b = item / (p.qtiles * p.heads);
+  const int kvb = (b + p.kv_batch_shift) % p.batch;
+  constexpr int QROWS = 64 * CWG;
+  const int q0 = p.q_row0 + qt * QROWS;
+  const int nkt = (p.nk + 127) / 128;
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const int T = (p.nk + 127) / 128;
 
   if (threadIdx.x == 0) {
     if ((smem_u32(smem) & 1023u) != 0) device_fatal("dynamic shared memory is not 1024-byte aligned");
-    for (int i = 0; i < 4; ++i) {
-      mbar_init(&q_full[i], 1);
-      mbar_init(&q_empty[i], 1);
-    }
-    for (int i = 0; i < KV_STAGES; ++i) {
-      mbar_init(&k_full[i], 1);
-      mbar_init(&k_empty[i], 1);
-      mbar_init(&v_full[i], 1);
-      mbar_init(&v_empty[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&s_full[i], 1);
-      mbar_init(&s_free[i], 4);
-      mbar_init(&p_full[i], 4);
-      mbar_init(&o_full[i], 1);
+    mbar_init(q_full, 1);
+    for (int s = 0; s < KV_STAGES; ++s) {
+      mbar_init(&k_full[s], 1);
+      mbar_init(&v_full[s], 1);
+      mbar_init(&kv_empty[s], 4 * CWG);  // one arrival per consumer warp
     }
     fence_mbar_init();
   }
-  if (warp == 1) {
-    tmem_alloc(tmem_slot, 512);
-    tmem_relinquish();
+  if (warp == 0 && lane == 0) {
+    tma_prefetch_desc(&tmQ);
+    tma_prefetch_desc(&tmK);
+    tma_prefetch_desc(&tmV);
   }
-  if constexpr (FEAT & AF_ONES) {
-    if (warp == 2 || warp == 3) {  // the two idle warps fill the ones tile (identical elements: swizzle-invariant)
-      uint32_t* o32 = reinterpret_cast<uint32_t*>(sOnes);
-      for (int i = threadIdx.x - 64; i < static_cast<int>(ONES_BYTES / 4); i += 64) o32[i] = 0x3F803F80u;  // bf16 1.0 x 2
-      fence_proxy_async_smem();
-    }
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  // columns: S_A [0,128) S_B [128,256) O_A [256,320) O_B [320,384) l_A [384,400) l_B [400,416) (AF_ONES)
   pdl_wait();
   pdl_launch_dependents();
 
-
-  auto decode = [&](int w, int& q0, int& head, int& b, int& kvb) {
-    const int qp = w % p.qpairs;
-    const int rest = w / p.qpairs;
-    head = rest % p.heads;
-    b = rest / p.heads;
-    q0 = p.q_row0 + qp * 256;
-    kvb = (b + p.kv_batch_shift) % p.batch;
-  };
-  const int my_items = (p.nitems > static_cast<int>(blockIdx.x))
-                           ? (p.nitems - 1 - static_cast<int>(blockIdx.x)) / static_cast<int>(gridDim.x) + 1
-                           : 0;
-
-  // register re-distribution: the softmax threads keep a whole 128-score row in registers
-  if (warp < 4) {
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 72;" ::: "memory");
   if (warp == 0) {
     // ===================== TMA producer =====================
-    if (elect_one()) {
-      tma_prefetch_desc(&tmQ);
-      tma_prefetch_desc(&tmK);
-      tma_prefetch_desc(&tmV);
-      int st = 0;
-      uint32_t ph = 0;
-      for (int it = 0; it < my_items; ++it) {
-        int q0, head, b, kvb;
-        decode(static_cast<int>(blockIdx.x) + it * static_cast<int>(gridDim.x), q0, head, b, kvb);
-        const int qb = it & 1;
-        for (int t = 0; t < 2; ++t) {  // a second tile beyond nq is zero-filled by TMA (and never stored)
-          mbar_wait(&q_empty[2 * t + qb], ((it >> 1) & 1) ^ 1);
-          mbar_arrive_expect_tx(&q_full[2 * t + qb], TILE_BYTES);
-          tma_load_3d(sQ + (2 * t + qb) * TILE_BYTES, &tmQ, &q_full[2 * t + qb], q_col0 + head * 64, q0 + t * 128, b);
-        }
-        for (int j = 0; j < T; ++j) {
-          mbar_wait(&k_empty[st], ph ^ 1);
-          mbar_arrive_expect_tx(&k_full[st], TILE_BYTES);
-          tma_load_3d(sK + st * TILE_BYTES, &tmK, &k_full[st], k_col0 + head * 64, j * 128, kvb);
-          mbar_wait(&v_empty[st], ph ^ 1);
-          mbar_arrive_expect_tx(&v_full[st], TILE_BYTES);
-          tma_load_3d(sV + st * TILE_BYTES, &tmV, &v_full[st], v_col0 + head * 64, j * 128, kvb);
-          if (++st == KV_STAGES) { st = 0; ph ^= 1; }
-        }
+    if (lane == 0) {
+      mbar_arrive_expect_tx(q_full, QROWS * 128);
+      tma_load_3d(sQ, &tmQ, q_full, q_col0 + head * 64, q0, b);  // rows >= nq are zero-filled
+      for (int j = 0; j < nkt; ++j) {
+        const int st = j % KV_STAGES;
+        mbar_wait(&kv_empty[st], ((j / KV_STAGES) & 1) ^ 1);
+        mbar_arrive_expect_tx(&k_full[st], TILE_BYTES);
+        tma_load_3d(sK + st * TILE_BYTES, &tmK, &k_full[st], k_col0 + head * 64, j * 128, kvb);
+        mbar_arrive_expect_tx(&v_full[st], TILE_BYTES);
+        tma_load_3d(sV + st * TILE_BYTES, &tmV, &v_full[st], v_col0 + head * 64, j * 128, kvb);
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    if (elect_one()) {
-      constexpr uint32_t idesc_s = make_idesc_bf16(128, 128, 0, 0);
-      constexpr uint32_t idesc_s16 = make_idesc_bf16(128, 16, 0, 0);  // narrow tail tile (<= 16 valid keys)
-      constexpr uint32_t idesc_o = make_idesc_bf16(128, 64, 0, 1);    // B (= V) is MN-major
-      const bool narrow_tail = (p.nk - (T - 1) * 128) <= 16;
-      const int total = my_items * T;  // key-tile steps of this CTA; step n = it * T + j
-      // state of the NEXT S to issue (same for both groups; advanced after group B)
-      int s_it = 0, s_j = 0, s_st = 0;
-      uint32_t s_ph = 0;
-      auto issue_s = [&](int t) {
-        const int qi = 2 * t + (s_it & 1);
-        if (s_j == 0) mbar_wait(&q_full[qi], (s_it >> 1) & 1);
-        mbar_wait(&k_full[s_st], s_ph);
-        tc_fence_after();
-        const uint64_t qdesc = make_smem_desc_sw128(smem_u32(sQ + qi * TILE_BYTES));
-        const uint64_t kdesc = make_smem_desc_sw128(smem_u32(sK + s_st * TILE_BYTES));
-        const uint32_t d = tmem_base + t * 128;
-        const uint32_t ids = (narrow_tail && s_j == T - 1) ? idesc_s16 : idesc_s;
+  } else if (warp >= 4) {
+    // ============ consumer warpgroups: 64 query rows each ============
+    // wgmma accumulator layout (m64 nN): register 4c + {0,1} = row g, columns 8c + 2t + {0,1}; 4c + {2,3} = row g + 8
+    const int wg = (warp - 4) >> 2, wq = (warp - 4) & 3;
+    const int g = lane >> 2, t = lane & 3;
+    float o[32];
 #pragma unroll
-        for (int k = 0; k < 4; ++k) umma_bf16(d, qdesc + 2 * k, kdesc + 2 * k, ids, k != 0);
-        if (t == 1) umma_commit(&k_empty[s_st]);      // both query tiles have read this K tile
-        if (s_j == T - 1) umma_commit(&q_empty[qi]);  // last read of this item's Q_t
-        umma_commit(&s_full[t]);
-        if (t == 1) {
-          if (++s_st == KV_STAGES) { s_st = 0; s_ph ^= 1; }
-          if (++s_j == T) { s_j = 0; ++s_it; }
-        }
-      };
-      if (total > 0) {
-        issue_s(0);
-        issue_s(1);
+    for (int i = 0; i < 32; ++i) o[i] = 0.0f;
+    float m0 = -INFINITY, m1 = -INFINITY;  // running maxima of the two rows (log2 units)
+    float l0 = 0.0f, l1 = 0.0f;            // this thread's part of the running row sums
+    mbar_wait(q_full, 0);
+    const uint64_t qdesc = make_smem_desc_sw128(smem_u32(sQ) + wg * 64 * 128);
+#pragma unroll 1
+    for (int j = 0; j < nkt; ++j) {
+      const int st = j % KV_STAGES;
+      const uint32_t ph = (j / KV_STAGES) & 1;
+      // ---- S = Q K^T (64 x 128 keys, K-major operands exactly as TMA wrote them) ----
+      float s[64];
+#pragma unroll
+      for (int i = 0; i < 64; ++i) s[i] = 0.0f;
+      mbar_wait(&k_full[st], ph);
+      const uint64_t kdesc = make_smem_desc_sw128(smem_u32(sK + st * TILE_BYTES));
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < 4; ++k) wgmma_m64n128k16_ss(s, qdesc + 2 * k, kdesc + 2 * k, 1u);
+      wgmma_commit();
+      wgmma_wait<0>();
+      fence_regs(s);
+      // ---- online softmax ----
+      const int kvalid = p.nk - j * 128;  // >= 1
+      if (kvalid < 128) {
+#pragma unroll
+        for (int i = 0; i < 64; ++i)
+          if (8 * (i >> 2) + 2 * t + (i & 1) >= kvalid) s[i] = -INFINITY;
       }
-      int v_st = 0, j = 0;
-      uint32_t v_ph = 0;
-      for (int n = 0; n < total; ++n) {
-        // S_t(n+1) as soon as group t holds S_t(n) in registers
-        if (n + 1 < total) {
-          for (int t = 0; t < 2; ++t) {
-            mbar_wait(&s_free[t], n & 1);
-            issue_s(t);
-          }
-        }
-        // O_t (+)= P_t(n) V(n) as soon as group t has written P_t(n)
-        for (int t = 0; t < 2; ++t) {
-          mbar_wait(&p_full[t], n & 1);
-          if (t == 0) mbar_wait(&v_full[v_st], v_ph);
-          tc_fence_after();
-          const uint64_t vdesc = make_smem_desc_sw128(smem_u32(sV + v_st * TILE_BYTES));
-          const uint64_t pdesc0 = make_smem_desc_sw128(smem_u32(sP + t * 2 * TILE_BYTES));
-          const uint64_t pdesc1 = make_smem_desc_sw128(smem_u32(sP + t * 2 * TILE_BYTES + TILE_BYTES));
-          const uint32_t d = tmem_base + 256 + t * 64;
-          const int ksteps = (narrow_tail && j == T - 1) ? 1 : 8;  // a narrow tail tile holds <= 16 keys
-          if constexpr (FEAT & AF_PTMEM) {
-            // A = P_t straight from tensor memory: 16 keys = 8 packed columns per step
-            const uint32_t tp = tmem_base + 384 + t * 64;
-            for (int k = 0; k < ksteps; ++k)
-              umma_bf16_ts(d, tp + 8 * k, vdesc + (2048 >> 4) * k, idesc_o, (j > 0 || k > 0) ? 1u : 0u);
-          } else
-          for (int k = 0; k < ksteps; ++k) {
-            const uint64_t pd = (k < 4 ? pdesc0 : pdesc1) + 2 * (k & 3);
-            // V advances 16 keys = 16 rows x 128 B = 2048 B per step; first key tile of an item overwrites O
-            umma_bf16(d, pd, vdesc + (2048 >> 4) * k, idesc_o, (j > 0 || k > 0) ? 1u : 0u);
-            // row sums: l_t (+)= P_t(n) 1 (all 16 columns equal; the ones tile is the same for every key step)
-            if constexpr (FEAT & AF_ONES)
-              umma_bf16(tmem_base + 384 + t * 16, pd, make_smem_desc_sw128(smem_u32(sOnes)), idesc_s16, (j > 0 || k > 0) ? 1u : 0u);
-          }
-          if (t == 1) umma_commit(&v_empty[v_st]);
-          umma_commit(&o_full[t]);
-        }
-        if (++v_st == KV_STAGES) { v_st = 0; v_ph ^= 1; }
-        if (++j == T) j = 0;
+      float mx0 = -INFINITY, mx1 = -INFINITY;
+#pragma unroll
+      for (int c = 0; c < 16; ++c) {
+        mx0 = fmaxf(mx0, fmaxf(s[4 * c], s[4 * c + 1]));
+        mx1 = fmaxf(mx1, fmaxf(s[4 * c + 2], s[4 * c + 3]));
       }
+      mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 1));
+      mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 2));
+      mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 1));
+      mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 2));
+      const float mn0 = fmaxf(m0, mx0 * p.scale_log2), mn1 = fmaxf(m1, mx1 * p.scale_log2);  // finite: >= 1 valid key
+      const float c0 = ex2_approx(m0 - mn0), c1 = ex2_approx(m1 - mn1);                    // first tile: 2^-inf = 0
+      m0 = mn0;
+      m1 = mn1;
+      l0 *= c0;
+      l1 *= c1;
+#pragma unroll
+      for (int c = 0; c < 8; ++c) {
+        o[4 * c] *= c0; o[4 * c + 1] *= c0;
+        o[4 * c + 2] *= c1; o[4 * c + 3] *= c1;
+      }
+      // P = 2^(S c - m) as bf16 A fragments of the P V wgmma (keys 16 kk .. 16 kk + 15 = accumulator columns 2 kk, 2 kk + 1)
+      uint32_t pa[8][4];
+#pragma unroll
+      for (int kk = 0; kk < 8; ++kk) {
+        float e[8];
+#pragma unroll
+        for (int i = 0; i < 8; ++i) e[i] = ex2_approx(fmaf(s[8 * kk + i], p.scale_log2, (i & 2) ? -m1 : -m0));
+        l0 += (e[0] + e[1]) + (e[4] + e[5]);
+        l1 += (e[2] + e[3]) + (e[6] + e[7]);
+        pa[kk][0] = pack_bf16x2(e[0], e[1]);
+        pa[kk][1] = pack_bf16x2(e[2], e[3]);
+        pa[kk][2] = pack_bf16x2(e[4], e[5]);
+        pa[kk][3] = pack_bf16x2(e[6], e[7]);
+      }
+      // ---- O += P V (V [keys][64] is the MN-major B operand: 16 keys = two 8-row groups = 2 KB per k16 step) ----
+      mbar_wait(&v_full[st], ph);
+      const uint32_t vbase = smem_u32(sV + st * TILE_BYTES);
+      wgmma_fence();
+#pragma unroll
+      for (int kk = 0; kk < 8; ++kk) wgmma_m64n64k16_rs_mn(o, pa[kk], make_smem_desc_sw128(vbase + kk * 2048));
+      wgmma_commit();
+      wgmma_wait<0>();
+      fence_regs(o);
+#pragma unroll
+      for (int kk = 0; kk < 8; ++kk) fence_regs(pa[kk]);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&kv_empty[st]);
     }
-  }
-  } else {
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 216;" ::: "memory");
-    // ===================== softmax warpgroups: one thread per query row =====================
-    const int grp = (warp - 4) >> 2;  // 0: query tile A, 1: query tile B of each item
-    const int quarter = warp & 3;
-    const int r = quarter * 32 + lane;
-    const uint32_t lane_addr = static_cast<uint32_t>(quarter * 32) << 16;
-    const int rx = r & 7;
-    const uint32_t tS = tmem_base + lane_addr + grp * 128;       // this group's S buffer
-    const uint32_t tO = tmem_base + lane_addr + 256 + grp * 64;  // this group's O accumulator
-    [[maybe_unused]] const uint32_t tL = tmem_base + lane_addr + 384 + grp * 16;  // this group's row sums (AF_ONES)
-    [[maybe_unused]] const uint32_t tP = tmem_base + lane_addr + 384 + grp * 64;  // this group's P tile (AF_PTMEM)
-    uint8_t* prow = sP + grp * 2 * TILE_BYTES + r * 128;         // this group's P buffer, row r
-    int n = 0;  // key-tile step counter (barrier parities)
-    // Enforced ping-pong of the MUFU-bound phase (STA_ATTN_PINGPONG, default on): the two groups take turns with the
-    // exponentials -- group t waits on named barrier 3 + t before its exp2 loop and hands the turn to the other
-    // group right after it -- so that one group's exp2 work overlaps the other's TMEM load / row maximum / P store /
-    // handshake instead of both contending for the same 16 MUFU lanes at the same time.  Both groups run the same
-    // number of key-tile steps, so the turns alternate A, B, A, B, ... for the whole kernel.
-    const bool pingpong = p.pingpong != 0;
-    auto turn_wait = [&]() { if (pingpong) named_bar_sync(3 + grp, 256); };
-    auto turn_pass = [&]() { if (pingpong) named_bar_arrive(3 + (grp ^ 1), 256); };
-    if (pingpong && grp == 1) named_bar_arrive(3, 256);  // group A goes first
-
-    for (int it = 0; it < my_items; ++it) {
-      int q0, head, b, kvb;
-      decode(static_cast<int>(blockIdx.x) + it * static_cast<int>(gridDim.x), q0, head, b, kvb);
-      // AF_SKIP: all 32 rows of this warp lie beyond nq: keep the barrier protocol in step (the same waits and arrivals as a
-      // live warp, in the same order) but do no TMEM traffic and no math.  The warp's P rows keep stale values: rows of O
-      // are independent and rows >= nq are never stored.
-      if ((FEAT & AF_SKIP) && (q0 + grp * 128 + quarter * 32 >= p.nq)) {
-        for (int j = 0; j < T; ++j, ++n) {
-          mbar_wait(&s_full[grp], n & 1);
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&s_free[grp]);
-          __syncwarp();  // the named barriers below are warp-aligned: reconverge after the one-lane arrival
-          if (j > 0) mbar_wait(&o_full[grp], (n - 1) & 1);
-          __syncwarp();
-          if (j == 0 && it > 0) named_bar_sync(1 + grp, 128);
-          turn_wait();
-          turn_pass();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&p_full[grp]);
-          __syncwarp();
-        }
-        mbar_wait(&o_full[grp], (n - 1) & 1);
-        __syncwarp();
-        named_bar_sync(1 + grp, 128);
-        continue;
-      }
-      float m_used = -INFINITY;  // maximum the exponentials of this row are currently relative to (log2 domain)
-      float l = 0.f;
-
-      for (int j = 0; j < T; ++j, ++n) {
-        const int nvalid = p.nk - j * 128;  // >= 1
-        mbar_wait(&s_full[grp], n & 1);
-        tc_fence_after();
-        if (nvalid <= 16 && j == T - 1) {
-          // ---- narrow tail tile: S is 128 x 16, P V uses a single 16-key step ----
-          uint32_t s16[16];
-          tmem_ld16(tS, s16);
-          tmem_ld_wait();
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&s_free[grp]);
-          float mxn = -INFINITY;
+    l0 += __shfl_xor_sync(0xffffffffu, l0, 1);
+    l0 += __shfl_xor_sync(0xffffffffu, l0, 2);
+    l1 += __shfl_xor_sync(0xffffffffu, l1, 1);
+    l1 += __shfl_xor_sync(0xffffffffu, l1, 2);
+    const float inv0 = 1.0f / l0, inv1 = 1.0f / l1;
+    const int row = q0 + wg * 64 + wq * 16 + g;
+    __nv_bfloat16* oa = p.out + (static_cast<long long>(b) * p.nq + row) * p.ldo + head * 64 + 2 * t;
+    __nv_bfloat16* ob = oa + 8 * p.ldo;
 #pragma unroll
-          for (int i = 0; i < 16; ++i) {
-            if (i >= nvalid) s16[i] = 0xff800000u;
-            mxn = fmaxf(mxn, __uint_as_float(s16[i]));
-          }
-          const float m_true = mxn * p.scale_log2;
-          const bool raise = m_true > m_used + kRescaleThreshold;
-          const float m_new = raise ? m_true : m_used;
-          const float factor = raise ? ex2_approx(m_used - m_new) : 1.0f;
-          l *= factor;
-          m_used = m_new;
-          if (j > 0) {
-            mbar_wait(&o_full[grp], (n - 1) & 1);
-            if (__any_sync(0xffffffffu, raise)) {
-              tc_fence_after();
-#pragma unroll
-              for (int c = 0; c < 64; c += 32) {
-                uint32_t o[32];
-                tmem_ld32(tO + c, o);
-                tmem_ld_wait();
-#pragma unroll
-                for (int i = 0; i < 32; ++i) o[i] = __float_as_uint(__uint_as_float(o[i]) * factor);
-                tmem_st32(tO + c, o);
-              }
-              if constexpr (FEAT & AF_ONES) {
-                const uint32_t lv = tmem_ld1(tL);
-                tmem_ld_wait();
-                tmem_st1(tL, __float_as_uint(__uint_as_float(lv) * factor));
-              }
-              tmem_st_wait();
-            }
-          }
-          if (j == 0 && it > 0) {
-            if (warp == 4 + 4 * grp && lane == 0) tma_store_wait_read();
-            named_bar_sync(1 + grp, 128);
-          }
-          float rs = 0.f;
-          turn_wait();
-#pragma unroll
-          for (int c = 0; c < 2; ++c) {
-            float e[8];
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-              e[i] = ex2_approx(fmaf(__uint_as_float(s16[8 * c + i]), p.scale_log2, -m_used));
-              if constexpr (!(FEAT & AF_ONES)) rs += e[i];
-            }
-            uint4 q;
-            q.x = pack_bf16x2(e[0], e[1]);
-            q.y = pack_bf16x2(e[2], e[3]);
-            q.z = pack_bf16x2(e[4], e[5]);
-            q.w = pack_bf16x2(e[6], e[7]);
-            if constexpr (FEAT & AF_PTMEM) tmem_st4(tP + 4 * c, q);
-            else *reinterpret_cast<uint4*>(prow + ((c ^ rx) << 4)) = q;
-          }
-          turn_pass();
-          l += rs;
-          if constexpr (FEAT & AF_PTMEM) tmem_st_wait();
-          else fence_proxy_async_smem();
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&p_full[grp]);
-          continue;
-        }
-        // ---- the whole score row into registers; release the S buffer for the next Q K^T ----
-        uint32_t s[128];
-        {
-          uint32_t (&s0)[32] = *reinterpret_cast<uint32_t(*)[32]>(&s[0]);
-          uint32_t (&s1)[32] = *reinterpret_cast<uint32_t(*)[32]>(&s[32]);
-          uint32_t (&s2)[32] = *reinterpret_cast<uint32_t(*)[32]>(&s[64]);
-          uint32_t (&s3)[32] = *reinterpret_cast<uint32_t(*)[32]>(&s[96]);
-          tmem_ld32(tS, s0);
-          tmem_ld32(tS + 32, s1);
-          tmem_ld32(tS + 64, s2);
-          tmem_ld32(tS + 96, s3);
-          tmem_ld_wait();
-        }
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&s_free[grp]);
-        if (nvalid < 128) {  // ragged last key tile: masked scores contribute exp2(-inf) = 0
-#pragma unroll
-          for (int i = 0; i < 128; ++i)
-            if (i >= nvalid) s[i] = 0xff800000u;
-        }
-        // ---- row maximum (4 independent chains) ----
-        float mx0 = -INFINITY, mx1 = -INFINITY, mx2 = -INFINITY, mx3 = -INFINITY;
-#pragma unroll
-        for (int i = 0; i < 128; i += 4) {
-          mx0 = fmaxf(mx0, __uint_as_float(s[i]));
-          mx1 = fmaxf(mx1, __uint_as_float(s[i + 1]));
-          mx2 = fmaxf(mx2, __uint_as_float(s[i + 2]));
-          mx3 = fmaxf(mx3, __uint_as_float(s[i + 3]));
-        }
-        const float m_true = fmaxf(fmaxf(mx0, mx1), fmaxf(mx2, mx3)) * p.scale_log2;
-        // lazy rescaling: keep the old reference maximum unless the row maximum grew by more than 2^8
-        const bool raise = m_true > m_used + kRescaleThreshold;  // always true on the first tile (m_used = -inf)
-        const float m_new = raise ? m_true : m_used;
-        const float factor = raise ? ex2_approx(m_used - m_new) : 1.0f;  // first tile: exp2(-inf) = 0
-        l *= factor;
-        m_used = m_new;
-        // the previous P V of this group must be complete before P is overwritten (and before O is rescaled)
-        if (j > 0) {
-          mbar_wait(&o_full[grp], (n - 1) & 1);
-          if (__any_sync(0xffffffffu, raise)) {
-            tc_fence_after();
-#pragma unroll
-            for (int c = 0; c < 64; c += 32) {
-              uint32_t o[32];
-              tmem_ld32(tO + c, o);
-              tmem_ld_wait();
-#pragma unroll
-              for (int i = 0; i < 32; ++i) o[i] = __float_as_uint(__uint_as_float(o[i]) * factor);
-              tmem_st32(tO + c, o);
-            }
-            if constexpr (FEAT & AF_ONES) {
-              const uint32_t lv = tmem_ld1(tL);
-              tmem_ld_wait();
-              tmem_st1(tL, __float_as_uint(__uint_as_float(lv) * factor));
-            }
-            tmem_st_wait();
-          }
-        }
-        if (j == 0 && it > 0) {
-          // the previous item's output tile was staged in this P buffer: its TMA store must have read it
-          if (warp == 4 + 4 * grp && lane == 0) tma_store_wait_read();
-          named_bar_sync(1 + grp, 128);
-        }
-        // ---- P = exp2(S*c - m_used) -> bf16, 128B-swizzled K-major tile in this group's P buffer ----
-        float rs0 = 0.f, rs1 = 0.f, rs2 = 0.f, rs3 = 0.f;
-        [[maybe_unused]] uint64_t rsA = 0, rsB = 0;  // AF_X2: two packed pairs of row-sum partials
-        [[maybe_unused]] const uint64_t sc2 = f32x2_pack(p.scale_log2, p.scale_log2), nm2 = f32x2_pack(-m_used, -m_used);
-        [[maybe_unused]] uint32_t pk[32];
-        turn_wait();
-#pragma unroll
-        for (int c = 0; c < 16; ++c) {  // 16-byte chunks of 8 keys
-          float e[8];
-          if constexpr (FEAT & AF_X2) {
-#pragma unroll
-            for (int i = 0; i < 8; i += 2) {
-              float t0, t1;
-              f32x2_unpack(f32x2_fma(f32x2_pack(__uint_as_float(s[8 * c + i]), __uint_as_float(s[8 * c + i + 1])), sc2, nm2), t0, t1);
-              e[i] = ex2_approx(t0);
-              e[i + 1] = ex2_approx(t1);
-            }
-            if constexpr (!(FEAT & AF_ONES)) {
-              rsA = f32x2_add(rsA, f32x2_pack(e[0], e[1]));
-              rsB = f32x2_add(rsB, f32x2_pack(e[2], e[3]));
-              rsA = f32x2_add(rsA, f32x2_pack(e[4], e[5]));
-              rsB = f32x2_add(rsB, f32x2_pack(e[6], e[7]));
-            }
-          } else {
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            const float x = fmaf(__uint_as_float(s[8 * c + i]), p.scale_log2, -m_used);
-            e[i] = ((FEAT & AF_EMU) && (i == 3 || i == 7)) ? ex2_fma(x) : ex2_approx(x);
-          }
-          if constexpr (!(FEAT & AF_ONES)) {
-            rs0 += e[0] + e[4];
-            rs1 += e[1] + e[5];
-            rs2 += e[2] + e[6];
-            rs3 += e[3] + e[7];
-          }
-          }
-          uint4 q;
-          q.x = pack_bf16x2(e[0], e[1]);
-          q.y = pack_bf16x2(e[2], e[3]);
-          q.z = pack_bf16x2(e[4], e[5]);
-          q.w = pack_bf16x2(e[6], e[7]);
-          if constexpr (FEAT & AF_PTMEM) {
-            // packed probabilities of 64 keys are collected in 32 registers and leave with one tcgen05.st
-            pk[4 * (c & 7) + 0] = q.x; pk[4 * (c & 7) + 1] = q.y; pk[4 * (c & 7) + 2] = q.z; pk[4 * (c & 7) + 3] = q.w;
-            if ((c & 7) == 7) tmem_st32(tP + 32 * (c >> 3), pk);
-          } else {
-            *reinterpret_cast<uint4*>(prow + (c >> 3) * TILE_BYTES + (((c & 7) ^ rx) << 4)) = q;
-          }
-        }
-        turn_pass();
-        if constexpr (FEAT & AF_X2) {
-          f32x2_unpack(rsA, rs0, rs1);
-          f32x2_unpack(rsB, rs2, rs3);
-        }
-        l += (rs0 + rs1) + (rs2 + rs3);
-        if constexpr (FEAT & AF_PTMEM) tmem_st_wait();
-        else fence_proxy_async_smem();
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&p_full[grp]);
-      }
-      // ---- item epilogue: O / l -> bf16 -> 128B-swizzled smem tile (the idle P buffer) -> one TMA store ----
-      mbar_wait(&o_full[grp], (n - 1) & 1);
-      tc_fence_after();
-      if constexpr (FEAT & AF_ONES) {
-        l = __uint_as_float(tmem_ld1(tL));
-        tmem_ld_wait();
-      }
-      const float inv_l = 1.0f / l;
-#pragma unroll
-      for (int c = 0; c < 64; c += 32) {
-        uint32_t o[32];
-        tmem_ld32(tO + c, o);
-        tmem_ld_wait();
-#pragma unroll
-        for (int jc = 0; jc < 4; ++jc) {
-          uint4 q;
-          q.x = pack_bf16x2(__uint_as_float(o[8 * jc + 0]) * inv_l, __uint_as_float(o[8 * jc + 1]) * inv_l);
-          q.y = pack_bf16x2(__uint_as_float(o[8 * jc + 2]) * inv_l, __uint_as_float(o[8 * jc + 3]) * inv_l);
-          q.z = pack_bf16x2(__uint_as_float(o[8 * jc + 4]) * inv_l, __uint_as_float(o[8 * jc + 5]) * inv_l);
-          q.w = pack_bf16x2(__uint_as_float(o[8 * jc + 6]) * inv_l, __uint_as_float(o[8 * jc + 7]) * inv_l);
-          *reinterpret_cast<uint4*>(prow + ((((c >> 3) + jc) ^ rx) << 4)) = q;
-        }
-      }
-      tc_fence_before();  // the next item's first P V overwrites O only after p_full, i.e. after these loads
-      fence_proxy_async_smem();
-      named_bar_sync(1 + grp, 128);
-      if (warp == 4 + 4 * grp && lane == 0) {
-        // rows >= nq (ragged last tile, or a dead second tile) are clipped by the TMA unit
-        tma_store_3d(&tmO, sP + grp * 2 * TILE_BYTES, head * 64, q0 + grp * 128, b);
-        tma_store_commit();
-      }
+    for (int c = 0; c < 8; ++c) {
+      if (row < p.nq) *reinterpret_cast<uint32_t*>(oa + 8 * c) = pack_bf16x2(o[4 * c] * inv0, o[4 * c + 1] * inv0);
+      if (row + 8 < p.nq) *reinterpret_cast<uint32_t*>(ob + 8 * c) = pack_bf16x2(o[4 * c + 2] * inv1, o[4 * c + 3] * inv1);
     }
-    if (pingpong && grp == 0) named_bar_sync(3, 256);  // consume group B's last hand-over
-    if (warp == 4 + 4 * grp && lane == 0) tma_store_wait_all();
-    tc_fence_before();
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
-  }
-}
-
-// ---------------------------------------------------------------------------
-// AF_1Q: the same pipeline with ONE 128-query tile per CTA and TWO CTAs per SM (256 threads, 112 KB of shared memory and 256
-// TMEM columns each: S 128 | O 64 | P 64).  The two query tiles that share an SM are then driven by two independent
-// MMA-issuing threads (in the pair kernel one in-order thread serves both softmax groups), work items are single tiles (the
-// decoder's 769 rows cost 7 tiles, not 4 pairs = 8), and the co-resident CTAs drift apart by themselves, so one CTA's exp2
-// phase overlaps the other's TMEM load / row maximum / handshakes without named-barrier ping-pong.  K / V tiles are loaded
-// once per CTA (twice per SM): L2 -> shared-memory traffic is not what bounds this kernel.
-// setmaxnreg: 128 registers per thread at launch (2 x 256 threads per SM), warps 0-3 shrink to 40, the softmax warpgroup
-// grows to 216 -- exactly the file.
-// ---------------------------------------------------------------------------
-constexpr int ATT1_THREADS = 256;
-constexpr int KV1_STAGES = 2;
-constexpr uint32_t ATT1_OFF_K = 2 * TILE_BYTES;                         // Q x2 | K x2 | V x2 | O staging | barriers
-constexpr uint32_t ATT1_OFF_V = ATT1_OFF_K + KV1_STAGES * TILE_BYTES;
-constexpr uint32_t ATT1_OFF_O = ATT1_OFF_V + KV1_STAGES * TILE_BYTES;
-constexpr uint32_t ATT1_OFF_BAR = ATT1_OFF_O + TILE_BYTES;
-constexpr uint32_t ATT1_SMEM = ATT1_OFF_BAR + 256;
-static_assert(2 * (ATT1_SMEM + 1024) <= 228 * 1024, "two attention CTAs per SM");
-
-template <bool X2>
-__global__ void __launch_bounds__(ATT1_THREADS, 2)
-attention_1q_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
-                    const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmO, const AttnParams p,
-                    int q_col0, int k_col0, int v_col0) {
-  extern __shared__ __align__(1024) uint8_t smem[];
-  uint8_t* sQ = smem;  // buffer b at sQ + b * TILE_BYTES
-  uint8_t* sK = smem + ATT1_OFF_K;
-  uint8_t* sV = smem + ATT1_OFF_V;
-  uint8_t* sO = smem + ATT1_OFF_O;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + ATT1_OFF_BAR);
-  uint64_t* q_full = bars + 0;   // [2]
-  uint64_t* q_empty = bars + 2;  // [2]
-  uint64_t* k_full = bars + 4;   // [2]
-  uint64_t* k_empty = bars + 6;  // [2]
-  uint64_t* v_full = bars + 8;   // [2]
-  uint64_t* v_empty = bars + 10; // [2]
-  uint64_t* s_full = bars + 12;  // MMA -> softmax: S ready
-  uint64_t* s_free = bars + 13;  // softmax -> MMA: S is in registers
-  uint64_t* p_full = bars + 14;  // softmax -> MMA: P written to TMEM (and O rescaled if needed)
-  uint64_t* o_full = bars + 15;  // MMA -> softmax: O += P V done
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 16);
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const int T = (p.nk + 127) / 128;
-
-  if (threadIdx.x == 0) {
-    if ((smem_u32(smem) & 1023u) != 0) device_fatal("dynamic shared memory is not 1024-byte aligned");
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&q_full[i], 1);
-      mbar_init(&q_empty[i], 1);
-      mbar_init(&k_full[i], 1);
-      mbar_init(&k_empty[i], 1);
-      mbar_init(&v_full[i], 1);
-      mbar_init(&v_empty[i], 1);
-    }
-    mbar_init(s_full, 1);
-    mbar_init(s_free, 4);
-    mbar_init(p_full, 4);
-    mbar_init(o_full, 1);
-    fence_mbar_init();
-  }
-  if (warp == 1) {
-    tmem_alloc(tmem_slot, 256);
-    tmem_relinquish();
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;  // columns: S [0,128) O [128,192) P [192,256)
-  pdl_wait();
-  pdl_launch_dependents();
-
-  const int qtiles = (p.nq - p.q_row0 + 127) / 128;
-  const int nitems = qtiles * p.heads * p.batch;
-  auto decode = [&](int w, int& q0, int& head, int& b, int& kvb) {
-    const int qt = w % qtiles;  // query tile fastest: the tiles of one (sample, head) run side by side and share K / V in L2
-    const int rest = w / qtiles;
-    head = rest % p.heads;
-    b = rest / p.heads;
-    q0 = p.q_row0 + qt * 128;
-    kvb = (b + p.kv_batch_shift) % p.batch;
-  };
-  const int my_items = (nitems > static_cast<int>(blockIdx.x))
-                           ? (nitems - 1 - static_cast<int>(blockIdx.x)) / static_cast<int>(gridDim.x) + 1
-                           : 0;
-
-  if (warp < 4) {
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;" ::: "memory");
-    if (warp == 0) {
-      // ===================== TMA producer =====================
-      if (elect_one()) {
-        tma_prefetch_desc(&tmQ);
-        tma_prefetch_desc(&tmK);
-        tma_prefetch_desc(&tmV);
-        int st = 0;
-        uint32_t ph = 0;
-        for (int it = 0; it < my_items; ++it) {
-          int q0, head, b, kvb;
-          decode(static_cast<int>(blockIdx.x) + it * static_cast<int>(gridDim.x), q0, head, b, kvb);
-          const int qb = it & 1;
-          mbar_wait(&q_empty[qb], ((it >> 1) & 1) ^ 1);
-          mbar_arrive_expect_tx(&q_full[qb], TILE_BYTES);
-          tma_load_3d(sQ + qb * TILE_BYTES, &tmQ, &q_full[qb], q_col0 + head * 64, q0, b);
-          for (int j = 0; j < T; ++j) {
-            mbar_wait(&k_empty[st], ph ^ 1);
-            mbar_arrive_expect_tx(&k_full[st], TILE_BYTES);
-            tma_load_3d(sK + st * TILE_BYTES, &tmK, &k_full[st], k_col0 + head * 64, j * 128, kvb);
-            mbar_wait(&v_empty[st], ph ^ 1);
-            mbar_arrive_expect_tx(&v_full[st], TILE_BYTES);
-            tma_load_3d(sV + st * TILE_BYTES, &tmV, &v_full[st], v_col0 + head * 64, j * 128, kvb);
-            if (++st == KV1_STAGES) { st = 0; ph ^= 1; }
-          }
-        }
-      }
-    } else if (warp == 1) {
-      // ===================== MMA issuer =====================
-      if (elect_one()) {
-        constexpr uint32_t idesc_s = make_idesc_bf16(128, 128, 0, 0);
-        constexpr uint32_t idesc_s16 = make_idesc_bf16(128, 16, 0, 0);  // narrow tail tile (<= 16 valid keys)
-        constexpr uint32_t idesc_o = make_idesc_bf16(128, 64, 0, 1);    // B (= V) is MN-major
-        const bool narrow_tail = (p.nk - (T - 1) * 128) <= 16;
-        const int total = my_items * T;
-        int s_it = 0, s_j = 0, s_st = 0;
-        uint32_t s_ph = 0;
-        auto issue_s = [&]() {
-          const int qi = s_it & 1;
-          if (s_j == 0) mbar_wait(&q_full[qi], (s_it >> 1) & 1);
-          mbar_wait(&k_full[s_st], s_ph);
-          tc_fence_after();
-          const uint64_t qdesc = make_smem_desc_sw128(smem_u32(sQ + qi * TILE_BYTES));
-          const uint64_t kdesc = make_smem_desc_sw128(smem_u32(sK + s_st * TILE_BYTES));
-          const uint32_t ids = (narrow_tail && s_j == T - 1) ? idesc_s16 : idesc_s;
-#pragma unroll
-          for (int k = 0; k < 4; ++k) umma_bf16(tmem_base, qdesc + 2 * k, kdesc + 2 * k, ids, k != 0);
-          umma_commit(&k_empty[s_st]);
-          if (s_j == T - 1) umma_commit(&q_empty[qi]);
-          umma_commit(s_full);
-          if (++s_st == KV1_STAGES) { s_st = 0; s_ph ^= 1; }
-          if (++s_j == T) { s_j = 0; ++s_it; }
-        };
-        if (total > 0) issue_s();
-        int v_st = 0, j = 0;
-        uint32_t v_ph = 0;
-        for (int n = 0; n < total; ++n) {
-          ATTN_STAMP(blockIdx.x == 0 && n < 24, 8 * n + 0);
-          if (n + 1 < total) {  // S(n+1) as soon as the softmax threads hold S(n) in registers
-            mbar_wait(s_free, n & 1);
-            ATTN_STAMP(blockIdx.x == 0 && n < 24, 8 * n + 1);
-            issue_s();
-          }
-          ATTN_STAMP(blockIdx.x == 0 && n < 24, 8 * n + 2);
-          mbar_wait(p_full, n & 1);
-          ATTN_STAMP(blockIdx.x == 0 && n < 24, 8 * n + 3);
-          mbar_wait(&v_full[v_st], v_ph);
-          ATTN_STAMP(blockIdx.x == 0 && n < 24, 8 * n + 4);
-          tc_fence_after();
-          const uint64_t vdesc = make_smem_desc_sw128(smem_u32(sV + v_st * TILE_BYTES));
-          const int ksteps = (narrow_tail && j == T - 1) ? 1 : 8;
-          for (int k = 0; k < ksteps; ++k)  // A = P from tensor memory (8 packed columns per 16 keys), B = V (MN-major)
-            umma_bf16_ts(tmem_base + 128, tmem_base + 192 + 8 * k, vdesc + (2048 >> 4) * k, idesc_o, (j > 0 || k > 0) ? 1u : 0u);
-          umma_commit(&v_empty[v_st]);
-          umma_commit(o_full);
-          ATTN_STAMP(blockIdx.x == 0 && n < 24, 8 * n + 5);
-          if (++v_st == KV1_STAGES) { v_st = 0; v_ph ^= 1; }
-          if (++j == T) j = 0;
-        }
-      }
-    }
-  } else {
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 216;" ::: "memory");
-    // ===================== softmax warpgroup: one thread per query row =====================
-    const int quarter = warp & 3;
-    const int r = quarter * 32 + lane;
-    const uint32_t lane_addr = static_cast<uint32_t>(quarter * 32) << 16;
-    const int rx = r & 7;
-    const uint32_t tS = tmem_base + lane_addr;
-    const uint32_t tO = tmem_base + lane_addr + 128;
-    const uint32_t tP = tmem_base + lane_addr + 192;
-    uint8_t* orow = sO + r * 128;
-    const bool store_thr = warp == 4 && lane == 0;
-    int n = 0;
-    for (int it = 0; it < my_items; ++it) {
-      int q0, head, b, kvb;
-      decode(static_cast<int>(blockIdx.x) + it * static_cast<int>(gridDim.x), q0, head, b, kvb);
-      float m_used = -INFINITY;
-      float l = 0.f;
-      for (int j = 0; j < T; ++j, ++n) {
-        const int nvalid = p.nk - j * 128;  // >= 1
-        [[maybe_unused]] const bool trc = blockIdx.x == 0 && threadIdx.x == 128 && n < 24;
-        ATTN_STAMP(trc, 256 + 8 * n + 0);
-        mbar_wait(s_full, n & 1);
-        ATTN_STAMP(trc, 256 + 8 * n + 1);
-        tc_fence_after();
-        if (nvalid <= 16 && j == T - 1) {
-          // ---- narrow tail tile: S is 128 x 16, P V uses a single 16-key step ----
-          uint32_t s16[16];
-          tmem_ld16(tS, s16);
-          tmem_ld_wait();
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(s_free);
-          float mxn = -INFINITY;
-#pragma unroll
-          for (int i = 0; i < 16; ++i) {
-            if (i >= nvalid) s16[i] = 0xff800000u;
-            mxn = fmaxf(mxn, __uint_as_float(s16[i]));
-          }
-          const float m_true = mxn * p.scale_log2;
-          const bool raise = m_true > m_used + kRescaleThreshold;
-          const float m_new = raise ? m_true : m_used;
-          const float factor = raise ? ex2_approx(m_used - m_new) : 1.0f;
-          l *= factor;
-          m_used = m_new;
-          if (j > 0) {
-            mbar_wait(o_full, (n - 1) & 1);
-            if (__any_sync(0xffffffffu, raise)) {
-              tc_fence_after();
-#pragma unroll
-              for (int c = 0; c < 64; c += 32) {
-                uint32_t o[32];
-                tmem_ld32(tO + c, o);
-                tmem_ld_wait();
-#pragma unroll
-                for (int i = 0; i < 32; ++i) o[i] = __float_as_uint(__uint_as_float(o[i]) * factor);
-                tmem_st32(tO + c, o);
-              }
-            }
-          }
-          float rs = 0.f;
-#pragma unroll
-          for (int c = 0; c < 2; ++c) {
-            float e[8];
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-              e[i] = ex2_approx(fmaf(__uint_as_float(s16[8 * c + i]), p.scale_log2, -m_used));
-              rs += e[i];
-            }
-            tmem_st4(tP + 4 * c, make_uint4(pack_bf16x2(e[0], e[1]), pack_bf16x2(e[2], e[3]), pack_bf16x2(e[4], e[5]),
-                                            pack_bf16x2(e[6], e[7])));
-          }
-          l += rs;
-          tmem_st_wait();
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(p_full);
-          continue;
-        }
-        // ---- the whole score row into registers; release the S buffer for the next Q K^T ----
-        uint32_t s[128];
-        {
-          uint32_t (&s0)[32] = *reinterpret_cast<uint32_t(*)[32]>(&s[0]);
-          uint32_t (&s1)[32] = *reinterpret_cast<uint32_t(*)[32]>(&s[32]);
-          uint32_t (&s2)[32] = *reinterpret_cast<uint32_t(*)[32]>(&s[64]);
-          uint32_t (&s3)[32] = *reinterpret_cast<uint32_t(*)[32]>(&s[96]);
-          tmem_ld32(tS, s0);
-          tmem_ld32(tS + 32, s1);
-          tmem_ld32(tS + 64, s2);
-          tmem_ld32(tS + 96, s3);
-          tmem_ld_wait();
-        }
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(s_free);
-        if (nvalid < 128) {  // ragged last key tile: masked scores contribute exp2(-inf) = 0
-#pragma unroll
-          for (int i = 0; i < 128; ++i)
-            if (i >= nvalid) s[i] = 0xff800000u;
-        }
-        float mx0 = -INFINITY, mx1 = -INFINITY, mx2 = -INFINITY, mx3 = -INFINITY;
-#pragma unroll
-        for (int i = 0; i < 128; i += 4) {
-          mx0 = fmaxf(mx0, __uint_as_float(s[i]));
-          mx1 = fmaxf(mx1, __uint_as_float(s[i + 1]));
-          mx2 = fmaxf(mx2, __uint_as_float(s[i + 2]));
-          mx3 = fmaxf(mx3, __uint_as_float(s[i + 3]));
-        }
-        const float m_true = fmaxf(fmaxf(mx0, mx1), fmaxf(mx2, mx3)) * p.scale_log2;
-        ATTN_STAMP(trc, 256 + 8 * n + 2);
-        // lazy rescaling: keep the old reference maximum unless the row maximum grew by more than 2^8
-        const bool raise = m_true > m_used + kRescaleThreshold;  // always true on the first tile (m_used = -inf)
-        const float m_new = raise ? m_true : m_used;
-        const float factor = raise ? ex2_approx(m_used - m_new) : 1.0f;  // first tile: exp2(-inf) = 0
-        l *= factor;
-        m_used = m_new;
-        // the previous P V must be complete before P is overwritten (and before O is rescaled)
-        if (j > 0) {
-          mbar_wait(o_full, (n - 1) & 1);
-          if (__any_sync(0xffffffffu, raise)) {
-            tc_fence_after();
-#pragma unroll
-            for (int c = 0; c < 64; c += 32) {
-              uint32_t o[32];
-              tmem_ld32(tO + c, o);
-              tmem_ld_wait();
-#pragma unroll
-              for (int i = 0; i < 32; ++i) o[i] = __float_as_uint(__uint_as_float(o[i]) * factor);
-              tmem_st32(tO + c, o);
-            }
-          }
-        }
-        ATTN_STAMP(trc, 256 + 8 * n + 3);
-        // ---- P = exp2(S*c - m_used) -> packed bf16 -> tensor memory (64 keys per tcgen05.st) ----
-        float rs0 = 0.f, rs1 = 0.f, rs2 = 0.f, rs3 = 0.f;
-        [[maybe_unused]] uint64_t rsA = 0, rsB = 0;  // X2: two packed pairs of row-sum partials
-        [[maybe_unused]] const uint64_t sc2 = f32x2_pack(p.scale_log2, p.scale_log2), nm2 = f32x2_pack(-m_used, -m_used);
-        uint32_t pk[32];
-#pragma unroll
-        for (int c = 0; c < 16; ++c) {
-          float e[8];
-          if constexpr (X2) {
-#pragma unroll
-            for (int i = 0; i < 8; i += 2) {
-              float t0, t1;
-              f32x2_unpack(f32x2_fma(f32x2_pack(__uint_as_float(s[8 * c + i]), __uint_as_float(s[8 * c + i + 1])), sc2, nm2), t0, t1);
-              e[i] = ex2_approx(t0);
-              e[i + 1] = ex2_approx(t1);
-            }
-            rsA = f32x2_add(rsA, f32x2_pack(e[0], e[1]));
-            rsB = f32x2_add(rsB, f32x2_pack(e[2], e[3]));
-            rsA = f32x2_add(rsA, f32x2_pack(e[4], e[5]));
-            rsB = f32x2_add(rsB, f32x2_pack(e[6], e[7]));
-          } else {
-#pragma unroll
-            for (int i = 0; i < 8; ++i) e[i] = ex2_approx(fmaf(__uint_as_float(s[8 * c + i]), p.scale_log2, -m_used));
-            rs0 += e[0] + e[4];
-            rs1 += e[1] + e[5];
-            rs2 += e[2] + e[6];
-            rs3 += e[3] + e[7];
-          }
-          pk[4 * (c & 7) + 0] = pack_bf16x2(e[0], e[1]);
-          pk[4 * (c & 7) + 1] = pack_bf16x2(e[2], e[3]);
-          pk[4 * (c & 7) + 2] = pack_bf16x2(e[4], e[5]);
-          pk[4 * (c & 7) + 3] = pack_bf16x2(e[6], e[7]);
-          if ((c & 7) == 7) tmem_st32(tP + 32 * (c >> 3), pk);
-        }
-        if constexpr (X2) {
-          f32x2_unpack(rsA, rs0, rs1);
-          f32x2_unpack(rsB, rs2, rs3);
-        }
-        l += (rs0 + rs1) + (rs2 + rs3);
-        ATTN_STAMP(trc, 256 + 8 * n + 5);
-        tmem_st_wait();
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(p_full);
-        ATTN_STAMP(trc, 256 + 8 * n + 6);
-      }
-      // ---- item epilogue: O / l -> bf16 -> 128B-swizzled staging tile -> one TMA store ----
-      mbar_wait(o_full, (n - 1) & 1);
-      tc_fence_after();
-      if (it > 0) {  // the previous item's TMA store must have finished reading the staging tile
-        if (store_thr) tma_store_wait_read();
-        named_bar_sync(1, 128);
-      }
-      const float inv_l = 1.0f / l;
-#pragma unroll
-      for (int c = 0; c < 64; c += 32) {
-        uint32_t o[32];
-        tmem_ld32(tO + c, o);
-        tmem_ld_wait();
-#pragma unroll
-        for (int jc = 0; jc < 4; ++jc) {
-          uint4 q;
-          q.x = pack_bf16x2(__uint_as_float(o[8 * jc + 0]) * inv_l, __uint_as_float(o[8 * jc + 1]) * inv_l);
-          q.y = pack_bf16x2(__uint_as_float(o[8 * jc + 2]) * inv_l, __uint_as_float(o[8 * jc + 3]) * inv_l);
-          q.z = pack_bf16x2(__uint_as_float(o[8 * jc + 4]) * inv_l, __uint_as_float(o[8 * jc + 5]) * inv_l);
-          q.w = pack_bf16x2(__uint_as_float(o[8 * jc + 6]) * inv_l, __uint_as_float(o[8 * jc + 7]) * inv_l);
-          *reinterpret_cast<uint4*>(orow + ((((c >> 3) + jc) ^ rx) << 4)) = q;
-        }
-      }
-      tc_fence_before();  // the next item's first P V overwrites O only after p_full, i.e. after these loads
-      fence_proxy_async_smem();
-      named_bar_sync(1, 128);
-      if (store_thr) {
-        tma_store_3d(&tmO, sO, head * 64, q0, b);  // rows >= nq are clipped by the TMA unit
-        tma_store_commit();
-      }
-    }
-    if (store_thr) tma_store_wait_all();
-    tc_fence_before();
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 256);
   }
 }
 
@@ -1181,21 +431,26 @@ attention_x3_kernel(const __nv_bfloat16* __restrict__ q, long long ldq, int q_co
   }
 }
 
-int make_qkv_map(CUtensorMap* m, const bf16* base, long long ld, int ntok, int batch) {
+int make_qkv_map(CUtensorMap* m, const bf16* base, long long ld, int ntok, int batch, uint32_t rows = 128) {
   uint64_t dims[3] = {(uint64_t)ld, (uint64_t)ntok, (uint64_t)batch};
   uint64_t strides[2] = {(uint64_t)ld * 2, (uint64_t)ld * 2 * (uint64_t)ntok};
-  uint32_t box[3] = {64, 128, 1};
+  uint32_t box[3] = {64, rows, 1};
   return make_tmap_bf16(m, base, 3, dims, strides, box);
 }
 
 }  // namespace
 
-// Default feature set, from the same-box A/B measurements in profiles/r02_attn_ab_*.log (stand-alone, n = 768 / 769):
-// round-1 kernel 586 / 405 TF/s; AF_PTMEM 647 / 453 (+10 %); AF_SKIP +1.7 % at n = 769 only (and compute-sanitizer's
-// synccheck objects to the ping-pong named barrier being reached from the dead-warp skeleton's own call site, so it stays
-// opt-in); AF_ONES +-0; AF_EMU -6 %; no ping-pong -14 %.  Variants that were built, measured and removed again (git history,
-// logs under profiles/): a two-pass register-light softmax (-15 %), two threads per query row at 96 registers (-45 %, spills).
-constexpr int kDefaultFeat = AF_PTMEM | AF_X2;
+template <int CWG>
+static int launch_attention_inst(const CUtensorMap& tmQ, const CUtensorMap& tmK, const CUtensorMap& tmV, const AttnParams& p,
+                                 const AttnLaunch& a, long long items, cudaStream_t stream) {
+  static PerDeviceOnce once;  // the opt-in is per device, not per process
+  STA_CHECK_CUDA(once.run([&] {
+    return cudaFuncSetAttribute(attention_fwd_kernel<CWG>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ATT_SMEM);
+  }));
+  STA_CHECK_CUDA(launch_pdl(attention_fwd_kernel<CWG>, dim3(static_cast<unsigned>(items)), dim3(att_threads<CWG>()), ATT_SMEM,
+                            stream, 1, tmQ, tmK, tmV, p, a.q_col0, a.k_col0, a.v_col0));
+  return 0;
+}
 
 int launch_attention(const AttnLaunch& a, cudaStream_t stream) {
   STA_REQUIRE(a.batch > 0 && a.heads > 0 && a.nq > 0 && a.nk > 0, "empty attention problem");
@@ -1210,112 +465,42 @@ int launch_attention(const AttnLaunch& a, cudaStream_t stream) {
                               a.kv_batch_shift, a.scale * 1.4426950408889634f));
     return 0;
   }
-  CUtensorMap tmQ, tmK, tmV;
-  if (make_qkv_map(&tmQ, a.q, a.ldq, a.nq, a.batch)) return 1;
-  if (make_qkv_map(&tmK, a.k, a.ldk, a.nk, a.batch)) return 1;
-  if (make_qkv_map(&tmV, a.v, a.ldv, a.nk, a.batch)) return 1;
-  CUtensorMap tmO;
-  if (make_qkv_map(&tmO, a.out, a.ldo, a.nq, a.batch)) return 1;
   AttnParams p;
   p.nq = a.nq;
   p.nk = a.nk;
   p.batch = a.batch;
+  p.heads = a.heads;
   p.kv_batch_shift = a.kv_batch_shift;
   p.scale_log2 = a.scale * 1.4426950408889634f;
   p.out = a.out;
   p.ldo = a.ldo;
-  p.heads = a.heads;
-  {
-    const char* e = getenv("STA_ATTN_TRACE");
-    p.dbg = e ? reinterpret_cast<long long*>(strtoull(e, nullptr, 0)) : nullptr;
-  }
   const size_t row0_smem = (((a.nk + 3) & ~3) + 16 + 32 * 64) * sizeof(float);
-  static int pingpong_env = -1, feat_env = -2;
-  if (pingpong_env < 0) {
-    const char* e = getenv("STA_ATTN_PINGPONG");  // 0 disables (A/B timing)
-    pingpong_env = (e && e[0] == '0') ? 0 : 1;
-    e = getenv("STA_ATTN_FEAT");  // feature set of the softmax warpgroups (A/B timing; see AttnFeat)
-    feat_env = e ? atoi(e) : -1;
-  }
-  p.pingpong = pingpong_env;
   const int split = (a.split_first_row && a.nq > 1 && row0_smem <= 48 * 1024) ? 1 : 0;
   p.q_row0 = split;
-  p.qpairs = (a.nq - split + 255) / 256;
-  p.nitems = p.qpairs * a.heads * a.batch;
+  // Query tile: 128 rows (two consumer warpgroups share every K / V tile) unless that grid leaves SMs idle (small
+  // problems: SLAM-mode keyframes, low resolutions), then 64 rows (one warpgroup) for twice the CTAs.
+  // STA_ATTN_QROWS=64|128 forces one of the two (A/B timing).
+  static int qrows_env = -1;
+  if (qrows_env < 0) {
+    const char* e = getenv("STA_ATTN_QROWS");
+    qrows_env = e ? atoi(e) : 0;
+  }
+  const long long items128 = static_cast<long long>((a.nq - split + 127) / 128) * a.heads * a.batch;
+  const int qrows = (qrows_env == 64 || qrows_env == 128) ? qrows_env : (items128 < num_sms() ? 64 : 128);
+  p.qtiles = (a.nq - split + qrows - 1) / qrows;
+  CUtensorMap tmQ, tmK, tmV;
+  if (make_qkv_map(&tmQ, a.q, a.ldq, a.nq, a.batch, static_cast<uint32_t>(qrows))) return 1;
+  if (make_qkv_map(&tmK, a.k, a.ldk, a.nk, a.batch)) return 1;
+  if (make_qkv_map(&tmV, a.v, a.ldv, a.nk, a.batch)) return 1;
   if (split) {
-    const size_t smem = row0_smem;
-    STA_CHECK_CUDA(launch_pdl(attention_row0_kernel, dim3(a.heads, a.batch), dim3(256), smem, stream, 1, a.q, a.ldq, a.q_col0, a.k,
-                              a.ldk, a.k_col0, a.v, a.ldv, a.v_col0, a.out, a.ldo, a.nq, a.nk, a.batch, a.kv_batch_shift,
+    STA_CHECK_CUDA(launch_pdl(attention_row0_kernel, dim3(a.heads, a.batch), dim3(256), row0_smem, stream, 1, a.q, a.ldq, a.q_col0,
+                              a.k, a.ldk, a.k_col0, a.v, a.ldv, a.v_col0, a.out, a.ldo, a.nq, a.nk, a.batch, a.kv_batch_shift,
                               p.scale_log2));
   }
-  int feat = feat_env >= 0 ? feat_env : kDefaultFeat;
-  if (feat_env < 0) {
-    // One query tile per CTA (attention_1q_kernel) when the pair kernel would waste work: an odd number of query tiles (the
-    // decoder's 769 rows = 7 tiles: the 4th pair carries a dead tile; 525 vs 457 TF/s) or fewer pairs than SMs (SLAM mode:
-    // twice as many work items).  On full pairs the two kernels are equal (648 vs 653 TF/s) and the pair kernel loads K / V
-    // once per SM instead of twice.
-    const int qtiles = (a.nq - split + 127) / 128;
-    if ((qtiles & 1) || p.nitems < num_sms()) feat = AF_1Q | AF_X2;
-  }
-  // Work items w = (query-tile pair fastest, head, sample) are dealt round-robin to the CTAs (w = blockIdx + it * grid), so
-  // that neighbouring CTAs work on the pairs of ONE (sample, head) at the same time and share its K / V tiles in L2.  The
-  // last pair of a 128k+1-row problem (the decoder's 769 rows) is much cheaper than the others (AF_SKIP): the grid is made
-  // coprime with the pair count, otherwise a CTA would only ever see one kind of item (148 = 4 x 37) and the cheap ones
-  // would not shorten the kernel at all.
-  int grid = p.nitems < num_sms() ? p.nitems : num_sms();
-  if ((feat & AF_SKIP) && (p.nq - p.q_row0) % 256 != 0 && p.nitems > grid) {
-    auto gcd = [](int x, int y) { while (y) { const int t = x % y; x = y; y = t; } return x; };
-    while (grid > 1 && gcd(grid, p.qpairs) != 1) --grid;
-  }
-#define STA_ATTN_CASE(F)                                                                                                    \
-  if (feat == (F)) {                                                                                                        \
-    static PerDeviceOnce once; /* the opt-in is per device, not per process */                                              \
-    STA_CHECK_CUDA(once.run([&] {                                                                                           \
-      return cudaFuncSetAttribute(attention_fwd_kernel<(F)>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ATT_SMEM);   \
-    }));                                                                                                                    \
-    STA_CHECK_CUDA(launch_pdl(attention_fwd_kernel<(F)>, dim3(grid), dim3(ATT_THREADS), ATT_SMEM, stream, 1, tmQ, tmK, tmV, \
-                              tmO, p, a.q_col0, a.k_col0, a.v_col0));                                                       \
-    return 0;                                                                                                               \
-  }
-  STA_ATTN_CASE(0)
-  STA_ATTN_CASE(AF_SKIP)
-  STA_ATTN_CASE(AF_ONES)
-  STA_ATTN_CASE(AF_SKIP | AF_ONES)
-  STA_ATTN_CASE(AF_PTMEM)
-  STA_ATTN_CASE(AF_SKIP | AF_PTMEM)
-  STA_ATTN_CASE(AF_SKIP | AF_PTMEM | AF_EMU)
-  STA_ATTN_CASE(AF_PTMEM | AF_X2)
-#undef STA_ATTN_CASE
-#define STA_ATTN_1Q_CASE(X2)                                                                                                \
-  if (feat == (AF_1Q | ((X2) ? AF_X2 : 0))) {                                                                               \
-    static PerDeviceOnce once;                                                                                              \
-    STA_CHECK_CUDA(once.run([&] {                                                                                           \
-      cudaError_t e =                                                                                                       \
-          cudaFuncSetAttribute(attention_1q_kernel<X2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ATT1_SMEM);       \
-      if (e != cudaSuccess) return e;                                                                                       \
-      /* two CTAs per SM need the full 228 KB shared-memory carve-out */                                                    \
-      e = cudaFuncSetAttribute(attention_1q_kernel<X2>, cudaFuncAttributePreferredSharedMemoryCarveout,                     \
-                               (int)cudaSharedmemCarveoutMaxShared);                                                        \
-      if (e != cudaSuccess) return e;                                                                                       \
-      if (getenv("STA_ATTN_DEBUG")) {                                                                                       \
-        int nb = -1;                                                                                                        \
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, attention_1q_kernel<X2>, ATT1_THREADS, ATT1_SMEM);               \
-        fprintf(stderr, "attention_1q_kernel<%d>: %d resident CTAs per SM (occupancy API)\n", (int)(X2), nb);               \
-      }                                                                                                                     \
-      return cudaSuccess;                                                                                                   \
-    }));                                                                                                                    \
-    const int items1 = ((a.nq - split + 127) / 128) * a.heads * a.batch;                                                    \
-    static const int ctas_per_sm = (getenv("STA_ATTN_1Q_CTAS") && getenv("STA_ATTN_1Q_CTAS")[0] == '1') ? 1 : 2; /* A/B */    \
-    const int grid1 = items1 < ctas_per_sm * num_sms() ? items1 : ctas_per_sm * num_sms();                                  \
-    STA_CHECK_CUDA(launch_pdl(attention_1q_kernel<X2>, dim3(grid1), dim3(ATT1_THREADS), ATT1_SMEM, stream, 1, tmQ, tmK, tmV, \
-                              tmO, p, a.q_col0, a.k_col0, a.v_col0));                                                       \
-    return 0;                                                                                                               \
-  }
-  STA_ATTN_1Q_CASE(false)
-  STA_ATTN_1Q_CASE(true)
-#undef STA_ATTN_1Q_CASE
-  set_last_error("launch_attention: no kernel instance for this STA_ATTN_FEAT value");
-  return 2;
+  const long long items = static_cast<long long>(p.qtiles) * a.heads * a.batch;
+  STA_REQUIRE(items < (1LL << 31), "grid limits");
+  return qrows == 64 ? launch_attention_inst<1>(tmQ, tmK, tmV, p, a, items, stream)
+                     : launch_attention_inst<2>(tmQ, tmK, tmV, p, a, items, stream);
 }
 
 }  // namespace sta

@@ -1,5 +1,5 @@
-// Device-side PTX wrappers for sm_100a: mbarrier, TMA (cp.async.bulk.tensor),
-// tcgen05 (MMA / TMEM alloc / TMEM load / commit), plus small math helpers.
+// Device-side PTX wrappers for sm_90a: mbarrier, TMA (cp.async.bulk.tensor),
+// wgmma (warpgroup MMA, shared-memory descriptors), plus small math helpers.
 // Everything here is hand-written inline PTX; no CUTLASS/CuTe types are used.
 #pragma once
 #include <cuda_runtime.h>
@@ -18,15 +18,15 @@ namespace sta {
 // (implemented as device printf + __trap(): the host then sees a launch failure
 // instead of a hung GPU)
 __device__ __forceinline__ void device_fatal(const char* what) {
-  printf("[sta_b200 device fatal] %s (block %d thread %d)\n", what, (int)blockIdx.x, (int)threadIdx.x);
+  printf("[sta device fatal] %s (block %d thread %d)\n", what, (int)blockIdx.x, (int)threadIdx.x);
   __trap();
 }
 
 // Programmatic dependent launch: every kernel of the forward pass is launched with
-// cudaLaunchAttributeProgrammaticStreamSerialization, so its CTAs may start (barrier init, TMEM allocation,
-// descriptor prefetch) while the previous kernel drains.  pdl_wait() blocks until the previous kernel has
-// completed and flushed its memory -- it must precede every global-memory access; pdl_launch_dependents()
-// lets the next kernel begin its own prologue.
+// cudaLaunchAttributeProgrammaticStreamSerialization, so its CTAs may start (barrier init, descriptor prefetch)
+// while the previous kernel drains.  pdl_wait() blocks until the previous kernel has completed and flushed its
+// memory -- it must precede every global-memory access; pdl_launch_dependents() lets the next kernel begin its
+// own prologue.
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 
@@ -57,7 +57,7 @@ __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
 __device__ __forceinline__ void fence_mbar_init() {
   asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
 }
-// generic-proxy writes to shared memory -> visible to the async proxy (TMA / tcgen05.mma reads)
+// generic-proxy writes to shared memory -> visible to the async proxy (TMA / wgmma reads)
 __device__ __forceinline__ void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
@@ -82,14 +82,13 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
   return ok != 0;
 }
 // Blocking wait with a watchdog: a broken pipeline traps (kernel error) instead
-// of hanging the GPU box.  ~4 s at 2 GHz.
+// of hanging the GPU.  ~4 s at 2 GHz.  No printf here: a function call between a wgmma and its wait_group
+// makes ptxas serialise every wgmma of the kernel.
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   if (mbar_try_wait(bar, parity)) return;
   long long t0 = clock64();
   while (!mbar_try_wait(bar, parity)) {
-    if (clock64() - t0 > 8000000000LL) {
-      device_fatal("mbarrier wait timed out");
-    }
+    if (clock64() - t0 > 8000000000LL) __trap();
   }
 }
 
@@ -148,229 +147,72 @@ __device__ __forceinline__ void tma_store_wait_read1() { asm volatile("cp.async.
 __device__ __forceinline__ void tma_store_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 
 // ---------------------------------------------------------------------------
-// tcgen05: TMEM allocation, MMA, commit, TMEM loads
+// wgmma (sm_90a warpgroup MMA): issued by all 128 threads of a warpgroup, accumulators in registers
 // ---------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t* slot_in_smem, uint32_t ncols) {  // whole warp
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(slot_in_smem)),
-               "r"(ncols)
-               : "memory");
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// The registers an in-flight wgmma reads or writes must not be touched (or reallocated) by the compiler before the matching
+// wgmma_wait(); an empty asm that "modifies" them after the wait pins every later use behind it.
+template <int R>
+__device__ __forceinline__ void fence_regs(float (&r)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(r[i])::"memory");
 }
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+template <int R>
+__device__ __forceinline__ void fence_regs(uint32_t (&r)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+r"(r[i])::"memory");
 }
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {  // whole warp
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
-// D[tmem] (+)= A[smem desc] * B[smem desc], bf16 x bf16 -> fp32, issued by ONE thread.
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                          uint32_t accumulate) {
+// D[64 x 128] (+)= A[64 x 16](smem desc) * B[128 x 16]^T(smem desc), both K-major, bf16 -> fp32 registers.
+__device__ __forceinline__ void wgmma_m64n128k16_ss(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
   asm volatile(
       "{\n\t"
       ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
+      "setp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "%64, %65, p, 1, 1, 0, 0;\n\t"
+      "}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
-// Same with the A operand in TENSOR MEMORY (lane = row, 32-bit column = two consecutive bf16 K-elements): used by the
-// attention kernel for O += P V with P written by tcgen05.st, so that P never travels through shared memory.
-__device__ __forceinline__ void umma_bf16_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t bdesc, uint32_t idesc,
-                                             uint32_t accumulate) {
+// D[64 x 64] += A[64 x 16](registers, bf16x2) * B[16 x 64](smem desc, MN-major), fp32 registers.
+__device__ __forceinline__ void wgmma_m64n64k16_rs_mn(float (&d)[32], const uint32_t (&a)[4], uint64_t bdesc) {
   asm volatile(
       "{\n\t"
       ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t"
-      "}\n" ::"r"(tmem_d),
-      "r"(tmem_a), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// All previously issued tcgen05.mma of this thread arrive on `bar` when complete
-// (implies tcgen05.fence::before_thread_sync).
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-
-// TMEM -> registers: lane (= row) i of this warp's 32-lane quarter, 32 consecutive fp32 columns.
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];\n"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-// 16-column variant (narrow tail tiles)
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];\n"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-// registers -> TMEM (same 32x32b shape as tmem_ld32), used to rescale the O accumulator in place
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};\n" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-      "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]), "r"(r[18]),
-      "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]),
-      "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};\n" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-      "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_st4(uint32_t taddr, const uint4& v) {  // 4 consecutive columns of this lane
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x4.b32 [%0], {%1, %2, %3, %4};" ::"r"(taddr), "r"(v.x), "r"(v.y), "r"(v.z),
-               "r"(v.w)
-               : "memory");
-}
-// single-column variants (one fp32 per lane)
-__device__ __forceinline__ uint32_t tmem_ld1(uint32_t taddr) {
-  uint32_t r;
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x1.b32 {%0}, [%1];" : "=r"(r) : "r"(taddr) : "memory");
-  return r;
-}
-__device__ __forceinline__ void tmem_st1(uint32_t taddr, uint32_t v) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x1.b32 [%0], {%1};" ::"r"(taddr), "r"(v) : "memory");
+      "setp.ne.b32 p, %37, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+      "{%32, %33, %34, %35}, %36, p, 1, 1, 1;\n\t"
+      "}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(1u));
 }
 
 // ---------------------------------------------------------------------------
-// CTA-pair (cta_group::2) variants.  A cluster of 2 CTAs on one TPC cooperates on a
-// 256 x N tile: each CTA stages its own 128 rows of A and N/2 rows of B, the leader CTA
-// (cluster rank 0) issues the MMAs, each CTA's TMEM holds its own 128 accumulator rows.
+// wgmma shared-memory matrix descriptors (PTX ISA "Matrix Descriptor Format", sm_90)
+// bits [0,14) start>>4 | [16,30) LBO>>4 | [32,46) SBO>>4 | [49,52) base offset | [62,64) layout (1 = SWIZZLE_128B)
 // ---------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// arrive on the barrier at the same shared-memory offset in CTA `cta` of the cluster
-__device__ __forceinline__ void mbar_arrive_remote(uint64_t* bar, uint32_t cta) {
-  asm volatile(
-      "{\n\t"
-      ".reg .b32 ra;\n\t"
-      "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
-      "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [ra];\n\t"
-      "}\n" ::"r"(smem_u32(bar)),
-      "r"(cta)
-      : "memory");
-}
-// In a CTA pair the shared::cluster address of a local object carries the CTA rank in bit 24;
-// clearing it addresses the same offset in the leader CTA (rank 0).
-constexpr uint32_t kPeerBitMask = 0xFEFFFFFFu;
-__device__ __forceinline__ void tma_load_2d_cg2(void* dst, const CUtensorMap* m, uint64_t* leader_bar, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], "
-      "[%2];" ::"r"(smem_u32(dst)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(leader_bar) & kPeerBitMask), "r"(c0), "r"(c1)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_4d_cg2(void* dst, const CUtensorMap* m, uint64_t* leader_bar, int c0, int c1,
-                                                int c2, int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, "
-      "%6}], [%2];" ::"r"(smem_u32(dst)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(leader_bar) & kPeerBitMask), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_alloc_cg2(uint32_t* slot_in_smem, uint32_t ncols) {  // one warp in EACH CTA
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(slot_in_smem)),
-               "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish_cg2() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_cg2(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void umma_bf16_cg2(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                              uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// completion of all prior MMAs arrives on `bar` (same offset) in both CTAs of the pair
-__device__ __forceinline__ void umma_commit_cg2(uint64_t* bar) {
-  const uint16_t mask = 3;
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-          smem_u32(bar)),
-      "h"(mask)
-      : "memory");
-}
-
-// ---------------------------------------------------------------------------
-// UMMA descriptors (bit layouts: PTX ISA "tcgen05 matrix / instruction descriptor")
-// ---------------------------------------------------------------------------
-// Shared-memory matrix descriptor for a SWIZZLE_128B tile whose rows are 128 bytes
-// (64 bf16) and whose 8-row groups are 1024 bytes apart.
-//  * K-major operand  ([rows][64 k] tile written by a TMA box {64, rows}): SBO = 1024
-//  * MN-major operand ([k][64 mn] tile written by a TMA box {64, k}):      SBO = 1024
-// bits [0,14) start>>4 | [16,30) LBO>>4 | [32,46) SBO>>4 | [46,48) version=1 | [61,64) layout=2 (SW128)
-__device__ __forceinline__ uint64_t make_smem_desc_sw128(uint32_t saddr) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((saddr & 0x3FFFF) >> 4);
-  d |= static_cast<uint64_t>(1) << 16;             // LBO (ignored for swizzled layouts with one atom)
-  d |= static_cast<uint64_t>(1024 >> 4) << 32;     // SBO
-  d |= static_cast<uint64_t>(1) << 46;             // descriptor version (Blackwell)
-  d |= static_cast<uint64_t>(2) << 61;             // SWIZZLE_128B
-  return d;
-}
-// Same layout with an arbitrary stride between the 8-row groups and a start address that is only 128-byte (one row)
-// aligned.  Used by the halo-staged 3x3 convolution, whose nine filter taps are nine row-shifted views of ONE staged input
-// tile.  MEASURED on B200 (tools/conv_ab.py, profiles/r02_conv_ab_2.log): the tensor core applies the 128-byte swizzle to the
-// ABSOLUTE shared-memory address bits (chunk bits [4,7) ^= row bits [7,10)), exactly as TMA wrote the tile, so a row-shifted
-// start needs NO "matrix base offset" (bits [49,52)); setting it to (start >> 7) & 7 shifts the pattern a second time and
-// gives wrong results for every tap with a column shift.
+// SWIZZLE_128B tile whose rows are 128 bytes (64 bf16) and whose 8-row groups are sbo_bytes apart (1024 for a TMA box
+// {64, rows}).  K-major operand ([rows][64 k]): one k16 step advances the start by 32 bytes (+2 encoded).  MN-major
+// operand ([k][64 mn], used with the transpose bit): SBO is the stride between groups of 8 k-rows, one k16 step
+// advances the start by 2 * sbo_bytes.
+// The swizzle is a function of the absolute shared-memory address (chunk bits [4,7) ^= row bits [7,10)), exactly as TMA
+// wrote the tile, so a start address that is only 128-byte aligned (a row-shifted view: the halo-staged convolution) needs
+// no base offset.
 __device__ __forceinline__ uint64_t make_smem_desc_sw128_rows(uint32_t saddr, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((saddr & 0x3FFFF) >> 4);
   d |= static_cast<uint64_t>(1) << 16;
   d |= static_cast<uint64_t>(sbo_bytes >> 4) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
+  d |= static_cast<uint64_t>(1) << 62;
   return d;
 }
-// Instruction descriptor: bf16 A/B, fp32 accumulate, M x N tile.
-// bits [4,6) c_format=1(f32) | [7,10) a_format=1(bf16) | [10,13) b_format=1(bf16) | 15 a_major | 16 b_major
-//      [17,23) N>>3 | [24,29) M>>4
-__host__ __device__ constexpr uint32_t make_idesc_bf16(int M, int N, int a_mn_major, int b_mn_major) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | (static_cast<uint32_t>(a_mn_major) << 15) |
-         (static_cast<uint32_t>(b_mn_major) << 16) | (static_cast<uint32_t>(N >> 3) << 17) |
-         (static_cast<uint32_t>(M >> 4) << 24);
-}
+__device__ __forceinline__ uint64_t make_smem_desc_sw128(uint32_t saddr) { return make_smem_desc_sw128_rows(saddr, 1024); }
 
 // ---------------------------------------------------------------------------
 // small helpers
@@ -395,45 +237,6 @@ __device__ __forceinline__ float ex2_approx(float x) {
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
-// Packed fp32 pairs (sm_100: FFMA2 / FADD2 work on 64-bit register pairs at the rate of the scalar instructions).  The
-// attention softmax issues FFMA + EX2 + FADD + 1/2 F2FP per score: with scalar FFMA / FADD two co-resident warps reach
-// 10.3 clk per warp-level EX2, with the packed forms 8.15 (the MUFU pipe itself: 8.0; tools/probe/mufu_probe.cu).
-__device__ __forceinline__ uint64_t f32x2_pack(float lo, float hi) {
-  uint64_t r;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
-  return r;
-}
-__device__ __forceinline__ void f32x2_unpack(uint64_t v, float& lo, float& hi) {
-  asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v));
-}
-__device__ __forceinline__ uint64_t f32x2_fma(uint64_t a, uint64_t b, uint64_t c) {
-  uint64_t d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-  return d;
-}
-__device__ __forceinline__ uint64_t f32x2_add(uint64_t a, uint64_t b) {
-  uint64_t d;
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
-}
-// 2^x on the FMA / ALU pipes (no MUFU), for x <= ~100: x = n + f with n = round(x), f in [-0.5, 0.5];
-// 2^f by a degree-3 minimax polynomial (max relative error 7.5e-5, far below the bf16 rounding of the softmax
-// probabilities it feeds), 2^n by adding n to the exponent field.  Inputs below -126 (incl. -inf) give ~1e-38.
-__device__ __forceinline__ float ex2_fma(float x) {
-  x = fmaxf(x, -126.0f);
-  const float t = x + 12582912.0f;  // 1.5 * 2^23: round(x) lands in the low mantissa bits (two's complement)
-  const float f = x - (t - 12582912.0f);
-  float p = fmaf(f, 0.0551716685f, 0.242611125f);
-  p = fmaf(f, p, 0.693260968f);
-  p = fmaf(f, p, 0.999928057f);
-  return __uint_as_float(__float_as_uint(p) + (__float_as_uint(t) << 23));
-}
-__device__ __forceinline__ float fmax3(float a, float b, float c) {
-  float r;
-  asm("max.f32 %0, %1, %2, %3;" : "=f"(r) : "f"(a), "f"(b), "f"(c));  // FMNMX3 (sm_100)
-  return r;
-}
-
 // Exact (erf) GELU, nn.GELU() default (sta_blocks.py:60,68), branch-free and to fp32 rounding level
 // (tools/fit_gelu.py reproduces the coefficients and the error bound).
 __device__ __forceinline__ float gelu_erf(float x) {
@@ -448,25 +251,6 @@ __device__ __forceinline__ float gelu_erf(float x) {
   q = fmaf(a, q, -1.1511993408203125f);
   q = fmaf(a, q, -0.9999947547912598f);
   return fmaf(-fabsf(x), ex2_approx(q), fmaxf(x, 0.0f));
-}
-
-// Two GELUs at once with the packed fp32 instructions (FFMA2): the polynomial is evaluated in n = -min(|x|, 6) (odd
-// coefficients change sign), and gelu(x) = max(x, 0) + n * 2^q(n).  Using the clamped n in the last product instead of -|x|
-// changes the result by at most (|x| - 6) * 1e-9.  13 instructions per pair instead of 22.
-__device__ __forceinline__ void gelu_erf2(float& x0, float& x1) {
-  const float n0 = fmaxf(-fabsf(x0), -6.0f), n1 = fmaxf(-fabsf(x1), -6.0f);
-  const uint64_t n = f32x2_pack(n0, n1);
-  uint64_t q = f32x2_fma(n, f32x2_pack(3.4195283660665154e-05f, 3.4195283660665154e-05f),
-                         f32x2_pack(0.0007779477164149284f, 0.0007779477164149284f));
-  q = f32x2_fma(n, q, f32x2_pack(0.008105806075036526f, 0.008105806075036526f));
-  q = f32x2_fma(n, q, f32x2_pack(0.053442906588315964f, 0.053442906588315964f));
-  q = f32x2_fma(n, q, f32x2_pack(-0.4587582051753998f, -0.4587582051753998f));
-  q = f32x2_fma(n, q, f32x2_pack(1.1511993408203125f, 1.1511993408203125f));
-  q = f32x2_fma(n, q, f32x2_pack(-0.9999947547912598f, -0.9999947547912598f));
-  float q0, q1;
-  f32x2_unpack(q, q0, q1);
-  const uint64_t r = f32x2_fma(n, f32x2_pack(ex2_approx(q0), ex2_approx(q1)), f32x2_pack(fmaxf(x0, 0.0f), fmaxf(x1, 0.0f)));
-  f32x2_unpack(r, x0, x1);
 }
 
 __device__ __forceinline__ void named_bar_arrive(uint32_t id, uint32_t nthreads) {

@@ -1,4 +1,4 @@
-// Host launcher for the tcgen05 GEMM / implicit-GEMM convolution (gemm.cuh).
+// Host launcher for the wgmma GEMM / implicit-GEMM convolution (gemm.cuh).
 #include "gemm.cuh"
 #include "host_util.h"
 #include "ops.h"
@@ -33,57 +33,23 @@ splitk_reduce_kernel(const float* __restrict__ partial, long long slice_elems, i
   }
 }
 
-template <int BN, int AMODE, int EPI, int CG, int EW, bool TMA>
-static int launch_inst(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmC, const GemmParams& p_in,
+template <int BN, int AMODE, int EPI, bool TMA>
+static int launch_inst(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmC, const GemmParams& p,
                        int num_tiles, cudaStream_t stream) {
-  GemmParams p = p_in;
-  using Cfg = GemmCfg<BN, CG, EW, EPI, TMA, AMODE == A_CONV3H>;
-  auto kern = gemm_tc_kernel<BN, AMODE, EPI, CG, EW, TMA>;
+  using Cfg = GemmCfg<BN, EPI, TMA, AMODE == A_CONV3H>;
+  auto kern = gemm_wg_kernel<BN, AMODE, EPI, TMA>;
   static PerDeviceOnce once;  // the opt-in is per device, not per process
   STA_CHECK_CUDA(once.run(
       [&] { return cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg::SMEM_BYTES); }));
-  // persistent: one CTA (CG=1) or one CTA pair (CG=2) per work-item slot
-  const int max_items = num_sms() / CG;
-  const int items = num_tiles < max_items ? num_tiles : max_items;
+  // persistent: one CTA per SM at most
+  const int items = num_tiles < num_sms() ? num_tiles : num_sms();
   if (items < 1) return 0;
-  // Wave-quantisation tail: with W work slots, num_tiles = k W + r leaves r tiles for a last, mostly idle wave (the
-  // encoder's N = 1024 layers: 384 tiles on 74 CTA pairs = 5 waves + 14 tiles).  If 2 r <= W those r tiles are issued as
-  // 2 r half tiles (256 x 128) instead: the last wave then takes half as long.  Same K order per output element, so the
-  // results are bit-identical to the full-tile schedule.  STA_GEMM_TAIL=0 disables (A/B timing).
-  p.tail_r = 0;
-  p.tail_first = num_tiles;
-  if (TMA && CG == 2 && BN == 256 && EPI == EPI_F32 && p.ksplit == 1 && num_tiles > items) {
-    static int tail_mode = -1;
-    if (tail_mode < 0) {
-      const char* e = getenv("STA_GEMM_TAIL");
-      tail_mode = (e && e[0] == '0') ? 0 : 1;
-    }
-    const int r = num_tiles % items;
-    if (tail_mode && r > 0 && 2 * r <= items) {
-      p.tail_r = r;
-      p.tail_first = num_tiles - r;
-    }
-  }
-  STA_CHECK_CUDA(launch_pdl(kern, dim3(items * CG), dim3(Cfg::THREADS), Cfg::SMEM_BYTES, stream, CG, tmA, tmB, tmC, p));
+  STA_CHECK_CUDA(launch_pdl(kern, dim3(items), dim3(Cfg::THREADS), Cfg::SMEM_BYTES, stream, 1, tmA, tmB, tmC, p));
   return 0;
-}
-
-// STA_GEMM_CTA_GROUP=1 forces the single-CTA kernels (A/B timing and debugging)
-static int cta_group_mode() {
-  static int mode = -1;
-  if (mode < 0) {
-    const char* e = getenv("STA_GEMM_CTA_GROUP");
-    mode = (e && e[0] == '1') ? 1 : 2;
-  }
-  return mode;
 }
 
 int launch_gemm(const GemmLaunch& g, cudaStream_t stream) {
   GemmParams p = g.p;
-  {
-    const char* e = getenv("STA_GEMM_TRACE");
-    p.dbg = e ? reinterpret_cast<long long*>(strtoull(e, nullptr, 0)) : nullptr;
-  }
   STA_REQUIRE(p.N % 32 == 0, "N must be a multiple of 32");
   STA_REQUIRE(!p.split || g.epi == EPI_F32 || g.epi == EPI_HEAD || g.epi == EPI_PIXSHUF || p.ldo >= 3LL * p.N,
               "split-precision bf16 outputs need ldo >= 3N");
@@ -91,11 +57,10 @@ int launch_gemm(const GemmLaunch& g, cudaStream_t stream) {
   STA_REQUIRE((reinterpret_cast<uintptr_t>(g.A) & 15) == 0 && (reinterpret_cast<uintptr_t>(g.Wt) & 15) == 0,
               "operands must be 16-byte aligned");
 
-  // BN = 256 for the wide trunk layers, 128 when N is not a multiple of 256.
-  int bn = (p.N % 256 == 0 && g.epi != EPI_PIXSHUF && g.epi != EPI_HEAD) ? 256 : 128;
-  int cg = cta_group_mode();
+  // 128 x 128 tiles: one m64n128 wgmma per consumer warpgroup and k16 step
+  const int bn = 128;
 
-  // TMA-store epilogue (epilogue_tile_tma) for the wide linear layers: bf16 / GELU / RoPE outputs without skip
+  // TMA-store epilogue (epilogue_tile_tma) for the linear layers: bf16 / GELU / RoPE outputs without skip
   // tensors, fp32 outputs that either have no residual or accumulate in place (out += ..., bulk reduce-add).
   static int tma_mode = -1, small_mode = -1, halo_mode = -1;
   if (tma_mode < 0) {
@@ -103,11 +68,11 @@ int launch_gemm(const GemmLaunch& g, cudaStream_t stream) {
     halo_mode = (eh && eh[0] == '0') ? 0 : 1;
     const char* e = getenv("STA_GEMM_TMA_EPI");  // 0 disables (A/B timing and debugging)
     tma_mode = (e && e[0] == '0') ? 0 : 1;
-    e = getenv("STA_GEMM_SMALL");  // 0 disables the small-problem route (A/B timing)
+    e = getenv("STA_GEMM_SMALL");  // 0 disables the split-K small-problem route (A/B timing)
     small_mode = (e && e[0] == '0') ? 0 : 1;
   }
   const int esz = (g.epi == EPI_F32) ? 4 : 2;
-  bool tma = tma_mode == 1 && bn == 256 && g.amode == A_LINEAR && p.out != nullptr && p.out2 == nullptr &&
+  bool tma = tma_mode == 1 && p.N % bn == 0 && g.amode == A_LINEAR && p.out != nullptr && p.out2 == nullptr &&
              (reinterpret_cast<uintptr_t>(p.out) & 15) == 0 && (p.ldo * esz) % 16 == 0;
   p.c_reduce = 0;
   if (g.epi == EPI_BF16) {
@@ -120,40 +85,27 @@ int launch_gemm(const GemmLaunch& g, cudaStream_t stream) {
   }
 
   // Small problems (one keyframe / a few edges in SLAM mode) are bound by streaming the weights through too few SMs:
-  // a 256-wide CTA-pair grid would occupy < half the GPU.  They use 128 x 128 single-CTA tiles, and the fp32
-  // residual-stream layers (out += A W^T + b) additionally split K across CTAs: every split stores its partial tile
-  // to scratch and a second tiny kernel sums them in a fixed order (deterministic, unlike reduce-adds racing).
+  // the fp32 residual-stream layers (out += A W^T + b) with fewer tiles than SMs split K across CTAs: every split
+  // stores its partial tile to scratch and a second tiny kernel sums them in a fixed order (deterministic, unlike
+  // reduce-adds racing).
   int ksplit = 1;
-  {
-    const int mt = (p.M + 127) / 128;
-    if (small_mode && tma && ((mt + 1) / 2) * (p.N / 256) * 2 < num_sms() / 2) {
-      bn = 128;
-      cg = 1;
-      const int tiles = mt * (p.N / 128), nkb = (p.K + 63) / 64;
-      if (g.epi == EPI_F32 && g.splitk_ws != nullptr) {
-        int ks = num_sms() / tiles;
-        if (ks > 8) ks = 8;
-        if (ks > nkb / 2) ks = nkb / 2;
-        const size_t need = static_cast<size_t>(ks) * mt * 128 * p.N * sizeof(float);
-        if (ks >= 2 && need <= g.splitk_ws_bytes && (reinterpret_cast<uintptr_t>(g.splitk_ws) & 15) == 0) ksplit = ks;
-      }
+  if (small_mode && tma && g.epi == EPI_F32 && g.splitk_ws != nullptr) {
+    const int tiles = ((p.M + 127) / 128) * (p.N / bn), nkb = (p.K + 63) / 64;
+    if (tiles < num_sms()) {
+      int ks = num_sms() / tiles;
+      if (ks > 8) ks = 8;
+      if (ks > nkb / 2) ks = nkb / 2;
+      const size_t need = static_cast<size_t>(ks) * ((p.M + 127) / 128) * 128 * p.N * sizeof(float);
+      if (ks >= 2 && need <= g.splitk_ws_bytes && (reinterpret_cast<uintptr_t>(g.splitk_ws) & 15) == 0) ksplit = ks;
     }
   }
   const int amode = (g.amode == A_CONV3 && halo_mode) ? A_CONV3H : g.amode;
-  if (small_mode && g.amode == A_CONV3 && g.epi == EPI_BF16 && bn == 256) {
-    // same for the DPT convolutions at low resolution (K = 9 * 256 streamed by a handful of CTA pairs otherwise)
-    const int mt = p.nimg * ((p.H + 7) / 8) * ((p.W + 15) / 16);
-    if (((mt + 1) / 2) * (p.N / 256) * 2 < num_sms() / 2) {
-      bn = 128;
-      cg = 1;
-    }
-  }
   CUtensorMap tmA, tmB;
   int m_tiles;
   if (g.amode == A_CONV3) {
     STA_REQUIRE(p.Cin % 64 == 0, "conv input channels must be a multiple of 64");
     STA_REQUIRE(p.K == 9 * p.Cin, "conv K must be 9*Cin");
-    const bool halo = amode == A_CONV3H;  // 16 x 8-pixel tiles fed from one 18 x 16-pixel box per channel chunk
+    const bool halo = amode == A_CONV3H;  // 16 x 8-pixel tiles fed from one 18 x 10-pixel box per channel chunk
     p.tiles_h = halo ? (p.H + 15) / 16 : (p.H + 7) / 8;
     p.tiles_w = halo ? (p.W + 7) / 8 : (p.W + 15) / 16;
     p.M = p.nimg * p.H * p.W;
@@ -174,11 +126,11 @@ int launch_gemm(const GemmLaunch& g, cudaStream_t stream) {
     STA_REQUIRE(g.ldw % 8 == 0, "ldw must be a multiple of 8 elements (16 bytes)");
     uint64_t dims[2] = {(uint64_t)p.K, (uint64_t)p.N};
     uint64_t strides[1] = {(uint64_t)g.ldw * 2};
-    uint32_t box[2] = {64, (uint32_t)(bn / cg)};
+    uint32_t box[2] = {64, (uint32_t)bn};
     if (make_tmap_bf16(&tmB, g.Wt, 2, dims, strides, box)) return 1;
   }
   const int n_tiles = (p.N + bn - 1) / bn;
-  const int num_tiles = ((m_tiles + cg - 1) / cg) * n_tiles * ksplit;
+  const int num_tiles = m_tiles * n_tiles * ksplit;
 
   CUtensorMap tmC = tmA;
   p.ksplit = 1;
@@ -206,50 +158,24 @@ int launch_gemm(const GemmLaunch& g, cudaStream_t stream) {
   }
   STA_REQUIRE(tma || ksplit == 1, "split-K needs the TMA epilogue");
 
-  // 8 epilogue warps everywhere: with the TMA-store epilogue every fused epilogue of the trunk fits under the
-  // K >= 768 mainloop, and the smaller CTA keeps a 5-deep operand ring (16 warps were measured slower end to end).
-  // Exception: the DPT convolutions that add skip tensors and / or write a second (ReLU) copy are epilogue-bound with 8
-  // warps (tools/conv_ab.py): they get 16.  STA_CONV_EW16=0 disables (A/B timing).
-  static int ew16_mode = -1;
-  if (ew16_mode < 0) {
-    const char* e = getenv("STA_CONV_EW16");
-    ew16_mode = (e && e[0] == '0') ? 0 : 1;
-  }
-  const int ew =
-      (ew16_mode && cg == 2 && amode == A_CONV3H && bn == 256 && g.epi == EPI_BF16 && (p.resid != nullptr || p.out2 != nullptr)) ? 16 : 8;
-
   int rc = -1;
-#define STA_GEMM_CASE3(BN_, AM_, EP_, EW_, TMA_)                                                                  \
-  if (rc < 0 && bn == BN_ && amode == AM_ && g.epi == EP_ && ew == EW_ && tma == TMA_)                            \
-    rc = (cg == 2) ? launch_inst<BN_, AM_, EP_, 2, EW_, TMA_>(tmA, tmB, tmC, p, num_tiles, stream)                \
-                   : launch_inst<BN_, AM_, EP_, 1, EW_, TMA_>(tmA, tmB, tmC, p, num_tiles, stream);
-#define STA_GEMM_CASE(BN_, AM_, EP_) STA_GEMM_CASE3(BN_, AM_, EP_, 8, false)
+#define STA_GEMM_CASE(AM_, EP_, TMA_) \
+  if (rc < 0 && amode == AM_ && g.epi == EP_ && tma == TMA_) rc = launch_inst<128, AM_, EP_, TMA_>(tmA, tmB, tmC, p, num_tiles, stream);
 
-  STA_GEMM_CASE3(256, A_LINEAR, EPI_GELU, 8, true)
-  STA_GEMM_CASE3(256, A_LINEAR, EPI_F32, 8, true)
-  STA_GEMM_CASE3(256, A_LINEAR, EPI_ROPE, 8, true)
-  STA_GEMM_CASE3(256, A_LINEAR, EPI_BF16, 8, true)
-  STA_GEMM_CASE3(128, A_LINEAR, EPI_GELU, 8, true)
-  STA_GEMM_CASE3(128, A_LINEAR, EPI_F32, 8, true)
-  STA_GEMM_CASE3(128, A_LINEAR, EPI_ROPE, 8, true)
-  STA_GEMM_CASE3(128, A_LINEAR, EPI_BF16, 8, true)
-  STA_GEMM_CASE(256, A_LINEAR, EPI_BF16)
-  STA_GEMM_CASE(256, A_LINEAR, EPI_GELU)
-  STA_GEMM_CASE(256, A_LINEAR, EPI_F32)
-  STA_GEMM_CASE(256, A_LINEAR, EPI_ROPE)
-  STA_GEMM_CASE(128, A_LINEAR, EPI_BF16)
-  STA_GEMM_CASE(128, A_LINEAR, EPI_F32)
-  STA_GEMM_CASE(128, A_LINEAR, EPI_PIXSHUF)
-  STA_GEMM_CASE(256, A_CONV3, EPI_BF16)
-  STA_GEMM_CASE(128, A_CONV3, EPI_BF16)
-  STA_GEMM_CASE(128, A_CONV3, EPI_HEAD)
-  STA_GEMM_CASE(256, A_CONV3H, EPI_BF16)
-  if (rc < 0 && ew == 16)  // CTA pair only (a single CTA has no room for 16 staging buffers beside the halo tiles)
-    rc = launch_inst<256, A_CONV3H, EPI_BF16, 2, 16, false>(tmA, tmB, tmC, p, num_tiles, stream);
-  STA_GEMM_CASE(128, A_CONV3H, EPI_BF16)
-  STA_GEMM_CASE(128, A_CONV3H, EPI_HEAD)
+  STA_GEMM_CASE(A_LINEAR, EPI_GELU, true)
+  STA_GEMM_CASE(A_LINEAR, EPI_F32, true)
+  STA_GEMM_CASE(A_LINEAR, EPI_ROPE, true)
+  STA_GEMM_CASE(A_LINEAR, EPI_BF16, true)
+  STA_GEMM_CASE(A_LINEAR, EPI_BF16, false)
+  STA_GEMM_CASE(A_LINEAR, EPI_GELU, false)
+  STA_GEMM_CASE(A_LINEAR, EPI_F32, false)
+  STA_GEMM_CASE(A_LINEAR, EPI_ROPE, false)
+  STA_GEMM_CASE(A_LINEAR, EPI_PIXSHUF, false)
+  STA_GEMM_CASE(A_CONV3, EPI_BF16, false)
+  STA_GEMM_CASE(A_CONV3, EPI_HEAD, false)
+  STA_GEMM_CASE(A_CONV3H, EPI_BF16, false)
+  STA_GEMM_CASE(A_CONV3H, EPI_HEAD, false)
 #undef STA_GEMM_CASE
-#undef STA_GEMM_CASE3
   if (rc == 0 && ksplit > 1) {
     const long long total = static_cast<long long>(p.M) * (p.N / 4);
     int blocks = static_cast<int>((total + 255) / 256);
@@ -259,7 +185,7 @@ int launch_gemm(const GemmLaunch& g, cudaStream_t stream) {
                               final_bias, final_out, p.ldo, p.M, p.N, final_accumulate));
   }
   if (rc >= 0) return rc;
-  set_last_error("launch_gemm: unsupported (BN, amode, epilogue) combination");
+  set_last_error("launch_gemm: unsupported (amode, epilogue) combination");
   return 2;
 }
 

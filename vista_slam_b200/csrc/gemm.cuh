@@ -1,15 +1,14 @@
-// Persistent warp-specialised tcgen05 GEMM / implicit-GEMM 3x3 convolution for sm_100a.
+// Persistent warp-specialised wgmma GEMM / implicit-GEMM 3x3 convolution for sm_90a.
 //
-//   D[M,N] = A[M,K] * W[N,K]^T  (bf16 operands, fp32 accumulation in TMEM)
+//   D[M,N] = A[M,K] * W[N,K]^T  (bf16 operands, fp32 accumulation in registers)
 //
-// Roles: warp 0 = TMA producer, warp 1 = MMA issuer (one elected thread issues tcgen05.mma),
-// warp 2 = TMEM allocator, warps 4.. = 8 or 16 epilogue warps
-// (TMEM -> registers -> fused epilogue -> global).  The accumulator is double
-// buffered in TMEM (2 x BN columns) so the epilogue of tile i overlaps the
-// mainloop of tile i+1.  Operand tiles are 128B-swizzled K-major [rows][64]
-// boxes written by TMA; the 3x3 convolution uses a 4-D NHWC tensor map and
-// shifts the box per filter tap (out-of-bounds = zero padding), so no im2col
-// buffer exists.
+// Roles: warp 0 = TMA producer (warps 1-3 idle), warps 4-11 = two consumer warpgroups.  Consumer warpgroup g
+// computes rows [64 g, 64 g + 64) of the 128 x BN tile with wgmma (m64 n128 k16, accumulators in registers) while
+// the producer keeps a STAGES-deep operand ring filled; the finished accumulators are written to a padded fp32 tile
+// in shared memory, from which the same eight warps run the fused epilogue (-> global).  The producer prefetches
+// the next tile's operands during the epilogue.  Operand tiles are 128B-swizzled K-major [rows][64] boxes written
+// by TMA; the 3x3 convolution uses a 4-D NHWC tensor map and shifts the box per filter tap (out-of-bounds = zero
+// padding), so no im2col buffer exists.
 //
 // Reference ops covered (vista_slam/sta_model): nn.Linear in blocks/sta_blocks.py:67-70,
 // 88-90,179-183; PatchEmbed conv sta_blocks.py:262 (after im2col); the DPT convs of
@@ -70,75 +69,75 @@ struct GemmParams {
   // (K here is the physical 3K); bf16 outputs / bf16 skip tensors use the (hi | lo | hi) row layout with logical
   // width N (ldo = 3N).  fp32 outputs are unaffected.
   int split;
-  // Wave-quantisation tail (TMA epilogue, CTA pair, BN = 256, EPI_F32, no split-K): the last tail_r work items, which would
-  // run as a partial wave on a few CTA pairs, are each issued as TWO 256 x 128 half tiles (see launch_gemm).
-  int tail_first;  // first tile index of the tail
-  int tail_r;      // number of tail tiles (0 = off)
-  long long* dbg;       // optional clock64 trace (env STA_GEMM_TRACE), else null
 };
 
-// CG = 1: one CTA per 128 x BN tile (tcgen05 cta_group::1).
-// CG = 2: a CTA pair (cluster of 2 on one TPC) per 256 x BN tile (cta_group::2): each CTA stages its own
-//         128 rows of A and BN/2 rows of B, so per-SM shared-memory traffic per MMA is halved for B.
 // TMA = true: the epilogue writes through shared memory + TMA tensor stores (epilogue_tile_tma), else the
-// transposing per-warp staging path (epilogue_tile).
+// coalesced per-warp path (epilogue_tile).
 // A_CONV3H: pixels per staged halo row.  10 = the 8-pixel tile plus its two halo columns (dense box, 8-row descriptor groups
-// 1280 B apart -- groups then start at any 128-byte multiple, which the absolute-address swizzle permits); 16 = padded rows
-// (groups 2048 B apart), 60 % more bytes per box.
+// 1280 B apart -- groups then start at any 128-byte multiple, which the absolute-address swizzle permits).
 constexpr int kHaloPitch = 10;
 constexpr int kRopeLd = 36;  // floats per staged sin/cos table row (32 + 4 pad: conflict-free row-per-lane reads)
-template <int BN, int CG, int EW, int EPI, bool TMA, bool HALO = false>
+template <int BN, int EPI, bool TMA, bool HALO = false>
 struct GemmCfg {
   static constexpr int BM = 128;
   static constexpr int BK = 64;
+  static_assert(BN == 128, "one consumer warpgroup covers the 128 columns of a tile (wgmma m64n128k16)");
   static constexpr uint32_t A_BYTES = BM * BK * 2;
-  static constexpr uint32_t B_BYTES = (BN / CG) * BK * 2;
+  static constexpr uint32_t B_BYTES = BN * BK * 2;
   static constexpr uint32_t BAR_BYTES = 256;
-  static constexpr int EPI_WARPS = EW;  // 8 (mainloop-bound launches) or 16 (epilogue-heavy: 4 warps per scheduler)
-  static constexpr int PARTS = EW / 4;  // column parts of a tile, one per epilogue warp of a lane quarter
+  static constexpr int EPI_WARPS = 8;   // the two consumer warpgroups
+  static constexpr int PARTS = EPI_WARPS / 4;  // column parts of a tile, one per epilogue warp of a lane quarter
   static constexpr uint32_t EPI_SMEM_BYTES = (EPI == EPI_HEAD) ? 3 * 128 * 4 * sizeof(float) : 0;  // partial sums
-  // per-warp staging: [32][36] fp32 transpose buffer, or one 4 KB SWIZZLE_128B box for the TMA store
-  static constexpr uint32_t STG_WARP_BYTES = TMA ? 4096 : 32 * 36 * sizeof(float);
-  static constexpr uint32_t STG_BYTES = EPI_WARPS * STG_WARP_BYTES;
+  // finished accumulators: [128 rows][BN + 4] fp32 (the pad makes row-per-lane 16-byte reads conflict-free)
+  static constexpr int ACC_LD = BN + 4;
+  static constexpr uint32_t ACC_BYTES = BM * ACC_LD * sizeof(float);
+  // per-warp staging of the TMA-store epilogue: one 4 KB SWIZZLE_128B box
+  static constexpr uint32_t STG_WARP_BYTES = 4096;
+  static constexpr uint32_t STG_BYTES = TMA ? EPI_WARPS * STG_WARP_BYTES : 0;
   static constexpr int ROPE_SMEM_ROWS = 64;  // positions -1 .. 62
   static constexpr uint32_t ROPE_SMEM_BYTES = (EPI == EPI_ROPE) ? ROPE_SMEM_ROWS * kRopeLd * sizeof(float) : 0;
   static constexpr uint32_t MAX_SMEM = 227 * 1024;
-  // halo-staged convolution (A_CONV3H): the ring holds B tiles only; two 18 x 16 x 64-channel input tiles besides it
+  // halo-staged convolution (A_CONV3H): the ring holds B tiles only; three 18 x 10 x 64-channel input tiles besides it
   static constexpr uint32_t HALO_TX_BYTES = 18 * kHaloPitch * 128;                 // bytes one box delivers
   static constexpr uint32_t HALO_BYTES = (HALO_TX_BYTES + 1023u) & ~1023u;        // stage stride (swizzle-pattern aligned)
-  static constexpr int HALO_STAGES = kHaloPitch == 16 ? 2 : 3;
+  static constexpr int HALO_STAGES = 3;
   static constexpr uint32_t HALO_TOTAL = HALO ? HALO_STAGES * HALO_BYTES : 0;
   static constexpr uint32_t STAGE_BYTES = HALO ? B_BYTES : A_BYTES + B_BYTES;
   static constexpr int STAGES_FIT =
-      (MAX_SMEM - BAR_BYTES - EPI_SMEM_BYTES - STG_BYTES - ROPE_SMEM_BYTES - HALO_TOTAL) / STAGE_BYTES;
+      (MAX_SMEM - BAR_BYTES - EPI_SMEM_BYTES - STG_BYTES - ACC_BYTES - ROPE_SMEM_BYTES - HALO_TOTAL) / STAGE_BYTES;
   static constexpr int STAGES = STAGES_FIT > 8 ? 8 : STAGES_FIT;
-  // layout: operand ring | halo tiles | staging (1024-byte aligned) | barriers | EPI_HEAD partials | RoPE table
+  // layout: operand ring | halo tiles | staging (1024-byte aligned) | accumulator tile | barriers | EPI_HEAD partials | RoPE
   static constexpr uint32_t OFF_HALO = STAGES * STAGE_BYTES;
   static constexpr uint32_t OFF_STG = OFF_HALO + HALO_TOTAL;
-  static constexpr uint32_t OFF_BAR = OFF_STG + STG_BYTES;
+  static constexpr uint32_t OFF_ACC = OFF_STG + STG_BYTES;
+  static constexpr uint32_t OFF_BAR = OFF_ACC + ACC_BYTES;
   static constexpr uint32_t OFF_EPI = OFF_BAR + BAR_BYTES;
   static constexpr uint32_t OFF_ROPE = OFF_EPI + EPI_SMEM_BYTES;
   static constexpr uint32_t SMEM_BYTES = OFF_ROPE + ROPE_SMEM_BYTES;
   static constexpr int THREADS = 128 + 32 * EPI_WARPS;
   static constexpr int EPI_THREADS = 32 * EPI_WARPS;
   static_assert(STAGES <= 8 && STAGES >= 3, "barrier area holds at most 8 stages");
-  static_assert(OFF_STG % 1024 == 0 && OFF_HALO % 1024 == 0 && STG_WARP_BYTES % 16 == 0, "staging alignment");
+  static_assert(OFF_STG % 1024 == 0 && OFF_HALO % 1024 == 0 && OFF_ACC % 16 == 0, "staging alignment");
+  static_assert(SMEM_BYTES <= MAX_SMEM, "shared memory");
 };
 
 // ---------------------------------------------------------------------------
-// Epilogue for one 128 x BN accumulator tile; executed by the 16 epilogue warps (4 per scheduler, so that the
-// global-load / TMEM-load latencies of one warp are covered by the others).
-// warp (quarter, part): TMEM lanes [32*quarter, +32), columns [part*BN/4, +BN/4).
+// Epilogue for one 128 x BN accumulator tile held in shared memory ([128][BN + 4] fp32); executed by the 8 consumer
+// warps.  warp (quarter, part): rows [32*quarter, +32), columns [part*BN/2, +BN/2).
 //
-// tcgen05.ld (32x32b) hands every thread one accumulator ROW (32 consecutive columns).  Storing
-// that way would make each warp store touch 32 different cache lines, so every 32x32 fp32 chunk
-// is transposed through a per-warp shared-memory staging buffer ([32][36] floats, conflict-free
-// for 128-bit accesses) into a COALESCED mapping -- lane -> (row = 4*it + lane/8, 4 columns at
-// (lane%8)*4) -- in which bias, residuals, activation and the global stores happen: a warp-wide
-// access covers 4 rows x 128 contiguous bytes (fp32) or 4 rows x 64 bytes (bf16).
+// Every 32x32 fp32 chunk is read in a COALESCED mapping -- lane -> (row = 4*it + lane/8, 4 columns at (lane%8)*4) --
+// in which bias, residuals, activation and the global stores happen: a warp-wide access covers 4 rows x 128
+// contiguous bytes (fp32) or 4 rows x 64 bytes (bf16).
 // ---------------------------------------------------------------------------
-constexpr int kStageLd = 36;                        // floats per staged row (32 + 4 pad)
-constexpr int kStageFloatsPerWarp = 32 * kStageLd;  // 4608 B per epilogue warp
+// 32 consecutive fp32 accumulators of one row (16-byte aligned)
+__device__ __forceinline__ void acc_ld32(const float* src, uint32_t (&r)[32]) {
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    const float4 v = reinterpret_cast<const float4*>(src)[j];
+    r[4 * j] = __float_as_uint(v.x); r[4 * j + 1] = __float_as_uint(v.y);
+    r[4 * j + 2] = __float_as_uint(v.z); r[4 * j + 3] = __float_as_uint(v.w);
+  }
+}
 
 template <int AMODE>
 __device__ __forceinline__ void tile_row(const GemmParams& p, int m_tile, int r_local, long long& orow, bool& valid) {
@@ -169,12 +168,6 @@ __device__ __forceinline__ void tile_row(const GemmParams& p, int m_tile, int r_
   }
 }
 
-__device__ __forceinline__ void stage_store32(float* stg, int lane, const float* v) {
-  float4* d = reinterpret_cast<float4*>(stg + lane * kStageLd);
-#pragma unroll
-  for (int j = 0; j < 8; ++j) d[j] = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
-}
-
 __device__ __forceinline__ uint2 pack4_bf16(const float4& v) {
   return make_uint2(pack_bf16x2(v.x, v.y), pack_bf16x2(v.z, v.w));
 }
@@ -191,13 +184,12 @@ __device__ __forceinline__ void store4_bf16(__nv_bfloat16* p, const float4& v, i
   }
 }
 
+// accs: the accumulator tile at this warp's first row (32 * quarter) and first column (part * BN / PARTS)
 template <int BN, int AMODE, int EPI, int EW>
-__device__ __forceinline__ void epilogue_tile(const GemmParams& p, uint32_t taddr, int m_tile, int n_tile,
-                                              int quarter, int part, float* epi_smem, float* stg,
-                                              const float* rope_s, uint64_t* tfull_bar, uint32_t tfull_phase) {
-  // Everything that does not depend on the accumulator (row bookkeeping, positions, residual prefetch) is done
-  // BEFORE waiting for the tile's MMAs, so its global-memory latency hides behind the mainloop.
+__device__ __forceinline__ void epilogue_tile(const GemmParams& p, const float* accs, int m_tile, int n_tile,
+                                              int quarter, int part, float* epi_smem, const float* rope_s) {
   constexpr int PARTS = EW / 4;
+  constexpr int LD = BN + 4;  // accumulator tile row stride (floats)
   constexpr int CH = BN / PARTS;  // columns per epilogue warp
   const int lane = threadIdx.x & 31;
   const int colbase = n_tile * BN + part * CH;
@@ -207,8 +199,6 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, uint32_t tadd
     // postprocess.py:10-62).  Row mapping: each thread owns 32 of the 128 channels of one pixel; the four
     // column parts are combined through shared memory.  Nothing but 16 bytes per pixel is written.
     static_assert(BN == 128, "EPI_HEAD expects the 128-channel head");
-    mbar_wait(tfull_bar, tfull_phase);
-    tc_fence_after();
     const int r_local = quarter * 32 + lane;
     long long orow;
     bool valid;
@@ -218,8 +208,7 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, uint32_t tadd
     for (int c = 0; c < CH; c += 32) {
       const int col = colbase + c;
       uint32_t acc[32];
-      tmem_ld32(taddr + c, acc);
-      tmem_ld_wait();
+      acc_ld32(accs + lane * LD + c, acc);
       const float4* wp = reinterpret_cast<const float4*>(p.head_w) + col;
 #pragma unroll
       for (int i = 0; i < 32; ++i) {
@@ -296,7 +285,7 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, uint32_t tadd
           py = pp.x;
           px = pp.y;
           if (py < -1 || py > p.rope_max_pos || px < -1 || px > p.rope_max_pos)
-            device_fatal("token position outside the RoPE table");
+            __trap();  // token position outside the RoPE table (no printf: see mbar_wait)
         }
         pos_y[it] = py;
         pos_x[it] = px;
@@ -304,7 +293,7 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, uint32_t tadd
     }
 
     // flush one staged 32-column chunk (global columns [col, col+32)) in the coalesced mapping
-    auto flush = [&](int col) {
+    auto flush = [&](int col, const float* stg) {
       if (col >= p.N) return;
       float4 b4 = make_float4(0.f, 0.f, 0.f, 0.f);
       long long pix_off = 0;
@@ -366,7 +355,7 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, uint32_t tadd
           // compiler can interleave the four rows of a batch
           const int it = hb * 4 + k;
           const bool ok = (vmask >> it) & 1u;
-          float4 v = *reinterpret_cast<const float4*>(stg + (it * 4 + crow) * kStageLd + cc);
+          float4 v = *reinterpret_cast<const float4*>(stg + (it * 4 + crow) * LD + cc);
           v.x += b4.x; v.y += b4.y; v.z += b4.z; v.w += b4.w;
           if constexpr (EPI == EPI_ROPE) {
             // 2-D RoPE (pos_embed/pos_embed.py:149-185, curope/kernels.cu:17-82).  A 32-column chunk is exactly
@@ -453,47 +442,31 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, uint32_t tadd
         }
       }
     }
-    mbar_wait(tfull_bar, tfull_phase);
-    tc_fence_after();
 #pragma unroll 1
-    for (int c = 0; c < CH; c += 32) {
-      uint32_t acc[32];
-      tmem_ld32(taddr + c, acc);
-      tmem_ld_wait();
-      stage_store32(stg, lane, reinterpret_cast<const float*>(acc));
-      __syncwarp();
-      flush(colbase + c);
-      __syncwarp();
-    }
+    for (int c = 0; c < CH; c += 32) flush(colbase + c, accs + c);
   }
 }
 
 // ---------------------------------------------------------------------------
-// TMA-store epilogue for the wide linear layers (BN = 256; EPI_BF16 / EPI_GELU / EPI_ROPE / EPI_F32).
+// TMA-store epilogue for the linear layers with N % 128 == 0 (EPI_BF16 / EPI_GELU / EPI_ROPE / EPI_F32).
 //
-// The math stays in the tcgen05.ld mapping -- one accumulator ROW per thread, 32 consecutive columns per load --
+// The math stays in a row-per-thread mapping -- one accumulator ROW per thread, 32 consecutive columns per load --
 // so bias, GELU and the RoPE rotation (whose (i, i+16) partners sit in the same thread) need no shuffles.  The
 // results go to a per-warp 32-row x 128-byte shared-memory box in the SWIZZLE_128B layout (conflict-free 16-byte
 // stores) and leave with ONE bulk tensor store per box issued by lane 0: no per-lane global stores, rows >= M are
 // clipped by the tensor map, and the in-place fp32 residual stream (x += proj(..)) becomes a bulk reduce-add
-// performed by the L2, so the epilogue never loads the residual.  The TMEM load of chunk c+1 is in flight while
-// chunk c is processed, and the accumulator stage is released as soon as the last load has landed.
+// performed by the L2, so the epilogue never loads the residual.
+// accrow: this thread's accumulator row at the warp's first column.
 // ---------------------------------------------------------------------------
-template <int BN, int EPI, int EW, typename Release>
-__device__ __forceinline__ void epilogue_tile_tma(const GemmParams& p, const CUtensorMap* tmC, uint32_t taddr, int m_tile,
-                                                  int colbase, int nch, int row_off, int quarter, int part, uint8_t* cbuf,
-                                                  const float* rope_s,
-                                                  uint64_t* tfull_bar, uint32_t tfull_phase, Release&& release,
-                                                  long long* trace) {
+template <int BN, int EPI, int EW>
+__device__ __forceinline__ void epilogue_tile_tma(const GemmParams& p, const CUtensorMap* tmC, const float* accrow, int m_tile,
+                                                  int colbase, int row_off, int quarter, uint8_t* cbuf,
+                                                  const float* rope_s) {
   constexpr int PARTS = EW / 4;
-  constexpr int CH = BN / PARTS;  // columns per epilogue warp of a full tile
-  constexpr int NCH = CH / 32;    // 32-column TMEM loads per full tile; nch <= NCH is what this tile has (half tiles: NCH / 2)
-  // 8 warps (168 registers): the next chunk's TMEM load is in flight while the current one is processed;
-  // 16 warps (96 registers) rely on the four warps per scheduler instead
-  constexpr bool PF = (EW == 8);
+  constexpr int CH = BN / PARTS;  // columns per epilogue warp
+  constexpr int NCH = CH / 32;    // 32-column chunks
   constexpr bool OUT_F32 = (EPI == EPI_F32);
   const int lane = threadIdx.x & 31;
-  (void)part;
   const int row0 = m_tile * 128 + quarter * 32;  // first row of this warp's box (token index)
   const int srow0 = row0 + row_off;              // ... in the output tensor (split-K partial slices)
   const uint32_t cb = smem_u32(cbuf);
@@ -507,54 +480,41 @@ __device__ __forceinline__ void epilogue_tile_tma(const GemmParams& p, const CUt
       py = pp.x;
       px = pp.y;
       if (py < -1 || py > p.rope_max_pos || px < -1 || px > p.rope_max_pos)
-        device_fatal("token position outside the RoPE table");
+        __trap();  // token position outside the RoPE table (no printf: see mbar_wait)
     }
   }
 
   // Split-precision parity mode, bf16 outputs: the tile is drained twice -- pass 0 stores hi = bf16(v) at columns
-  // [col, ..) and [2N + col, ..), pass 1 recomputes v from TMEM and stores lo = bf16(v - hi) at [N + col, ..) -- so the
-  // production register footprint is unchanged.  The accumulator stage is released in the last pass only.
+  // [col, ..) and [2N + col, ..), pass 1 re-reads v and stores lo = bf16(v - hi) at [N + col, ..) -- so the
+  // production register footprint is unchanged.
   const int npass = (!OUT_F32 && p.split) ? 2 : 1;
   const bool has_bias = p.bias != nullptr;
 #pragma unroll 1
   for (int pass = 0; pass < npass; ++pass) {
   // bias of chunk c is loaded one chunk ahead (warp-uniform addresses: L1 broadcast), so its latency never sits
-  // between the TMEM load and the math
+  // between the accumulator load and the math
   float4 bcur[8];
 #pragma unroll
   for (int j = 0; j < 8; ++j)
     bcur[j] = has_bias ? __ldg(reinterpret_cast<const float4*>(p.bias + colbase) + j) : make_float4(0.f, 0.f, 0.f, 0.f);
 
-  if (pass == 0) {
-    mbar_wait(tfull_bar, tfull_phase);
-    tc_fence_after();
-    if (trace) trace[0] = clock64();
-  }
-  uint32_t acc[PF ? 2 : 1][32];
-  tmem_ld32(taddr, acc[0]);
 #pragma unroll
   for (int c = 0; c < NCH; ++c) {
-    if (c >= nch) break;
-    tmem_ld_wait();
-    float* v = reinterpret_cast<float*>(acc[PF ? (c & 1) : 0]);
+    uint32_t acc[32];
+    acc_ld32(accrow + c * 32, acc);
+    float* v = reinterpret_cast<float*>(acc);
     const int col = colbase + c * 32;
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
       v[4 * j] += bcur[j].x; v[4 * j + 1] += bcur[j].y; v[4 * j + 2] += bcur[j].z; v[4 * j + 3] += bcur[j].w;
     }
-    if (c + 1 < nch) {
-      if constexpr (PF) tmem_ld32(taddr + (c + 1) * 32, acc[(c + 1) & 1]);
-      if (has_bias) {
+    if (c + 1 < NCH && has_bias) {
 #pragma unroll
-        for (int j = 0; j < 8; ++j) bcur[j] = __ldg(reinterpret_cast<const float4*>(p.bias + col + 32) + j);
-      }
-    } else if (pass == npass - 1) {
-      release();
+      for (int j = 0; j < 8; ++j) bcur[j] = __ldg(reinterpret_cast<const float4*>(p.bias + col + 32) + j);
     }
-    if (trace) trace[1 + 3 * c] = clock64();
     if constexpr (EPI == EPI_GELU) {
 #pragma unroll
-      for (int i = 0; i < 32; i += 2) gelu_erf2(v[i], v[i + 1]);
+      for (int i = 0; i < 32; ++i) v[i] = gelu_erf(v[i]);
     }
     if constexpr (EPI == EPI_BF16) {
       if (p.relu_main) {
@@ -581,7 +541,6 @@ __device__ __forceinline__ void epilogue_tile_tma(const GemmParams& p, const CUt
         }
       }
     }
-    if (trace) trace[2 + 3 * c] = clock64();
     // ---- registers -> swizzled box -> bulk tensor store ----
     if constexpr (OUT_F32) {
       // one box per chunk: 32 rows x 32 fp32 columns
@@ -626,26 +585,22 @@ __device__ __forceinline__ void epilogue_tile_tma(const GemmParams& p, const CUt
         }
       }
     }
-    if constexpr (!PF) {
-      if (c + 1 < nch) tmem_ld32(taddr + (c + 1) * 32, acc[0]);  // the registers are free again
-    }
-    if (trace) trace[3 + 3 * c] = clock64();
   }
   }  // pass
 }
 
-template <int BN, int AMODE, int EPI, int CG, int EW, bool TMA>
-__global__ void __launch_bounds__(GemmCfg<BN, CG, EW, EPI, TMA>::THREADS, 1)
-gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+template <int BN, int AMODE, int EPI, bool TMA>
+__global__ void __launch_bounds__(GemmCfg<BN, EPI, TMA>::THREADS, 1)
+gemm_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                const __grid_constant__ CUtensorMap tmC, const GemmParams p) {
   constexpr bool HALO = (AMODE == A_CONV3H);
-  using Cfg = GemmCfg<BN, CG, EW, EPI, TMA, HALO>;
-  static_assert(!TMA || (AMODE == A_LINEAR && (BN == 256 || BN == 128) &&
-                         (EPI == EPI_BF16 || EPI == EPI_GELU || EPI == EPI_F32 || EPI == EPI_ROPE)),
-                "TMA-store epilogue: wide linear layers only");
+  using Cfg = GemmCfg<BN, EPI, TMA, HALO>;
+  static_assert(!TMA || (AMODE == A_LINEAR && (EPI == EPI_BF16 || EPI == EPI_GELU || EPI == EPI_F32 || EPI == EPI_ROPE)),
+                "TMA-store epilogue: linear layers only");
   constexpr int STAGES = Cfg::STAGES;
   constexpr uint32_t A_BYTES = Cfg::A_BYTES;
   constexpr uint32_t B_BYTES = Cfg::B_BYTES;
+  constexpr int EW = Cfg::EPI_WARPS;
 
   extern __shared__ __align__(1024) uint8_t smem[];
   uint8_t* sA = smem;
@@ -654,59 +609,34 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Cfg::OFF_BAR);
   uint64_t* full = bars;
   uint64_t* empty = bars + STAGES;
-  uint64_t* tfull = bars + 2 * STAGES;
-  uint64_t* tempty = tfull + 2;
-  [[maybe_unused]] uint64_t* hfull = tempty + 2;   // halo tiles (A_CONV3H), up to 3 stages
-  [[maybe_unused]] uint64_t* hempty = tempty + 5;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty + 8);
-  static_assert(Cfg::HALO_STAGES <= 3 && (2 * STAGES + 12) * 8 + 4 <= Cfg::BAR_BYTES, "barrier area");
+  [[maybe_unused]] uint64_t* hfull = bars + 2 * STAGES;  // halo tiles (A_CONV3H)
+  [[maybe_unused]] uint64_t* hempty = hfull + Cfg::HALO_STAGES;
+  static_assert((2 * STAGES + 2 * Cfg::HALO_STAGES) * 8 <= Cfg::BAR_BYTES, "barrier area");
   [[maybe_unused]] float* epi_smem = reinterpret_cast<float*>(smem + Cfg::OFF_EPI);
-  uint8_t* stg_all = smem + Cfg::OFF_STG;
+  [[maybe_unused]] uint8_t* stg_all = smem + Cfg::OFF_STG;
+  float* acc_s = reinterpret_cast<float*>(smem + Cfg::OFF_ACC);
   [[maybe_unused]] float* rope_s = reinterpret_cast<float*>(smem + Cfg::OFF_ROPE);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const uint32_t cta_rank = (CG == 2) ? cluster_ctarank() : 0u;
-  const bool leader = (cta_rank == 0);
 
-  // 128-row tiles; a work item covers CG consecutive ones
-  const int m_tiles128 = is_conv(AMODE) ? p.nimg * p.tiles_h * p.tiles_w : (p.M + 127) / 128;
-  const int m_tiles = (m_tiles128 + CG - 1) / CG;
+  const int m_tiles = is_conv(AMODE) ? p.nimg * p.tiles_h * p.tiles_w : (p.M + 127) / 128;
   const int n_tiles = (p.N + BN - 1) / BN;
   const int ksplit = TMA ? p.ksplit : 1;
   const int num_tiles = m_tiles * n_tiles * ksplit;  // work items (m, n, ks), ks fastest
   const int cpb = is_conv(AMODE) ? (p.Cin / 64) : 1;  // 64-channel chunks per filter tap
   const int nkb = is_conv(AMODE) ? 9 * cpb : (p.K + 63) / 64;
-  const int first_tile = blockIdx.x / CG;
-  const int tile_step = gridDim.x / CG;
-  // work items: tiles [0, num_tiles), the last tail_r of them as two half tiles each (TMA epilogue / CTA pair / BN = 256 only)
-  constexpr bool TAIL = TMA && CG == 2 && BN == 256 && EPI == EPI_F32;
-  const int tail_r = TAIL ? p.tail_r : 0;
-  const int num_work = num_tiles + tail_r;
-  auto work_tile = [&](int w, int& half) {
-    half = -1;
-    if (TAIL && tail_r > 0 && w >= p.tail_first) {
-      const int q = w - p.tail_first;
-      half = q & 1;
-      return p.tail_first + (q >> 1);
-    }
-    return w;
-  };
 
   if (threadIdx.x == 0) {
     if ((smem_u32(smem) & 1023u) != 0) device_fatal("dynamic shared memory is not 1024-byte aligned");
     for (int s = 0; s < STAGES; ++s) {
-      mbar_init(&full[s], 1);   // the leader's producer arrives once (its expect_tx covers both CTAs' bytes)
-      mbar_init(&empty[s], 1);  // one (multicast) tcgen05.commit
+      mbar_init(&full[s], 1);    // the producer's expect_tx arrival
+      mbar_init(&empty[s], EW);  // one arrival per consumer warp
     }
-    mbar_init(&tfull[0], 1);
-    mbar_init(&tfull[1], 1);
-    mbar_init(&tempty[0], Cfg::EPI_WARPS * CG);  // every epilogue warp of the pair arrives on the leader's barrier
-    mbar_init(&tempty[1], Cfg::EPI_WARPS * CG);
     if constexpr (HALO) {
       for (int s = 0; s < Cfg::HALO_STAGES; ++s) {
         mbar_init(&hfull[s], 1);
-        mbar_init(&hempty[s], 1);
+        mbar_init(&hempty[s], EW);
       }
     }
     fence_mbar_init();
@@ -726,45 +656,27 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
             __ldg(reinterpret_cast<const float4*>(p.rope_tab + i));
     }
   }
-  if (warp == 2) {
-    if constexpr (CG == 2) {
-      tmem_alloc_cg2(tmem_slot, 2 * BN);
-      tmem_relinquish_cg2();
-    } else {
-      tmem_alloc(tmem_slot, 2 * BN);
-      tmem_relinquish();
-    }
-  }
-  tc_fence_before();
-  __syncthreads();  // CTA-level barrier also for CG == 2: orders the barrier init / TMEM-slot write for this CTA's readers
-                    // (and is what compute-sanitizer racecheck models; barrier.cluster alone is reported as a hazard)
-  if constexpr (CG == 2) cluster_sync_all();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
+  __syncthreads();
   pdl_wait();               // previous kernel's outputs (A operand, residuals) are complete and visible
   pdl_launch_dependents();  // the next kernel may start its prologue
 
   if (warp == 0) {
-    // ===================== TMA producer (one per CTA) =====================
-    if (elect_one()) {
+    // ===================== TMA producer =====================
+    if (lane == 0) {
       int stage = 0;
       uint32_t phase = 0;
       [[maybe_unused]] int hstage = 0;
       [[maybe_unused]] uint32_t hphase = 0;
-      for (int w = first_tile; w < num_work; w += tile_step) {
-        int half;
-        const int tile = work_tile(w, half);
+      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
         const int ks = tile % ksplit, mn = tile / ksplit;
-        const int m_tile = (mn / n_tiles) * CG + static_cast<int>(cta_rank);  // this CTA's 128-row tile
+        const int m_tile = mn / n_tiles;
         const int n_tile = mn % n_tiles;
         const int kb0 = ks * nkb / ksplit, kb1 = (ks + 1) * nkb / ksplit;
-        // half tile: this CTA's 64 weight rows are the first 64 of the (full-size) box it loads
-        const int b_row0 = (half < 0) ? n_tile * BN + static_cast<int>(cta_rank) * (BN / CG)
-                                      : n_tile * BN + half * (BN / 2) + static_cast<int>(cta_rank) * (BN / 4);
+        const int b_row0 = n_tile * BN;
         int cn = 0, ch0 = 0, cw0 = 0;
         if constexpr (is_conv(AMODE)) {
           const int tpi = p.tiles_h * p.tiles_w;
-          cn = m_tile / tpi;  // >= nimg for the padding tile of an odd tile count: TMA zero-fills
+          cn = m_tile / tpi;
           const int t = m_tile - cn * tpi;
           const int th = t / p.tiles_w;
           ch0 = th * (HALO ? 16 : 8);
@@ -774,173 +686,120 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
           // channel chunk outermost: one halo tile, then the nine taps' weight tiles
           for (int cc = 0; cc < cpb; ++cc) {
             mbar_wait(&hempty[hstage], hphase ^ 1);
-            if (CG == 1 || leader) mbar_arrive_expect_tx(&hfull[hstage], CG * Cfg::HALO_TX_BYTES);
-            if constexpr (CG == 2)
-              tma_load_4d_cg2(sH + hstage * Cfg::HALO_BYTES, &tmA, &hfull[hstage], cc * 64, cw0 - 1, ch0 - 1, cn);
-            else
-              tma_load_4d(sH + hstage * Cfg::HALO_BYTES, &tmA, &hfull[hstage], cc * 64, cw0 - 1, ch0 - 1, cn);
+            mbar_arrive_expect_tx(&hfull[hstage], Cfg::HALO_TX_BYTES);
+            tma_load_4d(sH + hstage * Cfg::HALO_BYTES, &tmA, &hfull[hstage], cc * 64, cw0 - 1, ch0 - 1, cn);
             if (++hstage == Cfg::HALO_STAGES) { hstage = 0; hphase ^= 1; }
             for (int tap = 0; tap < 9; ++tap) {
               mbar_wait(&empty[stage], phase ^ 1);
-              if (CG == 1 || leader) mbar_arrive_expect_tx(&full[stage], CG * B_BYTES);
-              if constexpr (CG == 2)
-                tma_load_2d_cg2(sB + stage * B_BYTES, &tmB, &full[stage], (tap * cpb + cc) * 64, b_row0);
-              else
-                tma_load_2d(sB + stage * B_BYTES, &tmB, &full[stage], (tap * cpb + cc) * 64, b_row0);
+              mbar_arrive_expect_tx(&full[stage], B_BYTES);
+              tma_load_2d(sB + stage * B_BYTES, &tmB, &full[stage], (tap * cpb + cc) * 64, b_row0);
               if (++stage == STAGES) { stage = 0; phase ^= 1; }
             }
           }
         } else {
-        for (int kb = kb0; kb < kb1; ++kb) {
-          mbar_wait(&empty[stage], phase ^ 1);
-          if (CG == 1 || leader) mbar_arrive_expect_tx(&full[stage], CG * (A_BYTES + B_BYTES));
-          if constexpr (AMODE == A_CONV3) {
-            const int tap = kb / cpb;
-            const int cc = kb - tap * cpb;
-            const int kh = tap / 3;
-            const int kw = tap - kh * 3;
-            if constexpr (CG == 2)
-              tma_load_4d_cg2(sA + stage * A_BYTES, &tmA, &full[stage], cc * 64, cw0 + kw - 1, ch0 + kh - 1, cn);
-            else
+          for (int kb = kb0; kb < kb1; ++kb) {
+            mbar_wait(&empty[stage], phase ^ 1);
+            mbar_arrive_expect_tx(&full[stage], A_BYTES + B_BYTES);
+            if constexpr (AMODE == A_CONV3) {
+              const int tap = kb / cpb;
+              const int cc = kb - tap * cpb;
+              const int kh = tap / 3;
+              const int kw = tap - kh * 3;
               tma_load_4d(sA + stage * A_BYTES, &tmA, &full[stage], cc * 64, cw0 + kw - 1, ch0 + kh - 1, cn);
-          } else {
-            if constexpr (CG == 2)
-              tma_load_2d_cg2(sA + stage * A_BYTES, &tmA, &full[stage], kb * 64, m_tile * 128);
-            else
+            } else {
               tma_load_2d(sA + stage * A_BYTES, &tmA, &full[stage], kb * 64, m_tile * 128);
-          }
-          if constexpr (CG == 2)
-            tma_load_2d_cg2(sB + stage * B_BYTES, &tmB, &full[stage], kb * 64, b_row0);
-          else
-            tma_load_2d(sB + stage * B_BYTES, &tmB, &full[stage], kb * 64, b_row0);
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ===================== MMA issuer (leader CTA only) =====================
-    if (leader && elect_one()) {
-      constexpr uint32_t idesc = make_idesc_bf16(128 * CG, BN, 0, 0);
-      int stage = 0;
-      uint32_t phase = 0;
-      [[maybe_unused]] int hstage = 0;
-      [[maybe_unused]] uint32_t hphase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      for (int w = first_tile; w < num_work; w += tile_step) {
-        int half;
-        const int tile = work_tile(w, half);
-        const uint32_t idesc_t = (half < 0) ? idesc : make_idesc_bf16(128 * CG, BN / 2, 0, 0);
-        const int tcount = (w - first_tile) / tile_step;
-        const bool trc = p.dbg && blockIdx.x == 0 && tcount < 40;
-        if (trc) p.dbg[256 + 4 * tcount + 0] = clock64();
-        mbar_wait(&tempty[acc], acc_phase ^ 1);
-        if (trc) p.dbg[256 + 4 * tcount + 1] = clock64();
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * BN;
-        const int ks = tile % ksplit;
-        const int kb0 = ks * nkb / ksplit, kb1 = (ks + 1) * nkb / ksplit;
-        if constexpr (HALO) {
-          for (int cc = 0; cc < cpb; ++cc) {
-            mbar_wait(&hfull[hstage], hphase);
-            const uint32_t hbase = smem_u32(sH + hstage * Cfg::HALO_BYTES);
-            for (int tap = 0; tap < 9; ++tap) {
-              mbar_wait(&full[stage], phase);
-              tc_fence_after();
-              const int kh = tap / 3, kw = tap - kh * 3;
-              // output pixel (y, x) of the 16 x 8 tile reads halo pixel (y + kh, x + kw); halo rows are kHaloPitch pixels
-              const uint64_t adesc = make_smem_desc_sw128_rows(hbase + (kh * kHaloPitch + kw) * 128, kHaloPitch * 128);
-              const uint64_t bdesc = make_smem_desc_sw128(smem_u32(sB + stage * B_BYTES));
-#pragma unroll
-              for (int k = 0; k < 4; ++k) {
-                if constexpr (CG == 2)
-                  umma_bf16_cg2(d_tmem, adesc + 2 * k, bdesc + 2 * k, idesc, (cc > 0 || tap > 0 || k != 0) ? 1u : 0u);
-                else
-                  umma_bf16(d_tmem, adesc + 2 * k, bdesc + 2 * k, idesc, (cc > 0 || tap > 0 || k != 0) ? 1u : 0u);
-              }
-              if constexpr (CG == 2) umma_commit_cg2(&empty[stage]); else umma_commit(&empty[stage]);
-              if (++stage == STAGES) { stage = 0; phase ^= 1; }
             }
-            if constexpr (CG == 2) umma_commit_cg2(&hempty[hstage]); else umma_commit(&hempty[hstage]);
-            if (++hstage == Cfg::HALO_STAGES) { hstage = 0; hphase ^= 1; }
+            tma_load_2d(sB + stage * B_BYTES, &tmB, &full[stage], kb * 64, b_row0);
+            if (++stage == STAGES) { stage = 0; phase ^= 1; }
           }
-        } else {
-        for (int kb = kb0; kb < kb1; ++kb) {
-          mbar_wait(&full[stage], phase);
-          tc_fence_after();
-          const uint64_t adesc = make_smem_desc_sw128(smem_u32(sA + stage * A_BYTES));
-          const uint64_t bdesc = make_smem_desc_sw128(smem_u32(sB + stage * B_BYTES));
-#pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            // advance 16 K-elements = 32 bytes inside the 128B swizzle atom (encoded >> 4)
-            if constexpr (CG == 2)
-              umma_bf16_cg2(d_tmem, adesc + 2 * k, bdesc + 2 * k, idesc_t, (kb > kb0 || k != 0) ? 1u : 0u);
-            else
-              umma_bf16(d_tmem, adesc + 2 * k, bdesc + 2 * k, idesc_t, (kb > kb0 || k != 0) ? 1u : 0u);
-          }
-          if constexpr (CG == 2) umma_commit_cg2(&empty[stage]); else umma_commit(&empty[stage]);
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
         }
-        }
-        if constexpr (CG == 2) umma_commit_cg2(&tfull[acc]); else umma_commit(&tfull[acc]);
-        if (trc) p.dbg[256 + 4 * tcount + 2] = clock64();
-        acc ^= 1;
-        if (acc == 0) acc_phase ^= 1;
       }
     }
   } else if (warp >= 4) {
-    // ============ epilogue warps (every CTA drains its own 128 accumulator rows) ============
-    const int quarter = warp & 3;
-    const int part = (warp - 4) >> 2;  // which quarter of the tile's columns
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    for (int w = first_tile; w < num_work; w += tile_step) {
-      int half;
-      const int tile = work_tile(w, half);
+    // ============ consumer warpgroups: mainloop (wgmma) + epilogue ============
+    const int wg = (warp - 4) >> 2;     // rows [64 wg, 64 wg + 64) of the tile in the mainloop
+    const int wq = (warp - 4) & 3;      // warp inside the warpgroup: 16 of those rows
+    const int quarter = warp & 3;       // epilogue mapping: rows [32 quarter, +32) ...
+    const int part = (warp - 4) >> 2;   // ... columns [part * BN / 2, +BN / 2)
+    int stage = 0;
+    uint32_t phase = 0;
+    [[maybe_unused]] int hstage = 0;
+    [[maybe_unused]] uint32_t hphase = 0;
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       const int ks = tile % ksplit, mn = tile / ksplit;
-      const int m_tile = (mn / n_tiles) * CG + static_cast<int>(cta_rank);
+      const int m_tile = mn / n_tiles;
       const int n_tile = mn % n_tiles;
-      const int tcount = (w - first_tile) / tile_step;
-      const bool trc = p.dbg && blockIdx.x == 0 && warp == 4 && lane == 0 && tcount < 40;
-      if (trc) p.dbg[4 * tcount + 0] = clock64();
-      if (trc) p.dbg[4 * tcount + 1] = clock64();
-      // columns of this epilogue warp: a quarter-of-the-parts slice of the full tile, or of the 128-column half tile
-      const int cols_w = (half < 0 ? BN : BN / 2) / Cfg::PARTS;
-      const uint32_t taddr = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16) + acc * BN + part * cols_w;
-      // hand the accumulator stage back to the MMA warp (called once all of this warp's TMEM loads have landed)
-      auto release = [&]() {
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) {
-          if (CG == 1 || leader) mbar_arrive(&tempty[acc]); else mbar_arrive_remote(&tempty[acc], 0);
-        }
+      const int kb0 = ks * nkb / ksplit, kb1 = (ks + 1) * nkb / ksplit;
+      float acc[BN / 2];
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) acc[i] = 0.0f;
+      // one k-block: four k16 steps; the previous k-block's wgmma group may still run, its stage is released
+      // once this one is issued
+      int prev = -1;
+      auto kblock = [&](uint64_t adesc, uint64_t bdesc) {
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < 4; ++k) wgmma_m64n128k16_ss(acc, adesc + 2 * k, bdesc + 2 * k, 1u);
+        wgmma_commit();
+        wgmma_wait<1>();
+        fence_regs(acc);
+        if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
+        prev = stage;
+        if (++stage == STAGES) { stage = 0; phase ^= 1; }
       };
-      if constexpr (TMA) {
-        epilogue_tile_tma<BN, EPI, EW>(p, &tmC, taddr, m_tile, n_tile * BN + (half < 0 ? 0 : half * (BN / 2)) + part * cols_w,
-                                       cols_w / 32, ks * p.split_rows, quarter, part,
-                                       stg_all + (warp - 4) * Cfg::STG_WARP_BYTES, rope_s, &tfull[acc], acc_phase, release,
-                                       (trc && tcount < 16) ? p.dbg + 512 + 16 * tcount : nullptr);
+      if constexpr (HALO) {
+        for (int cc = 0; cc < cpb; ++cc) {
+          mbar_wait(&hfull[hstage], hphase);
+          // output pixel (y, x) of the 16 x 8 tile reads halo pixel (y + kh, x + kw); halo rows are kHaloPitch pixels,
+          // and this warpgroup's 64 rows are the output rows y = 8 wg .. 8 wg + 7
+          const uint32_t hbase = smem_u32(sH + hstage * Cfg::HALO_BYTES) + wg * 8 * kHaloPitch * 128;
+          for (int tap = 0; tap < 9; ++tap) {
+            mbar_wait(&full[stage], phase);
+            const int kh = tap / 3, kw = tap - kh * 3;
+            kblock(make_smem_desc_sw128_rows(hbase + (kh * kHaloPitch + kw) * 128, kHaloPitch * 128),
+                   make_smem_desc_sw128(smem_u32(sB + stage * B_BYTES)));
+          }
+          wgmma_wait<0>();  // every read of this halo tile has completed
+          fence_regs(acc);
+          if (lane == 0) mbar_arrive(&hempty[hstage]);
+          if (++hstage == Cfg::HALO_STAGES) { hstage = 0; hphase ^= 1; }
+        }
       } else {
-        epilogue_tile<BN, AMODE, EPI, EW>(p, taddr, m_tile, n_tile, quarter, part, epi_smem,
-                                          reinterpret_cast<float*>(stg_all + (warp - 4) * Cfg::STG_WARP_BYTES), rope_s,
-                                          &tfull[acc], acc_phase);
-        release();
+        for (int kb = kb0; kb < kb1; ++kb) {
+          mbar_wait(&full[stage], phase);
+          kblock(make_smem_desc_sw128(smem_u32(sA + stage * A_BYTES) + wg * 64 * 128),
+                 make_smem_desc_sw128(smem_u32(sB + stage * B_BYTES)));
+        }
       }
-      if (trc) p.dbg[4 * tcount + 2] = clock64();
-      acc ^= 1;
-      if (acc == 0) acc_phase ^= 1;
+      wgmma_wait<0>();
+      fence_regs(acc);
+      if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
+
+      // accumulators -> shared tile (wgmma layout: register 4j + {0,1} = row g, columns 8j + 2t + {0,1}; 4j + {2,3} = row g + 8)
+      named_bar_sync(1, Cfg::EPI_THREADS);  // the previous tile's epilogue has finished reading the tile
+      {
+        const int r0 = wg * 64 + wq * 16 + (lane >> 2);
+        const int c0 = 2 * (lane & 3);
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+          *reinterpret_cast<float2*>(acc_s + r0 * Cfg::ACC_LD + 8 * j + c0) = make_float2(acc[4 * j], acc[4 * j + 1]);
+          *reinterpret_cast<float2*>(acc_s + (r0 + 8) * Cfg::ACC_LD + 8 * j + c0) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+        }
+      }
+      named_bar_sync(1, Cfg::EPI_THREADS);
+      const int cols_w = BN / Cfg::PARTS;
+      if constexpr (TMA) {
+        epilogue_tile_tma<BN, EPI, EW>(p, &tmC, acc_s + (quarter * 32 + lane) * Cfg::ACC_LD + part * cols_w, m_tile,
+                                       n_tile * BN + part * cols_w, ks * p.split_rows, quarter,
+                                       stg_all + (warp - 4) * Cfg::STG_WARP_BYTES, rope_s);
+      } else {
+        epilogue_tile<BN, AMODE, EPI, EW>(p, acc_s + quarter * 32 * Cfg::ACC_LD + part * cols_w, m_tile, n_tile, quarter,
+                                          part, epi_smem, rope_s);
+      }
     }
     if constexpr (TMA) {
       if (lane == 0) tma_store_wait_all();  // the bulk stores read this CTA's shared memory
     }
-  }
-
-  tc_fence_before();
-  if constexpr (CG == 2) cluster_sync_all(); else __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    if constexpr (CG == 2) tmem_dealloc_cg2(tmem_base, 2 * BN); else tmem_dealloc(tmem_base, 2 * BN);
   }
 }
 

@@ -66,13 +66,13 @@ int make_tmap(CUtensorMap* out, const void* base, int is_f32, int rank, const ui
 int num_sms() {
   static std::atomic<int> cache[64];  // zero-initialised; one slot per device ordinal
   int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess) return 148;
+  if (cudaGetDevice(&dev) != cudaSuccess) return 132;
   if (dev >= 0 && dev < 64) {
     const int c = cache[dev].load(std::memory_order_relaxed);
     if (c > 0) return c;
   }
   int n = 0;
-  if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) return 148;
+  if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) return 132;
   if (dev >= 0 && dev < 64) cache[dev].store(n, std::memory_order_relaxed);
   return n;
 }

@@ -1,4 +1,4 @@
-// Bandwidth-bound and tiny kernels of the STA forward pass (sm_100a, plain SIMT with
+// Bandwidth-bound and tiny kernels of the STA forward pass (sm_90a, plain SIMT with
 // 128-bit vector accesses): LayerNorm, patch im2col, token positions, casts,
 // bilinear x2 upsampling, strided im2col, pose head (MLP + 3x3 SVD orthogonalisation),
 // and the RoPE sin/cos table.

@@ -171,7 +171,7 @@ using namespace sta;
 
 struct StaModel {
   // Precision of the tensor-core operands: 0 = bf16 (production), 1 = split-precision "x3" parity mode -- every bf16
-  // activation is (hi | lo | hi), every bf16 weight (hi | hi | lo) (common.cuh), the same gemm_tc_kernel mainloop runs
+  // activation is (hi | lo | hi), every bf16 weight (hi | hi | lo) (common.cuh), the same gemm_wg_kernel mainloop runs
   // over 3K, attention runs in fp32 on the CUDA cores.  ~17 significant operand bits instead of 8; ~3.5x slower.
   int split = 0;
   int bmul() const { return split ? 3 : 1; }
@@ -746,16 +746,15 @@ int run_decoder(const Ctx& c, int B, int N, DecBufs& d, float* const* out1, floa
   m->launches++;
   RUN(launch_fill_pose_token(d.xd, m->pose_tok, S, M, kDecDim, c.st));
   RUN(emit(0));
-  // the pose token (query row 0) goes to the attention kernel's spare warps when that saves a pair of query tiles
-  // The pose token (query row 0) can go to a separate small kernel so that the tiled kernel runs 3 instead of 4
-  // query-tile pairs per (head, sample).  Measured on B200 the attention time drops (7.9 -> 7.5 ms per cfg-2 step) but
-  // the 24 extra launches cost more than that end to end (34.0 vs 33.4 ms), so it is off unless STA_ATTN_SPLIT_POSE=1.
+  // The pose token (query row 0) can go to a separate small kernel so that the tiled kernel runs one 128-query tile
+  // fewer per (head, sample) when M = 128 k + 1, at the price of 12 extra launches per view; off unless
+  // STA_ATTN_SPLIT_POSE=1.
   static int split_env = -1;
   if (split_env < 0) {
     const char* e = getenv("STA_ATTN_SPLIT_POSE");
     split_env = (e && e[0] == '1') ? 1 : 0;
   }
-  const int split_pose = (split_env && (M - 1 + 255) / 256 < (M + 255) / 256) ? 1 : 0;
+  const int split_pose = (split_env && (M - 1 + 127) / 128 < (M + 127) / 128) ? 1 : 0;
   for (int l = 0; l < 12; ++l) {
     const DecBlock& b = m->dec[l];
     // self-attention on norm1(x); norm_y(x) is what the partner view cross-attends to
@@ -917,8 +916,8 @@ int check_ready(StaModel* m) {
   return 0;
 }
 
-// DPT parts per view in the host entry point.  Two halves measured best on B200 (r02: exposed copy 2.0 ms per 16-pair step;
-// four parts of 4 images shorten the D2H tail but the smaller DPT batches cost more than that: 3.0 ms).
+// DPT parts per view in the host entry point: two halves, so that the device-to-host copy of the first half overlaps
+// the DPT of the second.
 int host_dpt_parts(int B) { return B >= 2 ? 2 : 1; }
 
 // one stream per handle at a time: order a call on `st` after everything this handle enqueued on its previous stream
@@ -1013,9 +1012,9 @@ int sta_create_ex(StaModel** out, int precision) {
   STA_CHECK_CUDA(cudaGetDevice(&dev));
   cudaDeviceProp prop;
   STA_CHECK_CUDA(cudaGetDeviceProperties(&prop, dev));
-  if (prop.major != 10) {
+  if (prop.major != 9 || prop.minor != 0) {
     char buf[160];
-    snprintf(buf, sizeof(buf), "sta_b200 needs a Blackwell sm_100 GPU (found %s, sm_%d%d); there is no fallback path",
+    snprintf(buf, sizeof(buf), "sta_b200 needs a Hopper sm_90 GPU (found %s, sm_%d%d); there is no fallback path",
              prop.name, prop.major, prop.minor);
     set_last_error(buf);
     return 3;
@@ -1563,8 +1562,8 @@ int sta_forward_pairs_host(StaModel* m, const void* img1_host, const void* img2_
 
   // Pipeline over chunks of pairs: the H2D copy of chunk c+1 and the D2H copy of chunk c-1 overlap the compute
   // of chunk c (separate copy streams, pinned host memory makes them truly asynchronous).
-  // one chunk of up to 16 pairs measured best on B200 (448 vs 433 pairs/s for two chunks of 8 at B = 16: the exposed
-  // H2D of a 16-pair chunk costs less than running the GEMMs at half the tile count); larger batches pipeline chunks
+  // one chunk of up to 16 pairs (the exposed H2D of a 16-pair chunk is meant to cost less than running the GEMMs at half
+  // the tile count); larger batches pipeline chunks
   int cp = B;
   {
     static int chunk_env = -1;  // STA_HOST_CHUNK=n overrides the pairs per pipelined chunk (tuning knob)

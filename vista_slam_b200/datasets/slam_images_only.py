@@ -37,7 +37,7 @@ class SLAM_image_only:
             raise ValueError("expected an HxWx3 uint8 RGB frame")
         frame = rgb_image.to(self.device, non_blocking=True).contiguous()
         if not frame.is_cuda:
-            raise RuntimeError("the B200 preprocessing has no CPU path")
+            raise RuntimeError("the CUDA preprocessing has no CPU path")
         H, W, _ = frame.shape
         oh, ow = self.output_shape(H, W, w_edge, h_edge)
         rgb = torch.empty(3, oh, ow, dtype=torch.float32, device=frame.device)

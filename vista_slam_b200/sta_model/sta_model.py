@@ -6,7 +6,7 @@ Same class name, constructor defaults, attributes, 665-key state_dict and entry 
 vista_slam/slam.py:95-106,142-189 and sta_model/train.py:208,278 (inference) call it unchanged.
 
 Nothing is computed in PyTorch: every entry point hands raw device pointers to the hand-written
-sm_100a kernels behind the C ABI (include/sta_b200.h, csrc/).  PyTorch only owns the parameter
+sm_90a kernels behind the C ABI (include/sta_b200.h, csrc/).  PyTorch only owns the parameter
 tensors, the input/output buffers and the CUDA stream.  There is no CPU or eager fallback: a
 call on a non-CUDA tensor, or without the built library, raises.
 """
@@ -128,7 +128,7 @@ def _attach(root, dotted, param):
 
 
 class SymmetricTwoViewAssociation(nn.Module):
-    """B200-native STA frontend with the reference's module surface (sta_model.py:26-52 for the defaults)."""
+    """H100-native STA frontend with the reference's module surface (sta_model.py:26-52 for the defaults)."""
 
     def __init__(self, img_size=(224, 224), patch_size=16, enc_embed_dim=1024, enc_depth=24, enc_num_heads=16,
                  dec_embed_dim=768, dec_depth=12, dec_num_heads=12, mlp_ratio=4, norm_layer=None, pos_embed="RoPE100",
@@ -149,7 +149,7 @@ class SymmetricTwoViewAssociation(nn.Module):
         for k, (got, want) in fixed.items():
             if got != want:
                 raise NotImplementedError(
-                    "the sm_100a kernels are specialised for the reference's default STA() configuration; "
+                    "the sm_90a kernels are specialised for the reference's default STA() configuration; "
                     "%s=%r is not supported (expected %r)" % (k, got, want))
         if norm_layer is not None:
             probe = norm_layer(8)
@@ -230,7 +230,7 @@ class SymmetricTwoViewAssociation(nn.Module):
     def _ready(self, like):
         """Create the C handle on the tensor's device and (re-)upload the packed weights if needed."""
         if not like.is_cuda:
-            raise RuntimeError("vista_slam_b200 runs only on CUDA (sm_100a) tensors; there is no CPU path")
+            raise RuntimeError("vista_slam_b200 runs only on CUDA (sm_90a) tensors; there is no CPU path")
         L = _lib.lib()
         key = (like.device.index, self._state_key())
         if self._handle is not None and self._uploaded_key == key:

@@ -26,7 +26,7 @@ def _scratch_for(device, V):
 
 def _f32_cuda(t, name):
     if not isinstance(t, torch.Tensor) or not t.is_cuda:
-        raise RuntimeError("%s must be a CUDA tensor (the B200 library has no CPU path)" % name)
+        raise RuntimeError("%s must be a CUDA tensor (the CUDA library has no CPU path)" % name)
     return t.detach().to(torch.float32).contiguous()
 
 
