@@ -28,7 +28,7 @@ typedef struct StaModel StaModel; /* opaque */
 
 /* ---- library ---- */
 const char* sta_last_error(void);
-int sta_version(void);                 /* ABI version, currently 1 */
+int sta_version(void);                 /* ABI version, currently 2 */
 int sta_device_synchronize(void);      /* cudaDeviceSynchronize + error check */
 
 /* ---- model lifetime (replaces STA() + load_state_dict + .to(cuda), slam.py:95-106) ---- */
@@ -150,12 +150,10 @@ typedef struct StaGemmDesc {
 int sta_op_gemm(const StaGemmDesc* d, void* stream);
 
 /* softmax(q k^T * scale) v, head_dim 64.  q/k/v: [batch][n*][ld*] bf16 with head h at columns
- * *_col0 + 64*h; out: [batch][nq][ldo] bf16.  kv sample for query sample b is (b + kv_batch_shift) % batch.
- * split_first_row != 0: query row 0 (the decoder's pose token) is computed by a small SIMT kernel and the
- * tensor-core kernel tiles rows [1, nq) -- same result, avoids a 128-row tile for one row when nq = 128k + 1. */
+ * *_col0 + 64*h; out: [batch][nq][ldo] bf16.  kv sample for query sample b is (b + kv_batch_shift) % batch. */
 int sta_op_attention(const void* q, int64_t ldq, int q_col0, const void* k, int64_t ldk, int k_col0, const void* v,
                      int64_t ldv, int v_col0, void* out, int64_t ldo, int batch, int heads, int nq, int nk,
-                     int kv_batch_shift, float scale, int split_first_row, void* stream);
+                     int kv_batch_shift, float scale, void* stream);
 
 int sta_op_layernorm(const float* x, int rows, int C, float eps, const float* g1, const float* b1, void* out1_bf16,
                      const float* g2, const float* b2, void* out2_bf16, int drop_first_of, void* stream);
@@ -195,8 +193,8 @@ int sta_regress_pairs_finish(StaModel* m, const int* edge_idx_host, int n_sel, f
                              void* stream);
 
 /* Launch-bound sizes (<= 8192 tokens per call: one keyframe, a few edges) of sta_encode and sta_regress_pairs are
- * captured into CUDA graphs per (entry point, batch, H, W) on their second use and replayed afterwards
- * (STA_CUDA_GRAPHS=0 disables).  Number of graph replays so far (tests / diagnostics): */
+ * captured into CUDA graphs per (entry point, batch, H, W) on their second use and replayed afterwards (not while
+ * sta_profile is enabled).  Number of graph replays so far (tests / diagnostics): */
 int64_t sta_graph_replays(StaModel* m);
 
 /* ---- pointmap consumers (SURVEY.md 8(f) rank 2): what OnlineSLAM.regress_two_views / connect_view_i_j compute from

@@ -10,7 +10,7 @@ import torch
 from conftest import GOLDEN_DIR, ROOT
 
 
-def test_library_exports_every_declared_symbol():
+def test_library_exports_every_declared_symbol_of_abi_version_2():
     from vista_slam_b200 import _lib
     L = _lib.lib()
     hdr = open(os.path.join(ROOT, "include", "sta_b200.h")).read()
@@ -18,7 +18,7 @@ def test_library_exports_every_declared_symbol():
     assert len(names) >= 25
     missing = [n for n in names if not hasattr(L, n)]
     assert not missing, missing
-    assert L.sta_version() == 1
+    assert L.sta_version() == 2
 
 
 def test_module_surface_matches_reference():

@@ -13,7 +13,7 @@ import time
 
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), ".."))
 
-GROUPS = ["gemm_basic", "gemm_epi", "conv", "attention", "misc", "x3", "perf"]
+GROUPS = ["gemm_basic", "gemm_epi", "conv", "coalesced_epi", "attention", "misc", "x3", "perf"]
 
 
 def report(name, got, ref, tol):
@@ -106,11 +106,11 @@ def group_gemm_epi():
     out = torch.zeros(M, N, device=dev, dtype=torch.bfloat16)
     run_gemm(gemm_desc(epi=EPI_BF16, A=A, lda=K, W=W, ldw=K, M=M, N=N, K=K, bias=bias, out=out, ldo=N, relu_main=1))
     report("epi bf16 relu main", out, base.relu(), 1e-2)
-    # N = 384 -> BN 128 path
+    # N = 384: an odd number of 128-column tiles, no bias
     W3 = (torch.randn(384, K, device=dev) / math.sqrt(K)).bfloat16()
     out = torch.zeros(M, 384, device=dev, dtype=torch.bfloat16)
     run_gemm(gemm_desc(epi=EPI_BF16, A=A, lda=K, W=W3, ldw=K, M=M, N=384, K=K, out=out, ldo=384))
-    report("epi bf16 N384 (BN128, no bias)", out, A.float() @ W3.float().t(), 1e-2)
+    report("epi bf16 N384 (no bias)", out, A.float() @ W3.float().t(), 1e-2)
     # F32 with residual in place
     x = torch.randn(M, N, device=dev)
     x0 = x.clone()
@@ -257,6 +257,34 @@ def group_conv():
     torch.cuda.synchronize()
 
 
+def group_coalesced_epi():
+    """Stores of the coalesced per-warp epilogue that the shapes of gemm_epi and conv do not reach."""
+    import torch
+    import torch.nn.functional as F
+    from vista_slam_b200._lib import EPI_BF16, EPI_F32
+    torch.manual_seed(6)
+    dev = "cuda"
+    # in-place fp32 residual update with N % 128 != 0: the epilogue loads the residual rows before it stores over them
+    M, N, K = 777, 320, 256
+    A = torch.randn(M, K, device=dev).bfloat16()
+    W = (torch.randn(N, K, device=dev) / math.sqrt(K)).bfloat16()
+    bias = torch.randn(N, device=dev)
+    x = torch.randn(M, N, device=dev)
+    x0 = x.clone()
+    run_gemm(gemm_desc(epi=EPI_F32, A=A, lda=K, W=W, ldw=K, M=M, N=N, K=K, bias=bias, out=x, ldo=N, resid=x))
+    report("f32 resid in place N320", x, x0 + A.float() @ W.float().t() + bias, 2e-3)
+    # conv with no bias, no residual, relu on the main output (the first conv of a DPT residual unit)
+    nimg, H, W, Cin, Cout = 2, 14, 18, 256, 256
+    x = torch.randn(nimg, H, W, Cin, device=dev).bfloat16()
+    wp = (torch.randn(Cout, 9 * Cin, device=dev) / math.sqrt(9 * Cin)).bfloat16()
+    out = torch.full((nimg, H, W, Cout), float("nan"), device=dev, dtype=torch.bfloat16)
+    run_gemm(gemm_desc(conv3x3=1, epi=EPI_BF16, A=x, W=wp, ldw=9 * Cin, N=Cout, K=9 * Cin, nimg=nimg, H=H, Wd=W, Cin=Cin,
+                       out=out, ldo=Cout, relu_main=1))
+    ref = F.conv2d(x.float().permute(0, 3, 1, 2), wp.float().view(Cout, 3, 3, Cin).permute(0, 3, 1, 2), padding=1)
+    report("conv3x3 no bias, relu main", out, ref.permute(0, 2, 3, 1).relu(), 1e-2)
+    torch.cuda.synchronize()
+
+
 def group_attention():
     import torch
     import torch.nn.functional as F
@@ -264,36 +292,40 @@ def group_attention():
     torch.manual_seed(3)
     dev = "cuda"
     L = lib()
-    for (batch, heads, n, shift, split) in [(2, 3, 128, 0, 0), (2, 3, 196, 0, 0), (2, 12, 769, 0, 0), (4, 12, 769, 2, 0),
-                                            (3, 16, 768, 0, 0), (4, 12, 769, 2, 1), (2, 12, 197, 0, 1), (2, 3, 130, 0, 1),
-                                            (2, 3, 257, 1, 1), (3, 2, 1, 0, 1), (2, 2, 901, 1, 1)]:
+    # launch_attention takes 128-row query tiles when that grid has at least one CTA per SM, else 64-row tiles.  On a
+    # 132-SM H100, (2, 12, 769), (4, 12, 769) and (3, 16, 768) take 128 rows, the others 64; both kinds include ragged
+    # last query and key tiles.
+    for (batch, heads, n, shift) in [(2, 3, 128, 0), (2, 3, 196, 0), (2, 12, 769, 0), (4, 12, 769, 2), (3, 16, 768, 0),
+                                     (2, 12, 197, 0), (2, 3, 130, 0), (2, 3, 257, 1), (3, 2, 1, 0), (2, 2, 901, 1)]:
         C = heads * 64
         qkv = torch.randn(batch, n, 3 * C, device=dev).bfloat16()
         out = torch.zeros(batch, n, C, device=dev, dtype=torch.bfloat16)
         check(L.sta_op_attention(ptr(qkv), 3 * C, 0, ptr(qkv), 3 * C, C, ptr(qkv), 3 * C, 2 * C, ptr(out), C, batch,
-                                 heads, n, n, shift, 0.125, split, cur_stream()), "attention")
+                                 heads, n, n, shift, 0.125, cur_stream()), "attention")
         torch.cuda.synchronize()
         q, k, v = [qkv[..., i * C:(i + 1) * C].float().view(batch, n, heads, 64).transpose(1, 2) for i in range(3)]
         if shift:
             idx = [(b + shift) % batch for b in range(batch)]
             k, v = k[idx], v[idx]
         ref = F.scaled_dot_product_attention(q, k, v, scale=0.125).transpose(1, 2).reshape(batch, n, C)
-        report("attention b%d h%d n%d shift%d split%d" % (batch, heads, n, shift, split), out, ref, 2e-2)
+        report("attention b%d h%d n%d shift%d" % (batch, heads, n, shift), out, ref, 2e-2)
     # adversarial for the lazy-rescale / speculative-maximum path: the keys of later tiles score much higher than those
-    # of earlier ones (row maxima jump by far more than 2^8 between key tiles), some rows only in the ragged last tile
-    batch, heads, n = 2, 3, 600
-    C = heads * 64
-    qkv = torch.randn(batch, n, 3 * C, device=dev)
-    growth = 1.0 + 5.0 * (torch.arange(n, device=dev) // 128).float()           # key tile t scaled by 1 + 5t
-    qkv[:, :, C:2 * C] *= growth[None, :, None]
-    qkv[0, 590:, C:2 * C] *= 4.0                                                  # a further jump inside the last tile
-    qkv = qkv.bfloat16()
-    out = torch.zeros(batch, n, C, device=dev, dtype=torch.bfloat16)
-    check(L.sta_op_attention(ptr(qkv), 3 * C, 0, ptr(qkv), 3 * C, C, ptr(qkv), 3 * C, 2 * C, ptr(out), C, batch, heads, n, n,
-                             0, 0.125, 0, cur_stream()), "attention")
-    q, k, v = [qkv[..., i * C:(i + 1) * C].float().view(batch, n, heads, 64).transpose(1, 2) for i in range(3)]
-    ref = F.scaled_dot_product_attention(q, k, v, scale=0.125).transpose(1, 2).reshape(batch, n, C)
-    report("attention growing maxima (rescale path)", out, ref, 2e-2)
+    # of earlier ones (row maxima jump by far more than 2^8 between key tiles), some rows only in the ragged last tile.
+    # 3 heads: 30 CTAs of 128 rows would leave SMs idle -> 64-row tiles; 16 heads: 160 CTAs -> 128-row tiles.
+    batch, n = 2, 600
+    for heads in (3, 16):
+        C = heads * 64
+        qkv = torch.randn(batch, n, 3 * C, device=dev)
+        growth = 1.0 + 5.0 * (torch.arange(n, device=dev) // 128).float()           # key tile t scaled by 1 + 5t
+        qkv[:, :, C:2 * C] *= growth[None, :, None]
+        qkv[0, 590:, C:2 * C] *= 4.0                                                  # a further jump inside the last tile
+        qkv = qkv.bfloat16()
+        out = torch.zeros(batch, n, C, device=dev, dtype=torch.bfloat16)
+        check(L.sta_op_attention(ptr(qkv), 3 * C, 0, ptr(qkv), 3 * C, C, ptr(qkv), 3 * C, 2 * C, ptr(out), C, batch, heads, n,
+                                 n, 0, 0.125, cur_stream()), "attention")
+        q, k, v = [qkv[..., i * C:(i + 1) * C].float().view(batch, n, heads, 64).transpose(1, 2) for i in range(3)]
+        ref = F.scaled_dot_product_attention(q, k, v, scale=0.125).transpose(1, 2).reshape(batch, n, C)
+        report("attention growing maxima (rescale path) h%d" % heads, out, ref, 2e-2)
 
 
 def group_misc():
@@ -527,14 +559,14 @@ def group_perf():
         ms = timeit(lambda: run_gemm(d))
         print("gemm-epi %-22s M%d N%d K%d: %.3f ms = %.0f TFLOP/s" % (name, M, N, K, ms, 2.0 * M * N * K / ms / 1e9), flush=True)
     L = lib()
-    for (batch, heads, n, split) in [(32, 16, 768, 0), (32, 12, 769, 0), (32, 12, 769, 1)]:
+    for (batch, heads, n) in [(32, 16, 768), (32, 12, 769)]:
         C = heads * 64
         qkv = torch.randn(batch, n, 3 * C, device=dev).bfloat16()
         out = torch.zeros(batch, n, C, device=dev, dtype=torch.bfloat16)
         ms = timeit(lambda: check(L.sta_op_attention(ptr(qkv), 3 * C, 0, ptr(qkv), 3 * C, C, ptr(qkv), 3 * C, 2 * C,
-                                                     ptr(out), C, batch, heads, n, n, 0, 0.125, split, cur_stream())))
+                                                     ptr(out), C, batch, heads, n, n, 0, 0.125, cur_stream())))
         fl = 4.0 * batch * heads * n * n * 64
-        print("attention b%d h%d n%d split%d: %.3f ms = %.0f TFLOP/s" % (batch, heads, n, split, ms, fl / ms / 1e9), flush=True)
+        print("attention b%d h%d n%d: %.3f ms = %.0f TFLOP/s" % (batch, heads, n, ms, fl / ms / 1e9), flush=True)
     # bandwidth kernels at the cfg-2 sizes (16 images per DPT pass, 32 images in the trunk)
     for (nimg, H, W, C) in [(16, 192, 256, 128), (16, 96, 128, 256), (16, 48, 64, 256)]:
         x = torch.randn(nimg, H, W, C, device=dev).bfloat16()

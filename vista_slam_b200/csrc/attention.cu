@@ -24,8 +24,6 @@
 #include <stdio.h>
 #include "ops.h"
 
-#include <stdlib.h>
-
 namespace sta {
 
 namespace {
@@ -43,7 +41,6 @@ constexpr uint32_t ATT_SMEM = ATT_OFF_BAR + 256;
 
 struct AttnParams {
   int nq, nk, batch, heads, qtiles, kv_batch_shift;
-  int q_row0;  // first query row handled by the tiled kernel (1 when row 0 goes to attention_row0_kernel)
   float scale_log2;
   __nv_bfloat16* out;
   long long ldo;
@@ -71,7 +68,7 @@ attention_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
   const int b = item / (p.qtiles * p.heads);
   const int kvb = (b + p.kv_batch_shift) % p.batch;
   constexpr int QROWS = 64 * CWG;
-  const int q0 = p.q_row0 + qt * QROWS;
+  const int q0 = qt * QROWS;
   const int nkt = (p.nk + 127) / 128;
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -206,116 +203,6 @@ attention_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
       if (row < p.nq) *reinterpret_cast<uint32_t*>(oa + 8 * c) = pack_bf16x2(o[4 * c] * inv0, o[4 * c + 1] * inv0);
       if (row + 8 < p.nq) *reinterpret_cast<uint32_t*>(ob + 8 * c) = pack_bf16x2(o[4 * c + 2] * inv1, o[4 * c + 3] * inv1);
     }
-  }
-}
-
-// ---------------------------------------------------------------------------
-// Query row 0 of every (sample, head) -- the decoder's pose token -- against all nk keys.
-// One CTA (256 threads) per (head, sample): scores -> shared memory, block max / sum, then P V with 16-byte
-// loads.  ~1e-4 of the attention FLOPs but latency-bound: the loads are batched so that the whole kernel is
-// about five DRAM round trips.
-// ---------------------------------------------------------------------------
-__global__ void __launch_bounds__(256, 3)
-attention_row0_kernel(const __nv_bfloat16* __restrict__ q, long long ldq, int q_col0, const __nv_bfloat16* __restrict__ k,
-                      long long ldk, int k_col0, const __nv_bfloat16* __restrict__ v, long long ldv, int v_col0,
-                      __nv_bfloat16* __restrict__ out, long long ldo, int nq, int nk, int batch, int kv_batch_shift,
-                      float scale_log2) {
-  extern __shared__ float sc[];  // nk scores | 16 floats of reduction scratch | 32 x 64 partial outputs
-  float* red = sc + ((nk + 3) & ~3);
-  __shared__ float qs[64];
-  pdl_wait();
-  pdl_launch_dependents();
-  // last samples first: their K / V rows are the most recent (still L2-resident) reads of the tiled kernel
-  const int head = blockIdx.x, b = static_cast<int>(gridDim.y) - 1 - static_cast<int>(blockIdx.y);
-  const int kvb = (b + kv_batch_shift) % batch;
-  const int tid = threadIdx.x;
-  if (tid < 64) qs[tid] = __bfloat162float(q[static_cast<long long>(b) * nq * ldq + q_col0 + head * 64 + tid]);
-  __syncthreads();
-  // ---- scores: two keys per thread per round (16 x 16-byte loads in flight; 769 keys = 2 DRAM round trips) ----
-  const __nv_bfloat16* kb = k + static_cast<long long>(kvb) * nk * ldk + k_col0 + head * 64;
-  float mx = -INFINITY;
-  for (int j0 = tid; j0 < nk; j0 += 512) {
-    const int j1 = j0 + 256;
-    const bool has1 = j1 < nk;
-    const uint4* kr0 = reinterpret_cast<const uint4*>(kb + static_cast<long long>(j0) * ldk);
-    const uint4* kr1 = reinterpret_cast<const uint4*>(kb + static_cast<long long>(has1 ? j1 : j0) * ldk);
-    uint4 w0[8], w1[8];
-#pragma unroll
-    for (int c = 0; c < 8; ++c) {
-      w0[c] = __ldg(kr0 + c);
-      w1[c] = __ldg(kr1 + c);
-    }
-    float a0 = 0.f, a1 = 0.f;
-#pragma unroll
-    for (int c = 0; c < 8; ++c) {
-      const float4 qa = *reinterpret_cast<const float4*>(qs + 8 * c);
-      const float4 qb = *reinterpret_cast<const float4*>(qs + 8 * c + 4);
-      a0 += qa.x * bf16_lo(w0[c].x) + qa.y * bf16_hi(w0[c].x) + qa.z * bf16_lo(w0[c].y) + qa.w * bf16_hi(w0[c].y) +
-            qb.x * bf16_lo(w0[c].z) + qb.y * bf16_hi(w0[c].z) + qb.z * bf16_lo(w0[c].w) + qb.w * bf16_hi(w0[c].w);
-      a1 += qa.x * bf16_lo(w1[c].x) + qa.y * bf16_hi(w1[c].x) + qa.z * bf16_lo(w1[c].y) + qa.w * bf16_hi(w1[c].y) +
-            qb.x * bf16_lo(w1[c].z) + qb.y * bf16_hi(w1[c].z) + qb.z * bf16_lo(w1[c].w) + qb.w * bf16_hi(w1[c].w);
-    }
-    a0 *= scale_log2;
-    sc[j0] = a0;
-    mx = fmaxf(mx, a0);
-    if (has1) {
-      a1 *= scale_log2;
-      sc[j1] = a1;
-      mx = fmaxf(mx, a1);
-    }
-  }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
-  if ((tid & 31) == 0) red[tid >> 5] = mx;
-  __syncthreads();
-  mx = red[0];
-#pragma unroll
-  for (int i = 1; i < 8; ++i) mx = fmaxf(mx, red[i]);
-  float sum = 0.f;
-  for (int j = tid; j < nk; j += 256) {
-    // P is rounded to bf16 like in the tiled kernel; the row sum uses the unrounded value
-    const float e = ex2_approx(sc[j] - mx);
-    sum += e;
-    sc[j] = __bfloat162float(__float2bfloat16(e));
-  }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
-  if ((tid & 31) == 0) red[8 + (tid >> 5)] = sum;
-  __syncthreads();
-  sum = 0.f;
-#pragma unroll
-  for (int i = 0; i < 8; ++i) sum += red[8 + i];
-  // ---- P V: thread (kg = tid / 8, fg = tid % 8) owns keys kg, kg + 32, ... and 8 features (one 16-byte load per
-  //      key, 13 in flight), then the 32 key groups are combined through shared memory ----
-  const int fg = tid & 7, kg = tid >> 3;
-  const __nv_bfloat16* vb = v + static_cast<long long>(kvb) * nk * ldv + v_col0 + head * 64 + 8 * fg;
-  float acc[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-  for (int j = kg; j < nk; j += 32 * 13) {
-    uint4 w[13];
-#pragma unroll
-    for (int u = 0; u < 13; ++u) {
-      const int jj = j + 32 * u;
-      w[u] = (jj < nk) ? __ldg(reinterpret_cast<const uint4*>(vb + static_cast<long long>(jj) * ldv)) : make_uint4(0u, 0u, 0u, 0u);
-    }
-#pragma unroll
-    for (int u = 0; u < 13; ++u) {
-      const int jj = j + 32 * u;
-      const float pj = (jj < nk) ? sc[jj] : 0.f;
-      acc[0] = fmaf(pj, bf16_lo(w[u].x), acc[0]); acc[1] = fmaf(pj, bf16_hi(w[u].x), acc[1]);
-      acc[2] = fmaf(pj, bf16_lo(w[u].y), acc[2]); acc[3] = fmaf(pj, bf16_hi(w[u].y), acc[3]);
-      acc[4] = fmaf(pj, bf16_lo(w[u].z), acc[4]); acc[5] = fmaf(pj, bf16_hi(w[u].z), acc[5]);
-      acc[6] = fmaf(pj, bf16_lo(w[u].w), acc[6]); acc[7] = fmaf(pj, bf16_hi(w[u].w), acc[7]);
-    }
-  }
-  float* part = red + 16;  // [32 key groups][64 features]
-#pragma unroll
-  for (int i = 0; i < 8; ++i) part[kg * 64 + 8 * fg + i] = acc[i];
-  __syncthreads();
-  if (tid < 64) {
-    float o = 0.f;
-#pragma unroll
-    for (int g = 0; g < 32; ++g) o += part[g * 64 + tid];
-    out[static_cast<long long>(b) * nq * ldo + head * 64 + tid] = __float2bfloat16(o / sum);
   }
 }
 
@@ -474,29 +361,15 @@ int launch_attention(const AttnLaunch& a, cudaStream_t stream) {
   p.scale_log2 = a.scale * 1.4426950408889634f;
   p.out = a.out;
   p.ldo = a.ldo;
-  const size_t row0_smem = (((a.nk + 3) & ~3) + 16 + 32 * 64) * sizeof(float);
-  const int split = (a.split_first_row && a.nq > 1 && row0_smem <= 48 * 1024) ? 1 : 0;
-  p.q_row0 = split;
   // Query tile: 128 rows (two consumer warpgroups share every K / V tile) unless that grid leaves SMs idle (small
   // problems: SLAM-mode keyframes, low resolutions), then 64 rows (one warpgroup) for twice the CTAs.
-  // STA_ATTN_QROWS=64|128 forces one of the two (A/B timing).
-  static int qrows_env = -1;
-  if (qrows_env < 0) {
-    const char* e = getenv("STA_ATTN_QROWS");
-    qrows_env = e ? atoi(e) : 0;
-  }
-  const long long items128 = static_cast<long long>((a.nq - split + 127) / 128) * a.heads * a.batch;
-  const int qrows = (qrows_env == 64 || qrows_env == 128) ? qrows_env : (items128 < num_sms() ? 64 : 128);
-  p.qtiles = (a.nq - split + qrows - 1) / qrows;
+  const long long items128 = static_cast<long long>((a.nq + 127) / 128) * a.heads * a.batch;
+  const int qrows = items128 < num_sms() ? 64 : 128;
+  p.qtiles = (a.nq + qrows - 1) / qrows;
   CUtensorMap tmQ, tmK, tmV;
   if (make_qkv_map(&tmQ, a.q, a.ldq, a.nq, a.batch, static_cast<uint32_t>(qrows))) return 1;
   if (make_qkv_map(&tmK, a.k, a.ldk, a.nk, a.batch)) return 1;
   if (make_qkv_map(&tmV, a.v, a.ldv, a.nk, a.batch)) return 1;
-  if (split) {
-    STA_CHECK_CUDA(launch_pdl(attention_row0_kernel, dim3(a.heads, a.batch), dim3(256), row0_smem, stream, 1, a.q, a.ldq, a.q_col0,
-                              a.k, a.ldk, a.k_col0, a.v, a.ldv, a.v_col0, a.out, a.ldo, a.nq, a.nk, a.batch, a.kv_batch_shift,
-                              p.scale_log2));
-  }
   const long long items = static_cast<long long>(p.qtiles) * a.heads * a.batch;
   STA_REQUIRE(items < (1LL << 31), "grid limits");
   return qrows == 64 ? launch_attention_inst<1>(tmQ, tmK, tmV, p, a, items, stream)

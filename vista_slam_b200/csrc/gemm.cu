@@ -3,8 +3,6 @@
 #include "host_util.h"
 #include "ops.h"
 
-#include <stdlib.h>
-
 namespace sta {
 
 // x[m][n] (+)= bias[n] + sum_ks partial[ks][m][n]  -- second pass of the split-K route (fixed summation order)
@@ -33,11 +31,11 @@ splitk_reduce_kernel(const float* __restrict__ partial, long long slice_elems, i
   }
 }
 
-template <int BN, int AMODE, int EPI, bool TMA>
+template <int AMODE, int EPI, bool TMA>
 static int launch_inst(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmC, const GemmParams& p,
                        int num_tiles, cudaStream_t stream) {
-  using Cfg = GemmCfg<BN, EPI, TMA, AMODE == A_CONV3H>;
-  auto kern = gemm_wg_kernel<BN, AMODE, EPI, TMA>;
+  using Cfg = GemmCfg<AMODE, EPI, TMA>;
+  auto kern = gemm_wg_kernel<AMODE, EPI, TMA>;
   static PerDeviceOnce once;  // the opt-in is per device, not per process
   STA_CHECK_CUDA(once.run(
       [&] { return cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg::SMEM_BYTES); }));
@@ -62,17 +60,9 @@ int launch_gemm(const GemmLaunch& g, cudaStream_t stream) {
 
   // TMA-store epilogue (epilogue_tile_tma) for the linear layers: bf16 / GELU / RoPE outputs without skip
   // tensors, fp32 outputs that either have no residual or accumulate in place (out += ..., bulk reduce-add).
-  static int tma_mode = -1, small_mode = -1, halo_mode = -1;
-  if (tma_mode < 0) {
-    const char* eh = getenv("STA_CONV_HALO");  // 0: one TMA box per filter tap (A_CONV3) instead of the halo-staged tile (A/B)
-    halo_mode = (eh && eh[0] == '0') ? 0 : 1;
-    const char* e = getenv("STA_GEMM_TMA_EPI");  // 0 disables (A/B timing and debugging)
-    tma_mode = (e && e[0] == '0') ? 0 : 1;
-    e = getenv("STA_GEMM_SMALL");  // 0 disables the split-K small-problem route (A/B timing)
-    small_mode = (e && e[0] == '0') ? 0 : 1;
-  }
+  // GELU and RoPE have no other epilogue.
   const int esz = (g.epi == EPI_F32) ? 4 : 2;
-  bool tma = tma_mode == 1 && p.N % bn == 0 && g.amode == A_LINEAR && p.out != nullptr && p.out2 == nullptr &&
+  bool tma = p.N % bn == 0 && g.amode == A_LINEAR && p.out != nullptr && p.out2 == nullptr &&
              (reinterpret_cast<uintptr_t>(p.out) & 15) == 0 && (p.ldo * esz) % 16 == 0;
   p.c_reduce = 0;
   if (g.epi == EPI_BF16) {
@@ -80,7 +70,10 @@ int launch_gemm(const GemmLaunch& g, cudaStream_t stream) {
   } else if (g.epi == EPI_F32) {
     tma = tma && p.rowmap_n == 0 && (p.resid == nullptr || p.resid == p.out);
     p.c_reduce = (p.resid != nullptr) ? 1 : 0;
-  } else if (g.epi != EPI_GELU && g.epi != EPI_ROPE) {
+  } else if (g.epi == EPI_GELU || g.epi == EPI_ROPE) {
+    STA_REQUIRE(tma, "GELU / RoPE epilogues need a linear layer with N % 128 == 0, a 16-byte aligned output and row "
+                     "stride, and no out2");
+  } else {
     tma = false;
   }
 
@@ -89,7 +82,7 @@ int launch_gemm(const GemmLaunch& g, cudaStream_t stream) {
   // stores its partial tile to scratch and a second tiny kernel sums them in a fixed order (deterministic, unlike
   // reduce-adds racing).
   int ksplit = 1;
-  if (small_mode && tma && g.epi == EPI_F32 && g.splitk_ws != nullptr) {
+  if (tma && g.epi == EPI_F32 && g.splitk_ws != nullptr) {
     const int tiles = ((p.M + 127) / 128) * (p.N / bn), nkb = (p.K + 63) / 64;
     if (tiles < num_sms()) {
       int ks = num_sms() / tiles;
@@ -99,20 +92,19 @@ int launch_gemm(const GemmLaunch& g, cudaStream_t stream) {
       if (ks >= 2 && need <= g.splitk_ws_bytes && (reinterpret_cast<uintptr_t>(g.splitk_ws) & 15) == 0) ksplit = ks;
     }
   }
-  const int amode = (g.amode == A_CONV3 && halo_mode) ? A_CONV3H : g.amode;
   CUtensorMap tmA, tmB;
   int m_tiles;
   if (g.amode == A_CONV3) {
     STA_REQUIRE(p.Cin % 64 == 0, "conv input channels must be a multiple of 64");
     STA_REQUIRE(p.K == 9 * p.Cin, "conv K must be 9*Cin");
-    const bool halo = amode == A_CONV3H;  // 16 x 8-pixel tiles fed from one 18 x 10-pixel box per channel chunk
-    p.tiles_h = halo ? (p.H + 15) / 16 : (p.H + 7) / 8;
-    p.tiles_w = halo ? (p.W + 7) / 8 : (p.W + 15) / 16;
+    // 16 x 8-pixel tiles fed from one 18 x 10-pixel box per channel chunk
+    p.tiles_h = (p.H + 15) / 16;
+    p.tiles_w = (p.W + 7) / 8;
     p.M = p.nimg * p.H * p.W;
     m_tiles = p.nimg * p.tiles_h * p.tiles_w;
     uint64_t dims[4] = {(uint64_t)p.Cin, (uint64_t)p.W, (uint64_t)p.H, (uint64_t)p.nimg};
     uint64_t strides[3] = {(uint64_t)p.Cin * 2, (uint64_t)p.W * p.Cin * 2, (uint64_t)p.H * p.W * p.Cin * 2};
-    uint32_t box[4] = {64, halo ? (uint32_t)kHaloPitch : 16u, halo ? 18u : 8u, 1};
+    uint32_t box[4] = {64, (uint32_t)kHaloPitch, 18u, 1};
     if (make_tmap_bf16(&tmA, g.A, 4, dims, strides, box)) return 1;
   } else {
     STA_REQUIRE(g.lda % 8 == 0, "lda must be a multiple of 8 elements (16 bytes)");
@@ -160,21 +152,17 @@ int launch_gemm(const GemmLaunch& g, cudaStream_t stream) {
 
   int rc = -1;
 #define STA_GEMM_CASE(AM_, EP_, TMA_) \
-  if (rc < 0 && amode == AM_ && g.epi == EP_ && tma == TMA_) rc = launch_inst<128, AM_, EP_, TMA_>(tmA, tmB, tmC, p, num_tiles, stream);
+  if (rc < 0 && g.amode == AM_ && g.epi == EP_ && tma == TMA_) rc = launch_inst<AM_, EP_, TMA_>(tmA, tmB, tmC, p, num_tiles, stream);
 
   STA_GEMM_CASE(A_LINEAR, EPI_GELU, true)
   STA_GEMM_CASE(A_LINEAR, EPI_F32, true)
   STA_GEMM_CASE(A_LINEAR, EPI_ROPE, true)
   STA_GEMM_CASE(A_LINEAR, EPI_BF16, true)
   STA_GEMM_CASE(A_LINEAR, EPI_BF16, false)
-  STA_GEMM_CASE(A_LINEAR, EPI_GELU, false)
   STA_GEMM_CASE(A_LINEAR, EPI_F32, false)
-  STA_GEMM_CASE(A_LINEAR, EPI_ROPE, false)
   STA_GEMM_CASE(A_LINEAR, EPI_PIXSHUF, false)
   STA_GEMM_CASE(A_CONV3, EPI_BF16, false)
   STA_GEMM_CASE(A_CONV3, EPI_HEAD, false)
-  STA_GEMM_CASE(A_CONV3H, EPI_BF16, false)
-  STA_GEMM_CASE(A_CONV3H, EPI_HEAD, false)
 #undef STA_GEMM_CASE
   if (rc == 0 && ksplit > 1) {
     const long long total = static_cast<long long>(p.M) * (p.N / 4);

@@ -7,8 +7,8 @@
 // the producer keeps a STAGES-deep operand ring filled; the finished accumulators are written to a padded fp32 tile
 // in shared memory, from which the same eight warps run the fused epilogue (-> global).  The producer prefetches
 // the next tile's operands during the epilogue.  Operand tiles are 128B-swizzled K-major [rows][64] boxes written
-// by TMA; the 3x3 convolution uses a 4-D NHWC tensor map and shifts the box per filter tap (out-of-bounds = zero
-// padding), so no im2col buffer exists.
+// by TMA; the 3x3 convolution loads one halo tile per channel chunk through a 4-D NHWC tensor map (out-of-bounds =
+// zero padding) and feeds every filter tap from shifted views of it, so no im2col buffer exists.
 //
 // Reference ops covered (vista_slam/sta_model): nn.Linear in blocks/sta_blocks.py:67-70,
 // 88-90,179-183; PatchEmbed conv sta_blocks.py:262 (after im2col); the DPT convs of
@@ -18,13 +18,11 @@
 
 namespace sta {
 
-// A_CONV3:  3x3 convolution, one TMA box (8 x 16 pixels x 64 channels, shifted by the tap) per filter tap and channel chunk.
-// A_CONV3H: 3x3 convolution, halo-staged: ONE box of 18 x 16 pixels x 64 channels per channel chunk feeds all nine taps --
-//           a tap is a row-shifted view of the staged tile (tile 16 rows x 8 pixels, 8-row descriptor groups 2048 bytes
-//           apart, descriptor base offset = the tap's column shift).  Shared-memory write traffic of the A operand drops from
-//           9 x 16 KB to 36 KB per channel chunk; the N = 128 head convolutions were bound by exactly that traffic.
-enum AMode : int { A_LINEAR = 0, A_CONV3 = 1, A_CONV3H = 2 };
-__host__ __device__ constexpr bool is_conv(int amode) { return amode != A_LINEAR; }
+// A_CONV3: 3x3 convolution, halo-staged: ONE box of 18 x 10 pixels x 64 channels per channel chunk feeds all nine taps --
+//          a tap is a row-shifted view of the staged tile (tile 16 rows x 8 pixels, descriptor base offset = the tap's
+//          shift).  Shared-memory write traffic of the A operand is 22.5 KB per channel chunk instead of 9 x 16 KB with one
+//          box per tap; the N = 128 head convolutions are bound by exactly that traffic.
+enum AMode : int { A_LINEAR = 0, A_CONV3 = 1 };
 enum Epi : int {
   EPI_BF16 = 0,     // out_bf16 = [relu](acc + bias [+ resid_bf16] [+ resid2_bf16]); optional relu copy in out2
   EPI_GELU = 1,     // out_bf16 = gelu_erf(acc + bias)
@@ -73,15 +71,16 @@ struct GemmParams {
 
 // TMA = true: the epilogue writes through shared memory + TMA tensor stores (epilogue_tile_tma), else the
 // coalesced per-warp path (epilogue_tile).
-// A_CONV3H: pixels per staged halo row.  10 = the 8-pixel tile plus its two halo columns (dense box, 8-row descriptor groups
+// A_CONV3: pixels per staged halo row.  10 = the 8-pixel tile plus its two halo columns (dense box, 8-row descriptor groups
 // 1280 B apart -- groups then start at any 128-byte multiple, which the absolute-address swizzle permits).
 constexpr int kHaloPitch = 10;
 constexpr int kRopeLd = 36;  // floats per staged sin/cos table row (32 + 4 pad: conflict-free row-per-lane reads)
-template <int BN, int EPI, bool TMA, bool HALO = false>
+template <int AMODE, int EPI, bool TMA>
 struct GemmCfg {
+  static constexpr bool CONV = (AMODE == A_CONV3);
   static constexpr int BM = 128;
+  static constexpr int BN = 128;  // one consumer warpgroup covers the 128 columns of a tile (wgmma m64n128k16)
   static constexpr int BK = 64;
-  static_assert(BN == 128, "one consumer warpgroup covers the 128 columns of a tile (wgmma m64n128k16)");
   static constexpr uint32_t A_BYTES = BM * BK * 2;
   static constexpr uint32_t B_BYTES = BN * BK * 2;
   static constexpr uint32_t BAR_BYTES = 256;
@@ -97,12 +96,12 @@ struct GemmCfg {
   static constexpr int ROPE_SMEM_ROWS = 64;  // positions -1 .. 62
   static constexpr uint32_t ROPE_SMEM_BYTES = (EPI == EPI_ROPE) ? ROPE_SMEM_ROWS * kRopeLd * sizeof(float) : 0;
   static constexpr uint32_t MAX_SMEM = 227 * 1024;
-  // halo-staged convolution (A_CONV3H): the ring holds B tiles only; three 18 x 10 x 64-channel input tiles besides it
+  // convolution: the ring holds B tiles only; three 18 x 10 x 64-channel halo input tiles besides it
   static constexpr uint32_t HALO_TX_BYTES = 18 * kHaloPitch * 128;                 // bytes one box delivers
   static constexpr uint32_t HALO_BYTES = (HALO_TX_BYTES + 1023u) & ~1023u;        // stage stride (swizzle-pattern aligned)
   static constexpr int HALO_STAGES = 3;
-  static constexpr uint32_t HALO_TOTAL = HALO ? HALO_STAGES * HALO_BYTES : 0;
-  static constexpr uint32_t STAGE_BYTES = HALO ? B_BYTES : A_BYTES + B_BYTES;
+  static constexpr uint32_t HALO_TOTAL = CONV ? HALO_STAGES * HALO_BYTES : 0;
+  static constexpr uint32_t STAGE_BYTES = CONV ? B_BYTES : A_BYTES + B_BYTES;
   static constexpr int STAGES_FIT =
       (MAX_SMEM - BAR_BYTES - EPI_SMEM_BYTES - STG_BYTES - ACC_BYTES - ROPE_SMEM_BYTES - HALO_TOTAL) / STAGE_BYTES;
   static constexpr int STAGES = STAGES_FIT > 8 ? 8 : STAGES_FIT;
@@ -141,17 +140,7 @@ __device__ __forceinline__ void acc_ld32(const float* src, uint32_t (&r)[32]) {
 
 template <int AMODE>
 __device__ __forceinline__ void tile_row(const GemmParams& p, int m_tile, int r_local, long long& orow, bool& valid) {
-  if constexpr (AMODE == A_CONV3) {
-    const int tpi = p.tiles_h * p.tiles_w;
-    const int n = m_tile / tpi;
-    const int t = m_tile - n * tpi;
-    const int th = t / p.tiles_w;
-    const int tw = t - th * p.tiles_w;
-    const int h = th * 8 + (r_local >> 4);
-    const int w = tw * 16 + (r_local & 15);
-    valid = (h < p.H) && (w < p.W) && (n < p.nimg);
-    orow = (static_cast<long long>(n) * p.H + h) * p.W + w;
-  } else if constexpr (AMODE == A_CONV3H) {  // 16 rows x 8 pixels per 128-row tile
+  if constexpr (AMODE == A_CONV3) {  // 16 rows x 8 pixels per 128-row tile
     const int tpi = p.tiles_h * p.tiles_w;
     const int n = m_tile / tpi;
     const int t = m_tile - n * tpi;
@@ -185,11 +174,13 @@ __device__ __forceinline__ void store4_bf16(__nv_bfloat16* p, const float4& v, i
 }
 
 // accs: the accumulator tile at this warp's first row (32 * quarter) and first column (part * BN / PARTS)
-template <int BN, int AMODE, int EPI, int EW>
+template <int AMODE, int EPI>
 __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const float* accs, int m_tile, int n_tile,
-                                              int quarter, int part, float* epi_smem, const float* rope_s) {
-  constexpr int PARTS = EW / 4;
-  constexpr int LD = BN + 4;  // accumulator tile row stride (floats)
+                                              int quarter, int part, float* epi_smem) {
+  using Cfg = GemmCfg<AMODE, EPI, false>;
+  constexpr int BN = Cfg::BN;
+  constexpr int PARTS = Cfg::PARTS;
+  constexpr int LD = Cfg::ACC_LD;  // accumulator tile row stride (floats)
   constexpr int CH = BN / PARTS;  // columns per epilogue warp
   const int lane = threadIdx.x & 31;
   const int colbase = n_tile * BN + part * CH;
@@ -198,7 +189,6 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const float* 
     // head.2 epilogue: ReLU -> head.4 (1x1, 128 -> 4) -> postprocess (dpt_block.py:319-323,
     // postprocess.py:10-62).  Row mapping: each thread owns 32 of the 128 channels of one pixel; the four
     // column parts are combined through shared memory.  Nothing but 16 bytes per pixel is written.
-    static_assert(BN == 128, "EPI_HEAD expects the 128-channel head");
     const int r_local = quarter * 32 + lane;
     long long orow;
     bool valid;
@@ -222,7 +212,7 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const float* 
     }
     if (part != 0)
       reinterpret_cast<float4*>(epi_smem)[(part - 1) * 128 + r_local] = make_float4(psum[0], psum[1], psum[2], psum[3]);
-    named_bar_sync(1, 32 * EW);
+    named_bar_sync(1, Cfg::EPI_THREADS);
     if (part == 0) {
       float4 o = reinterpret_cast<float4*>(epi_smem)[r_local];
 #pragma unroll
@@ -244,7 +234,7 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const float* 
         p.conf[orow] = 1.0f + expf(cf);
       }
     }
-    named_bar_sync(1, 32 * EW);
+    named_bar_sync(1, Cfg::EPI_THREADS);
     return;
   } else {
     // ---- coalesced mapping bookkeeping: this lane touches rows 4*it + (lane>>3), it = 0..7 ----
@@ -271,24 +261,6 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const float* 
         const int h = rem / p.ps_w;
         const int w = rem - h * p.ps_w;
         orow_c[it] = (static_cast<long long>(n) * p.ps_h + h) * p.ps_k * (p.ps_w * p.ps_k) + w * p.ps_k;
-      }
-    }
-
-    // EPI_ROPE: (y, x) token positions of this lane's 8 rows
-    [[maybe_unused]] int pos_y[8], pos_x[8];
-    if constexpr (EPI == EPI_ROPE) {
-#pragma unroll
-      for (int it = 0; it < 8; ++it) {
-        int py = 0, px = 0;
-        if ((vmask >> it) & 1u) {
-          const int2 pp = *reinterpret_cast<const int2*>(p.pos + 2 * orow_c[it]);
-          py = pp.x;
-          px = pp.y;
-          if (py < -1 || py > p.rope_max_pos || px < -1 || px > p.rope_max_pos)
-            __trap();  // token position outside the RoPE table (no printf: see mbar_wait)
-        }
-        pos_y[it] = py;
-        pos_x[it] = px;
       }
     }
 
@@ -357,31 +329,6 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const float* 
           const bool ok = (vmask >> it) & 1u;
           float4 v = *reinterpret_cast<const float4*>(stg + (it * 4 + crow) * LD + cc);
           v.x += b4.x; v.y += b4.y; v.z += b4.z; v.w += b4.w;
-          if constexpr (EPI == EPI_ROPE) {
-            // 2-D RoPE (pos_embed/pos_embed.py:149-185, curope/kernels.cu:17-82).  A 32-column chunk is exactly
-            // one half of a 64-wide head: the y-half (rotated by pos_y) or the x-half (pos_x).  Inside a half the
-            // pairs are (i, i+16): the partner columns live in lane ^ 4 of the same row group.
-            if (col < p.rope_cols) {  // uniform per chunk: the V columns are not rotated
-              const float4 w = make_float4(__shfl_xor_sync(0xffffffffu, v.x, 4), __shfl_xor_sync(0xffffffffu, v.y, 4),
-                                           __shfl_xor_sync(0xffffffffu, v.z, 4), __shfl_xor_sync(0xffffffffu, v.w, 4));
-              const int pz = ((col >> 5) & 1) ? pos_x[it] : pos_y[it];
-              const int ps = min(pz + 1, p.rope_smem_rows - 1);  // clamped shared-memory row (always safe to read)
-              const float4* tb = reinterpret_cast<const float4*>(rope_s + ps * kRopeLd) + ((cc & 15) >> 1);
-              float4 t0 = tb[0];  // (cos f, sin f, cos f+1, sin f+1)
-              float4 t1 = tb[1];  // (cos f+2, sin f+2, cos f+3, sin f+3)
-              if (pz + 1 >= p.rope_smem_rows) {  // beyond the staged rows (very large images): global table
-                const float4* tg =
-                    reinterpret_cast<const float4*>(p.rope_tab + static_cast<long long>(pz + 1) * 32) + ((cc & 15) >> 1);
-                t0 = __ldg(tg);
-                t1 = __ldg(tg + 1);
-              }
-              const float sg = (cc & 16) ? 1.0f : -1.0f;  // lower 16: u*cos - w*sin ; upper 16: u*cos + w*sin
-              v.x = fmaf(sg * w.x, t0.y, v.x * t0.x);
-              v.y = fmaf(sg * w.y, t0.w, v.y * t0.z);
-              v.z = fmaf(sg * w.z, t1.y, v.z * t1.x);
-              v.w = fmaf(sg * w.w, t1.w, v.w * t1.z);
-            }
-          }
           if constexpr (EPI == EPI_F32) {
             float* op = reinterpret_cast<float*>(p.out) + orow_c[it] * p.ldo + col + cc;
             if (p.resid) { v.x += rf[k].x; v.y += rf[k].y; v.z += rf[k].z; v.w += rf[k].w; }
@@ -390,28 +337,23 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const float* 
             __nv_bfloat16* op = reinterpret_cast<__nv_bfloat16*>(p.out) +
                                 (orow_c[it] + pix_off) * (p.split ? 3 * p.ps_cout : p.ps_cout) + co + cc;
             if (ok) store4_bf16(op, v, p.split, p.ps_cout);
-          } else {
+          } else {  // EPI_BF16
             const long long off = orow_c[it] * p.ldo + col + cc;
-            if constexpr (EPI == EPI_BF16) {
-              if (p.resid) {
-                add_bf16x4(v, ra[k]);
-                if (p.split && ok)  // residual (lo) part of the skip tensor
-                  add_bf16x4(v, *reinterpret_cast<const uint2*>(reinterpret_cast<const __nv_bfloat16*>(p.resid) + off + p.N));
-              }
-              if (p.resid2) {
-                add_bf16x4(v, rb[k]);
-                if (p.split && ok)
-                  add_bf16x4(v, *reinterpret_cast<const uint2*>(reinterpret_cast<const __nv_bfloat16*>(p.resid2) + off + p.N));
-              }
-              if (p.relu_main) { v.x = fmaxf(v.x, 0.f); v.y = fmaxf(v.y, 0.f); v.z = fmaxf(v.z, 0.f); v.w = fmaxf(v.w, 0.f); }
+            if (p.resid) {
+              add_bf16x4(v, ra[k]);
+              if (p.split && ok)  // residual (lo) part of the skip tensor
+                add_bf16x4(v, *reinterpret_cast<const uint2*>(reinterpret_cast<const __nv_bfloat16*>(p.resid) + off + p.N));
             }
-            if constexpr (EPI == EPI_GELU) { v.x = gelu_erf(v.x); v.y = gelu_erf(v.y); v.z = gelu_erf(v.z); v.w = gelu_erf(v.w); }
+            if (p.resid2) {
+              add_bf16x4(v, rb[k]);
+              if (p.split && ok)
+                add_bf16x4(v, *reinterpret_cast<const uint2*>(reinterpret_cast<const __nv_bfloat16*>(p.resid2) + off + p.N));
+            }
+            if (p.relu_main) { v.x = fmaxf(v.x, 0.f); v.y = fmaxf(v.y, 0.f); v.z = fmaxf(v.z, 0.f); v.w = fmaxf(v.w, 0.f); }
             if (p.out && ok) store4_bf16(reinterpret_cast<__nv_bfloat16*>(p.out) + off, v, p.split, p.N);
-            if constexpr (EPI == EPI_BF16) {
-              if (p.out2 && ok) {
-                v.x = fmaxf(v.x, 0.f); v.y = fmaxf(v.y, 0.f); v.z = fmaxf(v.z, 0.f); v.w = fmaxf(v.w, 0.f);
-                store4_bf16(reinterpret_cast<__nv_bfloat16*>(p.out2) + off, v, p.split, p.N);
-              }
+            if (p.out2 && ok) {
+              v.x = fmaxf(v.x, 0.f); v.y = fmaxf(v.y, 0.f); v.z = fmaxf(v.z, 0.f); v.w = fmaxf(v.w, 0.f);
+              store4_bf16(reinterpret_cast<__nv_bfloat16*>(p.out2) + off, v, p.split, p.N);
             }
           }
         }
@@ -458,12 +400,12 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const float* 
 // performed by the L2, so the epilogue never loads the residual.
 // accrow: this thread's accumulator row at the warp's first column.
 // ---------------------------------------------------------------------------
-template <int BN, int EPI, int EW>
+template <int EPI>
 __device__ __forceinline__ void epilogue_tile_tma(const GemmParams& p, const CUtensorMap* tmC, const float* accrow, int m_tile,
                                                   int colbase, int row_off, int quarter, uint8_t* cbuf,
                                                   const float* rope_s) {
-  constexpr int PARTS = EW / 4;
-  constexpr int CH = BN / PARTS;  // columns per epilogue warp
+  using Cfg = GemmCfg<A_LINEAR, EPI, true>;
+  constexpr int CH = Cfg::BN / Cfg::PARTS;  // columns per epilogue warp
   constexpr int NCH = CH / 32;    // 32-column chunks
   constexpr bool OUT_F32 = (EPI == EPI_F32);
   const int lane = threadIdx.x & 31;
@@ -589,27 +531,30 @@ __device__ __forceinline__ void epilogue_tile_tma(const GemmParams& p, const CUt
   }  // pass
 }
 
-template <int BN, int AMODE, int EPI, bool TMA>
-__global__ void __launch_bounds__(GemmCfg<BN, EPI, TMA>::THREADS, 1)
+template <int AMODE, int EPI, bool TMA>
+__global__ void __launch_bounds__(GemmCfg<AMODE, EPI, TMA>::THREADS, 1)
 gemm_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                const __grid_constant__ CUtensorMap tmC, const GemmParams p) {
-  constexpr bool HALO = (AMODE == A_CONV3H);
-  using Cfg = GemmCfg<BN, EPI, TMA, HALO>;
+  using Cfg = GemmCfg<AMODE, EPI, TMA>;
+  constexpr bool CONV = Cfg::CONV;
   static_assert(!TMA || (AMODE == A_LINEAR && (EPI == EPI_BF16 || EPI == EPI_GELU || EPI == EPI_F32 || EPI == EPI_ROPE)),
                 "TMA-store epilogue: linear layers only");
+  static_assert(TMA || EPI == EPI_BF16 || EPI == EPI_F32 || EPI == EPI_PIXSHUF || EPI == EPI_HEAD,
+                "GELU and RoPE have the TMA-store epilogue only");
+  constexpr int BN = Cfg::BN;
   constexpr int STAGES = Cfg::STAGES;
   constexpr uint32_t A_BYTES = Cfg::A_BYTES;
   constexpr uint32_t B_BYTES = Cfg::B_BYTES;
   constexpr int EW = Cfg::EPI_WARPS;
 
   extern __shared__ __align__(1024) uint8_t smem[];
-  uint8_t* sA = smem;
-  uint8_t* sB = smem + (HALO ? 0u : STAGES * A_BYTES);
+  [[maybe_unused]] uint8_t* sA = smem;
+  uint8_t* sB = smem + (CONV ? 0u : STAGES * A_BYTES);
   [[maybe_unused]] uint8_t* sH = smem + Cfg::OFF_HALO;
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Cfg::OFF_BAR);
   uint64_t* full = bars;
   uint64_t* empty = bars + STAGES;
-  [[maybe_unused]] uint64_t* hfull = bars + 2 * STAGES;  // halo tiles (A_CONV3H)
+  [[maybe_unused]] uint64_t* hfull = bars + 2 * STAGES;  // halo tiles (A_CONV3)
   [[maybe_unused]] uint64_t* hempty = hfull + Cfg::HALO_STAGES;
   static_assert((2 * STAGES + 2 * Cfg::HALO_STAGES) * 8 <= Cfg::BAR_BYTES, "barrier area");
   [[maybe_unused]] float* epi_smem = reinterpret_cast<float*>(smem + Cfg::OFF_EPI);
@@ -620,12 +565,12 @@ gemm_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
 
-  const int m_tiles = is_conv(AMODE) ? p.nimg * p.tiles_h * p.tiles_w : (p.M + 127) / 128;
+  const int m_tiles = CONV ? p.nimg * p.tiles_h * p.tiles_w : (p.M + 127) / 128;
   const int n_tiles = (p.N + BN - 1) / BN;
   const int ksplit = TMA ? p.ksplit : 1;
   const int num_tiles = m_tiles * n_tiles * ksplit;  // work items (m, n, ks), ks fastest
-  const int cpb = is_conv(AMODE) ? (p.Cin / 64) : 1;  // 64-channel chunks per filter tap
-  const int nkb = is_conv(AMODE) ? 9 * cpb : (p.K + 63) / 64;
+  const int cpb = CONV ? (p.Cin / 64) : 1;  // 64-channel chunks per filter tap
+  const int nkb = CONV ? 9 * cpb : (p.K + 63) / 64;
 
   if (threadIdx.x == 0) {
     if ((smem_u32(smem) & 1023u) != 0) device_fatal("dynamic shared memory is not 1024-byte aligned");
@@ -633,7 +578,7 @@ gemm_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       mbar_init(&full[s], 1);    // the producer's expect_tx arrival
       mbar_init(&empty[s], EW);  // one arrival per consumer warp
     }
-    if constexpr (HALO) {
+    if constexpr (CONV) {
       for (int s = 0; s < Cfg::HALO_STAGES; ++s) {
         mbar_init(&hfull[s], 1);
         mbar_init(&hempty[s], EW);
@@ -673,16 +618,13 @@ gemm_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         const int n_tile = mn % n_tiles;
         const int kb0 = ks * nkb / ksplit, kb1 = (ks + 1) * nkb / ksplit;
         const int b_row0 = n_tile * BN;
-        int cn = 0, ch0 = 0, cw0 = 0;
-        if constexpr (is_conv(AMODE)) {
+        if constexpr (CONV) {
           const int tpi = p.tiles_h * p.tiles_w;
-          cn = m_tile / tpi;
+          const int cn = m_tile / tpi;
           const int t = m_tile - cn * tpi;
           const int th = t / p.tiles_w;
-          ch0 = th * (HALO ? 16 : 8);
-          cw0 = (t - th * p.tiles_w) * (HALO ? 8 : 16);
-        }
-        if constexpr (HALO) {
+          const int ch0 = th * 16;
+          const int cw0 = (t - th * p.tiles_w) * 8;
           // channel chunk outermost: one halo tile, then the nine taps' weight tiles
           for (int cc = 0; cc < cpb; ++cc) {
             mbar_wait(&hempty[hstage], hphase ^ 1);
@@ -700,15 +642,7 @@ gemm_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
           for (int kb = kb0; kb < kb1; ++kb) {
             mbar_wait(&empty[stage], phase ^ 1);
             mbar_arrive_expect_tx(&full[stage], A_BYTES + B_BYTES);
-            if constexpr (AMODE == A_CONV3) {
-              const int tap = kb / cpb;
-              const int cc = kb - tap * cpb;
-              const int kh = tap / 3;
-              const int kw = tap - kh * 3;
-              tma_load_4d(sA + stage * A_BYTES, &tmA, &full[stage], cc * 64, cw0 + kw - 1, ch0 + kh - 1, cn);
-            } else {
-              tma_load_2d(sA + stage * A_BYTES, &tmA, &full[stage], kb * 64, m_tile * 128);
-            }
+            tma_load_2d(sA + stage * A_BYTES, &tmA, &full[stage], kb * 64, m_tile * 128);
             tma_load_2d(sB + stage * B_BYTES, &tmB, &full[stage], kb * 64, b_row0);
             if (++stage == STAGES) { stage = 0; phase ^= 1; }
           }
@@ -747,7 +681,7 @@ gemm_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         prev = stage;
         if (++stage == STAGES) { stage = 0; phase ^= 1; }
       };
-      if constexpr (HALO) {
+      if constexpr (CONV) {
         for (int cc = 0; cc < cpb; ++cc) {
           mbar_wait(&hfull[hstage], hphase);
           // output pixel (y, x) of the 16 x 8 tile reads halo pixel (y + kh, x + kw); halo rows are kHaloPitch pixels,
@@ -789,12 +723,12 @@ gemm_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       named_bar_sync(1, Cfg::EPI_THREADS);
       const int cols_w = BN / Cfg::PARTS;
       if constexpr (TMA) {
-        epilogue_tile_tma<BN, EPI, EW>(p, &tmC, acc_s + (quarter * 32 + lane) * Cfg::ACC_LD + part * cols_w, m_tile,
-                                       n_tile * BN + part * cols_w, ks * p.split_rows, quarter,
-                                       stg_all + (warp - 4) * Cfg::STG_WARP_BYTES, rope_s);
+        epilogue_tile_tma<EPI>(p, &tmC, acc_s + (quarter * 32 + lane) * Cfg::ACC_LD + part * cols_w, m_tile,
+                               n_tile * BN + part * cols_w, ks * p.split_rows, quarter,
+                               stg_all + (warp - 4) * Cfg::STG_WARP_BYTES, rope_s);
       } else {
-        epilogue_tile<BN, AMODE, EPI, EW>(p, acc_s + quarter * 32 * Cfg::ACC_LD + part * cols_w, m_tile, n_tile, quarter,
-                                          part, epi_smem, rope_s);
+        epilogue_tile<AMODE, EPI>(p, acc_s + quarter * 32 * Cfg::ACC_LD + part * cols_w, m_tile, n_tile, quarter, part,
+                                  epi_smem);
       }
     }
     if constexpr (TMA) {

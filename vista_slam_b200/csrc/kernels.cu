@@ -26,15 +26,15 @@ template <int C>
 __global__ void __launch_bounds__(256)
 layernorm_kernel(const float* __restrict__ x, int rows, float eps, const float* __restrict__ g1,
                  const float* __restrict__ b1, __nv_bfloat16* __restrict__ out1, const float* __restrict__ g2,
-                 const float* __restrict__ b2, __nv_bfloat16* __restrict__ out2, int drop_first_of, int split, int reverse) {
+                 const float* __restrict__ b2, __nv_bfloat16* __restrict__ out2, int drop_first_of, int split) {
   pdl_wait();
   pdl_launch_dependents();
   constexpr int V = C / 128;  // float4 per lane
   const long long ldo = split ? 3 * C : C;  // split-precision mode: rows are (hi | lo | hi)
-  // Blocks are scheduled in increasing blockIdx; `reverse` makes them walk the rows from the END: the residual GEMM that
-  // produced x wrote its rows in increasing order, so its last rows are the ones still resident in the 126 MB L2, and the
-  // consumer GEMM (increasing rows) then finds this kernel's most recent outputs -- the first rows -- in L2 as well.
-  const int blk = reverse ? static_cast<int>(gridDim.x) - 1 - static_cast<int>(blockIdx.x) : static_cast<int>(blockIdx.x);
+  // Blocks are scheduled in increasing blockIdx and walk the rows from the END: the residual GEMM that produced x wrote
+  // its rows in increasing order, so its last rows are the ones still resident in L2, and the consumer GEMM (increasing
+  // rows) then finds this kernel's most recent outputs -- the first rows -- in L2 as well.
+  const int blk = static_cast<int>(gridDim.x) - 1 - static_cast<int>(blockIdx.x);
   const int row = blk * 8 + (threadIdx.x >> 5);
   const int lane = threadIdx.x & 31;
   if (row >= rows) return;
@@ -103,17 +103,12 @@ int launch_layernorm(const float* x, int rows, int C, float eps, const float* g1
                      const float* g2, const float* b2, bf16* out2, int drop_first_of, cudaStream_t stream, int split) {
   if (rows <= 0) return 0;
   const int grid = (rows + 7) / 8;
-  static int reverse = -1;
-  if (reverse < 0) {
-    const char* e = getenv("STA_LN_REVERSE");  // 0 disables (A/B timing)
-    reverse = (e && e[0] == '0') ? 0 : 1;
-  }
   if (C == 1024)
     STA_CHECK_CUDA(launch_pdl(layernorm_kernel<1024>, dim3(grid), dim3(256), 0, stream, 1, x, rows, eps, g1, b1, out1, g2, b2, out2,
-                              drop_first_of, split, reverse));
+                              drop_first_of, split));
   else if (C == 768)
     STA_CHECK_CUDA(launch_pdl(layernorm_kernel<768>, dim3(grid), dim3(256), 0, stream, 1, x, rows, eps, g1, b1, out1, g2, b2, out2,
-                              drop_first_of, split, reverse));
+                              drop_first_of, split));
   else {
     set_last_error("layernorm: C must be 768 or 1024");
     return 2;

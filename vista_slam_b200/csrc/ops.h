@@ -1,5 +1,5 @@
-// Internal C++ launch API shared by the runtime (runtime.cu) and the op-level
-// C-ABI test entry points (capi.cu).  All functions return 0 on success and set
+// Internal C++ launch API shared by the model runtime and the op-level C-ABI
+// test entry points (both in runtime.cu).  All functions return 0 on success and set
 // sta::get_last_error() otherwise; all work is enqueued on `stream`.
 #pragma once
 #include <cuda_runtime.h>
@@ -39,10 +39,6 @@ struct AttnLaunch {
   int batch = 0, heads = 0, nq = 0, nk = 0;
   int kv_batch_shift = 0;   // k/v sample for query sample b is (b + shift) % batch  (cross-view attention)
   float scale = 0.125f;
-  // The decoder's token count is 128*k + 1 (pose token + patches).  With split_first_row the tiled kernel
-  // handles query rows [1, nq) -- whole 128-row tiles -- and a small SIMT kernel handles query row 0 of every
-  // (sample, head), instead of paying a whole extra query tile for one row.
-  int split_first_row = 0;
   // split-precision parity mode (common.cuh): q/k/v/out rows are (hi | lo | hi) with ld* the physical (3x) strides;
   // an fp32 SIMT kernel with exact exp2f computes softmax(q k^T) v from hi + lo and stores (hi | lo | hi).
   int split = 0;

@@ -225,7 +225,6 @@ struct StaModel {
   static constexpr size_t kSplitKBytes = static_cast<size_t>(48) << 20;
   std::vector<GraphEntry> graphs;
   cudaStream_t s_cap = nullptr;  // capture stream (the caller's stream may be the legacy default stream)
-  int graph_mode = -1;           // env STA_CUDA_GRAPHS (default on)
   int64_t graph_replays = 0;
 
   // ---- optional per-kernel-family timing (CUDA events on the launch stream) ----
@@ -516,8 +515,7 @@ int ln(const Ctx& c, const float* x, int rows, int C, const LNp& a, bf16* out1, 
                           drop_first_of, c.st, c.m->split);
 }
 int attn(const Ctx& c, const bf16* q, long long ldq, int qc, const bf16* k, long long ldk, int kc, const bf16* v,
-         long long ldv, int vc, bf16* out, long long ldo, int batch, int heads, int nq, int nk, int shift,
-         int split_first_row = 0) {
+         long long ldv, int vc, bf16* out, long long ldo, int batch, int heads, int nq, int nk, int shift) {
   AttnLaunch a;
   const int bm = c.m->bmul();  // the ld* arguments are logical widths
   a.q = q; a.ldq = ldq * bm; a.q_col0 = qc;
@@ -526,7 +524,6 @@ int attn(const Ctx& c, const bf16* q, long long ldq, int qc, const bf16* k, long
   a.out = out; a.ldo = ldo * bm;
   a.batch = batch; a.heads = heads; a.nq = nq; a.nk = nk;
   a.kv_batch_shift = shift;
-  a.split_first_row = split_first_row;
   a.split = c.m->split;
   a.scale = 0.125f;  // head_dim ** -0.5, sta_blocks.py:86
   c.m->launches++;
@@ -625,17 +622,9 @@ void drop_graphs(StaModel* m) {
   m->graphs.clear();
 }
 
-bool graphs_enabled(StaModel* m) {
-  if (m->graph_mode < 0) {
-    const char* e = getenv("STA_CUDA_GRAPHS");
-    m->graph_mode = (e && e[0] == '0') ? 0 : 1;
-  }
-  return m->graph_mode == 1 && !m->prof_on;
-}
-
 template <typename Body>
 int run_graphed(StaModel* m, cudaStream_t st, const std::vector<long long>& key, Body&& body) {
-  if (!graphs_enabled(m)) return body(Ctx{m, st});
+  if (m->prof_on) return body(Ctx{m, st});  // per-kernel timing events need eager launches
   StaModel::GraphEntry* ent = nullptr;
   for (auto& g : m->graphs)
     if (g.key == key) ent = &g;
@@ -746,29 +735,20 @@ int run_decoder(const Ctx& c, int B, int N, DecBufs& d, float* const* out1, floa
   m->launches++;
   RUN(launch_fill_pose_token(d.xd, m->pose_tok, S, M, kDecDim, c.st));
   RUN(emit(0));
-  // The pose token (query row 0) can go to a separate small kernel so that the tiled kernel runs one 128-query tile
-  // fewer per (head, sample) when M = 128 k + 1, at the price of 12 extra launches per view; off unless
-  // STA_ATTN_SPLIT_POSE=1.
-  static int split_env = -1;
-  if (split_env < 0) {
-    const char* e = getenv("STA_ATTN_SPLIT_POSE");
-    split_env = (e && e[0] == '1') ? 1 : 0;
-  }
-  const int split_pose = (split_env && (M - 1 + 127) / 128 < (M + 127) / 128) ? 1 : 0;
   for (int l = 0; l < 12; ++l) {
     const DecBlock& b = m->dec[l];
     // self-attention on norm1(x); norm_y(x) is what the partner view cross-attends to
     RUN(ln(c, d.xd, Td, kDecDim, b.n1, d.ln1, &b.ny, d.lny));
     RUN(linear(c, EPI_ROPE, d.ln1, Td, b.qkv, d.qkv, nullptr, d.pos, 2 * kDecDim));
     RUN(attn(c, d.qkv, 3 * kDecDim, 0, d.qkv, 3 * kDecDim, kDecDim, d.qkv, 3 * kDecDim, 2 * kDecDim, d.att, kDecDim, S,
-             kDecHeads, M, M, 0, split_pose));
+             kDecHeads, M, M, 0));
     RUN(linear(c, EPI_F32, d.att, Td, b.proj, d.xd, d.xd));
     // cross-attention: q from norm2(x), k/v from norm_y(partner input) -- kv sample = (s + B) % 2B
     RUN(linear(c, EPI_ROPE, d.lny, Td, b.ckv, d.kvc, nullptr, d.pos, kDecDim));
     RUN(ln(c, d.xd, Td, kDecDim, b.n2, d.ln1));
     RUN(linear(c, EPI_ROPE, d.ln1, Td, b.cq, d.qc, nullptr, d.pos, kDecDim));
     RUN(attn(c, d.qc, kDecDim, 0, d.kvc, 2 * kDecDim, 0, d.kvc, 2 * kDecDim, kDecDim, d.att, kDecDim, S, kDecHeads, M, M,
-             B, split_pose));
+             B));
     RUN(linear(c, EPI_F32, d.att, Td, b.cproj, d.xd, d.xd));
     // MLP
     RUN(ln(c, d.xd, Td, kDecDim, b.n3, d.ln1));
@@ -989,7 +969,7 @@ int forward_chunk(const Ctx& c, const void* img1, const void* img2, int img_is_b
 extern "C" {
 
 const char* sta_last_error(void) { return get_last_error(); }
-int sta_version(void) { return 1; }
+int sta_version(void) { return 2; }
 
 int sta_device_synchronize(void) {
   STA_CHECK_CUDA(cudaDeviceSynchronize());
@@ -1565,14 +1545,6 @@ int sta_forward_pairs_host(StaModel* m, const void* img1_host, const void* img2_
   // one chunk of up to 16 pairs (the exposed H2D of a 16-pair chunk is meant to cost less than running the GEMMs at half
   // the tile count); larger batches pipeline chunks
   int cp = B;
-  {
-    static int chunk_env = -1;  // STA_HOST_CHUNK=n overrides the pairs per pipelined chunk (tuning knob)
-    if (chunk_env < 0) {
-      const char* e = getenv("STA_HOST_CHUNK");
-      chunk_env = e ? atoi(e) : 0;
-    }
-    if (chunk_env > 0) cp = chunk_env < B ? chunk_env : B;
-  }
   if (cp > m->max_pairs_per_chunk) cp = m->max_pairs_per_chunk;
   int nchunks = (B + cp - 1) / cp;
   if (nchunks > StaModel::kMaxHostChunks) {
@@ -1671,7 +1643,7 @@ int sta_op_gemm(const StaGemmDesc* d, void* stream) {
 
 int sta_op_attention(const void* q, int64_t ldq, int q_col0, const void* k, int64_t ldk, int k_col0, const void* v,
                      int64_t ldv, int v_col0, void* out, int64_t ldo, int batch, int heads, int nq, int nk,
-                     int kv_batch_shift, float scale, int split_first_row, void* stream) {
+                     int kv_batch_shift, float scale, void* stream) {
   AttnLaunch a;
   a.q = static_cast<const bf16*>(q); a.ldq = ldq; a.q_col0 = q_col0;
   a.k = static_cast<const bf16*>(k); a.ldk = ldk; a.k_col0 = k_col0;
@@ -1680,7 +1652,6 @@ int sta_op_attention(const void* q, int64_t ldq, int q_col0, const void* k, int6
   a.batch = batch; a.heads = heads; a.nq = nq; a.nk = nk;
   a.kv_batch_shift = kv_batch_shift;
   a.scale = scale;
-  a.split_first_row = split_first_row;
   return launch_attention(a, static_cast<cudaStream_t>(stream));
 }
 
