@@ -247,6 +247,44 @@ int sta_preprocess_coeffs(int in_size, int out_size, int* ksize, int* bounds, in
 int sta_preprocess_rgb8(const uint8_t* rgb_dev, int H, int W, int res_w, int res_h, int w_edge, int h_edge,
                         float* rgb_out_dev, float* gray_out_dev, uint8_t* u8_out_dev, void* stream);
 
+/* ---- keyframe flow tracker: FlowTracker.compute_disparity (vista_slam/flow_tracker.py:26-66) on the device, with the
+ * reference's fixed constants: cv2.goodFeaturesToTrack(maxCorners=1000, qualityLevel=0.01, minDistance=8, blockSize=7)
+ * and cv2.calcOpticalFlowPyrLK(winSize=(21,21), maxLevel=3, criteria=(EPS|COUNT, 30, 0.01)).  A frame is [H][W] uint8
+ * (frame_is_f32 = 0) or the [H][W] fp32 gray in [0,1] that sta_preprocess_rgb8 writes (1), converted as
+ * (gray * 255).astype(uint8).  Frame sides must be in [32, 2048]; the size checks come before any CUDA call.
+ * A tracker handle owns two pyramids (keyframe and current frame), the keyframe's derivatives and corners, and scratch
+ * for one frame size.  One stream at a time: work on a new stream waits for the previous one. ---- */
+enum { STA_FLOW_MAX_CORNERS = 1000 };
+typedef struct StaFlowTracker StaFlowTracker; /* opaque */
+typedef struct StaFlowStats {
+  int32_t n_corners;     /* keyframe corners */
+  int32_t n_tracked;     /* points with status 1 */
+  double abs_sum;        /* sum over tracked points of |dx| + |dy| of the fp32 differences next - keyframe, in fp64 */
+  double mean_disparity; /* abs_sum / (2 n_tracked): the reference's mean of |dx| and |dy|; 0 when n_tracked = 0 */
+} StaFlowStats;
+int sta_flow_create(int H, int W, StaFlowTracker** out);
+void sta_flow_destroy(StaFlowTracker* t);
+/* initialize_keyframe: builds the frame's pyramid, its Scharr derivatives and its corners (asynchronous). */
+int sta_flow_set_keyframe(StaFlowTracker* t, const void* frame_dev, int frame_is_f32, void* stream);
+/* Builds the current frame's pyramid, tracks the keyframe corners into it and reduces the statistics.  The one host
+ * synchronisation of a tracked frame: stats_out (host) is valid on return. */
+int sta_flow_track(StaFlowTracker* t, const void* frame_dev, int frame_is_f32, StaFlowStats* stats_out, void* stream);
+/* The frame of the last sta_flow_track becomes the keyframe (a buffer swap, no rebuild); its derivatives and corners
+ * are enqueued asynchronously. */
+int sta_flow_promote(StaFlowTracker* t, void* stream);
+/* Device copies of the keyframe corners: pts_out [STA_FLOW_MAX_CORNERS][2] fp32 (x, y) in selection order, the first
+ * *count_out valid; and of the keyframe's level-0 image [H][W] uint8 and derivatives [H][W][2] int16 (either may be
+ * NULL). */
+int sta_flow_keyframe_points(StaFlowTracker* t, float* pts_out_dev, int* count_out_dev, void* stream);
+int sta_flow_keyframe_level0(StaFlowTracker* t, uint8_t* gray_out_dev, int16_t* deriv_out_dev, void* stream);
+/* Op-level entry points (the same kernels).  scratch: a device buffer of sta_flow_scratch_bytes(H, W) bytes (256-byte
+ * aligned); 0 for a refused size.  good_features: pts_out [STA_FLOW_MAX_CORNERS][2], count_out [1] (device).
+ * lk_track: pts [n][2] -> next_pts_out [n][2], status_out [n] uint8 (device). */
+size_t sta_flow_scratch_bytes(int H, int W);
+int sta_op_good_features(const uint8_t* gray_u8, int H, int W, float* pts_out, int* count_out, void* scratch, void* stream);
+int sta_op_lk_track(const uint8_t* prev_u8, const uint8_t* next_u8, int H, int W, const float* pts, int n,
+                    float* next_pts_out, uint8_t* status_out, void* scratch, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -34,6 +34,14 @@ class StaGemmDesc(Structure):
     ]
 
 
+FLOW_MAX_CORNERS = 1000
+
+
+class StaFlowStats(Structure):
+    _fields_ = [("n_corners", c_int32), ("n_tracked", c_int32), ("abs_sum", ctypes.c_double),
+                ("mean_disparity", ctypes.c_double)]
+
+
 _lib = None
 
 
@@ -97,6 +105,18 @@ def lib():
     L.sta_pose_graph_scratch_bytes.restype = ctypes.c_size_t
     L.sta_pose_graph_lm_step.argtypes = [vp, i, vp, vp, vp, i, vp, i, ctypes.c_double, ctypes.c_double, ctypes.c_double, vp, vp,
                                          vp, vp]
+    L.sta_flow_create.argtypes = [i, i, POINTER(vp)]
+    L.sta_flow_destroy.argtypes = [vp]
+    L.sta_flow_destroy.restype = None
+    L.sta_flow_set_keyframe.argtypes = [vp, vp, i, vp]
+    L.sta_flow_track.argtypes = [vp, vp, i, POINTER(StaFlowStats), vp]
+    L.sta_flow_promote.argtypes = [vp, vp]
+    L.sta_flow_keyframe_points.argtypes = [vp, vp, vp, vp]
+    L.sta_flow_keyframe_level0.argtypes = [vp, vp, vp, vp]
+    L.sta_flow_scratch_bytes.argtypes = [i, i]
+    L.sta_flow_scratch_bytes.restype = ctypes.c_size_t
+    L.sta_op_good_features.argtypes = [vp, i, i, vp, vp, vp, vp]
+    L.sta_op_lk_track.argtypes = [vp, vp, i, i, vp, i, vp, vp, vp, vp]
     _lib = L
     return L
 
