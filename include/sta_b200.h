@@ -285,6 +285,55 @@ int sta_op_good_features(const uint8_t* gray_u8, int H, int W, float* pts_out, i
 int sta_op_lk_track(const uint8_t* prev_u8, const uint8_t* next_u8, int H, int W, const float* pts, int n,
                     float* next_pts_out, uint8_t* status_out, void* scratch, void* stream);
 
+/* ---- loop detection: LoopDetector (vista_slam/loop_detector.py) on the device -- cv2.ORB_create().detectAndCompute
+ * with OpenCV's defaults, the DBoW3 vocabulary transform with BowVector::normalize(L1), L1Scoring::score and
+ * detect_loop.  Frames are [H][W] uint8 (frame_is_f32 = 0) or the fp32 gray in [0,1] of sta_preprocess_rgb8 (1),
+ * converted as (gray * 255).astype(uint8); sides must be in [32, 4096].
+ * A vocabulary is a DBoW3 text file (*.txt, load_fromtxt) or a binary stream (toStream, plain or QuickLZ), with 32-byte
+ * binary descriptors and L1 scoring; anything else is refused.  It is parsed on the host and uploaded once to the
+ * current device.  A detector owns ORB scratch for one frame size and the database of every view's vector. ---- */
+typedef struct StaVocab StaVocab;             /* opaque */
+typedef struct StaLoopDetector StaLoopDetector; /* opaque */
+enum { STA_ORB_MAX_KEYPOINTS = 4096 };
+int sta_vocab_load(const char* path, StaVocab** out);
+/* out6 = {k, L, scoring, weighting, nodes, words} */
+int sta_vocab_info(const StaVocab* v, int64_t* out6);
+void sta_vocab_destroy(StaVocab* v);
+int sta_loop_create(StaVocab* v, int loop_dist_min, int loop_nms, int loop_cand_thresh_neighbor, StaLoopDetector** out);
+void sta_loop_destroy(StaLoopDetector* d);
+int sta_loop_views(const StaLoopDetector* d);
+/* compute_bow_feat: ORB, transform and append the view's vector (None when ORB finds no keypoint); asynchronous. */
+int sta_loop_add_frame(StaLoopDetector* d, const void* frame_dev, int frame_is_f32, int H, int W, void* stream);
+/* detect_loop for the newest view i given farthest_neighbor in [0, i]: similarities against every earlier view in one
+ * launch, the candidate scan in one thread, and the one host synchronisation: n_out[2] = {candidates, length of view
+ * i's vector (-1: None)}; the first `cap` candidates are written to js_out / sims_out (host) in the reference's order
+ * (descending similarity, ties in descending j). */
+int sta_loop_detect(StaLoopDetector* d, int farthest_neighbor, int* n_out, int64_t* js_out, double* sims_out, int cap,
+                    void* stream);
+/* Test read-backs (synchronise): a view's vector (len -1 for None) and the similarity row of the last detect (NaN where
+ * either vector is None). */
+int sta_loop_view(StaLoopDetector* d, int view, int32_t* words_out, double* vals_out, int cap, int* len_out, void* stream);
+int sta_loop_similarities(StaLoopDetector* d, double* sims_out, int n, void* stream);
+/* Op-level entry points (the same kernels).  ORB: scratch of sta_orb_scratch_bytes(H, W) bytes (256-byte aligned; 0 for
+ * a refused size); outputs [STA_ORB_MAX_KEYPOINTS] in (level, y, x) order, count_out [1] (all device): xy in level
+ * pixels (int32 x, y), level, pts in level-0 pixels (fp32 x, y), angle (degrees), Harris response, desc [32].
+ * sta_orb_layout: out[0..9] = {total, pyramid, blurred, fast scores, candidates, responses, counters, alive, kept,
+ * histogram} byte offsets in the scratch, then per level {h, w, pixel offset, feature quota}. */
+size_t sta_orb_scratch_bytes(int H, int W);
+int sta_orb_layout(int H, int W, int64_t* out42);
+int sta_op_orb(const void* frame_dev, int frame_is_f32, int H, int W, int32_t* xy_out, int32_t* level_out, float* pts_out,
+               float* angle_out, float* response_out, uint8_t* desc_out, int32_t* count_out, void* scratch, void* stream);
+/* Per descriptor [n][32] (device): word id and weight of the leaf it descends to. */
+int sta_op_bow_transform(const StaVocab* v, const uint8_t* desc_dev, int n, int32_t* word_out, double* weight_out,
+                         void* stream);
+/* The normalised BowVector of n <= STA_ORB_MAX_KEYPOINTS (word, weight) pairs: words_out / vals_out [n], len_out [1]. */
+int sta_op_bow_vector(const StaVocab* v, const int32_t* word, const double* weight, int n, int32_t* words_out,
+                      double* vals_out, int32_t* len_out, void* stream);
+/* L1 score of one vector (qw, qv, *q_len_dev; -1 = None) against nviews CSR vectors (db_start int64, db_len -1 = None). */
+int sta_op_bow_score(const int32_t* qw, const double* qv, const int32_t* q_len_dev, const int32_t* db_word,
+                     const double* db_val, const int64_t* db_start, const int32_t* db_len, int nviews, double* sims_out,
+                     void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -35,6 +35,7 @@ class StaGemmDesc(Structure):
 
 
 FLOW_MAX_CORNERS = 1000
+ORB_MAX_KEYPOINTS = 4096
 
 
 class StaFlowStats(Structure):
@@ -117,6 +118,25 @@ def lib():
     L.sta_flow_scratch_bytes.restype = ctypes.c_size_t
     L.sta_op_good_features.argtypes = [vp, i, i, vp, vp, vp, vp]
     L.sta_op_lk_track.argtypes = [vp, vp, i, i, vp, i, vp, vp, vp, vp]
+    L.sta_vocab_load.argtypes = [c_char_p, POINTER(vp)]
+    L.sta_vocab_info.argtypes = [vp, POINTER(c_int64)]
+    L.sta_vocab_destroy.argtypes = [vp]
+    L.sta_vocab_destroy.restype = None
+    L.sta_loop_create.argtypes = [vp, i, i, i, POINTER(vp)]
+    L.sta_loop_destroy.argtypes = [vp]
+    L.sta_loop_destroy.restype = None
+    L.sta_loop_views.argtypes = [vp]
+    L.sta_loop_add_frame.argtypes = [vp, vp, i, i, i, vp]
+    L.sta_loop_detect.argtypes = [vp, i, POINTER(c_int), POINTER(c_int64), POINTER(ctypes.c_double), i, vp]
+    L.sta_loop_view.argtypes = [vp, i, POINTER(c_int32), POINTER(ctypes.c_double), i, POINTER(c_int), vp]
+    L.sta_loop_similarities.argtypes = [vp, POINTER(ctypes.c_double), i, vp]
+    L.sta_orb_scratch_bytes.argtypes = [i, i]
+    L.sta_orb_scratch_bytes.restype = ctypes.c_size_t
+    L.sta_orb_layout.argtypes = [i, i, POINTER(c_int64)]
+    L.sta_op_orb.argtypes = [vp, i, i, i, vp, vp, vp, vp, vp, vp, vp, vp, vp]
+    L.sta_op_bow_transform.argtypes = [vp, vp, i, vp, vp, vp]
+    L.sta_op_bow_vector.argtypes = [vp, vp, vp, i, vp, vp, vp, vp]
+    L.sta_op_bow_score.argtypes = [vp, vp, vp, vp, vp, vp, vp, i, vp, vp]
     _lib = L
     return L
 

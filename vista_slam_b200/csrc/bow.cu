@@ -1,0 +1,802 @@
+// DBoW3 bag-of-words loop detection on the device: what vista_slam/loop_detector.py::LoopDetector does on the host with
+// DBoW3Py (Vocabulary::load / transform / score, L1 scoring) around cv2 ORB.
+//
+// The vocabulary is parsed on the host (text format of Vocabulary::load_fromtxt, or the binary stream of
+// Vocabulary::fromStream, plain or QuickLZ-compressed) and uploaded once: node descriptors as 8 x u32, the children of
+// each node as a range of a child table in file order, weights (fp64) and word ids.  A detector owns the ORB scratch of
+// one frame size and a device-resident database (CSR) of every view's normalised bag-of-words vector.
+//
+// Bit-exact with the numpy restatement under oracle/ (tests/test_loop_gpu.py): the descent takes the first child of minimal
+// Hamming distance; a word's value is its weight added once per descriptor in fp64 (addWeight; all addends of a word
+// are equal, so the order of descriptors does not matter) or set once (addIfNotExist); the L1 norm, the division and the
+// score s += |v - w| - |v| - |w| are sequential fp64 in ascending word id; detect_loop runs in one thread.  One host
+// synchronisation per keyframe: the read-back of the candidate list.
+#include "../../include/sta_b200.h"
+#include "common.cuh"
+#include "host_util.h"
+#include "loop.h"
+
+#include <stdint.h>
+#include <stdio.h>
+#include <stdlib.h>
+#include <string.h>
+
+#include <fstream>
+#include <sstream>
+#include <string>
+#include <vector>
+
+namespace sta {
+namespace {
+
+constexpr uint64_t kMagic = 88877711233ull;
+constexpr int kBuildThreads = 1024;
+enum { kTfIdf = 0, kTf = 1, kIdf = 2, kBinary = 3 };
+
+struct HostVocab {
+  int k = 0, L = 0, scoring = 0, weighting = 0;
+  std::vector<uint32_t> desc;    // [n][8]
+  std::vector<int> parent;       // -1 for the root
+  std::vector<double> weight;
+  std::vector<int> word;         // -1: not a word
+  int n_words = 0;
+};
+
+bool fail(std::string* err, const std::string& msg) {
+  *err = msg;
+  return false;
+}
+
+bool validate_header(const HostVocab& v, std::string* err) {
+  if (v.scoring != 0) {
+    static const char* names[] = {"L1_NORM", "L2_NORM", "CHI_SQUARE", "KL", "BHATTACHARYYA", "DOT_PRODUCT"};
+    return fail(err, std::string("only L1 scoring is supported; the vocabulary uses ") +
+                         (v.scoring >= 0 && v.scoring < 6 ? names[v.scoring] : "an unknown scoring"));
+  }
+  if (v.weighting < 0 || v.weighting > 3) return fail(err, "unknown weighting type");
+  return true;
+}
+
+// Vocabulary::load_fromtxt
+bool load_text(const std::string& path, HostVocab* v, std::string* err) {
+  FILE* f = fopen(path.c_str(), "rb");
+  if (!f) return fail(err, "cannot open " + path);
+  std::string data;
+  {
+    char buf[1 << 16];
+    size_t n;
+    while ((n = fread(buf, 1, sizeof(buf), f)) > 0) data.append(buf, n);
+    fclose(f);
+  }
+  const char* p = data.c_str();
+  const char* end = p + data.size();
+  const char* eol = static_cast<const char*>(memchr(p, '\n', end - p));
+  if (!eol) eol = end;
+  int n1, n2;
+  if (sscanf(std::string(p, eol).c_str(), "%d %d %d %d", &v->k, &v->L, &n1, &n2) != 4 || v->k < 0 || v->k > 20 ||
+      v->L < 1 || v->L > 10 || n1 < 0 || n1 > 5 || n2 < 0 || n2 > 3)
+    return fail(err, "not a DBoW3 text vocabulary: " + path);
+  v->scoring = n1;
+  v->weighting = n2;
+  if (!validate_header(*v, err)) return false;
+  v->desc.assign(8, 0u);
+  v->parent.assign(1, -1);
+  v->weight.assign(1, 0.0);
+  v->word.assign(1, -1);
+  p = eol < end ? eol + 1 : end;
+  float vals[64];
+  while (p < end) {
+    eol = static_cast<const char*>(memchr(p, '\n', end - p));
+    if (!eol) eol = end;
+    if (eol == p) break;  // an empty line ends the node list
+    const std::string line(p, eol);
+    p = eol < end ? eol + 1 : end;
+    const char* s = line.c_str();
+    char* q;
+    const long pid = strtol(s, &q, 10);
+    if (q == s) break;
+    s = q;
+    const long leaf = strtol(s, &q, 10);
+    if (q == s) return fail(err, "malformed node line in " + path);
+    s = q;
+    int nv = 0;
+    for (;;) {
+      const float d = strtof(s, &q);
+      if (q == s) break;
+      if (nv == 64) return fail(err, "only binary (32-byte) descriptors are supported: a node has too many values");
+      vals[nv++] = d;
+      s = q;
+    }
+    if (nv != 33) return fail(err, "only binary 32-byte descriptors are supported (a node line has " + std::to_string(nv - 1) +
+                                       " descriptor values)");
+    const int nid = static_cast<int>(v->parent.size());
+    if (pid < 0 || pid >= nid) return fail(err, "node " + std::to_string(nid) + " names a parent that does not precede it");
+    v->parent.push_back(static_cast<int>(pid));
+    v->weight.push_back(static_cast<double>(vals[32]));
+    uint8_t bytes[32];
+    for (int i = 0; i < 32; ++i) bytes[i] = static_cast<uint8_t>(vals[i]);
+    uint32_t w8[8];
+    memcpy(w8, bytes, 32);
+    v->desc.insert(v->desc.end(), w8, w8 + 8);
+    v->word.push_back(leaf > 0 ? v->n_words++ : -1);
+  }
+  return true;
+}
+
+template <typename T>
+bool rd(const std::string& b, size_t& pos, T* out) {
+  if (pos + sizeof(T) > b.size()) return false;
+  memcpy(out, b.data() + pos, sizeof(T));
+  pos += sizeof(T);
+  return true;
+}
+
+// One QuickLZ 1.5 chunk as DBoW3's toStream writes them (compression level 1, streaming buffer 0), written from the
+// format: a header (flag byte: bit 0 compressed, bit 1 sizes as u32 rather than u8; then compressed and decompressed
+// sizes), then 32-bit control words whose bits, least significant first, select a match (1) or a literal byte (0); a
+// control word is spent when only its sentinel bit is left.  A match token names a 12-bit hash of the 3 bytes it
+// repeats and a length (low nibble + 2, or the next byte when the nibble is 0); the decoder keeps the table of the last
+// output position of each hash, updated for every position up to the start of a match and up to 3 bytes behind the
+// last literal (positions inside a match are not hashed).  The last UNCONDITIONAL_MATCHLEN + UNCOMPRESSED_END = 10
+// bytes are literals whatever the control bits say.  *used receives the chunk's compressed size.
+bool qlz1_chunk(const uint8_t* in, size_t avail, std::string* out, size_t* used, std::string* err) {
+  if (avail < 3) return fail(err, "truncated QuickLZ chunk");
+  const bool wide = (in[0] & 2) != 0;
+  const size_t hdr = wide ? 9 : 3;
+  if (avail < hdr) return fail(err, "truncated QuickLZ chunk");
+  uint32_t csize = 0, dsize = 0;
+  if (wide) {
+    memcpy(&csize, in + 1, 4);
+    memcpy(&dsize, in + 5, 4);
+  } else {
+    csize = in[1];
+    dsize = in[2];
+  }
+  if (csize < hdr || csize > avail) return fail(err, "truncated QuickLZ chunk");
+  *used = csize;
+  if (!(in[0] & 1)) {
+    if (csize - hdr < dsize) return fail(err, "corrupt QuickLZ chunk");
+    out->append(reinterpret_cast<const char*>(in + hdr), dsize);
+    return true;
+  }
+  std::vector<uint8_t> dst(dsize);
+  std::vector<uint32_t> table(4096, 0);
+  auto hash_at = [&](size_t p) {
+    const uint32_t v = dst[p] | (dst[p + 1] << 8) | (static_cast<uint32_t>(dst[p + 2]) << 16);
+    return ((v >> 12) ^ v) & 0xfffu;
+  };
+  const uint8_t* src = in + hdr;
+  const uint8_t* end = in + csize;
+  size_t d = 0;
+  long long last_hashed = -1;
+  const long long last_matchstart = static_cast<long long>(dsize) - 1 - 6 - 4;
+  auto hash_upto = [&](long long upto) {
+    while (last_hashed < upto) {
+      ++last_hashed;
+      table[hash_at(static_cast<size_t>(last_hashed))] = static_cast<uint32_t>(last_hashed);
+    }
+  };
+  uint32_t cword = 1;
+  while (d < dsize) {
+    if (cword == 1) {
+      if (end - src < 4) return fail(err, "corrupt QuickLZ chunk");
+      memcpy(&cword, src, 4);
+      src += 4;
+    }
+    if (cword & 1) {
+      cword >>= 1;
+      if (end - src < 3) return fail(err, "corrupt QuickLZ chunk");
+      const uint32_t fetch = src[0] | (src[1] << 8) | (static_cast<uint32_t>(src[2]) << 16);
+      const uint32_t from = table[(fetch >> 4) & 0xfff];
+      uint32_t len;
+      if (fetch & 0xf) {
+        len = (fetch & 0xf) + 2;
+        src += 2;
+      } else {
+        len = src[2];
+        src += 3;
+      }
+      if (from >= d || len > dsize - d) return fail(err, "corrupt QuickLZ chunk");
+      for (uint32_t k = 0; k < len; ++k) dst[d + k] = dst[from + k];
+      hash_upto(static_cast<long long>(d));
+      d += len;
+      last_hashed = static_cast<long long>(d) - 1;
+    } else if (static_cast<long long>(d) < last_matchstart) {
+      if (src >= end) return fail(err, "corrupt QuickLZ chunk");
+      dst[d++] = *src++;
+      cword >>= 1;
+      hash_upto(static_cast<long long>(d) - 3);
+    } else {
+      while (d < dsize) {
+        if (cword == 1) {
+          src += 4;
+          cword = 1u << 31;
+        }
+        if (src >= end) return fail(err, "corrupt QuickLZ chunk");
+        dst[d++] = *src++;
+        cword >>= 1;
+      }
+    }
+  }
+  out->append(reinterpret_cast<const char*>(dst.data()), dsize);
+  return true;
+}
+
+// Vocabulary::fromStream: a plain stream, or chunks of 10 000 bytes compressed with QuickLZ level 1
+bool load_binary(const std::string& file, HostVocab* v, std::string* err, std::vector<int>* order) {
+  size_t pos = 8;
+  uint32_t nnodes = 0;
+  uint8_t cflag;
+  if (!rd(file, pos, &cflag) || !rd(file, pos, &nnodes)) return fail(err, "truncated DBoW3 binary vocabulary");
+  if (nnodes == 0) return fail(err, "empty vocabulary");
+  std::string inflated;
+  if (cflag) {
+    uint32_t nchunks;
+    if (!rd(file, pos, &nchunks)) return fail(err, "truncated DBoW3 binary vocabulary");
+    for (uint32_t c = 0; c < nchunks; ++c) {
+      size_t used = 0;
+      if (pos >= file.size() ||
+          !qlz1_chunk(reinterpret_cast<const uint8_t*>(file.data()) + pos, file.size() - pos, &inflated, &used, err))
+        return fail(err, "DBoW3 vocabulary: " + (err->empty() ? std::string("truncated chunk") : *err));
+      pos += used;
+    }
+    pos = 0;
+  }
+  const std::string& data = cflag ? inflated : file;
+  if (!rd(data, pos, &v->k) || !rd(data, pos, &v->L) || !rd(data, pos, &v->scoring) || !rd(data, pos, &v->weighting))
+    return fail(err, "truncated DBoW3 binary vocabulary");
+  if (!validate_header(*v, err)) return false;
+  v->desc.assign(static_cast<size_t>(nnodes) * 8, 0u);
+  v->parent.assign(nnodes, -1);
+  v->weight.assign(nnodes, 0.0);
+  v->word.assign(nnodes, -1);
+  for (uint32_t i = 1; i < nnodes; ++i) {
+    uint32_t nid, pid;
+    double w;
+    int cols, rows, type;
+    if (!rd(data, pos, &nid) || !rd(data, pos, &pid) || !rd(data, pos, &w) || !rd(data, pos, &cols) ||
+        !rd(data, pos, &rows) || !rd(data, pos, &type))
+      return fail(err, "truncated DBoW3 binary vocabulary");
+    if (type != 0 || rows != 1 || cols != 32)
+      return fail(err, "only binary 32-byte (CV_8U) descriptors are supported");
+    if (nid == 0 || nid >= nnodes || pid >= nnodes) return fail(err, "node id out of range in the vocabulary");
+    if (pos + 32 > data.size()) return fail(err, "truncated DBoW3 binary vocabulary");
+    memcpy(&v->desc[static_cast<size_t>(nid) * 8], data.data() + pos, 32);
+    pos += 32;
+    v->parent[nid] = static_cast<int>(pid);
+    v->weight[nid] = w;
+    order->push_back(static_cast<int>(nid));
+  }
+  uint32_t nw;
+  if (!rd(data, pos, &nw)) return fail(err, "truncated DBoW3 binary vocabulary");
+  for (uint32_t i = 0; i < nw; ++i) {
+    uint32_t wid, nid;
+    if (!rd(data, pos, &wid) || !rd(data, pos, &nid)) return fail(err, "truncated DBoW3 binary vocabulary");
+    if (nid >= nnodes) return fail(err, "word names a node out of range");
+    v->word[nid] = static_cast<int>(wid);
+  }
+  v->n_words = static_cast<int>(nw);
+  return true;
+}
+
+}  // namespace
+}  // namespace sta
+
+struct StaVocab {
+  int k, L, scoring, weighting, n_nodes, n_words, device;
+  uint32_t* desc;     // [n][8]
+  int* child_start;   // [n + 1] into child
+  int* child;         // [n - 1], file order
+  double* weight;
+  int* word;
+};
+
+namespace sta {
+namespace {
+
+int upload_vocab(const HostVocab& v, const std::vector<int>& order, StaVocab** out) {
+  const int n = static_cast<int>(v.parent.size());
+  std::vector<int> count(n + 1, 0), start(n + 1, 0), child(n > 1 ? n - 1 : 1, 0);
+  for (int nid : order) count[v.parent[nid]]++;
+  for (int i = 0; i < n; ++i) start[i + 1] = start[i] + count[i];
+  std::vector<int> fill(start.begin(), start.end() - 1);
+  for (int nid : order) child[fill[v.parent[nid]]++] = nid;
+  StaVocab* h = new StaVocab();
+  h->k = v.k;
+  h->L = v.L;
+  h->scoring = v.scoring;
+  h->weighting = v.weighting;
+  h->n_nodes = n;
+  h->n_words = v.n_words;
+  cudaGetDevice(&h->device);
+  h->desc = nullptr;
+  h->child_start = h->child = h->word = nullptr;
+  h->weight = nullptr;
+  cudaError_t e = cudaMalloc(&h->desc, sizeof(uint32_t) * 8 * n);
+  if (e == cudaSuccess) e = cudaMalloc(&h->child_start, sizeof(int) * (n + 1));
+  if (e == cudaSuccess) e = cudaMalloc(&h->child, sizeof(int) * child.size());
+  if (e == cudaSuccess) e = cudaMalloc(&h->weight, sizeof(double) * n);
+  if (e == cudaSuccess) e = cudaMalloc(&h->word, sizeof(int) * n);
+  if (e == cudaSuccess) e = cudaMemcpy(h->desc, v.desc.data(), sizeof(uint32_t) * 8 * n, cudaMemcpyHostToDevice);
+  if (e == cudaSuccess) e = cudaMemcpy(h->child_start, start.data(), sizeof(int) * (n + 1), cudaMemcpyHostToDevice);
+  if (e == cudaSuccess) e = cudaMemcpy(h->child, child.data(), sizeof(int) * child.size(), cudaMemcpyHostToDevice);
+  if (e == cudaSuccess) e = cudaMemcpy(h->weight, v.weight.data(), sizeof(double) * n, cudaMemcpyHostToDevice);
+  if (e == cudaSuccess) e = cudaMemcpy(h->word, v.word.data(), sizeof(int) * n, cudaMemcpyHostToDevice);
+  if (e != cudaSuccess) {
+    cudaFree(h->desc);
+    cudaFree(h->child_start);
+    cudaFree(h->child);
+    cudaFree(h->weight);
+    cudaFree(h->word);
+    delete h;
+    set_last_error(std::string("vocabulary upload failed: ") + cudaGetErrorString(e));
+    return 1;
+  }
+  *out = h;
+  return 0;
+}
+
+// Vocabulary::transform(feature, word_id, weight): one thread per descriptor
+__global__ void transform_kernel(const uint8_t* desc, const int* n_dev, int n_host, StaVocab v, int* word_out,
+                                 double* weight_out) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  const int n = n_dev ? *n_dev : n_host;
+  if (i >= n) return;
+  uint32_t d[8];
+  for (int k = 0; k < 8; ++k) d[k] = *reinterpret_cast<const uint32_t*>(desc + 32 * i + 4 * k);
+  int node = 0;
+  while (v.child_start[node + 1] > v.child_start[node]) {
+    unsigned best = 0xffffffffu;
+    int next = node;
+    for (int c = v.child_start[node]; c < v.child_start[node + 1]; ++c) {
+      const int id = v.child[c];
+      const uint32_t* nd = v.desc + 8 * static_cast<long long>(id);
+      unsigned dist = 0;
+#pragma unroll
+      for (int k = 0; k < 8; ++k) dist += __popc(d[k] ^ nd[k]);
+      if (dist < best) {
+        best = dist;
+        next = id;
+      }
+    }
+    node = next;
+  }
+  word_out[i] = v.word[node];
+  weight_out[i] = v.weight[node];
+}
+
+// BowVector: accumulate (addWeight / addIfNotExist), then normalize(L1).  One CTA.  Writes the vector at entry offset
+// *entries_used of the database (words ascending) and its length; *entries_used advances.  len = -1 (None) when there
+// was no descriptor.
+__global__ void __launch_bounds__(kBuildThreads) build_kernel(const int* word, const double* weight, const int* n_dev,
+                                                              int n_host, int weighting, int* db_word, double* db_val,
+                                                              long long* db_start, int* db_len, int view,
+                                                              long long* entries_used) {
+  __shared__ int s_first[kOrbMaxKeypoints];  // rank -> descriptor of the sorted (word, index) list
+  __shared__ int s_cnt;
+  const int n = n_dev ? *n_dev : n_host;
+  const long long base = *entries_used;
+  if (threadIdx.x == 0) s_cnt = 0;
+  __syncthreads();
+  // rank sort of the descriptors with weight > 0 by (word, index)
+  for (int i = threadIdx.x; i < n; i += blockDim.x) {
+    if (!(weight[i] > 0.0)) continue;
+    const int wi = word[i];
+    int rank = 0;
+    for (int j = 0; j < n; ++j) {
+      if (!(weight[j] > 0.0)) continue;
+      const int wj = word[j];
+      rank += (wj < wi || (wj == wi && j < i)) ? 1 : 0;
+    }
+    s_first[rank] = i;
+    atomicAdd(&s_cnt, 1);
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    const int m = s_cnt;
+    int len = 0;
+    for (int r = 0; r < m;) {
+      const int wv = word[s_first[r]];
+      const double x = weight[s_first[r]];
+      double acc = x;
+      int e = r + 1;
+      for (; e < m && word[s_first[e]] == wv; ++e)
+        if (weighting == kTf || weighting == kTfIdf) acc = __dadd_rn(acc, x);
+      db_word[base + len] = wv;
+      db_val[base + len] = acc;
+      ++len;
+      r = e;
+    }
+    double norm = 0.0;
+    for (int i = 0; i < len; ++i) norm = __dadd_rn(norm, fabs(db_val[base + i]));
+    if (norm > 0.0)
+      for (int i = 0; i < len; ++i) db_val[base + i] = __ddiv_rn(db_val[base + i], norm);
+    db_start[view] = base;
+    db_len[view] = n > 0 ? len : -1;
+    *entries_used = base + len;
+  }
+}
+
+// L1Scoring::score of view q against views [0, nviews): one thread per view, a merge over ascending word ids.
+// sims[j] = NaN when either vector is None.
+__global__ void score_kernel(const int* qw, const double* qv, const int* q_len_dev, const long long* q_start_dev,
+                             const int* db_word, const double* db_val, const long long* db_start, const int* db_len,
+                             int nviews, double* sims) {
+  const int j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= nviews) return;
+  const int na = *q_len_dev;
+  const int nb = db_len[j];
+  if (na < 0 || nb < 0) {
+    sims[j] = __longlong_as_double(0x7ff8000000000000ll);
+    return;
+  }
+  const long long qa = q_start_dev ? *q_start_dev : 0;
+  const int* aw = qw + qa;
+  const double* av = qv + qa;
+  const int* bw = db_word + db_start[j];
+  const double* bv = db_val + db_start[j];
+  double s = 0.0;
+  int a = 0, b = 0;
+  while (a < na && b < nb) {
+    if (aw[a] == bw[b]) {
+      const double vi = av[a], wi = bv[b];
+      s = __dadd_rn(s, __dsub_rn(__dsub_rn(fabs(__dsub_rn(vi, wi)), fabs(vi)), fabs(wi)));
+      ++a;
+      ++b;
+    } else if (aw[a] < bw[b]) {
+      ++a;
+    } else {
+      ++b;
+    }
+  }
+  sims[j] = __ddiv_rn(-s, 2.0);
+}
+
+// loop_detector.py:23-50 over the precomputed similarities of view i; out: [0] = count, then (j, sim) pairs as
+// {int64 j, double sim}, sorted by descending similarity, ties keeping the scan's descending-j order.
+__global__ void detect_kernel(const double* sims, const int* db_len, int i, int farthest, int dist_min, int nms,
+                              int thresh_neighbor, long long* out) {
+  const bool none_i = db_len[i] < 0;
+  const int lo = i - thresh_neighbor > 0 ? i - thresh_neighbor : 0;
+  double th = 1.0;
+  bool any = false;
+  for (int j = lo; j < i; ++j) {
+    if (none_i || db_len[j] < 0) continue;
+    th = any ? fmin(th, sims[j]) : sims[j];
+    any = true;
+  }
+  long long n = 0;
+  long long* c = out + 2;
+  int last = farthest;
+  for (int j = farthest - 1; j >= 0; --j) {
+    if (last - j > nms && i - j > dist_min) {
+      if (none_i || db_len[j] < 0) continue;
+      const double s = sims[j];
+      if (s > th) {
+        // stable insertion by descending similarity
+        long long k = n;
+        while (k > 0 && __longlong_as_double(c[2 * (k - 1) + 1]) < s) {
+          c[2 * k] = c[2 * (k - 1)];
+          c[2 * k + 1] = c[2 * (k - 1) + 1];
+          --k;
+        }
+        c[2 * k] = j;
+        c[2 * k + 1] = __double_as_longlong(s);
+        ++n;
+        last = j;
+      }
+    }
+  }
+  out[0] = n;
+  out[1] = db_len[i];
+}
+
+}  // namespace
+}  // namespace sta
+
+using namespace sta;
+
+struct StaLoopDetector {
+  StaVocab* vocab;
+  int dist_min, nms, thresh_neighbor;
+  int H = 0, W = 0;
+  OrbLayout lay = {};
+  void* scratch = nullptr;        // ORB scratch
+  void* kp = nullptr;             // ORB outputs + transform outputs
+  int views = 0, view_cap = 0;
+  // Upper bound on the database entries in use, kept on the host: each appended view may add up to kOrbMaxKeypoints
+  // words, and the exact count (entries_dev) is only read back at the synchronisation of sta_loop_detect.
+  long long entries_bound = 0, entry_cap = 0;
+  cudaStream_t last_stream = nullptr;  // the stream of the last call, synchronised before destruction
+  int* db_word = nullptr;
+  double* db_val = nullptr;
+  long long* db_start = nullptr;
+  int* db_len = nullptr;
+  double* sims = nullptr;
+  long long* result = nullptr;    // device [2 + 2 view_cap]
+  long long* entries_dev = nullptr;
+  long long* pinned = nullptr;    // host copy of result
+};
+
+namespace {
+
+struct KpBufs {
+  int2* xy;
+  int* level;
+  float2* pts;
+  float* angle;
+  float* resp;
+  uint8_t* desc;
+  int* count;
+  int* word;
+  double* weight;
+};
+
+KpBufs kp_bufs(void* base) {
+  char* p = static_cast<char*>(base);
+  KpBufs b;
+  const int M = kOrbMaxKeypoints;
+  b.xy = reinterpret_cast<int2*>(p);          p += sizeof(int2) * M;
+  b.pts = reinterpret_cast<float2*>(p);       p += sizeof(float2) * M;
+  b.weight = reinterpret_cast<double*>(p);    p += sizeof(double) * M;
+  b.level = reinterpret_cast<int*>(p);        p += sizeof(int) * M;
+  b.angle = reinterpret_cast<float*>(p);      p += sizeof(float) * M;
+  b.resp = reinterpret_cast<float*>(p);       p += sizeof(float) * M;
+  b.word = reinterpret_cast<int*>(p);         p += sizeof(int) * M;
+  b.desc = reinterpret_cast<uint8_t*>(p);     p += 32 * M;
+  b.count = reinterpret_cast<int*>(p);
+  return b;
+}
+constexpr size_t kKpBytes = (8 + 8 + 8 + 4 + 4 + 4 + 4 + 32) * kOrbMaxKeypoints + 16;
+
+template <typename T>
+int grow(T** p, long long old_n, long long new_n, cudaStream_t st) {
+  T* q = nullptr;
+  STA_CHECK_CUDA(cudaMallocAsync(&q, sizeof(T) * new_n, st));
+  if (*p && old_n) STA_CHECK_CUDA(cudaMemcpyAsync(q, *p, sizeof(T) * old_n, cudaMemcpyDeviceToDevice, st));
+  if (*p) STA_CHECK_CUDA(cudaFreeAsync(*p, st));
+  *p = q;
+  return 0;
+}
+
+// room for one more view of up to kOrbMaxKeypoints words
+int reserve(StaLoopDetector* d, cudaStream_t st) {
+  if (d->views + 1 > d->view_cap) {
+    const int cap = d->view_cap ? 2 * d->view_cap : 256;
+    if (grow(&d->db_start, d->view_cap, cap, st) || grow(&d->db_len, d->view_cap, cap, st) ||
+        grow(&d->sims, 0, cap, st) || grow(&d->result, 0, 2 + 2LL * cap, st))
+      return 1;
+    if (d->pinned) cudaFreeHost(d->pinned);
+    STA_CHECK_CUDA(cudaMallocHost(&d->pinned, sizeof(long long) * (2 + 2LL * cap)));
+    d->view_cap = cap;
+  }
+  if (d->entries_bound + kOrbMaxKeypoints > d->entry_cap) {
+    long long cap = d->entry_cap ? 2 * d->entry_cap : 64LL * kOrbMaxKeypoints;
+    while (cap < d->entries_bound + kOrbMaxKeypoints) cap *= 2;
+    if (grow(&d->db_word, d->entry_cap, cap, st) || grow(&d->db_val, d->entry_cap, cap, st)) return 1;
+    d->entry_cap = cap;
+  }
+  return 0;
+}
+
+int bow_of_descriptors(StaVocab* v, const uint8_t* desc, const int* n_dev, int n_host, int* word, double* weight,
+                       cudaStream_t st) {
+  const int cap = n_dev ? kOrbMaxKeypoints : n_host;
+  if (cap > 0) transform_kernel<<<(cap + 127) / 128, 128, 0, st>>>(desc, n_dev, n_host, *v, word, weight);
+  STA_CHECK_CUDA(cudaGetLastError());
+  return 0;
+}
+
+}  // namespace
+
+extern "C" {
+
+int sta_vocab_load(const char* path, StaVocab** out) {
+  STA_REQUIRE(path && out, "null argument");
+  std::string p(path), err;
+  HostVocab v;
+  std::vector<int> order;
+  uint64_t sig = 0;
+  {
+    std::ifstream f(p, std::ios::binary);
+    STA_REQUIRE(f.good(), (std::string("cannot open vocabulary ") + p).c_str());
+    f.read(reinterpret_cast<char*>(&sig), sizeof(sig));
+  }
+  bool ok;
+  if (sig == kMagic) {
+    std::ifstream f(p, std::ios::binary);
+    const std::string data((std::istreambuf_iterator<char>(f)), std::istreambuf_iterator<char>());
+    ok = load_binary(data, &v, &err, &order);
+  } else if (p.find(".txt") != std::string::npos) {
+    ok = load_text(p, &v, &err);
+    for (int i = 1; ok && i < static_cast<int>(v.parent.size()); ++i) order.push_back(i);
+  } else {
+    ok = fail(&err, "unsupported vocabulary format (expected a DBoW3 .txt or binary file): " + p);
+  }
+  if (!ok) {
+    set_last_error("sta_vocab_load: " + err);
+    return 2;
+  }
+  return upload_vocab(v, order, out);
+}
+
+int sta_vocab_info(const StaVocab* v, int64_t* out6) {
+  STA_REQUIRE(v && out6, "null argument");
+  out6[0] = v->k;
+  out6[1] = v->L;
+  out6[2] = v->scoring;
+  out6[3] = v->weighting;
+  out6[4] = v->n_nodes;
+  out6[5] = v->n_words;
+  return 0;
+}
+
+void sta_vocab_destroy(StaVocab* v) {
+  if (!v) return;
+  cudaFree(v->desc);
+  cudaFree(v->child_start);
+  cudaFree(v->child);
+  cudaFree(v->weight);
+  cudaFree(v->word);
+  delete v;
+}
+
+int sta_op_bow_transform(const StaVocab* v, const uint8_t* desc_dev, int n, int32_t* word_out, double* weight_out,
+                         void* stream) {
+  STA_REQUIRE(v && n >= 0, "bad argument");
+  return bow_of_descriptors(const_cast<StaVocab*>(v), desc_dev, nullptr, n, word_out, weight_out,
+                            static_cast<cudaStream_t>(stream));
+}
+
+int sta_op_bow_vector(const StaVocab* v, const int32_t* word, const double* weight, int n, int32_t* words_out,
+                      double* vals_out, int32_t* len_out, void* stream) {
+  STA_REQUIRE(v && n >= 0 && n <= kOrbMaxKeypoints, "descriptor count must be in [0, 4096]");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  long long* tmp = nullptr;
+  STA_CHECK_CUDA(cudaMallocAsync(&tmp, sizeof(long long) * 2, st));
+  STA_CHECK_CUDA(cudaMemsetAsync(tmp, 0, sizeof(long long) * 2, st));
+  build_kernel<<<1, kBuildThreads, 0, st>>>(word, weight, nullptr, n, v->weighting, words_out, vals_out, tmp + 1,
+                                            len_out, 0, tmp);
+  STA_CHECK_CUDA(cudaGetLastError());
+  STA_CHECK_CUDA(cudaFreeAsync(tmp, st));
+  return 0;
+}
+
+int sta_op_bow_score(const int32_t* qw, const double* qv, const int32_t* q_len_dev, const int32_t* db_word,
+                     const double* db_val, const int64_t* db_start, const int32_t* db_len, int nviews, double* sims_out,
+                     void* stream) {
+  STA_REQUIRE(nviews >= 0, "bad view count");
+  if (nviews)
+    score_kernel<<<(nviews + 127) / 128, 128, 0, static_cast<cudaStream_t>(stream)>>>(
+        qw, qv, q_len_dev, nullptr, db_word, db_val, reinterpret_cast<const long long*>(db_start), db_len, nviews,
+        sims_out);
+  STA_CHECK_CUDA(cudaGetLastError());
+  return 0;
+}
+
+int sta_loop_create(StaVocab* v, int loop_dist_min, int loop_nms, int loop_cand_thresh_neighbor, StaLoopDetector** out) {
+  STA_REQUIRE(v && out, "null argument");
+  StaLoopDetector* d = new StaLoopDetector();
+  d->vocab = v;
+  d->dist_min = loop_dist_min;
+  d->nms = loop_nms;
+  d->thresh_neighbor = loop_cand_thresh_neighbor;
+  if (cudaMalloc(&d->entries_dev, sizeof(long long)) != cudaSuccess ||
+      cudaMemset(d->entries_dev, 0, sizeof(long long)) != cudaSuccess) {
+    delete d;
+    set_last_error("sta_loop_create: allocation failed");
+    return 1;
+  }
+  *out = d;
+  return 0;
+}
+
+void sta_loop_destroy(StaLoopDetector* d) {
+  if (!d) return;
+  if (d->last_stream) cudaStreamSynchronize(d->last_stream);
+  cudaFree(d->scratch);
+  cudaFree(d->kp);
+  cudaFree(d->db_word);
+  cudaFree(d->db_val);
+  cudaFree(d->db_start);
+  cudaFree(d->db_len);
+  cudaFree(d->sims);
+  cudaFree(d->result);
+  cudaFree(d->entries_dev);
+  if (d->pinned) cudaFreeHost(d->pinned);
+  delete d;
+}
+
+int sta_loop_views(const StaLoopDetector* d) { return d ? d->views : -1; }
+
+// compute_bow_feat: ORB + transform + append to the database (asynchronous)
+int sta_loop_add_frame(StaLoopDetector* d, const void* frame_dev, int frame_is_f32, int H, int W, void* stream) {
+  STA_REQUIRE(d, "null detector");
+  STA_REQUIRE(orb_size_ok(H, W), "ORB frame sides must be in [32, 4096]");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (H != d->H || W != d->W) {
+    const OrbLayout lay = orb_layout(H, W);
+    if (d->scratch) STA_CHECK_CUDA(cudaFreeAsync(d->scratch, st));
+    STA_CHECK_CUDA(cudaMallocAsync(&d->scratch, lay.total, st));
+    if (!d->kp) STA_CHECK_CUDA(cudaMallocAsync(&d->kp, kKpBytes, st));
+    d->lay = lay;
+    d->H = H;
+    d->W = W;
+  }
+  if (reserve(d, st)) return 1;
+  KpBufs b = kp_bufs(d->kp);
+  OrbOut o = {b.xy, b.level, b.pts, b.angle, b.resp, b.desc, b.count};
+  if (orb_run(d->lay, d->scratch, frame_dev, frame_is_f32, o, st)) return 1;
+  if (bow_of_descriptors(d->vocab, b.desc, b.count, 0, b.word, b.weight, st)) return 1;
+  build_kernel<<<1, kBuildThreads, 0, st>>>(b.word, b.weight, b.count, 0, d->vocab->weighting, d->db_word, d->db_val,
+                                            d->db_start, d->db_len, d->views, d->entries_dev);
+  STA_CHECK_CUDA(cudaGetLastError());
+  d->views += 1;
+  d->entries_bound += kOrbMaxKeypoints;
+  d->last_stream = st;
+  return 0;
+}
+
+// detect_loop for the newest view: scores against every earlier view, the candidate scan, and one read-back.
+// js_out / sims_out (host) receive up to `cap` candidates; n_out[2] = {number found, length of view i (-1: None)}.
+int sta_loop_detect(StaLoopDetector* d, int farthest_neighbor, int* n_out, int64_t* js_out, double* sims_out, int cap,
+                    void* stream) {
+  STA_REQUIRE(d && d->views > 0, "no view has been added");
+  const int i = d->views - 1;
+  STA_REQUIRE(farthest_neighbor >= 0 && farthest_neighbor <= i, "farthest_neighbor must be in [0, view index]");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  d->last_stream = st;
+  if (i > 0)
+    score_kernel<<<(i + 127) / 128, 128, 0, st>>>(d->db_word, d->db_val, d->db_len + i, d->db_start + i, d->db_word,
+                                                  d->db_val, d->db_start, d->db_len, i, d->sims);
+  detect_kernel<<<1, 1, 0, st>>>(d->sims, d->db_len, i, farthest_neighbor, d->dist_min, d->nms, d->thresh_neighbor,
+                                 d->result);
+  STA_CHECK_CUDA(cudaGetLastError());
+  const size_t nb = sizeof(long long) * (2 + 2LL * (i + 1));
+  STA_CHECK_CUDA(cudaMemcpyAsync(d->pinned, d->result, nb, cudaMemcpyDeviceToHost, st));
+  STA_CHECK_CUDA(cudaMemcpyAsync(&d->entries_bound, d->entries_dev, sizeof(long long), cudaMemcpyDeviceToHost, st));
+  unsigned overflow = 0;
+  STA_CHECK_CUDA(cudaMemcpyAsync(&overflow, static_cast<char*>(d->scratch) + d->lay.counters + 3 * sizeof(unsigned),
+                                 sizeof(unsigned), cudaMemcpyDeviceToHost, st));
+  STA_CHECK_CUDA(cudaStreamSynchronize(st));
+  STA_REQUIRE(!overflow, "the frame has more ORB candidates or keypoints than the detector holds");
+  const int n = static_cast<int>(d->pinned[0]);
+  n_out[0] = n;
+  n_out[1] = static_cast<int>(d->pinned[1]);
+  for (int k = 0; k < n && k < cap; ++k) {
+    js_out[k] = d->pinned[2 + 2 * k];
+    memcpy(&sims_out[k], &d->pinned[3 + 2 * k], sizeof(double));
+  }
+  return 0;
+}
+
+// Host copy of view `view`'s vector (synchronises): *len_out = -1 for None; up to cap entries are written.
+int sta_loop_view(StaLoopDetector* d, int view, int32_t* words_out, double* vals_out, int cap, int* len_out, void* stream) {
+  STA_REQUIRE(d && view >= 0 && view < d->views, "view out of range");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  int len;
+  long long start;
+  STA_CHECK_CUDA(cudaMemcpyAsync(&len, d->db_len + view, sizeof(int), cudaMemcpyDeviceToHost, st));
+  STA_CHECK_CUDA(cudaMemcpyAsync(&start, d->db_start + view, sizeof(long long), cudaMemcpyDeviceToHost, st));
+  STA_CHECK_CUDA(cudaStreamSynchronize(st));
+  *len_out = len;
+  const int m = len < cap ? len : cap;
+  if (m > 0) {
+    STA_CHECK_CUDA(cudaMemcpyAsync(words_out, d->db_word + start, sizeof(int) * m, cudaMemcpyDeviceToHost, st));
+    STA_CHECK_CUDA(cudaMemcpyAsync(vals_out, d->db_val + start, sizeof(double) * m, cudaMemcpyDeviceToHost, st));
+    STA_CHECK_CUDA(cudaStreamSynchronize(st));
+  }
+  return 0;
+}
+
+// Host copy of the similarity row of the last sta_loop_detect (NaN where a vector is None); n = view index.
+int sta_loop_similarities(StaLoopDetector* d, double* sims_out, int n, void* stream) {
+  STA_REQUIRE(d && n >= 0 && n < d->views, "bad count");
+  if (n == 0) return 0;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  STA_CHECK_CUDA(cudaMemcpyAsync(sims_out, d->sims, sizeof(double) * n, cudaMemcpyDeviceToHost, st));
+  STA_CHECK_CUDA(cudaStreamSynchronize(st));
+  return 0;
+}
+
+}  // extern "C"
