@@ -185,7 +185,8 @@ int sta_regress_pairs(StaModel* m, const float* feat_i_dev, const float* feat_j_
  * and _finish runs the DPT heads + pointmap consumers only for the n_sel surviving edges edge_idx_host[0..n_sel)
  * (indices into the K candidates; host memory).  Outputs of _finish are compact: pts3d_out [2][n_sel][H][W][3],
  * conf_out [2][n_sel][H][W], intri_out [n_sel][3][3], depth_out / conf_mean_out optional, scratch for V = 2 n_sel.
- * No other call on this handle may come between the two phases. */
+ * _begin records its shape and where it left the hooks in the handle.  Any other model call on this handle ends the
+ * pair: a later _finish is then refused with an error, before any launch. */
 int sta_regress_pairs_begin(StaModel* m, const float* feat_i_dev, const float* feat_j_dev, int K, int H, int W,
                             float* pose_out_dev, float* pose_conf_out_dev, void* stream);
 int sta_regress_pairs_finish(StaModel* m, const int* edge_idx_host, int n_sel, float* pts3d_out_dev, float* conf_out_dev,

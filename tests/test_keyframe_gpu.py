@@ -155,3 +155,40 @@ def test_gated_keyframe_step_keeps_the_reference_early_out(cuda_model):
     out = kf.regress_views_gated(i, js, -1.0)
     for e in range(4):
         assert torch.equal(out[e][2], full["conf"][:, e]) and torch.equal(out[e][4], full["depths"][:, e])
+
+
+def test_gated_finish_after_another_call_is_refused(cuda_model):
+    """sta_regress_pairs_finish reads the decoder hooks _begin left in the workspace.  An encode of the same image size
+    in between carves that workspace again (without reallocating it), so _finish must refuse instead of running the DPT
+    heads on overwritten hooks."""
+    import ctypes
+    from vista_slam_b200 import _lib
+    from vista_slam_b200.keyframe import KeyframeFrontend
+    H, W = 64, 80
+    imgs, _ = make_images(3, H, W, 7)
+    ts = torch.tensor([[H, W]])
+    kf = KeyframeFrontend(cuda_model)
+    for b in range(3):
+        kf.add_view(imgs[b:b + 1].cuda(), ts)
+    L, h = _lib.lib(), cuda_model._handle
+    f32 = dict(device="cuda", dtype=torch.float32)
+    fi, fj = torch.cat(kf.enc_features[:2]), torch.cat(kf.enc_features[1:])
+    pose, pconf = torch.empty(2, 2, 4, 4, **f32), torch.empty(2, 2, **f32)
+    pts, conf = torch.empty(2, 2, H, W, 3, **f32), torch.empty(2, 2, H, W, **f32)
+    idx = (ctypes.c_int * 2)(0, 1)
+
+    def begin():
+        _lib.check(L.sta_regress_pairs_begin(h, _lib.ptr(fi), _lib.ptr(fj), 2, H, W, _lib.ptr(pose), _lib.ptr(pconf),
+                                             _lib.cur_stream()), "sta_regress_pairs_begin")
+
+    def finish():
+        return L.sta_regress_pairs_finish(h, idx, 2, _lib.ptr(pts), _lib.ptr(conf), None, None, None, None,
+                                          _lib.cur_stream())
+
+    begin()
+    assert finish() == 0
+    begin()
+    cuda_model._encode_image(imgs[:1].cuda(), ts, normalize=False)
+    with pytest.raises(RuntimeError, match="sta_regress_pairs_begin"):
+        _lib.check(finish(), "sta_regress_pairs_finish")
+    torch.cuda.synchronize()

@@ -150,19 +150,37 @@ struct Slot {
 };
 
 struct Workspace {
-  char* base = nullptr;
+  char* base = nullptr;  // null: a dry run that only counts bytes (ws_need)
   size_t bytes = 0;
   size_t off = 0;
-  int nimg = 0, h = 0, w = 0;
+  bool overflow = false;  // a take went past `bytes`: the entry point refuses before its first launch (check_ws)
   int bmul = 1;  // bf16 activations are 3x wide in split-precision mode
   template <typename T>
   T* take(size_t n) {
     off = (off + 255) & ~static_cast<size_t>(255);
-    T* p = reinterpret_cast<T*>(base + off);
+    T* p = base ? reinterpret_cast<T*>(base + off) : nullptr;
     off += n * sizeof(T);
+    if (off > bytes) overflow = true;
     return p;
   }
   bf16* takeb(size_t n) { return take<bf16>(n * bmul); }  // bf16 activation buffer with n LOGICAL elements
+};
+
+struct EncBufs {
+  bf16 *patches, *lnb, *qkv, *att, *hid;
+  int* pos;
+};
+struct DecBufs {
+  float* xd;
+  bf16 *ln1, *lny, *qkv, *att, *qc, *kvc, *hid;
+  bf16* hook[4];  // the DPT hooks (dpt_head.py:112): bf16 encoder features (the decoder input), decoder outputs 6, 9, 12
+  int* pos;
+};
+struct DptBufs {
+  bf16 *a0, *l1, *a1, *l2, *l3, *a3, *col4, *l4;
+  bf16 *r_raw[4], *r_relu[4];
+  bf16 *t1, *t2, *s_raw, *s_relu, *o, *up, *path;  // sized for the largest level
+  bf16 *hc1, *hup;
 };
 
 }  // namespace sta
@@ -207,7 +225,9 @@ struct StaModel {
               ev_start = nullptr;
   int64_t launches = 0;
   int max_pairs_per_chunk = 16;
-  int rp_K = 0, rp_H = 0, rp_W = 0;  // state between sta_regress_pairs_begin and _finish
+  // What sta_regress_pairs_begin leaves for _finish (K = 0: nothing): the shape, the decoder buffers holding the hooks and
+  // the workspace offset past _begin's buffers.  Every other model entry point clears it (check_ready).
+  struct PairsBegun { int K = 0, H = 0, W = 0; DecBufs d = {}; size_t ws_off = 0; } rp;
   // The handle owns ONE workspace / io buffer / graph set: calls are ordered on whatever stream they are given.  When the
   // caller switches streams, the new stream first waits for the work this handle enqueued on the previous one.
   cudaStream_t last_stream = nullptr;
@@ -538,50 +558,132 @@ int attn(const Ctx& c, const bf16* q, long long ldq, int qc, const bf16* k, long
   } while (0)
 
 // ---------------------------------------------------------------------------
-// workspace
+// workspace: every entry point carves its buffers with the take functions below before its first launch, and
+// ws_need sizes the allocation by a dry run of the same functions
 // ---------------------------------------------------------------------------
-struct EncBufs {
-  bf16 *patches, *lnb, *qkv, *att, *hid;
-  int* pos;
-};
-struct DecBufs {
-  float* xd;
-  bf16 *enc_bf16, *ln1, *lny, *qkv, *att, *qc, *kvc, *hid, *hook[3];
-  int* pos;
-};
-struct DptBufs {
-  bf16 *a0, *l1, *a1, *l2, *l3, *a3, *col4, *l4;
-  bf16 *r_raw[4], *r_relu[4];
-  bf16 *t1, *t2, *s_raw, *s_relu, *o, *up, *path;  // sized for the largest level
-  bf16 *hc1, *hup;
+EncBufs take_enc(Workspace& ws, int nimg, int N) {
+  const size_t T = static_cast<size_t>(nimg) * N;
+  EncBufs e;
+  e.patches = ws.takeb(T * 768);
+  e.lnb = ws.takeb(T * 1024);
+  e.qkv = ws.takeb(T * 3072);
+  e.att = ws.takeb(T * 1024);
+  e.hid = ws.takeb(T * 4096);
+  e.pos = ws.take<int>(T * 2);
+  return e;
+}
+// The DPT head's four token inputs for nimg images of N tokens: [nimg*N][1024 | 768 | 768 | 768]
+void take_hooks(Workspace& ws, int nimg, int N, bf16* hook[4]) {
+  const size_t T = static_cast<size_t>(nimg) * N;
+  hook[0] = ws.takeb(T * 1024);
+  for (int q = 1; q < 4; ++q) hook[q] = ws.takeb(T * 768);
+}
+DecBufs take_dec(Workspace& ws, int S, int N) {
+  const size_t Td = static_cast<size_t>(S) * (N + 1);
+  DecBufs d;
+  d.xd = ws.take<float>(Td * 768);
+  d.ln1 = ws.takeb(Td * 768);
+  d.lny = ws.takeb(Td * 768);
+  d.qkv = ws.takeb(Td * 2304);
+  d.att = ws.takeb(Td * 768);
+  d.qc = ws.takeb(Td * 768);
+  d.kvc = ws.takeb(Td * 1536);
+  d.hid = ws.takeb(Td * 3072);
+  take_hooks(ws, S, N, d.hook);
+  d.pos = ws.take<int>(Td * 2);
+  return d;
+}
+// DPT head over up to nimg images of an h x w token grid
+DptBufs take_dpt(Workspace& ws, int nimg, int h, int w) {
+  const size_t N = static_cast<size_t>(h) * w, T = nimg * N;
+  const size_t h4 = (h + 1) / 2, w4 = (w + 1) / 2;
+  const size_t LP[4] = {16 * N, 4 * N, N, h4 * w4};  // pixels per image of the four levels
+  DptBufs b;
+  b.a0 = ws.takeb(T * 128);
+  b.l1 = ws.takeb(nimg * LP[0] * 128);
+  b.a1 = ws.takeb(T * 192);
+  b.l2 = ws.takeb(nimg * LP[1] * 192);
+  b.l3 = ws.takeb(T * 384);
+  b.a3 = ws.takeb(T * 768);
+  b.col4 = ws.takeb(nimg * LP[3] * 6912);
+  b.l4 = ws.takeb(nimg * LP[3] * 768);
+  for (int i = 0; i < 4; ++i) {
+    b.r_raw[i] = ws.takeb(nimg * LP[i] * 256);
+    b.r_relu[i] = ws.takeb(nimg * LP[i] * 256);
+  }
+  const size_t big = nimg * LP[0] * 256;
+  b.t1 = ws.takeb(big);
+  b.t2 = ws.takeb(big);
+  b.s_raw = ws.takeb(big);
+  b.s_relu = ws.takeb(big);
+  b.o = ws.takeb(big);
+  b.up = ws.takeb(nimg * 64 * N * 256);    // up, path: up to 8h x 8w
+  b.path = ws.takeb(nimg * 64 * N * 256);
+  b.hc1 = ws.takeb(nimg * 64 * N * 128);
+  b.hup = ws.takeb(nimg * 256 * N * 128);  // full resolution
+  return b;
+}
+
+// Staging rule of the graphed entry points: a graphed body may only touch memory whose address is a function of its
+// graph key (run_graphed), so it writes workspace buffers, which flush() copies to the caller's tensors after the
+// replay.  An eager body writes the caller's tensors directly and there is nothing to copy.  An output the caller did
+// not ask for (null) stays null.
+struct Staging {
+  Workspace& ws;
+  bool graphed;
+  struct Copy { float* user; const float* staged; size_t n; };
+  std::vector<Copy> copies;
+  float* out(float* user, size_t n) {  // the buffer a body writes for the caller's user[0, n)
+    if (!graphed || !user) return user;
+    float* p = ws.take<float>(n);
+    copies.push_back({user, p, n});
+    return p;
+  }
+  int flush(cudaStream_t st) const {
+    for (const Copy& c : copies)
+      STA_CHECK_CUDA(cudaMemcpyAsync(c.user, c.staged, c.n * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    return 0;
+  }
 };
 
-size_t ws_need(int nimg, int h, int w, int bmul = 1) {
-  if (bmul > 1) return ws_need(nimg, h, w) * bmul;  // split-precision mode: bf16 buffers are 3x wide (fp32 ones over-counted)
-  const size_t N = static_cast<size_t>(h) * w, T = nimg * N, Td = nimg * (N + 1);
-  size_t b = 0;
-  auto add = [&](size_t n) { b += ((n + 255) / 256) * 256 + 256; };
-  // encoder
-  add(T * 768 * 2); add(T * 1024 * 2); add(T * 3072 * 2); add(T * 1024 * 2); add(T * 4096 * 2); add(T * 8);
-  add(T * 1024 * 4);  // x (fp32 residual stream)
-  // decoder
-  add(Td * 768 * 4); add(T * 1024 * 2); add(Td * 768 * 2 * 2); add(Td * 2304 * 2); add(Td * 768 * 2 * 2);
-  add(Td * 1536 * 2); add(Td * 3072 * 2); add(T * 768 * 2 * 3); add(Td * 8);
-  // dpt
-  const size_t h4 = (h + 1) / 2, w4 = (w + 1) / 2;
-  const size_t P1 = 16 * N, P2 = 4 * N, P3 = N, P4 = h4 * w4;
-  add(T * 128 * 2); add(nimg * P1 * 128 * 2); add(T * 192 * 2); add(nimg * P2 * 192 * 2); add(T * 384 * 2);
-  add(T * 768 * 2); add(nimg * P4 * 6912 * 2); add(nimg * P4 * 768 * 2);
-  const size_t P[4] = {P1, P2, P3, P4};
-  for (int i = 0; i < 4; ++i) { add(nimg * P[i] * 256 * 2); add(nimg * P[i] * 256 * 2); }
-  for (int i = 0; i < 5; ++i) add(nimg * P1 * 256 * 2);       // t1, t2, s_raw, s_relu, o
-  add(nimg * 64 * N * 256 * 2); add(nimg * 64 * N * 256 * 2);  // up, path (up to 8h x 8w)
-  add(nimg * 64 * N * 128 * 2); add(nimg * 256 * N * 128 * 2); // hc1, hup (full res)
-  // static outputs of the graph-replayed keyframe step: pts3d, conf, depth (fp32, full res), poses, K, reduction scratch
-  add(nimg * 256 * N * 5 * 4); add(nimg * 32 * 4); add(pointmap_scratch_bytes(nimg));
-  // gated keyframe step: compact copies of the surviving edges' hooks (sta_regress_pairs_finish)
-  add(T * 1024 * 2); add(T * 768 * 2 * 3); add(nimg * 32 * 4);
-  return b + (1 << 20);
+// Outputs of the keyframe step for n edges, [view][edge] (view 0 = the i -> j direction): the DPT pointmaps and
+// confidences, then what the pointmap consumers write and their scratch.  Null: not asked for.
+struct PairOuts {
+  float *pts, *conf, *intri, *depth, *cmean;
+  void* scratch;
+};
+PairOuts stage_pair_outs(Staging& s, const PairOuts& u, int n, long long px) {
+  const size_t V = 2 * static_cast<size_t>(n);
+  PairOuts o;
+  o.pts = s.out(u.pts, V * px * 3);
+  o.conf = s.out(u.conf, V * px);
+  o.intri = s.out(u.intri, static_cast<size_t>(n) * 9);
+  o.depth = s.out(u.depth, V * px);
+  o.cmean = s.out(u.cmean, V);
+  o.scratch = s.graphed && u.intri ? s.ws.take<double>(pointmap_scratch_bytes(V) / sizeof(double)) : u.scratch;
+  return o;
+}
+
+// Workspace bytes for nimg images of an h x w token grid: a dry run of the take functions.  The envelope covers every
+// entry point: encoder + fp32 residual stream + decoder + DPT head (sta_forward_pairs), and on top of the decoder the
+// keyframe step's staged poses (_begin), compact hook copies and staged outputs (_finish with every edge kept and every
+// output asked for).
+size_t ws_need(int nimg, int h, int w, int bmul) {
+  Workspace dry;
+  dry.bmul = bmul;
+  const int N = h * w;
+  float any;  // stands for a caller's tensor: staging only asks whether there is one
+  bf16* hook[4];
+  take_enc(dry, nimg, N);
+  dry.take<float>(static_cast<size_t>(nimg) * N * kEncDim);
+  take_dec(dry, nimg, N);
+  take_dpt(dry, nimg, h, w);
+  Staging staged{dry, true};
+  staged.out(&any, static_cast<size_t>(nimg) * 16);
+  staged.out(&any, nimg);
+  take_hooks(dry, nimg, N, hook);
+  stage_pair_outs(staged, {&any, &any, &any, &any, &any, &any}, nimg / 2, 256LL * N);
+  return dry.off;
 }
 
 void drop_graphs(StaModel* m);
@@ -599,9 +701,11 @@ int ensure_ws(StaModel* m, int nimg, int h, int w) {
     m->ws.bytes = need;
   }
   m->ws.off = 0;
-  m->ws.nimg = nimg;
-  m->ws.h = h;
-  m->ws.w = w;
+  m->ws.overflow = false;
+  return 0;
+}
+int check_ws(const Workspace& ws) {
+  STA_REQUIRE(!ws.overflow, "internal: the workspace is smaller than the buffers this call carves");
   return 0;
 }
 
@@ -612,7 +716,8 @@ int ensure_ws(StaModel* m, int nimg, int h, int w) {
 // stream -- the caller's may be the legacy default stream -- with the programmatic-dependent-launch edges kept) and
 // replays the instantiated graph on the caller's stream from then on.  `body` must only touch memory whose
 // addresses are a function of the key (workspace offsets for that shape, weights): user pointers are handled by
-// the caller outside the graph.  Graphs die with the workspace they point into.
+// the caller outside the graph (Staging).  Graphs die with the workspace they point into.  Sizes that are not
+// launch-bound (`graphed` false) always run eagerly.
 // ---------------------------------------------------------------------------
 constexpr long long kGraphMaxTokens = 8192;  // only launch-bound problem sizes
 
@@ -623,8 +728,8 @@ void drop_graphs(StaModel* m) {
 }
 
 template <typename Body>
-int run_graphed(StaModel* m, cudaStream_t st, const std::vector<long long>& key, Body&& body) {
-  if (m->prof_on) return body(Ctx{m, st});  // per-kernel timing events need eager launches
+int run_graphed(StaModel* m, cudaStream_t st, bool graphed, const std::vector<long long>& key, Body&& body) {
+  if (!graphed || m->prof_on) return body(Ctx{m, st});  // per-kernel timing events need eager launches
   StaModel::GraphEntry* ent = nullptr;
   for (auto& g : m->graphs)
     if (g.key == key) ent = &g;
@@ -689,37 +794,9 @@ int run_encoder(const Ctx& c, int nimg, int N, float* x, EncBufs& e) {
   return 0;
 }
 
-EncBufs take_enc(Workspace& ws, int nimg, int N) {
-  const size_t T = static_cast<size_t>(nimg) * N;
-  EncBufs e;
-  e.patches = ws.takeb(T * 768);
-  e.lnb = ws.takeb(T * 1024);
-  e.qkv = ws.takeb(T * 3072);
-  e.att = ws.takeb(T * 1024);
-  e.hid = ws.takeb(T * 4096);
-  e.pos = ws.take<int>(T * 2);
-  return e;
-}
-DecBufs take_dec(Workspace& ws, int S, int N) {
-  const size_t T = static_cast<size_t>(S) * N, Td = static_cast<size_t>(S) * (N + 1);
-  DecBufs d;
-  d.xd = ws.take<float>(Td * 768);
-  d.enc_bf16 = ws.takeb(T * 1024);
-  d.ln1 = ws.takeb(Td * 768);
-  d.lny = ws.takeb(Td * 768);
-  d.qkv = ws.takeb(Td * 2304);
-  d.att = ws.takeb(Td * 768);
-  d.qc = ws.takeb(Td * 768);
-  d.kvc = ws.takeb(Td * 1536);
-  d.hid = ws.takeb(Td * 3072);
-  for (int i = 0; i < 3; ++i) d.hook[i] = ws.takeb(T * 768);
-  d.pos = ws.take<int>(Td * 2);
-  return d;
-}
-
 // ---------------------------------------------------------------------------
 // symmetric decoder over S = 2B samples (samples [0,B) = view 1, [B,2B) = view 2).
-// d.enc_bf16 (bf16 encoder features of all S samples) and d.pos must be filled.
+// d.hook[0] (bf16 encoder features of all S samples) and d.pos must be filled.
 // outs: optional 2 x 13 fp32 per-layer outputs (compat path), may be null.
 // ---------------------------------------------------------------------------
 int run_decoder(const Ctx& c, int B, int N, DecBufs& d, float* const* out1, float* const* out2) {
@@ -731,7 +808,7 @@ int run_decoder(const Ctx& c, int B, int N, DecBufs& d, float* const* out1, floa
     if (out2 && out2[idx]) { m->launches++; RUN(launch_copy_f32(d.xd + half, out2[idx], half, c.st)); }
     return 0;
   };
-  RUN(linear(c, EPI_F32, d.enc_bf16, T, m->dec_embed, d.xd, nullptr, nullptr, 0, N));
+  RUN(linear(c, EPI_F32, d.hook[0], T, m->dec_embed, d.xd, nullptr, nullptr, 0, N));
   m->launches++;
   RUN(launch_fill_pose_token(d.xd, m->pose_tok, S, M, kDecDim, c.st));
   RUN(emit(0));
@@ -756,12 +833,12 @@ int run_decoder(const Ctx& c, int B, int N, DecBufs& d, float* const* out1, floa
     RUN(linear(c, EPI_F32, d.hid, Td, b.fc2, d.xd, d.xd));
     if (l + 1 == 6 || l + 1 == 9) {  // DPT hooks [0, 7, 10, 13] -> decoder outputs 6, 9, 12 (dpt_head.py:112)
       m->launches++;
-      RUN(launch_cast_f32_bf16(d.xd, d.hook[l + 1 == 6 ? 0 : 1], Td, kDecDim, M, c.st, m->split));
+      RUN(launch_cast_f32_bf16(d.xd, d.hook[l + 1 == 6 ? 1 : 2], Td, kDecDim, M, c.st, m->split));
     }
     if (l + 1 < 12) RUN(emit(l + 1));
   }
   // dec_norm on the last output; bf16 copy without the pose token feeds the DPT head
-  RUN(ln(c, d.xd, Td, kDecDim, m->dec_norm, d.hook[2], nullptr, nullptr, M));
+  RUN(ln(c, d.xd, Td, kDecDim, m->dec_norm, d.hook[3], nullptr, nullptr, M));
   if ((out1 && out1[12]) || (out2 && out2[12])) {
     // compat path: fp32 LayerNorm-ed last layer
     const int rows_half = B * M;
@@ -780,38 +857,40 @@ int run_decoder(const Ctx& c, int B, int N, DecBufs& d, float* const* out1, floa
   return 0;
 }
 
+// bf16 decoder input of B feature pairs: the B view-1 samples, then the B view-2 samples
+int cast_features(const Ctx& c, const float* feat1, const float* feat2, int B, int N, DecBufs& d) {
+  const long long T = static_cast<long long>(B) * N;
+  c.m->launches += 2;
+  RUN(launch_cast_f32_bf16(feat1, d.hook[0], T, kEncDim, 0, c.st, c.m->split));
+  return launch_cast_f32_bf16(feat2, d.hook[0] + T * kEncDim * c.m->bmul(), T, kEncDim, 0, c.st, c.m->split);
+}
+
+// Decoder positions, the symmetric decoder over 2B samples (d.hook[0] must be filled) and the pose heads on the
+// dec_norm-ed pose tokens of both views: view 1 into pose / pose_conf, view 2 `view_stride` entries further.
+int decode_with_poses(const Ctx& c, int B, int h, int w, DecBufs& d, float* pose, float* pose_conf, int view_stride) {
+  StaModel* m = c.m;
+  const long long rows = static_cast<long long>(h * w + 1) * kDecDim;  // decoder rows of one sample
+  m->launches += 3;
+  RUN(launch_make_positions(d.pos, 2 * B, h, w, 1, c.st));
+  RUN(run_decoder(c, B, h * w, d, nullptr, nullptr));
+  RUN(launch_pose_head(d.xd, rows, B, 1, kLnEps, m->pose, pose, pose_conf, c.st));
+  return launch_pose_head(d.xd + B * rows, rows, B, 1, kLnEps, m->pose, pose + static_cast<long long>(view_stride) * 16,
+                          pose_conf + view_stride, c.st);
+}
+
 // ---------------------------------------------------------------------------
-// DPT head over nimg images.  hooks: bf16 token matrices [nimg*N][1024 | 768 | 768 | 768].
+// DPT head over images [first, first + nimg) of the four bf16 token inputs hook[q] ([images * N][1024 | 768 | 768 |
+// 768], take_hooks), into pts3d / conf (the outputs of those nimg images).  b: take_dpt for at least nimg images.
 // ---------------------------------------------------------------------------
-int run_dpt(const Ctx& c, Workspace& ws, int nimg, int h, int w, const bf16* hook0, const bf16* hook1,
-            const bf16* hook2, const bf16* hook3, float* pts3d, float* conf) {
+int run_dpt(const Ctx& c, const DptBufs& b, int h, int w, const bf16* const hook[4], int first, int nimg, float* pts3d,
+            float* conf) {
   StaModel* m = c.m;
   const int N = h * w, T = nimg * N;
   const int h4 = (h + 1) / 2, w4 = (w + 1) / 2;
   const int LH[4] = {4 * h, 2 * h, h, h4}, LW[4] = {4 * w, 2 * w, w, w4};
-  DptBufs b;
-  b.a0 = ws.takeb(static_cast<size_t>(T) * 128);
-  b.l1 = ws.takeb(static_cast<size_t>(nimg) * 16 * N * 128);
-  b.a1 = ws.takeb(static_cast<size_t>(T) * 192);
-  b.l2 = ws.takeb(static_cast<size_t>(nimg) * 4 * N * 192);
-  b.l3 = ws.takeb(static_cast<size_t>(T) * 384);
-  b.a3 = ws.takeb(static_cast<size_t>(T) * 768);
-  b.col4 = ws.takeb(static_cast<size_t>(nimg) * h4 * w4 * 6912);
-  b.l4 = ws.takeb(static_cast<size_t>(nimg) * h4 * w4 * 768);
-  for (int i = 0; i < 4; ++i) {
-    b.r_raw[i] = ws.takeb(static_cast<size_t>(nimg) * LH[i] * LW[i] * 256);
-    b.r_relu[i] = ws.takeb(static_cast<size_t>(nimg) * LH[i] * LW[i] * 256);
-  }
-  const size_t big = static_cast<size_t>(nimg) * 16 * N * 256;
-  b.t1 = ws.takeb(big);
-  b.t2 = ws.takeb(big);
-  b.s_raw = ws.takeb(big);
-  b.s_relu = ws.takeb(big);
-  b.o = ws.takeb(big);
-  b.up = ws.takeb(static_cast<size_t>(nimg) * 64 * N * 256);
-  b.path = ws.takeb(static_cast<size_t>(nimg) * 64 * N * 256);
-  b.hc1 = ws.takeb(static_cast<size_t>(nimg) * 64 * N * 128);
-  b.hup = ws.takeb(static_cast<size_t>(nimg) * 256 * N * 128);
+  const size_t tok0 = static_cast<size_t>(first) * N * m->bmul();  // first token row, times the bf16 row width factor
+  const bf16 *hook0 = hook[0] + tok0 * 1024, *hook1 = hook[1] + tok0 * 768, *hook2 = hook[2] + tok0 * 768,
+             *hook3 = hook[3] + tok0 * 768;
 
   // ---- act_postprocess (dpt_block.py:356-410) ----
   RUN(linear(c, EPI_BF16, hook0, T, m->act0, b.a0));
@@ -882,11 +961,14 @@ int run_dpt(const Ctx& c, Workspace& ws, int nimg, int h, int w, const bf16* hoo
   return 0;
 }
 
-int check_ready(StaModel* m) {
+// Every model entry point starts here.  All but sta_regress_pairs_finish end a begin/finish pair: they may carve the
+// workspace that holds _begin's decoder hooks again.
+int check_ready(StaModel* m, bool finishing_pairs = false) {
   if (!m) {
     set_last_error("null model handle");
     return 2;
   }
+  if (!finishing_pairs) m->rp = {};
   if (m->missing != 0) {
     char buf[128];
     snprintf(buf, sizeof(buf), "model is missing %d state-dict tensors", m->missing);
@@ -894,6 +976,34 @@ int check_ready(StaModel* m) {
     return 2;
   }
   return 0;
+}
+// B images of positive multiples of the 16-pixel patch, whose token grid fits the RoPE table
+int check_grid(int B, int H, int W) {
+  STA_REQUIRE(B > 0 && H % 16 == 0 && W % 16 == 0 && H > 0 && W > 0, "image size must be a positive multiple of 16");
+  STA_REQUIRE(H / 16 <= 1024 && W / 16 <= 1024, "token grid exceeds the RoPE table");
+  return 0;
+}
+int check_edges(const StaModel* m, int K) {
+  STA_REQUIRE(K > 0 && K <= m->max_pairs_per_chunk, "edge batch must be in [1, 16]");
+  return 0;
+}
+// The pointmap consumers run when any of their outputs is asked for; they then need the scratch buffer and intri_out.
+int check_consumers(const void* scratch, const float* intri_out, const float* depth_out, const float* conf_mean_out) {
+  if (intri_out || depth_out || conf_mean_out)
+    STA_REQUIRE(scratch != nullptr && intri_out != nullptr,
+                "the pointmap consumers need the scratch buffer and intri_out (depth_out / conf_mean_out are optional)");
+  return 0;
+}
+
+// The keyframe step after the decoder, for n edges whose token inputs hold [view][edge] images: the DPT head on each
+// view, then the pointmap consumers if they were asked for (o.intri is set exactly then, check_consumers).
+int pair_heads(const Ctx& c, const DptBufs& b, const bf16* const hook[4], int n, int H, int W, const PairOuts& o) {
+  const long long px = static_cast<long long>(H) * W;
+  for (int v = 0; v < 2; ++v)
+    RUN(run_dpt(c, b, H / 16, W / 16, hook, v * n, n, o.pts + v * n * px * 3, o.conf + v * n * px));
+  if (!o.intri) return 0;
+  c.m->launches += 2;
+  return launch_pointmap_consumers(o.pts, o.conf, 2 * n, H, W, 2, o.intri, o.depth, o.cmean, o.scratch, c.st);
 }
 
 // DPT parts per view in the host entry point: two halves, so that the device-to-host copy of the first half overlaps
@@ -916,12 +1026,14 @@ int forward_chunk(const Ctx& c, const void* img1, const void* img2, int img_is_b
                   float* pts3d, float* conf, float* pose, float* pose_conf, int B_total,
                   cudaEvent_t* ev_parts = nullptr) {
   StaModel* m = c.m;
-  const int h = H / 16, w = W / 16, N = h * w, S = 2 * B, M = N + 1;
+  const int h = H / 16, w = W / 16, N = h * w, S = 2 * B;
   RUN(ensure_ws(m, S, h, w));
   Workspace& ws = m->ws;
   float* x = ws.take<float>(static_cast<size_t>(S) * N * kEncDim);
   EncBufs e = take_enc(ws, S, N);
   DecBufs d = take_dec(ws, S, N);
+  const DptBufs dpt = take_dpt(ws, B, h, w);  // one view; the parts of the host entry point reuse it
+  RUN(check_ws(ws));
   // encode both views as one batch of 2B images: [view 1 batch ; view 2 batch]
   m->launches += 3;
   const size_t bm = m->bmul();  // physical / logical width of the bf16 activation rows
@@ -929,18 +1041,10 @@ int forward_chunk(const Ctx& c, const void* img1, const void* img2, int img_is_b
   RUN(launch_patch_im2col(img2, img_is_bf16, B, H, W, e.patches + static_cast<size_t>(B) * N * 768 * bm, c.st, m->split));
   RUN(launch_make_positions(e.pos, S, h, w, 0, c.st));
   RUN(run_encoder(c, S, N, x, e));
-  m->launches += 2;
-  RUN(launch_cast_f32_bf16(x, d.enc_bf16, static_cast<long long>(S) * N, kEncDim, 0, c.st, m->split));
-  RUN(launch_make_positions(d.pos, S, h, w, 1, c.st));
-  RUN(run_decoder(c, B, N, d, nullptr, nullptr));
-  // pose heads on the (dec_norm-ed) pose tokens of both views
-  {
-    // outputs are laid out [2][B_total]: view 1 block then view 2 block
-    m->launches += 2;
-    RUN(launch_pose_head(d.xd, static_cast<long long>(M) * kDecDim, B, 1, kLnEps, m->pose, pose, pose_conf, c.st));
-    RUN(launch_pose_head(d.xd + static_cast<long long>(B) * M * kDecDim, static_cast<long long>(M) * kDecDim, B, 1,
-                         kLnEps, m->pose, pose + static_cast<long long>(B_total) * 16, pose_conf + B_total, c.st));
-  }
+  m->launches += 1;
+  RUN(launch_cast_f32_bf16(x, d.hook[0], static_cast<long long>(S) * N, kEncDim, 0, c.st, m->split));
+  // pose outputs are laid out [2][B_total]: view 1 block then view 2 block
+  RUN(decode_with_poses(c, B, h, w, d, pose, pose_conf, B_total));
   // DPT heads: view 1 images then view 2 images (outputs are [2][B_total] blocks).  The host entry point passes events:
   // each view is then processed in `halves` parts (host_dpt_parts) and an event is recorded after every part, so that the
   // D2H copy of one part runs under the head of the next and only the last quarter of the outputs is exposed.
@@ -949,12 +1053,8 @@ int forward_chunk(const Ctx& c, const void* img1, const void* img2, int img_is_b
   for (int v = 0; v < 2; ++v) {
     for (int hf = 0; hf < halves; ++hf) {
       const int i0 = hf * (B / halves), nb = (hf == halves - 1) ? B - i0 : B / halves;
-      const size_t save = ws.off;
-      const size_t tok0 = (static_cast<size_t>(v) * B + i0) * N;
-      RUN(run_dpt(c, ws, nb, h, w, d.enc_bf16 + tok0 * 1024 * bm, d.hook[0] + tok0 * 768 * bm, d.hook[1] + tok0 * 768 * bm,
-                  d.hook[2] + tok0 * 768 * bm, pts3d + (static_cast<long long>(v) * B_total + i0) * px * 3,
-                  conf + (static_cast<long long>(v) * B_total + i0) * px));
-      ws.off = save;
+      const long long o = static_cast<long long>(v) * B_total + i0;
+      RUN(run_dpt(c, dpt, h, w, d.hook, v * B + i0, nb, pts3d + o * px * 3, conf + o * px));
       if (ev_parts) STA_CHECK_CUDA(cudaEventRecord(ev_parts[v * halves + hf], c.st));
     }
   }
@@ -1183,31 +1283,28 @@ int sta_load_tensor(StaModel* m, const char* name, const float* data, const int6
 int sta_encode(StaModel* m, const void* img_dev, int img_is_bf16, int B, int H, int W, float* feat_out_dev,
                int64_t* pos_out_dev, void* stream) {
   RUN(check_ready(m));
-  STA_REQUIRE(B > 0 && H % 16 == 0 && W % 16 == 0 && H > 0 && W > 0, "image size must be a positive multiple of 16");
-  STA_REQUIRE(H / 16 <= 1024 && W / 16 <= 1024, "token grid exceeds the RoPE table");
+  RUN(check_grid(B, H, W));
+  STA_REQUIRE(feat_out_dev != nullptr, "null pointer");
   Ctx c{m, static_cast<cudaStream_t>(stream)};
   RUN(enter_stream(m, c.st));
   const int h = H / 16, w = W / 16, N = h * w;
   RUN(ensure_ws(m, B, h, w));
   EncBufs e = take_enc(m->ws, B, N);
+  // launch-bound sizes: the encoder proper is replayed as a CUDA graph (staged features; the caller's tensor is
+  // long-lived: slam.py:145 keeps it for the whole run)
+  const bool graphed = static_cast<long long>(B) * N <= kGraphMaxTokens;
+  Staging staged{m->ws, graphed};
+  float* x = staged.out(feat_out_dev, static_cast<size_t>(B) * N * kEncDim);
+  RUN(check_ws(m->ws));
   m->launches += 1;
   RUN(launch_patch_im2col(img_dev, img_is_bf16, B, H, W, e.patches, c.st, m->split));
-  // launch-bound sizes: the encoder proper is replayed as a CUDA graph on workspace buffers, the features are
-  // then copied to the caller's tensor (which is long-lived: slam.py:145 keeps it for the whole run)
-  const bool graphed = static_cast<long long>(B) * N <= kGraphMaxTokens;
-  float* x = graphed ? m->ws.take<float>(static_cast<size_t>(B) * N * kEncDim) : feat_out_dev;
   auto body = [&](const Ctx& cc) -> int {
     m->launches += 1;
     RUN(launch_make_positions(e.pos, B, h, w, 0, cc.st));
     return run_encoder(cc, B, N, x, e);
   };
-  if (graphed) {
-    RUN(run_graphed(m, c.st, {1, B, H, W}, body));
-    STA_CHECK_CUDA(cudaMemcpyAsync(feat_out_dev, x, static_cast<size_t>(B) * N * kEncDim * sizeof(float),
-                                   cudaMemcpyDeviceToDevice, c.st));
-  } else {
-    RUN(body(c));
-  }
+  RUN(run_graphed(m, c.st, graphed, {1, B, H, W}, body));
+  RUN(staged.flush(c.st));
   if (pos_out_dev) {
     const long long n = 2LL * B * N;
     m->launches++;
@@ -1227,10 +1324,9 @@ int sta_decode(StaModel* m, const float* feat1_dev, const float* feat2_dev, cons
   // workspace sized as an (N x 1) token grid: only token counts matter for the decoder buffers
   RUN(ensure_ws(m, 2 * B, N, 1));
   DecBufs d = take_dec(m->ws, 2 * B, N);
-  m->launches += 3;
-  RUN(launch_cast_f32_bf16(feat1_dev, d.enc_bf16, static_cast<long long>(B) * N, kEncDim, 0, c.st, m->split));
-  RUN(launch_cast_f32_bf16(feat2_dev, d.enc_bf16 + static_cast<size_t>(B) * N * kEncDim * m->bmul(),
-                           static_cast<long long>(B) * N, kEncDim, 0, c.st, m->split));
+  RUN(check_ws(m->ws));
+  RUN(cast_features(c, feat1_dev, feat2_dev, B, N, d));
+  m->launches++;
   {
     const long long total = 2LL * B * (N + 1);
     build_dec_pos_kernel<<<static_cast<int>((total + 255) / 256), 256, 0, c.st>>>(
@@ -1257,17 +1353,15 @@ int sta_head_pts(StaModel* m, const float* enc_feat_dev, const float* dec6_dev, 
   const int h = H / 16, w = W / 16, N = h * w;
   RUN(ensure_ws(m, B, h, w));
   Workspace& ws = m->ws;
-  const size_t T = static_cast<size_t>(B) * N;
-  bf16* k0 = ws.takeb(T * 1024);
-  bf16* k1 = ws.takeb(T * 768);
-  bf16* k2 = ws.takeb(T * 768);
-  bf16* k3 = ws.takeb(T * 768);
+  bf16* hook[4];
+  take_hooks(ws, B, N, hook);
+  const DptBufs dpt = take_dpt(ws, B, h, w);
+  RUN(check_ws(ws));
+  const float* src[4] = {enc_feat_dev, dec6_dev, dec9_dev, dec12_dev};
   m->launches += 4;
-  RUN(launch_cast_f32_bf16(enc_feat_dev, k0, T, 1024, 0, c.st, m->split));
-  RUN(launch_cast_f32_bf16(dec6_dev, k1, T, 768, 0, c.st, m->split));
-  RUN(launch_cast_f32_bf16(dec9_dev, k2, T, 768, 0, c.st, m->split));
-  RUN(launch_cast_f32_bf16(dec12_dev, k3, T, 768, 0, c.st, m->split));
-  return run_dpt(c, ws, B, h, w, k0, k1, k2, k3, pts3d_out_dev, conf_out_dev);
+  for (int q = 0; q < 4; ++q)
+    RUN(launch_cast_f32_bf16(src[q], hook[q], static_cast<long long>(B) * N, q ? 768 : 1024, 0, c.st, m->split));
+  return run_dpt(c, dpt, h, w, hook, 0, B, pts3d_out_dev, conf_out_dev);
 }
 
 int64_t sta_graph_replays(StaModel* m) { return m ? m->graph_replays : 0; }
@@ -1276,211 +1370,117 @@ int sta_regress_pairs(StaModel* m, const float* feat_i_dev, const float* feat_j_
                       float* pose_out_dev, float* pose_conf_out_dev, float* pts3d_out_dev, float* conf_out_dev,
                       float* intri_out_dev, float* depth_out_dev, float* conf_mean_out_dev, void* scratch, void* stream) {
   RUN(check_ready(m));
-  STA_REQUIRE(K > 0 && K <= m->max_pairs_per_chunk, "edge batch must be in [1, 16]");
-  STA_REQUIRE(H % 16 == 0 && W % 16 == 0 && H > 0 && W > 0, "image size must be a positive multiple of 16");
-  STA_REQUIRE(H / 16 <= 1024 && W / 16 <= 1024, "token grid exceeds the RoPE table");
+  RUN(check_edges(m, K));
+  RUN(check_grid(K, H, W));
   STA_REQUIRE(feat_i_dev && feat_j_dev && pose_out_dev && pose_conf_out_dev && pts3d_out_dev && conf_out_dev,
               "null pointer");
+  RUN(check_consumers(scratch, intri_out_dev, depth_out_dev, conf_mean_out_dev));
   Ctx c{m, static_cast<cudaStream_t>(stream)};
   RUN(enter_stream(m, c.st));
-  const int h = H / 16, w = W / 16, N = h * w, S = 2 * K, M = N + 1;
+  const int h = H / 16, w = W / 16, N = h * w, S = 2 * K;
+  const long long px = static_cast<long long>(H) * W;
   RUN(ensure_ws(m, S, h, w));
   Workspace& ws = m->ws;
   DecBufs d = take_dec(ws, S, N);
-  const bool consumers = intri_out_dev || depth_out_dev || conf_mean_out_dev;
-  if (consumers)
-    STA_REQUIRE(scratch != nullptr && intri_out_dev != nullptr,
-                "the pointmap consumers need the scratch buffer and intri_out (depth_out / conf_mean_out are optional)");
-  const long long px = static_cast<long long>(H) * W;
-  // Launch-bound sizes: everything after the input casts is replayed as a CUDA graph that writes workspace
-  // buffers; the results are then copied to the caller's tensors.  Large batches write the caller's tensors directly.
-  const bool graphed = static_cast<long long>(S) * M <= kGraphMaxTokens;
-  float *o_pose = pose_out_dev, *o_pconf = pose_conf_out_dev, *o_pts = pts3d_out_dev, *o_conf = conf_out_dev;
-  float *o_intri = intri_out_dev, *o_depth = depth_out_dev, *o_cmean = conf_mean_out_dev;
-  void* o_scratch = scratch;
-  if (graphed) {
-    o_pose = ws.take<float>(static_cast<size_t>(S) * 16);
-    o_pconf = ws.take<float>(S);
-    o_pts = ws.take<float>(static_cast<size_t>(S) * px * 3);
-    o_conf = ws.take<float>(static_cast<size_t>(S) * px);
-    if (consumers) {
-      o_intri = ws.take<float>(static_cast<size_t>(K) * 9);
-      o_depth = depth_out_dev ? ws.take<float>(static_cast<size_t>(S) * px) : nullptr;
-      o_cmean = conf_mean_out_dev ? ws.take<float>(S) : nullptr;
-      o_scratch = ws.take<double>(pointmap_scratch_bytes(S) / sizeof(double));
-    }
-  }
-  m->launches += 2;
-  const size_t bm = m->bmul();
-  RUN(launch_cast_f32_bf16(feat_i_dev, d.enc_bf16, static_cast<long long>(K) * N, kEncDim, 0, c.st, m->split));
-  RUN(launch_cast_f32_bf16(feat_j_dev, d.enc_bf16 + static_cast<size_t>(K) * N * kEncDim * bm, static_cast<long long>(K) * N,
-                           kEncDim, 0, c.st, m->split));
+  // Launch-bound sizes: decoder, pose heads, DPT heads and consumers are replayed as one CUDA graph (staged outputs).
+  const bool graphed = static_cast<long long>(S) * (N + 1) <= kGraphMaxTokens;
+  Staging staged{ws, graphed};
+  float* o_pose = staged.out(pose_out_dev, static_cast<size_t>(S) * 16);
+  float* o_pconf = staged.out(pose_conf_out_dev, S);
+  const PairOuts o =
+      stage_pair_outs(staged, {pts3d_out_dev, conf_out_dev, intri_out_dev, depth_out_dev, conf_mean_out_dev, scratch}, K, px);
+  const DptBufs dpt = take_dpt(ws, K, h, w);
+  RUN(check_ws(ws));
+  RUN(cast_features(c, feat_i_dev, feat_j_dev, K, N, d));
   auto body = [&](const Ctx& cc) -> int {
-    m->launches += 3;
-    RUN(launch_make_positions(d.pos, S, h, w, 1, cc.st));
-    RUN(run_decoder(cc, K, N, d, nullptr, nullptr));
-    RUN(launch_pose_head(d.xd, static_cast<long long>(M) * kDecDim, K, 1, kLnEps, m->pose, o_pose, o_pconf, cc.st));
-    RUN(launch_pose_head(d.xd + static_cast<long long>(K) * M * kDecDim, static_cast<long long>(M) * kDecDim, K, 1,
-                         kLnEps, m->pose, o_pose + static_cast<long long>(K) * 16, o_pconf + K, cc.st));
-    for (int v = 0; v < 2; ++v) {
-      const size_t save = ws.off;
-      const size_t tok0 = static_cast<size_t>(v) * K * N;
-      RUN(run_dpt(cc, ws, K, h, w, d.enc_bf16 + tok0 * 1024 * bm, d.hook[0] + tok0 * 768 * bm, d.hook[1] + tok0 * 768 * bm,
-                  d.hook[2] + tok0 * 768 * bm, o_pts + static_cast<long long>(v) * K * px * 3,
-                  o_conf + static_cast<long long>(v) * K * px));
-      ws.off = save;
-    }
-    if (consumers) {
-      m->launches += 2;
-      RUN(launch_pointmap_consumers(o_pts, o_conf, S, H, W, 2, o_intri, o_depth, o_cmean, o_scratch, cc.st));
-    }
-    return 0;
+    RUN(decode_with_poses(cc, K, h, w, d, o_pose, o_pconf, K));
+    return pair_heads(cc, dpt, d.hook, K, H, W, o);
   };
-  if (!graphed) return body(c);
-  RUN(run_graphed(m, c.st, {2, K, H, W, consumers ? 1 : 0, depth_out_dev ? 1 : 0, conf_mean_out_dev ? 1 : 0}, body));
-  auto copy = [&](float* dst, const float* src, size_t n) -> int {
-    if (dst) STA_CHECK_CUDA(cudaMemcpyAsync(dst, src, n * sizeof(float), cudaMemcpyDeviceToDevice, c.st));
-    return 0;
-  };
-  RUN(copy(pose_out_dev, o_pose, static_cast<size_t>(S) * 16));
-  RUN(copy(pose_conf_out_dev, o_pconf, S));
-  RUN(copy(pts3d_out_dev, o_pts, static_cast<size_t>(S) * px * 3));
-  RUN(copy(conf_out_dev, o_conf, static_cast<size_t>(S) * px));
-  if (consumers) {
-    RUN(copy(intri_out_dev, o_intri, static_cast<size_t>(K) * 9));
-    RUN(copy(depth_out_dev, o_depth, static_cast<size_t>(S) * px));
-    RUN(copy(conf_mean_out_dev, o_cmean, S));
-  }
-  return 0;
+  RUN(run_graphed(m, c.st, graphed, {2, K, H, W, intri_out_dev ? 1 : 0, depth_out_dev ? 1 : 0, conf_mean_out_dev ? 1 : 0},
+                  body));
+  return staged.flush(c.st);
 }
 
 // ---------------------------------------------------------------------------
 // Gated keyframe step (SURVEY.md 8(f) rank 1 with the early-out of slam.py:169-170): phase 1 runs the decoder and the
 // pose heads for all K candidate edges and leaves the decoder hooks in the workspace; the caller reads the K pose
 // confidences ONCE, decides which edges survive (`conf >= thres or i - j == 1`) and phase 2 runs the DPT heads and the
-// pointmap consumers for the survivors only.  Nothing else may run on this handle between the two phases.
+// pointmap consumers for the survivors only.  Any other model call on this handle in between ends the pair (check_ready).
 // ---------------------------------------------------------------------------
 int sta_regress_pairs_begin(StaModel* m, const float* feat_i_dev, const float* feat_j_dev, int K, int H, int W,
                             float* pose_out_dev, float* pose_conf_out_dev, void* stream) {
   RUN(check_ready(m));
-  m->rp_K = 0;
-  STA_REQUIRE(K > 0 && K <= m->max_pairs_per_chunk, "edge batch must be in [1, 16]");
-  STA_REQUIRE(H % 16 == 0 && W % 16 == 0 && H > 0 && W > 0, "image size must be a positive multiple of 16");
-  STA_REQUIRE(H / 16 <= 1024 && W / 16 <= 1024, "token grid exceeds the RoPE table");
+  RUN(check_edges(m, K));
+  RUN(check_grid(K, H, W));
   STA_REQUIRE(feat_i_dev && feat_j_dev && pose_out_dev && pose_conf_out_dev, "null pointer");
   Ctx c{m, static_cast<cudaStream_t>(stream)};
   RUN(enter_stream(m, c.st));
-  const int h = H / 16, w = W / 16, N = h * w, S = 2 * K, M = N + 1;
+  const int h = H / 16, w = W / 16, N = h * w, S = 2 * K;
   RUN(ensure_ws(m, S, h, w));
   Workspace& ws = m->ws;
   DecBufs d = take_dec(ws, S, N);
-  float* o_pose = ws.take<float>(static_cast<size_t>(S) * 16);
-  float* o_pconf = ws.take<float>(S);
-  const size_t bm = m->bmul();
-  m->launches += 2;
-  RUN(launch_cast_f32_bf16(feat_i_dev, d.enc_bf16, static_cast<long long>(K) * N, kEncDim, 0, c.st, m->split));
-  RUN(launch_cast_f32_bf16(feat_j_dev, d.enc_bf16 + static_cast<size_t>(K) * N * kEncDim * bm, static_cast<long long>(K) * N,
-                           kEncDim, 0, c.st, m->split));
-  auto body = [&](const Ctx& cc) -> int {
-    m->launches += 3;
-    RUN(launch_make_positions(d.pos, S, h, w, 1, cc.st));
-    RUN(run_decoder(cc, K, N, d, nullptr, nullptr));
-    RUN(launch_pose_head(d.xd, static_cast<long long>(M) * kDecDim, K, 1, kLnEps, m->pose, o_pose, o_pconf, cc.st));
-    RUN(launch_pose_head(d.xd + static_cast<long long>(K) * M * kDecDim, static_cast<long long>(M) * kDecDim, K, 1, kLnEps,
-                         m->pose, o_pose + static_cast<long long>(K) * 16, o_pconf + K, cc.st));
-    return 0;
-  };
-  if (static_cast<long long>(S) * M <= kGraphMaxTokens) RUN(run_graphed(m, c.st, {3, K, H, W}, body));
-  else RUN(body(c));
-  STA_CHECK_CUDA(cudaMemcpyAsync(pose_out_dev, o_pose, static_cast<size_t>(S) * 16 * sizeof(float), cudaMemcpyDeviceToDevice, c.st));
-  STA_CHECK_CUDA(cudaMemcpyAsync(pose_conf_out_dev, o_pconf, static_cast<size_t>(S) * sizeof(float), cudaMemcpyDeviceToDevice, c.st));
-  m->rp_K = K;
-  m->rp_H = H;
-  m->rp_W = W;
+  const bool graphed = static_cast<long long>(S) * (N + 1) <= kGraphMaxTokens;
+  Staging staged{ws, graphed};
+  float* o_pose = staged.out(pose_out_dev, static_cast<size_t>(S) * 16);
+  float* o_pconf = staged.out(pose_conf_out_dev, S);
+  RUN(check_ws(ws));
+  RUN(cast_features(c, feat_i_dev, feat_j_dev, K, N, d));
+  auto body = [&](const Ctx& cc) -> int { return decode_with_poses(cc, K, h, w, d, o_pose, o_pconf, K); };
+  RUN(run_graphed(m, c.st, graphed, {3, K, H, W}, body));
+  RUN(staged.flush(c.st));
+  m->rp = {K, H, W, d, ws.off};
   return 0;
 }
 
 int sta_regress_pairs_finish(StaModel* m, const int* edge_idx_host, int n_sel, float* pts3d_out_dev, float* conf_out_dev,
                              float* intri_out_dev, float* depth_out_dev, float* conf_mean_out_dev, void* scratch,
                              void* stream) {
-  RUN(check_ready(m));
-  STA_REQUIRE(m->rp_K > 0, "sta_regress_pairs_finish without a preceding sta_regress_pairs_begin on this handle");
-  const int K = m->rp_K, H = m->rp_H, W = m->rp_W;
+  RUN(check_ready(m, /*finishing_pairs=*/true));
+  STA_REQUIRE(m->rp.K > 0, "sta_regress_pairs_finish without a preceding sta_regress_pairs_begin on this handle, or "
+                           "another call on the handle came between them");
+  const int K = m->rp.K, H = m->rp.H, W = m->rp.W;
   STA_REQUIRE(n_sel >= 0 && n_sel <= K, "more selected edges than candidates");
   if (n_sel == 0) return 0;
   STA_REQUIRE(edge_idx_host && pts3d_out_dev && conf_out_dev, "null pointer");
   for (int k = 0; k < n_sel; ++k) STA_REQUIRE(edge_idx_host[k] >= 0 && edge_idx_host[k] < K, "edge index out of range");
-  const bool consumers = intri_out_dev || depth_out_dev || conf_mean_out_dev;
-  if (consumers) STA_REQUIRE(scratch != nullptr && intri_out_dev != nullptr, "the pointmap consumers need scratch and intri_out");
+  RUN(check_consumers(scratch, intri_out_dev, depth_out_dev, conf_mean_out_dev));
   Ctx c{m, static_cast<cudaStream_t>(stream)};
   RUN(enter_stream(m, c.st));
-  const int h = H / 16, w = W / 16, N = h * w, S = 2 * K, S2 = 2 * n_sel;
-  RUN(ensure_ws(m, S, h, w));  // same shape as phase 1: no reallocation, and the same take sequence gives the same buffers
-  Workspace& ws = m->ws;
-  DecBufs d = take_dec(ws, S, N);
-  ws.take<float>(static_cast<size_t>(S) * 16);
-  ws.take<float>(S);
-  const size_t bm = m->bmul();
+  const int h = H / 16, w = W / 16, N = h * w, S2 = 2 * n_sel;
   const long long px = static_cast<long long>(H) * W;
+  const DecBufs& d = m->rp.d;
+  Workspace& ws = m->ws;
+  ws.off = m->rp.ws_off;  // _begin's buffers stay untouched
+  const bool graphed = 2LL * K * (N + 1) <= kGraphMaxTokens;
   // compact copies of the survivors' hooks: [view][edge] order, view 0 = the (i -> j) direction
   bf16* sel[4];
+  take_hooks(ws, S2, N, sel);
+  Staging staged{ws, graphed};
+  const PairOuts o = stage_pair_outs(
+      staged, {pts3d_out_dev, conf_out_dev, intri_out_dev, depth_out_dev, conf_mean_out_dev, scratch}, n_sel, px);
+  const DptBufs dpt = take_dpt(ws, n_sel, h, w);
+  RUN(check_ws(ws));
+  const size_t bm = m->bmul();
   const size_t width[4] = {1024 * bm, 768 * bm, 768 * bm, 768 * bm};
-  const bf16* src[4] = {d.enc_bf16, d.hook[0], d.hook[1], d.hook[2]};
-  for (int q = 0; q < 4; ++q) sel[q] = ws.take<bf16>(static_cast<size_t>(S2) * N * width[q]);
-  float* o_pts = ws.take<float>(static_cast<size_t>(S2) * px * 3);
-  float* o_conf = ws.take<float>(static_cast<size_t>(S2) * px);
-  float* o_intri = consumers ? ws.take<float>(static_cast<size_t>(n_sel) * 9) : nullptr;
-  float* o_depth = depth_out_dev ? ws.take<float>(static_cast<size_t>(S2) * px) : nullptr;
-  float* o_cmean = conf_mean_out_dev ? ws.take<float>(S2) : nullptr;
-  void* o_scratch = consumers ? ws.take<double>(pointmap_scratch_bytes(S2) / sizeof(double)) : nullptr;
-  STA_REQUIRE(ws.off <= ws.bytes, "internal: workspace too small for the gated keyframe step");
   for (int v = 0; v < 2; ++v)
     for (int k = 0; k < n_sel; ++k)
       for (int q = 0; q < 4; ++q) {
         const size_t rows = static_cast<size_t>(N) * width[q];
         STA_CHECK_CUDA(cudaMemcpyAsync(sel[q] + (static_cast<size_t>(v) * n_sel + k) * rows,
-                                       src[q] + (static_cast<size_t>(v) * K + edge_idx_host[k]) * rows, rows * sizeof(bf16),
+                                       d.hook[q] + (static_cast<size_t>(v) * K + edge_idx_host[k]) * rows, rows * sizeof(bf16),
                                        cudaMemcpyDeviceToDevice, c.st));
       }
-  auto body = [&](const Ctx& cc) -> int {
-    for (int v = 0; v < 2; ++v) {
-      const size_t save = ws.off;
-      const size_t tok0 = static_cast<size_t>(v) * n_sel * N;
-      RUN(run_dpt(cc, ws, n_sel, h, w, sel[0] + tok0 * width[0], sel[1] + tok0 * width[1], sel[2] + tok0 * width[2],
-                  sel[3] + tok0 * width[3], o_pts + static_cast<long long>(v) * n_sel * px * 3,
-                  o_conf + static_cast<long long>(v) * n_sel * px));
-      ws.off = save;
-    }
-    if (consumers) {
-      m->launches += 2;
-      RUN(launch_pointmap_consumers(o_pts, o_conf, S2, H, W, 2, o_intri, o_depth, o_cmean, o_scratch, cc.st));
-    }
-    return 0;
-  };
-  if (static_cast<long long>(S) * (N + 1) <= kGraphMaxTokens)
-    RUN(run_graphed(m, c.st, {4, K, n_sel, H, W, consumers ? 1 : 0, depth_out_dev ? 1 : 0, conf_mean_out_dev ? 1 : 0}, body));
-  else
-    RUN(body(c));
-  auto copy = [&](float* dst, const float* srcp, size_t n) -> int {
-    if (dst) STA_CHECK_CUDA(cudaMemcpyAsync(dst, srcp, n * sizeof(float), cudaMemcpyDeviceToDevice, c.st));
-    return 0;
-  };
-  RUN(copy(pts3d_out_dev, o_pts, static_cast<size_t>(S2) * px * 3));
-  RUN(copy(conf_out_dev, o_conf, static_cast<size_t>(S2) * px));
-  if (consumers) {
-    RUN(copy(intri_out_dev, o_intri, static_cast<size_t>(n_sel) * 9));
-    RUN(copy(depth_out_dev, o_depth, static_cast<size_t>(S2) * px));
-    RUN(copy(conf_mean_out_dev, o_cmean, S2));
-  }
-  return 0;
+  auto body = [&](const Ctx& cc) -> int { return pair_heads(cc, dpt, sel, n_sel, H, W, o); };
+  RUN(run_graphed(m, c.st, graphed,
+                  {4, K, n_sel, H, W, intri_out_dev ? 1 : 0, depth_out_dev ? 1 : 0, conf_mean_out_dev ? 1 : 0}, body));
+  return staged.flush(c.st);
 }
 
 int sta_forward_pairs(StaModel* m, const void* img1_dev, const void* img2_dev, int img_is_bf16, int B, int H, int W,
                       float* pts3d_out_dev, float* conf_out_dev, float* pose_out_dev, float* pose_conf_out_dev,
                       void* stream) {
   RUN(check_ready(m));
-  STA_REQUIRE(B > 0 && H % 16 == 0 && W % 16 == 0 && H > 0 && W > 0, "image size must be a positive multiple of 16");
-  STA_REQUIRE(H / 16 <= 1024 && W / 16 <= 1024, "token grid exceeds the RoPE table");
+  RUN(check_grid(B, H, W));
   Ctx c{m, static_cast<cudaStream_t>(stream)};
   RUN(enter_stream(m, c.st));
   const size_t esz = img_is_bf16 ? 2 : 4;
@@ -1500,8 +1500,7 @@ int sta_forward_pairs_host(StaModel* m, const void* img1_host, const void* img2_
                            int W, float* pts3d_out_host, float* conf_out_host, float* pose_out_host,
                            float* pose_conf_out_host, void* stream) {
   RUN(check_ready(m));
-  STA_REQUIRE(B > 0 && H % 16 == 0 && W % 16 == 0 && H > 0 && W > 0, "image size must be a positive multiple of 16");
-  STA_REQUIRE(H / 16 <= 1024 && W / 16 <= 1024, "token grid exceeds the RoPE table");
+  RUN(check_grid(B, H, W));
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   RUN(enter_stream(m, st));
   const size_t esz = img_is_bf16 ? 2 : 4;

@@ -9,6 +9,8 @@ with no host synchronisation inside -- the caller reads `pose_conf` once per key
 
 Results are numerically the per-edge results of the reference sequence (the decoder has no cross-sample op), so
 `regress_two_views(i, j)` is also offered as the K = 1 special case with the reference's return convention."""
+import ctypes
+
 import torch
 
 from . import _lib
@@ -33,6 +35,22 @@ class KeyframeFrontend:
         self.img_shapes.append((int(image.shape[-2]), int(image.shape[-1])))
         return len(self.enc_features) - 1
 
+    def _edge_batch(self, i, js):
+        """The inputs of a batched step over the K = len(js) edges (i, j): the library, the feature pairs fi / fj, the
+        image size, a float32 allocator on their device and the pose outputs [2, K, 4, 4] / [2, K] of both directions."""
+        K = len(js)
+        H, W = self.img_shapes[i]
+        if any(self.img_shapes[j] != (H, W) for j in js):
+            raise ValueError("all views of a batch must have the same size")
+        fi = self.enc_features[i].expand(K, -1, -1).contiguous() if K > 1 else self.enc_features[i]
+        fj = torch.cat([self.enc_features[j] for j in js], dim=0) if K > 1 else self.enc_features[js[0]]
+        L = self.frontend._ready(fi)
+
+        def f32(*shape):
+            return torch.empty(*shape, device=fi.device, dtype=torch.float32)
+
+        return L, fi, fj, H, W, f32, f32(2, K, 4, 4), f32(2, K)
+
     @torch.no_grad()
     def regress_views(self, i, js):
         """All edges (i, j) for j in js in one batch.  Returns a dict of CUDA tensors, edge-major:
@@ -42,22 +60,14 @@ class KeyframeFrontend:
         K = len(js)
         if K == 0:
             raise ValueError("no edges")
-        H, W = self.img_shapes[i]
-        if any(self.img_shapes[j] != (H, W) for j in js):
-            raise ValueError("all views of a batch must have the same size")
-        m = self.frontend
-        fi = self.enc_features[i].expand(K, -1, -1).contiguous() if K > 1 else self.enc_features[i]
-        fj = torch.cat([self.enc_features[j] for j in js], dim=0) if K > 1 else self.enc_features[js[0]]
-        L = m._ready(fi)
+        L, fi, fj, H, W, f32, pose, pconf = self._edge_batch(i, js)
+        pts = f32(2, K, H, W, 3)
+        conf = f32(2, K, H, W)
+        intri = f32(K, 3, 3)
+        depth = f32(2, K, H, W)
+        cmean = f32(2, K)
         dev = fi.device
-        f32 = dict(device=dev, dtype=torch.float32)
-        pose = torch.empty(2, K, 4, 4, **f32)
-        pconf = torch.empty(2, K, **f32)
-        pts = torch.empty(2, K, H, W, 3, **f32)
-        conf = torch.empty(2, K, H, W, **f32)
-        intri = torch.empty(K, 3, 3, **f32)
-        depth = torch.empty(2, K, H, W, **f32)
-        cmean = torch.empty(2, K, **f32)
+        m = self.frontend
         with torch.cuda.device(dev):
             _lib.check(L.sta_regress_pairs(m._handle, _lib.ptr(fi), _lib.ptr(fj), K, H, W, _lib.ptr(pose), _lib.ptr(pconf),
                                            _lib.ptr(pts), _lib.ptr(conf), _lib.ptr(intri), _lib.ptr(depth), _lib.ptr(cmean),
@@ -75,22 +85,13 @@ class KeyframeFrontend:
         (slam.py:153-189) minus the pypose conversion, which stays with the caller:
             (pose_ij [1,4,4], rel_pose_conf_ij [1], confs [2,H,W] | None, intri [3,3] | None, depths [2,H,W] | None)
         -- the last three are None for rejected edges, exactly where the reference returns None."""
-        import ctypes
         js = list(js)
         K = len(js)
         if K == 0:
             return []
-        H, W = self.img_shapes[i]
-        if any(self.img_shapes[j] != (H, W) for j in js):
-            raise ValueError("all views of a batch must have the same size")
-        m = self.frontend
-        fi = self.enc_features[i].expand(K, -1, -1).contiguous() if K > 1 else self.enc_features[i]
-        fj = torch.cat([self.enc_features[j] for j in js], dim=0) if K > 1 else self.enc_features[js[0]]
-        L = m._ready(fi)
+        L, fi, fj, H, W, f32, pose, pconf = self._edge_batch(i, js)
         dev = fi.device
-        f32 = dict(device=dev, dtype=torch.float32)
-        pose = torch.empty(2, K, 4, 4, **f32)
-        pconf = torch.empty(2, K, **f32)
+        m = self.frontend
         with torch.cuda.device(dev):
             _lib.check(L.sta_regress_pairs_begin(m._handle, _lib.ptr(fi), _lib.ptr(fj), K, H, W, _lib.ptr(pose), _lib.ptr(pconf),
                                                  _lib.cur_stream()), "sta_regress_pairs_begin")
@@ -100,10 +101,10 @@ class KeyframeFrontend:
             out = [(pose[0, k:k + 1], pconf[0, k:k + 1], None, None, None) for k in range(K)]
             if n == 0:
                 return out
-            pts = torch.empty(2, n, H, W, 3, **f32)
-            conf = torch.empty(2, n, H, W, **f32)
-            intri = torch.empty(n, 3, 3, **f32)
-            depth = torch.empty(2, n, H, W, **f32)
+            pts = f32(2, n, H, W, 3)
+            conf = f32(2, n, H, W)
+            intri = f32(n, 3, 3)
+            depth = f32(2, n, H, W)
             idx = (ctypes.c_int * n)(*keep)
             _lib.check(L.sta_regress_pairs_finish(m._handle, idx, n, _lib.ptr(pts), _lib.ptr(conf), _lib.ptr(intri),
                                                   _lib.ptr(depth), None, _lib.ptr(_scratch_for(dev, 2 * n)), _lib.cur_stream()),
