@@ -509,6 +509,7 @@ def group_x3():
 
 def group_perf():
     import torch
+    import torch.nn.functional as F
     from vista_slam_b200._lib import EPI_BF16, EPI_GELU, check, cur_stream, lib, ptr
     dev = "cuda"
     torch.manual_seed(5)
@@ -525,8 +526,9 @@ def group_perf():
         torch.cuda.synchronize()
         return e0.elapsed_time(e1) / n
 
+    # trunk shapes, plus one grid of 200 tiles (between one and two tiles per SM on a 132-SM H100)
     for (M, N, K, epi) in [(24576, 3072, 1024, EPI_BF16), (24576, 4096, 1024, EPI_GELU), (24576, 1024, 4096, EPI_BF16),
-                           (24576, 1024, 1024, EPI_BF16)]:
+                           (24576, 1024, 1024, EPI_BF16), (3200, 1024, 1024, EPI_BF16)]:
         A = torch.randn(M, K, device=dev).bfloat16()
         W = (torch.randn(N, K, device=dev) / math.sqrt(K)).bfloat16()
         bias = torch.randn(N, device=dev)
@@ -558,6 +560,54 @@ def group_perf():
             d = gemm_desc(epi=epi, A=A, lda=K, W=W, ldw=K, M=M, N=N, K=K, bias=bias, out=out, ldo=N)
         ms = timeit(lambda: run_gemm(d))
         print("gemm-epi %-22s M%d N%d K%d: %.3f ms = %.0f TFLOP/s" % (name, M, N, K, ms, 2.0 * M * N * K / ms / 1e9), flush=True)
+    # Per-tile fixed cost: time(K) = a + b K over a K sweep at a trunk shape.  a is what a tile costs besides its
+    # k-blocks (epilogue, pipeline fill and drain) where it is not hidden behind another tile's MMAs; a / time(1024) is
+    # its share of a K = 1024 layer.
+    M, N = 24576, 3072
+    ks, ts = [256, 512, 1024, 2048], []
+    for K in ks:
+        A = torch.randn(M, K, device=dev).bfloat16()
+        W = (torch.randn(N, K, device=dev) / math.sqrt(K)).bfloat16()
+        bias = torch.randn(N, device=dev)
+        out = torch.zeros(M, N, device=dev, dtype=torch.bfloat16)
+        d = gemm_desc(epi=EPI_BF16, A=A, lda=K, W=W, ldw=K, M=M, N=N, K=K, bias=bias, out=out, ldo=N)
+        ts.append(timeit(lambda: run_gemm(d), n=20))
+    n = len(ks)
+    mk, mt = sum(ks) / n, sum(ts) / n
+    slope = sum((k - mk) * (t - mt) for k, t in zip(ks, ts)) / sum((k - mk) ** 2 for k in ks)
+    icpt = mt - slope * mk
+    print("gemm K sweep M%d N%d: %s ms; fixed cost %.3f ms = %.0f %% of K=1024" %
+          (M, N, " ".join("K%d %.3f" % (k, t) for k, t in zip(ks, ts)), icpt, 100.0 * icpt / ts[ks.index(1024)]),
+          flush=True)
+    # cfg-2 DPT 3x3 convolutions (run_dpt in runtime.cu: 16 images per pass, token grid 24 x 32), against cuDNN
+    from vista_slam_b200._lib import EPI_HEAD
+    for (H, W, Cin, Cout, name) in [(96, 128, 128, 256, "layer1_rn"), (48, 64, 192, 256, "layer2_rn"),
+                                    (24, 32, 384, 256, "layer3_rn"), (12, 16, 768, 256, "layer4_rn"),
+                                    (96, 128, 256, 256, "refinenet1 rcu"), (48, 64, 256, 256, "refinenet2 rcu"),
+                                    (24, 32, 256, 256, "refinenet3 rcu"), (12, 16, 256, 256, "refinenet4 rcu"),
+                                    (192, 256, 256, 128, "head.0"), (384, 512, 128, 128, "head.2 (+head epilogue)")]:
+        nimg = 16
+        x = torch.randn(nimg, H, W, Cin, device=dev).bfloat16()
+        wp = (torch.randn(Cout, 9 * Cin, device=dev) / math.sqrt(9 * Cin)).bfloat16()
+        b = torch.randn(Cout, device=dev)
+        if Cout == 128 and H == 384:
+            w4t = (torch.randn(4, 128, device=dev) / math.sqrt(128)).t().contiguous()
+            b4 = torch.randn(4, device=dev)
+            pts = torch.zeros(nimg, H, W, 3, device=dev)
+            conf = torch.zeros(nimg, H, W, device=dev)
+            d = gemm_desc(conv3x3=1, epi=EPI_HEAD, A=x, W=wp, ldw=9 * Cin, N=Cout, K=9 * Cin, nimg=nimg, H=H, Wd=W,
+                          Cin=Cin, bias=b, head_w=w4t, head_b=b4, pts3d=pts, conf=conf)
+        else:
+            out = torch.zeros(nimg, H, W, Cout, device=dev, dtype=torch.bfloat16)
+            d = gemm_desc(conv3x3=1, epi=EPI_BF16, A=x, W=wp, ldw=9 * Cin, N=Cout, K=9 * Cin, nimg=nimg, H=H, Wd=W,
+                          Cin=Cin, bias=b, out=out, ldo=Cout)
+        ms = timeit(lambda: run_gemm(d))
+        xc = x.permute(0, 3, 1, 2)  # NCHW view of NHWC memory: cuDNN's channels-last path
+        wc = wp.view(Cout, 3, 3, Cin).permute(0, 3, 1, 2).contiguous(memory_format=torch.channels_last)
+        ms_t = timeit(lambda: F.conv2d(xc, wc, padding=1))
+        fl = 2.0 * nimg * H * W * Cout * 9 * Cin
+        print("conv3x3 %-24s %dx%dx%d C%d->%d: %.3f ms = %.0f TFLOP/s   (cuDNN conv2d %.3f ms = %.0f TFLOP/s)" %
+              (name, nimg, H, W, Cin, Cout, ms, fl / ms / 1e9, ms_t, fl / ms_t / 1e9), flush=True)
     L = lib()
     for (batch, heads, n) in [(32, 16, 768), (32, 12, 769)]:
         C = heads * 64

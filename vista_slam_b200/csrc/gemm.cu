@@ -55,7 +55,7 @@ int launch_gemm(const GemmLaunch& g, cudaStream_t stream) {
   STA_REQUIRE((reinterpret_cast<uintptr_t>(g.A) & 15) == 0 && (reinterpret_cast<uintptr_t>(g.Wt) & 15) == 0,
               "operands must be 16-byte aligned");
 
-  // 128 x 128 tiles: one m64n128 wgmma per consumer warpgroup and k16 step
+  // 128 x 128 tiles: two m64n128 wgmmas per consumer warpgroup and k16 step
   const int bn = 128;
 
   // TMA-store epilogue (epilogue_tile_tma) for the linear layers: bf16 / GELU / RoPE outputs without skip
@@ -138,14 +138,14 @@ int launch_gemm(const GemmLaunch& g, cudaStream_t stream) {
     p.c_reduce = 0;
     uint64_t dims[2] = {(uint64_t)p.N, (uint64_t)ksplit * p.split_rows};
     uint64_t strides[1] = {(uint64_t)p.N * 4};
-    uint32_t box[2] = {32, 32};
+    uint32_t box[2] = {32, 16};  // one 16-row group of a warp's accumulator fragments
     if (make_tmap(&tmC, g.splitk_ws, 1, 2, dims, strides, box)) return 1;
   } else if (tma) {
     ksplit = 1;
     // split-precision mode: bf16 rows are (hi | lo | hi), 3N wide
     uint64_t dims[2] = {(uint64_t)p.N * ((p.split && esz == 2) ? 3 : 1), (uint64_t)p.M};
     uint64_t strides[1] = {(uint64_t)p.ldo * esz};
-    uint32_t box[2] = {(uint32_t)(128 / esz), 32};
+    uint32_t box[2] = {(uint32_t)(128 / esz), 16};  // one 16-row group of a warp's accumulator fragments
     if (make_tmap(&tmC, p.out, esz == 4, 2, dims, strides, box)) return 1;
   }
   STA_REQUIRE(tma || ksplit == 1, "split-K needs the TMA epilogue");

@@ -2,13 +2,14 @@
 //
 //   D[M,N] = A[M,K] * W[N,K]^T  (bf16 operands, fp32 accumulation in registers)
 //
-// Roles: warp 0 = TMA producer (warps 1-3 idle), warps 4-11 = two consumer warpgroups.  Consumer warpgroup g
-// computes rows [64 g, 64 g + 64) of the 128 x BN tile with wgmma (m64 n128 k16, accumulators in registers) while
-// the producer keeps a STAGES-deep operand ring filled; the finished accumulators are written to a padded fp32 tile
-// in shared memory, from which the same eight warps run the fused epilogue (-> global).  The producer prefetches
-// the next tile's operands during the epilogue.  Operand tiles are 128B-swizzled K-major [rows][64] boxes written
-// by TMA; the 3x3 convolution loads one halo tile per channel chunk through a 4-D NHWC tensor map (out-of-bounds =
-// zero padding) and feeds every filter tap from shifted views of it, so no im2col buffer exists.
+// Roles: warpgroup 0 = TMA producer (warp 0 lane 0 issues the loads; the warpgroup drops to 40 registers), warpgroups 1
+// and 2 = consumers (232 registers each) that ping-pong whole 128 x BN tiles: consumer g takes tiles g, g + 2, .. of
+// the CTA's sequence, holds the tile's fp32 accumulators in registers (two m64n128k16 wgmmas per k16 step), and the two
+// take turns on the tensor cores, so one runs its fused epilogue (straight from the wgmma fragments) while the other runs
+// its mainloop.  The producer keeps a STAGES-deep operand ring filled in tile order.  Operand tiles are 128B-swizzled
+// K-major [rows][64] boxes written by TMA; the 3x3 convolution loads one halo tile per channel chunk through a 4-D NHWC
+// tensor map (out-of-bounds = zero padding) and feeds every filter tap from shifted views of it, so no im2col buffer
+// exists.
 //
 // Reference ops covered (vista_slam/sta_model): nn.Linear in blocks/sta_blocks.py:67-70,
 // 88-90,179-183; PatchEmbed conv sta_blocks.py:262 (after im2col); the DPT convs of
@@ -69,7 +70,7 @@ struct GemmParams {
   int split;
 };
 
-// TMA = true: the epilogue writes through shared memory + TMA tensor stores (epilogue_tile_tma), else the
+// TMA = true: the epilogue writes through per-warp swizzled boxes + TMA tensor stores (epilogue_tile_tma), else the
 // coalesced per-warp path (epilogue_tile).
 // A_CONV3: pixels per staged halo row.  10 = the 8-pixel tile plus its two halo columns (dense box, 8-row descriptor groups
 // 1280 B apart -- groups then start at any 128-byte multiple, which the absolute-address swizzle permits).
@@ -79,20 +80,23 @@ template <int AMODE, int EPI, bool TMA>
 struct GemmCfg {
   static constexpr bool CONV = (AMODE == A_CONV3);
   static constexpr int BM = 128;
-  static constexpr int BN = 128;  // one consumer warpgroup covers the 128 columns of a tile (wgmma m64n128k16)
+  static constexpr int BN = 128;  // two m64n128k16 wgmmas per k16 step cover a consumer warpgroup's whole tile
   static constexpr int BK = 64;
   static constexpr uint32_t A_BYTES = BM * BK * 2;
   static constexpr uint32_t B_BYTES = BN * BK * 2;
   static constexpr uint32_t BAR_BYTES = 256;
-  static constexpr int EPI_WARPS = 8;   // the two consumer warpgroups
-  static constexpr int PARTS = EPI_WARPS / 4;  // column parts of a tile, one per epilogue warp of a lane quarter
-  static constexpr uint32_t EPI_SMEM_BYTES = (EPI == EPI_HEAD) ? 3 * 128 * 4 * sizeof(float) : 0;  // partial sums
-  // finished accumulators: [128 rows][BN + 4] fp32 (the pad makes row-per-lane 16-byte reads conflict-free)
-  static constexpr int ACC_LD = BN + 4;
-  static constexpr uint32_t ACC_BYTES = BM * ACC_LD * sizeof(float);
-  // per-warp staging of the TMA-store epilogue: one 4 KB SWIZZLE_128B box
-  static constexpr uint32_t STG_WARP_BYTES = 4096;
-  static constexpr uint32_t STG_BYTES = TMA ? EPI_WARPS * STG_WARP_BYTES : 0;
+  static constexpr int EPI_WARPS = 8;  // the two consumer warpgroups
+  // Register split (setmaxnreg): the producer warpgroup only issues TMA loads; a consumer thread holds a 128 x 128 fp32
+  // accumulator tile's 128 values plus the epilogue's working set.
+  static constexpr uint32_t PRODUCER_REGS = 40;
+  static constexpr uint32_t CONSUMER_REGS = 232;
+  static_assert(128 * PRODUCER_REGS + 256 * CONSUMER_REGS <= 64 * 1024, "register file");
+  // Per-warp epilogue staging.  TMA-store epilogue: two 16-row x 128-byte SWIZZLE_128B boxes, alternated so that one
+  // is written while the bulk store of the other reads it.  Coalesced epilogue: one fp32 box of the warp's 32 accumulator
+  // rows x 32 columns (box_off: 16-byte chunks XOR-swizzled by row, so fragment writes and row reads are conflict-free).
+  static constexpr uint32_t TMA_BOX_BYTES = 16 * 128;
+  static constexpr uint32_t STG_WARP_BYTES = TMA ? 2 * TMA_BOX_BYTES : 32 * 32 * sizeof(float);
+  static constexpr uint32_t STG_BYTES = EPI_WARPS * STG_WARP_BYTES;
   static constexpr int ROPE_SMEM_ROWS = 64;  // positions -1 .. 62
   static constexpr uint32_t ROPE_SMEM_BYTES = (EPI == EPI_ROPE) ? ROPE_SMEM_ROWS * kRopeLd * sizeof(float) : 0;
   static constexpr uint32_t MAX_SMEM = 227 * 1024;
@@ -102,41 +106,28 @@ struct GemmCfg {
   static constexpr int HALO_STAGES = 3;
   static constexpr uint32_t HALO_TOTAL = CONV ? HALO_STAGES * HALO_BYTES : 0;
   static constexpr uint32_t STAGE_BYTES = CONV ? B_BYTES : A_BYTES + B_BYTES;
-  static constexpr int STAGES_FIT =
-      (MAX_SMEM - BAR_BYTES - EPI_SMEM_BYTES - STG_BYTES - ACC_BYTES - ROPE_SMEM_BYTES - HALO_TOTAL) / STAGE_BYTES;
+  static constexpr int STAGES_FIT = (MAX_SMEM - BAR_BYTES - STG_BYTES - ROPE_SMEM_BYTES - HALO_TOTAL) / STAGE_BYTES;
   static constexpr int STAGES = STAGES_FIT > 8 ? 8 : STAGES_FIT;
-  // layout: operand ring | halo tiles | staging (1024-byte aligned) | accumulator tile | barriers | EPI_HEAD partials | RoPE
+  // layout: operand ring | halo tiles | staging (1024-byte aligned) | barriers | RoPE
   static constexpr uint32_t OFF_HALO = STAGES * STAGE_BYTES;
   static constexpr uint32_t OFF_STG = OFF_HALO + HALO_TOTAL;
-  static constexpr uint32_t OFF_ACC = OFF_STG + STG_BYTES;
-  static constexpr uint32_t OFF_BAR = OFF_ACC + ACC_BYTES;
-  static constexpr uint32_t OFF_EPI = OFF_BAR + BAR_BYTES;
-  static constexpr uint32_t OFF_ROPE = OFF_EPI + EPI_SMEM_BYTES;
+  static constexpr uint32_t OFF_BAR = OFF_STG + STG_BYTES;
+  static constexpr uint32_t OFF_ROPE = OFF_BAR + BAR_BYTES;
   static constexpr uint32_t SMEM_BYTES = OFF_ROPE + ROPE_SMEM_BYTES;
   static constexpr int THREADS = 128 + 32 * EPI_WARPS;
   static constexpr int EPI_THREADS = 32 * EPI_WARPS;
   static_assert(STAGES <= 8 && STAGES >= 3, "barrier area holds at most 8 stages");
-  static_assert(OFF_STG % 1024 == 0 && OFF_HALO % 1024 == 0 && OFF_ACC % 16 == 0, "staging alignment");
+  static_assert(OFF_STG % 1024 == 0 && OFF_HALO % 1024 == 0 && STG_WARP_BYTES % 16 == 0, "staging alignment");
+  static_assert(!TMA || STG_WARP_BYTES % 1024 == 0, "SWIZZLE_128B boxes are 1024-byte aligned");
   static_assert(SMEM_BYTES <= MAX_SMEM, "shared memory");
 };
 
 // ---------------------------------------------------------------------------
-// Epilogue for one 128 x BN accumulator tile held in shared memory ([128][BN + 4] fp32); executed by the 8 consumer
-// warps.  warp (quarter, part): rows [32*quarter, +32), columns [part*BN/2, +BN/2).
-//
-// Every 32x32 fp32 chunk is read in a COALESCED mapping -- lane -> (row = 4*it + lane/8, 4 columns at (lane%8)*4) --
-// in which bias, residuals, activation and the global stores happen: a warp-wide access covers 4 rows x 128
-// contiguous bytes (fp32) or 4 rows x 64 bytes (bf16).
+// Accumulator fragments.  A consumer warpgroup holds its 128 x 128 tile as acc[h][64]: acc[h] is the m64n128 wgmma
+// fragment of tile rows [64 h, 64 h + 64).  Warp wq (of the warpgroup), lane = 4 r + t holds, in acc[h][4 j + 2 half + e],
+// row 64 h + 16 wq + 8 half + r, column 8 j + 2 t + e (j = 0..15).  So a thread holds rows r, r + 8, r + 64, r + 72 of
+// its warp's 16-row groups, and the four lanes of a quad hold all 128 columns of those rows.
 // ---------------------------------------------------------------------------
-// 32 consecutive fp32 accumulators of one row (16-byte aligned)
-__device__ __forceinline__ void acc_ld32(const float* src, uint32_t (&r)[32]) {
-#pragma unroll
-  for (int j = 0; j < 8; ++j) {
-    const float4 v = reinterpret_cast<const float4*>(src)[j];
-    r[4 * j] = __float_as_uint(v.x); r[4 * j + 1] = __float_as_uint(v.y);
-    r[4 * j + 2] = __float_as_uint(v.z); r[4 * j + 3] = __float_as_uint(v.w);
-  }
-}
 
 template <int AMODE>
 __device__ __forceinline__ void tile_row(const GemmParams& p, int m_tile, int r_local, long long& orow, bool& valid) {
@@ -173,71 +164,93 @@ __device__ __forceinline__ void store4_bf16(__nv_bfloat16* p, const float4& v, i
   }
 }
 
-// accs: the accumulator tile at this warp's first row (32 * quarter) and first column (part * BN / PARTS)
+// ---------------------------------------------------------------------------
+// Coalesced epilogue of one warp's 32 accumulator rows (all 128 columns of the tile), run straight from the fragments.
+//
+// Box row rho (0..31) of the per-warp fp32 box is tile row 16 wq + rho (rho < 16) or 64 + 16 wq + rho - 16.  Each 32-column
+// chunk is written into the box from the fragments and read back in a COALESCED mapping -- lane -> (box row
+// 4*it + lane/8, 4 columns at (lane%8)*4) -- in which bias, residuals, activation and the global stores happen: a warp-wide
+// access covers 4 rows x 128 contiguous bytes (fp32) or 4 rows x 64 bytes (bf16).
+// ---------------------------------------------------------------------------
+__device__ __forceinline__ int box_row_to_tile_row(int wq, int rho) { return 16 * wq + rho + 48 * (rho >> 4); }
+
+// float offset of (row, col) in the per-warp [32][32] fp32 box: 16-byte chunk col / 4 of a row lives at (col / 4) ^ (row & 7)
+__device__ __forceinline__ int box_off(int row, int col) { return row * 32 + ((((col >> 2) ^ row) & 7) << 2) + (col & 3); }
+
+// fragments of 32-column chunk c -> the per-warp box
+__device__ __forceinline__ void stage_chunk(float* box, const float (&acc)[2][64], int c) {
+  const int lane = threadIdx.x & 31;
+  const int r = lane >> 2, t = lane & 3;
+#pragma unroll
+  for (int h = 0; h < 2; ++h)
+#pragma unroll
+    for (int half = 0; half < 2; ++half)
+#pragma unroll
+      for (int jl = 0; jl < 4; ++jl) {
+        const int i = 4 * (4 * c + jl) + 2 * half;
+        *reinterpret_cast<float2*>(box + box_off(16 * h + 8 * half + r, 8 * jl + 2 * t)) = make_float2(acc[h][i], acc[h][i + 1]);
+      }
+}
+
 template <int AMODE, int EPI>
-__device__ __forceinline__ void epilogue_tile(const GemmParams& p, const float* accs, int m_tile, int n_tile,
-                                              int quarter, int part, float* epi_smem) {
+__device__ __forceinline__ void epilogue_tile(const GemmParams& p, const float (&acc)[2][64], int m_tile, int n_tile,
+                                              int wq, float* box) {
   using Cfg = GemmCfg<AMODE, EPI, false>;
   constexpr int BN = Cfg::BN;
-  constexpr int PARTS = Cfg::PARTS;
-  constexpr int LD = Cfg::ACC_LD;  // accumulator tile row stride (floats)
-  constexpr int CH = BN / PARTS;  // columns per epilogue warp
+  constexpr int NCH = BN / 32;  // 32-column chunks
   const int lane = threadIdx.x & 31;
-  const int colbase = n_tile * BN + part * CH;
+  const int colbase = n_tile * BN;
 
   if constexpr (EPI == EPI_HEAD) {
     // head.2 epilogue: ReLU -> head.4 (1x1, 128 -> 4) -> postprocess (dpt_block.py:319-323,
-    // postprocess.py:10-62).  Row mapping: each thread owns 32 of the 128 channels of one pixel; the four
-    // column parts are combined through shared memory.  Nothing but 16 bytes per pixel is written.
-    const int r_local = quarter * 32 + lane;
+    // postprocess.py:10-62).  Row mapping: lane = box row, so each thread walks the 128 channels of one pixel in order,
+    // with columns [0, 64) and [64, 128) summed in two chains that are added at the end.  Nothing but 16 bytes per
+    // pixel is written.
     long long orow;
     bool valid;
-    tile_row<AMODE>(p, m_tile, r_local, orow, valid);
-    float psum[4] = {0.f, 0.f, 0.f, 0.f};
-#pragma unroll 1
-    for (int c = 0; c < CH; c += 32) {
-      const int col = colbase + c;
-      uint32_t acc[32];
-      acc_ld32(accs + lane * LD + c, acc);
+    tile_row<AMODE>(p, m_tile, box_row_to_tile_row(wq, lane), orow, valid);
+    float psum[2][4] = {{0.f, 0.f, 0.f, 0.f}, {0.f, 0.f, 0.f, 0.f}};
+#pragma unroll
+    for (int c = 0; c < NCH; ++c) {
+      __syncwarp();  // the previous chunk's reads of the box are done
+      stage_chunk(box, acc, c);
+      __syncwarp();
+      const int col = colbase + 32 * c;
+      const int part = c / (NCH / 2);
       const float4* wp = reinterpret_cast<const float4*>(p.head_w) + col;
+#pragma unroll 1
+      for (int i4 = 0; i4 < 8; ++i4) {
+        const float4 a = *reinterpret_cast<const float4*>(box + box_off(lane, 4 * i4));
+        const float av[4] = {a.x, a.y, a.z, a.w};
 #pragma unroll
-      for (int i = 0; i < 32; ++i) {
-        float v = fmaxf(__uint_as_float(acc[i]) + __ldg(p.bias + col + i), 0.0f);
-        float4 w4 = __ldg(wp + i);
-        psum[0] = fmaf(v, w4.x, psum[0]);
-        psum[1] = fmaf(v, w4.y, psum[1]);
-        psum[2] = fmaf(v, w4.z, psum[2]);
-        psum[3] = fmaf(v, w4.w, psum[3]);
+        for (int e = 0; e < 4; ++e) {
+          const int i = 4 * i4 + e;
+          float v = fmaxf(av[e] + __ldg(p.bias + col + i), 0.0f);
+          float4 w4 = __ldg(wp + i);
+          psum[part][0] = fmaf(v, w4.x, psum[part][0]);
+          psum[part][1] = fmaf(v, w4.y, psum[part][1]);
+          psum[part][2] = fmaf(v, w4.z, psum[part][2]);
+          psum[part][3] = fmaf(v, w4.w, psum[part][3]);
+        }
       }
     }
-    if (part != 0)
-      reinterpret_cast<float4*>(epi_smem)[(part - 1) * 128 + r_local] = make_float4(psum[0], psum[1], psum[2], psum[3]);
-    named_bar_sync(1, Cfg::EPI_THREADS);
-    if (part == 0) {
-      float4 o = reinterpret_cast<float4*>(epi_smem)[r_local];
-#pragma unroll
-      for (int q = 1; q < PARTS - 1; ++q) {
-        const float4 t = reinterpret_cast<float4*>(epi_smem)[q * 128 + r_local];
-        o.x += t.x; o.y += t.y; o.z += t.z; o.w += t.w;
-      }
-      const float x = psum[0] + o.x + __ldg(p.head_b + 0);
-      const float y = psum[1] + o.y + __ldg(p.head_b + 1);
-      const float z = psum[2] + o.z + __ldg(p.head_b + 2);
-      const float cf = psum[3] + o.w + __ldg(p.head_b + 3);
-      if (valid) {
-        const float d = sqrtf(x * x + y * y + z * z);
-        const float dc = fmaxf(d, 1e-8f);
-        const float e = expm1f(d);
-        p.pts3d[orow * 3 + 0] = (x / dc) * e;
-        p.pts3d[orow * 3 + 1] = (y / dc) * e;
-        p.pts3d[orow * 3 + 2] = (z / dc) * e;
-        p.conf[orow] = 1.0f + expf(cf);
-      }
+    __syncwarp();
+    const float x = psum[0][0] + psum[1][0] + __ldg(p.head_b + 0);
+    const float y = psum[0][1] + psum[1][1] + __ldg(p.head_b + 1);
+    const float z = psum[0][2] + psum[1][2] + __ldg(p.head_b + 2);
+    const float cf = psum[0][3] + psum[1][3] + __ldg(p.head_b + 3);
+    if (valid) {
+      const float d = sqrtf(x * x + y * y + z * z);
+      const float dc = fmaxf(d, 1e-8f);
+      const float e = expm1f(d);
+      p.pts3d[orow * 3 + 0] = (x / dc) * e;
+      p.pts3d[orow * 3 + 1] = (y / dc) * e;
+      p.pts3d[orow * 3 + 2] = (z / dc) * e;
+      p.conf[orow] = 1.0f + expf(cf);
     }
-    named_bar_sync(1, Cfg::EPI_THREADS);
     return;
   } else {
-    // ---- coalesced mapping bookkeeping: this lane touches rows 4*it + (lane>>3), it = 0..7 ----
+    // ---- coalesced mapping bookkeeping: this lane touches box rows 4*it + (lane>>3), it = 0..7 ----
     const int crow = lane >> 3;
     const int cc = (lane & 7) * 4;  // first of this lane's 4 columns inside the 32-column chunk
     long long orow_c[8];
@@ -245,7 +258,7 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const float* 
 #pragma unroll
     for (int it = 0; it < 8; ++it) {
       bool v;
-      tile_row<AMODE>(p, m_tile, quarter * 32 + it * 4 + crow, orow_c[it], v);
+      tile_row<AMODE>(p, m_tile, box_row_to_tile_row(wq, it * 4 + crow), orow_c[it], v);
       vmask |= (v ? 1u : 0u) << it;
       if constexpr (EPI == EPI_F32) {
         if (p.rowmap_n > 0) {
@@ -266,7 +279,6 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const float* 
 
     // flush one staged 32-column chunk (global columns [col, col+32)) in the coalesced mapping
     auto flush = [&](int col, const float* stg) {
-      if (col >= p.N) return;
       float4 b4 = make_float4(0.f, 0.f, 0.f, 0.f);
       long long pix_off = 0;
       int co = 0;
@@ -327,7 +339,7 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const float* 
           // compiler can interleave the four rows of a batch
           const int it = hb * 4 + k;
           const bool ok = (vmask >> it) & 1u;
-          float4 v = *reinterpret_cast<const float4*>(stg + (it * 4 + crow) * LD + cc);
+          float4 v = *reinterpret_cast<const float4*>(stg + box_off(it * 4 + crow, cc));
           v.x += b4.x; v.y += b4.y; v.z += b4.z; v.w += b4.w;
           if constexpr (EPI == EPI_F32) {
             float* op = reinterpret_cast<float*>(p.out) + orow_c[it] * p.ldo + col + cc;
@@ -368,13 +380,13 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const float* 
         for (int it = 0; it < 8; ++it) {
           if ((vmask >> it) & 1u) {
 #pragma unroll
-            for (int c = 0; c < CH; c += 32) {
-              if (colbase + c < p.N) {
-                const char* a = reinterpret_cast<const char*>(p.resid) + (orow_c[it] * p.ldo + colbase + c + cc) * esz;
+            for (int c = 0; c < NCH; ++c) {
+              if (colbase + 32 * c < p.N) {
+                const char* a = reinterpret_cast<const char*>(p.resid) + (orow_c[it] * p.ldo + colbase + 32 * c + cc) * esz;
                 asm volatile("prefetch.global.L2 [%0];" ::"l"(a));
                 if constexpr (EPI == EPI_BF16) {
                   if (p.resid2) {
-                    const char* a2 = reinterpret_cast<const char*>(p.resid2) + (orow_c[it] * p.ldo + colbase + c + cc) * esz;
+                    const char* a2 = reinterpret_cast<const char*>(p.resid2) + (orow_c[it] * p.ldo + colbase + 32 * c + cc) * esz;
                     asm volatile("prefetch.global.L2 [%0];" ::"l"(a2));
                   }
                 }
@@ -384,151 +396,187 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const float* 
         }
       }
     }
-#pragma unroll 1
-    for (int c = 0; c < CH; c += 32) flush(colbase + c, accs + c);
+#pragma unroll
+    for (int c = 0; c < NCH; ++c) {
+      if (colbase + 32 * c < p.N) {  // warp-uniform
+        __syncwarp();  // the previous chunk's reads of the box are done
+        stage_chunk(box, acc, c);
+        __syncwarp();
+        flush(colbase + 32 * c, box);
+      }
+    }
+    __syncwarp();
   }
 }
 
 // ---------------------------------------------------------------------------
-// TMA-store epilogue for the linear layers with N % 128 == 0 (EPI_BF16 / EPI_GELU / EPI_ROPE / EPI_F32).
+// TMA-store epilogue for the linear layers with N % 128 == 0 (EPI_BF16 / EPI_GELU / EPI_ROPE / EPI_F32), run in
+// registers on the wgmma fragments.
 //
-// The math stays in a row-per-thread mapping -- one accumulator ROW per thread, 32 consecutive columns per load --
-// so bias, GELU and the RoPE rotation (whose (i, i+16) partners sit in the same thread) need no shuffles.  The
-// results go to a per-warp 32-row x 128-byte shared-memory box in the SWIZZLE_128B layout (conflict-free 16-byte
-// stores) and leave with ONE bulk tensor store per box issued by lane 0: no per-lane global stores, rows >= M are
-// clipped by the tensor map, and the in-place fp32 residual stream (x += proj(..)) becomes a bulk reduce-add
-// performed by the L2, so the epilogue never loads the residual.
-// accrow: this thread's accumulator row at the warp's first column.
+// Bias, GELU, ReLU and the RoPE rotation work on the fragments in place: a RoPE pair (i, i + 16) of a 32-column half-head
+// is fragment columns 8 j + 2 t and 8 (j + 2) + 2 t, both in the same thread.  The results go to a per-warp 16-row x
+// 128-byte shared-memory box in the SWIZZLE_128B layout (a 16-byte chunk is one fragment column group j, so the stores are
+// conflict-free) and leave with ONE bulk tensor store per box issued by lane 0: no per-lane global stores, rows >= M are
+// clipped by the tensor map, and the in-place fp32 residual stream (x += proj(..)) becomes a bulk reduce-add performed by
+// the L2, so the epilogue never loads the residual.  The warp's two boxes alternate (ubuf counts the boxes written).
 // ---------------------------------------------------------------------------
 template <int EPI>
-__device__ __forceinline__ void epilogue_tile_tma(const GemmParams& p, const CUtensorMap* tmC, const float* accrow, int m_tile,
-                                                  int colbase, int row_off, int quarter, uint8_t* cbuf,
-                                                  const float* rope_s) {
+__device__ __forceinline__ void epilogue_tile_tma(const GemmParams& p, const CUtensorMap* tmC, float (&acc)[2][64],
+                                                  int m_tile, int n_tile, int row_off, int wq, uint8_t* stg,
+                                                  const float* rope_s, uint32_t& ubuf) {
   using Cfg = GemmCfg<A_LINEAR, EPI, true>;
-  constexpr int CH = Cfg::BN / Cfg::PARTS;  // columns per epilogue warp
-  constexpr int NCH = CH / 32;    // 32-column chunks
   constexpr bool OUT_F32 = (EPI == EPI_F32);
   const int lane = threadIdx.x & 31;
-  const int row0 = m_tile * 128 + quarter * 32;  // first row of this warp's box (token index)
-  const int srow0 = row0 + row_off;              // ... in the output tensor (split-K partial slices)
-  const uint32_t cb = smem_u32(cbuf);
-  const uint32_t srow = cb + lane * 128;  // this thread's row inside the box
-  const uint32_t sx = lane & 7;           // 128B swizzle: 16-byte chunk j lives at j ^ (row & 7)
+  const int r = lane >> 2, t = lane & 3;
+  const int col0 = n_tile * Cfg::BN;
+  const int row0 = m_tile * 128 + 16 * wq;  // first row of this warp's 16-row group h = 0 (token index); h = 1 is + 64
 
-  [[maybe_unused]] int py = 0, px = 0;
-  if constexpr (EPI == EPI_ROPE) {
-    if (row0 + lane < p.M) {
-      const int2 pp = *reinterpret_cast<const int2*>(p.pos + 2 * static_cast<long long>(row0 + lane));
-      py = pp.x;
-      px = pp.y;
-      if (py < -1 || py > p.rope_max_pos || px < -1 || px > p.rope_max_pos)
-        __trap();  // token position outside the RoPE table (no printf: see mbar_wait)
+  // bias (adding 0 without one, as the accumulators always went through the same add)
+#pragma unroll
+  for (int j = 0; j < 16; ++j) {
+    const float2 b = p.bias ? __ldg(reinterpret_cast<const float2*>(p.bias + col0 + 8 * j + 2 * t)) : make_float2(0.f, 0.f);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      acc[h][4 * j] += b.x; acc[h][4 * j + 1] += b.y; acc[h][4 * j + 2] += b.x; acc[h][4 * j + 3] += b.y;
     }
   }
-
-  // Split-precision parity mode, bf16 outputs: the tile is drained twice -- pass 0 stores hi = bf16(v) at columns
-  // [col, ..) and [2N + col, ..), pass 1 re-reads v and stores lo = bf16(v - hi) at [N + col, ..) -- so the
-  // production register footprint is unchanged.
-  const int npass = (!OUT_F32 && p.split) ? 2 : 1;
-  const bool has_bias = p.bias != nullptr;
-#pragma unroll 1
-  for (int pass = 0; pass < npass; ++pass) {
-  // bias of chunk c is loaded one chunk ahead (warp-uniform addresses: L1 broadcast), so its latency never sits
-  // between the accumulator load and the math
-  float4 bcur[8];
+  if constexpr (EPI == EPI_GELU) {
 #pragma unroll
-  for (int j = 0; j < 8; ++j)
-    bcur[j] = has_bias ? __ldg(reinterpret_cast<const float4*>(p.bias + colbase) + j) : make_float4(0.f, 0.f, 0.f, 0.f);
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+      for (int i = 0; i < 64; ++i) acc[h][i] = gelu_erf(acc[h][i]);
+  }
+  if constexpr (EPI == EPI_BF16) {
+    if (p.relu_main) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int i = 0; i < 64; ++i) acc[h][i] = fmaxf(acc[h][i], 0.0f);
+    }
+  }
+  [[maybe_unused]] uint32_t pyx[2][2];  // [h][half]: (pos_y + 1) | (pos_x + 1) << 16 of this thread's four token rows
+  [[maybe_unused]] bool staged = true;
+  if constexpr (EPI == EPI_ROPE) {
+    // 2-D RoPE (pos_embed/pos_embed.py:149-185, curope/kernels.cu:17-82): a 32-column chunk q is one half of a 64-wide
+    // head -- the y-half (rotated by pos_y, q even) or the x-half (pos_x, q odd); inside it the pairs are (i, i + 16).
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+      for (int half = 0; half < 2; ++half) {
+        const int row = row0 + 64 * h + 8 * half + r;
+        pyx[h][half] = 0x00010001u;
+        if (row < p.M) {
+          const int2 pp = *reinterpret_cast<const int2*>(p.pos + 2 * static_cast<long long>(row));
+          if (pp.x < -1 || pp.x > p.rope_max_pos || pp.y < -1 || pp.y > p.rope_max_pos)
+            __trap();  // token position outside the RoPE table (no printf: see mbar_wait)
+          pyx[h][half] = static_cast<uint32_t>(pp.x + 1) | (static_cast<uint32_t>(pp.y + 1) << 16);
+        }
+      }
+    // does the shared-memory table hold every position of the warp?
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+      for (int half = 0; half < 2; ++half)
+        staged = staged && static_cast<int>(max(pyx[h][half] & 0xFFFFu, pyx[h][half] >> 16)) < p.rope_smem_rows;
+    staged = __all_sync(0xFFFFFFFFu, staged);
+  }
+  // RoPE of 32-column chunk q in the rows of acc[h]; run just before the chunk is written out, so the rotated values
+  // die right away.  The table rows come from shared memory when every position of the warp is staged there, else all
+  // from global memory (one address space per rotation keeps it within the register budget).
+  auto rope_chunk = [&](int h, int q) {
+    if constexpr (EPI == EPI_ROPE) {
+      if (col0 + 32 * q >= p.rope_cols) return;  // warp-uniform: the V columns are not rotated
+      auto rotate = [&](auto table_row) {
+#pragma unroll
+        for (int half = 0; half < 2; ++half) {
+          const int ps = static_cast<int>((q & 1) ? pyx[h][half] >> 16 : pyx[h][half] & 0xFFFFu);
+          const float4* tb = table_row(ps);
+#pragma unroll
+          for (int jj = 0; jj < 2; ++jj) {
+            const float4 tt = tb[4 * jj + t];  // (cos f, sin f, cos f+1, sin f+1), f = 8 jj + 2 t
+            const int ia = 4 * (4 * q + jj) + 2 * half;  // columns 8 jj + 2 t + {0, 1} of the half-head
+            const int ib = ia + 8;                       // ... + 16
+            const float a0 = acc[h][ia], b0 = acc[h][ib], a1 = acc[h][ia + 1], b1 = acc[h][ib + 1];
+            acc[h][ia] = fmaf(-b0, tt.y, a0 * tt.x);
+            acc[h][ib] = fmaf(a0, tt.y, b0 * tt.x);
+            acc[h][ia + 1] = fmaf(-b1, tt.w, a1 * tt.z);
+            acc[h][ib + 1] = fmaf(a1, tt.w, b1 * tt.z);
+          }
+        }
+      };
+      if (staged) rotate([&](int ps) { return reinterpret_cast<const float4*>(rope_s + ps * kRopeLd); });
+      else rotate([&](int ps) { return reinterpret_cast<const float4*>(p.rope_tab + static_cast<long long>(ps) * 32); });
+    }
+  };
 
+  // ---- registers -> swizzled boxes -> bulk tensor stores ----
+  // A box row is 128 bytes: 64 bf16 columns (fragment groups j = 8 c .. 8 c + 7) or 32 fp32 columns (j = 4 c .. 4 c + 3).
+  // Split-precision parity mode, bf16 outputs: hi = bf16(v) is stored at columns [col, ..) and [2N + col, ..), and
+  // lo = bf16(v - hi) from the same registers at [N + col, ..).
+  constexpr int NCH = OUT_F32 ? 4 : 2;
+  const uint32_t sb = smem_u32(stg);
+  const uint32_t sx = r;  // 128B swizzle: 16-byte chunk k of box row R lives at k ^ (R & 7), and R & 7 = r
+  auto next_box = [&]() -> uint32_t {
+    if (lane == 0) tma_store_wait_read1();  // the store that read this box two boxes ago is done with it
+    __syncwarp();
+    return sb + (ubuf++ & 1u) * Cfg::TMA_BOX_BYTES;
+  };
+  auto issue = [&](uint32_t box, int col, int row, bool second_copy) {
+    fence_proxy_async_smem();
+    __syncwarp();
+    if (lane == 0) {
+      const void* src = stg + (box - sb);
+      if constexpr (OUT_F32) {
+        if (p.c_reduce) tma_reduce_add_2d(tmC, src, col, row);
+        else tma_store_2d(tmC, src, col, row);
+      } else {
+        tma_store_2d(tmC, src, col, row);
+        if (second_copy) tma_store_2d(tmC, src, col + 2 * p.N, row);
+      }
+      tma_store_commit();
+    }
+  };
 #pragma unroll
   for (int c = 0; c < NCH; ++c) {
-    uint32_t acc[32];
-    acc_ld32(accrow + c * 32, acc);
-    float* v = reinterpret_cast<float*>(acc);
-    const int col = colbase + c * 32;
 #pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      v[4 * j] += bcur[j].x; v[4 * j + 1] += bcur[j].y; v[4 * j + 2] += bcur[j].z; v[4 * j + 3] += bcur[j].w;
-    }
-    if (c + 1 < NCH && has_bias) {
+    for (int h = 0; h < 2; ++h) {
+      const int row = row0 + 64 * h + row_off;
+      if constexpr (OUT_F32) {
+        const uint32_t box = next_box();
 #pragma unroll
-      for (int j = 0; j < 8; ++j) bcur[j] = __ldg(reinterpret_cast<const float4*>(p.bias + col + 32) + j);
-    }
-    if constexpr (EPI == EPI_GELU) {
+        for (int half = 0; half < 2; ++half)
 #pragma unroll
-      for (int i = 0; i < 32; ++i) v[i] = gelu_erf(v[i]);
-    }
-    if constexpr (EPI == EPI_BF16) {
-      if (p.relu_main) {
+          for (int jl = 0; jl < 4; ++jl) {
+            const int i = 4 * (4 * c + jl) + 2 * half;
+            asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(box + (8 * half + r) * 128 +
+                                                                   (((2 * jl + (t >> 1)) ^ sx) << 4) + (t & 1) * 8),
+                         "f"(acc[h][i]), "f"(acc[h][i + 1])
+                         : "memory");
+          }
+        issue(box, col0 + 32 * c, row, false);
+      } else {
+        const int npass = p.split ? 2 : 1;
+#pragma unroll 1
+        for (int pass = 0; pass < npass; ++pass) {
+          if (pass == 0) {
+            rope_chunk(h, 2 * c);
+            rope_chunk(h, 2 * c + 1);
+          }
+          const uint32_t box = next_box();
 #pragma unroll
-        for (int i = 0; i < 32; ++i) v[i] = fmaxf(v[i], 0.0f);
-      }
-    }
-    if constexpr (EPI == EPI_ROPE) {
-      // 2-D RoPE (pos_embed/pos_embed.py:149-185, curope/kernels.cu:17-82): a 32-column chunk is one half of a
-      // 64-wide head -- the y-half (rotated by pos_y) or the x-half (pos_x); inside it the pairs are (i, i + 16).
-      if (col < p.rope_cols) {  // warp-uniform: the V columns are not rotated
-        const int ps = (((col >> 5) & 1) ? px : py) + 1;
-        const float4* tb = (ps < p.rope_smem_rows)
-                               ? reinterpret_cast<const float4*>(rope_s + ps * kRopeLd)
-                               : reinterpret_cast<const float4*>(p.rope_tab + static_cast<long long>(ps) * 32);
+          for (int half = 0; half < 2; ++half)
 #pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          const float4 t = tb[j];  // (cos f, sin f, cos f+1, sin f+1), f = 2j
-          const float a0 = v[2 * j], b0 = v[2 * j + 16], a1 = v[2 * j + 1], b1 = v[2 * j + 17];
-          v[2 * j] = fmaf(-b0, t.y, a0 * t.x);
-          v[2 * j + 16] = fmaf(a0, t.y, b0 * t.x);
-          v[2 * j + 1] = fmaf(-b1, t.w, a1 * t.z);
-          v[2 * j + 17] = fmaf(a1, t.w, b1 * t.z);
-        }
-      }
-    }
-    // ---- registers -> swizzled box -> bulk tensor store ----
-    if constexpr (OUT_F32) {
-      // one box per chunk: 32 rows x 32 fp32 columns
-      if (lane == 0) tma_store_wait_read();
-      __syncwarp();
-#pragma unroll
-      for (int j = 0; j < 8; ++j)
-        asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(srow + ((j ^ sx) << 4)), "f"(v[4 * j]),
-                     "f"(v[4 * j + 1]), "f"(v[4 * j + 2]), "f"(v[4 * j + 3])
-                     : "memory");
-      fence_proxy_async_smem();
-      __syncwarp();
-      if (lane == 0) {
-        if (p.c_reduce) tma_reduce_add_2d(tmC, cbuf, col, srow0);
-        else tma_store_2d(tmC, cbuf, col, srow0);
-        tma_store_commit();
-      }
-    } else {
-      // one box per two chunks: 32 rows x 64 bf16 columns
-      const int sub = c & 1;
-      if (sub == 0) {
-        if (lane == 0) tma_store_wait_read();
-        __syncwarp();
-      }
-      if (pass == 1) {  // residual part: lo = v - bf16(v)
-#pragma unroll
-        for (int i = 0; i < 32; ++i) v[i] = bf16_resid(v[i]);
-      }
-#pragma unroll
-      for (int j = 0; j < 4; ++j)
-        asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(srow + (((sub * 4 + j) ^ sx) << 4)),
-                     "r"(pack_bf16x2(v[8 * j], v[8 * j + 1])), "r"(pack_bf16x2(v[8 * j + 2], v[8 * j + 3])),
-                     "r"(pack_bf16x2(v[8 * j + 4], v[8 * j + 5])), "r"(pack_bf16x2(v[8 * j + 6], v[8 * j + 7]))
-                     : "memory");
-      if (sub == 1) {
-        fence_proxy_async_smem();
-        __syncwarp();
-        if (lane == 0) {
-          tma_store_2d(tmC, cbuf, col - 32 + pass * p.N, srow0);
-          if (p.split && pass == 0) tma_store_2d(tmC, cbuf, col - 32 + 2 * p.N, srow0);  // second hi copy
-          tma_store_commit();
+            for (int jl = 0; jl < 8; ++jl) {
+              const int i = 4 * (8 * c + jl) + 2 * half;
+              const uint32_t v = pass ? pack_bf16x2_resid(acc[h][i], acc[h][i + 1]) : pack_bf16x2(acc[h][i], acc[h][i + 1]);
+              asm volatile("st.shared.b32 [%0], %1;" ::"r"(box + (8 * half + r) * 128 + ((jl ^ sx) << 4) + 4 * t), "r"(v)
+                           : "memory");
+            }
+          issue(box, col0 + 64 * c + pass * p.N, row, p.split && pass == 0);
         }
       }
     }
   }
-  }  // pass
 }
 
 template <int AMODE, int EPI, bool TMA>
@@ -545,7 +593,7 @@ gemm_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   constexpr int STAGES = Cfg::STAGES;
   constexpr uint32_t A_BYTES = Cfg::A_BYTES;
   constexpr uint32_t B_BYTES = Cfg::B_BYTES;
-  constexpr int EW = Cfg::EPI_WARPS;
+  constexpr uint32_t kOrderBar = 1;  // named barriers 1, 2: "consumer warpgroup 0 / 1 may issue its mainloop"
 
   extern __shared__ __align__(1024) uint8_t smem[];
   [[maybe_unused]] uint8_t* sA = smem;
@@ -557,9 +605,7 @@ gemm_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   [[maybe_unused]] uint64_t* hfull = bars + 2 * STAGES;  // halo tiles (A_CONV3)
   [[maybe_unused]] uint64_t* hempty = hfull + Cfg::HALO_STAGES;
   static_assert((2 * STAGES + 2 * Cfg::HALO_STAGES) * 8 <= Cfg::BAR_BYTES, "barrier area");
-  [[maybe_unused]] float* epi_smem = reinterpret_cast<float*>(smem + Cfg::OFF_EPI);
-  [[maybe_unused]] uint8_t* stg_all = smem + Cfg::OFF_STG;
-  float* acc_s = reinterpret_cast<float*>(smem + Cfg::OFF_ACC);
+  uint8_t* stg_all = smem + Cfg::OFF_STG;
   [[maybe_unused]] float* rope_s = reinterpret_cast<float*>(smem + Cfg::OFF_ROPE);
 
   const int warp = threadIdx.x >> 5;
@@ -575,13 +621,13 @@ gemm_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   if (threadIdx.x == 0) {
     if ((smem_u32(smem) & 1023u) != 0) device_fatal("dynamic shared memory is not 1024-byte aligned");
     for (int s = 0; s < STAGES; ++s) {
-      mbar_init(&full[s], 1);    // the producer's expect_tx arrival
-      mbar_init(&empty[s], EW);  // one arrival per consumer warp
+      mbar_init(&full[s], 1);  // the producer's expect_tx arrival
+      mbar_init(&empty[s], 4);  // one arrival per warp of the consumer warpgroup that read the stage
     }
     if constexpr (CONV) {
       for (int s = 0; s < Cfg::HALO_STAGES; ++s) {
         mbar_init(&hfull[s], 1);
-        mbar_init(&hempty[s], EW);
+        mbar_init(&hempty[s], 4);
       }
     }
     fence_mbar_init();
@@ -605,9 +651,10 @@ gemm_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   pdl_wait();               // previous kernel's outputs (A operand, residuals) are complete and visible
   pdl_launch_dependents();  // the next kernel may start its prologue
 
-  if (warp == 0) {
-    // ===================== TMA producer =====================
-    if (lane == 0) {
+  if (warp < 4) {
+    // ===================== TMA producer (warp 0, lane 0; warps 1-3 only give their registers away) =====================
+    setmaxnreg_dec<Cfg::PRODUCER_REGS>();
+    if (warp == 0 && lane == 0) {
       int stage = 0;
       uint32_t phase = 0;
       [[maybe_unused]] int hstage = 0;
@@ -649,90 +696,107 @@ gemm_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         }
       }
     }
-  } else if (warp >= 4) {
-    // ============ consumer warpgroups: mainloop (wgmma) + epilogue ============
-    const int wg = (warp - 4) >> 2;     // rows [64 wg, 64 wg + 64) of the tile in the mainloop
-    const int wq = (warp - 4) & 3;      // warp inside the warpgroup: 16 of those rows
-    const int quarter = warp & 3;       // epilogue mapping: rows [32 quarter, +32) ...
-    const int part = (warp - 4) >> 2;   // ... columns [part * BN / 2, +BN / 2)
-    int stage = 0;
-    uint32_t phase = 0;
-    [[maybe_unused]] int hstage = 0;
-    [[maybe_unused]] uint32_t hphase = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+  } else {
+    // ============ consumer warpgroups, ping-pong: whole tiles, mainloops in turn, epilogue under the other's mainloop ============
+    // Warpgroup wg takes tiles j = wg, wg + 2, .. of this CTA's sequence.  The ring is filled in tile order, so a
+    // warpgroup skips the stages of the other's tiles.  Turn-taking (two named barriers): before tile j > 0 wait for
+    // the other warpgroup to have issued tile j - 1; after issuing the last k-block of tile j hand the turn over if
+    // tile j + 1 exists -- so every wait meets exactly one arrival.
+    setmaxnreg_inc<Cfg::CONSUMER_REGS>();
+    const int wg = (warp - 4) >> 2;
+    const int wq = warp & 3;  // warp inside the warpgroup: rows [16 wq, +16) of each 64-row half of the tile
+    uint8_t* stg = stg_all + (warp - 4) * Cfg::STG_WARP_BYTES;
+    [[maybe_unused]] uint32_t ubuf = 0;
+    int kdone = 0;  // k-blocks (ring stages) of the CTA's earlier tiles
+    [[maybe_unused]] int hdone = 0;  // halo tiles of the CTA's earlier tiles
+    int j = 0;
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++j) {
       const int ks = tile % ksplit, mn = tile / ksplit;
+      const int kb0 = ks * nkb / ksplit, kb1 = (ks + 1) * nkb / ksplit;
+      if ((j & 1) != wg) {
+        kdone += kb1 - kb0;
+        hdone += cpb;
+        continue;
+      }
       const int m_tile = mn / n_tiles;
       const int n_tile = mn % n_tiles;
-      const int kb0 = ks * nkb / ksplit, kb1 = (ks + 1) * nkb / ksplit;
-      float acc[BN / 2];
+      int stage = kdone % STAGES;
+      uint32_t phase = (kdone / STAGES) & 1;
+      kdone += kb1 - kb0;
+      [[maybe_unused]] int hstage = hdone % Cfg::HALO_STAGES;
+      [[maybe_unused]] uint32_t hphase = (hdone / Cfg::HALO_STAGES) & 1;
+      hdone += cpb;
+
+      float acc[2][64];
 #pragma unroll
-      for (int i = 0; i < BN / 2; ++i) acc[i] = 0.0f;
-      // one k-block: four k16 steps; the previous k-block's wgmma group may still run, its stage is released
-      // once this one is issued
+      for (int i = 0; i < 64; ++i) { acc[0][i] = 0.0f; acc[1][i] = 0.0f; }
+      if (j > 0) named_bar_sync(kOrderBar + wg, 256);
+      // one k-block: four k16 steps, each two m64n128k16 wgmmas (tile rows 0-63 and 64-127); the previous k-block's
+      // wgmma group may still run, its stage is released once this one is issued
       int prev = -1;
-      auto kblock = [&](uint64_t adesc, uint64_t bdesc) {
+      auto kblock = [&](uint64_t adesc0, uint64_t adesc1, uint64_t bdesc) {
         wgmma_fence();
 #pragma unroll
-        for (int k = 0; k < 4; ++k) wgmma_m64n128k16_ss(acc, adesc + 2 * k, bdesc + 2 * k, 1u);
+        for (int k = 0; k < 4; ++k) {
+          wgmma_m64n128k16_ss(acc[0], adesc0 + 2 * k, bdesc + 2 * k, 1u);
+          wgmma_m64n128k16_ss(acc[1], adesc1 + 2 * k, bdesc + 2 * k, 1u);
+        }
         wgmma_commit();
         wgmma_wait<1>();
-        fence_regs(acc);
+        fence_regs(acc[0]);
+        fence_regs(acc[1]);
         if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
         prev = stage;
         if (++stage == STAGES) { stage = 0; phase ^= 1; }
       };
+      // the other warpgroup may issue once this tile's last k-block is issued (not finished)
+      auto hand_over = [&]() {
+        if (tile + static_cast<int>(gridDim.x) < num_tiles) named_bar_arrive(kOrderBar + (wg ^ 1), 256);
+      };
       if constexpr (CONV) {
         for (int cc = 0; cc < cpb; ++cc) {
           mbar_wait(&hfull[hstage], hphase);
-          // output pixel (y, x) of the 16 x 8 tile reads halo pixel (y + kh, x + kw); halo rows are kHaloPitch pixels,
-          // and this warpgroup's 64 rows are the output rows y = 8 wg .. 8 wg + 7
-          const uint32_t hbase = smem_u32(sH + hstage * Cfg::HALO_BYTES) + wg * 8 * kHaloPitch * 128;
+          // output pixel (y, x) of the 16 x 8 tile reads halo pixel (y + kh, x + kw); halo rows are kHaloPitch pixels.
+          // Tile rows 0-63 are the output rows y = 0..7, tile rows 64-127 are y = 8..15 (8 halo rows further).
+          const uint32_t hbase = smem_u32(sH + hstage * Cfg::HALO_BYTES);
           for (int tap = 0; tap < 9; ++tap) {
             mbar_wait(&full[stage], phase);
             const int kh = tap / 3, kw = tap - kh * 3;
-            kblock(make_smem_desc_sw128_rows(hbase + (kh * kHaloPitch + kw) * 128, kHaloPitch * 128),
+            const uint32_t tb = hbase + (kh * kHaloPitch + kw) * 128;
+            kblock(make_smem_desc_sw128_rows(tb, kHaloPitch * 128),
+                   make_smem_desc_sw128_rows(tb + 8 * kHaloPitch * 128, kHaloPitch * 128),
                    make_smem_desc_sw128(smem_u32(sB + stage * B_BYTES)));
           }
+          if (cc == cpb - 1) hand_over();
           wgmma_wait<0>();  // every read of this halo tile has completed
-          fence_regs(acc);
+          fence_regs(acc[0]);
+          fence_regs(acc[1]);
           if (lane == 0) mbar_arrive(&hempty[hstage]);
           if (++hstage == Cfg::HALO_STAGES) { hstage = 0; hphase ^= 1; }
         }
       } else {
         for (int kb = kb0; kb < kb1; ++kb) {
           mbar_wait(&full[stage], phase);
-          kblock(make_smem_desc_sw128(smem_u32(sA + stage * A_BYTES) + wg * 64 * 128),
+          const uint32_t a = smem_u32(sA + stage * A_BYTES);
+          kblock(make_smem_desc_sw128(a), make_smem_desc_sw128(a + 64 * 128),
                  make_smem_desc_sw128(smem_u32(sB + stage * B_BYTES)));
         }
+        hand_over();
       }
       wgmma_wait<0>();
-      fence_regs(acc);
+      fence_regs(acc[0]);
+      fence_regs(acc[1]);
       if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
 
-      // accumulators -> shared tile (wgmma layout: register 4j + {0,1} = row g, columns 8j + 2t + {0,1}; 4j + {2,3} = row g + 8)
-      named_bar_sync(1, Cfg::EPI_THREADS);  // the previous tile's epilogue has finished reading the tile
-      {
-        const int r0 = wg * 64 + wq * 16 + (lane >> 2);
-        const int c0 = 2 * (lane & 3);
-#pragma unroll
-        for (int j = 0; j < BN / 8; ++j) {
-          *reinterpret_cast<float2*>(acc_s + r0 * Cfg::ACC_LD + 8 * j + c0) = make_float2(acc[4 * j], acc[4 * j + 1]);
-          *reinterpret_cast<float2*>(acc_s + (r0 + 8) * Cfg::ACC_LD + 8 * j + c0) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
-        }
-      }
-      named_bar_sync(1, Cfg::EPI_THREADS);
-      const int cols_w = BN / Cfg::PARTS;
       if constexpr (TMA) {
-        epilogue_tile_tma<EPI>(p, &tmC, acc_s + (quarter * 32 + lane) * Cfg::ACC_LD + part * cols_w, m_tile,
-                               n_tile * BN + part * cols_w, ks * p.split_rows, quarter,
-                               stg_all + (warp - 4) * Cfg::STG_WARP_BYTES, rope_s);
+        epilogue_tile_tma<EPI>(p, &tmC, acc, m_tile, n_tile, ks * p.split_rows, wq, stg, rope_s, ubuf);
+        // After the warpgroup's last tile: the bulk stores read this CTA's shared memory.  (Waiting here rather than
+        // after the tile loop matters: with the wait after the loop, ptxas kept the consumer code inside the
+        // 168-register launch budget instead of the setmaxnreg budget, and the RoPE epilogue spilled.)
+        if (tile + 2 * static_cast<int>(gridDim.x) >= num_tiles && lane == 0) tma_store_wait_all();
       } else {
-        epilogue_tile<AMODE, EPI>(p, acc_s + quarter * 32 * Cfg::ACC_LD + part * cols_w, m_tile, n_tile, quarter, part,
-                                  epi_smem);
+        epilogue_tile<AMODE, EPI>(p, acc, m_tile, n_tile, wq, reinterpret_cast<float*>(stg));
       }
-    }
-    if constexpr (TMA) {
-      if (lane == 0) tma_store_wait_all();  // the bulk stores read this CTA's shared memory
     }
   }
 }
