@@ -154,6 +154,13 @@ int sta_op_gemm(const StaGemmDesc* d, void* stream);
 int sta_op_attention(const void* q, int64_t ldq, int q_col0, const void* k, int64_t ldk, int k_col0, const void* v,
                      int64_t ldv, int v_col0, void* out, int64_t ldo, int batch, int heads, int nq, int nk,
                      int kv_batch_shift, float scale, void* stream);
+/* The same in the split-precision parity mode (STA_PRECISION_X3): q/k/v/out rows are (hi | lo | hi) bf16, ld* are the
+ * physical strides (3x the logical width) and *_col0 are offsets of the hi columns; out stores (hi | lo | hi).
+ * Requires 0 <= kv_batch_shift < batch, *_col0 + 64*heads <= ld* (ld* / 3 in split mode), 64*heads <= ldo (ldo / 3)
+ * and a finite scale > 0 (both entry points). */
+int sta_op_attention_split(const void* q, int64_t ldq, int q_col0, const void* k, int64_t ldk, int k_col0,
+                           const void* v, int64_t ldv, int v_col0, void* out, int64_t ldo, int batch, int heads, int nq,
+                           int nk, int kv_batch_shift, float scale, void* stream);
 
 int sta_op_layernorm(const float* x, int rows, int C, float eps, const float* g1, const float* b1, void* out1_bf16,
                      const float* g2, const float* b2, void* out2_bf16, int drop_first_of, void* stream);

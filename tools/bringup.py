@@ -309,8 +309,9 @@ def group_attention():
             k, v = k[idx], v[idx]
         ref = F.scaled_dot_product_attention(q, k, v, scale=0.125).transpose(1, 2).reshape(batch, n, C)
         report("attention b%d h%d n%d shift%d" % (batch, heads, n, shift), out, ref, 2e-2)
-    # adversarial for the lazy-rescale / speculative-maximum path: the keys of later tiles score much higher than those
-    # of earlier ones (row maxima jump by far more than 2^8 between key tiles), some rows only in the ragged last tile.
+    # the online-softmax rescale: the keys of later tiles score much higher than those of earlier ones, so every new key
+    # tile raises the running row maximum and rescales the accumulated O and l (factors far below 2^-8), for some rows
+    # only in the ragged last tile.
     # 3 heads: 30 CTAs of 128 rows would leave SMs idle -> 64-row tiles; 16 heads: 160 CTAs -> 128-row tiles.
     batch, n = 2, 600
     for heads in (3, 16):

@@ -88,6 +88,7 @@ def lib():
     L.sta_profile_read.argtypes = [vp, POINTER(ctypes.c_double), POINTER(c_int64), POINTER(ctypes.c_double)]
     L.sta_op_gemm.argtypes = [POINTER(StaGemmDesc), vp]
     L.sta_op_attention.argtypes = [vp, i64, i, vp, i64, i, vp, i64, i, vp, i64, i, i, i, i, i, c_float, vp]
+    L.sta_op_attention_split.argtypes = L.sta_op_attention.argtypes
     L.sta_op_layernorm.argtypes = [vp, i, i, c_float, vp, vp, vp, vp, vp, vp, i, vp]
     L.sta_op_patch_im2col.argtypes = [vp, i, i, i, i, vp, vp]
     L.sta_op_upsample2x.argtypes = [vp, vp, i, i, i, i, vp]

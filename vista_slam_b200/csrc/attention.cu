@@ -21,6 +21,7 @@
 #include "common.cuh"
 #include "host_util.h"
 
+#include <math.h>
 #include <stdio.h>
 #include "ops.h"
 
@@ -343,9 +344,21 @@ int launch_attention(const AttnLaunch& a, cudaStream_t stream) {
   STA_REQUIRE(a.batch > 0 && a.heads > 0 && a.nq > 0 && a.nk > 0, "empty attention problem");
   STA_REQUIRE(a.ldq % 8 == 0 && a.ldk % 8 == 0 && a.ldv % 8 == 0 && a.ldo % 8 == 0, "row strides must be 16B multiples");
   STA_REQUIRE(a.q_col0 % 8 == 0 && a.k_col0 % 8 == 0 && a.v_col0 % 8 == 0, "column offsets must be 16B multiples");
-  if (a.split) {
+  if (a.split)
     STA_REQUIRE(a.ldq % 3 == 0 && a.ldk % 3 == 0 && a.ldv % 3 == 0 && a.ldo % 3 == 0 && (a.ldo / 3) % 8 == 0,
                 "split-precision rows are (hi | lo | hi): strides must be 3 x the logical width");
+  // Out-of-range values would not fail loudly: the TMA loads zero-fill coordinates outside a tensor map (a negative
+  // sample gives all-zero scores and values), while the split kernel reads whatever lies in front of or after a row.
+  // In split mode the *_col0 are hi-column offsets within the logical width ld / 3.
+  const long long wdiv = a.split ? 3 : 1, hcols = 64LL * a.heads;
+  STA_REQUIRE(a.kv_batch_shift >= 0 && a.kv_batch_shift < a.batch, "kv_batch_shift must lie in [0, batch)");
+  STA_REQUIRE(a.q_col0 >= 0 && a.q_col0 + hcols <= a.ldq / wdiv, "q head columns run past the row width");
+  STA_REQUIRE(a.k_col0 >= 0 && a.k_col0 + hcols <= a.ldk / wdiv, "k head columns run past the row width");
+  STA_REQUIRE(a.v_col0 >= 0 && a.v_col0 + hcols <= a.ldv / wdiv, "v head columns run past the row width");
+  STA_REQUIRE(hcols <= a.ldo / wdiv, "output rows are narrower than 64 x heads");
+  // the wgmma kernel takes the row maximum of the raw scores and scales afterwards: that is the maximum only for scale > 0
+  STA_REQUIRE(std::isfinite(a.scale) && a.scale > 0.0f, "scale must be finite and positive");
+  if (a.split) {
     STA_REQUIRE(a.heads <= 65535 && a.batch <= 65535, "grid limits");
     STA_CHECK_CUDA(launch_pdl(attention_x3_kernel, dim3((a.nq + 127) / 128, a.heads, a.batch), dim3(128), 0, stream, 1, a.q,
                               a.ldq, a.q_col0, a.k, a.ldk, a.k_col0, a.v, a.ldv, a.v_col0, a.out, a.ldo, a.nq, a.nk, a.batch,

@@ -1640,9 +1640,9 @@ int sta_op_gemm(const StaGemmDesc* d, void* stream) {
   return launch_gemm(g, static_cast<cudaStream_t>(stream));
 }
 
-int sta_op_attention(const void* q, int64_t ldq, int q_col0, const void* k, int64_t ldk, int k_col0, const void* v,
-                     int64_t ldv, int v_col0, void* out, int64_t ldo, int batch, int heads, int nq, int nk,
-                     int kv_batch_shift, float scale, void* stream) {
+static int op_attention(const void* q, int64_t ldq, int q_col0, const void* k, int64_t ldk, int k_col0, const void* v,
+                        int64_t ldv, int v_col0, void* out, int64_t ldo, int batch, int heads, int nq, int nk,
+                        int kv_batch_shift, float scale, int split, void* stream) {
   AttnLaunch a;
   a.q = static_cast<const bf16*>(q); a.ldq = ldq; a.q_col0 = q_col0;
   a.k = static_cast<const bf16*>(k); a.ldk = ldk; a.k_col0 = k_col0;
@@ -1651,7 +1651,20 @@ int sta_op_attention(const void* q, int64_t ldq, int q_col0, const void* k, int6
   a.batch = batch; a.heads = heads; a.nq = nq; a.nk = nk;
   a.kv_batch_shift = kv_batch_shift;
   a.scale = scale;
+  a.split = split;
   return launch_attention(a, static_cast<cudaStream_t>(stream));
+}
+int sta_op_attention(const void* q, int64_t ldq, int q_col0, const void* k, int64_t ldk, int k_col0, const void* v,
+                     int64_t ldv, int v_col0, void* out, int64_t ldo, int batch, int heads, int nq, int nk,
+                     int kv_batch_shift, float scale, void* stream) {
+  return op_attention(q, ldq, q_col0, k, ldk, k_col0, v, ldv, v_col0, out, ldo, batch, heads, nq, nk, kv_batch_shift,
+                      scale, 0, stream);
+}
+int sta_op_attention_split(const void* q, int64_t ldq, int q_col0, const void* k, int64_t ldk, int k_col0,
+                           const void* v, int64_t ldv, int v_col0, void* out, int64_t ldo, int batch, int heads, int nq,
+                           int nk, int kv_batch_shift, float scale, void* stream) {
+  return op_attention(q, ldq, q_col0, k, ldk, k_col0, v, ldv, v_col0, out, ldo, batch, heads, nq, nk, kv_batch_shift,
+                      scale, 1, stream);
 }
 
 int sta_op_layernorm(const float* x, int rows, int C, float eps, const float* g1, const float* b1, void* out1_bf16,
