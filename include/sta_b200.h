@@ -342,6 +342,51 @@ int sta_op_bow_score(const int32_t* qw, const double* qv, const int32_t* q_len_d
                      const double* db_val, const int64_t* db_start, const int32_t* db_len, int nviews, double* sims_out,
                      void* stream);
 
+/* ---- device pose graph: the bookkeeping of OnlineSLAM (vista_slam/slam.py:191-241 over pose_graph.py:5-54) and the
+ * gather of save_data_all / get_view (slam.py:299-412) on the device.  A graph handle owns fixed-capacity device tables,
+ * all poses starting as the identity (PoseGraphNodes.reset):
+ *   per node  pose [max_nodes][8] fp32 Sim3 in PyPose's layout (tx ty tz | qx qy qz qw | s), depth and conf
+ *             [max_nodes][H][W] fp32, intri [max_nodes][3][3], conf mean [max_nodes] fp32, node_to_view and
+ *             node_to_connected_view [max_nodes] int64 (-1 = unused);
+ *   per view  best node [max_views] int64 (-1) and its conf mean [max_views] fp32 (-100);
+ *   per edge  endpoints [max_edges][2] int64 (-1), measurement [max_edges][8] fp32 Sim3, weight [max_edges][7] fp32 (1).
+ * The map store is 8 H W max_nodes bytes: 1.44 GB at OnlineSLAM's defaults (3600 nodes) and 224 x 224.
+ * sta_graph_tables: the 12 device pointers in that order (pose, depth, conf, intri, conf mean, node_to_view,
+ * node_to_connected_view, best node, best mean, edges, measurements, weights). ---- */
+typedef struct StaGraph StaGraph; /* opaque */
+enum { STA_GRAPH_MAX_KEYFRAME_EDGES = 32, STA_GRAPH_FLAG_NOT_SO3 = 1 };
+int sta_graph_create(int max_nodes, int max_edges, int max_views, int H, int W, StaGraph** out);
+void sta_graph_destroy(StaGraph* g);
+int sta_graph_tables(const StaGraph* g, void** out12);
+/* Back to the state of sta_graph_create; clears the flags. */
+int sta_graph_reset(StaGraph* g, void* stream);
+/* Flags the device has raised (STA_GRAPH_FLAG_NOT_SO3: a pose rotation was not orthonormal with det +1 to 1e-3, which
+ * pp.mat2SE3(atol=1e-3) refuses).  The flags live in mapped host memory: this reads them without synchronising, so a
+ * flag raised by a launch is visible once the caller has synchronised with it. */
+int sta_graph_flags(const StaGraph* g, int* flags_out);
+/* Insert the n kept edges (i = view, j = js_host[k]) of one keyframe in the reference's order (connect_view_i_j per edge:
+ * node of i, its scale edge to i's first node when k > 0, node of j, its scale edge to first_j_host[k] when that is
+ * >= 0, then the pose edge (i, j)).  Node slots are node0 + 2k (i) and node0 + 2k + 1 (j); edges fill edge0, edge0 + 1, ...
+ * Host integers: js_host, cand_host (row of edge k in pose_dev / pose_conf_dev), first_j_host (first node of view j when
+ * edge k is inserted, -1 if none).  Device inputs, as regress_views_gated leaves them: pose_dev [*][4][4], pose_conf_dev
+ * [*], confs_dev / depths_dev [2][n][H][W] (row 0 view i, row 1 view j), intri_dev [n][3][3], conf_mean_dev [2][n].
+ * Two launches, no host synchronisation.  Refused before any launch: a capacity overflow, a map size other than the
+ * graph's, host memory as input, n outside [1, STA_GRAPH_MAX_KEYFRAME_EDGES]. */
+int sta_graph_add_keyframe(StaGraph* g, int view, int n, const int64_t* js_host, const int* cand_host,
+                           const int* first_j_host, int node0, int edge0, int H, int W, const float* pose_dev,
+                           const float* pose_conf_dev, const float* confs_dev, const float* depths_dev, const float* intri_dev,
+                           const float* conf_mean_dev, void* stream);
+/* Per view v in [view0, view0 + num_views), through its best node (every view must have one): pose_out [V][4][4] (rotation
+ * and translation, scale dropped), scale_out [V], depth_out / conf_out [V][H][W] (unscaled), intri_out [V][3][3].
+ * With points_out: the world point cloud of save_data_all -- depth s unprojected with K^-1, then R p + t, points with
+ * conf > conf_thres in (view, row, column) order, colours (img + 1) / 2 from imgs_dev [V][3][H][W] -- into points_out /
+ * colors_out [V H W][3] and *count_out (device int64).  scratch: sta_graph_export_scratch_bytes(V, H), 8-byte aligned.
+ * One launch without the cloud, three with it (count, exclusive scan, scatter); no host synchronisation. */
+size_t sta_graph_export_scratch_bytes(int num_views, int H);
+int sta_graph_export(StaGraph* g, int view0, int num_views, float conf_thres, const float* imgs_dev, float* pose_out,
+                     float* scale_out, float* depth_out, float* conf_out, float* intri_out, float* points_out,
+                     float* colors_out, int64_t* count_out, void* scratch, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -35,6 +35,8 @@ class StaGemmDesc(Structure):
 
 
 FLOW_MAX_CORNERS = 1000
+GRAPH_MAX_KEYFRAME_EDGES = 32
+GRAPH_FLAG_NOT_SO3 = 1
 ORB_MAX_KEYPOINTS = 4096
 
 
@@ -138,6 +140,17 @@ def lib():
     L.sta_op_bow_transform.argtypes = [vp, vp, i, vp, vp, vp]
     L.sta_op_bow_vector.argtypes = [vp, vp, vp, i, vp, vp, vp, vp]
     L.sta_op_bow_score.argtypes = [vp, vp, vp, vp, vp, vp, vp, i, vp, vp]
+    L.sta_graph_create.argtypes = [i, i, i, i, i, POINTER(vp)]
+    L.sta_graph_destroy.argtypes = [vp]
+    L.sta_graph_destroy.restype = None
+    L.sta_graph_tables.argtypes = [vp, POINTER(vp)]
+    L.sta_graph_reset.argtypes = [vp, vp]
+    L.sta_graph_flags.argtypes = [vp, POINTER(c_int)]
+    L.sta_graph_add_keyframe.argtypes = [vp, i, i, POINTER(c_int64), POINTER(c_int), POINTER(c_int), i, i, i, i, vp, vp, vp, vp,
+                                         vp, vp, vp]
+    L.sta_graph_export_scratch_bytes.argtypes = [i, i]
+    L.sta_graph_export_scratch_bytes.restype = ctypes.c_size_t
+    L.sta_graph_export.argtypes = [vp, i, i, c_float, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]
     _lib = L
     return L
 

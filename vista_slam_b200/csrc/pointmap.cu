@@ -9,39 +9,16 @@
 //
 // One pass over the data: per-thread fp32 partial sums -> warp shuffles -> one fp64 record per block; a second
 // tiny kernel combines the records in a fixed order in fp64 (deterministic, no atomics) and writes K / scale.
+// The scale reduction lives in pointmap.cuh, which the device pose graph (slam_graph.cu) shares.
 // 16 bytes read + 4 bytes written per pixel: the kernel is HBM-bound (100 MB at cfg-2, ~16 us).
 #include "common.cuh"
 #include "host_util.h"
 #include "ops.h"
+#include "pointmap.cuh"
 
 namespace sta {
 
 namespace {
-
-constexpr int kStatBlocks = 64;  // partial records per view
-constexpr int kStatVals = 8;     // doubles per record (5 used by the intrinsics pass, 3 by the scale pass)
-
-template <int NV>
-__device__ __forceinline__ void block_reduce_store(float (&s)[NV], double* rec) {
-  __shared__ float red[8][NV];
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-#pragma unroll
-  for (int i = 0; i < NV; ++i) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) s[i] += __shfl_xor_sync(0xffffffffu, s[i], o);
-  }
-  if (lane == 0) {
-#pragma unroll
-    for (int i = 0; i < NV; ++i) red[warp][i] = s[i];
-  }
-  __syncthreads();
-  if (threadIdx.x < NV) {
-    double t = 0.0;
-#pragma unroll
-    for (int w = 0; w < 8; ++w) t += static_cast<double>(red[w][threadIdx.x]);
-    rec[threadIdx.x] = t;
-  }
-}
 
 // grid (kStatBlocks, V), 256 threads
 __global__ void __launch_bounds__(256)
@@ -126,26 +103,14 @@ scale_stats_kernel(const float* __restrict__ Di, const float* __restrict__ Dj, c
                    const float* __restrict__ cj, long long n, double* __restrict__ partial) {
   pdl_wait();
   pdl_launch_dependents();
-  float s[3] = {0.f, 0.f, 0.f};
-  for (long long i = blockIdx.x * 256 + threadIdx.x; i < n; i += kStatBlocks * 256) {
-    const float a = Di[i], b = Dj[i], cc = ci[i] * cj[i];
-    const float w = fmaxf(cc, 1e-6f);
-    s[0] += w * a * b;
-    s[1] += w * a * a;
-    s[2] += sqrtf(cc);
-  }
-  block_reduce_store<3>(s, partial + static_cast<long long>(blockIdx.x) * kStatVals);
+  scale_partial(Di, Dj, ci, cj, n, blockIdx.x, partial + static_cast<long long>(blockIdx.x) * kStatVals);
 }
 
 __global__ void scale_finalize_kernel(const double* __restrict__ partial, long long n, float* __restrict__ out2) {
   pdl_wait();
   pdl_launch_dependents();
   if (threadIdx.x != 0) return;
-  double t[3] = {0.0, 0.0, 0.0};
-  for (int b = 0; b < kStatBlocks; ++b)
-    for (int i = 0; i < 3; ++i) t[i] += partial[static_cast<long long>(b) * kStatVals + i];
-  out2[0] = static_cast<float>(t[0] / t[1]);
-  out2[1] = static_cast<float>(t[2] / static_cast<double>(n));
+  scale_finalize(partial, n, out2);
 }
 
 }  // namespace

@@ -105,14 +105,22 @@ class KeyframeFrontend:
             conf = f32(2, n, H, W)
             intri = f32(n, 3, 3)
             depth = f32(2, n, H, W)
+            cmean = f32(2, n)
             idx = (ctypes.c_int * n)(*keep)
             _lib.check(L.sta_regress_pairs_finish(m._handle, idx, n, _lib.ptr(pts), _lib.ptr(conf), _lib.ptr(intri),
-                                                  _lib.ptr(depth), None, _lib.ptr(_scratch_for(dev, 2 * n)), _lib.cur_stream()),
+                                                  _lib.ptr(depth), _lib.ptr(cmean), _lib.ptr(_scratch_for(dev, 2 * n)),
+                                                  _lib.cur_stream()),
                        "sta_regress_pairs_finish")
         for pos, k in enumerate(keep):
             out[k] = (pose[0, k:k + 1], pconf[0, k:k + 1], conf[:, pos], intri[pos], depth[:, pos])
         self.last_pts3d = pts  # [2, n, H, W, 3] of the kept edges (diagnostics / tests)
         self.last_kept = keep
+        # the compact outputs of the kept edges, as the device pose graph takes them (OnlineSLAM.step):
+        # pose [K, 4, 4] and pose_conf [K] of all candidates (i -> j), conf / depths [2, n, H, W], intri [n, 3, 3],
+        # conf_mean [2, n]; and the K confidences read back for the gate
+        self.last_conf_host = [float(c) for c in conf_host]
+        self.last_batch = {"pose": pose[0], "pose_conf": pconf[0], "conf": conf, "depths": depth, "intri": intri,
+                           "conf_mean": cmean}
         return out
 
     @torch.no_grad()

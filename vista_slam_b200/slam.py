@@ -1,0 +1,463 @@
+"""Drop-in `OnlineSLAM` (vista_slam/slam.py) that keeps the pose graph and the map on the device.
+
+Same constructor (arguments and defaults) and the surface run.py, run_live.py and the evaluation scripts use: `device`,
+`verbose`, `view_num`, `imgs`, `flow_tracker`, `lc_detector`, `frontend`, `time_dict`, `load_frontend`, `step`, `reset`,
+`pose_graph_optimize`, `get_view`, `get_view_graph`, `save_data_all`, `get_pointmap_vis`, `save_pointmap`,
+`get_time_dict`.  It is built from this package's stages:
+
+  * KeyframeFrontend.regress_views_gated: one decoder pass over all candidate edges of a keyframe, one read-back of their
+    pose confidences (the gate), DPT heads and pointmap consumers for the kept edges only;
+  * LoopDetector and FlowTracker on the device;
+  * the device pose graph (csrc/slam_graph.cu, `sta_graph_*`): node / edge tables, the depth / confidence / intrinsics
+    store and the per-view best node live in fixed-capacity device arrays sized from the reference's formulas
+    (slam.py:33-36).  The map store takes 8 H W max_nodes bytes: 1.44 GB at the defaults (3600 nodes) and 224 x 224.
+    A keyframe's kept edges go in with two launches and no host synchronisation; save_data_all / get_view gather on the
+    device, and the world point cloud is built and compacted there (count, exclusive scan, scatter);
+  * PoseGraphOpt, working on slices of the node and edge tables.
+
+A step synchronises with the host twice, as the GPU stages need: the loop-candidate read (detect_loop runs first: it
+does not depend on the neighbour edges) and the gate read.  PGO iterations read back their accept / reject decision.
+A rotation that is not orthonormal (pp.mat2SE3(atol=1e-3) would raise) raises a device flag, which is read at the next
+of those read-backs and raises ValueError there.
+
+Importing this module does not import pypose, munch, colorama or open3d.  `get_view` returns a `View` (attribute and key
+access, as munch.Munch).  The PLY of save_data_all is written here: binary little-endian, float x y z and uchar
+red green blue (colours rounded from [0, 1]); whether that is byte-identical to open3d's writer is not checked."""
+import ctypes
+import os
+import time
+
+import numpy as np
+import torch
+from tqdm import tqdm
+
+from . import _lib
+from .flow_tracker import FlowTracker
+from .keyframe import KeyframeFrontend
+from .loop_detector import LoopDetector
+from .pose_graph import PoseGraphOpt
+
+def _msg(prefix, text):
+    """print_msg (utils/slam_utils.py:448-450) without colours."""
+    tqdm.write(prefix + text)
+
+
+class View(dict):
+    """A dict with attribute access (what munch.Munch gives get_view's callers)."""
+
+    def __getattr__(self, k):
+        try:
+            return self[k]
+        except KeyError:
+            raise AttributeError(k) from None
+
+    def __setattr__(self, k, v):
+        self[k] = v
+
+
+class _DeviceImages(list):
+    """The input images, kept on the device; reading one copies it to the host, as the reference's list holds
+    image.squeeze(0).cpu() (slam.py:148)."""
+
+    def __getitem__(self, v):
+        x = list.__getitem__(self, v)
+        return [t.cpu() for t in x] if isinstance(v, slice) else x.cpu()
+
+    def __iter__(self):
+        return (t.cpu() for t in list.__iter__(self))
+
+    def device_stack(self):
+        return torch.stack(list(list.__iter__(self)))
+
+
+class _DevArray:
+    def __init__(self, ptr, shape, typestr):
+        self.__cuda_array_interface__ = {"data": (ptr, False), "shape": tuple(shape), "typestr": typestr, "version": 3,
+                                         "strides": None}
+
+
+class _Graph:
+    """Owner of one sta_graph handle and torch views of its tables."""
+
+    def __init__(self, max_nodes, max_edges, max_views, H, W, device):
+        self.H, self.W, self.device = H, W, device
+        self.max_nodes, self.max_edges, self.max_views = max_nodes, max_edges, max_views
+        L = _lib.lib()
+        h = ctypes.c_void_p()
+        with torch.cuda.device(device):
+            _lib.check(L.sta_graph_create(max_nodes, max_edges, max_views, H, W, ctypes.byref(h)), "sta_graph_create")
+        self.h = h
+        p = (ctypes.c_void_p * 12)()
+        _lib.check(L.sta_graph_tables(h, p), "sta_graph_tables")
+        f4, i8 = "<f4", "<i8"
+        spec = [("pose", (max_nodes, 8), f4), ("depth", (max_nodes, H, W), f4), ("conf", (max_nodes, H, W), f4),
+                ("intri", (max_nodes, 3, 3), f4), ("cmean", (max_nodes,), f4), ("node_to_view", (max_nodes,), i8),
+                ("node_to_connected_view", (max_nodes,), i8), ("best_node", (max_views,), i8),
+                ("best_mean", (max_views,), f4), ("edges", (max_edges, 2), i8), ("meas", (max_edges, 8), f4),
+                ("weight", (max_edges, 7), f4)]
+        for k, (name, shape, ts) in enumerate(spec):
+            setattr(self, name, torch.as_tensor(_DevArray(p[k], shape, ts), device=device))
+
+    def __del__(self):
+        if getattr(self, "h", None) and _lib._lib is not None:
+            _lib.lib().sta_graph_destroy(self.h)
+            self.h = None
+
+    def flags(self):
+        f = ctypes.c_int()
+        _lib.check(_lib.lib().sta_graph_flags(self.h, ctypes.byref(f)), "sta_graph_flags")
+        return f.value
+
+
+class OnlineSLAM:
+    def __init__(self, ckpt_path: str, vocab_path: str,
+                 verbose: bool = False, max_view_num: int = 400,
+                 neighbor_edge_num: int = 3, loop_edge_num: int = 3,
+                 loop_dist_min: int = 40, loop_nms: int = 40,
+                 loop_cand_thresh_neighbor: int = 5,
+                 conf_thres: float = 4.2, rel_pose_thres: float = 0.75,
+                 flow_thres: float = 5.0, pgo_every: int = 500, live_mode: bool = False):
+        self.device = torch.device("cuda")
+        self.verbose = verbose
+        self.max_view_num = max_view_num
+        self.neighbor_edge_num = neighbor_edge_num
+        self.loop_edge_num = loop_edge_num
+        # slam.py:33-36
+        self.max_nodes = max_view_num * (neighbor_edge_num * 2 + loop_edge_num)
+        scale_edges_num = neighbor_edge_num * 2 + loop_edge_num - 1
+        pose_edges_num = (neighbor_edge_num * 2 + loop_edge_num) // 2 + 1
+        self.max_edges = max_view_num * (scale_edges_num + pose_edges_num)
+        self.conf_thres = conf_thres
+        self.rel_pose_thres = rel_pose_thres
+
+        self.frontend = self.load_frontend(ckpt_path)
+        total_params = sum(p.numel() for p in self.frontend.parameters())
+        if self.verbose:
+            _msg("[INFO] ", f"Total parameters: {total_params}")
+        self.kf = KeyframeFrontend(self.frontend)
+        self.img_shapes = []
+        self.imgs = _DeviceImages()
+        self.view_names = []
+
+        self.lc_detector = LoopDetector(vocab_path, loop_dist_min, loop_nms, loop_cand_thresh_neighbor)
+        self.image_resolution = (224, 224)
+        self.view_num = 0
+        self.pgo_every = pgo_every
+        self.flow_tracker = FlowTracker(flow_thres)
+        self.time_dict = self._zero_times()
+        self.live_mode = live_mode
+        self.loop_related_views = set()
+        self.pgo_window_size = 2 * pgo_every
+        self._graph = None  # created at the first keyframe, when the map size is known
+        self._reset_host_graph()
+
+    @staticmethod
+    def _zero_times():
+        return {"prepare_data": 0.0, "encoder": 0.0, "decoder": 0.0, "lc": 0.0, "pgo": 0.0, "graph_construction": 0.0}
+
+    def _reset_host_graph(self):
+        # integer mirror of PoseGraphNodes' lists (pose_graph.py:48-54): all of them follow from the keep decisions
+        self.view_to_node = {}
+        self.node_to_connected_view = []
+        self.num_nodes = 0
+        self.num_edges = 0
+
+    def reset(self):
+        """slam.py:76-93: the loop detector and loop_related_views are not reset."""
+        self.kf = KeyframeFrontend(self.frontend)
+        self.img_shapes = []
+        self.imgs = _DeviceImages()
+        self.view_names = []
+        self.view_num = 0
+        if self._graph is not None:
+            with torch.cuda.device(self._graph.device):
+                _lib.check(_lib.lib().sta_graph_reset(self._graph.h, _lib.cur_stream()), "sta_graph_reset")
+        self._reset_host_graph()
+        self.flow_tracker.reset()
+        self.time_dict = self._zero_times()
+
+    def load_frontend(self, ckpt_path: str):
+        from .sta_model.sta_model import SymmetricTwoViewAssociation as STA
+        frontend = STA()
+        checkpoint = torch.load(ckpt_path, map_location="cpu", weights_only=False)
+        frontend.load_state_dict(checkpoint["model"], strict=True)
+        del checkpoint
+        frontend.to(self.device)
+        frontend.eval()
+        return frontend
+
+    # ------------------------------------------------------------------------------------------------ graph
+    def _ensure_graph(self, image):
+        H, W = int(image.shape[-2]), int(image.shape[-1])
+        if self._graph is None:
+            self._graph = _Graph(self.max_nodes, self.max_edges, self.max_nodes, H, W, self.device)
+            self._identity = torch.zeros(8, dtype=torch.float32, device=self.device)
+            self._identity[6:] = 1.0
+
+    def _check_flags(self):
+        """Called right after a read-back, so every earlier graph launch has completed."""
+        if self._graph is not None and self._graph.flags() & _lib.GRAPH_FLAG_NOT_SO3:
+            raise ValueError("a relative pose's rotation is not orthonormal (pp.mat2SE3(atol=1e-3) refuses it)")
+
+    def _regress_keyframe(self, i, js):
+        """The frontend's part of a keyframe: (the K pose confidences on the host, indices of the kept candidates, the
+        device batch {pose [K,4,4], pose_conf [K], conf / depths [2,n,H,W], intri [n,3,3], conf_mean [2,n]})."""
+        out = self.kf.regress_views_gated(i, js, self.rel_pose_thres)
+        keep = [k for k, o in enumerate(out) if o[2] is not None]
+        return self.kf.last_conf_host, keep, self.kf.last_batch
+
+    def _add_keyframe(self, i, js, keep, batch):
+        """connect_view_i_j (slam.py:191-241) for the kept edges, in order: host integers, then two launches."""
+        g = self._graph
+        n = len(keep)
+        kept_js = [js[k] for k in keep]
+        if n > _lib.GRAPH_MAX_KEYFRAME_EDGES:
+            raise ValueError("at most %d kept edges per keyframe" % _lib.GRAPH_MAX_KEYFRAME_EDGES)
+        v2n = {v: list(self.view_to_node.get(v, [])) for v in set(kept_js) | {i}}
+        first_j, n_scale = [], n - 1
+        for k, j in enumerate(kept_js):
+            v2n[i].append(self.num_nodes + 2 * k)
+            first_j.append(v2n[j][0] if v2n[j] else -1)
+            n_scale += first_j[-1] >= 0
+            v2n[j].append(self.num_nodes + 2 * k + 1)
+        if self.num_nodes + 2 * n > g.max_nodes or i >= g.max_views:
+            raise IndexError("pose graph node capacity (%d) exceeded" % g.max_nodes)
+        if self.num_edges + n_scale + n > g.max_edges:
+            raise IndexError("pose graph edge capacity (%d) exceeded" % g.max_edges)
+        H, W = batch["conf"].shape[-2:]
+        args = ((ctypes.c_int64 * n)(*kept_js), (ctypes.c_int * n)(*keep), (ctypes.c_int * n)(*first_j))
+        with torch.cuda.device(g.device):
+            _lib.check(_lib.lib().sta_graph_add_keyframe(
+                g.h, i, n, *args, self.num_nodes, self.num_edges, H, W, _lib.ptr(batch["pose"]), _lib.ptr(batch["pose_conf"]),
+                _lib.ptr(batch["conf"]), _lib.ptr(batch["depths"]), _lib.ptr(batch["intri"]), _lib.ptr(batch["conf_mean"]),
+                _lib.cur_stream()), "sta_graph_add_keyframe")
+        self.view_to_node.update(v2n)
+        for j in kept_js:
+            self.node_to_connected_view += [j, i]
+        self.num_nodes += 2 * n
+        self.num_edges += n_scale + n
+
+    # ------------------------------------------------------------------------------------------------ step
+    def add_view(self, image, image_shape, view_name):
+        self.kf.add_view(image, image_shape)
+        self.img_shapes.append(image_shape)
+        self.imgs.append(image.squeeze(0).detach())
+        self.view_names.append(view_name)
+        self.view_num += 1
+
+    def step(self, value, force_pgo=False, log_intermediate_results=False, output_folder=None):
+        """slam.py:244-297."""
+        prepare_start = time.time()
+        image, image_shape, img_gray, view_name = value["rgb"], value["shape"], value["gray"], value["view_name"]
+        i = self.view_num
+        self._ensure_graph(image)
+        if i == 0:
+            self._graph.pose[0].copy_(self._identity)  # slam.py:251-253
+        self.time_dict["prepare_data"] += time.time() - prepare_start
+
+        enc_start = time.time()
+        self.add_view(image, image_shape, view_name)
+        self.time_dict["encoder"] += time.time() - enc_start
+
+        farthest_neighbor = max(0, i - self.neighbor_edge_num)
+        loop_start = time.time()
+        loop_candi_list = self.lc_detector.detect_loop(img_gray, farthest_neighbor)  # read-back: candidates
+        self.time_dict["lc"] += time.time() - loop_start
+        self._check_flags()
+
+        graph_start = time.time()
+        js = list(range(farthest_neighbor, i)) + [j for j, _ in loop_candi_list[:self.loop_edge_num]]
+        if js:
+            dec_start = time.time()
+            conf_host, keep, batch = self._regress_keyframe(i, js)  # read-back: the gate
+            self.time_dict["decoder"] += time.time() - dec_start
+            self._check_flags()
+            kept = set(keep)
+            for k, j in enumerate(js):
+                names = f"(view {i} [{self.view_names[i]}] -- view {j} [{self.view_names[j]}])"
+                if k not in kept:
+                    if self.verbose:
+                        _msg("[EdgeReject] ", f"Rejecting edge {names} with conf {conf_host[k]:.3f}")
+                elif i - j > self.neighbor_edge_num and self.verbose:  # slam.py:199-203
+                    _msg("[LoopClosure] ", f"Adding loop closure edge {names} with conf {conf_host[k]:.3f}")
+                    self.loop_related_views.add(i)
+                    self.loop_related_views.add(j)
+            if keep:
+                self._add_keyframe(i, js, keep, batch)
+        self.time_dict["graph_construction"] += time.time() - graph_start
+
+        if self.view_num % self.pgo_every == 0 or force_pgo:
+            if log_intermediate_results:
+                self.save_data_all(f"{output_folder}", save_view_graph=False, traj_name_postfix=f"{self.view_num - 1}",
+                                   save_poses=True, save_images=False, save_scales=True, save_depths=False,
+                                   save_intrinsics=False, save_confs=False, save_ply=False)
+            opt_start = time.time()
+            self.pose_graph_optimize()
+            self.time_dict["pgo"] += time.time() - opt_start
+            torch.cuda.empty_cache()
+            return True
+        return False
+
+    def pose_graph_optimize(self):
+        """slam.py:108-140 through PoseGraphOpt on the device tables (per-edge weights: DESIGN.md §4)."""
+        _msg("[PoseGraphOpt] ", f"Pose graph optimization (at keyframe {self.view_num}) ...")
+        if self.live_mode:
+            _msg("[PoseGraphOpt] ", "This may cause latency in live mode, please hold the camera steady if possible.")
+        N, E = self.num_nodes, self.num_edges
+        opt = set()
+        for v in range(max(0, self.view_num - self.pgo_window_size), self.view_num):
+            opt.update(self.view_to_node.get(v, []))
+        opt.update(self.loop_related_views)  # view ids, used as node ids (slam.py:120)
+        if N > 0 and E > 0:
+            g = self._graph
+            idx = torch.tensor(sorted(opt), dtype=torch.int64).to(self.device)
+            graph = PoseGraphOpt(g.pose[:N], to_optimize_idxs=idx)
+            graph.optimize(g.edges[:E], g.meas[:E], g.weight[:E])
+            g.pose[:N] = graph.get_nodes()
+            self._check_flags()
+        _msg("[PoseGraphOpt] ", "Pose graph optimization done.")
+        self.loop_related_views = set()
+
+    # ------------------------------------------------------------------------------------------------ export
+    def _export(self, view0, num_views, cloud):
+        """Device gather through the best nodes (and the world point cloud); no host synchronisation."""
+        for v in range(view0, view0 + num_views):
+            if not self.view_to_node.get(v):
+                raise IndexError("view %d has no node in the pose graph" % v)
+        g = self._graph
+        dev = g.device
+        H, W = g.H, g.W
+
+        def f32(*s):
+            return torch.empty(*s, dtype=torch.float32, device=dev)
+
+        out = {"pose": f32(num_views, 4, 4), "scale": f32(num_views, 1), "depth": f32(num_views, H, W),
+               "conf": f32(num_views, H, W), "intri": f32(num_views, 3, 3)}
+        imgs = pts = cols = cnt = scratch = None
+        if cloud:
+            imgs = self.imgs.device_stack()[view0:view0 + num_views].to(torch.float32).contiguous()
+            pts, cols = f32(num_views * H * W, 3), f32(num_views * H * W, 3)
+            cnt = torch.zeros(1, dtype=torch.int64, device=dev)
+            nbytes = int(_lib.lib().sta_graph_export_scratch_bytes(num_views, H))
+            scratch = torch.empty((nbytes + 7) // 8, dtype=torch.int64, device=dev)
+        with torch.cuda.device(dev):
+            _lib.check(_lib.lib().sta_graph_export(
+                g.h, view0, num_views, float(self.conf_thres), _lib.ptr(imgs), _lib.ptr(out["pose"]), _lib.ptr(out["scale"]),
+                _lib.ptr(out["depth"]), _lib.ptr(out["conf"]), _lib.ptr(out["intri"]), _lib.ptr(pts), _lib.ptr(cols),
+                _lib.ptr(cnt), _lib.ptr(scratch), _lib.cur_stream()), "sta_graph_export")
+        if cloud:
+            out.update(points=pts, colors=cols, count=cnt, images=imgs)
+        return out
+
+    def get_view(self, v, filter_outlier=True, return_pose=True, return_depth=True, return_intri=True):
+        """slam.py:299-326."""
+        ex = self._export(v, 1, cloud=False)
+        view = View()
+        if return_pose:
+            view["pose"] = ex["pose"][0].cpu()
+        self._check_flags()
+        if return_depth:
+            depth = (ex["depth"][0] * ex["scale"][0]).cpu()
+            if filter_outlier:
+                depth[ex["conf"][0].cpu() < self.conf_thres] = 0.0
+            view["depth"] = depth
+        if return_intri:
+            view["intri"] = ex["intri"][0].cpu()
+        return view
+
+    def get_view_graph(self):
+        """slam.py:328-336."""
+        return {v: [self.node_to_connected_view[u] for u in self.view_to_node.get(v, [])] for v in range(self.view_num)}
+
+    def save_data_all(self, output_folder,
+                      save_view_graph=True, traj_name_postfix=None,
+                      save_poses=True, save_images=True, save_scales=True,
+                      save_depths=True, save_intrinsics=True,
+                      save_confs=True, save_ply=True,
+                      gt_poses=None, gt_depths=None, gt_intrinsics=None):
+        """slam.py:338-421: the same files, keys, shapes and dtypes."""
+        if not os.path.exists(output_folder):
+            os.makedirs(output_folder)
+        if save_view_graph:
+            np.savez(f"{output_folder}/view_graph.npz", view_graph=self.get_view_graph(),
+                     loop_min_dist=self.lc_detector.loop_dist_min, view_names=self.view_names)
+        ex = self._export(0, self.view_num, cloud=save_ply)
+        poses = ex["pose"].cpu()
+        self._check_flags()
+        traj_postfix = f"_{traj_name_postfix}" if traj_name_postfix is not None else ""
+        if save_poses:
+            np.save(f"{output_folder}/trajectory{traj_postfix}.npy", poses.numpy())
+        if save_scales:
+            np.save(f"{output_folder}/scales{traj_postfix}.npy", ex["scale"].cpu().numpy())
+        if save_images:
+            images = (self.imgs.device_stack().float().permute(0, 2, 3, 1) + 1.0) / 2.0
+            np.save(f"{output_folder}/images.npy", images.cpu().numpy())
+        if save_depths:
+            np.save(f"{output_folder}/depths.npy", ex["depth"].cpu().numpy())
+        if save_confs:
+            np.savez(f"{output_folder}/confs.npz", confs=ex["conf"].cpu().numpy(), thres=self.conf_thres)
+        if save_intrinsics:
+            np.save(f"{output_folder}/intrinsics.npy", ex["intri"].cpu().numpy())
+        if save_ply:
+            n = int(ex["count"].cpu())
+            write_ply(f"{output_folder}/pointcloud.ply", ex["points"][:n].cpu().numpy(), ex["colors"][:n].cpu().numpy())
+        if gt_poses is not None:
+            np.save(f"{output_folder}/gt_poses.npy", np.array(gt_poses).astype(np.float32))
+        if gt_depths is not None:
+            np.save(f"{output_folder}/gt_depths.npy", np.array(gt_depths).astype(np.float32))
+        if gt_intrinsics is not None:
+            np.save(f"{output_folder}/gt_intrinsics.npy", gt_intrinsics)
+
+    def get_pointmap_vis(self, v):
+        """slam.py:423-432: the view's local point map (host) and an 8-bit rendering of it."""
+        view = self.get_view(v, filter_outlier=False, return_pose=False, return_depth=True, return_intri=True)
+        depth, intri = view.depth.numpy().astype(np.float64), view.intri.numpy().astype(np.float64)
+        H, W = depth.shape
+        yy, xx = np.meshgrid(np.arange(H), np.arange(W), indexing="ij")
+        pix = np.stack([xx, yy, np.ones_like(xx)], -1).astype(np.float64)
+        pcl = (pix @ np.linalg.inv(intri).T * depth[..., None]).astype(np.float32)
+        min_vals = pcl.min(axis=(0, 1), keepdims=True)
+        max_vals = pcl.max(axis=(0, 1), keepdims=True)
+        normalized = (pcl - min_vals) / (max_vals - min_vals + 1e-8)
+        return (normalized * 255).astype(np.uint8), pcl
+
+    def save_pointmap(self, v, output_folder):
+        import cv2
+        if not os.path.exists(output_folder):
+            os.makedirs(output_folder)
+        img, pcl = self.get_pointmap_vis(v)
+        np.save(f"{output_folder}/pointmap_cam_{v}.npy", pcl)
+        cv2.imwrite(f"{output_folder}/pointmap_cam_{v}.png", cv2.cvtColor(img, cv2.COLOR_RGB2BGR))
+
+    def get_time_dict(self):
+        time_dict = self.time_dict.copy()
+        time_dict["graph_construction"] = time_dict["graph_construction"] - time_dict["decoder"]
+        time_dict["total"] = sum(time_dict.values())
+        return time_dict
+
+
+def write_ply(path, points, colors):
+    """Binary little-endian PLY: float x y z, uchar red green blue (colours in [0, 1], rounded to 8 bits)."""
+    n = len(points)
+    rec = np.empty(n, dtype=[("x", "<f4"), ("y", "<f4"), ("z", "<f4"), ("r", "u1"), ("g", "u1"), ("b", "u1")])
+    for k, name in enumerate("xyz"):
+        rec[name] = points[:, k]
+    rgb = np.rint(np.clip(np.asarray(colors, np.float64), 0.0, 1.0) * 255.0).astype(np.uint8)
+    for k, name in enumerate("rgb"):
+        rec[name] = rgb[:, k]
+    header = ("ply\nformat binary_little_endian 1.0\nelement vertex %d\nproperty float x\nproperty float y\nproperty float z\n"
+              "property uchar red\nproperty uchar green\nproperty uchar blue\nend_header\n" % n)
+    with open(path, "wb") as f:
+        f.write(header.encode("ascii"))
+        f.write(rec.tobytes())
+
+
+def read_ply(path):
+    """(points [N,3] fp32, colours [N,3] uint8) of a file write_ply wrote."""
+    with open(path, "rb") as f:
+        data = f.read()
+    end = data.index(b"end_header\n") + len(b"end_header\n")
+    n = int([ln for ln in data[:end].decode().splitlines() if ln.startswith("element vertex")][0].split()[-1])
+    rec = np.frombuffer(data[end:], dtype=[("x", "<f4"), ("y", "<f4"), ("z", "<f4"), ("r", "u1"), ("g", "u1"), ("b", "u1")],
+                        count=n)
+    return np.stack([rec["x"], rec["y"], rec["z"]], -1), np.stack([rec["r"], rec["g"], rec["b"]], -1)
