@@ -387,6 +387,62 @@ int sta_graph_export(StaGraph* g, int view0, int num_views, float conf_thres, co
                      float* scale_out, float* depth_out, float* conf_out, float* intri_out, float* points_out,
                      float* colors_out, int64_t* count_out, void* scratch, void* stream);
 
+/* ---- reconstruction evaluation (vista_slam/eval/eval_recon.py:108-206): world clouds, open3d's voxel_down_sample, the
+ * moments of open3d's point-to-point ICP and the nearest-neighbour distances of the Chamfer metric.  Points are fp64
+ * [n][3] device arrays.  Every reduction runs in a fixed order without floating-point atomics, so repeated runs are
+ * bit-identical.  Host pointers are refused before any launch. ---- */
+
+/* Stable LSD radix sort of (key, index) pairs by the low nbits (0..64) of the keys, 8 bits per pass; idx null means
+ * 0 .. n-1.  The outputs may be the inputs.  n < 2^31.  scratch: sta_sort_scratch_bytes(n), 16-byte aligned. */
+size_t sta_sort_scratch_bytes(int64_t n);
+int sta_op_radix_sort(const uint64_t* keys, const uint32_t* idx, int64_t n, int nbits, uint64_t* keys_out, uint32_t* idx_out,
+                      void* scratch, void* stream);
+/* Both clouds of eval_recon in numpy boolean-indexing order (view, row, column):
+ *   ground truth  gt_depth > 0, unprojected with the shared gt_intri [3][3] and moved by gt_pose [N][4][4];
+ *   estimate      conf > thres and gt_depth > 0, depth (times scale[v] when scale [N] is given) unprojected with
+ *                 intri [N][3][3] and moved by pose [N][4][4].
+ * All inputs fp32; K^-1 from the fp64 adjugate, the rest in fp32; the points are written as fp64 into gt_out / est_out
+ * (room for N H W points each), the two counts into count_out [2] (device int64).  scratch:
+ * sta_eval_clouds_scratch_bytes(N, H), 8-byte aligned.  No host synchronisation. */
+size_t sta_eval_clouds_scratch_bytes(int N, int H);
+int sta_eval_clouds(int N, int H, int W, const float* gt_depth, const float* gt_pose, const float* gt_intri, const float* depth,
+                    const float* scale, const float* pose, const float* intri, const float* conf, float thres, double* gt_out,
+                    double* est_out, int64_t* count_out, void* scratch, void* stream);
+/* open3d voxel_down_sample: min_bound = min - v/2, key = floor((p - min_bound) / v) per axis in fp64, each voxel's
+ * point = the fp64 sum of its points in input order / their count, in ascending (kx, ky, kz) order.  out: room for n
+ * points; *count_host: the number written.  Refused: v <= 0, and v * INT_MAX < the padded extent (open3d's condition).
+ * Synchronises twice: to read the cloud's box (key widths, refusal) and the voxel count.  scratch:
+ * sta_voxel_scratch_bytes(n), 16-byte aligned. */
+size_t sta_voxel_scratch_bytes(int64_t n);
+int sta_voxel_down(const double* pts, int64_t n, double voxel, double* out, int64_t* count_host, void* scratch, void* stream);
+/* Nearest-neighbour index over one cloud (n may be 0): the points sorted by a 63-bit Morton code, leaves of 32 points
+ * under a complete binary tree of fp64 boxes.  The index copies what it needs; create synchronises the stream. */
+typedef struct StaNnIndex StaNnIndex; /* opaque */
+int sta_nn_create(const double* pts, int64_t n, StaNnIndex** out, void* stream);
+void sta_nn_destroy(StaNnIndex* ix);
+/* Per query: the nearest indexed point strictly within radius (d^2 < r^2, d^2 = (dx dx + dy dy) + dz dz with every
+ * operation rounded on its own).  dist_out [nq]: its distance, or radius when there is none; idx_out [nq]: its input
+ * index, or -1.  Exact whatever the tree's shape.  scratch: sta_nn_query_scratch_bytes(nq), 16-byte aligned. */
+size_t sta_nn_query_scratch_bytes(int64_t nq);
+int sta_nn_query(const StaNnIndex* ix, const double* q, int64_t nq, double radius, double* dist_out, int64_t* idx_out,
+                 void* scratch, void* stream);
+/* Moments of one point-to-point ICP step over corr [n] (index into dst, -1 = none), into out17 (device):
+ * [0] count, [1] sum d^2, [2..4] sum src, [5..7] sum dst, [8..16] the centred cross-covariance sum
+ * sum (dst - mean_dst)(src - mean_src)^T, row-major (means from the first pass: two passes, not raw moments).
+ * scratch: sta_reduce_scratch_bytes(). */
+size_t sta_reduce_scratch_bytes(void);
+int sta_op_moments(const double* src, const double* dst, const int64_t* corr, int64_t n, double* out17, void* scratch,
+                   void* stream);
+/* sta_nn_query of the source points in the target's index (target_pts: the cloud the index was built from), then
+ * sta_op_moments.  scratch: sta_icp_scratch_bytes(n), 16-byte aligned. */
+size_t sta_icp_scratch_bytes(int64_t n);
+int sta_icp_moments(const StaNnIndex* target, const double* target_pts, const double* src, int64_t n, double radius,
+                    double* out17, void* scratch, void* stream);
+/* In place: p <- M[:, :3] p + M[:, 3] with M the row-major 3x4 m12_host, fp64 without FMA contraction. */
+int sta_transform_points(double* pts, int64_t n, const double* m12_host, void* stream);
+/* *out_dev = sum of min(max(d, 0), clip)^2 over n values.  scratch: sta_reduce_scratch_bytes(). */
+int sta_sum_sq_clipped(const double* d, int64_t n, double clip, double* out_dev, void* scratch, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -151,6 +151,30 @@ def lib():
     L.sta_graph_export_scratch_bytes.argtypes = [i, i]
     L.sta_graph_export_scratch_bytes.restype = ctypes.c_size_t
     L.sta_graph_export.argtypes = [vp, i, i, c_float, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]
+    f64, sz = ctypes.c_double, ctypes.c_size_t
+    L.sta_sort_scratch_bytes.argtypes = [i64]
+    L.sta_sort_scratch_bytes.restype = sz
+    L.sta_op_radix_sort.argtypes = [vp, vp, i64, i, vp, vp, vp, vp]
+    L.sta_eval_clouds_scratch_bytes.argtypes = [i, i]
+    L.sta_eval_clouds_scratch_bytes.restype = sz
+    L.sta_eval_clouds.argtypes = [i, i, i, vp, vp, vp, vp, vp, vp, vp, vp, c_float, vp, vp, vp, vp, vp]
+    L.sta_voxel_scratch_bytes.argtypes = [i64]
+    L.sta_voxel_scratch_bytes.restype = sz
+    L.sta_voxel_down.argtypes = [vp, i64, f64, vp, POINTER(c_int64), vp, vp]
+    L.sta_nn_create.argtypes = [vp, i64, POINTER(vp), vp]
+    L.sta_nn_destroy.argtypes = [vp]
+    L.sta_nn_destroy.restype = None
+    L.sta_nn_query_scratch_bytes.argtypes = [i64]
+    L.sta_nn_query_scratch_bytes.restype = sz
+    L.sta_nn_query.argtypes = [vp, vp, i64, f64, vp, vp, vp, vp]
+    L.sta_reduce_scratch_bytes.argtypes = []
+    L.sta_reduce_scratch_bytes.restype = sz
+    L.sta_op_moments.argtypes = [vp, vp, vp, i64, vp, vp, vp]
+    L.sta_icp_scratch_bytes.argtypes = [i64]
+    L.sta_icp_scratch_bytes.restype = sz
+    L.sta_icp_moments.argtypes = [vp, vp, vp, i64, f64, vp, vp, vp]
+    L.sta_transform_points.argtypes = [vp, i64, POINTER(f64), vp]
+    L.sta_sum_sq_clipped.argtypes = [vp, i64, f64, vp, vp, vp]
     _lib = L
     return L
 

@@ -51,6 +51,16 @@ int make_tmap(CUtensorMap* out, const void* base, int is_f32, int rank, const ui
 
 int num_sms();  // of the CURRENT device (cached per device)
 
+// true for device (or managed) memory; host pointers and unknown addresses are false
+inline bool on_device(const void* p) {
+  cudaPointerAttributes at;
+  if (cudaPointerGetAttributes(&at, p) != cudaSuccess) {
+    cudaGetLastError();
+    return false;
+  }
+  return at.type == cudaMemoryTypeDevice || at.type == cudaMemoryTypeManaged;
+}
+
 // One-time per-DEVICE setup at a call site (cudaFuncSetAttribute is per device/context, not per process):
 //   static PerDeviceOnce once;  STA_CHECK_CUDA(once.run([&] { return cudaFuncSetAttribute(...); }));
 struct PerDeviceOnce {

@@ -13,6 +13,7 @@
 #include <string>
 
 #include "../../include/sta_b200.h"
+#include "cloud.cuh"
 #include "host_util.h"
 #include "pointmap.cuh"
 
@@ -251,15 +252,8 @@ export_gather_kernel(StaGraph g, int view0, float thres, float* pose_out, float*
     cnt += c > thres;
   }
   if (counts) {
-    cnt = __reduce_add_sync(0xffffffffu, cnt);
-    __shared__ int wsum[8];
-    if ((threadIdx.x & 31) == 0) wsum[threadIdx.x >> 5] = cnt;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      int t = 0;
-      for (int w = 0; w < 8; ++w) t += wsum[w];
-      counts[static_cast<long long>(v) * g.H + row] = t;
-    }
+    const int t = block_count_256(cnt);
+    if (threadIdx.x == 0) counts[static_cast<long long>(v) * g.H + row] = t;
   }
   if (row == 0 && threadIdx.x == 0) {
     const float* p = g.pose + b * 8;
@@ -278,33 +272,6 @@ export_gather_kernel(StaGraph g, int view0, float thres, float* pose_out, float*
   }
 }
 
-// one block of 1024 threads: exclusive scan of n counts in order (offsets[n] = total), total also to count_out
-__global__ void __launch_bounds__(1024) export_scan_kernel(const int* counts, long long n, long long* offsets, int64_t* count_out) {
-  __shared__ long long part[1024];
-  const long long per = (n + 1023) / 1024;
-  const long long lo = threadIdx.x * per, hi = min(n, lo + per);
-  long long t = 0;
-  for (long long i = lo; i < hi; ++i) t += counts[i];
-  part[threadIdx.x] = t;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    long long run = 0;
-    for (int i = 0; i < 1024; ++i) {
-      const long long c = part[i];
-      part[i] = run;
-      run += c;
-    }
-    offsets[n] = run;
-    *count_out = run;
-  }
-  __syncthreads();
-  long long run = part[threadIdx.x];
-  for (long long i = lo; i < hi; ++i) {
-    offsets[i] = run;
-    run += counts[i];
-  }
-}
-
 // grid (H, V), 256 threads: the points of row blockIdx.x of view blockIdx.y with conf > thres, in column order, at the
 // row's offset: world = R (K^-1 [x y 1]^T depth s) + t, colour = (img + 1) / 2.
 __global__ void __launch_bounds__(256)
@@ -314,55 +281,17 @@ export_scatter_kernel(StaGraph g, float thres, const float* pose_out, const floa
   const int v = blockIdx.y, row = blockIdx.x, W = g.W;
   const long long hw = static_cast<long long>(g.H) * W;
   const float* P = pose_out + v * 16;
-  const float* K = intri_out + v * 9;
-  // torch.inverse of the 3x3 intrinsics, evaluated in fp64 from the adjugate
-  const double k00 = K[0], k01 = K[1], k02 = K[2], k10 = K[3], k11 = K[4], k12 = K[5], k20 = K[6], k21 = K[7], k22 = K[8];
-  const double det = k00 * (k11 * k22 - k12 * k21) - k01 * (k10 * k22 - k12 * k20) + k02 * (k10 * k21 - k11 * k20);
-  const float Ki[9] = {static_cast<float>((k11 * k22 - k12 * k21) / det), static_cast<float>((k02 * k21 - k01 * k22) / det),
-                       static_cast<float>((k01 * k12 - k02 * k11) / det), static_cast<float>((k12 * k20 - k10 * k22) / det),
-                       static_cast<float>((k00 * k22 - k02 * k20) / det), static_cast<float>((k02 * k10 - k00 * k12) / det),
-                       static_cast<float>((k10 * k21 - k11 * k20) / det), static_cast<float>((k01 * k20 - k00 * k21) / det),
-                       static_cast<float>((k00 * k11 - k01 * k10) / det)};
+  float Ki[9];
+  inv3_f32(intri_out + v * 9, Ki);
   const float s = scale_out[v];
-  __shared__ int wsum[8];
-  long long base = offsets[static_cast<long long>(v) * g.H + row];
   const float* crow = conf_out + v * hw + static_cast<long long>(row) * W;
   const float* drow = depth_out + v * hw + static_cast<long long>(row) * W;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  for (int x0 = 0; x0 < W; x0 += 256) {
-    const int x = x0 + threadIdx.x;
-    const bool keep = x < W && crow[x] > thres;
-    const unsigned bal = __ballot_sync(0xffffffffu, keep);
-    if (lane == 0) wsum[warp] = __popc(bal);
-    __syncthreads();
-    int before = __popc(bal & ((1u << lane) - 1u)), total = 0;
-    for (int w = 0; w < 8; ++w) {
-      if (w < warp) before += wsum[w];
-      total += wsum[w];
-    }
-    if (keep) {
-      const float d = drow[x] * s;
-      const float u = static_cast<float>(x), r = static_cast<float>(row);
-      const float cx = (Ki[0] * u + Ki[1] * r + Ki[2]) * d, cy = (Ki[3] * u + Ki[4] * r + Ki[5]) * d,
-                  cz = (Ki[6] * u + Ki[7] * r + Ki[8]) * d;
-      const long long o = base + before;
-      for (int c = 0; c < 3; ++c) {
-        points[o * 3 + c] = P[c * 4] * cx + P[c * 4 + 1] * cy + P[c * 4 + 2] * cz + P[c * 4 + 3];
-        colors[o * 3 + c] = (imgs[(static_cast<long long>(v) * 3 + c) * hw + static_cast<long long>(row) * W + x] + 1.f) / 2.f;
-      }
-    }
-    base += total;
-    __syncthreads();
-  }
-}
-
-bool on_device(const void* p) {
-  cudaPointerAttributes at;
-  if (cudaPointerGetAttributes(&at, p) != cudaSuccess) {
-    cudaGetLastError();
-    return false;
-  }
-  return at.type == cudaMemoryTypeDevice || at.type == cudaMemoryTypeManaged;
+  row_compact_256(W, offsets[static_cast<long long>(v) * g.H + row], [&](int x) { return crow[x] > thres; },
+                  [&](int x, long long o) {
+                    unproject_f32(Ki, P, static_cast<float>(x), static_cast<float>(row), drow[x] * s, points + o * 3);
+                    for (int c = 0; c < 3; ++c)
+                      colors[o * 3 + c] = (imgs[(static_cast<long long>(v) * 3 + c) * hw + static_cast<long long>(row) * W + x] + 1.f) / 2.f;
+                  });
 }
 
 }  // namespace
@@ -527,7 +456,7 @@ int sta_graph_export(StaGraph* g, int view0, int num_views, float conf_thres, co
                                                               intri_out, counts);
   STA_CHECK_CUDA(cudaGetLastError());
   if (!cloud) return 0;
-  export_scan_kernel<<<1, 1024, 0, st>>>(counts, rows, offsets, count_out);
+  row_scan_kernel<<<1, 1024, 0, st>>>(counts, rows, offsets, count_out);
   STA_CHECK_CUDA(cudaGetLastError());
   export_scatter_kernel<<<dim3(g->H, num_views), 256, 0, st>>>(*g, conf_thres, pose_out, scale_out, intri_out, depth_out, conf_out,
                                                                imgs_dev, offsets, points_out, colors_out);
