@@ -318,6 +318,16 @@ int sta_loop_add_frame(StaLoopDetector* d, const void* frame_dev, int frame_is_f
  * (descending similarity, ties in descending j). */
 int sta_loop_detect(StaLoopDetector* d, int farthest_neighbor, int* n_out, int64_t* js_out, double* sims_out, int cap,
                     void* stream);
+/* Frame batches, every per-frame result equal to the calls above in frame order.  sta_loop_add_frames: compute_bow_feat
+ * for F >= 1 frames [F][H][W] of one size (ORB over all frames, one transform, vectors appended in frame order);
+ * asynchronous.  sta_loop_detect_many: detect_loop for the newest F views (F at most the frames of the last add call),
+ * farthest_host[f] in [0, view index of row f]; one score launch and one detect launch over the F rows, then the one
+ * host synchronisation: n_out [2F] = {candidates, length (-1: None)} per row, row f's first cap_per_view candidates at
+ * js_out / sims_out + f cap_per_view.  An ORB overflow is reported with the frame's index in the batch.  Afterwards
+ * sta_loop_similarities returns the last row. */
+int sta_loop_add_frames(StaLoopDetector* d, const void* frames_dev, int frames_is_f32, int F, int H, int W, void* stream);
+int sta_loop_detect_many(StaLoopDetector* d, int F, const int* farthest_host, int* n_out, int64_t* js_out,
+                         double* sims_out, int cap_per_view, void* stream);
 /* Test read-backs (synchronise): a view's vector (len -1 for None) and the similarity row of the last detect (NaN where
  * either vector is None). */
 int sta_loop_view(StaLoopDetector* d, int view, int32_t* words_out, double* vals_out, int cap, int* len_out, void* stream);
@@ -331,6 +341,12 @@ size_t sta_orb_scratch_bytes(int H, int W);
 int sta_orb_layout(int H, int W, int64_t* out42);
 int sta_op_orb(const void* frame_dev, int frame_is_f32, int H, int W, int32_t* xy_out, int32_t* level_out, float* pts_out,
                float* angle_out, float* response_out, uint8_t* desc_out, int32_t* count_out, void* scratch, void* stream);
+/* The same for F frames [F][H][W] of one size: scratch of F sta_orb_scratch_bytes(H, W) bytes (frame f's slice at f times
+ * that), outputs [F][STA_ORB_MAX_KEYPOINTS] (desc [F][STA_ORB_MAX_KEYPOINTS][32]), count_out [F]; each frame's outputs
+ * and scratch equal sta_op_orb's on that frame. */
+int sta_op_orb_many(const void* frames_dev, int frames_is_f32, int F, int H, int W, int32_t* xy_out, int32_t* level_out,
+                    float* pts_out, float* angle_out, float* response_out, uint8_t* desc_out, int32_t* count_out,
+                    void* scratch, void* stream);
 /* Per descriptor [n][32] (device): word id and weight of the leaf it descends to. */
 int sta_op_bow_transform(const StaVocab* v, const uint8_t* desc_dev, int n, int32_t* word_out, double* weight_out,
                          void* stream);

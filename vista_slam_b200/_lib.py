@@ -131,12 +131,16 @@ def lib():
     L.sta_loop_views.argtypes = [vp]
     L.sta_loop_add_frame.argtypes = [vp, vp, i, i, i, vp]
     L.sta_loop_detect.argtypes = [vp, i, POINTER(c_int), POINTER(c_int64), POINTER(ctypes.c_double), i, vp]
+    L.sta_loop_add_frames.argtypes = [vp, vp, i, i, i, i, vp]
+    L.sta_loop_detect_many.argtypes = [vp, i, POINTER(c_int), POINTER(c_int), POINTER(c_int64), POINTER(ctypes.c_double), i,
+                                       vp]
     L.sta_loop_view.argtypes = [vp, i, POINTER(c_int32), POINTER(ctypes.c_double), i, POINTER(c_int), vp]
     L.sta_loop_similarities.argtypes = [vp, POINTER(ctypes.c_double), i, vp]
     L.sta_orb_scratch_bytes.argtypes = [i, i]
     L.sta_orb_scratch_bytes.restype = ctypes.c_size_t
     L.sta_orb_layout.argtypes = [i, i, POINTER(c_int64)]
     L.sta_op_orb.argtypes = [vp, i, i, i, vp, vp, vp, vp, vp, vp, vp, vp, vp]
+    L.sta_op_orb_many.argtypes = [vp, i, i, i, i, vp, vp, vp, vp, vp, vp, vp, vp, vp]
     L.sta_op_bow_transform.argtypes = [vp, vp, i, vp, vp, vp]
     L.sta_op_bow_vector.argtypes = [vp, vp, vp, i, vp, vp, vp, vp]
     L.sta_op_bow_score.argtypes = [vp, vp, vp, vp, vp, vp, vp, i, vp, vp]

@@ -11,6 +11,11 @@
 // are equal, so the order of descriptors does not matter) or set once (addIfNotExist); the L1 norm, the division and the
 // score s += |v - w| - |v| - |w| are sequential fp64 in ascending word id; detect_loop runs in one thread.  One host
 // synchronisation per keyframe: the read-back of the candidate list.
+//
+// Frame batches (sta_loop_add_frames / sta_loop_detect_many) run the same per-frame arithmetic over F frames of one
+// size: ORB with a frame grid dimension, one transform over F x 4096 descriptor slots, one CTA per frame building its
+// vector into a staging slot, an append in frame order, then one score launch and one detect launch over F rows and one
+// read-back.  Every per-frame result equals the sequential path's.
 #include "../../include/sta_b200.h"
 #include "common.cuh"
 #include "host_util.h"
@@ -337,8 +342,15 @@ int upload_vocab(const HostVocab& v, const std::vector<int>& order, StaVocab** o
 }
 
 // Vocabulary::transform(feature, word_id, weight): one thread per descriptor
+// blockIdx.y = frame of a batch: its descriptors and outputs are kOrbMaxKeypoints slots after the previous frame's,
+// its count n_dev[f].
 __global__ void transform_kernel(const uint8_t* desc, const int* n_dev, int n_host, StaVocab v, int* word_out,
                                  double* weight_out) {
+  const long long f = blockIdx.y, m = f * kOrbMaxKeypoints;
+  desc += 32 * m;
+  word_out += m;
+  weight_out += m;
+  if (n_dev) n_dev += f;
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   const int n = n_dev ? *n_dev : n_host;
   if (i >= n) return;
@@ -365,17 +377,11 @@ __global__ void transform_kernel(const uint8_t* desc, const int* n_dev, int n_ho
   weight_out[i] = v.weight[node];
 }
 
-// BowVector: accumulate (addWeight / addIfNotExist), then normalize(L1).  One CTA.  Writes the vector at entry offset
-// *entries_used of the database (words ascending) and its length; *entries_used advances.  len = -1 (None) when there
-// was no descriptor.
-__global__ void __launch_bounds__(kBuildThreads) build_kernel(const int* word, const double* weight, const int* n_dev,
-                                                              int n_host, int weighting, int* db_word, double* db_val,
-                                                              long long* db_start, int* db_len, int view,
-                                                              long long* entries_used) {
+// BowVector of n descriptors: accumulate (addWeight / addIfNotExist), then normalize(L1), into out_word / out_val
+// (words ascending).  Run by a whole CTA; returns the length in thread 0.
+__device__ int build_vector(const int* word, const double* weight, int n, int weighting, int* out_word, double* out_val) {
   __shared__ int s_first[kOrbMaxKeypoints];  // rank -> descriptor of the sorted (word, index) list
   __shared__ int s_cnt;
-  const int n = n_dev ? *n_dev : n_host;
-  const long long base = *entries_used;
   if (threadIdx.x == 0) s_cnt = 0;
   __syncthreads();
   // rank sort of the descriptors with weight > 0 by (word, index)
@@ -392,9 +398,9 @@ __global__ void __launch_bounds__(kBuildThreads) build_kernel(const int* word, c
     atomicAdd(&s_cnt, 1);
   }
   __syncthreads();
+  int len = 0;
   if (threadIdx.x == 0) {
     const int m = s_cnt;
-    int len = 0;
     for (int r = 0; r < m;) {
       const int wv = word[s_first[r]];
       const double x = weight[s_first[r]];
@@ -402,39 +408,74 @@ __global__ void __launch_bounds__(kBuildThreads) build_kernel(const int* word, c
       int e = r + 1;
       for (; e < m && word[s_first[e]] == wv; ++e)
         if (weighting == kTf || weighting == kTfIdf) acc = __dadd_rn(acc, x);
-      db_word[base + len] = wv;
-      db_val[base + len] = acc;
+      out_word[len] = wv;
+      out_val[len] = acc;
       ++len;
       r = e;
     }
     double norm = 0.0;
-    for (int i = 0; i < len; ++i) norm = __dadd_rn(norm, fabs(db_val[base + i]));
+    for (int i = 0; i < len; ++i) norm = __dadd_rn(norm, fabs(out_val[i]));
     if (norm > 0.0)
-      for (int i = 0; i < len; ++i) db_val[base + i] = __ddiv_rn(db_val[base + i], norm);
+      for (int i = 0; i < len; ++i) out_val[i] = __ddiv_rn(out_val[i], norm);
+  }
+  return len;
+}
+
+// One CTA: the vector written at entry offset *entries_used of the database and its length; *entries_used advances.
+// len = -1 (None) when there was no descriptor.
+__global__ void __launch_bounds__(kBuildThreads) build_kernel(const int* word, const double* weight, const int* n_dev,
+                                                              int n_host, int weighting, int* db_word, double* db_val,
+                                                              long long* db_start, int* db_len, int view,
+                                                              long long* entries_used) {
+  const int n = n_dev ? *n_dev : n_host;
+  const long long base = *entries_used;
+  const int len = build_vector(word, weight, n, weighting, db_word + base, db_val + base);
+  if (threadIdx.x == 0) {
     db_start[view] = base;
     db_len[view] = n > 0 ? len : -1;
     *entries_used = base + len;
   }
 }
 
-// L1Scoring::score of view q against views [0, nviews): one thread per view, a merge over ascending word ids.
-// sims[j] = NaN when either vector is None.
-__global__ void score_kernel(const int* qw, const double* qv, const int* q_len_dev, const long long* q_start_dev,
-                             const int* db_word, const double* db_val, const long long* db_start, const int* db_len,
-                             int nviews, double* sims) {
-  const int j = blockIdx.x * blockDim.x + threadIdx.x;
-  if (j >= nviews) return;
-  const int na = *q_len_dev;
-  const int nb = db_len[j];
-  if (na < 0 || nb < 0) {
-    sims[j] = __longlong_as_double(0x7ff8000000000000ll);
-    return;
+// One CTA per frame of a batch: frame f's vector into staging slot f (kOrbMaxKeypoints entries), its length (-1: None)
+// into stage_len[f].  Frame f's descriptors are at slot f (kOrbMaxKeypoints apart), its count at n_dev[f].
+__global__ void __launch_bounds__(kBuildThreads) build_many_kernel(const int* word, const double* weight, const int* n_dev,
+                                                                   int weighting, int* stage_word, double* stage_val,
+                                                                   int* stage_len) {
+  const long long f = blockIdx.x, m = f * kOrbMaxKeypoints;
+  const int n = n_dev[f];
+  const int len = build_vector(word + m, weight + m, n, weighting, stage_word + m, stage_val + m);
+  if (threadIdx.x == 0) stage_len[f] = n > 0 ? len : -1;
+}
+
+// Appends the F staged vectors to the database in frame order (one CTA per frame); views view0 .. view0 + F - 1.
+// *entries_used is advanced by advance_entries_kernel afterwards, so every CTA reads the same base here.
+__global__ void append_many_kernel(const int* stage_word, const double* stage_val, const int* stage_len, int F, int view0,
+                                   int* db_word, double* db_val, long long* db_start, int* db_len,
+                                   const long long* entries_used) {
+  const int f = blockIdx.x;
+  long long base = *entries_used;
+  for (int g = 0; g < f; ++g) base += stage_len[g] > 0 ? stage_len[g] : 0;
+  const int len = stage_len[f];
+  for (int k = threadIdx.x; k < len; k += blockDim.x) {
+    db_word[base + k] = stage_word[static_cast<long long>(f) * kOrbMaxKeypoints + k];
+    db_val[base + k] = stage_val[static_cast<long long>(f) * kOrbMaxKeypoints + k];
   }
-  const long long qa = q_start_dev ? *q_start_dev : 0;
-  const int* aw = qw + qa;
-  const double* av = qv + qa;
-  const int* bw = db_word + db_start[j];
-  const double* bv = db_val + db_start[j];
+  if (threadIdx.x == 0) {
+    db_start[view0 + f] = base;
+    db_len[view0 + f] = len;
+  }
+}
+
+__global__ void advance_entries_kernel(const int* stage_len, int F, long long* entries_used) {
+  long long e = *entries_used;
+  for (int g = 0; g < F; ++g) e += stage_len[g] > 0 ? stage_len[g] : 0;
+  *entries_used = e;
+}
+
+// L1Scoring::score of vector a against vector b, a merge over ascending word ids; NaN when either is None (length -1).
+__device__ double l1_score(const int* aw, const double* av, int na, const int* bw, const double* bv, int nb) {
+  if (na < 0 || nb < 0) return __longlong_as_double(0x7ff8000000000000ll);
   double s = 0.0;
   int a = 0, b = 0;
   while (a < na && b < nb) {
@@ -449,13 +490,33 @@ __global__ void score_kernel(const int* qw, const double* qv, const int* q_len_d
       ++b;
     }
   }
-  sims[j] = __ddiv_rn(-s, 2.0);
+  return __ddiv_rn(-s, 2.0);
 }
 
-// loop_detector.py:23-50 over the precomputed similarities of view i; out: [0] = count, then (j, sim) pairs as
-// {int64 j, double sim}, sorted by descending similarity, ties keeping the scan's descending-j order.
-__global__ void detect_kernel(const double* sims, const int* db_len, int i, int farthest, int dist_min, int nms,
-                              int thresh_neighbor, long long* out) {
+// Score of view q against views [0, nviews): one thread per view.
+__global__ void score_kernel(const int* qw, const double* qv, const int* q_len_dev, const long long* q_start_dev,
+                             const int* db_word, const double* db_val, const long long* db_start, const int* db_len,
+                             int nviews, double* sims) {
+  const int j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= nviews) return;
+  const long long qa = q_start_dev ? *q_start_dev : 0;
+  sims[j] = l1_score(qw + qa, qv + qa, *q_len_dev, db_word + db_start[j], db_val + db_start[j], db_len[j]);
+}
+
+// Rows i = i0 + blockIdx.y of a batch: view i against views [0, i), into sims + blockIdx.y * stride.
+__global__ void score_many_kernel(const int* db_word, const double* db_val, const long long* db_start, const int* db_len,
+                                  int i0, double* sims, long long stride) {
+  const int i = i0 + blockIdx.y;
+  const int j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= i) return;
+  sims[blockIdx.y * stride + j] = l1_score(db_word + db_start[i], db_val + db_start[i], db_len[i], db_word + db_start[j],
+                                           db_val + db_start[j], db_len[j]);
+}
+
+// loop_detector.py:23-50 over the precomputed similarities of view i; out: [0] = count, [1] = length of view i, then
+// (j, sim) pairs as {int64 j, double sim}, sorted by descending similarity, ties keeping the scan's descending-j order.
+__device__ void detect_row(const double* sims, const int* db_len, int i, int farthest, int dist_min, int nms,
+                           int thresh_neighbor, long long* out) {
   const bool none_i = db_len[i] < 0;
   const int lo = i - thresh_neighbor > 0 ? i - thresh_neighbor : 0;
   double th = 1.0;
@@ -491,6 +552,22 @@ __global__ void detect_kernel(const double* sims, const int* db_len, int i, int 
   out[1] = db_len[i];
 }
 
+__global__ void detect_kernel(const double* sims, const int* db_len, int i, int farthest, int dist_min, int nms,
+                              int thresh_neighbor, long long* out) {
+  detect_row(sims, db_len, i, farthest, dist_min, nms, thresh_neighbor, out);
+}
+
+// One thread per row f of a batch (view i0 + f): out row f = {ORB overflow flag of frame f, then detect_row's count,
+// length and pairs}, `out_stride` entries apart.
+__global__ void detect_many_kernel(const double* sims, long long sims_stride, const int* db_len, int i0,
+                                   const int* farthest, int dist_min, int nms, int thresh_neighbor, long long* out,
+                                   long long out_stride, const unsigned* overflow, size_t overflow_stride) {
+  const int f = blockIdx.x;
+  long long* row = out + f * out_stride;
+  detect_row(sims + f * sims_stride, db_len, i0 + f, farthest[f], dist_min, nms, thresh_neighbor, row + 1);
+  row[0] = *reinterpret_cast<const unsigned*>(reinterpret_cast<const char*>(overflow) + f * overflow_stride);
+}
+
 }  // namespace
 }  // namespace sta
 
@@ -501,8 +578,20 @@ struct StaLoopDetector {
   int dist_min, nms, thresh_neighbor;
   int H = 0, W = 0;
   OrbLayout lay = {};
-  void* scratch = nullptr;        // ORB scratch
-  void* kp = nullptr;             // ORB outputs + transform outputs
+  void* scratch = nullptr;        // ORB scratch: frame_cap slices of lay.total bytes
+  void* kp = nullptr;             // ORB outputs + transform outputs: frame_cap slices of kKpSlice bytes
+  int frame_cap = 0, stage_cap = 0;
+  int newest_slice = 0;           // scratch slice of the newest view (its ORB overflow flag)
+  int last_batch = 0;             // frames of the last add call
+  int* stage_word = nullptr;      // [frame_cap][kOrbMaxKeypoints] vectors of a batch before the append
+  double* stage_val = nullptr;
+  int* stage_len = nullptr;       // [frame_cap]
+  double* sims_many = nullptr;    // [rows][views] of sta_loop_detect_many
+  long long* result_many = nullptr;
+  long long* pinned_many = nullptr;
+  long long many_cap = 0;         // entries of sims_many / result_many / pinned_many
+  int* farthest_dev = nullptr;    // [frame_cap]
+  int* farthest_pinned = nullptr;
   int views = 0, view_cap = 0;
   // Upper bound on the database entries in use, kept on the host: each appended view may add up to kOrbMaxKeypoints
   // words, and the exact count (entries_dev) is only read back at the synchronisation of sta_loop_detect.
@@ -532,10 +621,12 @@ struct KpBufs {
   double* weight;
 };
 
-KpBufs kp_bufs(void* base) {
+// Field-major buffers of `frames` frames: frame f's entries of each field start at slot f kOrbMaxKeypoints, its count
+// at count[f] (the output layout of orb_run).
+KpBufs kp_bufs(void* base, int frames) {
   char* p = static_cast<char*>(base);
   KpBufs b;
-  const int M = kOrbMaxKeypoints;
+  const size_t M = static_cast<size_t>(kOrbMaxKeypoints) * frames;
   b.xy = reinterpret_cast<int2*>(p);          p += sizeof(int2) * M;
   b.pts = reinterpret_cast<float2*>(p);       p += sizeof(float2) * M;
   b.weight = reinterpret_cast<double*>(p);    p += sizeof(double) * M;
@@ -547,7 +638,7 @@ KpBufs kp_bufs(void* base) {
   b.count = reinterpret_cast<int*>(p);
   return b;
 }
-constexpr size_t kKpBytes = (8 + 8 + 8 + 4 + 4 + 4 + 4 + 32) * kOrbMaxKeypoints + 16;
+size_t kp_bytes(int frames) { return ((8 + 8 + 8 + 4 + 4 + 4 + 4 + 32) * kOrbMaxKeypoints + 16) * static_cast<size_t>(frames); }
 
 template <typename T>
 int grow(T** p, long long old_n, long long new_n, cudaStream_t st) {
@@ -559,10 +650,11 @@ int grow(T** p, long long old_n, long long new_n, cudaStream_t st) {
   return 0;
 }
 
-// room for one more view of up to kOrbMaxKeypoints words
-int reserve(StaLoopDetector* d, cudaStream_t st) {
-  if (d->views + 1 > d->view_cap) {
-    const int cap = d->view_cap ? 2 * d->view_cap : 256;
+// room for F more views of up to kOrbMaxKeypoints words each
+int reserve(StaLoopDetector* d, cudaStream_t st, int F = 1) {
+  if (d->views + F > d->view_cap) {
+    int cap = d->view_cap ? 2 * d->view_cap : 256;
+    while (cap < d->views + F) cap *= 2;
     if (grow(&d->db_start, d->view_cap, cap, st) || grow(&d->db_len, d->view_cap, cap, st) ||
         grow(&d->sims, 0, cap, st) || grow(&d->result, 0, 2 + 2LL * cap, st))
       return 1;
@@ -570,20 +662,56 @@ int reserve(StaLoopDetector* d, cudaStream_t st) {
     STA_CHECK_CUDA(cudaMallocHost(&d->pinned, sizeof(long long) * (2 + 2LL * cap)));
     d->view_cap = cap;
   }
-  if (d->entries_bound + kOrbMaxKeypoints > d->entry_cap) {
+  const long long need = d->entries_bound + static_cast<long long>(F) * kOrbMaxKeypoints;
+  if (need > d->entry_cap) {
     long long cap = d->entry_cap ? 2 * d->entry_cap : 64LL * kOrbMaxKeypoints;
-    while (cap < d->entries_bound + kOrbMaxKeypoints) cap *= 2;
+    while (cap < need) cap *= 2;
     if (grow(&d->db_word, d->entry_cap, cap, st) || grow(&d->db_val, d->entry_cap, cap, st)) return 1;
     d->entry_cap = cap;
   }
   return 0;
 }
 
+// F frames (with n_dev): kOrbMaxKeypoints descriptor slots per frame, counts n_dev[0..F)
 int bow_of_descriptors(StaVocab* v, const uint8_t* desc, const int* n_dev, int n_host, int* word, double* weight,
-                       cudaStream_t st) {
+                       cudaStream_t st, int F = 1) {
   const int cap = n_dev ? kOrbMaxKeypoints : n_host;
-  if (cap > 0) transform_kernel<<<(cap + 127) / 128, 128, 0, st>>>(desc, n_dev, n_host, *v, word, weight);
+  if (cap > 0) transform_kernel<<<dim3((cap + 127) / 128, F), 128, 0, st>>>(desc, n_dev, n_host, *v, word, weight);
   STA_CHECK_CUDA(cudaGetLastError());
+  return 0;
+}
+
+// ORB scratch and keypoint buffers for F frames of H x W (the frame size may change between calls)
+int prepare_frames(StaLoopDetector* d, int F, int H, int W, cudaStream_t st) {
+  if (H != d->H || W != d->W || F > d->frame_cap) {
+    const OrbLayout lay = orb_layout(H, W);
+    const int cap = F > d->frame_cap ? F : d->frame_cap;
+    if (d->scratch) STA_CHECK_CUDA(cudaFreeAsync(d->scratch, st));
+    d->scratch = nullptr;
+    STA_CHECK_CUDA(cudaMallocAsync(&d->scratch, lay.total * cap, st));
+    if (cap > d->frame_cap) {
+      if (d->kp) STA_CHECK_CUDA(cudaFreeAsync(d->kp, st));
+      d->kp = nullptr;
+      STA_CHECK_CUDA(cudaMallocAsync(&d->kp, kp_bytes(cap), st));
+    }
+    d->lay = lay;
+    d->H = H;
+    d->W = W;
+    d->frame_cap = cap;
+  }
+  return 0;
+}
+
+int grow_batch(StaLoopDetector* d, int F, cudaStream_t st) {
+  if (F <= d->stage_cap) return 0;
+  const long long M = kOrbMaxKeypoints;
+  if (grow(&d->stage_word, 0, M * F, st) || grow(&d->stage_val, 0, M * F, st) || grow(&d->stage_len, 0, F, st) ||
+      grow(&d->farthest_dev, 0, F, st))
+    return 1;
+  if (d->farthest_pinned) cudaFreeHost(d->farthest_pinned);
+  d->farthest_pinned = nullptr;
+  STA_CHECK_CUDA(cudaMallocHost(&d->farthest_pinned, sizeof(int) * F));
+  d->stage_cap = F;
   return 0;
 }
 
@@ -703,7 +831,15 @@ void sta_loop_destroy(StaLoopDetector* d) {
   cudaFree(d->sims);
   cudaFree(d->result);
   cudaFree(d->entries_dev);
+  cudaFree(d->stage_word);
+  cudaFree(d->stage_val);
+  cudaFree(d->stage_len);
+  cudaFree(d->sims_many);
+  cudaFree(d->result_many);
+  cudaFree(d->farthest_dev);
   if (d->pinned) cudaFreeHost(d->pinned);
+  if (d->pinned_many) cudaFreeHost(d->pinned_many);
+  if (d->farthest_pinned) cudaFreeHost(d->farthest_pinned);
   delete d;
 }
 
@@ -714,17 +850,8 @@ int sta_loop_add_frame(StaLoopDetector* d, const void* frame_dev, int frame_is_f
   STA_REQUIRE(d, "null detector");
   STA_REQUIRE(orb_size_ok(H, W), "ORB frame sides must be in [32, 4096]");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (H != d->H || W != d->W) {
-    const OrbLayout lay = orb_layout(H, W);
-    if (d->scratch) STA_CHECK_CUDA(cudaFreeAsync(d->scratch, st));
-    STA_CHECK_CUDA(cudaMallocAsync(&d->scratch, lay.total, st));
-    if (!d->kp) STA_CHECK_CUDA(cudaMallocAsync(&d->kp, kKpBytes, st));
-    d->lay = lay;
-    d->H = H;
-    d->W = W;
-  }
-  if (reserve(d, st)) return 1;
-  KpBufs b = kp_bufs(d->kp);
+  if (prepare_frames(d, 1, H, W, st) || reserve(d, st)) return 1;
+  KpBufs b = kp_bufs(d->kp, d->frame_cap);
   OrbOut o = {b.xy, b.level, b.pts, b.angle, b.resp, b.desc, b.count};
   if (orb_run(d->lay, d->scratch, frame_dev, frame_is_f32, o, st)) return 1;
   if (bow_of_descriptors(d->vocab, b.desc, b.count, 0, b.word, b.weight, st)) return 1;
@@ -733,6 +860,34 @@ int sta_loop_add_frame(StaLoopDetector* d, const void* frame_dev, int frame_is_f
   STA_CHECK_CUDA(cudaGetLastError());
   d->views += 1;
   d->entries_bound += kOrbMaxKeypoints;
+  d->newest_slice = 0;
+  d->last_batch = 1;
+  d->last_stream = st;
+  return 0;
+}
+
+// compute_bow_feat for F frames [F][H][W] of one size: ORB over all frames, one transform, one build CTA per frame and
+// the append in frame order (asynchronous)
+int sta_loop_add_frames(StaLoopDetector* d, const void* frames_dev, int frames_is_f32, int F, int H, int W, void* stream) {
+  STA_REQUIRE(d && frames_dev, "null argument");
+  STA_REQUIRE(F >= 1, "the frame count must be at least 1");
+  STA_REQUIRE(orb_size_ok(H, W), "ORB frame sides must be in [32, 4096]");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (prepare_frames(d, F, H, W, st) || grow_batch(d, F, st) || reserve(d, st, F)) return 1;
+  KpBufs b = kp_bufs(d->kp, d->frame_cap);
+  OrbOut o = {b.xy, b.level, b.pts, b.angle, b.resp, b.desc, b.count};
+  if (orb_run(d->lay, d->scratch, frames_dev, frames_is_f32, o, st, F)) return 1;
+  if (bow_of_descriptors(d->vocab, b.desc, b.count, 0, b.word, b.weight, st, F)) return 1;
+  build_many_kernel<<<F, kBuildThreads, 0, st>>>(b.word, b.weight, b.count, d->vocab->weighting, d->stage_word,
+                                                 d->stage_val, d->stage_len);
+  append_many_kernel<<<F, 256, 0, st>>>(d->stage_word, d->stage_val, d->stage_len, F, d->views, d->db_word, d->db_val,
+                                        d->db_start, d->db_len, d->entries_dev);
+  advance_entries_kernel<<<1, 1, 0, st>>>(d->stage_len, F, d->entries_dev);
+  STA_CHECK_CUDA(cudaGetLastError());
+  d->views += F;
+  d->entries_bound += static_cast<long long>(F) * kOrbMaxKeypoints;
+  d->newest_slice = F - 1;
+  d->last_batch = F;
   d->last_stream = st;
   return 0;
 }
@@ -756,7 +911,9 @@ int sta_loop_detect(StaLoopDetector* d, int farthest_neighbor, int* n_out, int64
   STA_CHECK_CUDA(cudaMemcpyAsync(d->pinned, d->result, nb, cudaMemcpyDeviceToHost, st));
   STA_CHECK_CUDA(cudaMemcpyAsync(&d->entries_bound, d->entries_dev, sizeof(long long), cudaMemcpyDeviceToHost, st));
   unsigned overflow = 0;
-  STA_CHECK_CUDA(cudaMemcpyAsync(&overflow, static_cast<char*>(d->scratch) + d->lay.counters + 3 * sizeof(unsigned),
+  STA_CHECK_CUDA(cudaMemcpyAsync(&overflow,
+                                 static_cast<char*>(d->scratch) + d->newest_slice * d->lay.total + d->lay.counters +
+                                     3 * sizeof(unsigned),
                                  sizeof(unsigned), cudaMemcpyDeviceToHost, st));
   STA_CHECK_CUDA(cudaStreamSynchronize(st));
   STA_REQUIRE(!overflow, "the frame has more ORB candidates or keypoints than the detector holds");
@@ -766,6 +923,73 @@ int sta_loop_detect(StaLoopDetector* d, int farthest_neighbor, int* n_out, int64
   for (int k = 0; k < n && k < cap; ++k) {
     js_out[k] = d->pinned[2 + 2 * k];
     memcpy(&sims_out[k], &d->pinned[3 + 2 * k], sizeof(double));
+  }
+  return 0;
+}
+
+// detect_loop for each of the newest F views (the frames of the last sta_loop_add_frames, or fewer of its newest), row
+// f = view views - F + f against every earlier view: one score launch, one detect launch and one read-back.
+// n_out [2F] = {candidates, length (-1: None)} per row; row f's first cap_per_view candidates go to
+// js_out / sims_out + f cap_per_view (host).  Afterwards sta_loop_similarities returns the last row.
+int sta_loop_detect_many(StaLoopDetector* d, int F, const int* farthest_host, int* n_out, int64_t* js_out,
+                         double* sims_out, int cap_per_view, void* stream) {
+  STA_REQUIRE(d && farthest_host && n_out && (cap_per_view == 0 || (js_out && sims_out)), "null argument");
+  STA_REQUIRE(F >= 1 && F <= d->last_batch, "F must be in [1, frames of the last add call]");
+  STA_REQUIRE(cap_per_view >= 0, "bad capacity");
+  const int i0 = d->views - F;
+  for (int f = 0; f < F; ++f)
+    STA_REQUIRE(farthest_host[f] >= 0 && farthest_host[f] <= i0 + f, "farthest_neighbor must be in [0, view index]");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  d->last_stream = st;
+  const long long sims_stride = d->views, out_stride = 3 + 2LL * d->views;
+  const long long need = F * (out_stride > sims_stride ? out_stride : sims_stride);
+  if (need > d->many_cap) {
+    long long cap = d->many_cap ? 2 * d->many_cap : 1LL << 14;
+    while (cap < need) cap *= 2;
+    if (grow(&d->sims_many, 0, cap, st) || grow(&d->result_many, 0, cap, st)) return 1;
+    if (d->pinned_many) cudaFreeHost(d->pinned_many);
+    d->pinned_many = nullptr;
+    STA_CHECK_CUDA(cudaMallocHost(&d->pinned_many, sizeof(long long) * cap));
+    d->many_cap = cap;
+  }
+  memcpy(d->farthest_pinned, farthest_host, sizeof(int) * F);
+  STA_CHECK_CUDA(cudaMemcpyAsync(d->farthest_dev, d->farthest_pinned, sizeof(int) * F, cudaMemcpyHostToDevice, st));
+  const int i_last = d->views - 1;
+  if (i_last > 0)
+    score_many_kernel<<<dim3((i_last + 127) / 128, F), 128, 0, st>>>(d->db_word, d->db_val, d->db_start, d->db_len, i0,
+                                                                      d->sims_many, sims_stride);
+  const int first_slice = d->last_batch - F;  // scratch slice of row 0
+  detect_many_kernel<<<F, 1, 0, st>>>(d->sims_many, sims_stride, d->db_len, i0, d->farthest_dev, d->dist_min, d->nms,
+                                      d->thresh_neighbor, d->result_many, out_stride,
+                                      reinterpret_cast<const unsigned*>(static_cast<char*>(d->scratch) +
+                                                                        first_slice * d->lay.total + d->lay.counters +
+                                                                        3 * sizeof(unsigned)),
+                                      d->lay.total);
+  STA_CHECK_CUDA(cudaGetLastError());
+  if (i_last > 0)
+    STA_CHECK_CUDA(cudaMemcpyAsync(d->sims, d->sims_many + (F - 1) * sims_stride, sizeof(double) * i_last,
+                                   cudaMemcpyDeviceToDevice, st));
+  STA_CHECK_CUDA(cudaMemcpyAsync(d->pinned_many, d->result_many, sizeof(long long) * F * out_stride,
+                                 cudaMemcpyDeviceToHost, st));
+  STA_CHECK_CUDA(cudaMemcpyAsync(&d->entries_bound, d->entries_dev, sizeof(long long), cudaMemcpyDeviceToHost, st));
+  STA_CHECK_CUDA(cudaStreamSynchronize(st));
+  for (int f = 0; f < F; ++f) {
+    const long long* row = d->pinned_many + f * out_stride;
+    if (row[0]) {
+      set_last_error("frame " + std::to_string(f) +
+                     " of the batch has more ORB candidates or keypoints than the detector holds");
+      return 1;
+    }
+  }
+  for (int f = 0; f < F; ++f) {
+    const long long* row = d->pinned_many + f * out_stride;
+    const int n = static_cast<int>(row[1]);
+    n_out[2 * f] = n;
+    n_out[2 * f + 1] = static_cast<int>(row[2]);
+    for (int k = 0; k < n && k < cap_per_view; ++k) {
+      js_out[static_cast<long long>(f) * cap_per_view + k] = row[3 + 2 * k];
+      memcpy(&sims_out[static_cast<long long>(f) * cap_per_view + k], &row[4 + 2 * k], sizeof(double));
+    }
   }
   return 0;
 }

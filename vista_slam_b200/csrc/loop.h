@@ -23,8 +23,8 @@ struct OrbLayout {
 bool orb_size_ok(int H, int W);
 OrbLayout orb_layout(int H, int W);
 
-// Device outputs in canonical (level, y, x) order; count_dev [1] receives the number of keypoints and counters_dev
-// (inside the scratch) flags an overflow in counters[3].
+// Device outputs in canonical (level, y, x) order; count [1] receives the number of keypoints and the counters inside
+// the scratch (OrbLayout::counters) flag an overflow in counters[3].
 struct OrbOut {
   int2* xy;         // level coordinates
   int* level;
@@ -35,6 +35,9 @@ struct OrbOut {
   int* count;
 };
 
-int orb_run(const OrbLayout& s, void* scratch, const void* frame, int is_f32, const OrbOut& out, cudaStream_t st);
+// F frames of one size (frame-major [F][H][W] input, F scratch slices of s.total bytes, F output slots of
+// kOrbMaxKeypoints and F counts); each frame's result is the one of a call with F = 1.
+int orb_run(const OrbLayout& s, void* scratch, const void* frame, int is_f32, const OrbOut& out, cudaStream_t st,
+            int F = 1);
 
 }  // namespace sta

@@ -12,6 +12,10 @@
 // previous level; FAST scores; 3x3 non-max suppression, border filter and a per-level score histogram; the FAST
 // threshold of retainBest(2n); Harris responses (one warp per candidate); retainBest(n) on them by counting; the
 // canonical order; angles and descriptors (one warp per keypoint) on the blurred levels.
+//
+// A batch of F frames of one size runs the same launches with blockIdx.z = frame: frame f reads its input at f H W,
+// works in scratch slice f (OrbLayout::total bytes apart) and writes output slot f (kOrbMaxKeypoints apart, count f).
+// A frame's arithmetic does not depend on F.
 #include "../../include/sta_b200.h"
 #include "common.cuh"
 #include "host_util.h"
@@ -45,6 +49,18 @@ struct LevelGeom {
 
 inline size_t align256(size_t x) { return (x + 255) & ~size_t(255); }
 
+// p moved to the slice of frame blockIdx.z, `bytes` apart
+template <typename T>
+__device__ __forceinline__ T* frame_slice(T* p, size_t bytes) {
+  return reinterpret_cast<T*>(reinterpret_cast<uintptr_t>(p) + static_cast<uintptr_t>(blockIdx.z) * bytes);
+}
+
+__device__ __forceinline__ OrbOut frame_out(OrbOut o) {
+  const int f = blockIdx.z;
+  const long long m = static_cast<long long>(f) * kOrbMaxKeypoints;
+  return {o.xy + m, o.level + m, o.pts + m, o.angle + m, o.response + m, o.desc + 32 * m, o.count + f};
+}
+
 float level_scale(int l) { return static_cast<float>(pow(static_cast<double>(1.2f), static_cast<double>(l))); }
 
 LevelGeom geom_of(const OrbLayout& s) {
@@ -64,9 +80,11 @@ __device__ __forceinline__ int reflect101(int i, int n) {
   return i >= n ? 2 * (n - 1) - i : i;
 }
 
-__global__ void to_u8_kernel(const void* frame, int is_f32, int n, uint8_t* out) {
+__global__ void to_u8_kernel(const void* frame, int is_f32, int n, uint8_t* out, size_t fs) {
   int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
+  frame = frame_slice(static_cast<const char*>(frame), static_cast<size_t>(n) * (is_f32 ? 4 : 1));
+  out = frame_slice(out, fs);
   if (is_f32) {
     // (gray * 255).astype(np.uint8): an fp32 multiply, then truncation
     out[i] = static_cast<uint8_t>(static_cast<int>(__fmul_rn(static_cast<const float*>(frame)[i], 255.f)));
@@ -91,9 +109,11 @@ __device__ __forceinline__ void linear_coeff(int i, int src, int dst, int& ofs, 
 }
 
 // cv::resize(src, dst, dsize, 0, 0, INTER_LINEAR_EXACT): (sum of 8-bit x 8-bit weighted taps + 2^15) >> 16
-__global__ void resize_kernel(const uint8_t* src, int sh, int sw, uint8_t* dst, int dh, int dw) {
+__global__ void resize_kernel(const uint8_t* src, int sh, int sw, uint8_t* dst, int dh, int dw, size_t fs) {
   int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= dh * dw) return;
+  src = frame_slice(src, fs);
+  dst = frame_slice(dst, fs);
   const int y = i / dw, x = i - y * dw;
   int xo, xw1, yo, yw1;
   linear_coeff(x, sw, dw, xo, xw1);
@@ -108,7 +128,9 @@ __global__ void resize_kernel(const uint8_t* src, int sh, int sw, uint8_t* dst, 
 }
 
 // FAST-9 score (cornerScore<16>) where the pixel is a corner, else 0.  blockIdx.y = level.
-__global__ void fast_kernel(const uint8_t* pyr, LevelGeom g, uint8_t* score) {
+__global__ void fast_kernel(const uint8_t* pyr, LevelGeom g, uint8_t* score, size_t fs) {
+  pyr = frame_slice(pyr, fs);
+  score = frame_slice(score, fs);
   const int l = blockIdx.y;
   const int h = g.h[l], w = g.w[l];
   int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -141,7 +163,12 @@ __global__ void fast_kernel(const uint8_t* pyr, LevelGeom g, uint8_t* score) {
 }
 
 // Non-max suppression (strictly above all 8 neighbours), border filter, candidate list and score histogram.
-__global__ void nms_kernel(const uint8_t* score, LevelGeom g, int4* cand, unsigned* hist, unsigned* counters) {
+__global__ void nms_kernel(const uint8_t* score, LevelGeom g, int4* cand, unsigned* hist, unsigned* counters,
+                           size_t fs) {
+  score = frame_slice(score, fs);
+  cand = frame_slice(cand, fs);
+  hist = frame_slice(hist, fs);
+  counters = frame_slice(counters, fs);
   const int l = blockIdx.y;
   const int h = g.h[l], w = g.w[l];
   int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -166,7 +193,9 @@ __global__ void nms_kernel(const uint8_t* score, LevelGeom g, int4* cand, unsign
 }
 
 // retainBest(2 n_l) on the integer FAST score: the smallest kept score per level (256 = keep none).
-__global__ void fast_threshold_kernel(const unsigned* hist, LevelGeom g, int* thr) {
+__global__ void fast_threshold_kernel(const unsigned* hist, LevelGeom g, int* thr, size_t fs) {
+  hist = frame_slice(hist, fs);
+  thr = frame_slice(thr, fs);
   const int l = threadIdx.x;
   if (l >= kOrbLevels) return;
   const unsigned want = 2u * g.quota[l];
@@ -189,7 +218,13 @@ __global__ void fast_threshold_kernel(const unsigned* hist, LevelGeom g, int* th
 
 // HarrisResponses(blockSize 7, k 0.04) of the candidates that pass retainBest(2n); one warp per candidate.
 __global__ void harris_kernel(const uint8_t* pyr, LevelGeom g, const int4* cand, const int* thr, float* resp,
-                              int* alive, unsigned* counters) {
+                              int* alive, unsigned* counters, size_t fs) {
+  pyr = frame_slice(pyr, fs);
+  cand = frame_slice(cand, fs);
+  thr = frame_slice(thr, fs);
+  resp = frame_slice(resp, fs);
+  alive = frame_slice(alive, fs);
+  counters = frame_slice(counters, fs);
   const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
   const int n = min(counters[0], static_cast<unsigned>(kOrbMaxCandidates));
   if (warp >= n) return;
@@ -226,7 +261,12 @@ __global__ void harris_kernel(const uint8_t* pyr, LevelGeom g, const int4* cand,
 
 // retainBest(n_l) on the Harris response: keep a candidate when fewer than n_l of its level respond more strongly.
 __global__ void harris_select_kernel(const int4* cand, const float* resp, const int* alive, LevelGeom g, int* kept,
-                                     unsigned* counters) {
+                                     unsigned* counters, size_t fs) {
+  cand = frame_slice(cand, fs);
+  resp = frame_slice(resp, fs);
+  alive = frame_slice(alive, fs);
+  kept = frame_slice(kept, fs);
+  counters = frame_slice(counters, fs);
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   const int m = counters[1];
   if (i >= m) return;
@@ -249,7 +289,12 @@ __global__ void harris_select_kernel(const int4* cand, const float* resp, const 
 
 // Canonical order (level, y, x) by counting; writes the keypoint fields that need no image.
 __global__ void order_kernel(const int4* cand, const float* resp, const int* kept, LevelGeom g, unsigned* counters,
-                             OrbOut out) {
+                             OrbOut out, size_t fs) {
+  cand = frame_slice(cand, fs);
+  resp = frame_slice(resp, fs);
+  kept = frame_slice(kept, fs);
+  counters = frame_slice(counters, fs);
+  out = frame_out(out);
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   const int m = min(counters[2], static_cast<unsigned>(kOrbMaxKeypoints));
   if (i == 0) *out.count = m;
@@ -287,7 +332,9 @@ __device__ float fast_atan2(float y, float x) {
 }
 
 // ICAngles: intensity centroid over the radius-15 disc of the unsmoothed level; one warp per keypoint
-__global__ void angle_kernel(const uint8_t* pyr, LevelGeom g, OrbOut out) {
+__global__ void angle_kernel(const uint8_t* pyr, LevelGeom g, OrbOut out, size_t fs) {
+  pyr = frame_slice(pyr, fs);
+  out = frame_out(out);
   const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
   if (warp >= *out.count) return;
   const int l = out.level[warp];
@@ -317,7 +364,9 @@ __constant__ float c_gauss[7];
 
 // ORB's GaussianBlur(7x7, 2, REFLECT_101) of each level: fp32 row pass with fused multiply-adds left to right, then
 // the symmetric column pass (centre, then (above + below) * tap, fused), rounded half to even.  blockIdx.y = level.
-__global__ void blur_kernel(const uint8_t* pyr, LevelGeom g, uint8_t* blur) {
+__global__ void blur_kernel(const uint8_t* pyr, LevelGeom g, uint8_t* blur, size_t fs) {
+  pyr = frame_slice(pyr, fs);
+  blur = frame_slice(blur, fs);
   const int l = blockIdx.y;
   const int h = g.h[l], w = g.w[l];
   int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -343,7 +392,9 @@ __global__ void blur_kernel(const uint8_t* pyr, LevelGeom g, uint8_t* blur) {
 }
 
 // rBRIEF: lane b writes descriptor byte b from 8 pair tests of the blurred level; one warp per keypoint
-__global__ void desc_kernel(const uint8_t* blur, LevelGeom g, OrbOut out) {
+__global__ void desc_kernel(const uint8_t* blur, LevelGeom g, OrbOut out, size_t fs) {
+  blur = frame_slice(blur, fs);
+  out = frame_out(out);
   const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
   if (warp >= *out.count) return;
   const int l = out.level[warp];
@@ -439,7 +490,7 @@ OrbLayout orb_layout(int H, int W) {
   return s;
 }
 
-int orb_run(const OrbLayout& s, void* scratch, const void* frame, int is_f32, const OrbOut& out, cudaStream_t st) {
+int orb_run(const OrbLayout& s, void* scratch, const void* frame, int is_f32, const OrbOut& out, cudaStream_t st, int F) {
   if (upload_constants()) {
     set_last_error("orb: constant upload failed");
     return 1;
@@ -457,23 +508,24 @@ int orb_run(const OrbLayout& s, void* scratch, const void* frame, int is_f32, co
   int* kept = reinterpret_cast<int*>(base + s.kept);
   const LevelGeom g = geom_of(s);
   const int n0 = s.H * s.W;
-  STA_CHECK_CUDA(cudaMemsetAsync(base + s.hist, 0, s.alive - s.hist, st));
-  to_u8_kernel<<<(n0 + 255) / 256, 256, 0, st>>>(frame, is_f32, n0, pyr);
+  const size_t fs = s.total;  // scratch slice of one frame
+  STA_CHECK_CUDA(cudaMemset2DAsync(base + s.hist, fs, 0, s.alive - s.hist, F, st));
+  to_u8_kernel<<<dim3((n0 + 255) / 256, 1, F), 256, 0, st>>>(frame, is_f32, n0, pyr, fs);
   for (int l = 1; l < kOrbLevels; ++l) {
     const int n = s.h[l] * s.w[l];
-    resize_kernel<<<(n + 255) / 256, 256, 0, st>>>(pyr + s.lvl[l - 1], s.h[l - 1], s.w[l - 1], pyr + s.lvl[l], s.h[l],
-                                                   s.w[l]);
+    resize_kernel<<<dim3((n + 255) / 256, 1, F), 256, 0, st>>>(pyr + s.lvl[l - 1], s.h[l - 1], s.w[l - 1], pyr + s.lvl[l],
+                                                               s.h[l], s.w[l], fs);
   }
-  const dim3 grid_lv((n0 + 255) / 256, kOrbLevels);
-  fast_kernel<<<grid_lv, 256, 0, st>>>(pyr, g, score);
-  nms_kernel<<<grid_lv, 256, 0, st>>>(score, g, cand, hist, counters);
-  fast_threshold_kernel<<<1, 32, 0, st>>>(hist, g, thr);
-  harris_kernel<<<kOrbMaxCandidates / 8, 256, 0, st>>>(pyr, g, cand, thr, resp, alive, counters);
-  harris_select_kernel<<<kOrbMaxCandidates / 256, 256, 0, st>>>(cand, resp, alive, g, kept, counters);
-  order_kernel<<<kOrbMaxKeypoints / 256, 256, 0, st>>>(cand, resp, kept, g, counters, out);
-  angle_kernel<<<kOrbMaxKeypoints / 8, 256, 0, st>>>(pyr, g, out);
-  blur_kernel<<<grid_lv, 256, 0, st>>>(pyr, g, blur);
-  desc_kernel<<<kOrbMaxKeypoints / 8, 256, 0, st>>>(blur, g, out);
+  const dim3 grid_lv((n0 + 255) / 256, kOrbLevels, F);
+  fast_kernel<<<grid_lv, 256, 0, st>>>(pyr, g, score, fs);
+  nms_kernel<<<grid_lv, 256, 0, st>>>(score, g, cand, hist, counters, fs);
+  fast_threshold_kernel<<<dim3(1, 1, F), 32, 0, st>>>(hist, g, thr, fs);
+  harris_kernel<<<dim3(kOrbMaxCandidates / 8, 1, F), 256, 0, st>>>(pyr, g, cand, thr, resp, alive, counters, fs);
+  harris_select_kernel<<<dim3(kOrbMaxCandidates / 256, 1, F), 256, 0, st>>>(cand, resp, alive, g, kept, counters, fs);
+  order_kernel<<<dim3(kOrbMaxKeypoints / 256, 1, F), 256, 0, st>>>(cand, resp, kept, g, counters, out, fs);
+  angle_kernel<<<dim3(kOrbMaxKeypoints / 8, 1, F), 256, 0, st>>>(pyr, g, out, fs);
+  blur_kernel<<<grid_lv, 256, 0, st>>>(pyr, g, blur, fs);
+  desc_kernel<<<dim3(kOrbMaxKeypoints / 8, 1, F), 256, 0, st>>>(blur, g, out, fs);
   STA_CHECK_CUDA(cudaGetLastError());
   return 0;
 }
@@ -507,6 +559,19 @@ int sta_op_orb(const void* frame_dev, int frame_is_f32, int H, int W, int32_t* x
   OrbOut o = {reinterpret_cast<int2*>(xy_out), level_out, reinterpret_cast<float2*>(pts_out), angle_out, response_out,
               desc_out, count_out};
   return orb_run(s, scratch, frame_dev, frame_is_f32, o, static_cast<cudaStream_t>(stream));
+}
+
+// F frames [F][H][W] of one size: scratch of F sta_orb_scratch_bytes(H, W) bytes, outputs [F][STA_ORB_MAX_KEYPOINTS]
+// and count_out [F]
+int sta_op_orb_many(const void* frames_dev, int frames_is_f32, int F, int H, int W, int32_t* xy_out, int32_t* level_out,
+                    float* pts_out, float* angle_out, float* response_out, uint8_t* desc_out, int32_t* count_out,
+                    void* scratch, void* stream) {
+  STA_REQUIRE(orb_size_ok(H, W), "ORB frame sides must be in [32, 4096]");
+  STA_REQUIRE(F >= 1, "the frame count must be at least 1");
+  const OrbLayout s = orb_layout(H, W);
+  OrbOut o = {reinterpret_cast<int2*>(xy_out), level_out, reinterpret_cast<float2*>(pts_out), angle_out, response_out,
+              desc_out, count_out};
+  return orb_run(s, scratch, frames_dev, frames_is_f32, o, static_cast<cudaStream_t>(stream), F);
 }
 
 }  // extern "C"

@@ -8,13 +8,21 @@ both pose heads, both DPT heads and the pointmap consumers (per-edge shared intr
 with no host synchronisation inside -- the caller reads `pose_conf` once per keyframe.
 
 Results are numerically the per-edge results of the reference sequence (the decoder has no cross-sample op), so
-`regress_two_views(i, j)` is also offered as the K = 1 special case with the reference's return convention."""
+`regress_two_views(i, j)` is also offered as the K = 1 special case with the reference's return convention.
+
+Across keyframes (OnlineSLAM.step_many): `add_views` encodes many views per sta_encode call, and
+`regress_keyframes_gated` runs the gated step over the candidate edges of many keyframes in chunks of up to 16 edges,
+one pose-confidence read-back per chunk.  Batch sizes change the GEMMs' split-K, so these outputs equal the per-keyframe
+ones within rounding, not bit for bit."""
 import ctypes
 
 import torch
 
 from . import _lib
 from .utils.slam_utils import _scratch_for
+
+GRAPH_MAX_TOKENS = 8192  # runtime.cu kGraphMaxTokens: larger calls run without CUDA-graph replay
+MAX_EDGES = 16           # edges per sta_regress_pairs_begin call (check_edges)
 
 
 class KeyframeFrontend:
@@ -34,6 +42,117 @@ class KeyframeFrontend:
         self.enc_features.append(feat)
         self.img_shapes.append((int(image.shape[-2]), int(image.shape[-1])))
         return len(self.enc_features) - 1
+
+    @torch.no_grad()
+    def add_views(self, images, image_shapes=None):
+        """add_view for each image (1, 3, H, W) in order, all of one size, encoded B at a time with B N <= GRAPH_MAX_TOKENS
+        (N = H W / 256 tokens; 41 views at 224 x 224), so every call is replayed as a CUDA graph.  Returns the view
+        indices."""
+        images = list(images)
+        if not images:
+            return []
+        H, W = int(images[0].shape[-2]), int(images[0].shape[-1])
+        if any(tuple(x.shape[-2:]) != (H, W) for x in images):
+            raise ValueError("all views of a batch must have the same size")
+        B = max(1, GRAPH_MAX_TOKENS // ((H // 16) * (W // 16)))
+        first = len(self.enc_features)
+        for c in range(0, len(images), B):
+            chunk = images[c:c + B]
+            x = torch.cat([t.reshape(1, *t.shape[-3:]) for t in chunk]) if len(chunk) > 1 else chunk[0]
+            feat, _ = self.frontend._encode_image(x, None if image_shapes is None else image_shapes[c], normalize=False)
+            for b in range(len(chunk)):
+                self.enc_features.append(feat[b:b + 1])
+                self.img_shapes.append((H, W))
+        return list(range(first, len(self.enc_features)))
+
+    @staticmethod
+    def edge_chunks(items):
+        """Keyframe-major chunks of the edges of items = [(i, js), ...]: lists of item indices whose edges add up to at
+        most MAX_EDGES; a keyframe's edges are never split.  Keyframes without candidates belong to no chunk."""
+        chunks, cur, n = [], [], 0
+        for k, (_, js) in enumerate(items):
+            m = len(js)
+            if m == 0:
+                continue
+            if m > MAX_EDGES:
+                raise ValueError("a keyframe has more than %d candidate edges" % MAX_EDGES)
+            if n + m > MAX_EDGES:
+                chunks.append(cur)
+                cur, n = [], 0
+            cur.append(k)
+            n += m
+        if cur:
+            chunks.append(cur)
+        return chunks
+
+    def _read_confs(self, pconf):
+        """The gate's read-back: the candidates' pose confidences on the host."""
+        return [float(c) for c in pconf.cpu()]
+
+    @torch.no_grad()
+    def regress_keyframes_gated(self, items, rel_pose_thres):
+        """regress_views_gated over the keyframes items = [(i, js), ...], chunk by chunk (edge_chunks): per chunk ONE
+        sta_regress_pairs_begin over its edges, ONE read-back of their confidences, and one _finish for the survivors
+        (`conf >= thres or i - j == 1`).  When the call has more than one chunk, every chunk is padded to MAX_EDGES with
+        copies of its last edge (ignored), so that the CUDA-graph keys stay few.
+
+        A generator: it yields, per item in order, (the K confidences on the host, indices of the kept candidates, the
+        keyframe's device batch {pose [K,4,4], pose_conf [K], conf / depths [2,n,H,W], intri [n,3,3], conf_mean [2,n]})
+        -- what OnlineSLAM._add_keyframe takes -- or None for an item without candidates.  A chunk runs when its first
+        keyframe is asked for."""
+        items = [(i, list(js)) for i, js in items]
+        chunks = self.edge_chunks(items)
+        pad = len(chunks) > 1
+        at = 0
+        for chunk in chunks:
+            for k in range(at, chunk[0]):
+                yield None
+            yield from self._regress_chunk([items[k] for k in chunk], rel_pose_thres, pad)
+            at = chunk[-1] + 1
+        for k in range(at, len(items)):
+            yield None
+
+    def _regress_chunk(self, items, rel_pose_thres, pad):
+        edges = [(i, j) for i, js in items for j in js]
+        K = MAX_EDGES if pad else len(edges)
+        run = edges + [edges[-1]] * (K - len(edges))
+        H, W = self.img_shapes[edges[0][0]]
+        if any(self.img_shapes[v] != (H, W) for e in edges for v in e):
+            raise ValueError("all views of a batch must have the same size")
+        fi = torch.cat([self.enc_features[i] for i, _ in run], dim=0)
+        fj = torch.cat([self.enc_features[j] for _, j in run], dim=0)
+        L = self.frontend._ready(fi)
+        dev = fi.device
+
+        def f32(*shape):
+            return torch.empty(*shape, device=dev, dtype=torch.float32)
+
+        pose, pconf = f32(2, K, 4, 4), f32(2, K)
+        m = self.frontend
+        with torch.cuda.device(dev):
+            _lib.check(L.sta_regress_pairs_begin(m._handle, _lib.ptr(fi), _lib.ptr(fj), K, H, W, _lib.ptr(pose),
+                                                 _lib.ptr(pconf), _lib.cur_stream()), "sta_regress_pairs_begin")
+            conf_host = self._read_confs(pconf[0, :len(edges)])  # the one host synchronisation of the chunk
+            keep = [e for e, (i, j) in enumerate(edges) if not (conf_host[e] < rel_pose_thres and i - j != 1)]
+            n = len(keep)
+            if n:
+                conf, depth = f32(2, n, H, W), f32(2, n, H, W)
+                pts, intri, cmean = f32(2, n, H, W, 3), f32(n, 3, 3), f32(2, n)
+                idx = (ctypes.c_int * n)(*keep)
+                _lib.check(L.sta_regress_pairs_finish(m._handle, idx, n, _lib.ptr(pts), _lib.ptr(conf), _lib.ptr(intri),
+                                                      _lib.ptr(depth), _lib.ptr(cmean), _lib.ptr(_scratch_for(dev, 2 * n)),
+                                                      _lib.cur_stream()), "sta_regress_pairs_finish")
+        e0 = p0 = 0
+        for i, js in items:
+            e1 = e0 + len(js)
+            kf_keep = [e - e0 for e in keep if e0 <= e < e1]
+            p1 = p0 + len(kf_keep)
+            batch = {"pose": pose[0, e0:e1], "pose_conf": pconf[0, e0:e1]}
+            if kf_keep:
+                batch.update(conf=conf[:, p0:p1].contiguous(), depths=depth[:, p0:p1].contiguous(), intri=intri[p0:p1],
+                             conf_mean=cmean[:, p0:p1].contiguous())
+            yield conf_host[e0:e1], kf_keep, batch
+            e0, p0 = e1, p1
 
     def _edge_batch(self, i, js):
         """The inputs of a batched step over the K = len(js) edges (i, j): the library, the feature pairs fi / fj, the

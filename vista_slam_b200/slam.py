@@ -20,6 +20,11 @@ does not depend on the neighbour edges) and the gate read.  PGO iterations read 
 A rotation that is not orthonormal (pp.mat2SE3(atol=1e-3) would raise) raises a device flag, which is read at the next
 of those read-backs and raises ValueError there.
 
+`step_many(values)` steps through many keyframes of one size in one call, with the graph, the PGO calls and the host
+bookkeeping of calling `step` on each in order.  The frontend work does not depend on the pose graph, so it runs across
+keyframes at real batch sizes: the encoder over up to 41 views per call at 224 x 224, loop detection over all frames of
+the call with one read-back, and the gated edge regression in chunks of up to 16 edges with one read-back each.
+
 Importing this module does not import pypose, munch, colorama or open3d.  `get_view` returns a `View` (attribute and key
 access, as munch.Munch).  The PLY of save_data_all is written here: binary little-endian, float x y z and uchar
 red green blue (colours rounded from [0, 1]); whether that is byte-identical to open3d's writer is not checked."""
@@ -206,6 +211,11 @@ class OnlineSLAM:
         keep = [k for k, o in enumerate(out) if o[2] is not None]
         return self.kf.last_conf_host, keep, self.kf.last_batch
 
+    def _regress_keyframes(self, items):
+        """The frontend's part of many keyframes items = [(i, js), ...]: per item, in order, what _regress_keyframe
+        returns, or None when js is empty (KeyframeFrontend.regress_keyframes_gated; may be a generator)."""
+        return self.kf.regress_keyframes_gated(items, self.rel_pose_thres)
+
     def _add_keyframe(self, i, js, keep, batch):
         """connect_view_i_j (slam.py:191-241) for the kept edges, in order: host integers, then two launches."""
         g = self._graph
@@ -297,6 +307,96 @@ class OnlineSLAM:
             torch.cuda.empty_cache()
             return True
         return False
+
+    def step_many(self, values, force_pgo=False, log_intermediate_results=False, output_folder=None):
+        """[self.step(v, force_pgo=force_pgo and k == len(values) - 1, ...) for k, v in enumerate(values)]: the same
+        graph, PGO calls, host bookkeeping, messages and time buckets, with the frontend batched across keyframes.
+        Returns the is_optimized flags.  All values must have one image size (ValueError before any launch).
+
+        Order: all views are encoded (KeyframeFrontend.add_views) and loop-detected (LoopDetector.detect_loops, one
+        read-back) first; then edge chunk by edge chunk, the gate's read-back, the kept edges' heads, and the keyframes
+        of the chunk registered and inserted in order, with PGO where step would run it (so view_num, imgs and
+        view_names hold exactly the views inserted so far).  A capacity IndexError leaves the graph, view_num, imgs and
+        view_names as step would at that keyframe; the encoder cache and the loop database may then already hold later
+        views of the call.  A non-orthonormal rotation raises ValueError by the end of the call.
+
+        Host synchronisations: one for the loop candidates, one per edge chunk, one per PGO iteration, and one at the
+        end of the call unless a PGO ran last (reading the rotation flag)."""
+        values = list(values)
+        if not values:
+            return []
+        prepare_start = time.time()
+        images = [v["rgb"] for v in values]
+        size = tuple(images[0].shape[-2:])
+        if any(tuple(x.shape[-2:]) != size for x in images):
+            raise ValueError("all keyframes of a step_many call must have the same image size")
+        if self.kf.img_shapes and tuple(self.kf.img_shapes[0]) != size:
+            raise ValueError("the keyframes must have the size of the views already in the graph")
+        i0 = self.view_num
+        n = len(values)
+        self._ensure_graph(images[0])
+        if i0 == 0:
+            self._graph.pose[0].copy_(self._identity)
+        self.time_dict["prepare_data"] += time.time() - prepare_start
+
+        enc_start = time.time()
+        self.kf.add_views(images, [v["shape"] for v in values])
+        self.time_dict["encoder"] += time.time() - enc_start
+
+        far = [max(0, i0 + k - self.neighbor_edge_num) for k in range(n)]
+        loop_start = time.time()
+        loops = self.lc_detector.detect_loops([v["gray"] for v in values], far)  # read-back: candidates
+        self.time_dict["lc"] += time.time() - loop_start
+        self._check_flags()
+
+        items = [(i0 + k, list(range(far[k], i0 + k)) + [j for j, _ in loops[k][:self.loop_edge_num]]) for k in range(n)]
+        flags = []
+        checked = True
+        results = iter(self._regress_keyframes(items))
+        for k, (v, (i, js)) in enumerate(zip(values, items)):
+            graph_start = time.time()
+            dec_start = time.time()
+            res = next(results)  # the first keyframe of an edge chunk runs the chunk: read-back of its gate
+            self.time_dict["decoder"] += time.time() - dec_start
+            self._check_flags()
+            self.img_shapes.append(v["shape"])
+            self.imgs.append(v["rgb"].squeeze(0).detach())
+            self.view_names.append(v["view_name"])
+            self.view_num += 1
+            if js:
+                conf_host, keep, batch = res
+                kept = set(keep)
+                for e, j in enumerate(js):
+                    names = f"(view {i} [{self.view_names[i]}] -- view {j} [{self.view_names[j]}])"
+                    if e not in kept:
+                        if self.verbose:
+                            _msg("[EdgeReject] ", f"Rejecting edge {names} with conf {conf_host[e]:.3f}")
+                    elif i - j > self.neighbor_edge_num and self.verbose:  # slam.py:199-203
+                        _msg("[LoopClosure] ", f"Adding loop closure edge {names} with conf {conf_host[e]:.3f}")
+                        self.loop_related_views.add(i)
+                        self.loop_related_views.add(j)
+                if keep:
+                    self._add_keyframe(i, js, keep, batch)
+                    checked = False
+            self.time_dict["graph_construction"] += time.time() - graph_start
+
+            if self.view_num % self.pgo_every == 0 or (force_pgo and k == n - 1):
+                if log_intermediate_results:
+                    self.save_data_all(f"{output_folder}", save_view_graph=False, traj_name_postfix=f"{self.view_num - 1}",
+                                       save_poses=True, save_images=False, save_scales=True, save_depths=False,
+                                       save_intrinsics=False, save_confs=False, save_ply=False)
+                opt_start = time.time()
+                self.pose_graph_optimize()
+                self.time_dict["pgo"] += time.time() - opt_start
+                torch.cuda.empty_cache()
+                checked = self.num_nodes > 0 and self.num_edges > 0
+                flags.append(True)
+            else:
+                flags.append(False)
+        if not checked:
+            torch.cuda.current_stream().synchronize()
+            self._check_flags()
+        return flags
 
     def pose_graph_optimize(self):
         """slam.py:108-140 through PoseGraphOpt on the device tables (per-edge weights: DESIGN.md §4)."""
