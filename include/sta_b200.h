@@ -231,11 +231,45 @@ int sta_depth_scale(const float* Di, const float* Dj, const float* ci, const flo
  * PyPose's layout (tx ty tz | qx qy qz qw | s), edges [num_edges][2] int64 (i, j), weights [num_edges][7] fp32,
  * opt_idx [num_opt] int64 (the optimised nodes, all others stay fixed).  info_out (device) [4] fp64 = {loss before,
  * loss after, |delta|_2, Cholesky ok (1/0)}; loss = sum r^T W r.  fp64 inside, deterministic, no host synchronisation: the
- * caller reads info_out to accept or reject the step (as pp.optim.LM does).  scratch: sta_pose_graph_scratch_bytes. ---- */
+ * caller reads info_out to accept or reject the step (as pp.optim.LM does).  scratch: sta_pose_graph_scratch_bytes.
+ * The dense route keeps the 7 num_opt right-hand side in one CTA's shared memory (200 KB): it refuses num_opt above
+ * STA_PG_DENSE_MAX_OPT, and its scratch holds the dense (7 num_opt)^2 fp64 matrix.  Larger graphs take the
+ * block-sparse route below. ---- */
+enum { STA_PG_DENSE_MAX_OPT = 3657 };
 size_t sta_pose_graph_scratch_bytes(int num_nodes, int num_edges, int num_opt);
 int sta_pose_graph_lm_step(const float* nodes, int num_nodes, const int64_t* edges, const float* meas, const float* weights,
                            int num_edges, const int64_t* opt_idx, int num_opt, double damping, double dmin, double dmax,
                            float* nodes_out, double* info_out, void* scratch, void* stream);
+
+/* ---- block-sparse route of the same LM step, for any number of optimised nodes: identical residuals, Jacobians,
+ * normal equations (A, g and loss before equal the dense route's), damping, update and losses; A d = -g is solved by a
+ * block Cholesky factorisation with 7x7 blocks under a nested-dissection ordering, scheduled by elimination-tree levels.
+ * A plan holds the symbolic analysis of one edge list and one optimised set (fixed over the iterations of one
+ * optimisation), device copies of both and the per-iteration scratch.  sta_pg_plan_create takes HOST arrays
+ * edges [num_edges][2] and opt_idx [num_opt] (int64) and refuses, before anything reaches the device: an empty
+ * problem, edge endpoints outside [0, num_nodes), optimised indices out of range or repeated.  It allocates and
+ * uploads synchronously; the plan is used on the device that was current at creation. ---- */
+typedef struct StaPgPlan StaPgPlan; /* opaque */
+int sta_pg_plan_create(const int64_t* edges_host, int num_edges, int num_nodes, const int64_t* opt_idx_host, int num_opt,
+                       StaPgPlan** out);
+void sta_pg_plan_destroy(StaPgPlan* plan);
+/* out4 = {nonzero 7x7 blocks of L, elimination-tree levels, device bytes of the plan, block updates L_Ij L_Kj^T per
+ * factorisation} */
+int sta_pg_plan_info(const StaPgPlan* plan, int64_t* out4);
+/* The host analysis alone (no GPU needed): stats5 = {nonzero blocks of L, nonzero blocks of A's lower triangle, levels,
+ * block updates, device bytes a plan would take}.  Optional outputs (NULL to skip), sized from stats5 by a first call:
+ * order [num_opt] (positions of opt_idx in elimination order), level [num_opt] (elimination-tree level per position),
+ * colptr [num_opt + 1] and blk_row [L blocks] (block pattern of L by column, diagonal block first, then rows ascending),
+ * upd_ptr [L blocks + 1] and upd [2 updates] (per block of L, the pairs of block indices (L_Ij, L_Kj), j ascending). */
+int sta_pg_plan_analyze(const int64_t* edges_host, int num_edges, int num_nodes, const int64_t* opt_idx_host, int num_opt,
+                        int64_t* stats5, int* order, int* level, int* colptr, int* blk_row, int64_t* upd_ptr, int* upd);
+/* One LM step on the plan's edges and optimised set.  Device pointers as in sta_pose_graph_lm_step (nodes / nodes_out
+ * [num_nodes][8], meas [num_edges][8], weights [num_edges][7]); info_out has the same layout.  No host synchronisation;
+ * steps on one plan must not overlap (the scratch is the plan's). */
+int sta_pose_graph_lm_step_sparse(const StaPgPlan* plan, const float* nodes, const float* meas, const float* weights,
+                                  double damping, double dmin, double dmax, float* nodes_out, double* info_out, void* stream);
+/* The last step's update d (device, fp64 [num_opt][7] in opt_idx order), for checking the solve: stream-ordered copy. */
+int sta_pg_plan_last_delta(const StaPgPlan* plan, double* delta_out, void* stream);
 
 /* ---- image preprocessing (SURVEY.md 8(f) rank 3): SLAM_image_only.process_image
  * (vista_slam/datasets/slam_images_only.py:22-34 -> datasets/base/base_view_graph_dataset.py:171-225 ->

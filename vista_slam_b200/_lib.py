@@ -38,6 +38,7 @@ FLOW_MAX_CORNERS = 1000
 GRAPH_MAX_KEYFRAME_EDGES = 32
 GRAPH_FLAG_NOT_SO3 = 1
 ORB_MAX_KEYPOINTS = 4096
+PG_DENSE_MAX_OPT = 3657  # STA_PG_DENSE_MAX_OPT: above it PoseGraphOpt takes the block-sparse route
 
 
 class StaFlowStats(Structure):
@@ -109,6 +110,14 @@ def lib():
     L.sta_pose_graph_scratch_bytes.restype = ctypes.c_size_t
     L.sta_pose_graph_lm_step.argtypes = [vp, i, vp, vp, vp, i, vp, i, ctypes.c_double, ctypes.c_double, ctypes.c_double, vp, vp,
                                          vp, vp]
+    L.sta_pg_plan_create.argtypes = [vp, i, i, vp, i, POINTER(vp)]
+    L.sta_pg_plan_destroy.argtypes = [vp]
+    L.sta_pg_plan_destroy.restype = None
+    L.sta_pg_plan_info.argtypes = [vp, POINTER(c_int64)]
+    L.sta_pg_plan_analyze.argtypes = [vp, i, i, vp, i, POINTER(c_int64), vp, vp, vp, vp, vp, vp]
+    L.sta_pg_plan_last_delta.argtypes = [vp, vp, vp]
+    L.sta_pose_graph_lm_step_sparse.argtypes = [vp, vp, vp, vp, ctypes.c_double, ctypes.c_double, ctypes.c_double, vp, vp,
+                                                vp]
     L.sta_flow_create.argtypes = [i, i, POINTER(vp)]
     L.sta_flow_destroy.argtypes = [vp]
     L.sta_flow_destroy.restype = None

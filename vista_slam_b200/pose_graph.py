@@ -6,12 +6,43 @@ vista_slam/pose_graph.py:70-154): Levenberg-Marquardt with a trust-region dampin
 (sta_pose_graph_lm_step: residuals, Jacobians, normal equations, damped dense Cholesky solve, update and both losses, all on
 the device) followed by one 32-byte read-back for the accept / reject decision -- the same host round trip pp.optim.LM makes.
 Tensors use PyPose's Sim3 layout (tx ty tz | qx qy qz qw | s), fp32, CUDA only (no CPU path).
+
+Two routes solve the damped normal equations, chosen in the constructor from the number of optimised nodes:
+  * dense (num_opt <= _lib.PG_DENSE_MAX_OPT = 3657): sta_pose_graph_lm_step, a dense fp64 Cholesky of order 7 num_opt;
+  * block-sparse (above): sta_pose_graph_lm_step_sparse, a block Cholesky (7x7 blocks) over a plan -- ordering,
+    elimination tree, block pattern and update lists -- built on the host from the edge list and the optimised set.
+Both compute the same residuals, Jacobians, normal equations, damping, update and losses.
 """
 import ctypes
 
 import torch
 
 from . import _lib
+
+
+class _SparsePlan:
+    """Owner of one StaPgPlan (host analysis + device arrays + scratch) for one edge table and optimised set."""
+
+    def __init__(self, edges, num_nodes, idxs_opt):
+        L = _lib.lib()
+        e = edges.detach().to(torch.int64).contiguous().cpu()  # the one device-to-host copy of the edge table
+        o = idxs_opt.cpu()
+        h = ctypes.c_void_p()
+        _lib.check(L.sta_pg_plan_create(_lib.ptr(e), e.shape[0], num_nodes, _lib.ptr(o), o.shape[0], ctypes.byref(h)),
+                   "sta_pg_plan_create")
+        self.h = h
+        self._destroy = L.sta_pg_plan_destroy
+
+    def info(self):
+        """{"l_blocks", "levels", "device_bytes", "updates"} of the plan."""
+        out = (ctypes.c_int64 * 4)()
+        _lib.check(_lib.lib().sta_pg_plan_info(self.h, out), "sta_pg_plan_info")
+        return dict(zip(("l_blocks", "levels", "device_bytes", "updates"), map(int, out)))
+
+    def __del__(self):
+        if getattr(self, "h", None):
+            self._destroy(self.h)
+            self.h = None
 
 
 class PoseGraphOpt:
@@ -25,6 +56,8 @@ class PoseGraphOpt:
         self.idxs_opt = torch.as_tensor(to_optimize_idxs, device=nodes.device).long().contiguous()
         self._scratch = None
         self._info = torch.zeros(4, dtype=torch.float64, device=nodes.device)
+        self.sparse = self.idxs_opt.shape[0] > _lib.PG_DENSE_MAX_OPT
+        self._plan, self._plan_key = None, None
 
     def get_nodes(self):  # pose_graph.py:94-98
         return self.nodes.clone()
@@ -33,10 +66,37 @@ class PoseGraphOpt:
         m = torch.isin(edges, self.idxs_opt)
         return m[:, 0] | m[:, 1]
 
+    def plan(self, edges):
+        """The block-sparse route's plan for `edges`: built on the first call and reused while the same edges tensor
+        (same storage pointer, length and version counter) comes back, as it does across the iterations of optimize().
+        Building it costs one device-to-host copy of the edge table and a host analysis, once per optimize() call."""
+        key = (edges.data_ptr(), edges.shape[0], edges._version, edges.dtype)
+        if self._plan is None or self._plan_key != key:
+            self._plan = None
+            with torch.cuda.device(self.nodes.device):
+                self._plan = _SparsePlan(edges, self.nodes.shape[0], self.idxs_opt)
+            self._plan_key = key
+        return self._plan
+
     @torch.no_grad()
     def lm_step(self, edges, poses, weight, damping, dmin=1e-6, dmax=1e32):
-        """One damped Gauss-Newton solve; returns (candidate nodes, loss_before, loss_after, |delta|, cholesky_ok)."""
+        """One damped Gauss-Newton solve; returns (candidate nodes, loss_before, loss_after, |delta|, cholesky_ok).
+        Above PG_DENSE_MAX_OPT optimised nodes it runs on the block-sparse route (see plan())."""
         L = _lib.lib()
+        if self.sparse:
+            if poses.shape[0] != edges.shape[0] or weight.shape[0] != edges.shape[0]:
+                raise ValueError("edges, poses and weight must have one row per edge")
+            plan = self.plan(edges)
+            poses = poses.to(torch.float32).contiguous()
+            weight = weight.to(torch.float32).contiguous()
+            out = torch.empty_like(self.nodes)
+            with torch.cuda.device(self.nodes.device):
+                _lib.check(L.sta_pose_graph_lm_step_sparse(plan.h, _lib.ptr(self.nodes), _lib.ptr(poses), _lib.ptr(weight),
+                                                           float(damping), float(dmin), float(dmax), _lib.ptr(out),
+                                                           _lib.ptr(self._info), _lib.cur_stream()),
+                           "sta_pose_graph_lm_step_sparse")
+            info = self._info.cpu()  # the one host synchronisation of the iteration
+            return out, float(info[0]), float(info[1]), float(info[2]), bool(info[3] > 0.5)
         edges = edges.to(torch.int64).contiguous()
         poses = poses.to(torch.float32).contiguous()
         weight = weight.to(torch.float32).contiguous()
