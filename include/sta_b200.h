@@ -344,12 +344,13 @@ void sta_vocab_destroy(StaVocab* v);
 int sta_loop_create(StaVocab* v, int loop_dist_min, int loop_nms, int loop_cand_thresh_neighbor, StaLoopDetector** out);
 void sta_loop_destroy(StaLoopDetector* d);
 int sta_loop_views(const StaLoopDetector* d);
-/* compute_bow_feat: ORB, transform and append the view's vector (None when ORB finds no keypoint); asynchronous. */
+/* compute_bow_feat: ORB, transform and append the view's vector (None when ORB finds no keypoint); asynchronous.  The
+ * one-frame case of sta_loop_add_frames. */
 int sta_loop_add_frame(StaLoopDetector* d, const void* frame_dev, int frame_is_f32, int H, int W, void* stream);
 /* detect_loop for the newest view i given farthest_neighbor in [0, i]: similarities against every earlier view in one
  * launch, the candidate scan in one thread, and the one host synchronisation: n_out[2] = {candidates, length of view
  * i's vector (-1: None)}; the first `cap` candidates are written to js_out / sims_out (host) in the reference's order
- * (descending similarity, ties in descending j). */
+ * (descending similarity, ties in descending j).  The one-row case of sta_loop_detect_many. */
 int sta_loop_detect(StaLoopDetector* d, int farthest_neighbor, int* n_out, int64_t* js_out, double* sims_out, int cap,
                     void* stream);
 /* Frame batches, every per-frame result equal to the calls above in frame order.  sta_loop_add_frames: compute_bow_feat
@@ -358,12 +359,12 @@ int sta_loop_detect(StaLoopDetector* d, int farthest_neighbor, int* n_out, int64
  * farthest_host[f] in [0, view index of row f]; one score launch and one detect launch over the F rows, then the one
  * host synchronisation: n_out [2F] = {candidates, length (-1: None)} per row, row f's first cap_per_view candidates at
  * js_out / sims_out + f cap_per_view.  An ORB overflow is reported with the frame's index in the batch.  Afterwards
- * sta_loop_similarities returns the last row. */
+ * sta_loop_similarities returns the last row (n at most that row's view index). */
 int sta_loop_add_frames(StaLoopDetector* d, const void* frames_dev, int frames_is_f32, int F, int H, int W, void* stream);
 int sta_loop_detect_many(StaLoopDetector* d, int F, const int* farthest_host, int* n_out, int64_t* js_out,
                          double* sims_out, int cap_per_view, void* stream);
-/* Test read-backs (synchronise): a view's vector (len -1 for None) and the similarity row of the last detect (NaN where
- * either vector is None). */
+/* Test read-backs (synchronise): a view's vector (len -1 for None) and the last similarity row of the last detect (NaN
+ * where either vector is None). */
 int sta_loop_view(StaLoopDetector* d, int view, int32_t* words_out, double* vals_out, int cap, int* len_out, void* stream);
 int sta_loop_similarities(StaLoopDetector* d, double* sims_out, int n, void* stream);
 /* Op-level entry points (the same kernels).  ORB: scratch of sta_orb_scratch_bytes(H, W) bytes (256-byte aligned; 0 for

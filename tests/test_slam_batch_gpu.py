@@ -410,3 +410,37 @@ def test_step_many_real_frontend(cuda_model, monkeypatch):
     final.step_many(values)
     assert int(L.sta_graph_replays(cuda_model._handle)) - r0 == calls["n"] > 0
     _assert_same_state(_state(final), _state(again))
+
+
+def test_step_read_backs_real_frontend(cuda_model, monkeypatch):
+    """step with no PGO due: per keyframe ONE detect_loop, ONE gate read-back when the keyframe has candidates, and no
+    stream synchronisation (the rotation flag is read at the next read-back)."""
+    from vista_slam_b200.keyframe import KeyframeFrontend
+    counts = {"loops": 0, "gate": 0, "sync": 0}
+    slam = _real_slam(cuda_model, 0.5, {})
+    slam.pgo_every = 1000
+    det = slam.lc_detector
+    orig_loop, orig_read, orig_sync = det.detect_loop, KeyframeFrontend._read_confs, torch.cuda.Stream.synchronize
+
+    def loop(*a):
+        counts["loops"] += 1
+        return orig_loop(*a)
+
+    def read(self, t):
+        counts["gate"] += 1
+        return orig_read(self, t)
+
+    def sync(self):
+        counts["sync"] += 1
+        return orig_sync(self)
+
+    det.detect_loop = loop
+    monkeypatch.setattr(KeyframeFrontend, "_read_confs", read)
+    monkeypatch.setattr(torch.cuda.Stream, "synchronize", sync)
+    for i, v in enumerate(_frames_224(6)):
+        before = dict(counts)
+        assert slam.step(v) is False
+        assert counts["loops"] - before["loops"] == 1
+        assert counts["gate"] - before["gate"] == (1 if i > 0 else 0)
+        assert counts["sync"] == 0
+    assert slam.num_edges > 0

@@ -9,13 +9,12 @@
 // Bit-exact with the numpy restatement under oracle/ (tests/test_loop_gpu.py): the descent takes the first child of minimal
 // Hamming distance; a word's value is its weight added once per descriptor in fp64 (addWeight; all addends of a word
 // are equal, so the order of descriptors does not matter) or set once (addIfNotExist); the L1 norm, the division and the
-// score s += |v - w| - |v| - |w| are sequential fp64 in ascending word id; detect_loop runs in one thread.  One host
-// synchronisation per keyframe: the read-back of the candidate list.
+// score s += |v - w| - |v| - |w| are sequential fp64 in ascending word id; detect_loop runs in one thread per row.
 //
-// Frame batches (sta_loop_add_frames / sta_loop_detect_many) run the same per-frame arithmetic over F frames of one
-// size: ORB with a frame grid dimension, one transform over F x 4096 descriptor slots, one CTA per frame building its
-// vector into a staging slot, an append in frame order, then one score launch and one detect launch over F rows and one
-// read-back.  Every per-frame result equals the sequential path's.
+// One path serves F >= 1 frames of one size (sta_loop_add_frame / sta_loop_detect are its F = 1 case): ORB with a frame
+// grid dimension, one transform over F x 4096 descriptor slots, one CTA per frame building its vector into a staging
+// slot, an append in frame order, then one score launch and one detect launch over F rows and one host
+// synchronisation: the read-back of the candidate lists.  Every per-frame result is independent of F.
 #include "../../include/sta_b200.h"
 #include "common.cuh"
 #include "host_util.h"
@@ -421,40 +420,27 @@ __device__ int build_vector(const int* word, const double* weight, int n, int we
   return len;
 }
 
-// One CTA: the vector written at entry offset *entries_used of the database and its length; *entries_used advances.
-// len = -1 (None) when there was no descriptor.
+// One CTA per frame f: the vector of the descriptors at slot f (kOrbMaxKeypoints apart; count n_dev[f], or n_host
+// without n_dev) into out_word / out_val at slot f, its length (-1: None) into out_len[f].
 __global__ void __launch_bounds__(kBuildThreads) build_kernel(const int* word, const double* weight, const int* n_dev,
-                                                              int n_host, int weighting, int* db_word, double* db_val,
-                                                              long long* db_start, int* db_len, int view,
-                                                              long long* entries_used) {
-  const int n = n_dev ? *n_dev : n_host;
-  const long long base = *entries_used;
-  const int len = build_vector(word, weight, n, weighting, db_word + base, db_val + base);
-  if (threadIdx.x == 0) {
-    db_start[view] = base;
-    db_len[view] = n > 0 ? len : -1;
-    *entries_used = base + len;
-  }
+                                                              int n_host, int weighting, int* out_word, double* out_val,
+                                                              int* out_len) {
+  const long long f = blockIdx.x, m = f * kOrbMaxKeypoints;
+  const int n = n_dev ? n_dev[f] : n_host;
+  const int len = build_vector(word + m, weight + m, n, weighting, out_word + m, out_val + m);
+  if (threadIdx.x == 0) out_len[f] = n > 0 ? len : -1;
 }
 
-// One CTA per frame of a batch: frame f's vector into staging slot f (kOrbMaxKeypoints entries), its length (-1: None)
-// into stage_len[f].  Frame f's descriptors are at slot f (kOrbMaxKeypoints apart), its count at n_dev[f].
-__global__ void __launch_bounds__(kBuildThreads) build_many_kernel(const int* word, const double* weight, const int* n_dev,
-                                                                   int weighting, int* stage_word, double* stage_val,
-                                                                   int* stage_len) {
-  const long long f = blockIdx.x, m = f * kOrbMaxKeypoints;
-  const int n = n_dev[f];
-  const int len = build_vector(word + m, weight + m, n, weighting, stage_word + m, stage_val + m);
-  if (threadIdx.x == 0) stage_len[f] = n > 0 ? len : -1;
+// Database entries in use after view v: a None view (length -1) starts where the next one does.
+__device__ long long db_end(const long long* db_start, const int* db_len, int v) {
+  return db_start[v] + (db_len[v] > 0 ? db_len[v] : 0);
 }
 
 // Appends the F staged vectors to the database in frame order (one CTA per frame); views view0 .. view0 + F - 1.
-// *entries_used is advanced by advance_entries_kernel afterwards, so every CTA reads the same base here.
-__global__ void append_many_kernel(const int* stage_word, const double* stage_val, const int* stage_len, int F, int view0,
-                                   int* db_word, double* db_val, long long* db_start, int* db_len,
-                                   const long long* entries_used) {
+__global__ void append_kernel(const int* stage_word, const double* stage_val, const int* stage_len, int view0,
+                              int* db_word, double* db_val, long long* db_start, int* db_len) {
   const int f = blockIdx.x;
-  long long base = *entries_used;
+  long long base = view0 > 0 ? db_end(db_start, db_len, view0 - 1) : 0;
   for (int g = 0; g < f; ++g) base += stage_len[g] > 0 ? stage_len[g] : 0;
   const int len = stage_len[f];
   for (int k = threadIdx.x; k < len; k += blockDim.x) {
@@ -465,12 +451,6 @@ __global__ void append_many_kernel(const int* stage_word, const double* stage_va
     db_start[view0 + f] = base;
     db_len[view0 + f] = len;
   }
-}
-
-__global__ void advance_entries_kernel(const int* stage_len, int F, long long* entries_used) {
-  long long e = *entries_used;
-  for (int g = 0; g < F; ++g) e += stage_len[g] > 0 ? stage_len[g] : 0;
-  *entries_used = e;
 }
 
 // L1Scoring::score of vector a against vector b, a merge over ascending word ids; NaN when either is None (length -1).
@@ -493,24 +473,16 @@ __device__ double l1_score(const int* aw, const double* av, int na, const int* b
   return __ddiv_rn(-s, 2.0);
 }
 
-// Score of view q against views [0, nviews): one thread per view.
-__global__ void score_kernel(const int* qw, const double* qv, const int* q_len_dev, const long long* q_start_dev,
+// Row y = blockIdx.y: query y (length q_len[y], at entry q_start[y] of qw / qv, or 0 without q_start) against views
+// [0, i0 + y), one thread per view, into sims + y stride.
+__global__ void score_kernel(const int* qw, const double* qv, const long long* q_start, const int* q_len,
                              const int* db_word, const double* db_val, const long long* db_start, const int* db_len,
-                             int nviews, double* sims) {
+                             int i0, double* sims, long long stride) {
+  const int y = blockIdx.y;
   const int j = blockIdx.x * blockDim.x + threadIdx.x;
-  if (j >= nviews) return;
-  const long long qa = q_start_dev ? *q_start_dev : 0;
-  sims[j] = l1_score(qw + qa, qv + qa, *q_len_dev, db_word + db_start[j], db_val + db_start[j], db_len[j]);
-}
-
-// Rows i = i0 + blockIdx.y of a batch: view i against views [0, i), into sims + blockIdx.y * stride.
-__global__ void score_many_kernel(const int* db_word, const double* db_val, const long long* db_start, const int* db_len,
-                                  int i0, double* sims, long long stride) {
-  const int i = i0 + blockIdx.y;
-  const int j = blockIdx.x * blockDim.x + threadIdx.x;
-  if (j >= i) return;
-  sims[blockIdx.y * stride + j] = l1_score(db_word + db_start[i], db_val + db_start[i], db_len[i], db_word + db_start[j],
-                                           db_val + db_start[j], db_len[j]);
+  if (j >= i0 + y) return;
+  const long long qa = q_start ? q_start[y] : 0;
+  sims[y * stride + j] = l1_score(qw + qa, qv + qa, q_len[y], db_word + db_start[j], db_val + db_start[j], db_len[j]);
 }
 
 // loop_detector.py:23-50 over the precomputed similarities of view i; out: [0] = count, [1] = length of view i, then
@@ -552,20 +524,16 @@ __device__ void detect_row(const double* sims, const int* db_len, int i, int far
   out[1] = db_len[i];
 }
 
-__global__ void detect_kernel(const double* sims, const int* db_len, int i, int farthest, int dist_min, int nms,
-                              int thresh_neighbor, long long* out) {
-  detect_row(sims, db_len, i, farthest, dist_min, nms, thresh_neighbor, out);
-}
-
-// One thread per row f of a batch (view i0 + f): out row f = {ORB overflow flag of frame f, then detect_row's count,
-// length and pairs}, `out_stride` entries apart.
-__global__ void detect_many_kernel(const double* sims, long long sims_stride, const int* db_len, int i0,
-                                   const int* farthest, int dist_min, int nms, int thresh_neighbor, long long* out,
-                                   long long out_stride, const unsigned* overflow, size_t overflow_stride) {
+// One thread per row f (view i0 + f): out row f = {ORB overflow flag of frame f, then detect_row's count, length and
+// pairs}, `out_stride` entries apart; after the gridDim.x rows, the database entries in use.
+__global__ void detect_kernel(const double* sims, long long sims_stride, const long long* db_start, const int* db_len,
+                              int i0, const int* farthest, int dist_min, int nms, int thresh_neighbor, long long* out,
+                              long long out_stride, const unsigned* overflow, size_t overflow_stride) {
   const int f = blockIdx.x;
   long long* row = out + f * out_stride;
   detect_row(sims + f * sims_stride, db_len, i0 + f, farthest[f], dist_min, nms, thresh_neighbor, row + 1);
   row[0] = *reinterpret_cast<const unsigned*>(reinterpret_cast<const char*>(overflow) + f * overflow_stride);
+  if (f == static_cast<int>(gridDim.x) - 1) out[(f + 1) * out_stride] = db_end(db_start, db_len, i0 + f);
 }
 
 }  // namespace
@@ -581,30 +549,26 @@ struct StaLoopDetector {
   void* scratch = nullptr;        // ORB scratch: frame_cap slices of lay.total bytes
   void* kp = nullptr;             // ORB outputs + transform outputs: frame_cap slices of kKpSlice bytes
   int frame_cap = 0, stage_cap = 0;
-  int newest_slice = 0;           // scratch slice of the newest view (its ORB overflow flag)
   int last_batch = 0;             // frames of the last add call
-  int* stage_word = nullptr;      // [frame_cap][kOrbMaxKeypoints] vectors of a batch before the append
+  int* stage_word = nullptr;      // [stage_cap][kOrbMaxKeypoints] vectors of a batch before the append
   double* stage_val = nullptr;
-  int* stage_len = nullptr;       // [frame_cap]
-  double* sims_many = nullptr;    // [rows][views] of sta_loop_detect_many
-  long long* result_many = nullptr;
-  long long* pinned_many = nullptr;
-  long long many_cap = 0;         // entries of sims_many / result_many / pinned_many
-  int* farthest_dev = nullptr;    // [frame_cap]
-  int* farthest_pinned = nullptr;
+  int* stage_len = nullptr;       // [stage_cap]
+  int* farthest_pinned = nullptr; // [stage_cap], read by the detect kernel in place (mapped host memory)
+  double* sims = nullptr;         // [rows][views] of the last detect
+  long long* result = nullptr;    // its rows and the database entries in use
+  long long* pinned = nullptr;    // host copy of result
+  long long out_cap = 0;          // entries of sims / result / pinned
+  long long last_row = 0;         // offset in sims of the last detect's last row
+  int last_row_len = 0;           // its length (the view index of that row)
   int views = 0, view_cap = 0;
   // Upper bound on the database entries in use, kept on the host: each appended view may add up to kOrbMaxKeypoints
-  // words, and the exact count (entries_dev) is only read back at the synchronisation of sta_loop_detect.
+  // words, and the exact count is only read back at the synchronisation of a detect.
   long long entries_bound = 0, entry_cap = 0;
   cudaStream_t last_stream = nullptr;  // the stream of the last call, synchronised before destruction
   int* db_word = nullptr;
   double* db_val = nullptr;
   long long* db_start = nullptr;
   int* db_len = nullptr;
-  double* sims = nullptr;
-  long long* result = nullptr;    // device [2 + 2 view_cap]
-  long long* entries_dev = nullptr;
-  long long* pinned = nullptr;    // host copy of result
 };
 
 namespace {
@@ -651,15 +615,11 @@ int grow(T** p, long long old_n, long long new_n, cudaStream_t st) {
 }
 
 // room for F more views of up to kOrbMaxKeypoints words each
-int reserve(StaLoopDetector* d, cudaStream_t st, int F = 1) {
+int reserve(StaLoopDetector* d, cudaStream_t st, int F) {
   if (d->views + F > d->view_cap) {
     int cap = d->view_cap ? 2 * d->view_cap : 256;
     while (cap < d->views + F) cap *= 2;
-    if (grow(&d->db_start, d->view_cap, cap, st) || grow(&d->db_len, d->view_cap, cap, st) ||
-        grow(&d->sims, 0, cap, st) || grow(&d->result, 0, 2 + 2LL * cap, st))
-      return 1;
-    if (d->pinned) cudaFreeHost(d->pinned);
-    STA_CHECK_CUDA(cudaMallocHost(&d->pinned, sizeof(long long) * (2 + 2LL * cap)));
+    if (grow(&d->db_start, d->view_cap, cap, st) || grow(&d->db_len, d->view_cap, cap, st)) return 1;
     d->view_cap = cap;
   }
   const long long need = d->entries_bound + static_cast<long long>(F) * kOrbMaxKeypoints;
@@ -705,9 +665,7 @@ int prepare_frames(StaLoopDetector* d, int F, int H, int W, cudaStream_t st) {
 int grow_batch(StaLoopDetector* d, int F, cudaStream_t st) {
   if (F <= d->stage_cap) return 0;
   const long long M = kOrbMaxKeypoints;
-  if (grow(&d->stage_word, 0, M * F, st) || grow(&d->stage_val, 0, M * F, st) || grow(&d->stage_len, 0, F, st) ||
-      grow(&d->farthest_dev, 0, F, st))
-    return 1;
+  if (grow(&d->stage_word, 0, M * F, st) || grow(&d->stage_val, 0, M * F, st) || grow(&d->stage_len, 0, F, st)) return 1;
   if (d->farthest_pinned) cudaFreeHost(d->farthest_pinned);
   d->farthest_pinned = nullptr;
   STA_CHECK_CUDA(cudaMallocHost(&d->farthest_pinned, sizeof(int) * F));
@@ -779,14 +737,9 @@ int sta_op_bow_transform(const StaVocab* v, const uint8_t* desc_dev, int n, int3
 int sta_op_bow_vector(const StaVocab* v, const int32_t* word, const double* weight, int n, int32_t* words_out,
                       double* vals_out, int32_t* len_out, void* stream) {
   STA_REQUIRE(v && n >= 0 && n <= kOrbMaxKeypoints, "descriptor count must be in [0, 4096]");
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  long long* tmp = nullptr;
-  STA_CHECK_CUDA(cudaMallocAsync(&tmp, sizeof(long long) * 2, st));
-  STA_CHECK_CUDA(cudaMemsetAsync(tmp, 0, sizeof(long long) * 2, st));
-  build_kernel<<<1, kBuildThreads, 0, st>>>(word, weight, nullptr, n, v->weighting, words_out, vals_out, tmp + 1,
-                                            len_out, 0, tmp);
+  build_kernel<<<1, kBuildThreads, 0, static_cast<cudaStream_t>(stream)>>>(word, weight, nullptr, n, v->weighting,
+                                                                           words_out, vals_out, len_out);
   STA_CHECK_CUDA(cudaGetLastError());
-  STA_CHECK_CUDA(cudaFreeAsync(tmp, st));
   return 0;
 }
 
@@ -796,8 +749,8 @@ int sta_op_bow_score(const int32_t* qw, const double* qv, const int32_t* q_len_d
   STA_REQUIRE(nviews >= 0, "bad view count");
   if (nviews)
     score_kernel<<<(nviews + 127) / 128, 128, 0, static_cast<cudaStream_t>(stream)>>>(
-        qw, qv, q_len_dev, nullptr, db_word, db_val, reinterpret_cast<const long long*>(db_start), db_len, nviews,
-        sims_out);
+        qw, qv, nullptr, q_len_dev, db_word, db_val, reinterpret_cast<const long long*>(db_start), db_len, nviews,
+        sims_out, 0);
   STA_CHECK_CUDA(cudaGetLastError());
   return 0;
 }
@@ -809,12 +762,6 @@ int sta_loop_create(StaVocab* v, int loop_dist_min, int loop_nms, int loop_cand_
   d->dist_min = loop_dist_min;
   d->nms = loop_nms;
   d->thresh_neighbor = loop_cand_thresh_neighbor;
-  if (cudaMalloc(&d->entries_dev, sizeof(long long)) != cudaSuccess ||
-      cudaMemset(d->entries_dev, 0, sizeof(long long)) != cudaSuccess) {
-    delete d;
-    set_last_error("sta_loop_create: allocation failed");
-    return 1;
-  }
   *out = d;
   return 0;
 }
@@ -830,41 +777,15 @@ void sta_loop_destroy(StaLoopDetector* d) {
   cudaFree(d->db_len);
   cudaFree(d->sims);
   cudaFree(d->result);
-  cudaFree(d->entries_dev);
   cudaFree(d->stage_word);
   cudaFree(d->stage_val);
   cudaFree(d->stage_len);
-  cudaFree(d->sims_many);
-  cudaFree(d->result_many);
-  cudaFree(d->farthest_dev);
   if (d->pinned) cudaFreeHost(d->pinned);
-  if (d->pinned_many) cudaFreeHost(d->pinned_many);
   if (d->farthest_pinned) cudaFreeHost(d->farthest_pinned);
   delete d;
 }
 
 int sta_loop_views(const StaLoopDetector* d) { return d ? d->views : -1; }
-
-// compute_bow_feat: ORB + transform + append to the database (asynchronous)
-int sta_loop_add_frame(StaLoopDetector* d, const void* frame_dev, int frame_is_f32, int H, int W, void* stream) {
-  STA_REQUIRE(d, "null detector");
-  STA_REQUIRE(orb_size_ok(H, W), "ORB frame sides must be in [32, 4096]");
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (prepare_frames(d, 1, H, W, st) || reserve(d, st)) return 1;
-  KpBufs b = kp_bufs(d->kp, d->frame_cap);
-  OrbOut o = {b.xy, b.level, b.pts, b.angle, b.resp, b.desc, b.count};
-  if (orb_run(d->lay, d->scratch, frame_dev, frame_is_f32, o, st)) return 1;
-  if (bow_of_descriptors(d->vocab, b.desc, b.count, 0, b.word, b.weight, st)) return 1;
-  build_kernel<<<1, kBuildThreads, 0, st>>>(b.word, b.weight, b.count, 0, d->vocab->weighting, d->db_word, d->db_val,
-                                            d->db_start, d->db_len, d->views, d->entries_dev);
-  STA_CHECK_CUDA(cudaGetLastError());
-  d->views += 1;
-  d->entries_bound += kOrbMaxKeypoints;
-  d->newest_slice = 0;
-  d->last_batch = 1;
-  d->last_stream = st;
-  return 0;
-}
 
 // compute_bow_feat for F frames [F][H][W] of one size: ORB over all frames, one transform, one build CTA per frame and
 // the append in frame order (asynchronous)
@@ -878,59 +799,27 @@ int sta_loop_add_frames(StaLoopDetector* d, const void* frames_dev, int frames_i
   OrbOut o = {b.xy, b.level, b.pts, b.angle, b.resp, b.desc, b.count};
   if (orb_run(d->lay, d->scratch, frames_dev, frames_is_f32, o, st, F)) return 1;
   if (bow_of_descriptors(d->vocab, b.desc, b.count, 0, b.word, b.weight, st, F)) return 1;
-  build_many_kernel<<<F, kBuildThreads, 0, st>>>(b.word, b.weight, b.count, d->vocab->weighting, d->stage_word,
-                                                 d->stage_val, d->stage_len);
-  append_many_kernel<<<F, 256, 0, st>>>(d->stage_word, d->stage_val, d->stage_len, F, d->views, d->db_word, d->db_val,
-                                        d->db_start, d->db_len, d->entries_dev);
-  advance_entries_kernel<<<1, 1, 0, st>>>(d->stage_len, F, d->entries_dev);
+  build_kernel<<<F, kBuildThreads, 0, st>>>(b.word, b.weight, b.count, 0, d->vocab->weighting, d->stage_word,
+                                            d->stage_val, d->stage_len);
+  append_kernel<<<F, 256, 0, st>>>(d->stage_word, d->stage_val, d->stage_len, d->views, d->db_word, d->db_val,
+                                   d->db_start, d->db_len);
   STA_CHECK_CUDA(cudaGetLastError());
   d->views += F;
   d->entries_bound += static_cast<long long>(F) * kOrbMaxKeypoints;
-  d->newest_slice = F - 1;
   d->last_batch = F;
   d->last_stream = st;
   return 0;
 }
 
-// detect_loop for the newest view: scores against every earlier view, the candidate scan, and one read-back.
-// js_out / sims_out (host) receive up to `cap` candidates; n_out[2] = {number found, length of view i (-1: None)}.
-int sta_loop_detect(StaLoopDetector* d, int farthest_neighbor, int* n_out, int64_t* js_out, double* sims_out, int cap,
-                    void* stream) {
-  STA_REQUIRE(d && d->views > 0, "no view has been added");
-  const int i = d->views - 1;
-  STA_REQUIRE(farthest_neighbor >= 0 && farthest_neighbor <= i, "farthest_neighbor must be in [0, view index]");
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  d->last_stream = st;
-  if (i > 0)
-    score_kernel<<<(i + 127) / 128, 128, 0, st>>>(d->db_word, d->db_val, d->db_len + i, d->db_start + i, d->db_word,
-                                                  d->db_val, d->db_start, d->db_len, i, d->sims);
-  detect_kernel<<<1, 1, 0, st>>>(d->sims, d->db_len, i, farthest_neighbor, d->dist_min, d->nms, d->thresh_neighbor,
-                                 d->result);
-  STA_CHECK_CUDA(cudaGetLastError());
-  const size_t nb = sizeof(long long) * (2 + 2LL * (i + 1));
-  STA_CHECK_CUDA(cudaMemcpyAsync(d->pinned, d->result, nb, cudaMemcpyDeviceToHost, st));
-  STA_CHECK_CUDA(cudaMemcpyAsync(&d->entries_bound, d->entries_dev, sizeof(long long), cudaMemcpyDeviceToHost, st));
-  unsigned overflow = 0;
-  STA_CHECK_CUDA(cudaMemcpyAsync(&overflow,
-                                 static_cast<char*>(d->scratch) + d->newest_slice * d->lay.total + d->lay.counters +
-                                     3 * sizeof(unsigned),
-                                 sizeof(unsigned), cudaMemcpyDeviceToHost, st));
-  STA_CHECK_CUDA(cudaStreamSynchronize(st));
-  STA_REQUIRE(!overflow, "the frame has more ORB candidates or keypoints than the detector holds");
-  const int n = static_cast<int>(d->pinned[0]);
-  n_out[0] = n;
-  n_out[1] = static_cast<int>(d->pinned[1]);
-  for (int k = 0; k < n && k < cap; ++k) {
-    js_out[k] = d->pinned[2 + 2 * k];
-    memcpy(&sims_out[k], &d->pinned[3 + 2 * k], sizeof(double));
-  }
-  return 0;
+// compute_bow_feat: the one-frame case of sta_loop_add_frames
+int sta_loop_add_frame(StaLoopDetector* d, const void* frame_dev, int frame_is_f32, int H, int W, void* stream) {
+  return sta_loop_add_frames(d, frame_dev, frame_is_f32, 1, H, W, stream);
 }
 
 // detect_loop for each of the newest F views (the frames of the last sta_loop_add_frames, or fewer of its newest), row
-// f = view views - F + f against every earlier view: one score launch, one detect launch and one read-back.
-// n_out [2F] = {candidates, length (-1: None)} per row; row f's first cap_per_view candidates go to
-// js_out / sims_out + f cap_per_view (host).  Afterwards sta_loop_similarities returns the last row.
+// f = view views - F + f against every earlier view: one score launch, one detect launch and one read-back, which also
+// brings the database's entry count.  n_out [2F] = {candidates, length (-1: None)} per row; row f's first cap_per_view
+// candidates go to js_out / sims_out + f cap_per_view (host).  Afterwards sta_loop_similarities returns the last row.
 int sta_loop_detect_many(StaLoopDetector* d, int F, const int* farthest_host, int* n_out, int64_t* js_out,
                          double* sims_out, int cap_per_view, void* stream) {
   STA_REQUIRE(d && farthest_host && n_out && (cap_per_view == 0 || (js_out && sims_out)), "null argument");
@@ -941,48 +830,46 @@ int sta_loop_detect_many(StaLoopDetector* d, int F, const int* farthest_host, in
     STA_REQUIRE(farthest_host[f] >= 0 && farthest_host[f] <= i0 + f, "farthest_neighbor must be in [0, view index]");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   d->last_stream = st;
-  const long long sims_stride = d->views, out_stride = 3 + 2LL * d->views;
-  const long long need = F * (out_stride > sims_stride ? out_stride : sims_stride);
-  if (need > d->many_cap) {
-    long long cap = d->many_cap ? 2 * d->many_cap : 1LL << 14;
+  const long long sims_stride = d->views, out_stride = 3 + 2LL * d->views;  // out_stride > sims_stride
+  const long long need = F * out_stride + 1;
+  if (need > d->out_cap) {
+    long long cap = d->out_cap ? 2 * d->out_cap : 1LL << 14;
     while (cap < need) cap *= 2;
-    if (grow(&d->sims_many, 0, cap, st) || grow(&d->result_many, 0, cap, st)) return 1;
-    if (d->pinned_many) cudaFreeHost(d->pinned_many);
-    d->pinned_many = nullptr;
-    STA_CHECK_CUDA(cudaMallocHost(&d->pinned_many, sizeof(long long) * cap));
-    d->many_cap = cap;
+    if (grow(&d->sims, 0, cap, st) || grow(&d->result, 0, cap, st)) return 1;
+    if (d->pinned) cudaFreeHost(d->pinned);
+    d->pinned = nullptr;
+    STA_CHECK_CUDA(cudaMallocHost(&d->pinned, sizeof(long long) * cap));
+    d->out_cap = cap;
   }
-  memcpy(d->farthest_pinned, farthest_host, sizeof(int) * F);
-  STA_CHECK_CUDA(cudaMemcpyAsync(d->farthest_dev, d->farthest_pinned, sizeof(int) * F, cudaMemcpyHostToDevice, st));
+  memcpy(d->farthest_pinned, farthest_host, sizeof(int) * F);  // the previous detect has synchronised
   const int i_last = d->views - 1;
   if (i_last > 0)
-    score_many_kernel<<<dim3((i_last + 127) / 128, F), 128, 0, st>>>(d->db_word, d->db_val, d->db_start, d->db_len, i0,
-                                                                      d->sims_many, sims_stride);
+    score_kernel<<<dim3((i_last + 127) / 128, F), 128, 0, st>>>(d->db_word, d->db_val, d->db_start + i0, d->db_len + i0,
+                                                                 d->db_word, d->db_val, d->db_start, d->db_len, i0,
+                                                                 d->sims, sims_stride);
   const int first_slice = d->last_batch - F;  // scratch slice of row 0
-  detect_many_kernel<<<F, 1, 0, st>>>(d->sims_many, sims_stride, d->db_len, i0, d->farthest_dev, d->dist_min, d->nms,
-                                      d->thresh_neighbor, d->result_many, out_stride,
-                                      reinterpret_cast<const unsigned*>(static_cast<char*>(d->scratch) +
-                                                                        first_slice * d->lay.total + d->lay.counters +
-                                                                        3 * sizeof(unsigned)),
-                                      d->lay.total);
+  detect_kernel<<<F, 1, 0, st>>>(d->sims, sims_stride, d->db_start, d->db_len, i0, d->farthest_pinned, d->dist_min,
+                                 d->nms, d->thresh_neighbor, d->result, out_stride,
+                                 reinterpret_cast<const unsigned*>(static_cast<char*>(d->scratch) +
+                                                                   first_slice * d->lay.total + d->lay.counters +
+                                                                   3 * sizeof(unsigned)),
+                                 d->lay.total);
   STA_CHECK_CUDA(cudaGetLastError());
-  if (i_last > 0)
-    STA_CHECK_CUDA(cudaMemcpyAsync(d->sims, d->sims_many + (F - 1) * sims_stride, sizeof(double) * i_last,
-                                   cudaMemcpyDeviceToDevice, st));
-  STA_CHECK_CUDA(cudaMemcpyAsync(d->pinned_many, d->result_many, sizeof(long long) * F * out_stride,
-                                 cudaMemcpyDeviceToHost, st));
-  STA_CHECK_CUDA(cudaMemcpyAsync(&d->entries_bound, d->entries_dev, sizeof(long long), cudaMemcpyDeviceToHost, st));
+  d->last_row = (F - 1) * sims_stride;
+  d->last_row_len = i_last;
+  STA_CHECK_CUDA(cudaMemcpyAsync(d->pinned, d->result, sizeof(long long) * need, cudaMemcpyDeviceToHost, st));
   STA_CHECK_CUDA(cudaStreamSynchronize(st));
+  d->entries_bound = d->pinned[F * out_stride];
   for (int f = 0; f < F; ++f) {
-    const long long* row = d->pinned_many + f * out_stride;
+    const long long* row = d->pinned + f * out_stride;
     if (row[0]) {
-      set_last_error("frame " + std::to_string(f) +
-                     " of the batch has more ORB candidates or keypoints than the detector holds");
+      set_last_error((F == 1 ? std::string("the frame") : "frame " + std::to_string(f) + " of the batch") +
+                     " has more ORB candidates or keypoints than the detector holds");
       return 1;
     }
   }
   for (int f = 0; f < F; ++f) {
-    const long long* row = d->pinned_many + f * out_stride;
+    const long long* row = d->pinned + f * out_stride;
     const int n = static_cast<int>(row[1]);
     n_out[2 * f] = n;
     n_out[2 * f + 1] = static_cast<int>(row[2]);
@@ -992,6 +879,14 @@ int sta_loop_detect_many(StaLoopDetector* d, int F, const int* farthest_host, in
     }
   }
   return 0;
+}
+
+// detect_loop for the newest view: the one-row case of sta_loop_detect_many.
+// js_out / sims_out (host) receive up to `cap` candidates; n_out[2] = {number found, length of view i (-1: None)}.
+int sta_loop_detect(StaLoopDetector* d, int farthest_neighbor, int* n_out, int64_t* js_out, double* sims_out, int cap,
+                    void* stream) {
+  STA_REQUIRE(d && d->views > 0, "no view has been added");
+  return sta_loop_detect_many(d, 1, &farthest_neighbor, n_out, js_out, sims_out, cap, stream);
 }
 
 // Host copy of view `view`'s vector (synchronises): *len_out = -1 for None; up to cap entries are written.
@@ -1013,12 +908,12 @@ int sta_loop_view(StaLoopDetector* d, int view, int32_t* words_out, double* vals
   return 0;
 }
 
-// Host copy of the similarity row of the last sta_loop_detect (NaN where a vector is None); n = view index.
+// Host copy of the last row of the last detect (NaN where a vector is None); n = that row's view index.
 int sta_loop_similarities(StaLoopDetector* d, double* sims_out, int n, void* stream) {
-  STA_REQUIRE(d && n >= 0 && n < d->views, "bad count");
+  STA_REQUIRE(d && n >= 0 && n <= d->last_row_len, "bad count: n must be at most the view index of the last detect");
   if (n == 0) return 0;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  STA_CHECK_CUDA(cudaMemcpyAsync(sims_out, d->sims, sizeof(double) * n, cudaMemcpyDeviceToHost, st));
+  STA_CHECK_CUDA(cudaMemcpyAsync(sims_out, d->sims + d->last_row, sizeof(double) * n, cudaMemcpyDeviceToHost, st));
   STA_CHECK_CUDA(cudaStreamSynchronize(st));
   return 0;
 }

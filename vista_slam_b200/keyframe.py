@@ -35,13 +35,9 @@ class KeyframeFrontend:
     def view_num(self):
         return len(self.enc_features)
 
-    @torch.no_grad()
     def add_view(self, image, image_shape=None):
         """slam.py:142-151: encode one view (B = 1) and cache its features; returns the view index."""
-        feat, _ = self.frontend._encode_image(image, image_shape, normalize=False)
-        self.enc_features.append(feat)
-        self.img_shapes.append((int(image.shape[-2]), int(image.shape[-1])))
-        return len(self.enc_features) - 1
+        return self.add_views([image], [image_shape])[0]
 
     @torch.no_grad()
     def add_views(self, images, image_shapes=None):
@@ -198,48 +194,20 @@ class KeyframeFrontend:
     def regress_views_gated(self, i, js, rel_pose_thres):
         """The keyframe step with the reference's early-out (slam.py:169-170) kept: ONE decoder + pose-head pass over all
         candidate edges (i, j), ONE device-to-host copy of the K pose confidences, then the DPT heads and the pointmap
-        consumers only for the edges the reference would keep (`conf >= thres or i - j == 1`).
+        consumers only for the edges the reference would keep (`conf >= thres or i - j == 1`).  The one-keyframe,
+        unpadded case of regress_keyframes_gated.
 
         Returns a list with one entry per candidate, in the return convention of OnlineSLAM.regress_two_views
         (slam.py:153-189) minus the pypose conversion, which stays with the caller:
             (pose_ij [1,4,4], rel_pose_conf_ij [1], confs [2,H,W] | None, intri [3,3] | None, depths [2,H,W] | None)
         -- the last three are None for rejected edges, exactly where the reference returns None."""
         js = list(js)
-        K = len(js)
-        if K == 0:
+        if not js:
             return []
-        L, fi, fj, H, W, f32, pose, pconf = self._edge_batch(i, js)
-        dev = fi.device
-        m = self.frontend
-        with torch.cuda.device(dev):
-            _lib.check(L.sta_regress_pairs_begin(m._handle, _lib.ptr(fi), _lib.ptr(fj), K, H, W, _lib.ptr(pose), _lib.ptr(pconf),
-                                                 _lib.cur_stream()), "sta_regress_pairs_begin")
-            conf_host = pconf[0].cpu()  # the one host synchronisation of the keyframe (slam.py:169 has one per edge)
-            keep = [k for k, j in enumerate(js) if not (float(conf_host[k]) < rel_pose_thres and i - j != 1)]
-            n = len(keep)
-            out = [(pose[0, k:k + 1], pconf[0, k:k + 1], None, None, None) for k in range(K)]
-            if n == 0:
-                return out
-            pts = f32(2, n, H, W, 3)
-            conf = f32(2, n, H, W)
-            intri = f32(n, 3, 3)
-            depth = f32(2, n, H, W)
-            cmean = f32(2, n)
-            idx = (ctypes.c_int * n)(*keep)
-            _lib.check(L.sta_regress_pairs_finish(m._handle, idx, n, _lib.ptr(pts), _lib.ptr(conf), _lib.ptr(intri),
-                                                  _lib.ptr(depth), _lib.ptr(cmean), _lib.ptr(_scratch_for(dev, 2 * n)),
-                                                  _lib.cur_stream()),
-                       "sta_regress_pairs_finish")
-        for pos, k in enumerate(keep):
-            out[k] = (pose[0, k:k + 1], pconf[0, k:k + 1], conf[:, pos], intri[pos], depth[:, pos])
-        self.last_pts3d = pts  # [2, n, H, W, 3] of the kept edges (diagnostics / tests)
-        self.last_kept = keep
-        # the compact outputs of the kept edges, as the device pose graph takes them (OnlineSLAM.step):
-        # pose [K, 4, 4] and pose_conf [K] of all candidates (i -> j), conf / depths [2, n, H, W], intri [n, 3, 3],
-        # conf_mean [2, n]; and the K confidences read back for the gate
-        self.last_conf_host = [float(c) for c in conf_host]
-        self.last_batch = {"pose": pose[0], "pose_conf": pconf[0], "conf": conf, "depths": depth, "intri": intri,
-                           "conf_mean": cmean}
+        (_, keep, b), = self._regress_chunk([(i, js)], rel_pose_thres, pad=False)
+        out = [(b["pose"][k:k + 1], b["pose_conf"][k:k + 1], None, None, None) for k in range(len(js))]
+        for p, k in enumerate(keep):
+            out[k] = out[k][:2] + (b["conf"][:, p], b["intri"][p], b["depths"][:, p])
         return out
 
     @torch.no_grad()

@@ -5,8 +5,8 @@ Same constructor (arguments and defaults) and the surface run.py, run_live.py an
 `pose_graph_optimize`, `get_view`, `get_view_graph`, `save_data_all`, `get_pointmap_vis`, `save_pointmap`,
 `get_time_dict`.  It is built from this package's stages:
 
-  * KeyframeFrontend.regress_views_gated: one decoder pass over all candidate edges of a keyframe, one read-back of their
-    pose confidences (the gate), DPT heads and pointmap consumers for the kept edges only;
+  * KeyframeFrontend.regress_keyframes_gated: one decoder pass over all candidate edges of a keyframe, one read-back of
+    their pose confidences (the gate), DPT heads and pointmap consumers for the kept edges only;
   * LoopDetector and FlowTracker on the device;
   * the device pose graph (csrc/slam_graph.cu, `sta_graph_*`): node / edge tables, the depth / confidence / intrinsics
     store and the per-view best node live in fixed-capacity device arrays sized from the reference's formulas
@@ -207,9 +207,8 @@ class OnlineSLAM:
     def _regress_keyframe(self, i, js):
         """The frontend's part of a keyframe: (the K pose confidences on the host, indices of the kept candidates, the
         device batch {pose [K,4,4], pose_conf [K], conf / depths [2,n,H,W], intri [n,3,3], conf_mean [2,n]})."""
-        out = self.kf.regress_views_gated(i, js, self.rel_pose_thres)
-        keep = [k for k, o in enumerate(out) if o[2] is not None]
-        return self.kf.last_conf_host, keep, self.kf.last_batch
+        res, = self.kf.regress_keyframes_gated([(i, js)], self.rel_pose_thres)
+        return res
 
     def _regress_keyframes(self, items):
         """The frontend's part of many keyframes items = [(i, js), ...]: per item, in order, what _regress_keyframe
@@ -247,6 +246,37 @@ class OnlineSLAM:
         self.num_nodes += 2 * n
         self.num_edges += n_scale + n
 
+    def _insert_keyframe(self, i, js, conf_host, keep, batch):
+        """connect_view_i_j (slam.py:191-241) after the gate, for a registered view i: the reject and loop-closure
+        messages, loop_related_views, and the kept edges into the graph (_add_keyframe)."""
+        kept = set(keep)
+        for k, j in enumerate(js):
+            names = f"(view {i} [{self.view_names[i]}] -- view {j} [{self.view_names[j]}])"
+            if k not in kept:
+                if self.verbose:
+                    _msg("[EdgeReject] ", f"Rejecting edge {names} with conf {conf_host[k]:.3f}")
+            elif i - j > self.neighbor_edge_num and self.verbose:  # slam.py:199-203
+                _msg("[LoopClosure] ", f"Adding loop closure edge {names} with conf {conf_host[k]:.3f}")
+                self.loop_related_views.add(i)
+                self.loop_related_views.add(j)
+        if keep:
+            self._add_keyframe(i, js, keep, batch)
+
+    def _pgo_if_due(self, force_pgo, log_intermediate_results, output_folder):
+        """slam.py:282-297: PGO every pgo_every views or when forced, after logging the trajectory if asked.  Returns
+        whether it ran."""
+        if not (self.view_num % self.pgo_every == 0 or force_pgo):
+            return False
+        if log_intermediate_results:
+            self.save_data_all(f"{output_folder}", save_view_graph=False, traj_name_postfix=f"{self.view_num - 1}",
+                               save_poses=True, save_images=False, save_scales=True, save_depths=False,
+                               save_intrinsics=False, save_confs=False, save_ply=False)
+        opt_start = time.time()
+        self.pose_graph_optimize()
+        self.time_dict["pgo"] += time.time() - opt_start
+        torch.cuda.empty_cache()
+        return True
+
     # ------------------------------------------------------------------------------------------------ step
     def add_view(self, image, image_shape, view_name):
         self.kf.add_view(image, image_shape)
@@ -279,34 +309,12 @@ class OnlineSLAM:
         js = list(range(farthest_neighbor, i)) + [j for j, _ in loop_candi_list[:self.loop_edge_num]]
         if js:
             dec_start = time.time()
-            conf_host, keep, batch = self._regress_keyframe(i, js)  # read-back: the gate
+            res = self._regress_keyframe(i, js)  # read-back: the gate
             self.time_dict["decoder"] += time.time() - dec_start
             self._check_flags()
-            kept = set(keep)
-            for k, j in enumerate(js):
-                names = f"(view {i} [{self.view_names[i]}] -- view {j} [{self.view_names[j]}])"
-                if k not in kept:
-                    if self.verbose:
-                        _msg("[EdgeReject] ", f"Rejecting edge {names} with conf {conf_host[k]:.3f}")
-                elif i - j > self.neighbor_edge_num and self.verbose:  # slam.py:199-203
-                    _msg("[LoopClosure] ", f"Adding loop closure edge {names} with conf {conf_host[k]:.3f}")
-                    self.loop_related_views.add(i)
-                    self.loop_related_views.add(j)
-            if keep:
-                self._add_keyframe(i, js, keep, batch)
+            self._insert_keyframe(i, js, *res)
         self.time_dict["graph_construction"] += time.time() - graph_start
-
-        if self.view_num % self.pgo_every == 0 or force_pgo:
-            if log_intermediate_results:
-                self.save_data_all(f"{output_folder}", save_view_graph=False, traj_name_postfix=f"{self.view_num - 1}",
-                                   save_poses=True, save_images=False, save_scales=True, save_depths=False,
-                                   save_intrinsics=False, save_confs=False, save_ply=False)
-            opt_start = time.time()
-            self.pose_graph_optimize()
-            self.time_dict["pgo"] += time.time() - opt_start
-            torch.cuda.empty_cache()
-            return True
-        return False
+        return self._pgo_if_due(force_pgo, log_intermediate_results, output_folder)
 
     def step_many(self, values, force_pgo=False, log_intermediate_results=False, output_folder=None):
         """[self.step(v, force_pgo=force_pgo and k == len(values) - 1, ...) for k, v in enumerate(values)]: the same
@@ -364,35 +372,12 @@ class OnlineSLAM:
             self.view_names.append(v["view_name"])
             self.view_num += 1
             if js:
-                conf_host, keep, batch = res
-                kept = set(keep)
-                for e, j in enumerate(js):
-                    names = f"(view {i} [{self.view_names[i]}] -- view {j} [{self.view_names[j]}])"
-                    if e not in kept:
-                        if self.verbose:
-                            _msg("[EdgeReject] ", f"Rejecting edge {names} with conf {conf_host[e]:.3f}")
-                    elif i - j > self.neighbor_edge_num and self.verbose:  # slam.py:199-203
-                        _msg("[LoopClosure] ", f"Adding loop closure edge {names} with conf {conf_host[e]:.3f}")
-                        self.loop_related_views.add(i)
-                        self.loop_related_views.add(j)
-                if keep:
-                    self._add_keyframe(i, js, keep, batch)
-                    checked = False
+                self._insert_keyframe(i, js, *res)
+                checked = checked and not res[1]
             self.time_dict["graph_construction"] += time.time() - graph_start
-
-            if self.view_num % self.pgo_every == 0 or (force_pgo and k == n - 1):
-                if log_intermediate_results:
-                    self.save_data_all(f"{output_folder}", save_view_graph=False, traj_name_postfix=f"{self.view_num - 1}",
-                                       save_poses=True, save_images=False, save_scales=True, save_depths=False,
-                                       save_intrinsics=False, save_confs=False, save_ply=False)
-                opt_start = time.time()
-                self.pose_graph_optimize()
-                self.time_dict["pgo"] += time.time() - opt_start
-                torch.cuda.empty_cache()
+            flags.append(self._pgo_if_due(force_pgo and k == n - 1, log_intermediate_results, output_folder))
+            if flags[-1]:
                 checked = self.num_nodes > 0 and self.num_edges > 0
-                flags.append(True)
-            else:
-                flags.append(False)
         if not checked:
             torch.cuda.current_stream().synchronize()
             self._check_flags()
