@@ -38,8 +38,15 @@ int sta_create(StaModel** out);
  * mode -- every bf16 activation is carried as (hi | lo | hi) and every bf16 weight as (hi | hi | lo), so the same
  * wgmma kernels compute a_hi w_hi + a_lo w_hi + a_hi w_lo over K' = 3K (about 17 significant operand bits),
  * and attention runs in fp32 on the CUDA cores.  It exists to check the kernels against the fp32 reference at
- * north_star's tolerance (pointmaps 1e-3, pose 1e-4); ~3x the weight memory, several times slower. */
-enum { STA_PRECISION_BF16 = 0, STA_PRECISION_X3 = 1 };
+ * north_star's tolerance (pointmaps 1e-3, pose 1e-4); ~3x the weight memory, several times slower.
+ * STA_PRECISION_FP8: an opt-in mode that changes the numerics -- the linear layers of the 24 encoder and 12 decoder
+ * blocks (qkv, proj, fc1, fc2; qkv, proj, projq, projk|projv, cross proj, fc1, fc2) run on e4m3 operands with power-of-two
+ * scales, one per row and 128 columns of the activations and one per 128 x 128 block of the weights, each 128-wide
+ * k-block accumulated on its own and folded into fp32 with both scales.  Everything else (patch embedding,
+ * decoder_embed, attention, the DPT head, the pose head) is as in bf16 mode.  The trunk weights take half the bytes.
+ * With random-init weights its outputs move about 6-10x as far from fp32 as bf16's do; how that carries over to the
+ * trained checkpoint or to SLAM accuracy is not measured, so check it on your own data. */
+enum { STA_PRECISION_BF16 = 0, STA_PRECISION_X3 = 1, STA_PRECISION_FP8 = 2 };
 int sta_create_ex(StaModel** out, int precision);
 void sta_destroy(StaModel* m);
 
@@ -115,7 +122,8 @@ int sta_profile_read(StaModel* m, double* ms4, int64_t* counts4, double* flops4)
 
 /* ---- op-level entry points (used by the parity tests; same kernels the model uses) ---- */
 
-enum { STA_EPI_BF16 = 0, STA_EPI_GELU = 1, STA_EPI_F32 = 2, STA_EPI_ROPE = 3, STA_EPI_PIXSHUF = 4, STA_EPI_HEAD = 5 };
+enum { STA_EPI_BF16 = 0, STA_EPI_GELU = 1, STA_EPI_F32 = 2, STA_EPI_ROPE = 3, STA_EPI_PIXSHUF = 4, STA_EPI_HEAD = 5,
+       STA_EPI_GELU_FP8 = 6 };
 
 typedef struct StaGemmDesc {
   int conv3x3;          /* 0: A is [M][lda] bf16;  1: A is NHWC [nimg][H][W][Cin] bf16 (3x3, pad 1, stride 1) */
@@ -148,6 +156,41 @@ typedef struct StaGemmDesc {
 } StaGemmDesc;
 
 int sta_op_gemm(const StaGemmDesc* d, void* stream);
+
+/* The FP8 mode's GEMM (STA_PRECISION_FP8): out = A W^T + bias on e4m3 codes ("fn" format, max 448) with power-of-two
+ * scales: A [M][lda] with a_scale [M][K/128] (one per row and 128 columns), W [N][ldw] with w_scale [N/128][K/128] (one
+ * per 128 x 128 block).  N and K multiples of 128, lda and ldw multiples of 16.  Each 128-wide k-block is accumulated on
+ * its own and folded as acc = fma(blk, a_scale[m][kb] * w_scale[n/128][kb], acc).  Epilogues:
+ *   STA_EPI_F32       out fp32 [M][ldo]; resid NULL (out = ...) or resid == out (out += ..., in place)
+ *   STA_EPI_ROPE      out bf16 [M][ldo], 2-D RoPE on columns [0, rope_cols) with pos [M][2] int32 (y, x)
+ *   STA_EPI_GELU_FP8  out e4m3 [M][ldo] = gelu(.) / s with out_scale [M][N/128] = s, the scales defined as for the inputs
+ * (a group's scale is 2^e with e the smallest integer for which amax <= 448 * 2^e, 1 for an all-zero group). */
+typedef struct StaGemmFp8Desc {
+  int epi;
+  const void* A;
+  int64_t lda;
+  const float* a_scale;
+  const void* W;
+  int64_t ldw;
+  const float* w_scale;
+  int M, N, K;
+  const float* bias;    /* [N] fp32 or NULL */
+  void* out;
+  int64_t ldo;
+  const void* resid;    /* STA_EPI_F32: NULL or out */
+  float* out_scale;     /* STA_EPI_GELU_FP8 */
+  const int32_t* pos;   /* STA_EPI_ROPE */
+  int rope_cols;
+  void* splitk_ws;      /* optional fp32 scratch, as in StaGemmDesc */
+  int64_t splitk_ws_bytes;
+} StaGemmFp8Desc;
+int sta_op_gemm_fp8(const StaGemmFp8Desc* d, void* stream);
+/* The FP8 mode's quantisers: e4m3 codes [rows][C] plus scales [rows][C/128] as for the GEMM's A operand.
+ * sta_op_layernorm_fp8: LayerNorm of fp32 x (C = 768 or 1024) straight to e4m3, optionally a second output with other
+ * affine parameters (g2 / b2 / q2 / s2, or NULL).  sta_op_quant_fp8: bf16 rows -> e4m3 (C a multiple of 128). */
+int sta_op_layernorm_fp8(const float* x, int rows, int C, float eps, const float* g1, const float* b1, void* q1, float* s1,
+                         const float* g2, const float* b2, void* q2, float* s2, void* stream);
+int sta_op_quant_fp8(const void* in_bf16, int64_t rows, int C, void* q, float* s, void* stream);
 
 /* softmax(q k^T * scale) v, head_dim 64.  q/k/v: [batch][n*][ld*] bf16 with head h at columns
  * *_col0 + 64*h; out: [batch][nq][ldo] bf16.  kv sample for query sample b is (b + kv_batch_shift) % batch. */

@@ -11,8 +11,8 @@ from ctypes import POINTER, Structure, c_char_p, c_float, c_int, c_int32, c_int6
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("STA_B200_LIB") or os.path.join(_HERE, "csrc", "libsta_b200.so")  # env override: A/B timing of builds
 
-EPI_BF16, EPI_GELU, EPI_F32, EPI_ROPE, EPI_PIXSHUF, EPI_HEAD = range(6)
-PRECISION_BF16, PRECISION_X3 = 0, 1
+EPI_BF16, EPI_GELU, EPI_F32, EPI_ROPE, EPI_PIXSHUF, EPI_HEAD, EPI_GELU_FP8 = range(7)
+PRECISION_BF16, PRECISION_X3, PRECISION_FP8 = 0, 1, 2
 
 
 class StaGemmDesc(Structure):
@@ -31,6 +31,20 @@ class StaGemmDesc(Structure):
         ("head_w", c_void_p), ("head_b", c_void_p), ("pts3d", c_void_p), ("conf", c_void_p),
         ("splitk_ws", c_void_p), ("splitk_ws_bytes", c_int64),
         ("split_precision", c_int),
+    ]
+
+
+class StaGemmFp8Desc(Structure):
+    _fields_ = [
+        ("epi", c_int),
+        ("A", c_void_p), ("lda", c_int64), ("a_scale", c_void_p),
+        ("W", c_void_p), ("ldw", c_int64), ("w_scale", c_void_p),
+        ("M", c_int), ("N", c_int), ("K", c_int),
+        ("bias", c_void_p),
+        ("out", c_void_p), ("ldo", c_int64),
+        ("resid", c_void_p), ("out_scale", c_void_p),
+        ("pos", c_void_p), ("rope_cols", c_int),
+        ("splitk_ws", c_void_p), ("splitk_ws_bytes", c_int64),
     ]
 
 
@@ -90,6 +104,9 @@ def lib():
     L.sta_profile.argtypes = [vp, i]
     L.sta_profile_read.argtypes = [vp, POINTER(ctypes.c_double), POINTER(c_int64), POINTER(ctypes.c_double)]
     L.sta_op_gemm.argtypes = [POINTER(StaGemmDesc), vp]
+    L.sta_op_gemm_fp8.argtypes = [POINTER(StaGemmFp8Desc), vp]
+    L.sta_op_layernorm_fp8.argtypes = [vp, i, i, c_float, vp, vp, vp, vp, vp, vp, vp, vp, vp]
+    L.sta_op_quant_fp8.argtypes = [vp, i64, i, vp, vp, vp]
     L.sta_op_attention.argtypes = [vp, i64, i, vp, i64, i, vp, i64, i, vp, i64, i, i, i, i, i, c_float, vp]
     L.sta_op_attention_split.argtypes = L.sta_op_attention.argtypes
     L.sta_op_layernorm.argtypes = [vp, i, i, c_float, vp, vp, vp, vp, vp, vp, i, vp]

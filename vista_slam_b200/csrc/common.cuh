@@ -179,6 +179,19 @@ __device__ __forceinline__ void wgmma_m64n128k16_ss(float (&d)[64], uint64_t ade
       : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
       : "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
+// D[64 x 128] (+)= A[64 x 32](smem desc) * B[128 x 32]^T(smem desc), both K-major e4m3 -> fp32 registers.
+__device__ __forceinline__ void wgmma_m64n128k32_e4m3(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t"
+      ".reg .pred p;\n\t"
+      "setp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k32.f32.e4m3.e4m3 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "%64, %65, p, 1, 1;\n\t"
+      "}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(adesc), "l"(bdesc), "r"(accumulate));
+}
 // D[64 x 64] += A[64 x 16](registers, bf16x2) * B[16 x 64](smem desc, MN-major), fp32 registers.
 __device__ __forceinline__ void wgmma_m64n64k16_rs_mn(float (&d)[32], const uint32_t (&a)[4], uint64_t bdesc) {
   asm volatile(
@@ -230,6 +243,24 @@ __device__ __forceinline__ float bf16_hi(uint32_t v) { return __uint_as_float(v 
 __device__ __forceinline__ float bf16_resid(float v) { return v - __bfloat162float(__float2bfloat16_rn(v)); }
 __device__ __forceinline__ uint32_t pack_bf16x2_resid(float lo, float hi) {
   return pack_bf16x2(bf16_resid(lo), bf16_resid(hi));
+}
+
+// FP8 mode (STA_PRECISION_FP8): e4m3 ("fn", max 448) with one power-of-two scale s = 2^e per group, e the smallest
+// integer with amax <= 448 * 2^e (448 = 1.75 * 2^8), read from amax's exponent and mantissa bits.  An all-zero group
+// has s = 1; e >= -126 keeps s and 1 / s normal.  inv = 1 / s exactly, so q * s dequantises exactly.
+__device__ __forceinline__ void fp8_scale(float amax, float& s, float& inv) {
+  const uint32_t b = __float_as_uint(amax);
+  const int E = static_cast<int>((b >> 23) & 0xFFu);
+  int e = 0;
+  if (b != 0) e = (E == 0) ? -126 : max(E - 135 + ((b & 0x7FFFFFu) > 0x600000u ? 1 : 0), -126);
+  s = __uint_as_float(static_cast<uint32_t>(e + 127) << 23);
+  inv = __uint_as_float(static_cast<uint32_t>(127 - e) << 23);
+}
+// two e4m3 codes, round to nearest even, saturating: lo in the low byte
+__device__ __forceinline__ uint16_t cvt_e4m3x2(float lo, float hi) {
+  uint16_t r;
+  asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(r) : "f"(hi), "f"(lo));
+  return r;
 }
 
 __device__ __forceinline__ float ex2_approx(float x) {

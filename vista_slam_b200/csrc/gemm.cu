@@ -48,7 +48,14 @@ static int launch_inst(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUt
 
 int launch_gemm(const GemmLaunch& g, cudaStream_t stream) {
   GemmParams p = g.p;
+  const bool fp8 = g.amode == A_FP8;
   STA_REQUIRE(p.N % 32 == 0, "N must be a multiple of 32");
+  STA_REQUIRE(!fp8 || (p.N % 128 == 0 && p.K % 128 == 0 && p.K > 0 && p.M > 0 && !p.split),
+              "e4m3 operands need N and K multiples of 128");
+  STA_REQUIRE(!fp8 || (p.a_scale != nullptr && p.w_scale != nullptr), "e4m3 operands need their scales");
+  STA_REQUIRE(!fp8 || g.epi == EPI_F32 || g.epi == EPI_ROPE || g.epi == EPI_GELU_FP8,
+              "e4m3 operands: EPI_F32, EPI_ROPE or EPI_GELU_FP8");
+  STA_REQUIRE(g.epi != EPI_GELU_FP8 || (fp8 && p.out_scale != nullptr), "EPI_GELU_FP8 needs e4m3 operands and out_scale");
   STA_REQUIRE(!p.split || g.epi == EPI_F32 || g.epi == EPI_HEAD || g.epi == EPI_PIXSHUF || p.ldo >= 3LL * p.N,
               "split-precision bf16 outputs need ldo >= 3N");
   STA_REQUIRE(g.A != nullptr && g.Wt != nullptr, "null operand");
@@ -61,8 +68,8 @@ int launch_gemm(const GemmLaunch& g, cudaStream_t stream) {
   // TMA-store epilogue (epilogue_tile_tma) for the linear layers: bf16 / GELU / RoPE outputs without skip
   // tensors, fp32 outputs that either have no residual or accumulate in place (out += ..., bulk reduce-add).
   // GELU and RoPE have no other epilogue.
-  const int esz = (g.epi == EPI_F32) ? 4 : 2;
-  bool tma = p.N % bn == 0 && g.amode == A_LINEAR && p.out != nullptr && p.out2 == nullptr &&
+  const int esz = (g.epi == EPI_F32) ? 4 : (g.epi == EPI_GELU_FP8) ? 1 : 2;
+  bool tma = p.N % bn == 0 && (g.amode == A_LINEAR || fp8) && p.out != nullptr && p.out2 == nullptr &&
              (reinterpret_cast<uintptr_t>(p.out) & 15) == 0 && (p.ldo * esz) % 16 == 0;
   p.c_reduce = 0;
   if (g.epi == EPI_BF16) {
@@ -70,12 +77,14 @@ int launch_gemm(const GemmLaunch& g, cudaStream_t stream) {
   } else if (g.epi == EPI_F32) {
     tma = tma && p.rowmap_n == 0 && (p.resid == nullptr || p.resid == p.out);
     p.c_reduce = (p.resid != nullptr) ? 1 : 0;
-  } else if (g.epi == EPI_GELU || g.epi == EPI_ROPE) {
+  } else if (g.epi == EPI_GELU || g.epi == EPI_ROPE || g.epi == EPI_GELU_FP8) {
     STA_REQUIRE(tma, "GELU / RoPE epilogues need a linear layer with N % 128 == 0, a 16-byte aligned output and row "
                      "stride, and no out2");
   } else {
     tma = false;
   }
+  STA_REQUIRE(!fp8 || tma, "e4m3 operands need the TMA-store epilogue (16-byte aligned output, fp32 residual in place)");
+  const int bk = fp8 ? 128 : 64;  // k-block: one 128-byte operand row
 
   // Small problems (one keyframe / a few edges in SLAM mode) are bound by streaming the weights through too few SMs:
   // the fp32 residual-stream layers (out += A W^T + b) with fewer tiles than SMs split K across CTAs: every split
@@ -83,7 +92,7 @@ int launch_gemm(const GemmLaunch& g, cudaStream_t stream) {
   // reduce-adds racing).
   int ksplit = 1;
   if (tma && g.epi == EPI_F32 && g.splitk_ws != nullptr) {
-    const int tiles = ((p.M + 127) / 128) * (p.N / bn), nkb = (p.K + 63) / 64;
+    const int tiles = ((p.M + 127) / 128) * (p.N / bn), nkb = (p.K + bk - 1) / bk;
     if (tiles < num_sms()) {
       int ks = num_sms() / tiles;
       if (ks > 8) ks = 8;
@@ -107,19 +116,21 @@ int launch_gemm(const GemmLaunch& g, cudaStream_t stream) {
     uint32_t box[4] = {64, (uint32_t)kHaloPitch, 18u, 1};
     if (make_tmap_bf16(&tmA, g.A, 4, dims, strides, box)) return 1;
   } else {
-    STA_REQUIRE(g.lda % 8 == 0, "lda must be a multiple of 8 elements (16 bytes)");
+    const int oes = fp8 ? 1 : 2;  // operand bytes
+    STA_REQUIRE(g.lda * oes % 16 == 0, "lda must be a multiple of 16 bytes");
     m_tiles = (p.M + 127) / 128;
     uint64_t dims[2] = {(uint64_t)p.K, (uint64_t)p.M};
-    uint64_t strides[1] = {(uint64_t)g.lda * 2};
-    uint32_t box[2] = {64, 128};
-    if (make_tmap_bf16(&tmA, g.A, 2, dims, strides, box)) return 1;
+    uint64_t strides[1] = {(uint64_t)g.lda * oes};
+    uint32_t box[2] = {(uint32_t)bk, 128};
+    if (make_tmap(&tmA, g.A, fp8 ? 2 : 0, 2, dims, strides, box)) return 1;
   }
   {
-    STA_REQUIRE(g.ldw % 8 == 0, "ldw must be a multiple of 8 elements (16 bytes)");
+    const int oes = fp8 ? 1 : 2;
+    STA_REQUIRE(g.ldw * oes % 16 == 0, "ldw must be a multiple of 16 bytes");
     uint64_t dims[2] = {(uint64_t)p.K, (uint64_t)p.N};
-    uint64_t strides[1] = {(uint64_t)g.ldw * 2};
-    uint32_t box[2] = {64, (uint32_t)bn};
-    if (make_tmap_bf16(&tmB, g.Wt, 2, dims, strides, box)) return 1;
+    uint64_t strides[1] = {(uint64_t)g.ldw * oes};
+    uint32_t box[2] = {(uint32_t)bk, (uint32_t)bn};
+    if (make_tmap(&tmB, g.Wt, fp8 ? 2 : 0, 2, dims, strides, box)) return 1;
   }
   const int n_tiles = (p.N + bn - 1) / bn;
   const int num_tiles = m_tiles * n_tiles * ksplit;
@@ -146,7 +157,7 @@ int launch_gemm(const GemmLaunch& g, cudaStream_t stream) {
     uint64_t dims[2] = {(uint64_t)p.N * ((p.split && esz == 2) ? 3 : 1), (uint64_t)p.M};
     uint64_t strides[1] = {(uint64_t)p.ldo * esz};
     uint32_t box[2] = {(uint32_t)(128 / esz), 16};  // one 16-row group of a warp's accumulator fragments
-    if (make_tmap(&tmC, p.out, esz == 4, 2, dims, strides, box)) return 1;
+    if (make_tmap(&tmC, p.out, esz == 4 ? 1 : esz == 1 ? 2 : 0, 2, dims, strides, box)) return 1;
   }
   STA_REQUIRE(tma || ksplit == 1, "split-K needs the TMA epilogue");
 
@@ -163,6 +174,9 @@ int launch_gemm(const GemmLaunch& g, cudaStream_t stream) {
   STA_GEMM_CASE(A_LINEAR, EPI_PIXSHUF, false)
   STA_GEMM_CASE(A_CONV3, EPI_BF16, false)
   STA_GEMM_CASE(A_CONV3, EPI_HEAD, false)
+  STA_GEMM_CASE(A_FP8, EPI_F32, true)
+  STA_GEMM_CASE(A_FP8, EPI_ROPE, true)
+  STA_GEMM_CASE(A_FP8, EPI_GELU_FP8, true)
 #undef STA_GEMM_CASE
   if (rc == 0 && ksplit > 1) {
     const long long total = static_cast<long long>(p.M) * (p.N / 4);

@@ -23,7 +23,12 @@ namespace sta {
 //          a tap is a row-shifted view of the staged tile (tile 16 rows x 8 pixels, descriptor base offset = the tap's
 //          shift).  Shared-memory write traffic of the A operand is 22.5 KB per channel chunk instead of 9 x 16 KB with one
 //          box per tap; the N = 128 head convolutions are bound by exactly that traffic.
-enum AMode : int { A_LINEAR = 0, A_CONV3 = 1 };
+// A_FP8:   linear layer with e4m3 operands (A [M][K] and W [N][K] bytes, K contiguous) and power-of-two block scales: one
+//          per row and 128 columns of A (a_scale [M][K / 128]) and one per 128 x 128 block of W (w_scale [N / 128][K / 128]).
+//          A 128-byte row holds 128 e4m3 values, so the TMA boxes, the swizzle and the ring are those of the bf16 kernel
+//          with BK = 128.  Each 128-wide k-block accumulates in a fresh wgmma accumulator (four m64n128k32 MMAs per
+//          64-row half) that is folded into the fp32 tile as acc = fma(blk, a_scale[row] * w_scale, acc).
+enum AMode : int { A_LINEAR = 0, A_CONV3 = 1, A_FP8 = 2 };
 enum Epi : int {
   EPI_BF16 = 0,     // out_bf16 = [relu](acc + bias [+ resid_bf16] [+ resid2_bf16]); optional relu copy in out2
   EPI_GELU = 1,     // out_bf16 = gelu_erf(acc + bias)
@@ -31,6 +36,7 @@ enum Epi : int {
   EPI_ROPE = 3,     // out_bf16 = rope2d(acc + bias) on columns < rope_cols, plain on the rest
   EPI_PIXSHUF = 4,  // ConvTranspose2d(k = stride): scatter to the k x k sub-pixels, NHWC bf16
   EPI_HEAD = 5,     // relu(acc + bias) -> 1x1 conv (128 -> 4) -> pointmap/confidence post-process (fp32 out)
+  EPI_GELU_FP8 = 6, // out_e4m3 = gelu_erf(acc + bias) / s, out_scale[row][n_tile] = s (one power-of-two scale per 128 columns)
 };
 
 struct GemmParams {
@@ -68,6 +74,10 @@ struct GemmParams {
   // (K here is the physical 3K); bf16 outputs / bf16 skip tensors use the (hi | lo | hi) row layout with logical
   // width N (ldo = 3N).  fp32 outputs are unaffected.
   int split;
+  // A_FP8 operand scales (see AMode) and the EPI_GELU_FP8 output scales [M][N / 128]
+  const float* a_scale;
+  const float* w_scale;
+  float* out_scale;
 };
 
 // TMA = true: the epilogue writes through per-warp swizzled boxes + TMA tensor stores (epilogue_tile_tma), else the
@@ -79,11 +89,13 @@ constexpr int kRopeLd = 36;  // floats per staged sin/cos table row (32 + 4 pad:
 template <int AMODE, int EPI, bool TMA>
 struct GemmCfg {
   static constexpr bool CONV = (AMODE == A_CONV3);
+  static constexpr bool FP8 = (AMODE == A_FP8);
   static constexpr int BM = 128;
   static constexpr int BN = 128;  // two m64n128k16 wgmmas per k16 step cover a consumer warpgroup's whole tile
-  static constexpr int BK = 64;
-  static constexpr uint32_t A_BYTES = BM * BK * 2;
-  static constexpr uint32_t B_BYTES = BN * BK * 2;
+  static constexpr int ESZ = FP8 ? 1 : 2;  // operand bytes
+  static constexpr int BK = 128 / ESZ;     // one 128-byte K-major row per k-block
+  static constexpr uint32_t A_BYTES = BM * BK * ESZ;
+  static constexpr uint32_t B_BYTES = BN * BK * ESZ;
   static constexpr uint32_t BAR_BYTES = 256;
   static constexpr int EPI_WARPS = 8;  // the two consumer warpgroups
   // Register split (setmaxnreg): the producer warpgroup only issues TMA loads; a consumer thread holds a 128 x 128 fp32
@@ -440,7 +452,7 @@ __device__ __forceinline__ void epilogue_tile_tma(const GemmParams& p, const CUt
       acc[h][4 * j] += b.x; acc[h][4 * j + 1] += b.y; acc[h][4 * j + 2] += b.x; acc[h][4 * j + 3] += b.y;
     }
   }
-  if constexpr (EPI == EPI_GELU) {
+  if constexpr (EPI == EPI_GELU || EPI == EPI_GELU_FP8) {
 #pragma unroll
     for (int h = 0; h < 2; ++h)
 #pragma unroll
@@ -536,6 +548,37 @@ __device__ __forceinline__ void epilogue_tile_tma(const GemmParams& p, const CUt
       tma_store_commit();
     }
   };
+  if constexpr (EPI == EPI_GELU_FP8) {
+    // One 16-row x 128-byte box per 64-row half holds the tile's 128 e4m3 columns.  A row's 128 columns sit in one quad,
+    // so its amax takes two shuffles; lane t = 0 of the quad writes the row's scale.  Column 8 j + 2 t of box row R is
+    // byte 8 (j & 1) + 2 t of 16-byte chunk (j >> 1) ^ (R & 7).
+    const int nsb = p.N / 128;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const uint32_t box = next_box();
+#pragma unroll
+      for (int half = 0; half < 2; ++half) {
+        float am = 0.0f;
+#pragma unroll
+        for (int j = 0; j < 16; ++j)
+          am = fmaxf(am, fmaxf(fabsf(acc[h][4 * j + 2 * half]), fabsf(acc[h][4 * j + 2 * half + 1])));
+        am = fmaxf(am, __shfl_xor_sync(0xFFFFFFFFu, am, 1));
+        am = fmaxf(am, __shfl_xor_sync(0xFFFFFFFFu, am, 2));
+        float s, inv;
+        fp8_scale(am, s, inv);
+        const int row = row0 + 64 * h + 8 * half + r;
+        if (t == 0 && row < p.M) p.out_scale[static_cast<long long>(row) * nsb + n_tile] = s;
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+          const uint16_t q = cvt_e4m3x2(acc[h][4 * j + 2 * half] * inv, acc[h][4 * j + 2 * half + 1] * inv);
+          asm volatile("st.shared.b16 [%0], %1;" ::"r"(box + (8 * half + r) * 128 + (((j >> 1) ^ sx) << 4) + 8 * (j & 1) + 2 * t),
+                       "h"(q)
+                       : "memory");
+        }
+      }
+      issue(box, col0, row0 + 64 * h + row_off, false);
+    }
+  } else {
 #pragma unroll
   for (int c = 0; c < NCH; ++c) {
 #pragma unroll
@@ -577,6 +620,7 @@ __device__ __forceinline__ void epilogue_tile_tma(const GemmParams& p, const CUt
       }
     }
   }
+  }
 }
 
 template <int AMODE, int EPI, bool TMA>
@@ -585,8 +629,10 @@ gemm_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                const __grid_constant__ CUtensorMap tmC, const GemmParams p) {
   using Cfg = GemmCfg<AMODE, EPI, TMA>;
   constexpr bool CONV = Cfg::CONV;
-  static_assert(!TMA || (AMODE == A_LINEAR && (EPI == EPI_BF16 || EPI == EPI_GELU || EPI == EPI_F32 || EPI == EPI_ROPE)),
+  static_assert(!TMA || (AMODE == A_LINEAR && (EPI == EPI_BF16 || EPI == EPI_GELU || EPI == EPI_F32 || EPI == EPI_ROPE)) ||
+                    (AMODE == A_FP8 && (EPI == EPI_F32 || EPI == EPI_ROPE || EPI == EPI_GELU_FP8)),
                 "TMA-store epilogue: linear layers only");
+  static_assert(AMODE != A_FP8 || TMA, "e4m3 operands: TMA-store epilogues only");
   static_assert(TMA || EPI == EPI_BF16 || EPI == EPI_F32 || EPI == EPI_PIXSHUF || EPI == EPI_HEAD,
                 "GELU and RoPE have the TMA-store epilogue only");
   constexpr int BN = Cfg::BN;
@@ -616,7 +662,7 @@ gemm_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   const int ksplit = TMA ? p.ksplit : 1;
   const int num_tiles = m_tiles * n_tiles * ksplit;  // work items (m, n, ks), ks fastest
   const int cpb = CONV ? (p.Cin / 64) : 1;  // 64-channel chunks per filter tap
-  const int nkb = CONV ? 9 * cpb : (p.K + 63) / 64;
+  const int nkb = CONV ? 9 * cpb : (p.K + Cfg::BK - 1) / Cfg::BK;
 
   if (threadIdx.x == 0) {
     if ((smem_u32(smem) & 1023u) != 0) device_fatal("dynamic shared memory is not 1024-byte aligned");
@@ -689,8 +735,8 @@ gemm_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
           for (int kb = kb0; kb < kb1; ++kb) {
             mbar_wait(&empty[stage], phase ^ 1);
             mbar_arrive_expect_tx(&full[stage], A_BYTES + B_BYTES);
-            tma_load_2d(sA + stage * A_BYTES, &tmA, &full[stage], kb * 64, m_tile * 128);
-            tma_load_2d(sB + stage * B_BYTES, &tmB, &full[stage], kb * 64, b_row0);
+            tma_load_2d(sA + stage * A_BYTES, &tmA, &full[stage], kb * Cfg::BK, m_tile * 128);
+            tma_load_2d(sB + stage * B_BYTES, &tmB, &full[stage], kb * Cfg::BK, b_row0);
             if (++stage == STAGES) { stage = 0; phase ^= 1; }
           }
         }
@@ -753,7 +799,52 @@ gemm_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       auto hand_over = [&]() {
         if (tile + static_cast<int>(gridDim.x) < num_tiles) named_bar_arrive(kOrderBar + (wg ^ 1), 256);
       };
-      if constexpr (CONV) {
+      if constexpr (Cfg::FP8) {
+        // The two 64-row halves of a k-block run one after the other through one 64-register block accumulator (beside
+        // the 128 tile accumulators); the scales are loaded before the stage wait and used after the MMAs.  The turn
+        // passes once the wait on the tile's last stage is done (every stage of the tile is then filled, which is what
+        // keeps the other warpgroup's parity waits within one ring round), so the other warpgroup's MMAs overlap this
+        // one's last k-block and folds.
+        const int nks = p.K / 128;
+        const int r = lane >> 2;
+        const int rbase = m_tile * 128 + 16 * wq + r;  // + 64 h + 8 half
+        for (int kb = kb0; kb < kb1; ++kb) {
+          float as[2][2];
+#pragma unroll
+          for (int h = 0; h < 2; ++h)
+#pragma unroll
+            for (int half = 0; half < 2; ++half) {
+              const int row = rbase + 64 * h + 8 * half;
+              as[h][half] = row < p.M ? __ldg(p.a_scale + static_cast<long long>(row) * nks + kb) : 0.0f;
+            }
+          const float wsc = __ldg(p.w_scale + n_tile * nks + kb);
+          mbar_wait(&full[stage], phase);
+          if (kb == kb1 - 1) hand_over();
+          const uint32_t a = smem_u32(sA + stage * A_BYTES);
+          const uint64_t bdesc = make_smem_desc_sw128(smem_u32(sB + stage * B_BYTES));
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            float blk[64];
+            const uint64_t adesc = make_smem_desc_sw128(a + h * 64 * 128);
+            wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < 4; ++k) wgmma_m64n128k32_e4m3(blk, adesc + 2 * k, bdesc + 2 * k, k > 0 ? 1u : 0u);
+            wgmma_commit();
+            wgmma_wait<0>();
+            fence_regs(blk);
+            const float s0 = as[h][0] * wsc, s1 = as[h][1] * wsc;
+#pragma unroll
+            for (int j = 0; j < 16; ++j) {
+              acc[h][4 * j] = fmaf(blk[4 * j], s0, acc[h][4 * j]);
+              acc[h][4 * j + 1] = fmaf(blk[4 * j + 1], s0, acc[h][4 * j + 1]);
+              acc[h][4 * j + 2] = fmaf(blk[4 * j + 2], s1, acc[h][4 * j + 2]);
+              acc[h][4 * j + 3] = fmaf(blk[4 * j + 3], s1, acc[h][4 * j + 3]);
+            }
+          }
+          if (lane == 0) mbar_arrive(&empty[stage]);
+          if (++stage == STAGES) { stage = 0; phase ^= 1; }
+        }
+      } else if constexpr (CONV) {
         for (int cc = 0; cc < cpb; ++cc) {
           mbar_wait(&hfull[hstage], hphase);
           // output pixel (y, x) of the 16 x 8 tile reads halo pixel (y + kh, x + kw); halo rows are kHaloPitch pixels.

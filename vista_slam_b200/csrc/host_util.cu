@@ -33,7 +33,7 @@ int make_tmap_bf16(CUtensorMap* out, const void* base, int rank, const uint64_t*
   return make_tmap(out, base, /*is_f32=*/0, rank, dims, strides_bytes, box);
 }
 
-int make_tmap(CUtensorMap* out, const void* base, int is_f32, int rank, const uint64_t* dims,
+int make_tmap(CUtensorMap* out, const void* base, int kind, int rank, const uint64_t* dims,
               const uint64_t* strides_bytes, const uint32_t* box) {
   EncodeTiledFn fn = get_encode_fn();
   if (!fn) {
@@ -50,7 +50,10 @@ int make_tmap(CUtensorMap* out, const void* base, int is_f32, int rank, const ui
     estr[i] = 1;
     if (i + 1 < rank) gstr[i] = strides_bytes[i];
   }
-  CUresult r = fn(out, is_f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, (cuuint32_t)rank, const_cast<void*>(base), gdim, gstr, bx,
+  const CUtensorMapDataType dt = kind == 1   ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32
+                                : kind == 2 ? CU_TENSOR_MAP_DATA_TYPE_UINT8
+                                            : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
+  CUresult r = fn(out, dt, (cuuint32_t)rank, const_cast<void*>(base), gdim, gstr, bx,
                   estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {

@@ -45,8 +45,8 @@ const char* get_last_error();
 int make_tmap_bf16(CUtensorMap* out, const void* base, int rank, const uint64_t* dims,
                    const uint64_t* strides_bytes, const uint32_t* box);
 
-// Same for bf16 (is_f32 = 0) or fp32 (is_f32 = 1) elements.
-int make_tmap(CUtensorMap* out, const void* base, int is_f32, int rank, const uint64_t* dims,
+// Same for bf16 (kind = 0), fp32 (kind = 1) or 8-bit (kind = 2: e4m3 codes) elements.
+int make_tmap(CUtensorMap* out, const void* base, int kind, int rank, const uint64_t* dims,
               const uint64_t* strides_bytes, const uint32_t* box);
 
 int num_sms();  // of the CURRENT device (cached per device)

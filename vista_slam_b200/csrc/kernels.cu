@@ -22,6 +22,30 @@ namespace sta {
 // the first row of every `drop_first_of` rows (pose token) from the output.
 // Reference: nn.LayerNorm(eps=1e-6) sta_model.py:43.
 // ---------------------------------------------------------------------------
+// the row's values (v[i] = columns 4 (lane + 32 i) .. + 3), its mean and 1 / sqrt(var + eps)
+template <int V>
+__device__ __forceinline__ void ln_row_stats(const float4* xp, float eps, float4 (&v)[V], float& mean, float& rstd) {
+  constexpr int C = 128 * V;
+  float sum = 0.f;
+#pragma unroll
+  for (int i = 0; i < V; ++i) {
+    v[i] = xp[(threadIdx.x & 31) + 32 * i];
+    sum += (v[i].x + v[i].y) + (v[i].z + v[i].w);
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
+  mean = sum * (1.0f / C);
+  float sq = 0.f;
+#pragma unroll
+  for (int i = 0; i < V; ++i) {
+    float a = v[i].x - mean, b = v[i].y - mean, c = v[i].z - mean, d = v[i].w - mean;
+    sq += (a * a + b * b) + (c * c + d * d);
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) sq += __shfl_xor_sync(0xffffffffu, sq, o);
+  rstd = rsqrtf(sq * (1.0f / C) + eps);
+}
+
 template <int C>
 __global__ void __launch_bounds__(256)
 layernorm_kernel(const float* __restrict__ x, int rows, float eps, const float* __restrict__ g1,
@@ -45,26 +69,9 @@ layernorm_kernel(const float* __restrict__ x, int rows, float eps, const float* 
     if (t == 0) return;
     orow = static_cast<long long>(s) * (drop_first_of - 1) + (t - 1);
   }
-  const float4* xp = reinterpret_cast<const float4*>(x + static_cast<long long>(row) * C);
   float4 v[V];
-  float sum = 0.f;
-#pragma unroll
-  for (int i = 0; i < V; ++i) {
-    v[i] = xp[lane + 32 * i];
-    sum += (v[i].x + v[i].y) + (v[i].z + v[i].w);
-  }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
-  const float mean = sum * (1.0f / C);
-  float sq = 0.f;
-#pragma unroll
-  for (int i = 0; i < V; ++i) {
-    float a = v[i].x - mean, b = v[i].y - mean, c = v[i].z - mean, d = v[i].w - mean;
-    sq += (a * a + b * b) + (c * c + d * d);
-  }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) sq += __shfl_xor_sync(0xffffffffu, sq, o);
-  const float rstd = rsqrtf(sq * (1.0f / C) + eps);
+  float mean, rstd;
+  ln_row_stats<V>(reinterpret_cast<const float4*>(x + static_cast<long long>(row) * C), eps, v, mean, rstd);
 #pragma unroll
   for (int i = 0; i < V; ++i) {
     const int c4 = lane + 32 * i;
@@ -113,6 +120,102 @@ int launch_layernorm(const float* x, int rows, int C, float eps, const float* g1
     set_last_error("layernorm: C must be 768 or 1024");
     return 2;
   }
+  STA_CHECK_CUDA(cudaGetLastError());
+  return 0;
+}
+
+// ---------------------------------------------------------------------------
+// FP8 mode (common.cuh fp8_scale): e4m3 rows [rows][C] with one power-of-two scale per row and 128 columns
+// ([rows][C / 128] fp32).  A warp's 32 lanes hold one 128-column group, 4 values each.
+// ---------------------------------------------------------------------------
+__device__ __forceinline__ void quant_group_store(float y0, float y1, float y2, float y3, uint32_t* q, float* s) {
+  float am = fmaxf(fmaxf(fabsf(y0), fabsf(y1)), fmaxf(fabsf(y2), fabsf(y3)));
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) am = fmaxf(am, __shfl_xor_sync(0xffffffffu, am, o));
+  float sc, inv;
+  fp8_scale(am, sc, inv);
+  *q = static_cast<uint32_t>(cvt_e4m3x2(y0 * inv, y1 * inv)) | (static_cast<uint32_t>(cvt_e4m3x2(y2 * inv, y3 * inv)) << 16);
+  if ((threadIdx.x & 31) == 0) *s = sc;
+}
+
+// LayerNorm straight to e4m3 (the FP8 mode's trunk linears read it), statistics as layernorm_kernel; optional second
+// output with other affine parameters (decoder norm1 / norm_y).
+template <int C>
+__global__ void __launch_bounds__(256)
+layernorm_fp8_kernel(const float* __restrict__ x, int rows, float eps, const float* __restrict__ g1,
+                     const float* __restrict__ b1, uint8_t* __restrict__ q1, float* __restrict__ s1,
+                     const float* __restrict__ g2, const float* __restrict__ b2, uint8_t* __restrict__ q2,
+                     float* __restrict__ s2) {
+  pdl_wait();
+  pdl_launch_dependents();
+  constexpr int V = C / 128;
+  const int blk = static_cast<int>(gridDim.x) - 1 - static_cast<int>(blockIdx.x);  // rows from the end: layernorm_kernel
+  const int row = blk * 8 + (threadIdx.x >> 5);
+  const int lane = threadIdx.x & 31;
+  if (row >= rows) return;
+  float4 v[V];
+  float mean, rstd;
+  ln_row_stats<V>(reinterpret_cast<const float4*>(x + static_cast<long long>(row) * C), eps, v, mean, rstd);
+#pragma unroll
+  for (int i = 0; i < V; ++i) {
+    const int c4 = lane + 32 * i;
+    const float n0 = (v[i].x - mean) * rstd, n1 = (v[i].y - mean) * rstd, n2 = (v[i].z - mean) * rstd,
+                n3 = (v[i].w - mean) * rstd;
+    {
+      const float4 g = __ldg(reinterpret_cast<const float4*>(g1) + c4);
+      const float4 bb = __ldg(reinterpret_cast<const float4*>(b1) + c4);
+      quant_group_store(n0 * g.x + bb.x, n1 * g.y + bb.y, n2 * g.z + bb.z, n3 * g.w + bb.w,
+                        reinterpret_cast<uint32_t*>(q1 + static_cast<long long>(row) * C) + c4, s1 + static_cast<long long>(row) * V + i);
+    }
+    if (q2) {
+      const float4 g = __ldg(reinterpret_cast<const float4*>(g2) + c4);
+      const float4 bb = __ldg(reinterpret_cast<const float4*>(b2) + c4);
+      quant_group_store(n0 * g.x + bb.x, n1 * g.y + bb.y, n2 * g.z + bb.z, n3 * g.w + bb.w,
+                        reinterpret_cast<uint32_t*>(q2 + static_cast<long long>(row) * C) + c4, s2 + static_cast<long long>(row) * V + i);
+    }
+  }
+}
+
+int launch_layernorm_fp8(const float* x, int rows, int C, float eps, const float* g1, const float* b1, uint8_t* q1, float* s1,
+                         const float* g2, const float* b2, uint8_t* q2, float* s2, cudaStream_t stream) {
+  if (rows <= 0) return 0;
+  STA_REQUIRE(x && g1 && b1 && q1 && s1 && (!q2 || (g2 && b2 && s2)), "layernorm_fp8: null pointer");
+  const int grid = (rows + 7) / 8;
+  if (C == 1024)
+    STA_CHECK_CUDA(launch_pdl(layernorm_fp8_kernel<1024>, dim3(grid), dim3(256), 0, stream, 1, x, rows, eps, g1, b1, q1, s1, g2,
+                              b2, q2, s2));
+  else if (C == 768)
+    STA_CHECK_CUDA(launch_pdl(layernorm_fp8_kernel<768>, dim3(grid), dim3(256), 0, stream, 1, x, rows, eps, g1, b1, q1, s1, g2,
+                              b2, q2, s2));
+  else {
+    set_last_error("layernorm_fp8: C must be 768 or 1024");
+    return 2;
+  }
+  STA_CHECK_CUDA(cudaGetLastError());
+  return 0;
+}
+
+// bf16 [rows][C] -> e4m3 + scales (the attention output ahead of the FP8 mode's proj GEMMs): one warp per row and
+// 128-column group
+__global__ void __launch_bounds__(256)
+quant_fp8_kernel(const __nv_bfloat16* __restrict__ in, long long groups, uint8_t* __restrict__ q,
+                 float* __restrict__ s) {
+  pdl_wait();
+  pdl_launch_dependents();
+  const long long gi = static_cast<long long>(blockIdx.x) * 8 + (threadIdx.x >> 5);
+  if (gi >= groups) return;
+  const int lane = threadIdx.x & 31;
+  const uint2 u = reinterpret_cast<const uint2*>(in + gi * 128)[lane];
+  quant_group_store(bf16_lo(u.x), bf16_hi(u.x), bf16_lo(u.y), bf16_hi(u.y), reinterpret_cast<uint32_t*>(q + gi * 128) + lane,
+                    s + gi);
+}
+
+int launch_quant_fp8(const bf16* in, long long rows, int C, uint8_t* q, float* s, cudaStream_t stream) {
+  if (rows <= 0) return 0;
+  STA_REQUIRE(C > 0 && C % 128 == 0, "quant_fp8: C must be a positive multiple of 128");
+  STA_REQUIRE(in && q && s, "quant_fp8: null pointer");
+  const long long groups = rows * (C / 128);
+  STA_CHECK_CUDA(launch_pdl(quant_fp8_kernel, dim3(static_cast<unsigned>((groups + 7) / 8)), dim3(256), 0, stream, 1, in, groups, q, s));
   STA_CHECK_CUDA(cudaGetLastError());
   return 0;
 }

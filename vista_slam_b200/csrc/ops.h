@@ -15,11 +15,11 @@ typedef __nv_bfloat16 bf16;
 struct GemmLaunch {
   int amode = A_LINEAR;
   int epi = EPI_BF16;
-  // A operand.  A_LINEAR: [M][lda] bf16 (K contiguous).  A_CONV3: NHWC [nimg][H][W][Cin] bf16.
-  const bf16* A = nullptr;
+  // A operand.  A_LINEAR: [M][lda] bf16 (K contiguous).  A_CONV3: NHWC [nimg][H][W][Cin] bf16.  A_FP8: [M][lda] e4m3.
+  const void* A = nullptr;
   long long lda = 0;
-  // weights: [N][ldw] bf16, K contiguous (K = 9*Cin ordered (kh, kw, cin) for A_CONV3)
-  const bf16* Wt = nullptr;
+  // weights: [N][ldw] bf16 (A_FP8: e4m3), K contiguous (K = 9*Cin ordered (kh, kw, cin) for A_CONV3)
+  const void* Wt = nullptr;
   long long ldw = 0;
   GemmParams p = {};
   // optional fp32 scratch for split-K partials (small, weight-streaming-bound problems); unused if null
@@ -48,6 +48,10 @@ int launch_attention(const AttnLaunch& a, cudaStream_t stream);
 // ---- bandwidth-bound kernels (kernels.cu) ----
 int launch_layernorm(const float* x, int rows, int C, float eps, const float* g1, const float* b1, bf16* out1,
                      const float* g2, const float* b2, bf16* out2, int drop_first_of, cudaStream_t stream, int split = 0);
+// FP8 mode: e4m3 rows plus one power-of-two scale per row and 128 columns (common.cuh fp8_scale)
+int launch_layernorm_fp8(const float* x, int rows, int C, float eps, const float* g1, const float* b1, uint8_t* q1, float* s1,
+                         const float* g2, const float* b2, uint8_t* q2, float* s2, cudaStream_t stream);
+int launch_quant_fp8(const bf16* in, long long rows, int C, uint8_t* q, float* s, cudaStream_t stream);
 int launch_patch_im2col(const void* img, int img_is_bf16, int B, int H, int W, bf16* out, cudaStream_t stream, int split = 0);
 int launch_make_positions(int* pos, int B, int h, int w, int with_pose_token, cudaStream_t stream);
 int launch_pos_from_int64(const long long* pos64, int rows, int* pos32, cudaStream_t stream);

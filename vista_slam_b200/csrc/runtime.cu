@@ -58,6 +58,27 @@ __global__ void pack_convT_kernel(const float* __restrict__ src, __nv_bfloat16* 
   put_weight(dst + (static_cast<long long>(kk) * Cout_pad + co) * (split ? 3 * Cin_pad : Cin_pad) + ci, src[idx], split,
              Cin_pad);
 }
+// FP8 mode: one 128 x 128 block (blockIdx.y, blockIdx.x) of a trunk weight [rows][cols] fp32 -> e4m3 codes (row stride
+// ldd) and the block's power-of-two scale at sdst[blockIdx.y * sld + blockIdx.x] (common.cuh fp8_scale)
+__global__ void __launch_bounds__(256)
+pack_linear_fp8_kernel(const float* __restrict__ src, int cols, uint8_t* __restrict__ dst, long long ldd, float* __restrict__ sdst,
+                       int sld) {
+  __shared__ float red[8];
+  const int r = blockIdx.y * 128 + (threadIdx.x >> 1), c0 = blockIdx.x * 128 + (threadIdx.x & 1) * 64;
+  const float* sp = src + static_cast<long long>(r) * cols + c0;
+  float am = 0.f;
+  for (int c = 0; c < 64; ++c) am = fmaxf(am, fabsf(sp[c]));
+  for (int o = 16; o > 0; o >>= 1) am = fmaxf(am, __shfl_xor_sync(0xffffffffu, am, o));
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = am;
+  __syncthreads();
+  am = red[0];
+  for (int w = 1; w < 8; ++w) am = fmaxf(am, red[w]);
+  float s, inv;
+  fp8_scale(am, s, inv);
+  uint16_t* dp = reinterpret_cast<uint16_t*>(dst + static_cast<long long>(r) * ldd + c0);
+  for (int c = 0; c < 64; c += 2) dp[c / 2] = cvt_e4m3x2(sp[c] * inv, sp[c + 1] * inv);
+  if (threadIdx.x == 0) sdst[blockIdx.y * sld + blockIdx.x] = s;
+}
 // [rows][cols] fp32 -> [cols][rows] fp32
 __global__ void transpose_f32_kernel(const float* __restrict__ src, float* __restrict__ dst, int rows, int cols) {
   const int idx = blockIdx.x * blockDim.x + threadIdx.x;
@@ -119,6 +140,14 @@ struct Lin {
   bf16* w = nullptr;  // [N][K]
   float* b = nullptr; // [N] or null
   int N = 0, K = 0;   // K is the PHYSICAL reduction length: 3 x the logical one in split-precision mode
+  // FP8 mode, trunk linears (w is then null): e4m3 codes [N][K] and one scale per 128 x 128 block [N / 128][K / 128]
+  uint8_t* q = nullptr;
+  float* qs = nullptr;
+};
+// FP8 mode: e4m3 activation rows [rows][C] and their scales [rows][C / 128]
+struct Fp8Act {
+  uint8_t* q = nullptr;
+  float* s = nullptr;
 };
 struct LNp {
   float *g = nullptr, *b = nullptr;
@@ -139,12 +168,13 @@ struct Refine {
   Lin out;  // 1x1
 };
 
-enum PackKind { PK_F32, PK_LINEAR, PK_CONV3, PK_CONVT, PK_TRANSPOSE_F32, PK_IGNORE };
+enum PackKind { PK_F32, PK_LINEAR, PK_CONV3, PK_CONVT, PK_TRANSPOSE_F32, PK_IGNORE, PK_LINEAR_FP8 };
 struct Slot {
   PackKind kind;
   std::vector<int64_t> shape;  // expected source shape
   void* dst = nullptr;
-  long long ldd = 0;            // PK_LINEAR: destination row stride
+  long long ldd = 0;            // PK_LINEAR / PK_LINEAR_FP8: destination row stride
+  float* sdst = nullptr;        // PK_LINEAR_FP8: block scales, row stride ldd / 128
   int cin_pad = 0, cout_pad = 0, k = 0;
   bool loaded = false;
 };
@@ -155,6 +185,7 @@ struct Workspace {
   size_t off = 0;
   bool overflow = false;  // a take went past `bytes`: the entry point refuses before its first launch (check_ws)
   int bmul = 1;  // bf16 activations are 3x wide in split-precision mode
+  int fp8 = 0;   // FP8 mode: the trunk linears read e4m3 activations (Fp8Act) instead of bf16 ones
   template <typename T>
   T* take(size_t n) {
     off = (off + 255) & ~static_cast<size_t>(255);
@@ -164,15 +195,23 @@ struct Workspace {
     return p;
   }
   bf16* takeb(size_t n) { return take<bf16>(n * bmul); }  // bf16 activation buffer with n LOGICAL elements
+  Fp8Act takeq(size_t rows, int C) {
+    Fp8Act a;
+    a.q = take<uint8_t>(rows * C);
+    a.s = take<float>(rows * (C / 128));
+    return a;
+  }
 };
 
 struct EncBufs {
-  bf16 *patches, *lnb, *qkv, *att, *hid;
+  bf16 *patches, *lnb, *qkv, *att, *hid;  // lnb, hid: null in FP8 mode
   int* pos;
+  Fp8Act ln8, att8, hid8;  // FP8 mode only
 };
 struct DecBufs {
   float* xd;
-  bf16 *ln1, *lny, *qkv, *att, *qc, *kvc, *hid;
+  bf16 *ln1, *lny, *qkv, *att, *qc, *kvc, *hid;  // ln1, lny, hid: null in FP8 mode
+  Fp8Act ln8, lny8, att8, hid8;                  // FP8 mode only
   bf16* hook[4];  // the DPT hooks (dpt_head.py:112): bf16 encoder features (the decoder input), decoder outputs 6, 9, 12
   int* pos;
 };
@@ -193,6 +232,9 @@ struct StaModel {
   // over 3K, attention runs in fp32 on the CUDA cores.  ~17 significant operand bits instead of 8; ~3.5x slower.
   int split = 0;
   int bmul() const { return split ? 3 : 1; }
+  // 2 = FP8 mode (STA_PRECISION_FP8): the linears of the 24 encoder and 12 decoder blocks run on e4m3 operands with
+  // power-of-two block scales (gemm.cuh A_FP8), everything else as in bf16 mode.
+  int fp8 = 0;
   // ---- weights ----
   char* arena = nullptr;
   size_t arena_bytes = 0, arena_off = 0;
@@ -277,6 +319,12 @@ struct StaModel {
 
 namespace {
 
+#define RUN(expr)            \
+  do {                       \
+    int _rc = (expr);        \
+    if (_rc) return _rc;     \
+  } while (0)
+
 constexpr float kLnEps = 1e-6f;
 constexpr int kEncDim = 1024, kDecDim = 768, kEncHeads = 16, kDecHeads = 12;
 
@@ -295,14 +343,29 @@ void add_slot(StaModel* m, const std::string& name, PackKind kind, std::vector<i
 }
 
 // linear [N][K] (+bias) registered under prefix.weight / prefix.bias; optional zero padding of N
+// FP8 mode: the e4m3 slot of a trunk weight [rows][K] whose first row is row0 of L's packed matrix
+void add_fp8_slot(StaModel* m, const std::string& name, const Lin* L, int row0, int rows) {
+  add_slot(m, name, PK_LINEAR_FP8, {rows, L->K}, L->q + static_cast<size_t>(row0) * L->K, L->K);
+  m->slots[name].sdst = L->qs + static_cast<size_t>(row0 / 128) * (L->K / 128);
+}
+void alloc_fp8(StaModel* m, Lin* L) {
+  L->q = m->alloc<uint8_t>(static_cast<size_t>(L->N) * L->K);
+  L->qs = m->alloc<float>(static_cast<size_t>(L->N / 128) * (L->K / 128));
+}
+// trunk = a linear of the encoder / decoder blocks: e4m3 in FP8 mode
 void reg_linear(StaModel* m, const std::string& prefix, Lin* L, int N, int K, bool bias = true, int N_pad = 0,
-                std::vector<int64_t> wshape = {}) {
+                std::vector<int64_t> wshape = {}, bool trunk = false) {
   const int Np = N_pad > 0 ? N_pad : N;
   L->N = Np;
   L->K = K * m->bmul();
-  L->w = m->alloc<bf16>(static_cast<size_t>(Np) * L->K);
   if (wshape.empty()) wshape = {N, K};
-  add_slot(m, prefix + ".weight", PK_LINEAR, wshape, L->w, L->K);
+  if (trunk && m->fp8) {
+    alloc_fp8(m, L);
+    add_fp8_slot(m, prefix + ".weight", L, 0, N);
+  } else {
+    L->w = m->alloc<bf16>(static_cast<size_t>(Np) * L->K);
+    add_slot(m, prefix + ".weight", PK_LINEAR, wshape, L->w, L->K);
+  }
   if (bias) {
     L->b = m->alloc<float>(Np);
     add_slot(m, prefix + ".bias", PK_F32, {N}, L->b);
@@ -347,11 +410,11 @@ int build_registry(StaModel* m) {
     const std::string p = "enc_blocks." + std::to_string(i) + ".";
     EncBlock& b = m->enc[i];
     reg_ln(m, p + "norm1", &b.n1, kEncDim);
-    reg_linear(m, p + "attn.qkv", &b.qkv, 3 * kEncDim, kEncDim);
-    reg_linear(m, p + "attn.proj", &b.proj, kEncDim, kEncDim);
+    reg_linear(m, p + "attn.qkv", &b.qkv, 3 * kEncDim, kEncDim, true, 0, {}, true);
+    reg_linear(m, p + "attn.proj", &b.proj, kEncDim, kEncDim, true, 0, {}, true);
     reg_ln(m, p + "norm2", &b.n2, kEncDim);
-    reg_linear(m, p + "mlp.fc1", &b.fc1, 4 * kEncDim, kEncDim);
-    reg_linear(m, p + "mlp.fc2", &b.fc2, kEncDim, 4 * kEncDim);
+    reg_linear(m, p + "mlp.fc1", &b.fc1, 4 * kEncDim, kEncDim, true, 0, {}, true);
+    reg_linear(m, p + "mlp.fc2", &b.fc2, kEncDim, 4 * kEncDim, true, 0, {}, true);
   }
   add_slot(m, "enc_norm.weight", PK_IGNORE, {kEncDim}, nullptr);  // never applied (normalize=False everywhere)
   add_slot(m, "enc_norm.bias", PK_IGNORE, {kEncDim}, nullptr);
@@ -360,24 +423,31 @@ int build_registry(StaModel* m) {
     const std::string p = "dec_block." + std::to_string(i) + ".";
     DecBlock& b = m->dec[i];
     reg_ln(m, p + "norm1", &b.n1, kDecDim);
-    reg_linear(m, p + "attn.qkv", &b.qkv, 3 * kDecDim, kDecDim);
-    reg_linear(m, p + "attn.proj", &b.proj, kDecDim, kDecDim);
-    reg_linear(m, p + "cross_attn.projq", &b.cq, kDecDim, kDecDim);
+    reg_linear(m, p + "attn.qkv", &b.qkv, 3 * kDecDim, kDecDim, true, 0, {}, true);
+    reg_linear(m, p + "attn.proj", &b.proj, kDecDim, kDecDim, true, 0, {}, true);
+    reg_linear(m, p + "cross_attn.projq", &b.cq, kDecDim, kDecDim, true, 0, {}, true);
     // projk and projv are fused into one [1536][768] matrix (both act on norm_y(y))
     b.ckv.N = 2 * kDecDim;
     b.ckv.K = kDecDim * m->bmul();
-    b.ckv.w = m->alloc<bf16>(static_cast<size_t>(2) * kDecDim * b.ckv.K);
-    b.ckv.b = m->alloc<float>(2 * kDecDim);
-    add_slot(m, p + "cross_attn.projk.weight", PK_LINEAR, {kDecDim, kDecDim}, b.ckv.w, b.ckv.K);
+    if (m->fp8) {
+      alloc_fp8(m, &b.ckv);
+      add_fp8_slot(m, p + "cross_attn.projk.weight", &b.ckv, 0, kDecDim);
+      add_fp8_slot(m, p + "cross_attn.projv.weight", &b.ckv, kDecDim, kDecDim);
+      b.ckv.b = m->alloc<float>(2 * kDecDim);
+    } else {
+      b.ckv.w = m->alloc<bf16>(static_cast<size_t>(2) * kDecDim * b.ckv.K);
+      b.ckv.b = m->alloc<float>(2 * kDecDim);
+      add_slot(m, p + "cross_attn.projk.weight", PK_LINEAR, {kDecDim, kDecDim}, b.ckv.w, b.ckv.K);
+      add_slot(m, p + "cross_attn.projv.weight", PK_LINEAR, {kDecDim, kDecDim},
+               b.ckv.w + static_cast<size_t>(kDecDim) * b.ckv.K, b.ckv.K);
+    }
     add_slot(m, p + "cross_attn.projk.bias", PK_F32, {kDecDim}, b.ckv.b);
-    add_slot(m, p + "cross_attn.projv.weight", PK_LINEAR, {kDecDim, kDecDim},
-             b.ckv.w + static_cast<size_t>(kDecDim) * b.ckv.K, b.ckv.K);
     add_slot(m, p + "cross_attn.projv.bias", PK_F32, {kDecDim}, b.ckv.b + kDecDim);
-    reg_linear(m, p + "cross_attn.proj", &b.cproj, kDecDim, kDecDim);
+    reg_linear(m, p + "cross_attn.proj", &b.cproj, kDecDim, kDecDim, true, 0, {}, true);
     reg_ln(m, p + "norm2", &b.n2, kDecDim);
     reg_ln(m, p + "norm3", &b.n3, kDecDim);
-    reg_linear(m, p + "mlp.fc1", &b.fc1, 4 * kDecDim, kDecDim);
-    reg_linear(m, p + "mlp.fc2", &b.fc2, kDecDim, 4 * kDecDim);
+    reg_linear(m, p + "mlp.fc1", &b.fc1, 4 * kDecDim, kDecDim, true, 0, {}, true);
+    reg_linear(m, p + "mlp.fc2", &b.fc2, kDecDim, 4 * kDecDim, true, 0, {}, true);
     reg_ln(m, p + "norm_y", &b.ny, kDecDim);
   }
   reg_ln(m, "dec_norm", &m->dec_norm, kDecDim);
@@ -470,7 +540,7 @@ struct ProfScope {
   }
 };
 
-int gemm(const Ctx& c, int amode, int epi, const bf16* A, long long lda, const Lin& L, GemmParams p) {
+int gemm(const Ctx& c, int amode, int epi, const void* A, long long lda, const Lin& L, GemmParams p) {
   GemmLaunch g;
   g.amode = amode;
   g.epi = epi;
@@ -479,6 +549,10 @@ int gemm(const Ctx& c, int amode, int epi, const bf16* A, long long lda, const L
   g.splitk_ws = c.m->splitk_ws;
   g.splitk_ws_bytes = c.m->splitk_ws ? StaModel::kSplitKBytes : 0;
   g.Wt = L.w;
+  if (amode == A_FP8) {
+    g.Wt = L.q;
+    p.w_scale = L.qs;
+  }
   g.ldw = L.K;
   p.N = L.N;
   p.K = L.K;
@@ -491,6 +565,17 @@ int gemm(const Ctx& c, int amode, int epi, const bf16* A, long long lda, const L
   ProfScope ps(c, amode == A_CONV3 ? PROF_CONV : PROF_GEMM, 2.0 * rows * L.N * L.K);
   return launch_gemm(g, c.st);
 }
+int set_rope(GemmParams& p, const int* pos, int rope_cols) {
+  p.pos = pos;
+  p.rope_cols = rope_cols;
+  p.rope_tab = rope_table(&p.rope_max_pos);
+  if (!p.rope_tab) {
+    set_last_error("failed to build the RoPE table");
+    return 1;
+  }
+  p.rope_smem_rows = 64;  // positions -1..62 from shared memory, larger ones from the global table
+  return 0;
+}
 // plain linear on rows
 int linear(const Ctx& c, int epi, const bf16* A, int M, const Lin& L, void* out, const void* resid = nullptr,
            const int* pos = nullptr, int rope_cols = 0, int rowmap_n = 0) {
@@ -500,17 +585,25 @@ int linear(const Ctx& c, int epi, const bf16* A, int M, const Lin& L, void* out,
   p.ldo = L.N;
   p.resid = resid;
   p.rowmap_n = rowmap_n;
-  if (epi == EPI_ROPE) {
-    p.pos = pos;
-    p.rope_cols = rope_cols;
-    p.rope_tab = rope_table(&p.rope_max_pos);
-    if (!p.rope_tab) {
-      set_last_error("failed to build the RoPE table");
-      return 1;
-    }
-    p.rope_smem_rows = 64;  // positions -1..62 from shared memory, larger ones from the global table
-  }
+  if (epi == EPI_ROPE) RUN(set_rope(p, pos, rope_cols));
   return gemm(c, A_LINEAR, epi, A, L.K, L, p);
+}
+// FP8 mode: a trunk linear on e4m3 rows a.  EPI_F32: out += a W^T + b in place (the residual stream); EPI_ROPE: bf16 q/k/v
+// rows for the attention kernel; EPI_GELU_FP8: e4m3 rows + scales into *q.
+int linear_fp8(const Ctx& c, int epi, const Fp8Act& a, int M, const Lin& L, void* out, const int* pos = nullptr,
+               int rope_cols = 0, const Fp8Act* q = nullptr) {
+  GemmParams p = {};
+  p.M = M;
+  p.out = out;
+  p.ldo = L.N;
+  p.a_scale = a.s;
+  if (epi == EPI_F32) p.resid = out;
+  if (epi == EPI_ROPE) RUN(set_rope(p, pos, rope_cols));
+  if (epi == EPI_GELU_FP8) {
+    p.out = q->q;
+    p.out_scale = q->s;
+  }
+  return gemm(c, A_FP8, epi, a.q, L.K, L, p);
 }
 int conv3(const Ctx& c, const bf16* in, int nimg, int H, int W, int Cin, const Lin& L, bf16* out, bf16* out_relu,
           const bf16* resid, const bf16* resid2, int relu_main) {
@@ -534,6 +627,19 @@ int ln(const Ctx& c, const float* x, int rows, int C, const LNp& a, bf16* out1, 
   return launch_layernorm(x, rows, C, kLnEps, a.g, a.b, out1, b2 ? b2->g : nullptr, b2 ? b2->b : nullptr, out2,
                           drop_first_of, c.st, c.m->split);
 }
+int ln_fp8(const Ctx& c, const float* x, int rows, int C, const LNp& a, const Fp8Act& o1, const LNp* b2 = nullptr,
+           const Fp8Act* o2 = nullptr) {
+  c.m->launches++;
+  ProfScope ps(c, PROF_LN, 0.0);
+  return launch_layernorm_fp8(x, rows, C, kLnEps, a.g, a.b, o1.q, o1.s, b2 ? b2->g : nullptr, b2 ? b2->b : nullptr,
+                              o2 ? o2->q : nullptr, o2 ? o2->s : nullptr, c.st);
+}
+// FP8 mode: bf16 attention output -> e4m3 (counted with the LayerNorms: both are row-wise bandwidth-bound passes)
+int quant_fp8(const Ctx& c, const bf16* in, long long rows, int C, const Fp8Act& o) {
+  c.m->launches++;
+  ProfScope ps(c, PROF_LN, 0.0);
+  return launch_quant_fp8(in, rows, C, o.q, o.s, c.st);
+}
 int attn(const Ctx& c, const bf16* q, long long ldq, int qc, const bf16* k, long long ldk, int kc, const bf16* v,
          long long ldv, int vc, bf16* out, long long ldo, int batch, int heads, int nq, int nk, int shift) {
   AttnLaunch a;
@@ -551,12 +657,6 @@ int attn(const Ctx& c, const bf16* q, long long ldq, int qc, const bf16* k, long
   return launch_attention(a, c.st);
 }
 
-#define RUN(expr)            \
-  do {                       \
-    int _rc = (expr);        \
-    if (_rc) return _rc;     \
-  } while (0)
-
 // ---------------------------------------------------------------------------
 // workspace: every entry point carves its buffers with the take functions below before its first launch, and
 // ws_need sizes the allocation by a dry run of the same functions
@@ -565,11 +665,16 @@ EncBufs take_enc(Workspace& ws, int nimg, int N) {
   const size_t T = static_cast<size_t>(nimg) * N;
   EncBufs e;
   e.patches = ws.takeb(T * 768);
-  e.lnb = ws.takeb(T * 1024);
+  e.lnb = ws.fp8 ? nullptr : ws.takeb(T * 1024);
   e.qkv = ws.takeb(T * 3072);
   e.att = ws.takeb(T * 1024);
-  e.hid = ws.takeb(T * 4096);
+  e.hid = ws.fp8 ? nullptr : ws.takeb(T * 4096);
   e.pos = ws.take<int>(T * 2);
+  if (ws.fp8) {
+    e.ln8 = ws.takeq(T, 1024);
+    e.att8 = ws.takeq(T, 1024);
+    e.hid8 = ws.takeq(T, 4096);
+  }
   return e;
 }
 // The DPT head's four token inputs for nimg images of N tokens: [nimg*N][1024 | 768 | 768 | 768]
@@ -582,15 +687,21 @@ DecBufs take_dec(Workspace& ws, int S, int N) {
   const size_t Td = static_cast<size_t>(S) * (N + 1);
   DecBufs d;
   d.xd = ws.take<float>(Td * 768);
-  d.ln1 = ws.takeb(Td * 768);
-  d.lny = ws.takeb(Td * 768);
+  d.ln1 = ws.fp8 ? nullptr : ws.takeb(Td * 768);
+  d.lny = ws.fp8 ? nullptr : ws.takeb(Td * 768);
   d.qkv = ws.takeb(Td * 2304);
   d.att = ws.takeb(Td * 768);
   d.qc = ws.takeb(Td * 768);
   d.kvc = ws.takeb(Td * 1536);
-  d.hid = ws.takeb(Td * 3072);
+  d.hid = ws.fp8 ? nullptr : ws.takeb(Td * 3072);
   take_hooks(ws, S, N, d.hook);
   d.pos = ws.take<int>(Td * 2);
+  if (ws.fp8) {
+    d.ln8 = ws.takeq(Td, 768);
+    d.lny8 = ws.takeq(Td, 768);
+    d.att8 = ws.takeq(Td, 768);
+    d.hid8 = ws.takeq(Td, 3072);
+  }
   return d;
 }
 // DPT head over up to nimg images of an h x w token grid
@@ -668,9 +779,10 @@ PairOuts stage_pair_outs(Staging& s, const PairOuts& u, int n, long long px) {
 // entry point: encoder + fp32 residual stream + decoder + DPT head (sta_forward_pairs), and on top of the decoder the
 // keyframe step's staged poses (_begin), compact hook copies and staged outputs (_finish with every edge kept and every
 // output asked for).
-size_t ws_need(int nimg, int h, int w, int bmul) {
+size_t ws_need(int nimg, int h, int w, int bmul, int fp8) {
   Workspace dry;
   dry.bmul = bmul;
+  dry.fp8 = fp8;
   const int N = h * w;
   float any;  // stands for a caller's tensor: staging only asks whether there is one
   bf16* hook[4];
@@ -689,8 +801,9 @@ size_t ws_need(int nimg, int h, int w, int bmul) {
 void drop_graphs(StaModel* m);
 
 int ensure_ws(StaModel* m, int nimg, int h, int w) {
-  const size_t need = ws_need(nimg, h, w, m->bmul());
+  const size_t need = ws_need(nimg, h, w, m->bmul(), m->fp8);
   m->ws.bmul = m->bmul();
+  m->ws.fp8 = m->fp8;
   if (m->ws.bytes < need) {
     STA_CHECK_CUDA(cudaDeviceSynchronize());
     drop_graphs(m);  // they point into the old workspace
@@ -782,6 +895,18 @@ int run_encoder(const Ctx& c, int nimg, int N, float* x, EncBufs& e) {
   RUN(linear(c, EPI_F32, e.patches, T, m->patch, x));
   for (int l = 0; l < 24; ++l) {
     const EncBlock& b = m->enc[l];
+    if (m->fp8) {
+      RUN(ln_fp8(c, x, T, kEncDim, b.n1, e.ln8));
+      RUN(linear_fp8(c, EPI_ROPE, e.ln8, T, b.qkv, e.qkv, e.pos, 2 * kEncDim));
+      RUN(attn(c, e.qkv, 3 * kEncDim, 0, e.qkv, 3 * kEncDim, kEncDim, e.qkv, 3 * kEncDim, 2 * kEncDim, e.att, kEncDim,
+               nimg, kEncHeads, N, N, 0));
+      RUN(quant_fp8(c, e.att, T, kEncDim, e.att8));
+      RUN(linear_fp8(c, EPI_F32, e.att8, T, b.proj, x));
+      RUN(ln_fp8(c, x, T, kEncDim, b.n2, e.ln8));
+      RUN(linear_fp8(c, EPI_GELU_FP8, e.ln8, T, b.fc1, nullptr, nullptr, 0, &e.hid8));
+      RUN(linear_fp8(c, EPI_F32, e.hid8, T, b.fc2, x));
+      continue;
+    }
     RUN(ln(c, x, T, kEncDim, b.n1, e.lnb));
     RUN(linear(c, EPI_ROPE, e.lnb, T, b.qkv, e.qkv, nullptr, e.pos, 2 * kEncDim));
     RUN(attn(c, e.qkv, 3 * kEncDim, 0, e.qkv, 3 * kEncDim, kEncDim, e.qkv, 3 * kEncDim, 2 * kEncDim, e.att, kEncDim,
@@ -814,6 +939,24 @@ int run_decoder(const Ctx& c, int B, int N, DecBufs& d, float* const* out1, floa
   RUN(emit(0));
   for (int l = 0; l < 12; ++l) {
     const DecBlock& b = m->dec[l];
+    if (m->fp8) {  // the same sequence with e4m3 operands for every linear
+      RUN(ln_fp8(c, d.xd, Td, kDecDim, b.n1, d.ln8, &b.ny, &d.lny8));
+      RUN(linear_fp8(c, EPI_ROPE, d.ln8, Td, b.qkv, d.qkv, d.pos, 2 * kDecDim));
+      RUN(attn(c, d.qkv, 3 * kDecDim, 0, d.qkv, 3 * kDecDim, kDecDim, d.qkv, 3 * kDecDim, 2 * kDecDim, d.att, kDecDim, S,
+               kDecHeads, M, M, 0));
+      RUN(quant_fp8(c, d.att, Td, kDecDim, d.att8));
+      RUN(linear_fp8(c, EPI_F32, d.att8, Td, b.proj, d.xd));
+      RUN(linear_fp8(c, EPI_ROPE, d.lny8, Td, b.ckv, d.kvc, d.pos, kDecDim));
+      RUN(ln_fp8(c, d.xd, Td, kDecDim, b.n2, d.ln8));
+      RUN(linear_fp8(c, EPI_ROPE, d.ln8, Td, b.cq, d.qc, d.pos, kDecDim));
+      RUN(attn(c, d.qc, kDecDim, 0, d.kvc, 2 * kDecDim, 0, d.kvc, 2 * kDecDim, kDecDim, d.att, kDecDim, S, kDecHeads, M,
+               M, B));
+      RUN(quant_fp8(c, d.att, Td, kDecDim, d.att8));
+      RUN(linear_fp8(c, EPI_F32, d.att8, Td, b.cproj, d.xd));
+      RUN(ln_fp8(c, d.xd, Td, kDecDim, b.n3, d.ln8));
+      RUN(linear_fp8(c, EPI_GELU_FP8, d.ln8, Td, b.fc1, nullptr, nullptr, 0, &d.hid8));
+      RUN(linear_fp8(c, EPI_F32, d.hid8, Td, b.fc2, d.xd));
+    } else {
     // self-attention on norm1(x); norm_y(x) is what the partner view cross-attends to
     RUN(ln(c, d.xd, Td, kDecDim, b.n1, d.ln1, &b.ny, d.lny));
     RUN(linear(c, EPI_ROPE, d.ln1, Td, b.qkv, d.qkv, nullptr, d.pos, 2 * kDecDim));
@@ -831,6 +974,7 @@ int run_decoder(const Ctx& c, int B, int N, DecBufs& d, float* const* out1, floa
     RUN(ln(c, d.xd, Td, kDecDim, b.n3, d.ln1));
     RUN(linear(c, EPI_GELU, d.ln1, Td, b.fc1, d.hid));
     RUN(linear(c, EPI_F32, d.hid, Td, b.fc2, d.xd, d.xd));
+    }
     if (l + 1 == 6 || l + 1 == 9) {  // DPT hooks [0, 7, 10, 13] -> decoder outputs 6, 9, 12 (dpt_head.py:112)
       m->launches++;
       RUN(launch_cast_f32_bf16(d.xd, d.hook[l + 1 == 6 ? 1 : 2], Td, kDecDim, M, c.st, m->split));
@@ -1079,8 +1223,8 @@ int sta_device_synchronize(void) {
 int sta_create(StaModel** out) { return sta_create_ex(out, STA_PRECISION_BF16); }
 
 int sta_create_ex(StaModel** out, int precision) {
-  if (precision != STA_PRECISION_BF16 && precision != STA_PRECISION_X3) {
-    set_last_error("sta_create_ex: unknown precision (0 = bf16, 1 = split-precision x3 parity mode)");
+  if (precision != STA_PRECISION_BF16 && precision != STA_PRECISION_X3 && precision != STA_PRECISION_FP8) {
+    set_last_error("sta_create_ex: unknown precision (0 = bf16, 1 = split-precision x3 parity mode, 2 = fp8)");
     return 2;
   }
   if (!out) {
@@ -1101,8 +1245,16 @@ int sta_create_ex(StaModel** out, int precision) {
   }
   StaModel* m = new StaModel();
   m->split = (precision == STA_PRECISION_X3) ? 1 : 0;
+  m->fp8 = (precision == STA_PRECISION_FP8) ? 1 : 0;
   // 438.5 M params: ~877 MB bf16 + fp32 vectors + padding (3x the bf16 part in split-precision mode)
   m->arena_bytes = static_cast<size_t>(m->split ? 2800 : 960) << 20;
+  if (m->fp8) {  // 415 M trunk weights at one byte: the exact size, from a dry run of the registry (no arena yet)
+    build_registry(m);
+    m->arena_bytes = (m->arena_off + 255) & ~static_cast<size_t>(255);
+    m->slots.clear();
+    m->missing = 0;
+    m->arena_off = 0;
+  }
   cudaError_t e = cudaMalloc(&m->arena, m->arena_bytes);
   if (e != cudaSuccess) {
     set_last_error(std::string("cudaMalloc(weight arena) failed: ") + cudaGetErrorString(e));
@@ -1254,6 +1406,13 @@ int sta_load_tensor(StaModel* m, const char* name, const float* data, const int6
       const int rows = static_cast<int>(s.shape[0]);
       const int cols = static_cast<int>(numel / rows);
       pack_linear_kernel<<<blocks, threads>>>(src, static_cast<bf16*>(s.dst), rows, cols, s.ldd, m->split);
+      break;
+    }
+    case PK_LINEAR_FP8: {
+      const int rows = static_cast<int>(s.shape[0]), cols = static_cast<int>(s.shape[1]);
+      STA_REQUIRE(rows % 128 == 0 && cols % 128 == 0, "fp8 weights come in 128 x 128 blocks");
+      pack_linear_fp8_kernel<<<dim3(cols / 128, rows / 128), 256>>>(src, cols, static_cast<uint8_t*>(s.dst), s.ldd, s.sdst,
+                                                                    static_cast<int>(s.ldd / 128));
       break;
     }
     case PK_CONV3:
@@ -1638,6 +1797,42 @@ int sta_op_gemm(const StaGemmDesc* d, void* stream) {
   p.split = d->split_precision;
   g.p = p;
   return launch_gemm(g, static_cast<cudaStream_t>(stream));
+}
+
+int sta_op_gemm_fp8(const StaGemmFp8Desc* d, void* stream) {
+  if (!d) {
+    set_last_error("sta_op_gemm_fp8: null descriptor");
+    return 2;
+  }
+  STA_REQUIRE(d->epi == STA_EPI_F32 || d->epi == STA_EPI_ROPE || d->epi == STA_EPI_GELU_FP8,
+              "sta_op_gemm_fp8: epi must be STA_EPI_F32, STA_EPI_ROPE or STA_EPI_GELU_FP8");
+  GemmLaunch g;
+  g.amode = A_FP8;
+  g.epi = d->epi;
+  g.A = d->A;
+  g.lda = d->lda;
+  g.Wt = d->W;
+  g.ldw = d->ldw;
+  g.splitk_ws = d->splitk_ws;
+  g.splitk_ws_bytes = d->splitk_ws ? static_cast<size_t>(d->splitk_ws_bytes) : 0;
+  GemmParams p = {};
+  p.M = d->M; p.N = d->N; p.K = d->K;
+  p.bias = d->bias;
+  p.out = d->out; p.ldo = d->ldo;
+  p.resid = d->resid;
+  p.a_scale = d->a_scale; p.w_scale = d->w_scale; p.out_scale = d->out_scale;
+  if (d->epi == STA_EPI_ROPE) RUN(set_rope(p, d->pos, d->rope_cols));
+  g.p = p;
+  return launch_gemm(g, static_cast<cudaStream_t>(stream));
+}
+int sta_op_layernorm_fp8(const float* x, int rows, int C, float eps, const float* g1, const float* b1, void* q1, float* s1,
+                         const float* g2, const float* b2, void* q2, float* s2, void* stream) {
+  return launch_layernorm_fp8(x, rows, C, eps, g1, b1, static_cast<uint8_t*>(q1), s1, g2, b2, static_cast<uint8_t*>(q2), s2,
+                              static_cast<cudaStream_t>(stream));
+}
+int sta_op_quant_fp8(const void* in_bf16, int64_t rows, int C, void* q, float* s, void* stream) {
+  return launch_quant_fp8(static_cast<const bf16*>(in_bf16), rows, C, static_cast<uint8_t*>(q), s,
+                          static_cast<cudaStream_t>(stream));
 }
 
 static int op_attention(const void* q, int64_t ldq, int q_col0, const void* k, int64_t ldk, int k_col0, const void* v,

@@ -135,10 +135,12 @@ class SymmetricTwoViewAssociation(nn.Module):
                  output_mode="pts3d", head_type="dpt", depth_mode=("exp", -inf, inf), conf_mode=("exp", 1, inf),
                  freeze="none", landscape_only=True, patch_embed_cls="PatchEmbedDust3R", precision="bf16"):
         super().__init__()
-        # `precision` is the one extension of the reference signature: "bf16" (production; every benchmark number)
-        # or "x3" = split-precision parity mode (include/sta_b200.h, STA_PRECISION_X3) used by the parity tests.
-        if precision not in ("bf16", "x3"):
-            raise ValueError("precision must be 'bf16' or 'x3'")
+        # `precision` is the one extension of the reference signature: "bf16" (production; every benchmark number),
+        # "x3" = split-precision parity mode (include/sta_b200.h, STA_PRECISION_X3) used by the parity tests, or "fp8" =
+        # e4m3 operands with block scales for the encoder and decoder linears (STA_PRECISION_FP8): an opt-in that changes
+        # the numerics (INTEGRATION.md section 5).
+        if precision not in ("bf16", "x3", "fp8"):
+            raise ValueError("precision must be 'bf16', 'x3' or 'fp8'")
         self.precision = precision
         fixed = dict(patch_size=(patch_size, 16), enc_embed_dim=(enc_embed_dim, 1024), enc_depth=(enc_depth, 24),
                      enc_num_heads=(enc_num_heads, 16), dec_embed_dim=(dec_embed_dim, 768), dec_depth=(dec_depth, 12),
@@ -263,7 +265,7 @@ class SymmetricTwoViewAssociation(nn.Module):
 
     def _create(self, L):
         h = ctypes.c_void_p()
-        prec = _lib.PRECISION_X3 if self.precision == "x3" else _lib.PRECISION_BF16
+        prec = {"bf16": _lib.PRECISION_BF16, "x3": _lib.PRECISION_X3, "fp8": _lib.PRECISION_FP8}[self.precision]
         _lib.check(L.sta_create_ex(ctypes.byref(h), prec), "sta_create_ex")
         return h
 
