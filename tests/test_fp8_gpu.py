@@ -34,7 +34,10 @@ TAU = 1.25e-4
 # single token through an SVD amplifies it most on the smallest golden (12 tokens: the oracle's own pose deviation from
 # fp32 is 4-13x bf16's there and changes by 3x with the host's BLAS; the kernels' reached 0.79), so the pose bounds are
 # also allowed POSE_FACTOR x the oracle's own deviation from fp32, and that golden's pose is only checked to be a rigid
-# transform.
+# transform.  That deviation is ill-conditioning, not the pose head: on that golden the head kernel matches a float64
+# head on the FP8 model's own pose tokens with err / bound < 1e-4 (tests/test_pose_head_gpu.py), while those tokens
+# are 11% from the bf16 model's and the resulting rotations differ by up to 0.82 (H100 80GB HBM3, 700 W).
+# Sample 0's tokens give det A < 0 with sigma2 - sigma3 = 0.17, so a token error reaches R amplified by 2 / 0.17 = 12.
 TOL_ORACLE = {"pts3d_pred": 1.5e-1, "conf": 1.5e-1, "relative_pose": 2.5e-1, "relative_pose_conf": 6e-2}
 POSE_FACTOR = 4.0
 ILL_CONDITIONED_POSE = {"pair_b2_48x64"}

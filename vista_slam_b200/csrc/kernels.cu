@@ -661,7 +661,22 @@ __device__ void svd_orthogonalize_3x3(const float* A, float* R) {
       Vs[i][j] = V[i][src];
     }
   }
-  if (sig[order[2]] <= 1e-20f) {  // rank deficient: complete U with u0 x u1
+  // rank deficient: complete U to an orthonormal basis.  Rank 0: u0 = e0.  Rank <= 1: u1 = the coordinate axis least
+  // aligned with u0, made orthogonal to it.  Rank <= 2: u2 = u0 x u1.
+  if (sig[order[0]] <= 1e-20f) {
+    U[0][0] = 1.f; U[1][0] = 0.f; U[2][0] = 0.f;
+  }
+  if (sig[order[1]] <= 1e-20f) {
+    const float a0 = fabsf(U[0][0]), a1 = fabsf(U[1][0]), a2 = fabsf(U[2][0]);
+    const int k = (a0 <= a1 && a0 <= a2) ? 0 : (a1 <= a2 ? 1 : 2);
+    float v[3];
+#pragma unroll
+    for (int i = 0; i < 3; ++i) v[i] = (i == k ? 1.f : 0.f) - U[k][0] * U[i][0];
+    const float inv = rsqrtf(v[0] * v[0] + v[1] * v[1] + v[2] * v[2]);  // |v|^2 = 1 - u0_k^2 >= 2/3
+#pragma unroll
+    for (int i = 0; i < 3; ++i) U[i][1] = v[i] * inv;
+  }
+  if (sig[order[2]] <= 1e-20f) {
     U[0][2] = U[1][0] * U[2][1] - U[2][0] * U[1][1];
     U[1][2] = U[2][0] * U[0][1] - U[0][0] * U[2][1];
     U[2][2] = U[0][0] * U[1][1] - U[1][0] * U[0][1];
