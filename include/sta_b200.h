@@ -65,6 +65,11 @@ int sta_missing_tensors(StaModel* m);
  * and the receiving ranks call sta_mark_all_loaded. */
 int sta_weight_arena(StaModel* m, void** dev_ptr_out, int64_t* bytes_out);
 int sta_mark_all_loaded(StaModel* m);
+/* Read-only: where the state-dict tensor `name` lands in the arena.  data_out: its packed destination (device memory;
+ * NULL for a name the forward pass ignores), ld_out: its row stride in elements for the linear packings (0 otherwise),
+ * scales_out: for an FP8-mode trunk weight (e4m3 codes, row stride ld_out bytes) its 128 x 128 block scales, fp32
+ * [rows / 128][ld_out / 128], else NULL.  Returns non-zero for an unknown name. */
+int sta_weight_slot(StaModel* m, const char* name, void** data_out, int64_t* ld_out, float** scales_out);
 
 /* ---- model-level forward entry points ---- */
 

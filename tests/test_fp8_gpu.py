@@ -1,33 +1,28 @@
-"""GPU: the FP8 mode (STA(precision="fp8"), include/sta_b200.h STA_PRECISION_FP8) -- its quantisers and GEMM against
-exactly known operands, the whole model against the CPU restatement of the recipe (oracle/fp8_oracle.py) and the fp32
+"""GPU: the FP8 mode (STA(precision="fp8"), include/sta_b200.h STA_PRECISION_FP8) -- the bf16 quantiser, tile offsets
+and a planted long sum of its GEMM (every launch at the model's sizes: tests/test_layers_fp8_gpu.py), the whole model against the CPU restatement of the recipe (oracle/fp8_oracle.py) and the fp32
 goldens, its effect on the other modes, its memory, and OnlineSLAM on top of it."""
 import ctypes
 import json
 import math
 import os
 
-import numpy as np
 import pytest
 import torch
 import torch.nn.functional as F
 
 from conftest import GOLDEN_DIR
-from oracle.fp8_oracle import Fp8Oracle, dequantize_blocks, dequantize_rows, fp8_scale, quantize_blocks, quantize_rows
+from oracle.fp8_oracle import Fp8Oracle, dequantize_blocks, dequantize_rows, quantize_blocks, quantize_rows
 from oracle.sta_oracle import make_images
 from test_gemm_schedule_gpu import _copies, _tile_rows
 from test_model_gpu import KEYS, golden_case, maxn, medn
 
 pytestmark = pytest.mark.gpu
 
-import tools.bringup as bu  # noqa: E402  (rope_ref)
 from vista_slam_b200 import _lib  # noqa: E402
 from vista_slam_b200._lib import EPI_F32, EPI_GELU_FP8, EPI_ROPE, StaGemmFp8Desc  # noqa: E402
 
 DEV = "cuda"
 CASES = ["pair_64x80", "pair_b2_48x64", "pair_224x224", "pair_384x512"]
-# GEMM: |out - fp64 product of the dequantised operands| <= TAU * sum_k |a_k w_k| per element (every trunk shape below);
-# largest ratio measured: 6.1e-5 (H100 80GB HBM3, 700 W power limit).
-TAU = 1.25e-4
 # FP8 model against the fp8 oracle: max-normalised deviation over the four goldens and both views, about twice what was
 # measured for the dense outputs (pts3d 7.0e-2, conf 4.8e-2 on an H100).  The kernels and the oracle round the same
 # recipe from slightly different fp32 values (LayerNorm, GEMM sums), so each carries its own e4m3 noise; the pose of a
@@ -44,21 +39,10 @@ ILL_CONDITIONED_POSE = {"pair_b2_48x64"}
 # dense outputs against fp32: max and median deviation relative to the oracle's own (largest measured: 1.27x median,
 # pair_64x80 main view)
 MAX_VS_ORACLE, MED_VS_ORACLE = 1.6, 1.3
-# trunk (N, K) of the encoder (qkv, proj, fc1, fc2) and decoder (qkv, proj/projq/cross proj, projk|projv, fc1, fc2)
-TRUNK = [(3072, 1024), (1024, 1024), (4096, 1024), (1024, 4096), (2304, 768), (768, 768), (1536, 768), (3072, 768),
-         (768, 3072)]
-EPIS = {(3072, 1024): EPI_ROPE, (1024, 1024): EPI_F32, (4096, 1024): EPI_GELU_FP8, (1024, 4096): EPI_F32,
-        (2304, 768): EPI_ROPE, (768, 768): EPI_F32, (1536, 768): EPI_ROPE, (3072, 768): EPI_GELU_FP8, (768, 3072): EPI_F32}
 
 
 def _u8(q):
     return q.view(torch.uint8)
-
-
-def _ord(codes):
-    """e4m3 codes (uint8) -> integers that are monotonic in the value (sign-magnitude; -0 = +0)"""
-    c = codes.to(torch.int32)
-    return torch.where(c >= 128, -(c - 128), c)
 
 
 def _operands(M, N, K, g):
@@ -71,7 +55,7 @@ def _operands(M, N, K, g):
     return aq, as_, dequantize_rows(aq, as_).double(), wq, ws, dequantize_blocks(wq, ws).double()
 
 
-def _gemm(epi, aq, as_, wq, ws, M, N, K, bias, out, resid=None, out_scale=None, pos=None, ws_split=None):
+def _gemm(epi, aq, as_, wq, ws, M, N, K, bias, out, resid=None, out_scale=None, pos=None, rope_cols=0):
     d = StaGemmFp8Desc()
     d.epi, d.M, d.N, d.K = epi, M, N, K
     d.A, d.lda, d.a_scale = aq.data_ptr(), K, as_.data_ptr()
@@ -81,40 +65,12 @@ def _gemm(epi, aq, as_, wq, ws, M, N, K, bias, out, resid=None, out_scale=None, 
     d.resid = None if resid is None else resid.data_ptr()
     d.out_scale = None if out_scale is None else out_scale.data_ptr()
     if pos is not None:
-        d.pos, d.rope_cols = pos.data_ptr(), 2 * N // 3
-    if ws_split is not None:
-        d.splitk_ws, d.splitk_ws_bytes = ws_split.data_ptr(), ws_split.numel() * 4
+        d.pos, d.rope_cols = pos.data_ptr(), rope_cols
     _lib.check(_lib.lib().sta_op_gemm_fp8(ctypes.byref(d), _lib.cur_stream()), "sta_op_gemm_fp8")
 
 
 def _dev(*ts):
     return [_u8(t).to(DEV) if t.dtype == torch.float8_e4m3fn else t.to(DEV) for t in ts]
-
-
-def _near_boundary(amax, rel):
-    """groups whose amax lies within rel (relative) of a scale boundary 448 * 2^e"""
-    a = amax.double().clamp_min(1e-300)
-    r = torch.log2(a / 448.0)
-    return ((torch.exp2(torch.round(r)) * 448.0 - a).abs() <= rel * a)
-
-
-def _check_quantised(q_dev, s_dev, ref64, rel_boundary, codes=True):
-    """e4m3 codes + scales against the quantisation of an fp64 reference: equal scales except near a boundary, codes
-    within one e4m3 step where the scales agree"""
-    rows, C = ref64.shape
-    amax = ref64.reshape(rows, C // 128, 128).abs().amax(-1)
-    s_ref, _ = fp8_scale(amax.float())
-    s = s_dev.cpu()
-    near = _near_boundary(amax, rel_boundary)
-    assert bool(((s == s_ref) | near).all()), "scales"
-    if not codes:
-        return
-    same = (s == s_ref).repeat_interleave(128, 1)
-    # quantise ref / s with scale 1: the reference codes at the scale the kernel chose
-    ref_codes = ((ref64.reshape(rows, C // 128, 128) / s.double()[..., None]).reshape(rows, C).float().clamp(-448, 448)
-                 .to(torch.float8_e4m3fn))
-    d = (_ord(q_dev.cpu()) - _ord(_u8(ref_codes))).abs()
-    assert int(d[same].max()) <= 1, "codes"
 
 
 def test_quant_bf16_is_bit_identical_to_cpu():
@@ -128,97 +84,6 @@ def test_quant_bf16_is_bit_identical_to_cpu():
     torch.cuda.synchronize()
     q_ref, s_ref = quantize_rows(x.float())
     assert torch.equal(q.cpu(), _u8(q_ref)) and torch.equal(s.cpu(), s_ref)
-
-
-@pytest.mark.parametrize("C", [768, 1024])
-def test_layernorm_fp8_matches_fp64_quantisation(C):
-    g = torch.Generator().manual_seed(C)
-    rows = 517
-    x = torch.randn(rows, C, generator=g) * 3 + torch.randn(rows, 1, generator=g)
-    g1, b1 = 1 + 0.3 * torch.randn(C, generator=g), 0.1 * torch.randn(C, generator=g)
-    g2, b2 = 1 + 0.3 * torch.randn(C, generator=g), 0.1 * torch.randn(C, generator=g)
-    outs = [(torch.empty(rows, C, dtype=torch.uint8, device=DEV), torch.empty(rows, C // 128, device=DEV)) for _ in range(2)]
-    xd, g1d, b1d, g2d, b2d = _dev(x, g1, b1, g2, b2)
-    _lib.check(_lib.lib().sta_op_layernorm_fp8(xd.data_ptr(), rows, C, 1e-6, g1d.data_ptr(), b1d.data_ptr(),
-                                               outs[0][0].data_ptr(), outs[0][1].data_ptr(), g2d.data_ptr(), b2d.data_ptr(),
-                                               outs[1][0].data_ptr(), outs[1][1].data_ptr(), _lib.cur_stream()))
-    torch.cuda.synchronize()
-    for (q, s), (gg, bb) in zip(outs, ((g1, b1), (g2, b2))):
-        ref = F.layer_norm(x.double(), (C,), gg.double(), bb.double(), 1e-6)
-        _check_quantised(q, s, ref, 2.0 ** -23)  # one fp32 ulp
-
-
-def _ref_and_bound(aq64, wq64, bias):
-    ref = aq64 @ wq64.t() + bias.double()
-    S = aq64.abs() @ wq64.abs().t()
-    return ref, S
-
-
-def _run_case(epi, N, K, M, g, record):
-    aq, as_, a64, wq, ws, w64 = _operands(M, N, K, g)
-    bias = torch.randn(N, generator=g) * 0.1
-    ref, S = _ref_and_bound(a64, w64, bias)
-    aqd, asd, wqd, wsd, biasd = _dev(aq, as_, wq, ws, bias)
-    if epi == EPI_F32:
-        x0 = torch.randn(M, N, generator=g)
-        x = x0.to(DEV)
-        _gemm(epi, aqd, asd, wqd, wsd, M, N, K, biasd, x, resid=x)
-        torch.cuda.synchronize()
-        err = (x.cpu().double() - x0.double() - ref).abs()
-        # plus the fp32 roundings of the bias add and the residual add
-        bound = S + (x0.double().abs() + ref.abs() + bias.double().abs()) * 2.0 ** -22 / TAU
-        record.append(float((err / bound).max()))
-        assert bool((err <= TAU * bound + 1e-30).all()), (N, K, float((err / S).max()))
-    elif epi == EPI_ROPE:
-        pos = torch.randint(-1, 40, (M, 2), generator=g, dtype=torch.int32)
-        out = torch.full((M, N), float("nan"), device=DEV, dtype=torch.bfloat16)
-        _gemm(epi, aqd, asd, wqd, wsd, M, N, K, biasd, out, pos=pos.to(DEV))
-        torch.cuda.synchronize()
-        rc = 2 * N // 3
-        rot = bu.rope_ref(ref[:, :rc].reshape(M, rc // 64, 64), pos).reshape(M, rc)
-        rref = torch.cat([rot, ref[:, rc:]], 1)
-        Sp = torch.cat([S[:, :rc].reshape(M, -1, 2, 16).flip(2).reshape(M, rc) + S[:, :rc], S[:, rc:]], 1)
-        err = (out.cpu().double() - rref).abs()
-        record.append(float(((err - rref.abs() * 2.0 ** -8).clamp_min(0) / Sp).max()))
-        assert bool((err <= TAU * Sp + rref.abs() * 2.0 ** -8 + 1e-30).all()), (N, K)
-    else:
-        q = torch.empty(M, N, dtype=torch.uint8, device=DEV)
-        s = torch.empty(M, N // 128, device=DEV)
-        _gemm(epi, aqd, asd, wqd, wsd, M, N, K, biasd, q, out_scale=s)
-        torch.cuda.synchronize()
-        gel = F.gelu(ref)
-        # GELU of a sum known to TAU * S: the scales agree except near a boundary; the codes are bounded below through
-        # the values (near zero the GEMM's error TAU * S is many e4m3 steps)
-        _check_quantised(q, s, gel, 1e-5 + 2 * TAU * float((S / ref.abs().amax()).max()), codes=False)
-        deq = dequantize_rows(_u8(q.cpu()).view(torch.float8_e4m3fn), s.cpu()).double()
-        step = s.cpu().double().repeat_interleave(128, 1) * 2.0 ** -9
-        assert bool(((deq - gel).abs() <= gel.abs() * 2.0 ** -3 + step + 1.2 * TAU * S).all()), (N, K)
-
-
-def test_gemm_every_trunk_shape_against_fp64():
-    g = torch.Generator().manual_seed(17)
-    record = []
-    for (N, K) in TRUNK:
-        _run_case(EPIS[(N, K)], N, K, 300, g, record)  # 300 rows: a ragged last tile
-    for (N, K) in ((1024, 1024), (768, 3072)):  # the other epilogues on these shapes too
-        _run_case(EPI_ROPE, N if N % 192 == 0 else 768, K, 300, g, record)
-        _run_case(EPI_GELU_FP8, N, K, 300, g, record)
-    print("fp8 GEMM: max |err| / sum|a w| =", max(record), record)
-
-
-def test_gemm_split_k_small_problem():
-    g = torch.Generator().manual_seed(23)
-    M, N, K = 200, 1024, 4096
-    aq, as_, a64, wq, ws, w64 = _operands(M, N, K, g)
-    bias = torch.randn(N, generator=g) * 0.1
-    ref, S = _ref_and_bound(a64, w64, bias)
-    aqd, asd, wqd, wsd, biasd = _dev(aq, as_, wq, ws, bias)
-    x = torch.zeros(M, N, device=DEV)
-    split = torch.zeros(8 * 256 * N, device=DEV)
-    _gemm(EPI_F32, aqd, asd, wqd, wsd, M, N, K, biasd, x, resid=x, ws_split=split)
-    torch.cuda.synchronize()
-    assert split.abs().sum().item() > 0, "the split-K route was not taken"
-    assert bool(((x.cpu().double() - ref).abs() <= TAU * S + 1e-30).all())
 
 
 @pytest.mark.parametrize("epi,N,K", [(EPI_ROPE, 3072, 1024), (EPI_F32, 1024, 1024), (EPI_GELU_FP8, 4096, 1024),
@@ -246,7 +111,7 @@ def test_block_is_bit_identical_at_any_tile_offset(epi, N, K):
                 return [x]
             if epi == EPI_ROPE:
                 o = torch.full((rows, N), float("nan"), device=DEV, dtype=torch.bfloat16)
-                _gemm(epi, a, sa, Wd, Wsd, rows, N, K, Bd, o, pos=P[:rows].contiguous())
+                _gemm(epi, a, sa, Wd, Wsd, rows, N, K, Bd, o, pos=P[:rows].contiguous(), rope_cols=2048)  # enc.qkv
                 return [o]
             q, s = torch.empty(rows, N, dtype=torch.uint8, device=DEV), torch.empty(rows, N // 128, device=DEV)
             _gemm(epi, a, sa, Wd, Wsd, rows, N, K, Bd, q, out_scale=s)

@@ -86,6 +86,7 @@ def lib():
     L.sta_missing_tensors.argtypes = [vp]
     L.sta_weight_arena.argtypes = [vp, POINTER(vp), POINTER(c_int64)]
     L.sta_mark_all_loaded.argtypes = [vp]
+    L.sta_weight_slot.argtypes = [vp, c_char_p, POINTER(vp), POINTER(c_int64), POINTER(vp)]
     L.sta_encode.argtypes = [vp, vp, i, i, i, i, vp, vp, vp]
     L.sta_decode.argtypes = [vp, vp, vp, vp, vp, i, i, POINTER(vp), POINTER(vp), vp]
     L.sta_head_pose.argtypes = [vp, vp, i, vp, vp, vp]

@@ -1351,6 +1351,22 @@ int sta_weight_arena(StaModel* m, void** ptr, int64_t* bytes) {
   *bytes = static_cast<int64_t>((m->arena_off + 255) & ~static_cast<size_t>(255));
   return 0;
 }
+int sta_weight_slot(StaModel* m, const char* name, void** data_out, int64_t* ld_out, float** scales_out) {
+  if (!m || !name || !data_out || !ld_out || !scales_out) {
+    set_last_error("sta_weight_slot: null argument");
+    return 2;
+  }
+  const auto it = m->slots.find(name);
+  if (it == m->slots.end()) {
+    set_last_error(std::string("sta_weight_slot: no slot named ") + name);
+    return 4;
+  }
+  const Slot& s = it->second;
+  *data_out = s.dst;
+  *ld_out = static_cast<int64_t>(s.ldd);
+  *scales_out = s.kind == PK_LINEAR_FP8 ? s.sdst : nullptr;
+  return 0;
+}
 int sta_mark_all_loaded(StaModel* m) {  // after the arena was filled by a broadcast from another rank
   if (!m) return 2;
   for (auto& kv : m->slots) kv.second.loaded = true;
