@@ -411,6 +411,19 @@ int sta_loop_detect(StaLoopDetector* d, int farthest_neighbor, int* n_out, int64
 int sta_loop_add_frames(StaLoopDetector* d, const void* frames_dev, int frames_is_f32, int F, int H, int W, void* stream);
 int sta_loop_detect_many(StaLoopDetector* d, int F, const int* farthest_host, int* n_out, int64_t* js_out,
                          double* sims_out, int cap_per_view, void* stream);
+/* The same over the frames of several detectors (SLAM sessions stepped together).  Frame f belongs to dets[f]; a
+ * detector's frames are consecutive and in its own order; all detectors share one StaVocab (refused before any launch
+ * otherwise).  Every per-frame result equals the detector's own sta_loop_add_frames / sta_loop_detect_many.
+ * sta_loop_add_frames_group: ORB over the F frames, one transform, one build CTA per frame and one append launch into
+ * each frame's own database; asynchronous.  sta_loop_detect_group: for the frames of the last group add of dets[0]
+ * (the same dets and F, no view added to them since), farthest_host[f] in [0, view index of frame f in its detector];
+ * one score and one detect launch over all rows, then the one host synchronisation; outputs as sta_loop_detect_many's.
+ * The ORB scratch, staging and result buffers of a group are dets[0]'s.  After a group detect, sta_loop_similarities
+ * is refused on its detectors until their own next detect. */
+int sta_loop_add_frames_group(StaLoopDetector* const* dets, int F, const void* frames_dev, int frames_is_f32,
+                              int H, int W, void* stream);
+int sta_loop_detect_group(StaLoopDetector* const* dets, int F, const int* farthest_host, int* n_out,
+                          int64_t* js_out, double* sims_out, int cap_per_view, void* stream);
 /* Test read-backs (synchronise): a view's vector (len -1 for None) and the last similarity row of the last detect (NaN
  * where either vector is None). */
 int sta_loop_view(StaLoopDetector* d, int view, int32_t* words_out, double* vals_out, int cap, int* len_out, void* stream);

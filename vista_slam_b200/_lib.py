@@ -161,6 +161,9 @@ def lib():
     L.sta_loop_add_frames.argtypes = [vp, vp, i, i, i, i, vp]
     L.sta_loop_detect_many.argtypes = [vp, i, POINTER(c_int), POINTER(c_int), POINTER(c_int64), POINTER(ctypes.c_double), i,
                                        vp]
+    L.sta_loop_add_frames_group.argtypes = [POINTER(vp), i, vp, i, i, i, vp]
+    L.sta_loop_detect_group.argtypes = [POINTER(vp), i, POINTER(c_int), POINTER(c_int), POINTER(c_int64),
+                                        POINTER(ctypes.c_double), i, vp]
     L.sta_loop_view.argtypes = [vp, i, POINTER(c_int32), POINTER(ctypes.c_double), i, POINTER(c_int), vp]
     L.sta_loop_similarities.argtypes = [vp, POINTER(ctypes.c_double), i, vp]
     L.sta_orb_scratch_bytes.argtypes = [i, i]

@@ -15,6 +15,11 @@
 // grid dimension, one transform over F x 4096 descriptor slots, one CTA per frame building its vector into a staging
 // slot, an append in frame order, then one score launch and one detect launch over F rows and one host
 // synchronisation: the read-back of the candidate lists.  Every per-frame result is independent of F.
+//
+// A group call (sta_loop_add_frames_group / sta_loop_detect_group) runs that path over the frames of several detectors
+// that share one vocabulary, frame f belonging to dets[f]: ORB, transform and build over all frames in dets[0]'s
+// workspace, then the append, score and detect launches read per row a GroupRow (mapped pinned memory) naming the row's
+// database, view and loop parameters.  Every per-frame result is the one of the detector's own calls.
 #include "../../include/sta_b200.h"
 #include "common.cuh"
 #include "host_util.h"
@@ -340,6 +345,16 @@ int upload_vocab(const HostVocab& v, const std::vector<int>& order, StaVocab** o
   return 0;
 }
 
+// Row f of a group call: the database of frame f's detector, the view the frame becomes there, the batch index of that
+// detector's first frame, and its detect_loop parameters.
+struct GroupRow {
+  int* db_word;
+  double* db_val;
+  long long* db_start;
+  int* db_len;
+  int view, first, dist_min, nms, thresh_neighbor;
+};
+
 // Vocabulary::transform(feature, word_id, weight): one thread per descriptor
 // blockIdx.y = frame of a batch: its descriptors and outputs are kOrbMaxKeypoints slots after the previous frame's,
 // its count n_dev[f].
@@ -436,20 +451,32 @@ __device__ long long db_end(const long long* db_start, const int* db_len, int v)
   return db_start[v] + (db_len[v] > 0 ? db_len[v] : 0);
 }
 
-// Appends the F staged vectors to the database in frame order (one CTA per frame); views view0 .. view0 + F - 1.
+// Appends the F staged vectors to the database in frame order (one CTA per frame); views view0 .. view0 + F - 1.  With
+// rows (a group call), frame f goes to rows[f]'s database as view rows[f].view, after the frames of its detector that
+// precede it in the batch.
 __global__ void append_kernel(const int* stage_word, const double* stage_val, const int* stage_len, int view0,
-                              int* db_word, double* db_val, long long* db_start, int* db_len) {
+                              int* db_word, double* db_val, long long* db_start, int* db_len, const GroupRow* rows) {
   const int f = blockIdx.x;
+  int first = 0;
+  if (rows) {
+    const GroupRow r = rows[f];
+    db_word = r.db_word;
+    db_val = r.db_val;
+    db_start = r.db_start;
+    db_len = r.db_len;
+    first = r.first;
+    view0 = r.view - (f - first);
+  }
   long long base = view0 > 0 ? db_end(db_start, db_len, view0 - 1) : 0;
-  for (int g = 0; g < f; ++g) base += stage_len[g] > 0 ? stage_len[g] : 0;
+  for (int g = first; g < f; ++g) base += stage_len[g] > 0 ? stage_len[g] : 0;
   const int len = stage_len[f];
   for (int k = threadIdx.x; k < len; k += blockDim.x) {
     db_word[base + k] = stage_word[static_cast<long long>(f) * kOrbMaxKeypoints + k];
     db_val[base + k] = stage_val[static_cast<long long>(f) * kOrbMaxKeypoints + k];
   }
   if (threadIdx.x == 0) {
-    db_start[view0 + f] = base;
-    db_len[view0 + f] = len;
+    db_start[view0 + f - first] = base;
+    db_len[view0 + f - first] = len;
   }
 }
 
@@ -474,12 +501,25 @@ __device__ double l1_score(const int* aw, const double* av, int na, const int* b
 }
 
 // Row y = blockIdx.y: query y (length q_len[y], at entry q_start[y] of qw / qv, or 0 without q_start) against views
-// [0, i0 + y), one thread per view, into sims + y stride.
+// [0, i0 + y), one thread per view, into sims + y stride.  With rows (a group call), row y is view rows[y].view of
+// rows[y]'s database against the earlier views of that database.
 __global__ void score_kernel(const int* qw, const double* qv, const long long* q_start, const int* q_len,
                              const int* db_word, const double* db_val, const long long* db_start, const int* db_len,
-                             int i0, double* sims, long long stride) {
+                             int i0, double* sims, long long stride, const GroupRow* rows) {
   const int y = blockIdx.y;
   const int j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (rows) {
+    __shared__ GroupRow row;
+    if (threadIdx.x == 0) row = rows[y];
+    __syncthreads();
+    const int i = row.view;
+    if (j >= i) return;
+    const long long* st = row.db_start;
+    const int* ln = row.db_len;
+    sims[y * stride + j] = l1_score(row.db_word + st[i], row.db_val + st[i], ln[i], row.db_word + st[j],
+                                    row.db_val + st[j], ln[j]);
+    return;
+  }
   if (j >= i0 + y) return;
   const long long qa = q_start ? q_start[y] : 0;
   sims[y * stride + j] = l1_score(qw + qa, qv + qa, q_len[y], db_word + db_start[j], db_val + db_start[j], db_len[j]);
@@ -525,15 +565,31 @@ __device__ void detect_row(const double* sims, const int* db_len, int i, int far
 }
 
 // One thread per row f (view i0 + f): out row f = {ORB overflow flag of frame f, then detect_row's count, length and
-// pairs}, `out_stride` entries apart; after the gridDim.x rows, the database entries in use.
+// pairs}, `out_stride` entries apart; after the gridDim.x rows, the database entries in use.  With rows (a group call),
+// row f is view rows[f].view of rows[f]'s database with that row's parameters, and every row f writes its database's
+// entries in use at gridDim.x out_stride + f.
 __global__ void detect_kernel(const double* sims, long long sims_stride, const long long* db_start, const int* db_len,
                               int i0, const int* farthest, int dist_min, int nms, int thresh_neighbor, long long* out,
-                              long long out_stride, const unsigned* overflow, size_t overflow_stride) {
+                              long long out_stride, const unsigned* overflow, size_t overflow_stride,
+                              const GroupRow* rows) {
   const int f = blockIdx.x;
+  int i = i0 + f;
+  if (rows) {
+    const GroupRow r = rows[f];
+    db_start = r.db_start;
+    db_len = r.db_len;
+    i = r.view;
+    dist_min = r.dist_min;
+    nms = r.nms;
+    thresh_neighbor = r.thresh_neighbor;
+  }
   long long* row = out + f * out_stride;
-  detect_row(sims + f * sims_stride, db_len, i0 + f, farthest[f], dist_min, nms, thresh_neighbor, row + 1);
+  detect_row(sims + f * sims_stride, db_len, i, farthest[f], dist_min, nms, thresh_neighbor, row + 1);
   row[0] = *reinterpret_cast<const unsigned*>(reinterpret_cast<const char*>(overflow) + f * overflow_stride);
-  if (f == static_cast<int>(gridDim.x) - 1) out[(f + 1) * out_stride] = db_end(db_start, db_len, i0 + f);
+  if (rows)
+    out[gridDim.x * out_stride + f] = db_end(db_start, db_len, i);
+  else if (f == static_cast<int>(gridDim.x) - 1)
+    out[(f + 1) * out_stride] = db_end(db_start, db_len, i);
 }
 
 }  // namespace
@@ -569,6 +625,14 @@ struct StaLoopDetector {
   double* db_val = nullptr;
   long long* db_start = nullptr;
   int* db_len = nullptr;
+  // Group calls of which this detector is dets[0]: the row table of the last group add (mapped host memory, read by its
+  // append, score and detect launches), that add's detectors per frame and each one's view count after it.
+  GroupRow* rows_pinned = nullptr;
+  int rows_cap = 0;
+  std::vector<StaLoopDetector*> group_dets;
+  std::vector<int> group_views;
+  bool group_pending = false;   // the last group add's append may still read rows_pinned (no group detect since)
+  bool group_detected = false;  // this detector's last detect was a group detect: sta_loop_similarities is refused
 };
 
 namespace {
@@ -673,6 +737,42 @@ int grow_batch(StaLoopDetector* d, int F, cudaStream_t st) {
   return 0;
 }
 
+// sims / result / pinned of at least `need` entries
+int grow_results(StaLoopDetector* d, long long need, cudaStream_t st) {
+  if (need <= d->out_cap) return 0;
+  long long cap = d->out_cap ? 2 * d->out_cap : 1LL << 14;
+  while (cap < need) cap *= 2;
+  if (grow(&d->sims, 0, cap, st) || grow(&d->result, 0, cap, st)) return 1;
+  if (d->pinned) cudaFreeHost(d->pinned);
+  d->pinned = nullptr;
+  STA_CHECK_CUDA(cudaMallocHost(&d->pinned, sizeof(long long) * cap));
+  d->out_cap = cap;
+  return 0;
+}
+
+// The ORB overflow of a batch's frames as the error of its first such frame (after the read-back of a detect)
+int report_overflow(const long long* pinned, int F, long long out_stride) {
+  for (int f = 0; f < F; ++f) {
+    if (pinned[f * out_stride]) {
+      set_last_error((F == 1 ? std::string("the frame") : "frame " + std::to_string(f) + " of the batch") +
+                     " has more ORB candidates or keypoints than the detector holds");
+      return 1;
+    }
+  }
+  return 0;
+}
+
+// One detect row's results from the pinned read-back into n_out / js_out / sims_out (host)
+void copy_row(const long long* row, int f, int* n_out, int64_t* js_out, double* sims_out, int cap_per_view) {
+  const int n = static_cast<int>(row[1]);
+  n_out[2 * f] = n;
+  n_out[2 * f + 1] = static_cast<int>(row[2]);
+  for (int k = 0; k < n && k < cap_per_view; ++k) {
+    js_out[static_cast<long long>(f) * cap_per_view + k] = row[3 + 2 * k];
+    memcpy(&sims_out[static_cast<long long>(f) * cap_per_view + k], &row[4 + 2 * k], sizeof(double));
+  }
+}
+
 }  // namespace
 
 extern "C" {
@@ -750,7 +850,7 @@ int sta_op_bow_score(const int32_t* qw, const double* qv, const int32_t* q_len_d
   if (nviews)
     score_kernel<<<(nviews + 127) / 128, 128, 0, static_cast<cudaStream_t>(stream)>>>(
         qw, qv, nullptr, q_len_dev, db_word, db_val, reinterpret_cast<const long long*>(db_start), db_len, nviews,
-        sims_out, 0);
+        sims_out, 0, nullptr);
   STA_CHECK_CUDA(cudaGetLastError());
   return 0;
 }
@@ -782,6 +882,7 @@ void sta_loop_destroy(StaLoopDetector* d) {
   cudaFree(d->stage_len);
   if (d->pinned) cudaFreeHost(d->pinned);
   if (d->farthest_pinned) cudaFreeHost(d->farthest_pinned);
+  if (d->rows_pinned) cudaFreeHost(d->rows_pinned);
   delete d;
 }
 
@@ -802,7 +903,7 @@ int sta_loop_add_frames(StaLoopDetector* d, const void* frames_dev, int frames_i
   build_kernel<<<F, kBuildThreads, 0, st>>>(b.word, b.weight, b.count, 0, d->vocab->weighting, d->stage_word,
                                             d->stage_val, d->stage_len);
   append_kernel<<<F, 256, 0, st>>>(d->stage_word, d->stage_val, d->stage_len, d->views, d->db_word, d->db_val,
-                                   d->db_start, d->db_len);
+                                   d->db_start, d->db_len, nullptr);
   STA_CHECK_CUDA(cudaGetLastError());
   d->views += F;
   d->entries_bound += static_cast<long long>(F) * kOrbMaxKeypoints;
@@ -832,52 +933,29 @@ int sta_loop_detect_many(StaLoopDetector* d, int F, const int* farthest_host, in
   d->last_stream = st;
   const long long sims_stride = d->views, out_stride = 3 + 2LL * d->views;  // out_stride > sims_stride
   const long long need = F * out_stride + 1;
-  if (need > d->out_cap) {
-    long long cap = d->out_cap ? 2 * d->out_cap : 1LL << 14;
-    while (cap < need) cap *= 2;
-    if (grow(&d->sims, 0, cap, st) || grow(&d->result, 0, cap, st)) return 1;
-    if (d->pinned) cudaFreeHost(d->pinned);
-    d->pinned = nullptr;
-    STA_CHECK_CUDA(cudaMallocHost(&d->pinned, sizeof(long long) * cap));
-    d->out_cap = cap;
-  }
+  if (grow_results(d, need, st)) return 1;
+  d->group_detected = false;
   memcpy(d->farthest_pinned, farthest_host, sizeof(int) * F);  // the previous detect has synchronised
   const int i_last = d->views - 1;
   if (i_last > 0)
     score_kernel<<<dim3((i_last + 127) / 128, F), 128, 0, st>>>(d->db_word, d->db_val, d->db_start + i0, d->db_len + i0,
                                                                  d->db_word, d->db_val, d->db_start, d->db_len, i0,
-                                                                 d->sims, sims_stride);
+                                                                 d->sims, sims_stride, nullptr);
   const int first_slice = d->last_batch - F;  // scratch slice of row 0
   detect_kernel<<<F, 1, 0, st>>>(d->sims, sims_stride, d->db_start, d->db_len, i0, d->farthest_pinned, d->dist_min,
                                  d->nms, d->thresh_neighbor, d->result, out_stride,
                                  reinterpret_cast<const unsigned*>(static_cast<char*>(d->scratch) +
                                                                    first_slice * d->lay.total + d->lay.counters +
                                                                    3 * sizeof(unsigned)),
-                                 d->lay.total);
+                                 d->lay.total, nullptr);
   STA_CHECK_CUDA(cudaGetLastError());
   d->last_row = (F - 1) * sims_stride;
   d->last_row_len = i_last;
   STA_CHECK_CUDA(cudaMemcpyAsync(d->pinned, d->result, sizeof(long long) * need, cudaMemcpyDeviceToHost, st));
   STA_CHECK_CUDA(cudaStreamSynchronize(st));
   d->entries_bound = d->pinned[F * out_stride];
-  for (int f = 0; f < F; ++f) {
-    const long long* row = d->pinned + f * out_stride;
-    if (row[0]) {
-      set_last_error((F == 1 ? std::string("the frame") : "frame " + std::to_string(f) + " of the batch") +
-                     " has more ORB candidates or keypoints than the detector holds");
-      return 1;
-    }
-  }
-  for (int f = 0; f < F; ++f) {
-    const long long* row = d->pinned + f * out_stride;
-    const int n = static_cast<int>(row[1]);
-    n_out[2 * f] = n;
-    n_out[2 * f + 1] = static_cast<int>(row[2]);
-    for (int k = 0; k < n && k < cap_per_view; ++k) {
-      js_out[static_cast<long long>(f) * cap_per_view + k] = row[3 + 2 * k];
-      memcpy(&sims_out[static_cast<long long>(f) * cap_per_view + k], &row[4 + 2 * k], sizeof(double));
-    }
-  }
+  if (report_overflow(d->pinned, F, out_stride)) return 1;
+  for (int f = 0; f < F; ++f) copy_row(d->pinned + f * out_stride, f, n_out, js_out, sims_out, cap_per_view);
   return 0;
 }
 
@@ -887,6 +965,117 @@ int sta_loop_detect(StaLoopDetector* d, int farthest_neighbor, int* n_out, int64
                     void* stream) {
   STA_REQUIRE(d && d->views > 0, "no view has been added");
   return sta_loop_detect_many(d, 1, &farthest_neighbor, n_out, js_out, sims_out, cap, stream);
+}
+
+// sta_loop_add_frames over the frames of several detectors: frame f belongs to dets[f], each detector's frames are
+// consecutive, and all share one vocabulary (refused before any launch otherwise).  ORB, transform and build run over
+// all F frames in dets[0]'s workspace; one append launch writes each frame into its own detector's database through
+// dets[0]'s row table.  Asynchronous, unless dets[0]'s previous group add has had no group detect yet: its append may
+// still read the row table, so the stream is synchronised before the table is rewritten.
+int sta_loop_add_frames_group(StaLoopDetector* const* dets, int F, const void* frames_dev, int frames_is_f32, int H,
+                              int W, void* stream) {
+  STA_REQUIRE(dets && frames_dev, "null argument");
+  STA_REQUIRE(F >= 1, "the frame count must be at least 1");
+  STA_REQUIRE(orb_size_ok(H, W), "ORB frame sides must be in [32, 4096]");
+  for (int f = 0; f < F; ++f) {
+    STA_REQUIRE(dets[f], "null detector");
+    STA_REQUIRE(dets[f]->vocab == dets[0]->vocab, "all detectors of a group must share one vocabulary");
+    if (f > 0 && dets[f] != dets[f - 1])
+      for (int g = 0; g < f - 1; ++g) STA_REQUIRE(dets[g] != dets[f], "a detector's frames must be consecutive");
+  }
+  StaLoopDetector* d0 = dets[0];
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (d0->group_pending && d0->last_stream) STA_CHECK_CUDA(cudaStreamSynchronize(d0->last_stream));
+  d0->group_pending = false;
+  if (prepare_frames(d0, F, H, W, st) || grow_batch(d0, F, st)) return 1;
+  if (F > d0->rows_cap) {
+    if (d0->rows_pinned) cudaFreeHost(d0->rows_pinned);
+    d0->rows_pinned = nullptr;
+    d0->rows_cap = 0;
+    STA_CHECK_CUDA(cudaMallocHost(&d0->rows_pinned, sizeof(GroupRow) * F));
+    d0->rows_cap = F;
+  }
+  for (int f = 0, e; f < F; f = e) {
+    for (e = f + 1; e < F && dets[e] == dets[f];) ++e;
+    if (reserve(dets[f], st, e - f)) return 1;
+  }
+  // the row table after every reserve, which may move a database
+  for (int f = 0, first = 0; f < F; ++f) {
+    if (f > 0 && dets[f] != dets[f - 1]) first = f;
+    StaLoopDetector* d = dets[f];
+    d0->rows_pinned[f] = {d->db_word, d->db_val, d->db_start, d->db_len, d->views + f - first, first,
+                          d->dist_min, d->nms, d->thresh_neighbor};
+  }
+  KpBufs b = kp_bufs(d0->kp, d0->frame_cap);
+  OrbOut o = {b.xy, b.level, b.pts, b.angle, b.resp, b.desc, b.count};
+  if (orb_run(d0->lay, d0->scratch, frames_dev, frames_is_f32, o, st, F)) return 1;
+  if (bow_of_descriptors(d0->vocab, b.desc, b.count, 0, b.word, b.weight, st, F)) return 1;
+  build_kernel<<<F, kBuildThreads, 0, st>>>(b.word, b.weight, b.count, 0, d0->vocab->weighting, d0->stage_word,
+                                            d0->stage_val, d0->stage_len);
+  append_kernel<<<F, 256, 0, st>>>(d0->stage_word, d0->stage_val, d0->stage_len, 0, nullptr, nullptr, nullptr, nullptr,
+                                   d0->rows_pinned);
+  STA_CHECK_CUDA(cudaGetLastError());
+  d0->group_pending = true;
+  for (int f = 0; f < F; ++f) {
+    StaLoopDetector* d = dets[f];
+    d->views++;
+    d->entries_bound += kOrbMaxKeypoints;
+    d->last_batch = 0;  // the frames' ORB state is in dets[0]'s scratch: the detector's own detect waits for its own add
+    d->last_stream = st;
+  }
+  d0->last_batch = 0;
+  d0->group_dets.assign(dets, dets + F);
+  d0->group_views.resize(F);
+  for (int f = 0; f < F; ++f) d0->group_views[f] = dets[f]->views;
+  return 0;
+}
+
+// sta_loop_detect_many over the rows of the last sta_loop_add_frames_group of dets[0], with the same dets and F and no
+// view added to any of them since: one score launch and one detect launch over all rows, each against its own
+// database with its own detector's parameters, then one read-back, which also brings every detector's entry count.
+// The outputs are laid out as sta_loop_detect_many's.  Afterwards sta_loop_similarities is refused on these detectors
+// until their own next detect.
+int sta_loop_detect_group(StaLoopDetector* const* dets, int F, const int* farthest_host, int* n_out, int64_t* js_out,
+                          double* sims_out, int cap_per_view, void* stream) {
+  STA_REQUIRE(dets && dets[0] && farthest_host && n_out && (cap_per_view == 0 || (js_out && sims_out)), "null argument");
+  STA_REQUIRE(cap_per_view >= 0, "bad capacity");
+  StaLoopDetector* d0 = dets[0];
+  STA_REQUIRE(F >= 1 && F == static_cast<int>(d0->group_dets.size()),
+              "F must be the frame count of the last group add of dets[0]");
+  int max_view = 0;
+  for (int f = 0; f < F; ++f) {
+    STA_REQUIRE(dets[f] == d0->group_dets[f] && dets[f]->views == d0->group_views[f],
+                "the detectors must be those of the last group add of dets[0], with no view added since");
+    const int i = d0->rows_pinned[f].view;
+    STA_REQUIRE(farthest_host[f] >= 0 && farthest_host[f] <= i, "farthest_neighbor must be in [0, view index]");
+    max_view = i > max_view ? i : max_view;
+  }
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const long long sims_stride = max_view + 1, out_stride = 3 + 2LL * (max_view + 1);  // out_stride > sims_stride
+  const long long need = F * out_stride + F;
+  if (grow_results(d0, need, st)) return 1;
+  memcpy(d0->farthest_pinned, farthest_host, sizeof(int) * F);  // every earlier detect has synchronised
+  if (max_view > 0)
+    score_kernel<<<dim3((max_view + 127) / 128, F), 128, 0, st>>>(nullptr, nullptr, nullptr, nullptr, nullptr, nullptr,
+                                                                   nullptr, nullptr, 0, d0->sims, sims_stride,
+                                                                   d0->rows_pinned);
+  detect_kernel<<<F, 1, 0, st>>>(d0->sims, sims_stride, nullptr, nullptr, 0, d0->farthest_pinned, 0, 0, 0, d0->result,
+                                 out_stride,
+                                 reinterpret_cast<const unsigned*>(static_cast<char*>(d0->scratch) + d0->lay.counters +
+                                                                   3 * sizeof(unsigned)),
+                                 d0->lay.total, d0->rows_pinned);
+  STA_CHECK_CUDA(cudaGetLastError());
+  STA_CHECK_CUDA(cudaMemcpyAsync(d0->pinned, d0->result, sizeof(long long) * need, cudaMemcpyDeviceToHost, st));
+  STA_CHECK_CUDA(cudaStreamSynchronize(st));
+  d0->group_pending = false;
+  for (int f = 0; f < F; ++f) {
+    dets[f]->group_detected = true;
+    dets[f]->last_stream = st;
+    if (f == F - 1 || dets[f + 1] != dets[f]) dets[f]->entries_bound = d0->pinned[F * out_stride + f];
+  }
+  if (report_overflow(d0->pinned, F, out_stride)) return 1;
+  for (int f = 0; f < F; ++f) copy_row(d0->pinned + f * out_stride, f, n_out, js_out, sims_out, cap_per_view);
+  return 0;
 }
 
 // Host copy of view `view`'s vector (synchronises): *len_out = -1 for None; up to cap entries are written.
@@ -910,7 +1099,9 @@ int sta_loop_view(StaLoopDetector* d, int view, int32_t* words_out, double* vals
 
 // Host copy of the last row of the last detect (NaN where a vector is None); n = that row's view index.
 int sta_loop_similarities(StaLoopDetector* d, double* sims_out, int n, void* stream) {
-  STA_REQUIRE(d && n >= 0 && n <= d->last_row_len, "bad count: n must be at most the view index of the last detect");
+  STA_REQUIRE(d, "null argument");
+  STA_REQUIRE(!d->group_detected, "the detector's last detect was a group detect, whose rows it does not keep");
+  STA_REQUIRE(n >= 0 && n <= d->last_row_len, "bad count: n must be at most the view index of the last detect");
   if (n == 0) return 0;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   STA_CHECK_CUDA(cudaMemcpyAsync(sims_out, d->sims + d->last_row, sizeof(double) * n, cudaMemcpyDeviceToHost, st));

@@ -13,7 +13,11 @@ Results are numerically the per-edge results of the reference sequence (the deco
 Across keyframes (OnlineSLAM.step_many): `add_views` encodes many views per sta_encode call, and
 `regress_keyframes_gated` runs the gated step over the candidate edges of many keyframes in chunks of up to 16 edges,
 one pose-confidence read-back per chunk.  Batch sizes change the GEMMs' split-K, so these outputs equal the per-keyframe
-ones within rounding, not bit for bit."""
+ones within rounding, not bit for bit.
+
+Across caches (SLAMSessions): `add_views_group` encodes the new views of several caches that share one STA in the same
+calls, and `regress_keyframes_gated_group` runs the gated step over keyframes of several caches, a chunk's edges mixing
+caches.  One cache through them launches exactly what add_views / regress_keyframes_gated launch."""
 import ctypes
 
 import torch
@@ -39,27 +43,13 @@ class KeyframeFrontend:
         """slam.py:142-151: encode one view (B = 1) and cache its features; returns the view index."""
         return self.add_views([image], [image_shape])[0]
 
-    @torch.no_grad()
     def add_views(self, images, image_shapes=None):
         """add_view for each image (1, 3, H, W) in order, all of one size, encoded B at a time with B N <= GRAPH_MAX_TOKENS
         (N = H W / 256 tokens; 41 views at 224 x 224), so every call is replayed as a CUDA graph.  Returns the view
         indices."""
         images = list(images)
-        if not images:
-            return []
-        H, W = int(images[0].shape[-2]), int(images[0].shape[-1])
-        if any(tuple(x.shape[-2:]) != (H, W) for x in images):
-            raise ValueError("all views of a batch must have the same size")
-        B = max(1, GRAPH_MAX_TOKENS // ((H // 16) * (W // 16)))
-        first = len(self.enc_features)
-        for c in range(0, len(images), B):
-            chunk = images[c:c + B]
-            x = torch.cat([t.reshape(1, *t.shape[-3:]) for t in chunk]) if len(chunk) > 1 else chunk[0]
-            feat, _ = self.frontend._encode_image(x, None if image_shapes is None else image_shapes[c], normalize=False)
-            for b in range(len(chunk)):
-                self.enc_features.append(feat[b:b + 1])
-                self.img_shapes.append((H, W))
-        return list(range(first, len(self.enc_features)))
+        shapes = [None] * len(images) if image_shapes is None else list(image_shapes)
+        return add_views_group([self], [images], [shapes])[0]
 
     @staticmethod
     def edge_chunks(items):
@@ -85,7 +75,6 @@ class KeyframeFrontend:
         """The gate's read-back: the candidates' pose confidences on the host."""
         return [float(c) for c in pconf.cpu()]
 
-    @torch.no_grad()
     def regress_keyframes_gated(self, items, rel_pose_thres):
         """regress_views_gated over the keyframes items = [(i, js), ...], chunk by chunk (edge_chunks): per chunk ONE
         sta_regress_pairs_begin over its edges, ONE read-back of their confidences, and one _finish for the survivors
@@ -96,27 +85,19 @@ class KeyframeFrontend:
         keyframe's device batch {pose [K,4,4], pose_conf [K], conf / depths [2,n,H,W], intri [n,3,3], conf_mean [2,n]})
         -- what OnlineSLAM._add_keyframe takes -- or None for an item without candidates.  A chunk runs when its first
         keyframe is asked for."""
-        items = [(i, list(js)) for i, js in items]
-        chunks = self.edge_chunks(items)
-        pad = len(chunks) > 1
-        at = 0
-        for chunk in chunks:
-            for k in range(at, chunk[0]):
-                yield None
-            yield from self._regress_chunk([items[k] for k in chunk], rel_pose_thres, pad)
-            at = chunk[-1] + 1
-        for k in range(at, len(items)):
-            yield None
+        return regress_keyframes_gated_group([(self, i, js) for i, js in items], rel_pose_thres)
 
+    @torch.no_grad()
     def _regress_chunk(self, items, rel_pose_thres, pad):
-        edges = [(i, j) for i, js in items for j in js]
+        """One edge chunk of items = [(cache, i, js), ...], the caches sharing self's STA."""
+        edges = [(c, i, j) for c, i, js in items for j in js]
         K = MAX_EDGES if pad else len(edges)
         run = edges + [edges[-1]] * (K - len(edges))
-        H, W = self.img_shapes[edges[0][0]]
-        if any(self.img_shapes[v] != (H, W) for e in edges for v in e):
+        H, W = edges[0][0].img_shapes[edges[0][1]]
+        if any(c.img_shapes[v] != (H, W) for c, i, j in edges for v in (i, j)):
             raise ValueError("all views of a batch must have the same size")
-        fi = torch.cat([self.enc_features[i] for i, _ in run], dim=0)
-        fj = torch.cat([self.enc_features[j] for _, j in run], dim=0)
+        fi = torch.cat([c.enc_features[i] for c, i, _ in run], dim=0)
+        fj = torch.cat([c.enc_features[j] for c, _, j in run], dim=0)
         L = self.frontend._ready(fi)
         dev = fi.device
 
@@ -129,7 +110,7 @@ class KeyframeFrontend:
             _lib.check(L.sta_regress_pairs_begin(m._handle, _lib.ptr(fi), _lib.ptr(fj), K, H, W, _lib.ptr(pose),
                                                  _lib.ptr(pconf), _lib.cur_stream()), "sta_regress_pairs_begin")
             conf_host = self._read_confs(pconf[0, :len(edges)])  # the one host synchronisation of the chunk
-            keep = [e for e, (i, j) in enumerate(edges) if not (conf_host[e] < rel_pose_thres and i - j != 1)]
+            keep = [e for e, (_, i, j) in enumerate(edges) if not (conf_host[e] < rel_pose_thres and i - j != 1)]
             n = len(keep)
             if n:
                 conf, depth = f32(2, n, H, W), f32(2, n, H, W)
@@ -139,7 +120,7 @@ class KeyframeFrontend:
                                                       _lib.ptr(depth), _lib.ptr(cmean), _lib.ptr(_scratch_for(dev, 2 * n)),
                                                       _lib.cur_stream()), "sta_regress_pairs_finish")
         e0 = p0 = 0
-        for i, js in items:
+        for _, i, js in items:
             e1 = e0 + len(js)
             kf_keep = [e - e0 for e in keep if e0 <= e < e1]
             p1 = p0 + len(kf_keep)
@@ -204,7 +185,7 @@ class KeyframeFrontend:
         js = list(js)
         if not js:
             return []
-        (_, keep, b), = self._regress_chunk([(i, js)], rel_pose_thres, pad=False)
+        (_, keep, b), = self._regress_chunk([(self, i, js)], rel_pose_thres, pad=False)
         out = [(b["pose"][k:k + 1], b["pose_conf"][k:k + 1], None, None, None) for k in range(len(js))]
         for p, k in enumerate(keep):
             out[k] = out[k][:2] + (b["conf"][:, p], b["intri"][p], b["depths"][:, p])
@@ -216,3 +197,52 @@ class KeyframeFrontend:
         (pose_ij [1,4,4], rel_pose_conf_ij [1], confs [2,H,W], intri [3,3], depths [2,H,W])."""
         r = self.regress_views(i, [j])
         return r["pose"], r["pose_conf"], r["conf"][:, 0], r["intri"][0], r["depths"][:, 0]
+
+
+@torch.no_grad()
+def add_views_group(caches, images_per_cache, shapes_per_cache=None):
+    """KeyframeFrontend.add_views for several caches that share one STA, as one sequence of encoder calls: the new views
+    of all caches in order (cache by cache), all of one size, B at a time as add_views chunks them, each feature
+    appended to its own cache.  Returns each cache's new view indices."""
+    caches = list(caches)
+    images = [list(x) for x in images_per_cache]
+    shapes = [[None] * len(x) for x in images] if shapes_per_cache is None else [list(x) for x in shapes_per_cache]
+    if any(c.frontend is not caches[0].frontend for c in caches):
+        raise ValueError("the caches of a group must share one STA")
+    flat = [(c, im, sh) for c, ims, shs in zip(caches, images, shapes) for im, sh in zip(ims, shs)]
+    firsts = [c.view_num for c in caches]
+    if flat:
+        H, W = int(flat[0][1].shape[-2]), int(flat[0][1].shape[-1])
+        if any(tuple(im.shape[-2:]) != (H, W) for _, im, _ in flat):
+            raise ValueError("all views of a batch must have the same size")
+        B = max(1, GRAPH_MAX_TOKENS // ((H // 16) * (W // 16)))
+        for c0 in range(0, len(flat), B):
+            chunk = flat[c0:c0 + B]
+            x = torch.cat([im.reshape(1, *im.shape[-3:]) for _, im, _ in chunk]) if len(chunk) > 1 else chunk[0][1]
+            feat, _ = caches[0].frontend._encode_image(x, chunk[0][2], normalize=False)
+            for b, (c, _, _) in enumerate(chunk):
+                c.enc_features.append(feat[b:b + 1])
+                c.img_shapes.append((H, W))
+    return [list(range(f, c.view_num)) for f, c in zip(firsts, caches)]
+
+
+def regress_keyframes_gated_group(items, rel_pose_thres):
+    """KeyframeFrontend.regress_keyframes_gated over keyframes items = [(cache, i, js), ...] of several caches that share
+    one STA: the same chunks of at most MAX_EDGES edges (a keyframe never split, padded when there is more than one
+    chunk), a chunk's edges mixing caches, one confidence read-back per chunk.  A generator with the same yields, per
+    item in order."""
+    items = [(c, i, list(js)) for c, i, js in items]
+    if any(c.frontend is not items[0][0].frontend for c, _, _ in items):
+        raise ValueError("the caches of a group must share one STA")
+    chunks = KeyframeFrontend.edge_chunks([(i, js) for _, i, js in items])
+    pad = len(chunks) > 1
+    at = 0
+    for chunk in chunks:
+        # a keyframe without candidates may sit between two of a chunk's keyframes (another session's first view)
+        members = set(chunk)
+        results = items[chunk[0]][0]._regress_chunk([items[k] for k in chunk], rel_pose_thres, pad)
+        for k in range(at, chunk[-1] + 1):
+            yield next(results) if k in members else None
+        at = chunk[-1] + 1
+    for k in range(at, len(items)):
+        yield None

@@ -4,8 +4,9 @@
 the DBoW3 vocabulary transform and L1 scores against the earlier keyframes -- but runs ORB (csrc/orb.cu) and the
 bag-of-words transform, database and scoring (csrc/bow.cu) as CUDA kernels, with one host synchronisation per call: the
 read-back of the candidate list.  `detect_loops(images, farthest_neighbors)` does the same for many frames of one size
-with one host synchronisation for all of them.  The frame may stay on the device from SLAM_image_only.process_image.  There is no CPU
-path.
+with one host synchronisation for all of them, and `detect_loops_group(detectors, ...)` for the frames of several detectors
+that share one `Vocabulary` (SLAM sessions stepped together).  The frame may stay on the device from
+SLAM_image_only.process_image.  There is no CPU path.
 
 The vocabulary is a DBoW3 text file (what the shipped configs name, e.g. pretrains/ORBvoc.txt) or a DBoW3 binary file,
 plain or QuickLZ-compressed, with binary descriptors and L1 scoring."""
@@ -55,7 +56,8 @@ class BowVector:
 
 class LoopDetector:
     def __init__(self, vocab_path, loop_dist_min, loop_nms, loop_cand_thresh_neighbor):
-        self.vocab = Vocabulary(vocab_path)
+        """vocab_path: a vocabulary file, or a loaded Vocabulary that several detectors share."""
+        self.vocab = vocab_path if isinstance(vocab_path, Vocabulary) else Vocabulary(vocab_path)
         self.bow_feats = []
         self.loop_dist_min = loop_dist_min            # if node i has a loop edge to node j, then |i-j| > loop_dist_min
         self.loop_nms = loop_nms                      # non-maximum suppression for loop closure
@@ -150,7 +152,7 @@ class LoopDetector:
 
     def similarities(self):
         """fp64 scores of the newest view against every earlier one from the last detect_loop (NaN where either
-        vector is None)."""
+        vector is None).  Refused after a detect_loops_group, until this detector's own next detection."""
         i = len(self.bow_feats) - 1
         out = np.zeros(max(i, 0), np.float64)
         if i > 0:
@@ -176,6 +178,66 @@ class LoopDetector:
                                                 vals.ctypes.data_as(ctypes.POINTER(ctypes.c_double)), max(n, 0),
                                                 ctypes.byref(ln), _lib.cur_stream()), "sta_loop_view")
         return words, vals
+
+
+def detect_loops_group(detectors, images_per_detector, farthest_per_detector):
+    """detect_loops on each detector with its own images and farthest neighbours, as one batch over all of them: ORB,
+    the transform and the appends over every frame, one score and one detect launch over all rows and ONE host
+    synchronisation.  The detectors must be distinct and share one Vocabulary, and all frames one size and type; a
+    detector may have no frame.  Refusals come before any launch.  Returns, per detector, its list of candidate lists."""
+    detectors = list(detectors)
+    images = [list(x) for x in images_per_detector]
+    far = [[int(f) for f in x] for x in farthest_per_detector]
+    if not (len(images) == len(far) == len(detectors)):
+        raise ValueError("one image list and one farthest_neighbor list per detector")
+    if len({id(d) for d in detectors}) != len(detectors):
+        raise ValueError("a detector appears twice in the group")
+    if any(d.vocab is not detectors[0].vocab for d in detectors):
+        raise ValueError("all detectors of a group must share one Vocabulary")
+    owners = []
+    for k, (det, ims, fs) in enumerate(zip(detectors, images, far)):
+        if len(ims) != len(fs):
+            raise ValueError("one farthest_neighbor per image (detector %d)" % k)
+        i0 = len(det.bow_feats)
+        for f, x in enumerate(fs):
+            if not 0 <= x <= i0 + f:
+                raise ValueError("farthest_neighbor of frame %d of detector %d must be in [0, %d]" % (f, k, i0 + f))
+        owners += [k] * len(ims)
+    out = [[] for _ in detectors]
+    F = len(owners)
+    if F == 0:
+        return out
+    device = detectors[owners[0]]._device
+    frames = [_as_device_frame(im, device) for ims in images for im in ims]
+    if any(t.shape != frames[0][0].shape or k != frames[0][1] for t, k in frames):
+        raise ValueError("all frames of a batch must have the same size and type")
+    batch = torch.stack([t for t, _ in frames]).contiguous() if F > 1 else frames[0][0]
+    H, W = frames[0][0].shape
+    dets = (ctypes.c_void_p * F)(*[detectors[k]._h.value for k in owners])
+    L = _lib.lib()
+    with torch.cuda.device(batch.device):
+        _lib.check(L.sta_loop_add_frames_group(dets, F, _lib.ptr(batch), frames[0][1], H, W, _lib.cur_stream()),
+                   "sta_loop_add_frames_group")
+    # the views are in the device databases from here on, so bow_feats gets their entries even if detection fails
+    first = {}
+    for k in sorted(set(owners)):
+        first[k] = len(detectors[k].bow_feats)
+        detectors[k].bow_feats.extend(BowVector(detectors[k], first[k] + f) for f in range(len(images[k])))
+    n = (ctypes.c_int * (2 * F))()
+    cap = max(max(len(detectors[k].bow_feats) for k in owners) - 1, 1)
+    js = (ctypes.c_int64 * (F * cap))()
+    sims = (ctypes.c_double * (F * cap))()
+    fars = [x for fs in far for x in fs]
+    with torch.cuda.device(device):
+        _lib.check(L.sta_loop_detect_group(dets, F, (ctypes.c_int * F)(*fars), n, js, sims, cap, _lib.cur_stream()),
+                   "sta_loop_detect_group")
+    for f, k in enumerate(owners):
+        det = detectors[k]
+        view = first[k] + len(out[k])
+        if n[2 * f + 1] < 0:
+            det.bow_feats[view] = None
+        out[k].append([(int(js[f * cap + c]), float(sims[f * cap + c])) for c in range(n[2 * f])])
+    return out
 
 
 def orb_detect_and_compute(gray):

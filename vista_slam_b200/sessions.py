@@ -1,0 +1,181 @@
+"""Several OnlineSLAM sessions stepped together on one GPU, sharing one STA frontend and one loop-closure vocabulary.
+
+An evaluation that runs a list of scenes, or a server that runs SLAM for several cameras, holds one session per
+sequence.  On its own, each OnlineSLAM loads its own copy of the checkpoint and of the vocabulary, and a keyframe at a
+time leaves most of the GPU idle.  `SLAMSessions` loads both once, and `step({k: [value, ...], ...})` runs the new
+keyframes of every named session through one batched frontend pass:
+
+  * one sequence of encoder calls over all new views (keyframe.add_views_group);
+  * one loop-detection pass over all their frames with one read-back (loop_detector.detect_loops_group);
+  * the gated edge regression in chunks of at most 16 edges that mix sessions, one read-back per chunk
+    (keyframe.regress_keyframes_gated_group).
+
+Graph insertion and PGO stay per session, in the order step_many would run them.  A call leaves every session as
+`for k in sorted(values): sessions[k].step_many(values[k], force_pgo=k in force_pgo, ...)` would: the graph tables,
+host bookkeeping, loop candidates, gate decisions, PGO calls, written files and returned flags.  Frontend floats may
+differ from that loop within rounding, as step_many's differ from step's, because batch sizes change the GEMMs' split-K.
+
+Timing: each session's time_dict gets its share of the batched phases.  The wall time of the encoder calls and of the
+loop detection is split evenly across the sessions that have keyframes in the call; the time of an edge chunk's
+regression is split evenly across the sessions with keyframes in that chunk (added to their "decoder" and
+"graph_construction" buckets, as step_many counts the decoder inside graph construction).  Preparation, graph insertion
+and PGO are timed per session.
+
+All sessions run on the current CUDA device and stream.  The class is not thread-safe."""
+import operator
+import time
+
+import torch
+
+from .keyframe import KeyframeFrontend, add_views_group, regress_keyframes_gated_group
+from .loop_detector import Vocabulary, detect_loops_group
+from .slam import OnlineSLAM
+
+
+def _share(sessions, key, seconds):
+    for s in sessions:
+        s.time_dict[key] += seconds / len(sessions)
+
+
+class SLAMSessions:
+    def __init__(self, ckpt_path, vocab_path, num_sessions, frontend=None, **online_slam_kwargs):
+        """num_sessions OnlineSLAM sessions built with online_slam_kwargs.  The checkpoint at ckpt_path is loaded once,
+        or `frontend`, an already-built STA (e.g. STA(precision="fp8") with its weights loaded), is used instead.  The
+        vocabulary at vocab_path (or a loaded Vocabulary) is parsed and uploaded once; every session's LoopDetector
+        uses it."""
+        n = operator.index(num_sessions)
+        if n < 1:
+            raise ValueError("num_sessions must be at least 1")
+        self.vocab = vocab_path if isinstance(vocab_path, Vocabulary) else Vocabulary(vocab_path)
+        self.sessions = []
+        for _ in range(n):
+            model = frontend if frontend is not None else (self.sessions[0].frontend if self.sessions else ckpt_path)
+            self.sessions.append(self._new_session(model, online_slam_kwargs))
+        self.frontend = self.sessions[0].frontend
+
+    def _new_session(self, frontend, kwargs):
+        """One session on the shared frontend (a model or, for the first session, the checkpoint path)."""
+        return OnlineSLAM(frontend, self.vocab, **kwargs)
+
+    def __len__(self):
+        return len(self.sessions)
+
+    def __getitem__(self, k):
+        return self.sessions[k]
+
+    def _index(self, k):
+        try:
+            k = operator.index(k)
+        except TypeError:
+            raise ValueError("unknown session index %r" % (k,)) from None
+        if not 0 <= k < len(self.sessions):
+            raise ValueError("unknown session index %d (there are %d sessions)" % (k, len(self.sessions)))
+        return k
+
+    def _calls(self, values):
+        """[(k, [value, ...]), ...] sorted by session from a mapping or a sequence of (k, values) pairs."""
+        pairs = list(values.items()) if hasattr(values, "items") else [tuple(p) for p in values]
+        calls, seen = [], set()
+        for k, vs in pairs:
+            k = self._index(k)
+            if k in seen:
+                raise ValueError("session %d is named twice" % k)
+            seen.add(k)
+            calls.append((k, list(vs)))
+        return sorted(calls, key=lambda c: c[0])
+
+    def _detect_loops(self, sessions, grays, fars):
+        """Loop candidates of the sessions' new frames, per session: one detect_loops_group (one read-back)."""
+        return detect_loops_group([s.lc_detector for s in sessions], grays, fars)
+
+    def _regress_keyframes(self, items):
+        """The gated regression of items = [(session, i, js), ...] in edge chunks that mix sessions: per item in order,
+        what OnlineSLAM._regress_keyframes yields."""
+        return regress_keyframes_gated_group([(s.kf, i, js) for s, i, js in items], self.sessions[0].rel_pose_thres)
+
+    def step(self, values, force_pgo=(), log_intermediate_results=False, output_folders=None):
+        """Step sessions through new keyframes: values = {k: [value, ...], ...} (or (k, [value, ...]) pairs) names any
+        subset of the sessions; force_pgo holds the sessions whose last keyframe of the call forces a PGO;
+        output_folders = {k: folder} for log_intermediate_results.  Returns {k: [is_optimized, ...]}.
+
+        Refused with ValueError before any launch, with no session changed: an unknown or repeated session index,
+        keyframes of different sizes within the call, or a size other than a session's existing views.  A capacity
+        IndexError in one session propagates; every session is then left as a prefix of its own step_many would leave
+        it (the encoder caches and loop databases may hold later views of the call).  A non-orthonormal rotation
+        raises ValueError by the end of the call.
+
+        Host synchronisations: one for the loop candidates of all sessions, one per edge chunk, one per PGO iteration,
+        and one at the end of the call unless every session's flag has been read since its last graph launch."""
+        calls = self._calls(values)
+        force = {self._index(k) for k in force_pgo}
+        flags = {k: [] for k, _ in calls}
+        calls = [(k, vs) for k, vs in calls if vs]
+        if not calls:
+            return flags
+        size = tuple(calls[0][1][0]["rgb"].shape[-2:])
+        for k, vs in calls:
+            if any(tuple(v["rgb"].shape[-2:]) != size for v in vs):
+                raise ValueError("all keyframes of a call must have the same image size")
+            kf = self.sessions[k].kf
+            if kf.img_shapes and tuple(kf.img_shapes[0]) != size:
+                raise ValueError("the keyframes of session %d must have the size of its views" % k)
+        sess = [self.sessions[k] for k, _ in calls]
+        i0 = [s.view_num for s in sess]
+        for s, (_, vs) in zip(sess, calls):
+            t = time.time()
+            s._ensure_graph(vs[0]["rgb"])
+            if s.view_num == 0:
+                s._graph.pose[0].copy_(s._identity)
+            s.time_dict["prepare_data"] += time.time() - t
+
+        t = time.time()
+        add_views_group([s.kf for s in sess], [[v["rgb"] for v in vs] for _, vs in calls],
+                        [[v["shape"] for v in vs] for _, vs in calls])
+        _share(sess, "encoder", time.time() - t)
+
+        fars = [[max(0, i + m - s.neighbor_edge_num) for m in range(len(vs))] for s, i, (_, vs) in zip(sess, i0, calls)]
+        t = time.time()
+        loops = self._detect_loops(sess, [[v["gray"] for v in vs] for _, vs in calls], fars)  # read-back: candidates
+        _share(sess, "lc", time.time() - t)
+        for s in sess:
+            s._check_flags()
+
+        items, owner = [], []
+        for c, (s, i, (_, vs)) in enumerate(zip(sess, i0, calls)):
+            for m in range(len(vs)):
+                items.append((s, i + m, list(range(fars[c][m], i + m)) + [j for j, _ in loops[c][m][:s.loop_edge_num]]))
+                owner.append(c)
+        # the sessions of each item's edge chunk, which share the chunk's regression time
+        part = [[sess[c]] for c in owner]
+        for chunk in KeyframeFrontend.edge_chunks([(i, js) for _, i, js in items]):
+            members = [sess[c] for c in sorted({owner[t] for t in chunk})]
+            for t in chunk:
+                part[t] = members
+
+        checked = [True] * len(calls)
+        results = iter(self._regress_keyframes(items))
+        for t, (s, i, js) in enumerate(items):
+            c = owner[t]
+            k, vs = calls[c]
+            m = i - i0[c]
+            dec_start = time.time()
+            res = next(results)  # the first keyframe of an edge chunk runs the chunk: read-back of its gate
+            dt = time.time() - dec_start
+            _share(part[t], "decoder", dt)
+            _share(part[t], "graph_construction", dt)
+            graph_start = time.time()
+            s._check_flags()
+            s._register_keyframe(vs[m], i, js, res)
+            if js:
+                checked[c] = checked[c] and not res[1]
+            s.time_dict["graph_construction"] += time.time() - graph_start
+            folder = output_folders.get(k) if output_folders else None
+            flags[k].append(s._pgo_if_due(k in force and m == len(vs) - 1, log_intermediate_results, folder))
+            if flags[k][-1]:
+                checked[c] = s.num_nodes > 0 and s.num_edges > 0
+        if not all(checked):
+            torch.cuda.current_stream().synchronize()
+            for s, ok in zip(sess, checked):
+                if not ok:
+                    s._check_flags()
+        return flags

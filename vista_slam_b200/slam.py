@@ -182,6 +182,10 @@ class OnlineSLAM:
         self.time_dict = self._zero_times()
 
     def load_frontend(self, ckpt_path: str):
+        """The STA of the checkpoint at ckpt_path; an already-built STA passed in place of the path is used as it is
+        (SLAMSessions: sessions sharing one model)."""
+        if isinstance(ckpt_path, torch.nn.Module):
+            return ckpt_path
         from .sta_model.sta_model import SymmetricTwoViewAssociation as STA
         frontend = STA()
         checkpoint = torch.load(ckpt_path, map_location="cpu", weights_only=False)
@@ -367,12 +371,8 @@ class OnlineSLAM:
             res = next(results)  # the first keyframe of an edge chunk runs the chunk: read-back of its gate
             self.time_dict["decoder"] += time.time() - dec_start
             self._check_flags()
-            self.img_shapes.append(v["shape"])
-            self.imgs.append(v["rgb"].squeeze(0).detach())
-            self.view_names.append(v["view_name"])
-            self.view_num += 1
+            self._register_keyframe(v, i, js, res)
             if js:
-                self._insert_keyframe(i, js, *res)
                 checked = checked and not res[1]
             self.time_dict["graph_construction"] += time.time() - graph_start
             flags.append(self._pgo_if_due(force_pgo and k == n - 1, log_intermediate_results, output_folder))
@@ -382,6 +382,15 @@ class OnlineSLAM:
             torch.cuda.current_stream().synchronize()
             self._check_flags()
         return flags
+
+    def _register_keyframe(self, v, i, js, res):
+        """Keyframe i of step_many after its gate: the view's host lists, then its kept edges (_insert_keyframe)."""
+        self.img_shapes.append(v["shape"])
+        self.imgs.append(v["rgb"].squeeze(0).detach())
+        self.view_names.append(v["view_name"])
+        self.view_num += 1
+        if js:
+            self._insert_keyframe(i, js, *res)
 
     def pose_graph_optimize(self):
         """slam.py:108-140 through PoseGraphOpt on the device tables (per-edge weights: DESIGN.md §4)."""
