@@ -158,9 +158,15 @@ typedef struct StaGemmDesc {
   int64_t splitk_ws_bytes;
   int split_precision;  /* 1: operands are already expanded along K as A (hi|lo|hi) x W (hi|hi|lo) (K = 3x logical);
                            bf16 outputs / skip tensors use (hi|lo|hi) rows of logical width N (ldo >= 3N) */
+  int tile_n;           /* 0: automatic (sta_gemm_auto_tile_n);  128: 128 x 128 tiles;  256: 128 x 256 tiles (linear
+                           layers with the TMA-store epilogue, N % 256 == 0, no split-K, not split precision; an error
+                           elsewhere).  Both tile shapes give bit-identical results. */
 } StaGemmDesc;
 
 int sta_op_gemm(const StaGemmDesc* d, void* stream);
+/* The tile columns (256 or 128) the automatic choice takes for a linear layer (M x N, depth K) with epilogue epi that
+ * runs the TMA-store epilogue without split-K on a GPU with num_sms SMs.  A function of these arguments only. */
+int sta_gemm_auto_tile_n(int M, int N, int K, int epi, int num_sms);
 
 /* The FP8 mode's GEMM (STA_PRECISION_FP8): out = A W^T + bias on e4m3 codes ("fn" format, max 448) with power-of-two
  * scales: A [M][lda] with a_scale [M][K/128] (one per row and 128 columns), W [N][ldw] with w_scale [N/128][K/128] (one

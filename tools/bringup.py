@@ -527,6 +527,29 @@ def group_perf():
         torch.cuda.synchronize()
         return e0.elapsed_time(e1) / n
 
+    def tile_times(d, flop):
+        """Both tile shapes of a linear layer forced through tile_n (the automatic choice is the untagged time)."""
+        if d.N % 256 or d.conv3x3:
+            return ""
+        res = []
+        for tn in (128, 256):
+            d.tile_n = tn
+            ms = timeit(lambda: run_gemm(d))
+            res.append("tile_n %d %.3f ms = %.0f TFLOP/s" % (tn, ms, flop / ms / 1e9))
+        d.tile_n = 0
+        return "   [" + ", ".join(res) + "]"
+
+    # the cuBLAS kernel torch.matmul picks for the encoder's qkv shape (its name carries the tile shape)
+    A = torch.randn(24576, 1024, device=dev).bfloat16()
+    W = torch.randn(3072, 1024, device=dev).bfloat16()
+    torch.matmul(A, W.t())
+    torch.cuda.synchronize()
+    with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
+        torch.matmul(A, W.t())
+        torch.cuda.synchronize()
+    names = sorted({e.name for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA})
+    print("torch.matmul M24576 N3072 K1024 kernels:", names, flush=True)
+
     # trunk shapes, plus one grid of 200 tiles (between one and two tiles per SM on a 132-SM H100)
     for (M, N, K, epi) in [(24576, 3072, 1024, EPI_BF16), (24576, 4096, 1024, EPI_GELU), (24576, 1024, 4096, EPI_BF16),
                            (24576, 1024, 1024, EPI_BF16), (3200, 1024, 1024, EPI_BF16)]:
@@ -537,8 +560,9 @@ def group_perf():
         d = gemm_desc(epi=epi, A=A, lda=K, W=W, ldw=K, M=M, N=N, K=K, bias=bias, out=out, ldo=N)
         ms = timeit(lambda: run_gemm(d))
         ms_t = timeit(lambda: torch.matmul(A, W.t()))
-        print("gemm M%d N%d K%d epi%d: %.3f ms = %.0f TFLOP/s   (torch.matmul %.3f ms = %.0f TFLOP/s)" %
-              (M, N, K, epi, ms, 2.0 * M * N * K / ms / 1e9, ms_t, 2.0 * M * N * K / ms_t / 1e9), flush=True)
+        print("gemm M%d N%d K%d epi%d: %.3f ms = %.0f TFLOP/s   (torch.matmul %.3f ms = %.0f TFLOP/s)%s" %
+              (M, N, K, epi, ms, 2.0 * M * N * K / ms / 1e9, ms_t, 2.0 * M * N * K / ms_t / 1e9,
+               tile_times(d, 2.0 * M * N * K)), flush=True)
     # epilogue variants on the trunk shapes
     from vista_slam_b200._lib import EPI_F32, EPI_ROPE
     M = 24576
@@ -560,7 +584,8 @@ def group_perf():
             out = torch.zeros(M, N, device=dev, dtype=torch.bfloat16)
             d = gemm_desc(epi=epi, A=A, lda=K, W=W, ldw=K, M=M, N=N, K=K, bias=bias, out=out, ldo=N)
         ms = timeit(lambda: run_gemm(d))
-        print("gemm-epi %-22s M%d N%d K%d: %.3f ms = %.0f TFLOP/s" % (name, M, N, K, ms, 2.0 * M * N * K / ms / 1e9), flush=True)
+        print("gemm-epi %-22s M%d N%d K%d: %.3f ms = %.0f TFLOP/s%s" % (name, M, N, K, ms, 2.0 * M * N * K / ms / 1e9,
+                                                                       tile_times(d, 2.0 * M * N * K)), flush=True)
     # Per-tile fixed cost: time(K) = a + b K over a K sweep at a trunk shape.  a is what a tile costs besides its
     # k-blocks (epilogue, pipeline fill and drain) where it is not hidden behind another tile's MMAs; a / time(1024) is
     # its share of a K = 1024 layer.

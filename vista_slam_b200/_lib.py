@@ -31,6 +31,7 @@ class StaGemmDesc(Structure):
         ("head_w", c_void_p), ("head_b", c_void_p), ("pts3d", c_void_p), ("conf", c_void_p),
         ("splitk_ws", c_void_p), ("splitk_ws_bytes", c_int64),
         ("split_precision", c_int),
+        ("tile_n", c_int),
     ]
 
 

@@ -46,6 +46,43 @@ static int launch_inst(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUt
   return 0;
 }
 
+template <int EPI>
+static int launch_wide(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmC, const GemmParams& p,
+                       int num_tiles, cudaStream_t stream) {
+  using Cfg = GemmWideCfg<EPI>;
+  auto kern = gemm_wide_kernel<EPI>;
+  static PerDeviceOnce once;
+  STA_CHECK_CUDA(once.run(
+      [&] { return cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg::SMEM_BYTES); }));
+  const int items = num_tiles < num_sms() ? num_tiles : num_sms();
+  if (items < 1) return 0;
+  STA_CHECK_CUDA(launch_pdl(kern, dim3(items), dim3(Cfg::THREADS), Cfg::SMEM_BYTES, stream, 1, tmA, tmB, tmC, p));
+  return 0;
+}
+
+// Wave efficiency of a persistent grid: tiles over the tile slots of the waves it takes.
+static double wave_efficiency(long long tiles, int sms) {
+  const long long waves = (tiles + sms - 1) / sms;
+  return static_cast<double>(tiles) / static_cast<double>(waves * sms);
+}
+
+// The 128 x 256 kernel needs less shared-memory traffic per MAC than the 128 x 128 kernel, but its epilogue is not
+// hidden behind another tile's MMAs and it has half as many tiles.  Per-layer times at cfg-2 on the 700 W H100
+// (DESIGN.md section 5): it wins where the 128 x 128 kernel is bound by that traffic -- many column tiles (enc qkv
+// N = 3072: 0.301 -> 0.249 ms, enc fc1 N = 4096: 0.377 -> 0.330 ms, dec qkv N = 2304: 0.174 -> 0.153 ms) or a long k loop
+// (enc fc2 K = 4096: 0.376 -> 0.296 ms) -- and loses where both are short (enc proj N = K = 1024: 0.128 -> 0.134 ms).
+// So it is taken for N >= 2048 or K >= 2048, and only when its wave efficiency is at most 5 points below the 128 x 128
+// kernel's: the decoder's N = 768 layers (87.7 % against 97.5 % at M = 24608 on 132 SMs) and the one-keyframe SLAM
+// shapes (a few tiles on a mostly idle GPU) keep 128 x 128 tiles.
+int gemm_auto_tile_n(int M, int N, int K, int epi, int num_sms) {
+  if (M <= 0 || N % 256 != 0 || num_sms <= 0 || (N < 2048 && K < 2048)) return 128;
+  if (epi != EPI_BF16 && epi != EPI_GELU && epi != EPI_F32 && epi != EPI_ROPE) return 128;
+  const long long m_tiles = (M + 127) / 128;
+  const double wide = wave_efficiency(m_tiles * (N / 256), num_sms);
+  const double narrow = wave_efficiency(m_tiles * (N / 128), num_sms);
+  return wide >= narrow - 0.05 ? 256 : 128;
+}
+
 int launch_gemm(const GemmLaunch& g, cudaStream_t stream) {
   GemmParams p = g.p;
   const bool fp8 = g.amode == A_FP8;
@@ -101,6 +138,15 @@ int launch_gemm(const GemmLaunch& g, cudaStream_t stream) {
       if (ks >= 2 && need <= g.splitk_ws_bytes && (reinterpret_cast<uintptr_t>(g.splitk_ws) & 15) == 0) ksplit = ks;
     }
   }
+  // 128 x 256 tiles (gemm_wide_kernel) for the plain linear layers with the TMA-store epilogue
+  STA_REQUIRE(g.tile_n == 0 || g.tile_n == 128 || g.tile_n == 256, "tile_n must be 0, 128 or 256");
+  const bool wide_ok = tma && g.amode == A_LINEAR && !p.split && ksplit == 1 && p.N % 256 == 0 &&
+                       (g.epi == EPI_BF16 || g.epi == EPI_GELU || g.epi == EPI_F32 || g.epi == EPI_ROPE);
+  STA_REQUIRE(g.tile_n != 256 || wide_ok,
+              "tile_n = 256 needs a linear layer with the TMA-store epilogue, N % 256 == 0, no split-K and no "
+              "split precision");
+  const bool wide = wide_ok && (g.tile_n == 256 || (g.tile_n == 0 && gemm_auto_tile_n(p.M, p.N, p.K, g.epi, num_sms()) == 256));
+  const int bn_tile = wide ? 256 : bn;
   CUtensorMap tmA, tmB;
   int m_tiles;
   if (g.amode == A_CONV3) {
@@ -129,10 +175,10 @@ int launch_gemm(const GemmLaunch& g, cudaStream_t stream) {
     STA_REQUIRE(g.ldw * oes % 16 == 0, "ldw must be a multiple of 16 bytes");
     uint64_t dims[2] = {(uint64_t)p.K, (uint64_t)p.N};
     uint64_t strides[1] = {(uint64_t)g.ldw * oes};
-    uint32_t box[2] = {(uint32_t)bk, (uint32_t)bn};
+    uint32_t box[2] = {(uint32_t)bk, (uint32_t)bn_tile};
     if (make_tmap(&tmB, g.Wt, fp8 ? 2 : 0, 2, dims, strides, box)) return 1;
   }
-  const int n_tiles = (p.N + bn - 1) / bn;
+  const int n_tiles = (p.N + bn_tile - 1) / bn_tile;
   const int num_tiles = m_tiles * n_tiles * ksplit;
 
   CUtensorMap tmC = tmA;
@@ -162,6 +208,12 @@ int launch_gemm(const GemmLaunch& g, cudaStream_t stream) {
   STA_REQUIRE(tma || ksplit == 1, "split-K needs the TMA epilogue");
 
   int rc = -1;
+  if (wide) {
+    if (g.epi == EPI_GELU) rc = launch_wide<EPI_GELU>(tmA, tmB, tmC, p, num_tiles, stream);
+    else if (g.epi == EPI_F32) rc = launch_wide<EPI_F32>(tmA, tmB, tmC, p, num_tiles, stream);
+    else if (g.epi == EPI_ROPE) rc = launch_wide<EPI_ROPE>(tmA, tmB, tmC, p, num_tiles, stream);
+    else rc = launch_wide<EPI_BF16>(tmA, tmB, tmC, p, num_tiles, stream);
+  }
 #define STA_GEMM_CASE(AM_, EP_, TMA_) \
   if (rc < 0 && g.amode == AM_ && g.epi == EP_ && tma == TMA_) rc = launch_inst<AM_, EP_, TMA_>(tmA, tmB, tmC, p, num_tiles, stream);
 

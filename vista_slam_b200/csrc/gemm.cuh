@@ -892,4 +892,300 @@ gemm_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   }
 }
 
+// ---------------------------------------------------------------------------
+// Wide linear GEMM: 128 x 256 tiles, both consumer warpgroups on the same tile.
+//
+// Warpgroup g computes tile rows [64 g, 64 g + 64) x 256 columns with one m64n256k16 wgmma per k16 step.  Against the
+// 128 x 128 ping-pong kernel, a k16 step reads 2 x 2 KB of A and 8 KB of B from shared memory for 2 x 64 x 256 x 16 MACs
+// (instead of 2 x 2 KB + 2 x 4 KB for two 64 x 128 halves of half the columns per warpgroup), and TMA writes 48 KB per
+// k-block of 128 x 256 x 64 MACs instead of 32 KB per 128 x 128 x 64: the shared-memory traffic per MAC drops from about
+// 160 to 128 bytes per clock at full tensor rate, the SM's shared-memory bandwidth.  The price is that the epilogue is no
+// longer hidden behind the other warpgroup's mainloop; the producer keeps the ring filled meanwhile, so the next tile's
+// first k-blocks are waiting when it ends.
+//
+// Fragment: warp wq of warpgroup g, lane = 4 r + t holds in acc[4 j + 2 half + e] tile row 64 g + 16 wq + 8 half + r,
+// column 8 j + 2 t + e (j = 0..31).  Each output element sees the same k16 steps in the same order as in the 128 x 128
+// kernel, and the epilogue runs the same operations on it, so the two kernels give bit-identical results.
+// Linear layers only (A_LINEAR, not split-precision), TMA-store epilogue, N % 256 == 0, no split-K.
+// ---------------------------------------------------------------------------
+template <int EPI>
+struct GemmWideCfg {
+  static constexpr int BM = 128;
+  static constexpr int BN = 256;
+  static constexpr int BK = 64;
+  static constexpr uint32_t A_BYTES = BM * BK * 2;
+  static constexpr uint32_t B_BYTES = BN * BK * 2;
+  static constexpr uint32_t STAGE_BYTES = A_BYTES + B_BYTES;
+  static constexpr uint32_t BAR_BYTES = 256;
+  static constexpr int EPI_WARPS = 8;
+  static constexpr uint32_t PRODUCER_REGS = 40;
+  static constexpr uint32_t CONSUMER_REGS = 232;
+  static constexpr uint32_t TMA_BOX_BYTES = 16 * 128;
+  // Per-warp staging: two alternating 16-row x 128-byte boxes, or one with the RoPE table, which leaves room for a
+  // fourth ring stage (enc qkv at cfg-2 on the 700 W H100: 0.241 ms with 4 stages and one box, 0.254 ms with 3 and two).
+  static constexpr int STG_BOXES = (EPI == EPI_ROPE) ? 1 : 2;
+  static constexpr uint32_t STG_WARP_BYTES = STG_BOXES * TMA_BOX_BYTES;
+  static constexpr uint32_t STG_BYTES = EPI_WARPS * STG_WARP_BYTES;
+  static constexpr int ROPE_SMEM_ROWS = 64;
+  static constexpr uint32_t ROPE_SMEM_BYTES = (EPI == EPI_ROPE) ? ROPE_SMEM_ROWS * kRopeLd * sizeof(float) : 0;
+  static constexpr uint32_t MAX_SMEM = 227 * 1024;
+  static constexpr int STAGES_FIT = (MAX_SMEM - BAR_BYTES - STG_BYTES - ROPE_SMEM_BYTES) / STAGE_BYTES;
+  static constexpr int STAGES = STAGES_FIT > 4 ? 4 : STAGES_FIT;
+  // layout: operand ring (A tiles, then B tiles) | staging | barriers | RoPE
+  static constexpr uint32_t OFF_STG = STAGES * STAGE_BYTES;
+  static constexpr uint32_t OFF_BAR = OFF_STG + STG_BYTES;
+  static constexpr uint32_t OFF_ROPE = OFF_BAR + BAR_BYTES;
+  static constexpr uint32_t SMEM_BYTES = OFF_ROPE + ROPE_SMEM_BYTES;
+  static constexpr int THREADS = 128 + 32 * EPI_WARPS;
+  static constexpr int EPI_THREADS = 32 * EPI_WARPS;
+  static_assert(128 * PRODUCER_REGS + 256 * CONSUMER_REGS <= 64 * 1024, "register file");
+  static_assert(STAGES == 4 && 2 * STAGES * 8 <= BAR_BYTES, "ring");
+  static_assert(OFF_STG % 1024 == 0 && STG_WARP_BYTES % 1024 == 0, "SWIZZLE_128B boxes are 1024-byte aligned");
+  static_assert(SMEM_BYTES <= MAX_SMEM, "shared memory");
+};
+
+// TMA-store epilogue of one warp's 16 rows x 256 columns (EPI_BF16 / EPI_GELU / EPI_ROPE / EPI_F32): the operations of
+// epilogue_tile_tma, element for element, on the wide fragment.  A warp writes four bf16 boxes (64 columns each) or eight
+// fp32 boxes (32 columns each) per tile, through its staging boxes in turn.
+template <int EPI>
+__device__ __forceinline__ void epilogue_wide_tma(const GemmParams& p, const CUtensorMap* tmC, float (&acc)[128],
+                                                  int row0, int col0, uint8_t* stg, const float* rope_s, uint32_t& ubuf) {
+  using Cfg = GemmWideCfg<EPI>;
+  constexpr bool OUT_F32 = (EPI == EPI_F32);
+  const int lane = threadIdx.x & 31;
+  const int r = lane >> 2, t = lane & 3;
+
+#pragma unroll
+  for (int j = 0; j < 32; ++j) {
+    const float2 b = p.bias ? __ldg(reinterpret_cast<const float2*>(p.bias + col0 + 8 * j + 2 * t)) : make_float2(0.f, 0.f);
+    acc[4 * j] += b.x; acc[4 * j + 1] += b.y; acc[4 * j + 2] += b.x; acc[4 * j + 3] += b.y;
+  }
+  if constexpr (EPI == EPI_GELU) {
+#pragma unroll
+    for (int i = 0; i < 128; ++i) acc[i] = gelu_erf(acc[i]);
+  }
+  if constexpr (EPI == EPI_BF16) {
+    if (p.relu_main) {
+#pragma unroll
+      for (int i = 0; i < 128; ++i) acc[i] = fmaxf(acc[i], 0.0f);
+    }
+  }
+  [[maybe_unused]] uint32_t pyx[2];  // [half]: (pos_y + 1) | (pos_x + 1) << 16 of this thread's two token rows
+  [[maybe_unused]] bool staged = true;
+  if constexpr (EPI == EPI_ROPE) {
+#pragma unroll
+    for (int half = 0; half < 2; ++half) {
+      const int row = row0 + 8 * half + r;
+      pyx[half] = 0x00010001u;
+      if (row < p.M) {
+        const int2 pp = *reinterpret_cast<const int2*>(p.pos + 2 * static_cast<long long>(row));
+        if (pp.x < -1 || pp.x > p.rope_max_pos || pp.y < -1 || pp.y > p.rope_max_pos)
+          __trap();  // token position outside the RoPE table (no printf: see mbar_wait)
+        pyx[half] = static_cast<uint32_t>(pp.x + 1) | (static_cast<uint32_t>(pp.y + 1) << 16);
+      }
+      staged = staged && static_cast<int>(max(pyx[half] & 0xFFFFu, pyx[half] >> 16)) < p.rope_smem_rows;
+    }
+    staged = __all_sync(0xFFFFFFFFu, staged);
+  }
+  // RoPE of 32-column chunk q (fragment groups j = 4 q .. 4 q + 3; pair (i, i + 16) is j and j + 2), as in
+  // epilogue_tile_tma
+  auto rope_chunk = [&](int q) {
+    if constexpr (EPI == EPI_ROPE) {
+      if (col0 + 32 * q >= p.rope_cols) return;  // warp-uniform: the V columns are not rotated
+      auto rotate = [&](auto table_row) {
+#pragma unroll
+        for (int half = 0; half < 2; ++half) {
+          const int ps = static_cast<int>((q & 1) ? pyx[half] >> 16 : pyx[half] & 0xFFFFu);
+          const float4* tb = table_row(ps);
+#pragma unroll
+          for (int jj = 0; jj < 2; ++jj) {
+            const float4 tt = tb[4 * jj + t];
+            const int ia = 4 * (4 * q + jj) + 2 * half;
+            const int ib = ia + 8;
+            const float a0 = acc[ia], b0 = acc[ib], a1 = acc[ia + 1], b1 = acc[ib + 1];
+            acc[ia] = fmaf(-b0, tt.y, a0 * tt.x);
+            acc[ib] = fmaf(a0, tt.y, b0 * tt.x);
+            acc[ia + 1] = fmaf(-b1, tt.w, a1 * tt.z);
+            acc[ib + 1] = fmaf(a1, tt.w, b1 * tt.z);
+          }
+        }
+      };
+      if (staged) rotate([&](int ps) { return reinterpret_cast<const float4*>(rope_s + ps * kRopeLd); });
+      else rotate([&](int ps) { return reinterpret_cast<const float4*>(p.rope_tab + static_cast<long long>(ps) * 32); });
+    }
+  };
+
+  const uint32_t sb = smem_u32(stg);
+  const uint32_t sx = r;  // 128B swizzle: 16-byte chunk k of box row R lives at k ^ (R & 7), and R & 7 = r
+  auto next_box = [&]() -> uint32_t {
+    if constexpr (Cfg::STG_BOXES == 1) {
+      if (lane == 0) tma_store_wait_read();  // the store of the previous box is done reading it
+      __syncwarp();
+      return sb;
+    } else {
+      if (lane == 0) tma_store_wait_read1();  // the store that read this box two boxes ago is done with it
+      __syncwarp();
+      return sb + (ubuf++ & 1u) * Cfg::TMA_BOX_BYTES;
+    }
+  };
+  auto issue = [&](uint32_t box, int col) {
+    fence_proxy_async_smem();
+    __syncwarp();
+    if (lane == 0) {
+      const void* src = stg + (box - sb);
+      if constexpr (OUT_F32) {
+        if (p.c_reduce) tma_reduce_add_2d(tmC, src, col, row0);
+        else tma_store_2d(tmC, src, col, row0);
+      } else {
+        tma_store_2d(tmC, src, col, row0);
+      }
+      tma_store_commit();
+    }
+  };
+  if constexpr (OUT_F32) {
+#pragma unroll
+    for (int c = 0; c < 8; ++c) {  // box c: columns [32 c, 32 c + 32) = fragment groups j = 4 c .. 4 c + 3
+      const uint32_t box = next_box();
+#pragma unroll
+      for (int half = 0; half < 2; ++half)
+#pragma unroll
+        for (int jl = 0; jl < 4; ++jl) {
+          const int i = 4 * (4 * c + jl) + 2 * half;
+          asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(box + (8 * half + r) * 128 +
+                                                                 (((2 * jl + (t >> 1)) ^ sx) << 4) + (t & 1) * 8),
+                       "f"(acc[i]), "f"(acc[i + 1])
+                       : "memory");
+        }
+      issue(box, col0 + 32 * c);
+    }
+  } else {
+#pragma unroll
+    for (int c = 0; c < 4; ++c) {  // box c: columns [64 c, 64 c + 64) = fragment groups j = 8 c .. 8 c + 7
+      rope_chunk(2 * c);
+      rope_chunk(2 * c + 1);
+      const uint32_t box = next_box();
+#pragma unroll
+      for (int half = 0; half < 2; ++half)
+#pragma unroll
+        for (int jl = 0; jl < 8; ++jl) {
+          const int i = 4 * (8 * c + jl) + 2 * half;
+          asm volatile("st.shared.b32 [%0], %1;" ::"r"(box + (8 * half + r) * 128 + ((jl ^ sx) << 4) + 4 * t),
+                       "r"(pack_bf16x2(acc[i], acc[i + 1]))
+                       : "memory");
+        }
+      issue(box, col0 + 64 * c);
+    }
+  }
+}
+
+template <int EPI>
+__global__ void __launch_bounds__(GemmWideCfg<EPI>::THREADS, 1)
+gemm_wide_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                 const __grid_constant__ CUtensorMap tmC, const GemmParams p) {
+  using Cfg = GemmWideCfg<EPI>;
+  static_assert(EPI == EPI_BF16 || EPI == EPI_GELU || EPI == EPI_F32 || EPI == EPI_ROPE, "wide tiles: TMA-store epilogues");
+  constexpr int STAGES = Cfg::STAGES;
+  constexpr uint32_t A_BYTES = Cfg::A_BYTES;
+  constexpr uint32_t B_BYTES = Cfg::B_BYTES;
+
+  extern __shared__ __align__(1024) uint8_t smem[];
+  uint8_t* sA = smem;
+  uint8_t* sB = smem + STAGES * A_BYTES;
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + Cfg::OFF_BAR);
+  uint64_t* empty = full + STAGES;
+  uint8_t* stg_all = smem + Cfg::OFF_STG;
+  [[maybe_unused]] float* rope_s = reinterpret_cast<float*>(smem + Cfg::OFF_ROPE);
+
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+  const int n_tiles = p.N / Cfg::BN;
+  const int num_tiles = ((p.M + 127) / 128) * n_tiles;  // (m, n), n fastest
+  const int nkb = (p.K + Cfg::BK - 1) / Cfg::BK;
+
+  if (threadIdx.x == 0) {
+    if ((smem_u32(smem) & 1023u) != 0) device_fatal("dynamic shared memory is not 1024-byte aligned");
+    for (int s = 0; s < STAGES; ++s) {
+      mbar_init(&full[s], 1);   // the producer's expect_tx arrival
+      mbar_init(&empty[s], 8);  // one arrival per consumer warp: both warpgroups read every stage
+    }
+    fence_mbar_init();
+  }
+  if (warp == 0 && lane == 0) {
+    tma_prefetch_desc(&tmA);
+    tma_prefetch_desc(&tmB);
+    tma_prefetch_desc(&tmC);
+  }
+  if constexpr (EPI == EPI_ROPE) {  // constant table: staged before the PDL wait, as in gemm_wg_kernel
+    if (warp >= 4) {
+      const int nfl = p.rope_smem_rows * 32;
+      for (int i = (threadIdx.x - 128) * 4; i < nfl; i += Cfg::EPI_THREADS * 4)
+        *reinterpret_cast<float4*>(rope_s + (i >> 5) * kRopeLd + (i & 31)) =
+            __ldg(reinterpret_cast<const float4*>(p.rope_tab + i));
+    }
+  }
+  __syncthreads();
+  pdl_wait();
+  pdl_launch_dependents();
+
+  if (warp < 4) {
+    // ===================== TMA producer (warp 0, lane 0) =====================
+    setmaxnreg_dec<Cfg::PRODUCER_REGS>();
+    if (warp == 0 && lane == 0) {
+      int stage = 0;
+      uint32_t phase = 0;
+      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+        const int m_tile = tile / n_tiles;
+        const int n_tile = tile - m_tile * n_tiles;
+        for (int kb = 0; kb < nkb; ++kb) {
+          mbar_wait(&empty[stage], phase ^ 1);
+          mbar_arrive_expect_tx(&full[stage], A_BYTES + B_BYTES);
+          tma_load_2d(sA + stage * A_BYTES, &tmA, &full[stage], kb * Cfg::BK, m_tile * 128);
+          tma_load_2d(sB + stage * B_BYTES, &tmB, &full[stage], kb * Cfg::BK, n_tile * Cfg::BN);
+          if (++stage == STAGES) { stage = 0; phase ^= 1; }
+        }
+      }
+    }
+  } else {
+    // ============ consumer warpgroups: both on every tile, warpgroup wg on rows [64 wg, 64 wg + 64) ============
+    setmaxnreg_inc<Cfg::CONSUMER_REGS>();
+    const int wg = (warp - 4) >> 2;
+    const int wq = warp & 3;
+    uint8_t* stg = stg_all + (warp - 4) * Cfg::STG_WARP_BYTES;
+    uint32_t ubuf = 0;
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+      const int m_tile = tile / n_tiles;
+      const int n_tile = tile - m_tile * n_tiles;
+      float acc[128];
+#pragma unroll
+      for (int i = 0; i < 128; ++i) acc[i] = 0.0f;
+      // one k-block: four k16 steps of one m64n256k16 wgmma; the previous k-block's wgmma group may still run, its
+      // stage is released once this one is issued
+      int prev = -1;
+      for (int kb = 0; kb < nkb; ++kb) {
+        mbar_wait(&full[stage], phase);
+        const uint64_t adesc = make_smem_desc_sw128(smem_u32(sA + stage * A_BYTES) + wg * 64 * 128);
+        const uint64_t bdesc = make_smem_desc_sw128(smem_u32(sB + stage * B_BYTES));
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < 4; ++k) wgmma_m64n256k16_ss(acc, adesc + 2 * k, bdesc + 2 * k, 1u);
+        wgmma_commit();
+        wgmma_wait<1>();
+        fence_regs(acc);
+        if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
+        prev = stage;
+        if (++stage == STAGES) { stage = 0; phase ^= 1; }
+      }
+      wgmma_wait<0>();
+      fence_regs(acc);
+      if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
+
+      epilogue_wide_tma<EPI>(p, &tmC, acc, m_tile * 128 + 64 * wg + 16 * wq, n_tile * Cfg::BN, stg, rope_s, ubuf);
+      // after the CTA's last tile: the bulk stores read this CTA's shared memory
+      if (tile + static_cast<int>(gridDim.x) >= num_tiles && lane == 0) tma_store_wait_all();
+    }
+  }
+}
+
 }  // namespace sta

@@ -25,9 +25,15 @@ struct GemmLaunch {
   // optional fp32 scratch for split-K partials (small, weight-streaming-bound problems); unused if null
   void* splitk_ws = nullptr;
   size_t splitk_ws_bytes = 0;
+  // tile columns: 0 = automatic (gemm_auto_tile_n), 128 = the 128 x 128 kernel, 256 = the 128 x 256 kernel (error where
+  // it does not apply).  Both give bit-identical results.
+  int tile_n = 0;
 };
 
 int launch_gemm(const GemmLaunch& g, cudaStream_t stream);
+// Tile columns the automatic choice takes for a linear layer (M x N, depth K) with epilogue epi that runs the TMA-store
+// epilogue without split-K on a GPU with num_sms SMs: 256 or 128.  A function of these arguments only.
+int gemm_auto_tile_n(int M, int N, int K, int epi, int num_sms);
 
 // ---- attention (attention.cu) ----
 struct AttnLaunch {

@@ -1812,8 +1812,11 @@ int sta_op_gemm(const StaGemmDesc* d, void* stream) {
   p.head_w = d->head_w; p.head_b = d->head_b; p.pts3d = d->pts3d; p.conf = d->conf;
   p.split = d->split_precision;
   g.p = p;
+  g.tile_n = d->tile_n;
   return launch_gemm(g, static_cast<cudaStream_t>(stream));
 }
+
+int sta_gemm_auto_tile_n(int M, int N, int K, int epi, int num_sms) { return gemm_auto_tile_n(M, N, K, epi, num_sms); }
 
 int sta_op_gemm_fp8(const StaGemmFp8Desc* d, void* stream) {
   if (!d) {
