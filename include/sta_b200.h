@@ -295,6 +295,32 @@ int sta_pose_graph_lm_step(const float* nodes, int num_nodes, const int64_t* edg
                            int num_edges, const int64_t* opt_idx, int num_opt, double damping, double dmin, double dmax,
                            float* nodes_out, double* info_out, void* scratch, void* stream);
 
+/* ---- the same dense LM step on a group of G independent graphs, in one launch sequence: each graph has its own nodes,
+ * edges, measurements, weights, optimised set, damping and nodes_out (the device pointers and layouts of
+ * sta_pose_graph_lm_step), and its info row info_out[4 k .. 4 k + 3] (device, G x 4 fp64, the layout above).  Each
+ * graph's nodes_out and info row are bit-identical to its own sta_pose_graph_lm_step, whichever graphs share the group
+ * and in whatever order: no reduction crosses graphs.  No host synchronisation; read all G info rows back with one copy.
+ * The descriptor table is read on the call (it travels as a kernel parameter), so it may be rebuilt for every step.
+ * Refused with a status before any launch: a null table, info_out or scratch, G outside [1, STA_PG_GROUP_MAX], a null
+ * pointer or an empty graph (no nodes, edges or optimised nodes), num_opt > num_nodes, num_opt above
+ * STA_PG_DENSE_MAX_OPT, and scratch_bytes below sta_pose_graph_group_scratch_bytes.  The scratch holds the descriptor
+ * table and each graph's scratch one after another; the scratch-size function returns 0 for a table it would refuse.
+ * A group of one runs sta_pose_graph_lm_step's launch sequence. ---- */
+enum { STA_PG_GROUP_MAX = 16 };
+typedef struct StaPgGraph {
+  const float* nodes;     /* [num_nodes][8] */
+  const int64_t* edges;   /* [num_edges][2] */
+  const float* meas;      /* [num_edges][8] */
+  const float* weights;   /* [num_edges][7] */
+  const int64_t* opt_idx; /* [num_opt] */
+  float* nodes_out;       /* [num_nodes][8] */
+  int num_nodes, num_edges, num_opt;
+  double damping;
+} StaPgGraph;
+size_t sta_pose_graph_group_scratch_bytes(const StaPgGraph* graphs, int G);
+int sta_pose_graph_lm_step_group(const StaPgGraph* graphs, int G, double dmin, double dmax, double* info_out, void* scratch,
+                                 size_t scratch_bytes, void* stream);
+
 /* ---- block-sparse route of the same LM step, for any number of optimised nodes: identical residuals, Jacobians,
  * normal equations (A, g and loss before equal the dense route's), damping, update and losses; A d = -g is solved by a
  * block Cholesky factorisation with 7x7 blocks under a nested-dissection ordering, scheduled by elimination-tree levels.

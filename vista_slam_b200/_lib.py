@@ -54,6 +54,16 @@ GRAPH_MAX_KEYFRAME_EDGES = 32
 GRAPH_FLAG_NOT_SO3 = 1
 ORB_MAX_KEYPOINTS = 4096
 PG_DENSE_MAX_OPT = 3657  # STA_PG_DENSE_MAX_OPT: above it PoseGraphOpt takes the block-sparse route
+PG_GROUP_MAX = 16  # STA_PG_GROUP_MAX: graphs per sta_pose_graph_lm_step_group call
+
+
+class StaPgGraph(Structure):
+    _fields_ = [
+        ("nodes", c_void_p), ("edges", c_void_p), ("meas", c_void_p), ("weights", c_void_p), ("opt_idx", c_void_p),
+        ("nodes_out", c_void_p),
+        ("num_nodes", c_int), ("num_edges", c_int), ("num_opt", c_int),
+        ("damping", ctypes.c_double),
+    ]
 
 
 class StaFlowStats(Structure):
@@ -129,6 +139,10 @@ def lib():
     L.sta_pose_graph_scratch_bytes.restype = ctypes.c_size_t
     L.sta_pose_graph_lm_step.argtypes = [vp, i, vp, vp, vp, i, vp, i, ctypes.c_double, ctypes.c_double, ctypes.c_double, vp, vp,
                                          vp, vp]
+    L.sta_pose_graph_group_scratch_bytes.argtypes = [POINTER(StaPgGraph), i]
+    L.sta_pose_graph_group_scratch_bytes.restype = ctypes.c_size_t
+    L.sta_pose_graph_lm_step_group.argtypes = [POINTER(StaPgGraph), i, ctypes.c_double, ctypes.c_double, vp, vp,
+                                               ctypes.c_size_t, vp]
     L.sta_pg_plan_create.argtypes = [vp, i, i, vp, i, POINTER(vp)]
     L.sta_pg_plan_destroy.argtypes = [vp]
     L.sta_pg_plan_destroy.restype = None

@@ -226,11 +226,10 @@ __device__ bool mat7_inv(double* A, double* Inv) {
 // ---------------------------------------------------------------------------
 // one thread per edge: residual (and, if J != null, dr/d delta_j; dr/d delta_i = -that)
 // ---------------------------------------------------------------------------
-__global__ void __launch_bounds__(64)
-pg_edge_kernel(const float* __restrict__ nodes, const long long* __restrict__ edges, const float* __restrict__ meas,
-               const int* __restrict__ opt_map, int E, double* __restrict__ r_out, double* __restrict__ J_out,
-               int* __restrict__ related) {
-  const int e = blockIdx.x * blockDim.x + threadIdx.x;
+// (the bodies are device functions so that the dense route's group kernels run the same code per graph)
+__device__ __forceinline__ void pg_edge(int e, const float* __restrict__ nodes, const long long* __restrict__ edges,
+                                        const float* __restrict__ meas, const int* __restrict__ opt_map, int E,
+                                        double* __restrict__ r_out, double* __restrict__ J_out, int* __restrict__ related) {
   if (e >= E) return;
   const long long i = edges[2 * e], j = edges[2 * e + 1];
   const bool rel = opt_map[i] >= 0 || opt_map[j] >= 0;  // pose_graph.py:150-154
@@ -256,11 +255,16 @@ pg_edge_kernel(const float* __restrict__ nodes, const long long* __restrict__ ed
   mat7_mul(Jinv, Ad, J);
   for (int k = 0; k < 49; ++k) J_out[49 * e + k] = J[k];
 }
+__global__ void __launch_bounds__(64)
+pg_edge_kernel(const float* __restrict__ nodes, const long long* __restrict__ edges, const float* __restrict__ meas,
+               const int* __restrict__ opt_map, int E, double* __restrict__ r_out, double* __restrict__ J_out,
+               int* __restrict__ related) {
+  pg_edge(blockIdx.x * blockDim.x + threadIdx.x, nodes, edges, meas, opt_map, E, r_out, J_out, related);
+}
 
 // nodes_out = Exp(delta_a) * node for optimised nodes (LieTensor.add_), copy for fixed ones
-__global__ void pg_update_kernel(const float* __restrict__ nodes, const int* __restrict__ opt_map, const double* __restrict__ delta,
-                                 int num_nodes, float* __restrict__ out) {
-  const int v = blockIdx.x * blockDim.x + threadIdx.x;
+__device__ __forceinline__ void pg_update(int v, const float* __restrict__ nodes, const int* __restrict__ opt_map,
+                                          const double* __restrict__ delta, int num_nodes, float* __restrict__ out) {
   if (v >= num_nodes) return;
   const int a = opt_map[v];
   if (a < 0) {
@@ -274,11 +278,15 @@ __global__ void pg_update_kernel(const float* __restrict__ nodes, const int* __r
   for (int k = 0; k < 4; ++k) out[8 * v + 3 + k] = static_cast<float>(Y.q[k] * qn);
   out[8 * v + 7] = static_cast<float>(Y.s);
 }
+__global__ void pg_update_kernel(const float* __restrict__ nodes, const int* __restrict__ opt_map, const double* __restrict__ delta,
+                                 int num_nodes, float* __restrict__ out) {
+  pg_update(blockIdx.x * blockDim.x + threadIdx.x, nodes, opt_map, delta, num_nodes, out);
+}
 
-// loss = sum_e r_e^T W_e r_e (related edges), |delta|_2 -> info; fixed-order reduction in one CTA
-__global__ void __launch_bounds__(256) pg_loss_kernel(const double* __restrict__ r, const float* __restrict__ weights,
-                                                      const int* __restrict__ related, int E, const double* __restrict__ delta,
-                                                      int n7, double* __restrict__ info, int slot) {
+// loss = sum_e r_e^T W_e r_e (related edges), |delta|_2 -> info; fixed-order reduction in one CTA of 256 threads
+__device__ __forceinline__ void pg_loss(const double* __restrict__ r, const float* __restrict__ weights,
+                                        const int* __restrict__ related, int E, const double* __restrict__ delta, int n7,
+                                        double* __restrict__ info, int slot) {
   __shared__ double red[256];
   double s = 0.0;
   for (int e = threadIdx.x; e < E; e += 256) {
@@ -304,6 +312,11 @@ __global__ void __launch_bounds__(256) pg_loss_kernel(const double* __restrict__
     }
     if (threadIdx.x == 0) info[2] = sqrt(red[0]);
   }
+}
+__global__ void __launch_bounds__(256) pg_loss_kernel(const double* __restrict__ r, const float* __restrict__ weights,
+                                                      const int* __restrict__ related, int E, const double* __restrict__ delta,
+                                                      int n7, double* __restrict__ info, int slot) {
+  pg_loss(r, weights, related, E, delta, n7, info, slot);
 }
 
 }  // namespace

@@ -3,8 +3,9 @@
 Mirror of the optimisation OnlineSLAM.pose_graph_optimize runs through PyPose (vista_slam/slam.py:108-140 over
 vista_slam/pose_graph.py:70-154): Levenberg-Marquardt with a trust-region damping on the nodes listed in
 `to_optimize_idxs`, all other nodes fixed, edge weights diag(conf_e).  Each iteration is ONE C call
-(sta_pose_graph_lm_step: residuals, Jacobians, normal equations, damped dense Cholesky solve, update and both losses, all on
-the device) followed by one 32-byte read-back for the accept / reject decision -- the same host round trip pp.optim.LM makes.
+(sta_pose_graph_lm_step, or its group form sta_pose_graph_lm_step_group, which optimize() uses with one graph: residuals,
+Jacobians, normal equations, damped dense Cholesky solve, update and both losses, all on the device) followed by one
+32-byte read-back for the accept / reject decision -- the same host round trip pp.optim.LM makes.
 Tensors use PyPose's Sim3 layout (tx ty tz | qx qy qz qw | s), fp32, CUDA only (no CPU path).
 
 Two routes solve the damped normal equations, chosen in the constructor from the number of optimised nodes:
@@ -12,6 +13,13 @@ Two routes solve the damped normal equations, chosen in the constructor from the
   * block-sparse (above): sta_pose_graph_lm_step_sparse, a block Cholesky (7x7 blocks) over a plan -- ordering,
     elimination tree, block pattern and update lists -- built on the host from the edge list and the optimised set.
 Both compute the same residuals, Jacobians, normal equations, damping, update and losses.
+
+Groups: optimize_group(graphs, edges, poses, weights) optimises several independent graphs together and leaves each one
+exactly as its own optimize() would.  Each LM iteration steps every dense-route graph still running with ONE
+sta_pose_graph_lm_step_group launch sequence (the kernels take a graph index, so one launch covers every graph's
+Cholesky panel, triangular solve and so on) and reads all their info rows back with ONE copy; each graph keeps its own
+trust radius and plateau count and leaves the group when its plateau rule stops it.  Block-sparse-route members run
+their own iterations, unchanged, in the same call.  optimize() is a group of one.
 """
 import ctypes
 
@@ -43,6 +51,38 @@ class _SparsePlan:
         if getattr(self, "h", None):
             self._destroy(self.h)
             self.h = None
+
+
+def _read_info(info):
+    """The host copy of a step's info rows (device fp64 [..., 4]): the one host synchronisation of an LM iteration."""
+    return info.cpu()
+
+
+def _lm_iterations(graphs, step, steps, patience, decreasing, radius):
+    """slam.py:121-134 for each of `graphs`: LM(TrustRegion(radius), min=1e-6) driven by StopOnPlateau(steps, patience,
+    decreasing).  step(active graph indices, their dampings) -> per active graph (candidate nodes, loss before, loss
+    after, Cholesky ok).  A graph leaves the active set when its plateau rule stops it.  Returns the loss histories."""
+    n = len(graphs)
+    radii, stall, losses = [radius] * n, [0] * n, [[] for _ in range(n)]
+    active = list(range(n))
+    for _ in range(steps):
+        if not active:
+            break
+        results = step(active, [1.0 / radii[k] for k in active])
+        still = []
+        for k, (cand, l0, l1, ok) in zip(active, results):
+            if ok and l1 <= l0:
+                graphs[k].nodes = cand
+                radii[k] = min(radii[k] * 2.0, 1e32)
+            else:  # rejected step: keep the nodes, shrink the trust region
+                radii[k] = max(radii[k] * 0.5, 1e-32)
+                l1 = l0
+            losses[k].append(l1)
+            stall[k] = stall[k] + 1 if (l0 - l1) < decreasing else 0
+            if stall[k] < patience:
+                still.append(k)
+        active = still
+    return losses
 
 
 class PoseGraphOpt:
@@ -95,7 +135,7 @@ class PoseGraphOpt:
                                                            float(damping), float(dmin), float(dmax), _lib.ptr(out),
                                                            _lib.ptr(self._info), _lib.cur_stream()),
                            "sta_pose_graph_lm_step_sparse")
-            info = self._info.cpu()  # the one host synchronisation of the iteration
+            info = _read_info(self._info)  # the one host synchronisation of the iteration
             return out, float(info[0]), float(info[1]), float(info[2]), bool(info[3] > 0.5)
         edges = edges.to(torch.int64).contiguous()
         poses = poses.to(torch.float32).contiguous()
@@ -110,24 +150,91 @@ class PoseGraphOpt:
                                                 _lib.ptr(self.idxs_opt), No, float(damping), float(dmin), float(dmax),
                                                 _lib.ptr(out), _lib.ptr(self._info), _lib.ptr(self._scratch), _lib.cur_stream()),
                        "sta_pose_graph_lm_step")
-        info = self._info.cpu()  # the one host synchronisation of the iteration
+        info = _read_info(self._info)  # the one host synchronisation of the iteration
         return out, float(info[0]), float(info[1]), float(info[2]), bool(info[3] > 0.5)
 
     @torch.no_grad()
     def optimize(self, edges, poses, weight, steps=20, patience=3, decreasing=1e-4, radius=1e4):
         """slam.py:121-134: LM(TrustRegion(radius=1e4), min=1e-6) driven by StopOnPlateau(steps=20, patience=3,
         decreasing=1e-4).  `weight` is [E, 7] (the diagonal of the reference's diag_embed).  Returns the loss history."""
-        losses, stall = [], 0
-        for _ in range(steps):
-            cand, l0, l1, _, ok = self.lm_step(edges, poses, weight, 1.0 / radius)
-            if ok and l1 <= l0:
-                self.nodes = cand
-                radius = min(radius * 2.0, 1e32)
-            else:  # rejected step: keep the nodes, shrink the trust region
-                radius = max(radius * 0.5, 1e-32)
-                l1 = l0
-            losses.append(l1)
-            stall = stall + 1 if (l0 - l1) < decreasing else 0
-            if stall >= patience:
-                break
+        return PoseGraphOpt.optimize_group([self], [edges], [poses], [weight], steps=steps, patience=patience,
+                                           decreasing=decreasing, radius=radius)[0]
+
+    @staticmethod
+    @torch.no_grad()
+    def optimize_group(graphs, edges, poses, weights, steps=20, patience=3, decreasing=1e-4, radius=1e4):
+        """optimize() on several graphs at once: graphs[k] with edges[k], poses[k], weights[k].  Leaves every graph
+        exactly as its own optimize() would and returns each graph's loss history.  Per iteration, the dense-route
+        graphs still running take one sta_pose_graph_lm_step_group launch sequence and one read-back of all their info
+        rows; block-sparse-route graphs run their own iterations in this call.  Refused with ValueError before any
+        launch: lists of different lengths, graphs on different devices, one PoseGraphOpt named twice, and edges, poses
+        and weights whose row counts disagree."""
+        graphs = list(graphs)
+        edges, poses, weights = list(edges), list(poses), list(weights)
+        if not len(graphs) == len(edges) == len(poses) == len(weights):
+            raise ValueError("graphs, edges, poses and weights must have one entry per graph")
+        if len({id(g) for g in graphs}) != len(graphs):
+            raise ValueError("a PoseGraphOpt is named twice in the group")
+        if graphs and len({g.nodes.device for g in graphs}) != 1:
+            raise ValueError("every graph of a group must be on one device")
+        for e, p, w in zip(edges, poses, weights):
+            if p.shape[0] != e.shape[0] or w.shape[0] != e.shape[0]:
+                raise ValueError("edges, poses and weight must have one row per edge")
+        kw = dict(steps=steps, patience=patience, decreasing=decreasing, radius=radius)
+        losses = [None] * len(graphs)
+        dense = [k for k, g in enumerate(graphs) if not g.sparse]
+        for k, g in enumerate(graphs):
+            if g.sparse:
+                def sparse_step(active, damping, g=g, k=k):
+                    cand, l0, l1, _, ok = g.lm_step(edges[k], poses[k], weights[k], damping[0])
+                    return [(cand, l0, l1, ok)]
+                losses[k] = _lm_iterations([g], sparse_step, **kw)[0]
+        if dense:
+            group = _DenseGroup([graphs[k] for k in dense], [edges[k] for k in dense], [poses[k] for k in dense],
+                                [weights[k] for k in dense])
+            for k, h in zip(dense, _lm_iterations([graphs[k] for k in dense], group.step, **kw)):
+                losses[k] = h
         return losses
+
+
+class _DenseGroup:
+    """The dense-route LM step over a fixed list of graphs, of which any subset steps together: one scratch buffer and
+    one info table for the whole group, inputs converted once."""
+
+    def __init__(self, graphs, edges, poses, weights, dmin=1e-6, dmax=1e32):
+        self.graphs = graphs
+        self.edges = [e.to(torch.int64).contiguous() for e in edges]
+        self.poses = [p.to(torch.float32).contiguous() for p in poses]
+        self.weights = [w.to(torch.float32).contiguous() for w in weights]
+        self.dmin, self.dmax = dmin, dmax
+        self.device = graphs[0].nodes.device
+        self.info = torch.empty(len(graphs), 4, dtype=torch.float64, device=self.device)
+        self.scratch = None
+        self.L = _lib.lib()
+
+    def _table(self, members, dampings, outs):
+        tab = (_lib.StaPgGraph * len(members))()
+        for t, (k, damping, out) in enumerate(zip(members, dampings, outs)):
+            g = self.graphs[k]
+            tab[t] = _lib.StaPgGraph(g.nodes.data_ptr(), self.edges[k].data_ptr(), self.poses[k].data_ptr(),
+                                     self.weights[k].data_ptr(), g.idxs_opt.data_ptr(), out.data_ptr(), g.nodes.shape[0],
+                                     self.edges[k].shape[0], g.idxs_opt.shape[0], float(damping))
+        return tab
+
+    def step(self, members, dampings):
+        """One LM step of graphs[members] (at most PG_GROUP_MAX per launch sequence) -> per member (candidate nodes,
+        loss before, loss after, Cholesky ok); one info read-back in all."""
+        outs = [torch.empty_like(self.graphs[k].nodes) for k in members]
+        rows = len(members)
+        with torch.cuda.device(self.device):
+            for c0 in range(0, rows, _lib.PG_GROUP_MAX):
+                c1 = min(rows, c0 + _lib.PG_GROUP_MAX)
+                tab = self._table(members[c0:c1], dampings[c0:c1], outs[c0:c1])
+                need = int(self.L.sta_pose_graph_group_scratch_bytes(tab, c1 - c0))  # 0: the step refuses the table
+                if need and (self.scratch is None or self.scratch.numel() * 8 < need):
+                    self.scratch = torch.empty((need + 7) // 8, dtype=torch.float64, device=self.device)
+                _lib.check(self.L.sta_pose_graph_lm_step_group(tab, c1 - c0, self.dmin, self.dmax,
+                                                               _lib.ptr(self.info[c0:c1]), _lib.ptr(self.scratch), need,
+                                                               _lib.cur_stream()), "sta_pose_graph_lm_step_group")
+        info = _read_info(self.info[:rows])  # the one host synchronisation of the iteration
+        return [(out, float(r[0]), float(r[1]), bool(r[3] > 0.5)) for out, r in zip(outs, info)]

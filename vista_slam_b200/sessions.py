@@ -10,7 +10,10 @@ keyframes of every named session through one batched frontend pass:
   * the gated edge regression in chunks of at most 16 edges that mix sessions, one read-back per chunk
     (keyframe.regress_keyframes_gated_group).
 
-Graph insertion and PGO stay per session, in the order step_many would run them.  A call leaves every session as
+Graph insertion and PGO stay per session, in the order step_many would run them.  `optimize(ks)` runs the PGO of the
+named sessions now, together: one PoseGraphOpt.optimize_group, whose LM iterations step every session's graph with one
+launch sequence and one read-back.  With pgo_every beyond the sequence length, an evaluation over a scene list ends with
+one `optimize(range(len(scenes)))`, and a live server runs `optimize` on the sessions that are due.  A call leaves every session as
 `for k in sorted(values): sessions[k].step_many(values[k], force_pgo=k in force_pgo, ...)` would: the graph tables,
 host bookkeeping, loop candidates, gate decisions, PGO calls, written files and returned flags.  Frontend floats may
 differ from that loop within rounding, as step_many's differ from step's, because batch sizes change the GEMMs' split-K.
@@ -19,7 +22,7 @@ Timing: each session's time_dict gets its share of the batched phases.  The wall
 loop detection is split evenly across the sessions that have keyframes in the call; the time of an edge chunk's
 regression is split evenly across the sessions with keyframes in that chunk (added to their "decoder" and
 "graph_construction" buckets, as step_many counts the decoder inside graph construction).  Preparation, graph insertion
-and PGO are timed per session.
+and step's PGO are timed per session; the wall time of an optimize call is split evenly across its sessions ("pgo").
 
 All sessions run on the current CUDA device and stream.  The class is not thread-safe."""
 import operator
@@ -29,6 +32,7 @@ import torch
 
 from .keyframe import KeyframeFrontend, add_views_group, regress_keyframes_gated_group
 from .loop_detector import Vocabulary, detect_loops_group
+from .pose_graph import PoseGraphOpt
 from .slam import OnlineSLAM
 
 
@@ -179,3 +183,30 @@ class SLAMSessions:
                 if not ok:
                     s._check_flags()
         return flags
+
+    def optimize(self, ks):
+        """Optimise the pose graphs of sessions ks now, together.  Leaves each session as sessions[k].pose_graph_optimize()
+        would: the same optimised node set (the window and the loop-related views), the same poses bit for bit,
+        loop_related_views cleared and the same messages (every session's opening messages, then the optimisation,
+        then every session's closing message); a session without nodes or edges only prints them.  An unknown or
+        repeated index raises ValueError before anything runs.  Host synchronisations: one per LM iteration of the
+        group (block-sparse-route graphs, above PG_DENSE_MAX_OPT optimised nodes, add their own)."""
+        order, seen = [], set()
+        for k in ks:
+            k = self._index(k)
+            if k in seen:
+                raise ValueError("session %d is named twice" % k)
+            seen.add(k)
+            order.append(k)
+        if not order:
+            return
+        sess = [self.sessions[k] for k in order]
+        t = time.time()
+        problems = [s._pgo_begin() for s in sess]
+        run = [p for p in problems if p is not None]
+        if run:
+            PoseGraphOpt.optimize_group([g for g, _ in run], *[[a[i] for _, a in run] for i in range(3)])
+        for s, p in zip(sess, problems):
+            s._pgo_end(p)
+        _share(sess, "pgo", time.time() - t)
+        torch.cuda.empty_cache()

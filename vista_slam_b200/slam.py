@@ -394,6 +394,16 @@ class OnlineSLAM:
 
     def pose_graph_optimize(self):
         """slam.py:108-140 through PoseGraphOpt on the device tables (per-edge weights: DESIGN.md §4)."""
+        problem = self._pgo_begin()
+        if problem is not None:
+            graph, args = problem
+            graph.optimize(*args)
+        self._pgo_end(problem)
+
+    def _pgo_begin(self):
+        """The first half of a PGO (slam.py:108-120): its messages, then (PoseGraphOpt over the node table with the
+        optimised node set, (edges, measurements, weights)), or None for a graph without nodes or edges.  The optimised
+        set is the nodes of the last pgo_window_size views and the loop-related views (view ids, used as node ids)."""
         _msg("[PoseGraphOpt] ", f"Pose graph optimization (at keyframe {self.view_num}) ...")
         if self.live_mode:
             _msg("[PoseGraphOpt] ", "This may cause latency in live mode, please hold the camera steady if possible.")
@@ -402,12 +412,17 @@ class OnlineSLAM:
         for v in range(max(0, self.view_num - self.pgo_window_size), self.view_num):
             opt.update(self.view_to_node.get(v, []))
         opt.update(self.loop_related_views)  # view ids, used as node ids (slam.py:120)
-        if N > 0 and E > 0:
-            g = self._graph
-            idx = torch.tensor(sorted(opt), dtype=torch.int64).to(self.device)
-            graph = PoseGraphOpt(g.pose[:N], to_optimize_idxs=idx)
-            graph.optimize(g.edges[:E], g.meas[:E], g.weight[:E])
-            g.pose[:N] = graph.get_nodes()
+        if not (N > 0 and E > 0):
+            return None
+        g = self._graph
+        idx = torch.tensor(sorted(opt), dtype=torch.int64).to(self.device)
+        return PoseGraphOpt(g.pose[:N], to_optimize_idxs=idx), (g.edges[:E], g.meas[:E], g.weight[:E])
+
+    def _pgo_end(self, problem):
+        """The second half of a PGO, after the optimisation of _pgo_begin's problem: the poses written back, the
+        message, loop_related_views cleared."""
+        if problem is not None:
+            self._graph.pose[:self.num_nodes] = problem[0].get_nodes()
             self._check_flags()
         _msg("[PoseGraphOpt] ", "Pose graph optimization done.")
         self.loop_related_views = set()
