@@ -368,6 +368,11 @@ int sta_preprocess_geometry(int H, int W, int res_w, int res_h, int w_edge, int 
 int sta_preprocess_coeffs(int in_size, int out_size, int* ksize, int* bounds, int* kk, int64_t kk_capacity);
 int sta_preprocess_rgb8(const uint8_t* rgb_dev, int H, int W, int res_w, int res_h, int w_edge, int h_edge,
                         float* rgb_out_dev, float* gray_out_dev, uint8_t* u8_out_dev, void* stream);
+/* F same-size frames in one launch pair, each bit-identical to its own sta_preprocess_rgb8 (its F = 1 case): rgb
+ * [F][H][W][3] -> rgb_out [F][3][oh][ow], gray_out [F][oh][ow] or NULL, u8_out [F][oh][ow][3] or NULL.  F in
+ * [1, 65535]; the cached intermediate image grows to the largest F of its geometry. */
+int sta_preprocess_rgb8_many(const uint8_t* rgb_dev, int F, int H, int W, int res_w, int res_h, int w_edge, int h_edge,
+                             float* rgb_out_dev, float* gray_out_dev, uint8_t* u8_out_dev, void* stream);
 
 /* ---- keyframe flow tracker: FlowTracker.compute_disparity (vista_slam/flow_tracker.py:26-66) on the device, with the
  * reference's fixed constants: cv2.goodFeaturesToTrack(maxCorners=1000, qualityLevel=0.01, minDistance=8, blockSize=7)
@@ -375,7 +380,7 @@ int sta_preprocess_rgb8(const uint8_t* rgb_dev, int H, int W, int res_w, int res
  * (frame_is_f32 = 0) or the [H][W] fp32 gray in [0,1] that sta_preprocess_rgb8 writes (1), converted as
  * (gray * 255).astype(uint8).  Frame sides must be in [32, 2048]; the size checks come before any CUDA call.
  * A tracker handle owns two pyramids (keyframe and current frame), the keyframe's derivatives and corners, and scratch
- * for one frame size.  One stream at a time: work on a new stream waits for the previous one. ---- */
+ * for one frame size, plus the frame pyramids of its group tracks (below).  One stream at a time: work on a new stream waits for the previous one. ---- */
 enum { STA_FLOW_MAX_CORNERS = 1000 };
 typedef struct StaFlowTracker StaFlowTracker; /* opaque */
 typedef struct StaFlowStats {
@@ -397,6 +402,26 @@ int sta_flow_promote(StaFlowTracker* t, void* stream);
 /* Device copies of the keyframe corners: pts_out [STA_FLOW_MAX_CORNERS][2] fp32 (x, y) in selection order, the first
  * *count_out valid; and of the keyframe's level-0 image [H][W] uint8 and derivatives [H][W][2] int16 (either may be
  * NULL). */
+/* Groups: the same over many frames and many trackers (SLAM sessions, or a run of frames of one tracker), with every
+ * per-frame result equal to the tracker's own one-frame calls; the calls above are the one-frame case.  All trackers
+ * of a group share one frame size; frames are [n][H][W] uint8 or fp32 gray as above.  Refused before any launch: n or
+ * F < 1, a null pointer, mixed tracker sizes, and the per-call conditions below.
+ * sta_flow_set_keyframe_group: initialize_keyframe of frame i on ts[i] (n distinct trackers); asynchronous.
+ * sta_flow_track_group: frame f belongs to ts[f]; a tracker's frames are consecutive and in its own order, and every
+ * one is tracked against the tracker's current keyframe (which must exist) in one launch per stage, then the one host
+ * synchronisation: stats_out [F] (host).  held_host [F] (or NULL: none) marks the frames whose pyramids the tracker
+ * still holds from its last group track: the frames after the one sta_flow_promote_group promoted, reused in order
+ * as a prefix of its frames here (at most as many as it holds).  frames_dev holds only the other frames, in group
+ * order (NULL when there are none).
+ * sta_flow_promote_group: frame frame_host[i] (its index among ts[i]'s frames of its last group track) becomes the
+ * keyframe of ts[i] (n distinct trackers) without a rebuild; their derivatives and corners are enqueued as one
+ * sequence; asynchronous.  The LK output and statistics of a group are in ts[0]'s buffers; each tracker holds up to
+ * its largest group's frame pyramids, allocated on first use. */
+int sta_flow_set_keyframe_group(StaFlowTracker* const* ts, int n, const void* frames_dev, int frames_is_f32,
+                                void* stream);
+int sta_flow_track_group(StaFlowTracker* const* ts, int F, const int* held_host, const void* frames_dev,
+                         int frames_is_f32, StaFlowStats* stats_out, void* stream);
+int sta_flow_promote_group(StaFlowTracker* const* ts, int n, const int* frame_host, void* stream);
 int sta_flow_keyframe_points(StaFlowTracker* t, float* pts_out_dev, int* count_out_dev, void* stream);
 int sta_flow_keyframe_level0(StaFlowTracker* t, uint8_t* gray_out_dev, int16_t* deriv_out_dev, void* stream);
 /* Op-level entry points (the same kernels).  scratch: a device buffer of sta_flow_scratch_bytes(H, W) bytes (256-byte

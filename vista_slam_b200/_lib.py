@@ -131,6 +131,7 @@ def lib():
     L.sta_preprocess_geometry.argtypes = [i, i, i, i, i, i, POINTER(c_int)]
     L.sta_preprocess_coeffs.argtypes = [i, i, POINTER(c_int), POINTER(c_int), POINTER(c_int), i64]
     L.sta_preprocess_rgb8.argtypes = [vp, i, i, i, i, i, i, vp, vp, vp, vp]
+    L.sta_preprocess_rgb8_many.argtypes = [vp, i, i, i, i, i, i, i, vp, vp, vp, vp]
     L.sta_pointmap_scratch_bytes.argtypes = [i]
     L.sta_pointmap_scratch_bytes.restype = ctypes.c_size_t
     L.sta_pointmap_consumers.argtypes = [vp, vp, i, i, i, i, vp, vp, vp, vp, vp]
@@ -157,6 +158,9 @@ def lib():
     L.sta_flow_set_keyframe.argtypes = [vp, vp, i, vp]
     L.sta_flow_track.argtypes = [vp, vp, i, POINTER(StaFlowStats), vp]
     L.sta_flow_promote.argtypes = [vp, vp]
+    L.sta_flow_set_keyframe_group.argtypes = [POINTER(vp), i, vp, i, vp]
+    L.sta_flow_track_group.argtypes = [POINTER(vp), i, POINTER(c_int), vp, i, POINTER(StaFlowStats), vp]
+    L.sta_flow_promote_group.argtypes = [POINTER(vp), i, POINTER(c_int), vp]
     L.sta_flow_keyframe_points.argtypes = [vp, vp, vp, vp]
     L.sta_flow_keyframe_level0.argtypes = [vp, vp, vp, vp]
     L.sta_flow_scratch_bytes.argtypes = [i, i]

@@ -12,13 +12,22 @@
 //
 // Buffers (one arena per frame size): two padded pyramids (the keyframe's and the current frame's, swapped when a frame
 // becomes the keyframe), the keyframe's Scharr derivatives, the corner selection scratch, the keyframe corners, the LK
-// output and the statistics the host reads once per tracked frame.
+// output and the statistics the host reads once per tracked frame.  A group track (sta_flow_track_group) adds frame
+// pyramid slots per tracker, and LK output and statistics for every frame of the group.
+//
+// Every stage runs over a batch: the pyramid kernels over frames, LK and the statistics over (frame, keyframe) items,
+// the derivative and corner kernels over keyframes, each with the batch index in blockIdx.y (one CTA per keyframe in
+// select_kernel, one per item in flow_stats_kernel).  The per-item pointers travel in a __grid_constant__ table of at
+// most kMaxBatch entries; a larger batch is several launches.  The one-frame entry points are batches of one.
 #include "../../include/sta_b200.h"
 #include "common.cuh"
 #include "host_util.h"
 
 #include <float.h>
 #include <stdint.h>
+
+#include <algorithm>
+#include <vector>
 
 namespace sta {
 
@@ -38,6 +47,7 @@ constexpr float kEigScale2 = static_cast<float>(1.0 / (7140.0 * 7140.0));  // So
 constexpr int kMaxCorners = STA_FLOW_MAX_CORNERS;
 constexpr int kMinSide = 32, kMaxSide = 2048;
 constexpr int kSelectThreads = 1024;
+constexpr int kMaxBatch = 64;  // frames, keyframes or LK items per launch (the LK table is 3.5 KB of parameters)
 
 struct Levels {
   int nlev;
@@ -106,6 +116,20 @@ Layout make_layout(int H, int W) {
   return s;
 }
 
+// per-keyframe pointers of a derivative / corner batch: its pyramid, its arena (a Layout's derivatives, corner scratch
+// and counters) and where its corners and their count go
+struct KfBatch {
+  const uint8_t* pyr[kMaxBatch];
+  char* arena[kMaxBatch];
+  float2* pts[kMaxBatch];
+  int* count[kMaxBatch];
+};
+
+template <typename T>
+__host__ __device__ __forceinline__ T* at(void* arena, size_t off) {
+  return reinterpret_cast<T*>(static_cast<char*>(arena) + off);
+}
+
 __device__ __forceinline__ int refl101(int i, int n) {  // BORDER_REFLECT_101 for -n < i < 2n - 1
   i = abs(i);
   return i >= n ? 2 * (n - 1) - i : i;
@@ -116,10 +140,18 @@ __device__ __forceinline__ int refl101(int i, int n) {  // BORDER_REFLECT_101 fo
 // ---------------------------------------------------------------------------------------------------------------------
 // level 0 with its REFLECT_101 border; an fp32 gray in [0, 1] becomes (gray * 255).astype(uint8): one fp32 multiply,
 // then truncation
+// per-frame pointers of a pyramid batch: the source frame (level 0 only) and the padded pyramid it builds
+struct FrameBatch {
+  const void* src[kMaxBatch];
+  uint8_t* pyr[kMaxBatch];
+};
+
 __global__ void __launch_bounds__(256)
-level0_kernel(const void* __restrict__ frame, int is_f32, int H, int W, uint8_t* __restrict__ dst) {
+level0_kernel(const __grid_constant__ FrameBatch b, int is_f32, int H, int W) {
   pdl_wait();
   pdl_launch_dependents();
+  const void* frame = b.src[blockIdx.y];
+  uint8_t* dst = b.pyr[blockIdx.y];
   const int pw = W + 2 * kPad, ph = H + 2 * kPad;
   const int idx = blockIdx.x * 256 + threadIdx.x;
   if (idx >= pw * ph) return;
@@ -137,9 +169,11 @@ level0_kernel(const void* __restrict__ frame, int is_f32, int H, int W, uint8_t*
 // pyrDown: 5x5 [1 4 6 4 1]^2 / 256 with rounding.  The source level's border already holds REFLECT_101 values, which is
 // what pyrDown reads outside the level; the destination's own border is written by reflecting its coordinates.
 __global__ void __launch_bounds__(256)
-pyrdown_kernel(const uint8_t* __restrict__ src, int sw, uint8_t* __restrict__ dst, int dw, int dh) {
+pyrdown_kernel(const __grid_constant__ FrameBatch b, long long src_ofs, int sw, long long dst_ofs, int dw, int dh) {
   pdl_wait();
   pdl_launch_dependents();
+  const uint8_t* src = b.pyr[blockIdx.y] + src_ofs;
+  uint8_t* dst = b.pyr[blockIdx.y] + dst_ofs;
   const int spw = sw + 2 * kPad;
   const int pw = dw + 2 * kPad, ph = dh + 2 * kPad;
   const int idx = blockIdx.x * 256 + threadIdx.x;
@@ -160,9 +194,11 @@ pyrdown_kernel(const uint8_t* __restrict__ src, int sw, uint8_t* __restrict__ ds
 
 // calcSharrDeriv: int16 (dI/dx, dI/dy) with 3-10-3 smoothing (REFLECT_101: the level's border), zero outside the level
 __global__ void __launch_bounds__(256)
-scharr_kernel(const uint8_t* __restrict__ img, int w, int h, short2* __restrict__ deriv) {
+scharr_kernel(const __grid_constant__ KfBatch b, size_t deriv_off, long long ofs, int w, int h) {
   pdl_wait();
   pdl_launch_dependents();
+  const uint8_t* img = b.pyr[blockIdx.y] + ofs;
+  short2* deriv = at<short2>(b.arena[blockIdx.y], deriv_off) + ofs;
   const int pw = w + 2 * kPad, ph = h + 2 * kPad;
   const int idx = blockIdx.x * 256 + threadIdx.x;
   if (idx >= pw * ph) return;
@@ -183,10 +219,14 @@ scharr_kernel(const uint8_t* __restrict__ img, int w, int h, short2* __restrict_
 // Shi-Tomasi corners (goodFeaturesToTrack -> cornerMinEigenVal)
 // ---------------------------------------------------------------------------------------------------------------------
 // integer 3x3 Sobel (dx, dy) of level 0 (REFLECT_101)
+// (also clears the keyframe's selection counters, which the following kernels accumulate into)
 __global__ void __launch_bounds__(256)
-sobel_kernel(const uint8_t* __restrict__ img, int W, int H, short2* __restrict__ sob) {
+sobel_kernel(const __grid_constant__ KfBatch b, const __grid_constant__ Layout s, int W, int H) {
   pdl_wait();
   pdl_launch_dependents();
+  const uint8_t* img = b.pyr[blockIdx.y];
+  short2* sob = at<short2>(b.arena[blockIdx.y], s.sob);
+  if (blockIdx.x == 0 && threadIdx.x < kNumCounters) at<unsigned>(b.arena[blockIdx.y], s.counters)[threadIdx.x] = 0u;
   const int idx = blockIdx.x * 256 + threadIdx.x;
   if (idx >= W * H) return;
   const int y = idx / W, x = idx - y * W;
@@ -209,9 +249,12 @@ __device__ __forceinline__ float float_from_order_key(unsigned k) {
 // exact 7x7 box sums of dx^2, dx dy, dy^2 (REFLECT_101), scaled once: lambda_min = (a + c) - sqrt((a - c)^2 + b^2) with
 // a = sum(dx^2)/2, b = sum(dx dy), c = sum(dy^2)/2; and the global maximum
 __global__ void __launch_bounds__(256)
-min_eigen_kernel(const short2* __restrict__ sob, int W, int H, float* __restrict__ eig, unsigned* __restrict__ counters) {
+min_eigen_kernel(const __grid_constant__ KfBatch kb, const __grid_constant__ Layout s, int W, int H) {
   pdl_wait();
   pdl_launch_dependents();
+  const short2* sob = at<const short2>(kb.arena[blockIdx.y], s.sob);
+  float* eig = at<float>(kb.arena[blockIdx.y], s.eig);
+  unsigned* counters = at<unsigned>(kb.arena[blockIdx.y], s.counters);
   const int idx = blockIdx.x * 256 + threadIdx.x;
   unsigned key = 0;
   if (idx < W * H) {
@@ -248,10 +291,13 @@ __device__ __forceinline__ float thresholded(float v, float thr) { return v > th
 // threshold(eig, max * 0.01, TOZERO), then the candidates: non-zero, equal to their 3x3 dilation, not on the 1-pixel
 // border.  state: 1 = candidate (undecided), 0 = not a candidate
 __global__ void __launch_bounds__(256)
-candidates_kernel(const float* __restrict__ eig, int W, int H, uint8_t* __restrict__ state, int* __restrict__ cand,
-                  unsigned* __restrict__ counters) {
+candidates_kernel(const __grid_constant__ KfBatch kb, const __grid_constant__ Layout s, int W, int H) {
   pdl_wait();
   pdl_launch_dependents();
+  const float* eig = at<const float>(kb.arena[blockIdx.y], s.eig);
+  uint8_t* state = at<uint8_t>(kb.arena[blockIdx.y], s.state);
+  int* cand = at<int>(kb.arena[blockIdx.y], s.cand);
+  unsigned* counters = at<unsigned>(kb.arena[blockIdx.y], s.counters);
   const int idx = blockIdx.x * 256 + threadIdx.x;
   if (idx >= W * H) return;
   const int y = idx / W, x = idx - y * W;
@@ -284,13 +330,17 @@ __device__ __forceinline__ unsigned long long rank_key(const float* eig, int p) 
 // higher-ranked neighbour, reject one with an accepted higher-ranked neighbour, and repeat until nothing changes.  Every
 // round decides at least the highest undecided candidate.  Updates are in place: a candidate only moves from undecided
 // to final, and each rule reads final states only to conclude.  Then the accepted corners are listed.
-// state: 1 undecided, 2 accepted, 3 rejected.
+// state: 1 undecided, 2 accepted, 3 rejected.  One CTA per keyframe.
 __global__ void __launch_bounds__(kSelectThreads)
-select_kernel(const float* __restrict__ eig, int W, int H, uint8_t* state_, const int* __restrict__ cand, int* __restrict__ acc,
-              unsigned* __restrict__ counters) {
+select_kernel(const __grid_constant__ KfBatch kb, const __grid_constant__ Layout s, int W, int H) {
   pdl_wait();
   pdl_launch_dependents();
-  volatile uint8_t* state = state_;
+  char* a = kb.arena[blockIdx.x];
+  const float* eig = at<const float>(a, s.eig);
+  volatile uint8_t* state = at<uint8_t>(a, s.state);
+  const int* cand = at<const int>(a, s.cand);
+  int* acc = at<int>(a, s.acc);
+  unsigned* counters = at<unsigned>(a, s.counters);
   __shared__ int changed;
   const int n = static_cast<int>(counters[kCntCand]);
   for (;;) {
@@ -343,10 +393,14 @@ select_kernel(const float* __restrict__ eig, int W, int H, uint8_t* state_, cons
 // order the accepted corners by rank (a corner's position is the number of higher-ranked accepted corners) and keep the
 // first 1000: the same as stopping the sequential walk at 1000
 __global__ void __launch_bounds__(256)
-rank_kernel(const float* __restrict__ eig, int W, const int* __restrict__ acc, const unsigned* __restrict__ counters,
-            float2* __restrict__ pts, int* __restrict__ count) {
+rank_kernel(const __grid_constant__ KfBatch kb, const __grid_constant__ Layout s, int W) {
   pdl_wait();
   pdl_launch_dependents();
+  const float* eig = at<const float>(kb.arena[blockIdx.y], s.eig);
+  const int* acc = at<const int>(kb.arena[blockIdx.y], s.acc);
+  const unsigned* counters = at<const unsigned>(kb.arena[blockIdx.y], s.counters);
+  float2* pts = kb.pts[blockIdx.y];
+  int* count = kb.count[blockIdx.y];
   __shared__ unsigned long long tile[256];
   const int n = static_cast<int>(counters[kCntAcc]);
   const int i = blockIdx.x * 256 + threadIdx.x;
@@ -387,12 +441,31 @@ __device__ __forceinline__ long long warp_sum_ll(long long v) {
   return v;
 }
 
+// one LK item: the keyframe's pyramid I, derivatives dI, corners pts and device corner count n_dev (NULL: the kernel's
+// n_host), the frame's pyramid J, and the item's output slots
+struct LkItem {
+  const uint8_t* I;
+  const short2* dI;
+  const uint8_t* J;
+  const float2* pts;
+  const int* n_dev;
+  float2* next;
+  uint8_t* status;
+};
+struct LkBatch {
+  LkItem it[kMaxBatch];
+};
+
 __global__ void __launch_bounds__(128)
-lk_kernel(const __grid_constant__ Levels lv, const uint8_t* __restrict__ I, const short2* __restrict__ dI, const uint8_t* __restrict__ J,
-          const float2* __restrict__ pts, const int* __restrict__ n_dev, int n_host, float2* __restrict__ next_out,
-          uint8_t* __restrict__ status_out) {
+lk_kernel(const __grid_constant__ Levels lv, const __grid_constant__ LkBatch b, int n_host) {
   pdl_wait();
   pdl_launch_dependents();
+  const LkItem& item = b.it[blockIdx.y];
+  const uint8_t* __restrict__ I = item.I;
+  const short2* __restrict__ dI = item.dI;
+  const uint8_t* __restrict__ J = item.J;
+  const float2* __restrict__ pts = item.pts;
+  const int* n_dev = item.n_dev;
   const int lane = threadIdx.x & 31;
   const int pid = blockIdx.x * 4 + (threadIdx.x >> 5);
   const int n = n_dev ? *n_dev : n_host;
@@ -499,18 +572,23 @@ lk_kernel(const __grid_constant__ Levels lv, const uint8_t* __restrict__ I, cons
     }
   }
   if (lane == 0) {
-    next_out[pid] = nxt;
-    status_out[pid] = static_cast<uint8_t>(status);
+    item.next[pid] = nxt;
+    item.status[pid] = static_cast<uint8_t>(status);
   }
 }
 
 // keyframe corner count, tracked count, sum over tracked points of |dx| + |dy| (fp32 differences, fp64 sum in a fixed
-// order) and the mean disparity sum / (2 count) of flow_tracker.py:50-51
+// order) and the mean disparity sum / (2 count) of flow_tracker.py:50-51; one CTA per LK item, out[item]
 __global__ void __launch_bounds__(256)
-flow_stats_kernel(const float2* __restrict__ kf, const float2* __restrict__ nxt, const uint8_t* __restrict__ status,
-                  const int* __restrict__ n_dev, StaFlowStats* __restrict__ out) {
+flow_stats_kernel(const __grid_constant__ LkBatch b, StaFlowStats* __restrict__ out_base) {
   pdl_wait();
   pdl_launch_dependents();
+  const LkItem& item = b.it[blockIdx.x];
+  const float2* __restrict__ kf = item.pts;
+  const float2* __restrict__ nxt = item.next;
+  const uint8_t* __restrict__ status = item.status;
+  const int* __restrict__ n_dev = item.n_dev;
+  StaFlowStats* out = out_base + blockIdx.x;
   __shared__ double ssum[256];
   __shared__ int scnt[256];
   const int n = *n_dev;
@@ -543,69 +621,84 @@ flow_stats_kernel(const float2* __restrict__ kf, const float2* __restrict__ nxt,
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
-// host-side sequences
+// host-side sequences: each takes a batch of n >= 1 and launches it in chunks of kMaxBatch
 // ---------------------------------------------------------------------------------------------------------------------
 inline unsigned blocks_for(long long n, int per) { return static_cast<unsigned>((n + per - 1) / per); }
 
-template <typename T>
-T* at(void* arena, size_t off) {
-  return reinterpret_cast<T*>(static_cast<char*>(arena) + off);
+inline long long padded_elems(const Levels& lv, int l) {
+  return static_cast<long long>(lv.w[l] + 2 * kPad) * (lv.h[l] + 2 * kPad);
 }
 
-int build_pyramid(const Layout& s, const void* frame, int is_f32, uint8_t* pyr, cudaStream_t st) {
+// the pyramids of n frames of one size: src[i] ([H][W] uint8, or the fp32 gray when is_f32) -> padded pyramid pyr[i]
+int build_pyramids(const Layout& s, int n, const void* const* src, int is_f32, uint8_t* const* pyr, cudaStream_t st) {
   const Levels& lv = s.lv;
-  const long long n0 = static_cast<long long>(lv.w[0] + 2 * kPad) * (lv.h[0] + 2 * kPad);
-  STA_CHECK_CUDA(launch_pdl(level0_kernel, dim3(blocks_for(n0, 256)), dim3(256), 0, st, 1, frame, is_f32, lv.h[0], lv.w[0],
-                            pyr));
-  for (int l = 1; l < lv.nlev; ++l) {
-    const long long nl = static_cast<long long>(lv.w[l] + 2 * kPad) * (lv.h[l] + 2 * kPad);
-    STA_CHECK_CUDA(launch_pdl(pyrdown_kernel, dim3(blocks_for(nl, 256)), dim3(256), 0, st, 1,
-                              static_cast<const uint8_t*>(pyr + lv.ofs[l - 1]), lv.w[l - 1], pyr + lv.ofs[l], lv.w[l],
-                              lv.h[l]));
+  for (int c0 = 0; c0 < n; c0 += kMaxBatch) {
+    const int m = n - c0 < kMaxBatch ? n - c0 : kMaxBatch;
+    FrameBatch b = {};
+    for (int i = 0; i < m; ++i) {
+      b.src[i] = src[c0 + i];
+      b.pyr[i] = pyr[c0 + i];
+    }
+    STA_CHECK_CUDA(launch_pdl(level0_kernel, dim3(blocks_for(padded_elems(lv, 0), 256), m), dim3(256), 0, st, 1, b, is_f32,
+                              lv.h[0], lv.w[0]));
+    for (int l = 1; l < lv.nlev; ++l)
+      STA_CHECK_CUDA(launch_pdl(pyrdown_kernel, dim3(blocks_for(padded_elems(lv, l), 256), m), dim3(256), 0, st, 1, b,
+                                lv.ofs[l - 1], lv.w[l - 1], lv.ofs[l], lv.w[l], lv.h[l]));
   }
   return 0;
 }
 
-int build_derivs(const Layout& s, const uint8_t* pyr, short2* deriv, cudaStream_t st) {
-  const Levels& lv = s.lv;
-  for (int l = 0; l < lv.nlev; ++l) {
-    const long long nl = static_cast<long long>(lv.w[l] + 2 * kPad) * (lv.h[l] + 2 * kPad);
-    STA_CHECK_CUDA(launch_pdl(scharr_kernel, dim3(blocks_for(nl, 256)), dim3(256), 0, st, 1, pyr + lv.ofs[l], lv.w[l],
-                              lv.h[l], deriv + lv.ofs[l]));
-  }
-  return 0;
-}
+// one keyframe of a derivative / corner batch: its pyramid, the arena (Layout) its scratch lives in, and where its
+// corners [1000] and their count go
+struct KfJob {
+  const uint8_t* pyr;
+  void* arena;
+  float2* pts;
+  int* count;
+};
 
-// corners of the level-0 image of `pyr` -> pts [1000] float2, *count
-int good_features(const Layout& s, void* arena, const uint8_t* pyr, float2* pts, int* count, cudaStream_t st) {
-  const int W = s.lv.w[0], H = s.lv.h[0];
+// for n keyframes: the Scharr derivatives of every level (derivs), then the corners of level 0 (corners)
+int keyframe_products(const Layout& s, int n, const KfJob* jobs, bool derivs, bool corners, cudaStream_t st) {
+  const Levels& lv = s.lv;
+  const int W = lv.w[0], H = lv.h[0];
   const long long hw = static_cast<long long>(W) * H;
-  unsigned* counters = at<unsigned>(arena, s.counters);
-  short2* sob = at<short2>(arena, s.sob);
-  float* eig = at<float>(arena, s.eig);
-  uint8_t* state = at<uint8_t>(arena, s.state);
-  int* cand = at<int>(arena, s.cand);
-  int* acc = at<int>(arena, s.acc);
-  STA_CHECK_CUDA(cudaMemsetAsync(counters, 0, kNumCounters * sizeof(unsigned), st));
-  STA_CHECK_CUDA(launch_pdl(sobel_kernel, dim3(blocks_for(hw, 256)), dim3(256), 0, st, 1, pyr, W, H, sob));
-  STA_CHECK_CUDA(launch_pdl(min_eigen_kernel, dim3(blocks_for(hw, 256)), dim3(256), 0, st, 1,
-                            static_cast<const short2*>(sob), W, H, eig, counters));
-  STA_CHECK_CUDA(launch_pdl(candidates_kernel, dim3(blocks_for(hw, 256)), dim3(256), 0, st, 1,
-                            static_cast<const float*>(eig), W, H, state, cand, counters));
-  STA_CHECK_CUDA(launch_pdl(select_kernel, dim3(1), dim3(kSelectThreads), 0, st, 1, static_cast<const float*>(eig), W, H,
-                            state, static_cast<const int*>(cand), acc, counters));
-  STA_CHECK_CUDA(launch_pdl(rank_kernel, dim3(blocks_for(s.acc_cap, 256)), dim3(256), 0, st, 1,
-                            static_cast<const float*>(eig), W, static_cast<const int*>(acc),
-                            static_cast<const unsigned*>(counters), pts, count));
+  for (int c0 = 0; c0 < n; c0 += kMaxBatch) {
+    const int m = n - c0 < kMaxBatch ? n - c0 : kMaxBatch;
+    KfBatch b = {};
+    for (int i = 0; i < m; ++i) {
+      b.pyr[i] = jobs[c0 + i].pyr;
+      b.arena[i] = static_cast<char*>(jobs[c0 + i].arena);
+      b.pts[i] = jobs[c0 + i].pts;
+      b.count[i] = jobs[c0 + i].count;
+    }
+    if (derivs) {
+      for (int l = 0; l < lv.nlev; ++l)
+        STA_CHECK_CUDA(launch_pdl(scharr_kernel, dim3(blocks_for(padded_elems(lv, l), 256), m), dim3(256), 0, st, 1, b,
+                                  s.deriv, lv.ofs[l], lv.w[l], lv.h[l]));
+    }
+    if (corners) {
+      STA_CHECK_CUDA(launch_pdl(sobel_kernel, dim3(blocks_for(hw, 256), m), dim3(256), 0, st, 1, b, s, W, H));
+      STA_CHECK_CUDA(launch_pdl(min_eigen_kernel, dim3(blocks_for(hw, 256), m), dim3(256), 0, st, 1, b, s, W, H));
+      STA_CHECK_CUDA(launch_pdl(candidates_kernel, dim3(blocks_for(hw, 256), m), dim3(256), 0, st, 1, b, s, W, H));
+      STA_CHECK_CUDA(launch_pdl(select_kernel, dim3(m), dim3(kSelectThreads), 0, st, 1, b, s, W, H));
+      STA_CHECK_CUDA(launch_pdl(rank_kernel, dim3(blocks_for(s.acc_cap, 256), m), dim3(256), 0, st, 1, b, s, W));
+    }
+  }
   return 0;
 }
 
-int lk(const Layout& s, const uint8_t* I, const short2* dI, const uint8_t* J, const float2* pts, const int* n_dev,
-       int n_host, float2* next_out, uint8_t* status_out, cudaStream_t st) {
-  const int n_max = n_dev ? kMaxCorners : n_host;
-  if (n_max == 0) return 0;
-  STA_CHECK_CUDA(launch_pdl(lk_kernel, dim3(blocks_for(n_max, 4)), dim3(128), 0, st, 1, s.lv, I, dI, J, pts, n_dev, n_host,
-                            next_out, status_out));
+// LK of n items (n_host points each where an item has no device count), then, if stats is not NULL, each item's
+// statistics into stats[i]
+int track_items(const Layout& s, int n, const LkItem* items, int n_host, StaFlowStats* stats, cudaStream_t st) {
+  for (int c0 = 0; c0 < n; c0 += kMaxBatch) {
+    const int m = n - c0 < kMaxBatch ? n - c0 : kMaxBatch;
+    LkBatch b = {};
+    for (int i = 0; i < m; ++i) b.it[i] = items[c0 + i];
+    const int n_max = b.it[0].n_dev ? kMaxCorners : n_host;
+    if (n_max > 0)
+      STA_CHECK_CUDA(launch_pdl(lk_kernel, dim3(blocks_for(n_max, 4), m), dim3(128), 0, st, 1, s.lv, b, n_host));
+    if (stats) STA_CHECK_CUDA(launch_pdl(flow_stats_kernel, dim3(m), dim3(256), 0, st, 1, b, stats + c0));
+  }
   return 0;
 }
 
@@ -624,12 +717,24 @@ struct StaFlowTracker {
   int H = 0, W = 0;
   Layout s;
   void* arena = nullptr;
-  int kf = 0;                          // which pyramid holds the keyframe
+  uint8_t* kf_pyr = nullptr;   // the keyframe's pyramid
+  uint8_t* cur_pyr = nullptr;  // the frame of the last sta_flow_track; sta_flow_promote swaps the two
   bool has_kf = false, has_cur = false;  // a keyframe was set / a frame was tracked since
   StaFlowStats* pinned = nullptr;      // host copy of the statistics
   cudaStream_t last_stream = nullptr;
   bool has_stream = false;
   cudaEvent_t ev_switch = nullptr;
+  // Group tracks.  Frame pyramid slots, allocated on first use and grown to the most frames this tracker had in one
+  // group: frame j of its last group track is in slots[j] (group_n frames).  A group promotion of frame j swaps
+  // slots[j] with kf_pyr, and the frames after it stay held in slots[held_first, held_first + held_n) for the next
+  // group track to reuse.
+  std::vector<uint8_t*> slots;
+  std::vector<void*> slot_allocs;
+  int group_n = 0, held_first = 0, held_n = 0;
+  // when this tracker is the first of a group: LK output and statistics of every frame of the group
+  int gcap = 0;
+  void* gbuf = nullptr;  // [gcap][1000] float2 next points, [gcap][1000] uint8 status, [gcap] StaFlowStats
+  StaFlowStats* gpinned = nullptr;
 };
 
 namespace {
@@ -649,13 +754,64 @@ int bind_stream(StaFlowTracker* t, cudaStream_t st) {
   return 0;
 }
 
-uint8_t* pyr_of(StaFlowTracker* t, int which) { return at<uint8_t>(t->arena, t->s.pyr[which]); }
+KfJob kf_job(StaFlowTracker* t) {
+  return KfJob{t->kf_pyr, t->arena, at<float2>(t->arena, t->s.corners), at<int>(t->arena, t->s.ncorners)};
+}
 
-// derivatives + corners of the keyframe pyramid
-int keyframe_products(StaFlowTracker* t, cudaStream_t st) {
-  const Layout& s = t->s;
-  if (int rc = build_derivs(s, pyr_of(t, t->kf), at<short2>(t->arena, s.deriv), st)) return rc;
-  return good_features(s, t->arena, pyr_of(t, t->kf), at<float2>(t->arena, s.corners), at<int>(t->arena, s.ncorners), st);
+LkItem lk_item(StaFlowTracker* t, const uint8_t* J, float2* next, uint8_t* status) {
+  return LkItem{t->kf_pyr, at<const short2>(t->arena, t->s.deriv), J, at<const float2>(t->arena, t->s.corners),
+                at<const int>(t->arena, t->s.ncorners), next, status};
+}
+
+// a one-frame call ends whatever group track the tracker was in
+void end_group(StaFlowTracker* t) { t->group_n = t->held_n = 0; }
+
+size_t group_stats_offset(int cap) {
+  return (static_cast<size_t>(cap) * kMaxCorners * (sizeof(float2) + 1) + 255) & ~static_cast<size_t>(255);
+}
+
+int ensure_group_buffers(StaFlowTracker* t, int F) {
+  if (F <= t->gcap) return 0;
+  const int cap = (F + 15) / 16 * 16;
+  // the previous buffers' last use ended in the synchronisation of the group track that used them
+  if (t->gbuf) cudaFree(t->gbuf);
+  if (t->gpinned) cudaFreeHost(t->gpinned);
+  t->gbuf = nullptr;
+  t->gpinned = nullptr;
+  t->gcap = 0;
+  STA_CHECK_CUDA(cudaMalloc(&t->gbuf, group_stats_offset(cap) + cap * sizeof(StaFlowStats)));
+  STA_CHECK_CUDA(cudaMallocHost(reinterpret_cast<void**>(&t->gpinned), cap * sizeof(StaFlowStats)));
+  t->gcap = cap;
+  return 0;
+}
+
+int ensure_slots(StaFlowTracker* t, int m) {
+  const int have = static_cast<int>(t->slots.size());
+  if (m <= have) return 0;
+  const size_t bytes = (static_cast<size_t>(t->s.lv.total) + 255) & ~static_cast<size_t>(255);
+  void* p = nullptr;
+  STA_CHECK_CUDA(cudaMalloc(&p, bytes * (m - have)));
+  t->slot_allocs.push_back(p);
+  for (int i = 0; i < m - have; ++i) t->slots.push_back(static_cast<uint8_t*>(p) + bytes * i);
+  return 0;
+}
+
+// the trackers of a group: non-null, of one frame size, and either one entry per tracker (distinct) or a tracker's
+// frames consecutive.  Refusals only, no CUDA call.
+int check_group(StaFlowTracker* const* ts, int F, bool distinct) {
+  STA_REQUIRE(ts != nullptr && F >= 1, "empty group");
+  for (int f = 0; f < F; ++f) {
+    STA_REQUIRE(ts[f] != nullptr, "null tracker");
+    STA_REQUIRE(ts[f]->H == ts[0]->H && ts[f]->W == ts[0]->W, "the trackers of a group must share one frame size");
+    if (f > 0 && ts[f] == ts[f - 1]) {
+      STA_REQUIRE(!distinct, "a tracker appears twice in the group");
+      continue;
+    }
+    for (int g = 0; g < f; ++g)
+      STA_REQUIRE(ts[g] != ts[f], distinct ? "a tracker appears twice in the group"
+                                           : "a tracker's frames must be consecutive in the group");
+  }
+  return 0;
 }
 
 }  // namespace
@@ -679,28 +835,53 @@ int sta_flow_create(int H, int W, StaFlowTracker** out) {
     sta_flow_destroy(t);
     return 1;
   }
+  t->kf_pyr = at<uint8_t>(t->arena, t->s.pyr[0]);
+  t->cur_pyr = at<uint8_t>(t->arena, t->s.pyr[1]);
   *out = t;
   return 0;
 }
 
 void sta_flow_destroy(StaFlowTracker* t) {
   if (!t) return;
-  if (t->arena || t->pinned) cudaDeviceSynchronize();
+  if (t->arena || t->pinned || t->gbuf || !t->slot_allocs.empty()) cudaDeviceSynchronize();
   if (t->arena) cudaFree(t->arena);
+  for (void* p : t->slot_allocs) cudaFree(p);
+  if (t->gbuf) cudaFree(t->gbuf);
   if (t->pinned) cudaFreeHost(t->pinned);
+  if (t->gpinned) cudaFreeHost(t->gpinned);
   if (t->ev_switch) cudaEventDestroy(t->ev_switch);
   delete t;
 }
 
 int sta_flow_set_keyframe(StaFlowTracker* t, const void* frame_dev, int frame_is_f32, void* stream) {
   STA_REQUIRE(t != nullptr && frame_dev != nullptr, "null argument");
+  return sta_flow_set_keyframe_group(&t, 1, frame_dev, frame_is_f32, stream);
+}
+
+int sta_flow_set_keyframe_group(StaFlowTracker* const* ts, int n, const void* frames_dev, int frames_is_f32,
+                                void* stream) {
+  if (int rc = check_group(ts, n, true)) return rc;
+  STA_REQUIRE(frames_dev != nullptr, "null frames");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (int rc = bind_stream(t, st)) return rc;
-  if (int rc = build_pyramid(t->s, frame_dev, frame_is_f32, pyr_of(t, t->kf), st)) return rc;
-  if (int rc = keyframe_products(t, st)) return rc;
+  const Layout& s = ts[0]->s;
+  const size_t frame_bytes = static_cast<size_t>(ts[0]->H) * ts[0]->W * (frames_is_f32 ? sizeof(float) : 1);
+  std::vector<const void*> src(n);
+  std::vector<uint8_t*> dst(n);
+  std::vector<KfJob> jobs(n);
+  for (int i = 0; i < n; ++i) {
+    if (int rc = bind_stream(ts[i], st)) return rc;
+    src[i] = static_cast<const char*>(frames_dev) + frame_bytes * i;
+    dst[i] = ts[i]->kf_pyr;
+    jobs[i] = kf_job(ts[i]);
+  }
+  if (int rc = build_pyramids(s, n, src.data(), frames_is_f32, dst.data(), st)) return rc;
+  if (int rc = keyframe_products(s, n, jobs.data(), true, true, st)) return rc;
   STA_CHECK_CUDA(cudaGetLastError());
-  t->has_kf = true;
-  t->has_cur = false;
+  for (int i = 0; i < n; ++i) {
+    ts[i]->has_kf = true;
+    ts[i]->has_cur = false;
+    end_group(ts[i]);
+  }
   return 0;
 }
 
@@ -710,22 +891,79 @@ int sta_flow_track(StaFlowTracker* t, const void* frame_dev, int frame_is_f32, S
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (int rc = bind_stream(t, st)) return rc;
   const Layout& s = t->s;
-  const int cur = 1 - t->kf;
-  if (int rc = build_pyramid(s, frame_dev, frame_is_f32, pyr_of(t, cur), st)) return rc;
+  end_group(t);
+  if (int rc = build_pyramids(s, 1, &frame_dev, frame_is_f32, &t->cur_pyr, st)) return rc;
   t->has_cur = true;
-  const int* n_dev = at<int>(t->arena, s.ncorners);
-  const float2* kf_pts = at<float2>(t->arena, s.corners);
-  float2* next_pts = at<float2>(t->arena, s.next_pts);
-  uint8_t* status = at<uint8_t>(t->arena, s.status);
-  if (int rc = lk(s, pyr_of(t, t->kf), at<short2>(t->arena, s.deriv), pyr_of(t, cur), kf_pts, n_dev, 0, next_pts, status,
-                  st))
-    return rc;
+  const LkItem item = lk_item(t, t->cur_pyr, at<float2>(t->arena, s.next_pts), at<uint8_t>(t->arena, s.status));
   StaFlowStats* dstats = at<StaFlowStats>(t->arena, s.stats);
-  STA_CHECK_CUDA(launch_pdl(flow_stats_kernel, dim3(1), dim3(256), 0, st, 1, kf_pts, static_cast<const float2*>(next_pts),
-                            static_cast<const uint8_t*>(status), n_dev, dstats));
+  if (int rc = track_items(s, 1, &item, 0, dstats, st)) return rc;
   STA_CHECK_CUDA(cudaMemcpyAsync(t->pinned, dstats, sizeof(StaFlowStats), cudaMemcpyDeviceToHost, st));
   STA_CHECK_CUDA(cudaStreamSynchronize(st));
   *stats_out = *t->pinned;
+  return 0;
+}
+
+int sta_flow_track_group(StaFlowTracker* const* ts, int F, const int* held_host, const void* frames_dev,
+                         int frames_is_f32, StaFlowStats* stats_out, void* stream) {
+  if (int rc = check_group(ts, F, false)) return rc;
+  STA_REQUIRE(stats_out != nullptr, "null argument");
+  // per frame: its index among its tracker's frames, and whether it is held
+  std::vector<int> j_of(F);
+  int n_new = 0;
+  for (int f = 0; f < F; ++f) {
+    StaFlowTracker* t = ts[f];
+    STA_REQUIRE(t->has_kf, "no keyframe: call sta_flow_set_keyframe first");
+    j_of[f] = (f > 0 && ts[f - 1] == t) ? j_of[f - 1] + 1 : 0;
+    const bool held = held_host && held_host[f];
+    if (held) {
+      STA_REQUIRE(j_of[f] == 0 || held_host[f - 1], "a tracker's held frames must come first");
+      STA_REQUIRE(j_of[f] < t->held_n, "more held frames than the tracker holds");
+    } else {
+      ++n_new;
+    }
+  }
+  STA_REQUIRE(n_new == 0 || frames_dev != nullptr, "null frames");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const Layout& s = ts[0]->s;
+  for (int f = 0; f < F; ++f) {
+    StaFlowTracker* t = ts[f];
+    if (j_of[f] != 0) continue;
+    if (int rc = bind_stream(t, st)) return rc;
+    int m = 1;
+    while (f + m < F && ts[f + m] == t) ++m;
+    // the held frames move to the front of the slots, in order
+    const int k = held_host ? static_cast<int>(std::count(held_host + f, held_host + f + m, 1)) : 0;
+    if (k > 0) std::rotate(t->slots.begin(), t->slots.begin() + t->held_first, t->slots.end());
+    if (int rc = ensure_slots(t, m)) return rc;
+  }
+  if (int rc = ensure_group_buffers(ts[0], F)) return rc;
+  float2* gnext = static_cast<float2*>(ts[0]->gbuf);
+  uint8_t* gstatus = reinterpret_cast<uint8_t*>(gnext + static_cast<size_t>(ts[0]->gcap) * kMaxCorners);
+  StaFlowStats* gstats = at<StaFlowStats>(ts[0]->gbuf, group_stats_offset(ts[0]->gcap));
+  const size_t frame_bytes = static_cast<size_t>(s.lv.w[0]) * s.lv.h[0] * (frames_is_f32 ? sizeof(float) : 1);
+  std::vector<const void*> src;
+  std::vector<uint8_t*> dst;
+  std::vector<LkItem> items(F);
+  for (int f = 0; f < F; ++f) {
+    StaFlowTracker* t = ts[f];
+    uint8_t* J = t->slots[j_of[f]];
+    if (!(held_host && held_host[f])) {
+      src.push_back(static_cast<const char*>(frames_dev) + frame_bytes * src.size());
+      dst.push_back(J);
+    }
+    items[f] = lk_item(t, J, gnext + static_cast<size_t>(f) * kMaxCorners, gstatus + static_cast<size_t>(f) * kMaxCorners);
+  }
+  for (int f = 0; f < F; ++f) {
+    ts[f]->has_cur = false;
+    ts[f]->held_n = 0;
+    ts[f]->group_n = j_of[f] + 1;
+  }
+  if (n_new > 0)
+    if (int rc = build_pyramids(s, n_new, src.data(), frames_is_f32, dst.data(), st)) return rc;
+  if (int rc = track_items(s, F, items.data(), 0, gstats, st)) return rc;
+  STA_CHECK_CUDA(cudaMemcpyAsync(ts[0]->gpinned, gstats, F * sizeof(StaFlowStats), cudaMemcpyDeviceToHost, st));
+  STA_CHECK_CUDA(cudaStreamSynchronize(st));
+  for (int f = 0; f < F; ++f) stats_out[f] = ts[0]->gpinned[f];
   return 0;
 }
 
@@ -734,9 +972,34 @@ int sta_flow_promote(StaFlowTracker* t, void* stream) {
   STA_REQUIRE(t->has_cur, "no tracked frame to promote");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (int rc = bind_stream(t, st)) return rc;
-  t->kf = 1 - t->kf;
+  std::swap(t->kf_pyr, t->cur_pyr);
   t->has_cur = false;
-  if (int rc = keyframe_products(t, st)) return rc;
+  end_group(t);
+  const KfJob job = kf_job(t);
+  if (int rc = keyframe_products(t->s, 1, &job, true, true, st)) return rc;
+  STA_CHECK_CUDA(cudaGetLastError());
+  return 0;
+}
+
+int sta_flow_promote_group(StaFlowTracker* const* ts, int n, const int* frame_host, void* stream) {
+  if (int rc = check_group(ts, n, true)) return rc;
+  STA_REQUIRE(frame_host != nullptr, "null argument");
+  for (int i = 0; i < n; ++i)
+    STA_REQUIRE(frame_host[i] >= 0 && frame_host[i] < ts[i]->group_n, "no such frame in the tracker's last group track");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  std::vector<KfJob> jobs(n);
+  for (int i = 0; i < n; ++i) {
+    StaFlowTracker* t = ts[i];
+    if (int rc = bind_stream(t, st)) return rc;
+    const int j = frame_host[i];
+    std::swap(t->kf_pyr, t->slots[j]);
+    t->held_first = j + 1;
+    t->held_n = t->group_n - j - 1;
+    t->group_n = 0;
+    t->has_cur = false;
+    jobs[i] = kf_job(t);
+  }
+  if (int rc = keyframe_products(ts[0]->s, n, jobs.data(), true, true, st)) return rc;
   STA_CHECK_CUDA(cudaGetLastError());
   return 0;
 }
@@ -758,8 +1021,7 @@ int sta_flow_keyframe_level0(StaFlowTracker* t, uint8_t* gray_out_dev, int16_t* 
   const int pw = t->W + 2 * kPad;
   const size_t inner = static_cast<size_t>(kPad) * pw + kPad;
   if (gray_out_dev)
-    STA_CHECK_CUDA(cudaMemcpy2DAsync(gray_out_dev, t->W, pyr_of(t, t->kf) + inner, pw, t->W, t->H, cudaMemcpyDeviceToDevice,
-                                     st));
+    STA_CHECK_CUDA(cudaMemcpy2DAsync(gray_out_dev, t->W, t->kf_pyr + inner, pw, t->W, t->H, cudaMemcpyDeviceToDevice, st));
   if (deriv_out_dev)
     STA_CHECK_CUDA(cudaMemcpy2DAsync(deriv_out_dev, t->W * sizeof(short2), at<short2>(t->arena, t->s.deriv) + inner,
                                      pw * sizeof(short2), t->W * sizeof(short2), t->H, cudaMemcpyDeviceToDevice, st));
@@ -773,10 +1035,10 @@ int sta_op_good_features(const uint8_t* gray_u8, int H, int W, float* pts_out, i
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const Layout s = make_layout(H, W);
   uint8_t* pyr = at<uint8_t>(scratch, s.pyr[0]);
-  const long long n0 = static_cast<long long>(W + 2 * kPad) * (H + 2 * kPad);
-  STA_CHECK_CUDA(launch_pdl(level0_kernel, dim3(blocks_for(n0, 256)), dim3(256), 0, st, 1,
-                            static_cast<const void*>(gray_u8), 0, H, W, pyr));
-  if (int rc = good_features(s, scratch, pyr, reinterpret_cast<float2*>(pts_out), count_out, st)) return rc;
+  const void* src = gray_u8;
+  if (int rc = build_pyramids(s, 1, &src, 0, &pyr, st)) return rc;
+  const KfJob job{pyr, scratch, reinterpret_cast<float2*>(pts_out), count_out};
+  if (int rc = keyframe_products(s, 1, &job, false, true, st)) return rc;
   STA_CHECK_CUDA(cudaGetLastError());
   return 0;
 }
@@ -788,15 +1050,14 @@ int sta_op_lk_track(const uint8_t* prev_u8, const uint8_t* next_u8, int H, int W
   STA_REQUIRE(prev_u8 && next_u8 && scratch && (n == 0 || (pts && next_pts_out && status_out)), "null pointer");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const Layout s = make_layout(H, W);
-  uint8_t* I = at<uint8_t>(scratch, s.pyr[0]);
-  uint8_t* J = at<uint8_t>(scratch, s.pyr[1]);
-  short2* dI = at<short2>(scratch, s.deriv);
-  if (int rc = build_pyramid(s, prev_u8, 0, I, st)) return rc;
-  if (int rc = build_pyramid(s, next_u8, 0, J, st)) return rc;
-  if (int rc = build_derivs(s, I, dI, st)) return rc;
-  if (int rc = lk(s, I, dI, J, reinterpret_cast<const float2*>(pts), nullptr, n, reinterpret_cast<float2*>(next_pts_out),
-                  status_out, st))
-    return rc;
+  uint8_t* pyr[2] = {at<uint8_t>(scratch, s.pyr[0]), at<uint8_t>(scratch, s.pyr[1])};
+  const void* src[2] = {prev_u8, next_u8};
+  if (int rc = build_pyramids(s, 2, src, 0, pyr, st)) return rc;
+  const KfJob job{pyr[0], scratch, nullptr, nullptr};
+  if (int rc = keyframe_products(s, 1, &job, true, false, st)) return rc;
+  const LkItem item{pyr[0], at<const short2>(scratch, s.deriv), pyr[1], reinterpret_cast<const float2*>(pts), nullptr,
+                    reinterpret_cast<float2*>(next_pts_out), status_out};
+  if (int rc = track_items(s, 1, &item, n, nullptr, st)) return rc;
   STA_CHECK_CUDA(cudaGetLastError());
   return 0;
 }

@@ -116,12 +116,15 @@ __device__ __forceinline__ int clip8(int v) {
   return v < 0 ? 0 : (v > 255 ? 255 : v);
 }
 
-// horizontal pass: src frame rows [t, t + H1), columns [l, l + W1)  ->  tmp [H1][rw][3] uint8
+// horizontal pass: src frame rows [t, t + H1), columns [l, l + W1)  ->  tmp [H1][rw][3] uint8; frame blockIdx.y of
+// [F][src_h][src_w][3] into tmp [F][H1][rw][3]
 __global__ void __launch_bounds__(256)
-resample_h_kernel(const uint8_t* __restrict__ src, int src_w, int l, int t, int H1, int rw, int ksize,
+resample_h_kernel(const uint8_t* __restrict__ src, int src_h, int src_w, int l, int t, int H1, int rw, int ksize,
                   const int* __restrict__ bounds, const int* __restrict__ kk, uint8_t* __restrict__ tmp) {
   pdl_wait();
   pdl_launch_dependents();
+  src += static_cast<long long>(blockIdx.y) * src_h * src_w * 3;
+  tmp += static_cast<long long>(blockIdx.y) * H1 * rw * 3;
   const int idx = blockIdx.x * 256 + threadIdx.x;
   if (idx >= H1 * rw) return;
   const int y = idx / rw, xx = idx - y * rw;
@@ -142,13 +145,19 @@ resample_h_kernel(const uint8_t* __restrict__ src, int src_w, int l, int t, int 
 }
 
 // vertical pass restricted to the final crop + ToTensor / Normalize / Grayscale:
-// tmp [H1][rw][3] -> rgb [3][oh][ow] fp32 in [-1, 1], gray [oh][ow] fp32 in [0, 1], u8 [oh][ow][3] (optional)
+// tmp [H1][rw][3] -> rgb [3][oh][ow] fp32 in [-1, 1], gray [oh][ow] fp32 in [0, 1], u8 [oh][ow][3] (optional);
+// frame blockIdx.y of [F] of each
 __global__ void __launch_bounds__(256)
-resample_v_finish_kernel(const uint8_t* __restrict__ tmp, int rw, int l2, int t2, int ow, int oh, int ksize,
+resample_v_finish_kernel(const uint8_t* __restrict__ tmp, int H1, int rw, int l2, int t2, int ow, int oh, int ksize,
                          const int* __restrict__ bounds, const int* __restrict__ kk, int vertical_identity,
                          float* __restrict__ rgb, float* __restrict__ gray, uint8_t* __restrict__ u8) {
   pdl_wait();
   pdl_launch_dependents();
+  const long long plane = static_cast<long long>(ow) * oh, f = blockIdx.y;
+  tmp += f * H1 * rw * 3;
+  rgb += f * 3 * plane;
+  if (gray) gray += f * plane;
+  if (u8) u8 += f * plane * 3;
   const int idx = blockIdx.x * 256 + threadIdx.x;
   if (idx >= ow * oh) return;
   const int py = idx / ow, px = idx - py * ow;
@@ -175,7 +184,6 @@ resample_v_finish_kernel(const uint8_t* __restrict__ tmp, int rw, int l2, int t2
   // every operation rounded separately as the elementwise torch kernels do
   const float f0 = __fdiv_rn(static_cast<float>(c0), 255.0f), f1 = __fdiv_rn(static_cast<float>(c1), 255.0f),
               f2 = __fdiv_rn(static_cast<float>(c2), 255.0f);
-  const long long plane = static_cast<long long>(ow) * oh;
   rgb[idx] = __fdiv_rn(__fsub_rn(f0, 0.5f), 0.5f);
   rgb[plane + idx] = __fdiv_rn(__fsub_rn(f1, 0.5f), 0.5f);
   rgb[2 * plane + idx] = __fdiv_rn(__fsub_rn(f2, 0.5f), 0.5f);
@@ -187,16 +195,18 @@ resample_v_finish_kernel(const uint8_t* __restrict__ tmp, int rw, int l2, int t2
   }
 }
 
-// per (device, frame geometry): coefficient tables and the intermediate image; SLAM streams have one frame size
+// per (device, frame geometry): coefficient tables and the intermediate images of up to tmp_frames frames; SLAM
+// streams have one frame size
 struct Plan {
   Geometry g;
   int ksize_h = 0, ksize_v = 0;
   int *d_bh = nullptr, *d_kh = nullptr, *d_bv = nullptr, *d_kv = nullptr;
   uint8_t* d_tmp = nullptr;
+  int tmp_frames = 0;
 };
 typedef std::tuple<int, int, int, int, int, int, int> PlanKey;
 
-int get_plan(int H, int W, int res_w, int res_h, int w_edge, int h_edge, const Plan** out) {
+int get_plan(int H, int W, int res_w, int res_h, int w_edge, int h_edge, Plan** out) {
   static std::mutex mu;
   static std::map<PlanKey, Plan> plans;
   int dev = 0;
@@ -224,7 +234,20 @@ int get_plan(int H, int W, int res_w, int res_h, int w_edge, int h_edge, const P
   };
   if (upload(bh, &p.d_bh) || upload(kh, &p.d_kh) || upload(bv, &p.d_bv) || upload(kv, &p.d_kv)) return 1;
   STA_CHECK_CUDA(cudaMalloc(&p.d_tmp, static_cast<size_t>(p.g.H1) * p.g.rw * 3));
+  p.tmp_frames = 1;
   *out = &plans.emplace(key, p).first->second;
+  return 0;
+}
+
+// room for F intermediate images; the old buffer's last use is on `stream` (a geometry is used on one stream at a time)
+int grow_tmp(Plan* p, int F, cudaStream_t stream) {
+  if (F <= p->tmp_frames) return 0;
+  STA_CHECK_CUDA(cudaStreamSynchronize(stream));
+  STA_CHECK_CUDA(cudaFree(p->d_tmp));
+  p->d_tmp = nullptr;
+  p->tmp_frames = 0;
+  STA_CHECK_CUDA(cudaMalloc(&p->d_tmp, static_cast<size_t>(F) * p->g.H1 * p->g.rw * 3));
+  p->tmp_frames = F;
   return 0;
 }
 
@@ -250,10 +273,11 @@ int preprocess_coeffs(int in_size, int out_size, int* ksize_out, int* bounds_out
   return 0;
 }
 
-int launch_preprocess_rgb8(const uint8_t* rgb_dev, int H, int W, int res_w, int res_h, int w_edge, int h_edge,
+int launch_preprocess_rgb8(const uint8_t* rgb_dev, int F, int H, int W, int res_w, int res_h, int w_edge, int h_edge,
                            float* rgb_out, float* gray_out, uint8_t* u8_out, int* out_hw_host, int query_only,
                            cudaStream_t stream) {
   STA_REQUIRE(H > 0 && W > 0 && res_w > 0 && res_h > 0 && w_edge >= 0 && h_edge >= 0, "bad arguments");
+  STA_REQUIRE(F >= 1 && F <= 65535, "frame count must be in [1, 65535]");
   if (query_only) {
     Geometry g;
     if (int rc = make_geometry(H, W, res_w, res_h, w_edge, h_edge, &g)) return rc;
@@ -261,17 +285,19 @@ int launch_preprocess_rgb8(const uint8_t* rgb_dev, int H, int W, int res_w, int 
     return 0;
   }
   STA_REQUIRE(rgb_dev && rgb_out, "null pointer");
-  const Plan* p = nullptr;
+  Plan* p = nullptr;
   if (int rc = get_plan(H, W, res_w, res_h, w_edge, h_edge, &p)) return rc;
+  if (int rc = grow_tmp(p, F, stream)) return rc;
   const Geometry& g = p->g;
   if (out_hw_host) { out_hw_host[0] = g.oh; out_hw_host[1] = g.ow; }
   // horizontal pass (an identity pass still copies the crop window: same code, the coefficients are then 1 << 22)
   const int n1 = g.H1 * g.rw;
-  STA_CHECK_CUDA(launch_pdl(resample_h_kernel, dim3((n1 + 255) / 256), dim3(256), 0, stream, 1, rgb_dev, W, g.l, g.t, g.H1,
-                            g.rw, p->ksize_h, static_cast<const int*>(p->d_bh), static_cast<const int*>(p->d_kh), p->d_tmp));
+  STA_CHECK_CUDA(launch_pdl(resample_h_kernel, dim3((n1 + 255) / 256, F), dim3(256), 0, stream, 1, rgb_dev, H, W, g.l, g.t,
+                            g.H1, g.rw, p->ksize_h, static_cast<const int*>(p->d_bh), static_cast<const int*>(p->d_kh),
+                            p->d_tmp));
   const int n2 = g.ow * g.oh;
-  STA_CHECK_CUDA(launch_pdl(resample_v_finish_kernel, dim3((n2 + 255) / 256), dim3(256), 0, stream, 1,
-                            static_cast<const uint8_t*>(p->d_tmp), g.rw, g.l2, g.t2, g.ow, g.oh, p->ksize_v,
+  STA_CHECK_CUDA(launch_pdl(resample_v_finish_kernel, dim3((n2 + 255) / 256, F), dim3(256), 0, stream, 1,
+                            static_cast<const uint8_t*>(p->d_tmp), g.H1, g.rw, g.l2, g.t2, g.ow, g.oh, p->ksize_v,
                             static_cast<const int*>(p->d_bv), static_cast<const int*>(p->d_kv), g.rh == g.H1 ? 1 : 0, rgb_out,
                             gray_out, u8_out));
   STA_CHECK_CUDA(cudaGetLastError());

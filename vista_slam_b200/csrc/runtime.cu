@@ -1938,7 +1938,8 @@ int sta_pose_graph_lm_step(const float* nodes, int num_nodes, const int64_t* edg
 // image preprocessing (preprocess.cu)
 // ---------------------------------------------------------------------------
 int sta_preprocess_shape(int H, int W, int res_w, int res_h, int w_edge, int h_edge, int* out_hw) {
-  return launch_preprocess_rgb8(nullptr, H, W, res_w, res_h, w_edge, h_edge, nullptr, nullptr, nullptr, out_hw, 1, nullptr);
+  return launch_preprocess_rgb8(nullptr, 1, H, W, res_w, res_h, w_edge, h_edge, nullptr, nullptr, nullptr, out_hw, 1,
+                                nullptr);
 }
 int sta_preprocess_geometry(int H, int W, int res_w, int res_h, int w_edge, int h_edge, int* out10) {
   if (!out10) {
@@ -1952,7 +1953,12 @@ int sta_preprocess_coeffs(int in_size, int out_size, int* ksize, int* bounds, in
 }
 int sta_preprocess_rgb8(const uint8_t* rgb_dev, int H, int W, int res_w, int res_h, int w_edge, int h_edge,
                         float* rgb_out_dev, float* gray_out_dev, uint8_t* u8_out_dev, void* stream) {
-  return launch_preprocess_rgb8(rgb_dev, H, W, res_w, res_h, w_edge, h_edge, rgb_out_dev, gray_out_dev, u8_out_dev,
+  return sta_preprocess_rgb8_many(rgb_dev, 1, H, W, res_w, res_h, w_edge, h_edge, rgb_out_dev, gray_out_dev, u8_out_dev,
+                                  stream);
+}
+int sta_preprocess_rgb8_many(const uint8_t* rgb_dev, int F, int H, int W, int res_w, int res_h, int w_edge, int h_edge,
+                             float* rgb_out_dev, float* gray_out_dev, uint8_t* u8_out_dev, void* stream) {
+  return launch_preprocess_rgb8(rgb_dev, F, H, W, res_w, res_h, w_edge, h_edge, rgb_out_dev, gray_out_dev, u8_out_dev,
                                 nullptr, 0, static_cast<cudaStream_t>(stream));
 }
 

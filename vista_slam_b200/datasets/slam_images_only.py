@@ -48,6 +48,46 @@ class SLAM_image_only:
                        "sta_preprocess_rgb8")
         return {"gray": gray, "rgb": rgb, "img_name": osp.basename(img_name)}
 
+    @torch.no_grad()
+    def process_images(self, rgb_frames, img_names=None, w_edge=10, h_edge=10):
+        """process_image over F same-size HxWx3 uint8 RGB frames (a list, or an (F, H, W, 3) array or tensor) in one
+        launch pair -> {'rgb': (F,3,h,w), 'gray': (F,1,h,w), 'img_name': [basenames]}, CUDA tensors, every frame
+        bit-identical to its own process_image.  rgb[i:i+1] and gray[i] are what step_many and compute_disparity
+        take; gray feeds FlowTracker.compute_disparities as it is."""
+        if isinstance(rgb_frames, (np.ndarray, torch.Tensor)):
+            frames = [rgb_frames[i] for i in range(rgb_frames.shape[0])] if rgb_frames.ndim == 4 else None
+        else:
+            frames = list(rgb_frames)
+        if frames is None or any(not isinstance(f, (np.ndarray, torch.Tensor)) or f.ndim != 3 or f.shape[2] != 3
+                                 or f.dtype not in (np.uint8, torch.uint8) for f in frames):
+            raise ValueError("expected HxWx3 uint8 RGB frames")
+        F = len(frames)
+        if F and len({tuple(f.shape) for f in frames}) > 1:
+            raise ValueError("all frames must have the same size")
+        names = [""] * F if img_names is None else [osp.basename(n) for n in img_names]
+        if len(names) != F:
+            raise ValueError("one image name per frame")
+        if F == 0:
+            raise ValueError("no frames")
+        H, W, _ = frames[0].shape
+        oh, ow = self.output_shape(H, W, w_edge, h_edge)
+        if isinstance(rgb_frames, (np.ndarray, torch.Tensor)):
+            batch = torch.as_tensor(rgb_frames)
+        elif all(isinstance(f, np.ndarray) for f in frames):
+            batch = torch.from_numpy(np.stack(frames))
+        else:
+            batch = torch.stack([torch.as_tensor(f).to(self.device) for f in frames])
+        batch = batch.to(self.device, non_blocking=True).contiguous()
+        if not batch.is_cuda:
+            raise RuntimeError("the CUDA preprocessing has no CPU path")
+        rgb = torch.empty(F, 3, oh, ow, dtype=torch.float32, device=batch.device)
+        gray = torch.empty(F, 1, oh, ow, dtype=torch.float32, device=batch.device)
+        with torch.cuda.device(batch.device):
+            _lib.check(_lib.lib().sta_preprocess_rgb8_many(_lib.ptr(batch), F, H, W, self.resolution[0], self.resolution[1],
+                                                           w_edge, h_edge, _lib.ptr(rgb), _lib.ptr(gray), None,
+                                                           _lib.cur_stream()), "sta_preprocess_rgb8_many")
+        return {"gray": gray, "rgb": rgb, "img_name": names}
+
     def __getitem__(self, i):
         """slam_images_only.py:36-40 (run.py:180,193 index the dataset): read frame i from disk as RGB uint8 (cv2 decodes
         BGR; imread_cv2 in vista_slam/utils/image.py converts) and preprocess it on the device."""
