@@ -351,6 +351,36 @@ int sta_pose_graph_lm_step_sparse(const StaPgPlan* plan, const float* nodes, con
 /* The last step's update d (device, fp64 [num_opt][7] in opt_idx order), for checking the solve: stream-ordered copy. */
 int sta_pg_plan_last_delta(const StaPgPlan* plan, double* delta_out, void* stream);
 
+/* ---- the block-sparse LM step over a group of G plans (1 <= G <= STA_PG_GROUP_MAX), in one launch sequence whose
+ * length does not grow with G: one launch per kernel and elimination-tree level covers every member, the grid's y
+ * dimension selecting the member.  Each active member's nodes_out and info row (info_out[4 k .. 4 k + 3], device,
+ * G x 4 fp64) are bit-identical to sta_pose_graph_lm_step_sparse on its own plan, whatever the other members, their
+ * order and which of them are active: no reduction crosses plans.  An inactive member (active = 0) is neither read nor
+ * written, its info row included.  No host synchronisation; steps and dampings may change on every call.
+ * The group plan borrows the member plans' device arrays and scratch and uploads only its own small tables (creation
+ * synchronises once): the member plans must outlive it, steps on one group plan must not overlap, and a member plan may
+ * be stepped on its own between group steps, in stream order.  A member's sta_pg_plan_last_delta gives its last
+ * update, from whichever entry point ran it.
+ * Refused with a status before any launch: a null pointer, G outside [1, STA_PG_GROUP_MAX], a plan named twice
+ * (its scratch would be shared), a plan created on a device other than the current one, and, at a step, a null
+ * info_out or steps table, an active member with a null nodes, meas, weights or nodes_out, or a current device other
+ * than the group plan's. ---- */
+typedef struct StaPgGroupPlan StaPgGroupPlan; /* opaque */
+int sta_pg_group_plan_create(const StaPgPlan* const* plans, int G, StaPgGroupPlan** out);
+void sta_pg_group_plan_destroy(StaPgGroupPlan* gp);
+/* out4 = {G, elimination-tree levels (the most of any member), kernel launches per step, device bytes of the group plan} */
+int sta_pg_group_plan_info(const StaPgGroupPlan* gp, int64_t* out4);
+typedef struct StaPgSparseStep {
+  const float* nodes;   /* [num_nodes][8] of the member's plan */
+  const float* meas;    /* [num_edges][8] */
+  const float* weights; /* [num_edges][7] */
+  float* nodes_out;     /* [num_nodes][8] */
+  double damping;
+  int active;           /* 0: the member sits this step out */
+} StaPgSparseStep;
+int sta_pose_graph_lm_step_sparse_group(const StaPgGroupPlan* gp, const StaPgSparseStep* steps /* [G] */, double dmin,
+                                        double dmax, double* info_out, void* stream);
+
 /* ---- image preprocessing (SURVEY.md 8(f) rank 3): SLAM_image_only.process_image
  * (vista_slam/datasets/slam_images_only.py:22-34 -> datasets/base/base_view_graph_dataset.py:171-225 ->
  * utils/cropping.py:54-84,102-118 with PIL LANCZOS -> utils/image.py:13) on the device, bit-exact with PIL's 8-bit

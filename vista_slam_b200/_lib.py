@@ -54,7 +54,7 @@ GRAPH_MAX_KEYFRAME_EDGES = 32
 GRAPH_FLAG_NOT_SO3 = 1
 ORB_MAX_KEYPOINTS = 4096
 PG_DENSE_MAX_OPT = 3657  # STA_PG_DENSE_MAX_OPT: above it PoseGraphOpt takes the block-sparse route
-PG_GROUP_MAX = 16  # STA_PG_GROUP_MAX: graphs per sta_pose_graph_lm_step_group call
+PG_GROUP_MAX = 16  # STA_PG_GROUP_MAX: graphs per sta_pose_graph_lm_step_group call or sta_pg_group_plan
 
 
 class StaPgGraph(Structure):
@@ -63,6 +63,13 @@ class StaPgGraph(Structure):
         ("nodes_out", c_void_p),
         ("num_nodes", c_int), ("num_edges", c_int), ("num_opt", c_int),
         ("damping", ctypes.c_double),
+    ]
+
+
+class StaPgSparseStep(Structure):
+    _fields_ = [
+        ("nodes", c_void_p), ("meas", c_void_p), ("weights", c_void_p), ("nodes_out", c_void_p),
+        ("damping", ctypes.c_double), ("active", c_int),
     ]
 
 
@@ -152,6 +159,12 @@ def lib():
     L.sta_pg_plan_last_delta.argtypes = [vp, vp, vp]
     L.sta_pose_graph_lm_step_sparse.argtypes = [vp, vp, vp, vp, ctypes.c_double, ctypes.c_double, ctypes.c_double, vp, vp,
                                                 vp]
+    L.sta_pg_group_plan_create.argtypes = [POINTER(vp), i, POINTER(vp)]
+    L.sta_pg_group_plan_destroy.argtypes = [vp]
+    L.sta_pg_group_plan_destroy.restype = None
+    L.sta_pg_group_plan_info.argtypes = [vp, POINTER(c_int64)]
+    L.sta_pose_graph_lm_step_sparse_group.argtypes = [vp, POINTER(StaPgSparseStep), ctypes.c_double, ctypes.c_double, vp,
+                                                      vp]
     L.sta_flow_create.argtypes = [i, i, POINTER(vp)]
     L.sta_flow_destroy.argtypes = [vp]
     L.sta_flow_destroy.restype = None

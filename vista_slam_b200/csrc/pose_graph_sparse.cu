@@ -36,6 +36,7 @@ namespace sta {
 namespace {
 
 constexpr int kLeaf = 8;  // nested dissection stops at this many nodes
+size_t align_up(size_t n) { return (n + 255) & ~static_cast<size_t>(255); }
 
 struct PgSymbolic {
   int num_nodes = 0, num_edges = 0, n = 0;
@@ -331,13 +332,13 @@ __global__ void sp_info_init_kernel(double* info) { info[3] = 1.0; }  // Cholesk
 // order, same arithmetic: diag += s, A_aa -= s for a self-edge, then A_aa + diag), then pg_damp_kernel's damping, and g_a
 // on threads 49..55.  Off-diagonal block (I, K) = A[order[I]][order[K]]: minus the sum of s over the edges joining the two
 // nodes, in edge order, as row owner order[I] computes it in pg_assemble_kernel.  Fill blocks come out zero.
-__global__ void __launch_bounds__(64)
-sp_assemble_kernel(const long long* __restrict__ edges, const float* __restrict__ weights, const int* __restrict__ opt_map,
-                   const double* __restrict__ r, const double* __restrict__ J, const int* __restrict__ order,
-                   const int* __restrict__ blk_row, const int* __restrict__ blk_col, const int* __restrict__ inc_ptr,
-                   const int* __restrict__ inc, const int* __restrict__ oasm_ptr, const int* __restrict__ oasm, double dmin,
-                   double dmax, double damping, double* __restrict__ L, double* __restrict__ g) {
-  const int b = blockIdx.x;
+__device__ __forceinline__ void sp_assemble(int b, const long long* __restrict__ edges, const float* __restrict__ weights,
+                                            const int* __restrict__ opt_map, const double* __restrict__ r,
+                                            const double* __restrict__ J, const int* __restrict__ order,
+                                            const int* __restrict__ blk_row, const int* __restrict__ blk_col,
+                                            const int* __restrict__ inc_ptr, const int* __restrict__ inc,
+                                            const int* __restrict__ oasm_ptr, const int* __restrict__ oasm, double dmin,
+                                            double dmax, double damping, double* __restrict__ L, double* __restrict__ g) {
   const int t = threadIdx.x;
   const int p = t / 7, q = t - 7 * p;
   const int I = blk_row[b], K = blk_col[b];
@@ -386,12 +387,19 @@ sp_assemble_kernel(const long long* __restrict__ edges, const float* __restrict_
     g[7 * a + (t - 49)] = gv;
   }
 }
+__global__ void __launch_bounds__(64)
+sp_assemble_kernel(const long long* __restrict__ edges, const float* __restrict__ weights, const int* __restrict__ opt_map,
+                   const double* __restrict__ r, const double* __restrict__ J, const int* __restrict__ order,
+                   const int* __restrict__ blk_row, const int* __restrict__ blk_col, const int* __restrict__ inc_ptr,
+                   const int* __restrict__ inc, const int* __restrict__ oasm_ptr, const int* __restrict__ oasm, double dmin,
+                   double dmax, double damping, double* __restrict__ L, double* __restrict__ g) {
+  sp_assemble(blockIdx.x, edges, weights, opt_map, r, J, order, blk_row, blk_col, inc_ptr, inc, oasm_ptr, oasm, dmin, dmax,
+              damping, L, g);
+}
 
 // one CTA per block (I, K) of the level's columns: A_IK -= sum_j L_Ij L_Kj^T over its update list, in list order
-__global__ void __launch_bounds__(64)
-sp_update_kernel(const int* __restrict__ lvl_blk, const long long* __restrict__ upd_ptr, const int2* __restrict__ upd,
-                 double* L) {
-  const int b = lvl_blk[blockIdx.x];
+__device__ __forceinline__ void sp_update(int b, const long long* __restrict__ upd_ptr, const int2* __restrict__ upd,
+                                          double* L) {
   const int t = threadIdx.x;
   if (t >= 49) return;
   const int p = t / 7, q = t - 7 * p;
@@ -406,14 +414,17 @@ sp_update_kernel(const int* __restrict__ lvl_blk, const long long* __restrict__ 
   }
   L[49ll * b + t] = acc;
 }
+__global__ void __launch_bounds__(64)
+sp_update_kernel(const int* __restrict__ lvl_blk, const long long* __restrict__ upd_ptr, const int2* __restrict__ upd,
+                 double* L) {
+  sp_update(lvl_blk[blockIdx.x], upd_ptr, upd, L);
+}
 
 // one CTA per column K of the level: Cholesky of the 7x7 diagonal block (chol_diag_kernel's recurrence on its lower
 // triangle; a non-positive pivot clears info[3] and is replaced by 1), then X L_KK^T = A_IK for every off-diagonal block,
 // one thread per block row (chol_trsm_kernel's recurrence)
-__global__ void __launch_bounds__(128)
-sp_factor_kernel(const int* __restrict__ lvl_col, const int* __restrict__ colptr, double* L, double* info) {
+__device__ __forceinline__ void sp_factor(int K, const int* __restrict__ colptr, double* L, double* info) {
   __shared__ double S[7][8];
-  const int K = lvl_col[blockIdx.x];
   const int t = threadIdx.x;
   const int b0 = colptr[K], nb = colptr[K + 1] - b0;
   double* D = L + 49ll * b0;
@@ -442,14 +453,17 @@ sp_factor_kernel(const int* __restrict__ lvl_col, const int* __restrict__ colptr
     for (int c = 0; c < 7; ++c) ar[c] = x[c];
   }
 }
+__global__ void __launch_bounds__(128)
+sp_factor_kernel(const int* __restrict__ lvl_col, const int* __restrict__ colptr, double* L, double* info) {
+  sp_factor(lvl_col[blockIdx.x], colptr, L, info);
+}
 
 // forward solve L y = -g (positions), one CTA per block row I of the level: rows of earlier levels are final
-__global__ void __launch_bounds__(32)
-sp_forward_kernel(const int* __restrict__ lvl_col, const int* __restrict__ order, const int* __restrict__ colptr,
-                  const int* __restrict__ row_ptr, const int* __restrict__ row_blk, const int* __restrict__ blk_col,
-                  const double* __restrict__ L, const double* __restrict__ g, double* y) {
+__device__ __forceinline__ void sp_forward(int I, const int* __restrict__ order, const int* __restrict__ colptr,
+                                           const int* __restrict__ row_ptr, const int* __restrict__ row_blk,
+                                           const int* __restrict__ blk_col, const double* __restrict__ L,
+                                           const double* __restrict__ g, double* y) {
   __shared__ double b[7];
-  const int I = lvl_col[blockIdx.x];
   const int t = threadIdx.x;
   if (t < 7) {
     double s = -g[7 * order[I] + t];
@@ -473,14 +487,19 @@ sp_forward_kernel(const int* __restrict__ lvl_col, const int* __restrict__ order
   __syncthreads();
   if (t < 7) y[7ll * I + t] = b[t];
 }
+__global__ void __launch_bounds__(32)
+sp_forward_kernel(const int* __restrict__ lvl_col, const int* __restrict__ order, const int* __restrict__ colptr,
+                  const int* __restrict__ row_ptr, const int* __restrict__ row_blk, const int* __restrict__ blk_col,
+                  const double* __restrict__ L, const double* __restrict__ g, double* y) {
+  sp_forward(lvl_col[blockIdx.x], order, colptr, row_ptr, row_blk, blk_col, L, g, y);
+}
 
 // backward solve L^T x = y, one CTA per column K of the level (levels descending): x overwrites y in place, and
 // delta[order[K]] = x_K
-__global__ void __launch_bounds__(32)
-sp_backward_kernel(const int* __restrict__ lvl_col, const int* __restrict__ order, const int* __restrict__ colptr,
-                   const int* __restrict__ blk_row, const double* __restrict__ L, double* y, double* __restrict__ delta) {
+__device__ __forceinline__ void sp_backward(int K, const int* __restrict__ order, const int* __restrict__ colptr,
+                                            const int* __restrict__ blk_row, const double* __restrict__ L, double* y,
+                                            double* __restrict__ delta) {
   __shared__ double b[7];
-  const int K = lvl_col[blockIdx.x];
   const int t = threadIdx.x;
   if (t < 7) {
     double s = y[7ll * K + t];
@@ -506,6 +525,128 @@ sp_backward_kernel(const int* __restrict__ lvl_col, const int* __restrict__ orde
     delta[7ll * order[K] + t] = b[t];
   }
 }
+__global__ void __launch_bounds__(32)
+sp_backward_kernel(const int* __restrict__ lvl_col, const int* __restrict__ order, const int* __restrict__ colptr,
+                   const int* __restrict__ blk_row, const double* __restrict__ L, double* y, double* __restrict__ delta) {
+  sp_backward(lvl_col[blockIdx.x], order, colptr, blk_row, L, y, delta);
+}
+
+// ---------------------------------------------------------------------------
+// group form: one launch sequence steps the active members of a group plan.  blockIdx.y selects the member's descriptor
+// (the last grid dimension of the loss kernels' grid (member)); CTAs past the member's edge, block, column or node
+// count, and levels at or above its level count, return at once.  A member's CTAs run the solo kernels' bodies on its
+// own plan arrays and scratch, so its result does not depend on the group around it.
+// ---------------------------------------------------------------------------
+constexpr int SP_GROUP_MAX = STA_PG_GROUP_MAX;
+
+// a member plan as the kernels see it (uploaded once with the group plan)
+struct SpMember {
+  PgDev d;
+  const int4* lvl;  // [nlev] {first block, blocks, first column, columns} of each level in lvl_blk / lvl_col
+  int nlev, num_nodes, num_edges, n7, nnzb;
+};
+// one active member's step inputs (a kernel parameter of the setup kernel, every step)
+struct SpStepArgs {
+  const float* nodes;
+  const float* meas;
+  const float* weights;
+  float* nodes_out;
+  double* info_out;
+  double damping;
+  int member;
+};
+struct SpGroupParams {
+  SpStepArgs s[SP_GROUP_MAX];
+};
+static_assert(sizeof(SpGroupParams) + 32 <= 4096, "the step arguments must fit the kernel-parameter space");
+struct SpDesc {
+  SpMember m;
+  SpStepArgs s;
+};
+
+// the active members' descriptors into the group plan's table, and each one's Cholesky-ok flag (info[3]) set
+__global__ void sp_group_setup_kernel(const __grid_constant__ SpGroupParams p, int A, const SpMember* __restrict__ members,
+                                      SpDesc* __restrict__ descs) {
+  const int k = threadIdx.x;
+  if (k >= A) return;
+  descs[k].m = members[p.s[k].member];
+  descs[k].s = p.s[k];
+  members[p.s[k].member].d.info[3] = 1.0;
+}
+
+// grid (x, member): residuals and Jacobians at the nodes (second = 0), or residuals alone at the candidate (second = 1)
+__global__ void __launch_bounds__(64) sp_edge_group_kernel(const SpDesc* __restrict__ gd, int second) {
+  const SpDesc& g = gd[blockIdx.y];
+  const PgDev& d = g.m.d;
+  pg_edge(blockIdx.x * blockDim.x + threadIdx.x, second ? g.s.nodes_out : g.s.nodes, d.edges, g.s.meas, d.opt_map,
+          g.m.num_edges, second ? d.r2 : d.r, second ? nullptr : d.J, d.related);
+}
+
+// grid (block of L, member)
+__global__ void __launch_bounds__(64) sp_assemble_group_kernel(const SpDesc* __restrict__ gd, double dmin, double dmax) {
+  const SpDesc& g = gd[blockIdx.y];
+  if (static_cast<int>(blockIdx.x) >= g.m.nnzb) return;
+  const PgDev& d = g.m.d;
+  sp_assemble(blockIdx.x, d.edges, g.s.weights, d.opt_map, d.r, d.J, d.order, d.blk_row, d.blk_col, d.inc_ptr, d.inc,
+              d.oasm_ptr, d.oasm, dmin, dmax, g.s.damping, d.L, d.g);
+}
+
+// grid (member): loss before (second = 0), or loss after and |delta| (second = 1), then the member's info row out
+__global__ void __launch_bounds__(256) sp_loss_group_kernel(const SpDesc* __restrict__ gd, int second) {
+  const SpDesc& g = gd[blockIdx.x];
+  const PgDev& d = g.m.d;
+  if (!second) {
+    pg_loss(d.r, g.s.weights, d.related, g.m.num_edges, nullptr, 0, d.info, 0);
+    return;
+  }
+  pg_loss(d.r2, g.s.weights, d.related, g.m.num_edges, d.delta, g.m.n7, d.info, 1);
+  if (threadIdx.x == 0)  // info[1], info[2] are this thread's own writes; info[0] and info[3] come from earlier launches
+    for (int k = 0; k < 4; ++k) g.s.info_out[k] = d.info[k];
+}
+
+// grid (block of the level, member), levels >= 1
+__global__ void __launch_bounds__(64) sp_update_group_kernel(const SpDesc* __restrict__ gd, int l) {
+  const SpDesc& g = gd[blockIdx.y];
+  if (l >= g.m.nlev) return;
+  const int4 v = g.m.lvl[l];
+  if (static_cast<int>(blockIdx.x) >= v.y) return;
+  sp_update(g.m.d.lvl_blk[v.x + blockIdx.x], g.m.d.upd_ptr, g.m.d.upd, g.m.d.L);
+}
+
+// grid (column of the level, member)
+__global__ void __launch_bounds__(128) sp_factor_group_kernel(const SpDesc* __restrict__ gd, int l) {
+  const SpDesc& g = gd[blockIdx.y];
+  if (l >= g.m.nlev) return;
+  const int4 v = g.m.lvl[l];
+  if (static_cast<int>(blockIdx.x) >= v.w) return;
+  sp_factor(g.m.d.lvl_col[v.z + blockIdx.x], g.m.d.colptr, g.m.d.L, g.m.d.info);
+}
+
+// grid (column of the level, member)
+__global__ void __launch_bounds__(32) sp_forward_group_kernel(const SpDesc* __restrict__ gd, int l) {
+  const SpDesc& g = gd[blockIdx.y];
+  if (l >= g.m.nlev) return;
+  const int4 v = g.m.lvl[l];
+  if (static_cast<int>(blockIdx.x) >= v.w) return;
+  const PgDev& d = g.m.d;
+  sp_forward(d.lvl_col[v.z + blockIdx.x], d.order, d.colptr, d.row_ptr, d.row_blk, d.blk_col, d.L, d.g, d.y);
+}
+
+// grid (column of the level, member)
+__global__ void __launch_bounds__(32) sp_backward_group_kernel(const SpDesc* __restrict__ gd, int l) {
+  const SpDesc& g = gd[blockIdx.y];
+  if (l >= g.m.nlev) return;
+  const int4 v = g.m.lvl[l];
+  if (static_cast<int>(blockIdx.x) >= v.w) return;
+  const PgDev& d = g.m.d;
+  sp_backward(d.lvl_col[v.z + blockIdx.x], d.order, d.colptr, d.blk_row, d.L, d.y, d.delta);
+}
+
+// grid (x, member): nodes_out = Exp(delta_a) node for the optimised nodes, copies of the fixed ones
+__global__ void sp_node_update_group_kernel(const SpDesc* __restrict__ gd) {
+  const SpDesc& g = gd[blockIdx.y];
+  pg_update(blockIdx.x * blockDim.x + threadIdx.x, g.s.nodes, g.m.d.opt_map, g.m.d.delta, g.m.num_nodes, g.s.nodes_out);
+}
 
 }  // namespace
 }  // namespace sta
@@ -518,7 +659,24 @@ struct StaPgPlan {
   int device = 0;
 };
 
+// a group plan: the member plans (borrowed, not owned), the maxima that size its grids, and one device allocation holding
+// the members' descriptors, their level tables and the per-step descriptor table
+struct StaPgGroupPlan {
+  std::vector<const StaPgPlan*> plans;
+  std::vector<int> max_blk, max_col;  // [levels] the largest block / column count any member has at each level
+  int nlev = 0, max_edges = 0, max_nnzb = 0, max_nodes = 0;
+  void* arena = nullptr;
+  sta::SpMember* members = nullptr;
+  sta::SpDesc* descs = nullptr;
+  size_t bytes = 0;
+  int device = 0;
+};
+
 using namespace sta;
+
+namespace {
+int group_launches(int nlev) { return 4 * nlev + 6; }  // setup, edge, assemble, loss, 2 nlev - 1 factor, 2 nlev solve, 3 after
+}  // namespace
 
 extern "C" {
 
@@ -649,6 +807,126 @@ int sta_pg_plan_last_delta(const StaPgPlan* plan, double* delta_out, void* strea
   STA_REQUIRE(plan && delta_out, "null argument");
   STA_CHECK_CUDA(cudaMemcpyAsync(delta_out, plan->d.delta, sizeof(double) * 7 * plan->S.n, cudaMemcpyDeviceToDevice,
                                  static_cast<cudaStream_t>(stream)));
+  return 0;
+}
+
+int sta_pg_group_plan_create(const StaPgPlan* const* plans, int G, StaPgGroupPlan** out) {
+  STA_REQUIRE(out != nullptr, "null output pointer");
+  *out = nullptr;
+  STA_REQUIRE(plans != nullptr, "null plan table");
+  STA_REQUIRE(G >= 1 && G <= SP_GROUP_MAX, "a group holds 1 to STA_PG_GROUP_MAX plans");
+  for (int k = 0; k < G; ++k) {
+    STA_REQUIRE(plans[k] != nullptr, "null plan");
+    for (int j = 0; j < k; ++j)
+      STA_REQUIRE(plans[j] != plans[k], "a plan is named twice in the group (its scratch would be shared)");
+  }
+  int dev = -1;
+  STA_CHECK_CUDA(cudaGetDevice(&dev));
+  for (int k = 0; k < G; ++k) STA_REQUIRE(plans[k]->device == dev, "a plan was created on another device");
+  StaPgGroupPlan* gp = new StaPgGroupPlan();
+  gp->device = dev;
+  gp->plans.assign(plans, plans + G);
+  // layout: members [G], descs [G], then each member's level table
+  size_t off = align_up(sizeof(SpMember) * G);
+  const size_t descs_off = off;
+  off += align_up(sizeof(SpDesc) * G);
+  std::vector<size_t> lvl_off(G);
+  for (int k = 0; k < G; ++k) {
+    const PgSymbolic& S = plans[k]->S;
+    lvl_off[k] = off;
+    off += align_up(sizeof(int4) * S.nlev);
+    gp->nlev = std::max(gp->nlev, S.nlev);
+    gp->max_edges = std::max(gp->max_edges, S.num_edges);
+    gp->max_nodes = std::max(gp->max_nodes, S.num_nodes);
+    gp->max_nnzb = std::max(gp->max_nnzb, static_cast<int>(S.nnzb()));
+  }
+  gp->bytes = off;
+  gp->max_blk.assign(gp->nlev, 0);
+  gp->max_col.assign(gp->nlev, 0);
+  std::vector<char> host(off, 0);
+  cudaError_t e = cudaMalloc(&gp->arena, off);
+  char* base = static_cast<char*>(gp->arena);
+  for (int k = 0; k < G && e == cudaSuccess; ++k) {
+    const PgSymbolic& S = plans[k]->S;
+    int4* lv = reinterpret_cast<int4*>(host.data() + lvl_off[k]);
+    for (int l = 0; l < S.nlev; ++l) {
+      lv[l] = make_int4(S.lvl_blk_ptr[l], S.lvl_blk_ptr[l + 1] - S.lvl_blk_ptr[l], S.lvl_col_ptr[l],
+                        S.lvl_col_ptr[l + 1] - S.lvl_col_ptr[l]);
+      gp->max_blk[l] = std::max(gp->max_blk[l], lv[l].y);
+      gp->max_col[l] = std::max(gp->max_col[l], lv[l].w);
+    }
+    SpMember& m = reinterpret_cast<SpMember*>(host.data())[k];
+    m.d = plans[k]->d;
+    m.lvl = reinterpret_cast<const int4*>(base + lvl_off[k]);
+    m.nlev = S.nlev;
+    m.num_nodes = S.num_nodes;
+    m.num_edges = S.num_edges;
+    m.n7 = 7 * S.n;
+    m.nnzb = static_cast<int>(S.nnzb());
+  }
+  if (e == cudaSuccess) e = cudaMemcpy(gp->arena, host.data(), off, cudaMemcpyHostToDevice);
+  if (e != cudaSuccess) {
+    set_last_error(std::string("sta_pg_group_plan_create: ") + cudaGetErrorString(e));
+    sta_pg_group_plan_destroy(gp);
+    return 1;
+  }
+  gp->members = reinterpret_cast<SpMember*>(base);
+  gp->descs = reinterpret_cast<SpDesc*>(base + descs_off);
+  *out = gp;
+  return 0;
+}
+
+void sta_pg_group_plan_destroy(StaPgGroupPlan* gp) {
+  if (!gp) return;
+  if (gp->arena) {
+    cudaDeviceSynchronize();
+    cudaFree(gp->arena);
+  }
+  delete gp;
+}
+
+int sta_pg_group_plan_info(const StaPgGroupPlan* gp, int64_t* out4) {
+  STA_REQUIRE(gp && out4, "null argument");
+  out4[0] = static_cast<int64_t>(gp->plans.size());
+  out4[1] = gp->nlev;
+  out4[2] = group_launches(gp->nlev);
+  out4[3] = static_cast<int64_t>(gp->bytes);
+  return 0;
+}
+
+int sta_pose_graph_lm_step_sparse_group(const StaPgGroupPlan* gp, const StaPgSparseStep* steps, double dmin, double dmax,
+                                        double* info_out, void* stream) {
+  STA_REQUIRE(gp && steps && info_out, "null pointer");
+  const int G = static_cast<int>(gp->plans.size());
+  SpGroupParams p = {};
+  int A = 0;
+  for (int k = 0; k < G; ++k) {
+    const StaPgSparseStep& q = steps[k];
+    if (!q.active) continue;
+    STA_REQUIRE(q.nodes && q.meas && q.weights && q.nodes_out, "null pointer in an active member");
+    p.s[A++] = SpStepArgs{q.nodes, q.meas, q.weights, q.nodes_out, info_out + 4 * k, q.damping, k};
+  }
+  int dev = -1;
+  STA_CHECK_CUDA(cudaGetDevice(&dev));
+  STA_REQUIRE(dev == gp->device, "the group plan was created on another device");
+  if (A == 0) return 0;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const unsigned a = static_cast<unsigned>(A);
+  SpDesc* descs = gp->descs;
+  sp_group_setup_kernel<<<1, 32, 0, st>>>(p, A, gp->members, descs);
+  sp_edge_group_kernel<<<dim3((gp->max_edges + 63) / 64, a), 64, 0, st>>>(descs, 0);
+  sp_assemble_group_kernel<<<dim3(gp->max_nnzb, a), 64, 0, st>>>(descs, dmin, dmax);
+  sp_loss_group_kernel<<<a, 256, 0, st>>>(descs, 0);
+  for (int l = 0; l < gp->nlev; ++l) {
+    if (l > 0) sp_update_group_kernel<<<dim3(gp->max_blk[l], a), 64, 0, st>>>(descs, l);  // leaves have no updates
+    sp_factor_group_kernel<<<dim3(gp->max_col[l], a), 128, 0, st>>>(descs, l);
+  }
+  for (int l = 0; l < gp->nlev; ++l) sp_forward_group_kernel<<<dim3(gp->max_col[l], a), 32, 0, st>>>(descs, l);
+  for (int l = gp->nlev - 1; l >= 0; --l) sp_backward_group_kernel<<<dim3(gp->max_col[l], a), 32, 0, st>>>(descs, l);
+  sp_node_update_group_kernel<<<dim3((gp->max_nodes + 127) / 128, a), 128, 0, st>>>(descs);
+  sp_edge_group_kernel<<<dim3((gp->max_edges + 63) / 64, a), 64, 0, st>>>(descs, 1);
+  sp_loss_group_kernel<<<a, 256, 0, st>>>(descs, 1);
+  STA_CHECK_CUDA(cudaGetLastError());
   return 0;
 }
 

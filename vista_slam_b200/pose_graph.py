@@ -8,18 +8,20 @@ Jacobians, normal equations, damped dense Cholesky solve, update and both losses
 32-byte read-back for the accept / reject decision -- the same host round trip pp.optim.LM makes.
 Tensors use PyPose's Sim3 layout (tx ty tz | qx qy qz qw | s), fp32, CUDA only (no CPU path).
 
-Two routes solve the damped normal equations, chosen in the constructor from the number of optimised nodes:
+Two routes solve the damped normal equations, chosen in the constructor (route=None) from the number of optimised nodes:
   * dense (num_opt <= _lib.PG_DENSE_MAX_OPT = 3657): sta_pose_graph_lm_step, a dense fp64 Cholesky of order 7 num_opt;
   * block-sparse (above): sta_pose_graph_lm_step_sparse, a block Cholesky (7x7 blocks) over a plan -- ordering,
     elimination tree, block pattern and update lists -- built on the host from the edge list and the optimised set.
-Both compute the same residuals, Jacobians, normal equations, damping, update and losses.
+Both compute the same residuals, Jacobians, normal equations, damping, update and losses; route="sparse" takes the
+block-sparse route at any size (much faster from a few hundred optimised nodes on), route="dense" insists on the dense one.
 
 Groups: optimize_group(graphs, edges, poses, weights) optimises several independent graphs together and leaves each one
 exactly as its own optimize() would.  Each LM iteration steps every dense-route graph still running with ONE
 sta_pose_graph_lm_step_group launch sequence (the kernels take a graph index, so one launch covers every graph's
-Cholesky panel, triangular solve and so on) and reads all their info rows back with ONE copy; each graph keeps its own
-trust radius and plateau count and leaves the group when its plateau rule stops it.  Block-sparse-route members run
-their own iterations, unchanged, in the same call.  optimize() is a group of one.
+Cholesky panel, triangular solve and so on), every block-sparse-route graph still running with ONE
+sta_pose_graph_lm_step_sparse_group launch sequence (one launch per elimination-tree level covers every graph), and
+reads all their info rows back with ONE copy; each graph keeps its own trust radius and plateau count and leaves the
+group when its plateau rule stops it.  optimize() is a group of one.
 """
 import ctypes
 
@@ -86,7 +88,12 @@ def _lm_iterations(graphs, step, steps, patience, decreasing, radius):
 
 
 class PoseGraphOpt:
-    def __init__(self, nodes, to_optimize_idxs="all"):
+    def __init__(self, nodes, to_optimize_idxs="all", route=None):
+        """route: None picks the block-sparse route above _lib.PG_DENSE_MAX_OPT optimised nodes and the dense one
+        otherwise; "sparse" always takes the block-sparse route; "dense" always takes the dense one and raises
+        ValueError above its limit.  The routes' results agree to rounding, not bit for bit (different orderings)."""
+        if route not in (None, "dense", "sparse"):
+            raise ValueError("route must be None, 'dense' or 'sparse', not %r" % (route,))
         if not nodes.is_cuda:
             raise RuntimeError("vista_slam_b200.pose_graph runs only on CUDA tensors")
         self.nodes = nodes.detach().to(torch.float32).contiguous().clone()
@@ -96,7 +103,10 @@ class PoseGraphOpt:
         self.idxs_opt = torch.as_tensor(to_optimize_idxs, device=nodes.device).long().contiguous()
         self._scratch = None
         self._info = torch.zeros(4, dtype=torch.float64, device=nodes.device)
-        self.sparse = self.idxs_opt.shape[0] > _lib.PG_DENSE_MAX_OPT
+        num_opt = self.idxs_opt.shape[0]
+        if route == "dense" and num_opt > _lib.PG_DENSE_MAX_OPT:
+            raise ValueError("route='dense' takes at most %d optimised nodes, not %d" % (_lib.PG_DENSE_MAX_OPT, num_opt))
+        self.sparse = num_opt > _lib.PG_DENSE_MAX_OPT if route is None else route == "sparse"
         self._plan, self._plan_key = None, None
 
     def get_nodes(self):  # pose_graph.py:94-98
@@ -165,10 +175,10 @@ class PoseGraphOpt:
     def optimize_group(graphs, edges, poses, weights, steps=20, patience=3, decreasing=1e-4, radius=1e4):
         """optimize() on several graphs at once: graphs[k] with edges[k], poses[k], weights[k].  Leaves every graph
         exactly as its own optimize() would and returns each graph's loss history.  Per iteration, the dense-route
-        graphs still running take one sta_pose_graph_lm_step_group launch sequence and one read-back of all their info
-        rows; block-sparse-route graphs run their own iterations in this call.  Refused with ValueError before any
-        launch: lists of different lengths, graphs on different devices, one PoseGraphOpt named twice, and edges, poses
-        and weights whose row counts disagree."""
+        graphs still running take one sta_pose_graph_lm_step_group launch sequence, the block-sparse-route ones one
+        sta_pose_graph_lm_step_sparse_group launch sequence (per PG_GROUP_MAX graphs), and all their info rows come
+        back with one read-back.  Refused with ValueError before any launch: lists of different lengths, graphs on
+        different devices, one PoseGraphOpt named twice, and edges, poses and weights whose row counts disagree."""
         graphs = list(graphs)
         edges, poses, weights = list(edges), list(poses), list(weights)
         if not len(graphs) == len(edges) == len(poses) == len(weights):
@@ -180,20 +190,33 @@ class PoseGraphOpt:
         for e, p, w in zip(edges, poses, weights):
             if p.shape[0] != e.shape[0] or w.shape[0] != e.shape[0]:
                 raise ValueError("edges, poses and weight must have one row per edge")
-        kw = dict(steps=steps, patience=patience, decreasing=decreasing, radius=radius)
-        losses = [None] * len(graphs)
+        if not graphs:
+            return []
         dense = [k for k, g in enumerate(graphs) if not g.sparse]
-        for k, g in enumerate(graphs):
-            if g.sparse:
-                def sparse_step(active, damping, g=g, k=k):
-                    cand, l0, l1, _, ok = g.lm_step(edges[k], poses[k], weights[k], damping[0])
-                    return [(cand, l0, l1, ok)]
-                losses[k] = _lm_iterations([g], sparse_step, **kw)[0]
-        if dense:
-            group = _DenseGroup([graphs[k] for k in dense], [edges[k] for k in dense], [poses[k] for k in dense],
-                                [weights[k] for k in dense])
-            for k, h in zip(dense, _lm_iterations([graphs[k] for k in dense], group.step, **kw)):
-                losses[k] = h
+        sparse = [k for k, g in enumerate(graphs) if g.sparse]
+        nd = len(dense)
+        # one info table: the dense group's rows first (compact over its active graphs), then one row per sparse graph
+        info = torch.empty(len(graphs), 4, dtype=torch.float64, device=graphs[0].nodes.device)
+        pick = lambda ks, a: [a[k] for k in ks]
+        dg = _DenseGroup(pick(dense, graphs), pick(dense, edges), pick(dense, poses), pick(dense, weights),
+                         info=info[:nd]) if dense else None
+        sg = _SparseGroup(pick(sparse, graphs), pick(sparse, edges), pick(sparse, poses), pick(sparse, weights),
+                          info=info[nd:]) if sparse else None
+
+        def step(active, dampings):  # positions in dense + sparse, ascending: the dense ones come first
+            da = [(t, d) for t, d in zip(active, dampings) if t < nd]
+            sa = [(t - nd, d) for t, d in zip(active, dampings) if t >= nd]
+            outs = dg.launch([t for t, _ in da], [d for _, d in da]) if da else []
+            outs += sg.launch([m for m, _ in sa], [d for _, d in sa]) if sa else []
+            rows = _read_info(info if sa else info[:len(da)])  # the one host synchronisation of the iteration
+            at = list(range(len(da))) + [nd + m for m, _ in sa]
+            return [(out, float(rows[r][0]), float(rows[r][1]), bool(rows[r][3] > 0.5)) for out, r in zip(outs, at)]
+
+        order = dense + sparse
+        losses = [None] * len(graphs)
+        for k, h in zip(order, _lm_iterations(pick(order, graphs), step, steps=steps, patience=patience,
+                                              decreasing=decreasing, radius=radius)):
+            losses[k] = h
         return losses
 
 
@@ -201,14 +224,14 @@ class _DenseGroup:
     """The dense-route LM step over a fixed list of graphs, of which any subset steps together: one scratch buffer and
     one info table for the whole group, inputs converted once."""
 
-    def __init__(self, graphs, edges, poses, weights, dmin=1e-6, dmax=1e32):
+    def __init__(self, graphs, edges, poses, weights, dmin=1e-6, dmax=1e32, info=None):
         self.graphs = graphs
         self.edges = [e.to(torch.int64).contiguous() for e in edges]
         self.poses = [p.to(torch.float32).contiguous() for p in poses]
         self.weights = [w.to(torch.float32).contiguous() for w in weights]
         self.dmin, self.dmax = dmin, dmax
         self.device = graphs[0].nodes.device
-        self.info = torch.empty(len(graphs), 4, dtype=torch.float64, device=self.device)
+        self.info = torch.empty(len(graphs), 4, dtype=torch.float64, device=self.device) if info is None else info
         self.scratch = None
         self.L = _lib.lib()
 
@@ -224,6 +247,12 @@ class _DenseGroup:
     def step(self, members, dampings):
         """One LM step of graphs[members] (at most PG_GROUP_MAX per launch sequence) -> per member (candidate nodes,
         loss before, loss after, Cholesky ok); one info read-back in all."""
+        outs = self.launch(members, dampings)
+        info = _read_info(self.info[:len(members)])  # the one host synchronisation of the iteration
+        return [(out, float(r[0]), float(r[1]), bool(r[3] > 0.5)) for out, r in zip(outs, info)]
+
+    def launch(self, members, dampings):
+        """Enqueue one LM step of graphs[members] -> their candidate nodes; info rows at self.info[:len(members)]."""
         outs = [torch.empty_like(self.graphs[k].nodes) for k in members]
         rows = len(members)
         with torch.cuda.device(self.device):
@@ -236,5 +265,78 @@ class _DenseGroup:
                 _lib.check(self.L.sta_pose_graph_lm_step_group(tab, c1 - c0, self.dmin, self.dmax,
                                                                _lib.ptr(self.info[c0:c1]), _lib.ptr(self.scratch), need,
                                                                _lib.cur_stream()), "sta_pose_graph_lm_step_group")
-        info = _read_info(self.info[:rows])  # the one host synchronisation of the iteration
-        return [(out, float(r[0]), float(r[1]), bool(r[3] > 0.5)) for out, r in zip(outs, info)]
+        return outs
+
+
+class _SparseGroup:
+    """The block-sparse-route LM step over a fixed list of graphs, of which any subset steps together: each graph's
+    plan (PoseGraphOpt.plan), one group plan over them per PG_GROUP_MAX graphs, and one info row per graph.  A single
+    graph takes sta_pose_graph_lm_step_sparse, as PoseGraphOpt.lm_step does."""
+
+    def __init__(self, graphs, edges, poses, weights, dmin=1e-6, dmax=1e32, info=None):
+        self.graphs = graphs
+        self.plans = [g.plan(e) for g, e in zip(graphs, edges)]  # held here: the group plans borrow them
+        self.poses = [p.to(torch.float32).contiguous() for p in poses]
+        self.weights = [w.to(torch.float32).contiguous() for w in weights]
+        self.dmin, self.dmax = dmin, dmax
+        self.device = graphs[0].nodes.device
+        self.info = torch.empty(len(graphs), 4, dtype=torch.float64, device=self.device) if info is None else info
+        self.L = _lib.lib()
+        self._destroy = self.L.sta_pg_group_plan_destroy
+        self.chunks = []  # (first graph, end, group plan)
+        if len(graphs) > 1:
+            with torch.cuda.device(self.device):
+                for c0 in range(0, len(graphs), _lib.PG_GROUP_MAX):
+                    c1 = min(len(graphs), c0 + _lib.PG_GROUP_MAX)
+                    h = ctypes.c_void_p()
+                    tab = (ctypes.c_void_p * (c1 - c0))(*[p.h for p in self.plans[c0:c1]])
+                    _lib.check(self.L.sta_pg_group_plan_create(tab, c1 - c0, ctypes.byref(h)), "sta_pg_group_plan_create")
+                    self.chunks.append((c0, c1, h))
+
+    def plan_info(self):
+        """{"G", "levels", "launches", "device_bytes"} of each group plan."""
+        out = []
+        for _, _, h in self.chunks:
+            v = (ctypes.c_int64 * 4)()
+            _lib.check(self.L.sta_pg_group_plan_info(h, v), "sta_pg_group_plan_info")
+            out.append(dict(zip(("G", "levels", "launches", "device_bytes"), map(int, v))))
+        return out
+
+    def launch(self, members, dampings):
+        """Enqueue one LM step of graphs[members] -> their candidate nodes; graph k's info row at self.info[k]."""
+        outs = [torch.empty_like(self.graphs[k].nodes) for k in members]
+        damp = dict(zip(members, dampings))
+        out_of = dict(zip(members, outs))
+        with torch.cuda.device(self.device):
+            if not self.chunks:  # one graph
+                g = self.graphs[0]
+                _lib.check(self.L.sta_pose_graph_lm_step_sparse(self.plans[0].h, _lib.ptr(g.nodes), _lib.ptr(self.poses[0]),
+                                                                _lib.ptr(self.weights[0]), float(damp[0]), self.dmin,
+                                                                self.dmax, _lib.ptr(outs[0]), _lib.ptr(self.info[0]),
+                                                                _lib.cur_stream()), "sta_pose_graph_lm_step_sparse")
+                return outs
+            for c0, c1, h in self.chunks:
+                if not any(c0 <= k < c1 for k in members):
+                    continue
+                steps = (_lib.StaPgSparseStep * (c1 - c0))()
+                for k in range(c0, c1):
+                    if k in damp:
+                        steps[k - c0] = _lib.StaPgSparseStep(self.graphs[k].nodes.data_ptr(), self.poses[k].data_ptr(),
+                                                             self.weights[k].data_ptr(), out_of[k].data_ptr(),
+                                                             float(damp[k]), 1)
+                _lib.check(self.L.sta_pose_graph_lm_step_sparse_group(h, steps, self.dmin, self.dmax,
+                                                                      _lib.ptr(self.info[c0:c1]), _lib.cur_stream()),
+                           "sta_pose_graph_lm_step_sparse_group")
+        return outs
+
+    def step(self, members, dampings):
+        """One LM step of graphs[members] -> per member (candidate nodes, loss before, loss after, Cholesky ok); one
+        info read-back in all."""
+        outs = self.launch(members, dampings)
+        info = _read_info(self.info)  # the one host synchronisation of the iteration
+        return [(out, float(info[k][0]), float(info[k][1]), bool(info[k][3] > 0.5)) for k, out in zip(members, outs)]
+
+    def __del__(self):
+        for _, _, h in getattr(self, "chunks", []):
+            self._destroy(h)
+        self.chunks = []

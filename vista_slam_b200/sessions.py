@@ -190,7 +190,7 @@ class SLAMSessions:
         loop_related_views cleared and the same messages (every session's opening messages, then the optimisation,
         then every session's closing message); a session without nodes or edges only prints them.  An unknown or
         repeated index raises ValueError before anything runs.  Host synchronisations: one per LM iteration of the
-        group (block-sparse-route graphs, above PG_DENSE_MAX_OPT optimised nodes, add their own)."""
+        group, whichever route each session's graph takes (OnlineSLAM.pgo_route)."""
         order, seen = [], set()
         for k in ks:
             k = self._index(k)

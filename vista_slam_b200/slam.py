@@ -153,6 +153,7 @@ class OnlineSLAM:
         self.live_mode = live_mode
         self.loop_related_views = set()
         self.pgo_window_size = 2 * pgo_every
+        self.pgo_route = None  # PoseGraphOpt's route: None (by size), "sparse" or "dense"
         self._graph = None  # created at the first keyframe, when the map size is known
         self._reset_host_graph()
 
@@ -416,7 +417,8 @@ class OnlineSLAM:
             return None
         g = self._graph
         idx = torch.tensor(sorted(opt), dtype=torch.int64).to(self.device)
-        return PoseGraphOpt(g.pose[:N], to_optimize_idxs=idx), (g.edges[:E], g.meas[:E], g.weight[:E])
+        graph = PoseGraphOpt(g.pose[:N], to_optimize_idxs=idx, route=self.pgo_route)
+        return graph, (g.edges[:E], g.meas[:E], g.weight[:E])
 
     def _pgo_end(self, problem):
         """The second half of a PGO, after the optimisation of _pgo_begin's problem: the poses written back, the
