@@ -575,6 +575,13 @@ int sta_graph_add_keyframe(StaGraph* g, int view, int n, const int64_t* js_host,
                            const int* first_j_host, int node0, int edge0, int H, int W, const float* pose_dev,
                            const float* pose_conf_dev, const float* confs_dev, const float* depths_dev, const float* intri_dev,
                            const float* conf_mean_dev, void* stream);
+/* Re-derive node poses after their parents' poses changed: for t = 0 .. count - 1 in order, with (node, parent, edge) =
+ * triples_host[3t .. 3t + 2], pose[node] = pose[parent] * measurement[edge], the Sim(3) product sta_graph_add_keyframe
+ * uses when it inserts a node.  Listed in insertion order (a keyframe's first j node before its i node), the triples of
+ * nodes inserted since a pose snapshot bring them to the poses they would have had if inserted after the snapshot's
+ * poses were written, bit for bit.  One single-thread launch per 256 triples, no host synchronisation.  Refused before
+ * any launch: a node or parent outside [0, max_nodes), a node that is its own parent, an edge outside [0, max_edges). */
+int sta_graph_replay_nodes(StaGraph* g, int count, const int* triples_host, void* stream);
 /* Per view v in [view0, view0 + num_views), through its best node (every view must have one): pose_out [V][4][4] (rotation
  * and translation, scale dropped), scale_out [V], depth_out / conf_out [V][H][W] (unscaled), intri_out [V][3][3].
  * With points_out: the world point cloud of save_data_all -- depth s unprojected with K^-1, then R p + t, points with

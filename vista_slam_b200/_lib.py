@@ -214,6 +214,7 @@ def lib():
     L.sta_graph_flags.argtypes = [vp, POINTER(c_int)]
     L.sta_graph_add_keyframe.argtypes = [vp, i, i, POINTER(c_int64), POINTER(c_int), POINTER(c_int), i, i, i, i, vp, vp, vp, vp,
                                          vp, vp, vp]
+    L.sta_graph_replay_nodes.argtypes = [vp, i, POINTER(c_int), vp]
     L.sta_graph_export_scratch_bytes.argtypes = [i, i]
     L.sta_graph_export_scratch_bytes.restype = ctypes.c_size_t
     L.sta_graph_export.argtypes = [vp, i, i, c_float, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]

@@ -208,6 +208,24 @@ __global__ void graph_link_kernel(StaGraph g, KfArgs a) {
   __threadfence_system();
 }
 
+// Triples (node, parent, edge) of one replay launch: 256 x 12 bytes keeps the parameters under 4 KB.
+constexpr int kReplayChunk = 256;
+struct ReplayArgs {
+  int count;
+  int t[kReplayChunk][3];
+};
+
+// one thread: pose[node] = pose[parent] * meas[edge] for each triple in order, through graph_link_kernel's sim3_mul, so
+// a node re-derived from the same parent pose and measurement gets the bits its insertion would have given it
+__global__ void __launch_bounds__(32) graph_replay_kernel(float* pose, const float* meas, ReplayArgs a) {
+  if (threadIdx.x != 0) return;
+  for (int t = 0; t < a.count; ++t) {
+    const int* r = a.t[t];
+    sim3_mul(pose + static_cast<long long>(r[1]) * 8, meas + static_cast<long long>(r[2]) * 8,
+             pose + static_cast<long long>(r[0]) * 8);
+  }
+}
+
 // grid-stride over max(max_nodes, max_edges, max_views): the state of PoseGraphNodes/Edges.reset (pose_graph.py:19-54)
 __global__ void graph_reset_kernel(StaGraph g) {
   const long long n = max(max(g.max_nodes, g.max_edges), g.max_views);
@@ -424,6 +442,28 @@ int sta_graph_add_keyframe(StaGraph* g, int view, int n, const int64_t* js_host,
   STA_CHECK_CUDA(cudaGetLastError());
   graph_link_kernel<<<1, 64, 0, st>>>(*g, a);
   STA_CHECK_CUDA(cudaGetLastError());
+  return 0;
+}
+
+int sta_graph_replay_nodes(StaGraph* g, int count, const int* triples_host, void* stream) {
+  STA_REQUIRE(g != nullptr, "null graph");
+  STA_REQUIRE(count >= 0, "negative triple count");
+  STA_REQUIRE(count == 0 || triples_host != nullptr, "null triples");
+  for (int t = 0; t < count; ++t) {
+    const int node = triples_host[3 * t], parent = triples_host[3 * t + 1], edge = triples_host[3 * t + 2];
+    STA_REQUIRE(node >= 0 && node < g->max_nodes, "replayed node out of range");
+    STA_REQUIRE(parent >= 0 && parent < g->max_nodes && parent != node, "parent out of range or the node itself");
+    STA_REQUIRE(edge >= 0 && edge < g->max_edges, "edge out of range");
+  }
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  for (int t0 = 0; t0 < count; t0 += kReplayChunk) {
+    ReplayArgs a;
+    a.count = count - t0 < kReplayChunk ? count - t0 : kReplayChunk;
+    for (int t = 0; t < a.count; ++t)
+      for (int c = 0; c < 3; ++c) a.t[t][c] = triples_host[3 * (t0 + t) + c];
+    graph_replay_kernel<<<1, 32, 0, st>>>(g->pose, g->meas, a);
+    STA_CHECK_CUDA(cudaGetLastError());
+  }
   return 0;
 }
 

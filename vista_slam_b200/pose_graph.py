@@ -60,31 +60,62 @@ def _read_info(info):
     return info.cpu()
 
 
-def _lm_iterations(graphs, step, steps, patience, decreasing, radius):
-    """slam.py:121-134 for each of `graphs`: LM(TrustRegion(radius), min=1e-6) driven by StopOnPlateau(steps, patience,
-    decreasing).  step(active graph indices, their dampings) -> per active graph (candidate nodes, loss before, loss
-    after, Cholesky ok).  A graph leaves the active set when its plateau rule stops it.  Returns the loss histories."""
-    n = len(graphs)
-    radii, stall, losses = [radius] * n, [0] * n, [[] for _ in range(n)]
-    active = list(range(n))
-    for _ in range(steps):
-        if not active:
-            break
-        results = step(active, [1.0 / radii[k] for k in active])
+class _LMState:
+    """slam.py:121-134 for each of n graphs as a state machine: LM(TrustRegion(radius), min=1e-6) driven by
+    StopOnPlateau(steps, patience, decreasing).  dampings() gives the active graphs' dampings for the next step;
+    advance(graphs, results) takes that step's results, per active graph (candidate nodes, loss before, loss after,
+    Cholesky ok), accepts or rejects each candidate, and drops the graphs whose plateau rule stops them.  done once no
+    graph is active or `steps` steps have run.  _lm_iterations drives it in a loop, PoseGraphRun one poll at a time."""
+
+    def __init__(self, n, steps, patience, decreasing, radius):
+        self.steps, self.patience, self.decreasing = steps, patience, decreasing
+        self.radii, self.stall, self.losses = [radius] * n, [0] * n, [[] for _ in range(n)]
+        self.active = list(range(n))
+        self.iterations = 0
+
+    @property
+    def done(self):
+        return not self.active or self.iterations >= self.steps
+
+    def dampings(self):
+        return [1.0 / self.radii[k] for k in self.active]
+
+    def advance(self, graphs, results):
         still = []
-        for k, (cand, l0, l1, ok) in zip(active, results):
+        for k, (cand, l0, l1, ok) in zip(self.active, results):
             if ok and l1 <= l0:
                 graphs[k].nodes = cand
-                radii[k] = min(radii[k] * 2.0, 1e32)
+                self.radii[k] = min(self.radii[k] * 2.0, 1e32)
             else:  # rejected step: keep the nodes, shrink the trust region
-                radii[k] = max(radii[k] * 0.5, 1e-32)
+                self.radii[k] = max(self.radii[k] * 0.5, 1e-32)
                 l1 = l0
-            losses[k].append(l1)
-            stall[k] = stall[k] + 1 if (l0 - l1) < decreasing else 0
-            if stall[k] < patience:
+            self.losses[k].append(l1)
+            self.stall[k] = self.stall[k] + 1 if (l0 - l1) < self.decreasing else 0
+            if self.stall[k] < self.patience:
                 still.append(k)
-        active = still
-    return losses
+        self.active = still
+        self.iterations += 1
+
+
+def _lm_iterations(graphs, step, steps, patience, decreasing, radius):
+    """slam.py:121-134 for each of `graphs` (_LMState).  step(active graph indices, their dampings) -> per active graph
+    (candidate nodes, loss before, loss after, Cholesky ok).  Returns the loss histories."""
+    state = _LMState(len(graphs), steps, patience, decreasing, radius)
+    while not state.done:
+        state.advance(graphs, step(state.active, state.dampings()))
+    return state.losses
+
+
+def _check_group(graphs, edges, poses, weights):
+    if not len(graphs) == len(edges) == len(poses) == len(weights):
+        raise ValueError("graphs, edges, poses and weights must have one entry per graph")
+    if len({id(g) for g in graphs}) != len(graphs):
+        raise ValueError("a PoseGraphOpt is named twice in the group")
+    if graphs and len({g.nodes.device for g in graphs}) != 1:
+        raise ValueError("every graph of a group must be on one device")
+    for e, p, w in zip(edges, poses, weights):
+        if p.shape[0] != e.shape[0] or w.shape[0] != e.shape[0]:
+            raise ValueError("edges, poses and weight must have one row per edge")
 
 
 class PoseGraphOpt:
@@ -181,43 +212,128 @@ class PoseGraphOpt:
         different devices, one PoseGraphOpt named twice, and edges, poses and weights whose row counts disagree."""
         graphs = list(graphs)
         edges, poses, weights = list(edges), list(poses), list(weights)
-        if not len(graphs) == len(edges) == len(poses) == len(weights):
-            raise ValueError("graphs, edges, poses and weights must have one entry per graph")
-        if len({id(g) for g in graphs}) != len(graphs):
-            raise ValueError("a PoseGraphOpt is named twice in the group")
-        if graphs and len({g.nodes.device for g in graphs}) != 1:
-            raise ValueError("every graph of a group must be on one device")
-        for e, p, w in zip(edges, poses, weights):
-            if p.shape[0] != e.shape[0] or w.shape[0] != e.shape[0]:
-                raise ValueError("edges, poses and weight must have one row per edge")
+        _check_group(graphs, edges, poses, weights)
         if not graphs:
             return []
-        dense = [k for k, g in enumerate(graphs) if not g.sparse]
-        sparse = [k for k, g in enumerate(graphs) if g.sparse]
-        nd = len(dense)
-        # one info table: the dense group's rows first (compact over its active graphs), then one row per sparse graph
-        info = torch.empty(len(graphs), 4, dtype=torch.float64, device=graphs[0].nodes.device)
-        pick = lambda ks, a: [a[k] for k in ks]
-        dg = _DenseGroup(pick(dense, graphs), pick(dense, edges), pick(dense, poses), pick(dense, weights),
-                         info=info[:nd]) if dense else None
-        sg = _SparseGroup(pick(sparse, graphs), pick(sparse, edges), pick(sparse, poses), pick(sparse, weights),
-                          info=info[nd:]) if sparse else None
+        group = _Group(graphs, edges, poses, weights)
 
-        def step(active, dampings):  # positions in dense + sparse, ascending: the dense ones come first
-            da = [(t, d) for t, d in zip(active, dampings) if t < nd]
-            sa = [(t - nd, d) for t, d in zip(active, dampings) if t >= nd]
-            outs = dg.launch([t for t, _ in da], [d for _, d in da]) if da else []
-            outs += sg.launch([m for m, _ in sa], [d for _, d in sa]) if sa else []
-            rows = _read_info(info if sa else info[:len(da)])  # the one host synchronisation of the iteration
-            at = list(range(len(da))) + [nd + m for m, _ in sa]
-            return [(out, float(rows[r][0]), float(rows[r][1]), bool(rows[r][3] > 0.5)) for out, r in zip(outs, at)]
+        def step(active, dampings):
+            outs, info, at = group.launch(active, dampings)
+            return _Group.results(_read_info(info), outs, at)  # the one host synchronisation of the iteration
 
-        order = dense + sparse
         losses = [None] * len(graphs)
-        for k, h in zip(order, _lm_iterations(pick(order, graphs), step, steps=steps, patience=patience,
-                                              decreasing=decreasing, radius=radius)):
+        for k, h in zip(group.order, _lm_iterations([graphs[k] for k in group.order], step, steps=steps,
+                                                    patience=patience, decreasing=decreasing, radius=radius)):
             losses[k] = h
         return losses
+
+    @torch.no_grad()
+    def start(self, edges, poses, weight, steps=20, patience=3, decreasing=1e-4, radius=1e4):
+        """optimize() without waiting for it: returns a PoseGraphRun that steps this graph on a side stream, one LM
+        iteration per poll().  Same kernels, dampings and accept / plateau decisions as optimize(), so the nodes and the
+        loss history it ends with are optimize()'s, bit for bit.  The row-count refusal of optimize_group applies."""
+        return PoseGraphRun(self, edges, poses, weight, steps, patience, decreasing, radius)
+
+
+class _Group:
+    """optimize_group's LM step over a fixed list of graphs, dense-route graphs first (`order`): one info table (the
+    dense group's rows first, compact over its active graphs, then one row per sparse graph).  launch(active, dampings)
+    enqueues one step of the active positions in `order` and returns (their candidate nodes, the info rows to read
+    back, the row of each); results() turns the host copy of those rows into the step's results."""
+
+    def __init__(self, graphs, edges, poses, weights):
+        dense = [k for k, g in enumerate(graphs) if not g.sparse]
+        sparse = [k for k, g in enumerate(graphs) if g.sparse]
+        self.nd = len(dense)
+        self.order = dense + sparse
+        self.info = torch.empty(len(graphs), 4, dtype=torch.float64, device=graphs[0].nodes.device)
+        pick = lambda ks, a: [a[k] for k in ks]
+        self.dg = _DenseGroup(pick(dense, graphs), pick(dense, edges), pick(dense, poses), pick(dense, weights),
+                              info=self.info[:self.nd]) if dense else None
+        self.sg = _SparseGroup(pick(sparse, graphs), pick(sparse, edges), pick(sparse, poses), pick(sparse, weights),
+                               info=self.info[self.nd:]) if sparse else None
+
+    def launch(self, active, dampings):  # positions in dense + sparse, ascending: the dense ones come first
+        nd = self.nd
+        da = [(t, d) for t, d in zip(active, dampings) if t < nd]
+        sa = [(t - nd, d) for t, d in zip(active, dampings) if t >= nd]
+        outs = self.dg.launch([t for t, _ in da], [d for _, d in da]) if da else []
+        outs += self.sg.launch([m for m, _ in sa], [d for _, d in sa]) if sa else []
+        at = list(range(len(da))) + [nd + m for m, _ in sa]
+        return outs, (self.info if sa else self.info[:len(da)]), at
+
+    @staticmethod
+    def results(rows, outs, at):
+        return [(out, float(rows[r][0]), float(rows[r][1]), bool(rows[r][3] > 0.5)) for out, r in zip(outs, at)]
+
+
+class PoseGraphRun:
+    """A PoseGraphOpt.optimize() in the background (PoseGraphOpt.start): each LM iteration is enqueued on a non-blocking
+    side stream, its info row copied into pinned host memory and an event recorded.  poll() never waits: when the
+    event has completed it takes the iteration's accept / reject decision and enqueues the next one.  wait() waits on
+    that event until the run is done.
+
+    Streams: the side stream starts after the work already queued on the stream that was current at start() (the
+    "main" stream, which holds the PoseGraphOpt's snapshot of the nodes); the main-stream tensors the run reads are
+    recorded on the side stream.  Once done, the main stream is ordered after the run, so graph.nodes can be read
+    there.  A block-sparse plan is built in start(), on the main stream.  Nothing here synchronises the device."""
+
+    def __init__(self, graph, edges, poses, weight, steps, patience, decreasing, radius):
+        _check_group([graph], [edges], [poses], [weight])
+        dev = graph.nodes.device
+        self.graph = graph
+        self.main = torch.cuda.current_stream(dev)
+        if graph.sparse:
+            graph.plan(edges)  # its one edge-table copy waits only on the main stream's queued work
+        self.stream = torch.cuda.Stream(dev)
+        self.stream.wait_stream(self.main)
+        for t in (graph.nodes, graph.idxs_opt, edges, poses, weight):
+            t.record_stream(self.stream)  # no-op for memory the caching allocator does not own (the SLAM tables)
+        self.state = _LMState(1, steps, patience, decreasing, radius)
+        self.pinned = torch.empty(1, 4, dtype=torch.float64, pin_memory=True)
+        self.event = torch.cuda.Event()
+        with torch.cuda.stream(self.stream):
+            self.group = _Group([graph], [edges], [poses], [weight])
+        self._launch()
+
+    @property
+    def done(self):
+        return self.state.done
+
+    @property
+    def losses(self):
+        """The loss history so far: optimize()'s return value once done."""
+        return self.state.losses[0]
+
+    def _launch(self):
+        if self.state.done:
+            self.main.wait_stream(self.stream)
+            self.graph.nodes.record_stream(self.main)
+            self.group = self._pending = None
+            return
+        with torch.cuda.stream(self.stream):
+            outs, info, at = self.group.launch(self.state.active, self.state.dampings())
+            self.pinned[:info.shape[0]].copy_(info, non_blocking=True)
+            self.event.record(self.stream)
+        self._pending = (outs, info.shape[0], at)
+
+    @torch.no_grad()
+    def poll(self):
+        """Take the iteration in flight if it has finished, and enqueue the next; never waits.  Returns done."""
+        if self.state.done:
+            return True
+        if not self.event.query():
+            return False
+        outs, rows, at = self._pending
+        self.state.advance([self.graph], _Group.results(self.pinned[:rows], outs, at))
+        self._launch()
+        return self.state.done
+
+    def wait(self):
+        """Run to the end, waiting on each iteration's event.  Returns the loss history."""
+        while not self.poll():
+            self.event.synchronize()
+        return self.losses
 
 
 class _DenseGroup:

@@ -109,7 +109,9 @@ class SLAMSessions:
         raises ValueError by the end of the call.
 
         Host synchronisations: one for the loop candidates of all sessions, one per edge chunk, one per PGO iteration,
-        and one at the end of the call unless every session's flag has been read since its last graph launch."""
+        and one at the end of the call unless every session's flag has been read since its last graph launch.  A
+        session with pgo_background runs its PGOs on their own side streams (OnlineSLAM.step_many); every session with
+        a pending one is polled after each keyframe of the call."""
         calls = self._calls(values)
         force = {self._index(k) for k in force_pgo}
         flags = {k: [] for k, _ in calls}
@@ -172,10 +174,13 @@ class SLAMSessions:
             s._register_keyframe(vs[m], i, js, res)
             if js:
                 checked[c] = checked[c] and not res[1]
+            for p in self.sessions:
+                if p.pgo_pending:
+                    p._pgo_poll()
             s.time_dict["graph_construction"] += time.time() - graph_start
             folder = output_folders.get(k) if output_folders else None
             flags[k].append(s._pgo_if_due(k in force and m == len(vs) - 1, log_intermediate_results, folder))
-            if flags[k][-1]:
+            if flags[k][-1] and not s.pgo_background:
                 checked[c] = s.num_nodes > 0 and s.num_edges > 0
         if not all(checked):
             torch.cuda.current_stream().synchronize()
@@ -190,7 +195,8 @@ class SLAMSessions:
         loop_related_views cleared and the same messages (every session's opening messages, then the optimisation,
         then every session's closing message); a session without nodes or edges only prints them.  An unknown or
         repeated index raises ValueError before anything runs.  Host synchronisations: one per LM iteration of the
-        group, whichever route each session's graph takes (OnlineSLAM.pgo_route)."""
+        group, whichever route each session's graph takes (OnlineSLAM.pgo_route).  A pending background PGO of a named
+        session is folded first (OnlineSLAM.wait_pgo)."""
         order, seen = [], set()
         for k in ks:
             k = self._index(k)
@@ -201,6 +207,8 @@ class SLAMSessions:
         if not order:
             return
         sess = [self.sessions[k] for k in order]
+        for s in sess:
+            s.wait_pgo()
         t = time.time()
         problems = [s._pgo_begin() for s in sess]
         run = [p for p in problems if p is not None]

@@ -25,6 +25,12 @@ bookkeeping of calling `step` on each in order.  The frontend work does not depe
 keyframes at real batch sizes: the encoder over up to 41 views per call at 224 x 224, loop detection over all frames of
 the call with one read-back, and the gated edge regression in chunks of up to 16 edges with one read-back each.
 
+`pgo_background = True` (default False) runs each due PGO on a side stream while step goes on (PoseGraphOpt.start):
+step and step_many poll it at every keyframe without waiting, and fold it when it is done -- its poses written, the
+nodes inserted since its launch re-derived from them (sta_graph_replay_nodes) -- which leaves the graph bit-identical
+to the synchronous path.  Until the fold, get_view shows the poses from before the PGO; the next due PGO,
+pose_graph_optimize, save_data_all, reset and wait_pgo wait for a pending run (INTEGRATION.md §5).
+
 Importing this module does not import pypose, munch, colorama or open3d.  `get_view` returns a `View` (attribute and key
 access, as munch.Munch).  The PLY of save_data_all is written here: binary little-endian, float x y z and uchar
 red green blue (colours rounded from [0, 1]); whether that is byte-identical to open3d's writer is not checked."""
@@ -154,6 +160,8 @@ class OnlineSLAM:
         self.loop_related_views = set()
         self.pgo_window_size = 2 * pgo_every
         self.pgo_route = None  # PoseGraphOpt's route: None (by size), "sparse" or "dense"
+        self.pgo_background = False  # run due PGOs on a side stream while step goes on (see the module docstring)
+        self._pgo_run = None  # a background PGO not yet folded: (PoseGraphRun, its problem, nodes to replay)
         self._graph = None  # created at the first keyframe, when the map size is known
         self._reset_host_graph()
 
@@ -175,6 +183,9 @@ class OnlineSLAM:
         self.imgs = _DeviceImages()
         self.view_names = []
         self.view_num = 0
+        if self._pgo_run is not None:  # discarded, once its queued work has finished with the tables
+            self._pgo_run[0].wait()
+            self._pgo_run = None
         if self._graph is not None:
             with torch.cuda.device(self._graph.device):
                 _lib.check(_lib.lib().sta_graph_reset(self._graph.h, _lib.cur_stream()), "sta_graph_reset")
@@ -245,6 +256,19 @@ class OnlineSLAM:
                 g.h, i, n, *args, self.num_nodes, self.num_edges, H, W, _lib.ptr(batch["pose"]), _lib.ptr(batch["pose_conf"]),
                 _lib.ptr(batch["conf"]), _lib.ptr(batch["depths"]), _lib.ptr(batch["intri"]), _lib.ptr(batch["conf_mean"]),
                 _lib.cur_stream()), "sta_graph_add_keyframe")
+        if self._pgo_run is not None:  # the nodes a pending background PGO's fold re-derives, in link order
+            rec, e = self._pgo_run[2], self.num_edges
+            for k in range(n):
+                ni = self.num_nodes + 2 * k
+                if k > 0:
+                    rec.append((ni, self.num_nodes, e))
+                    e += 1
+                if first_j[k] >= 0:
+                    rec.append((ni + 1, first_j[k], e))
+                    e += 1
+                if k == 0:
+                    rec.append((ni, ni + 1, e))
+                e += 1
         self.view_to_node.update(v2n)
         for j in kept_js:
             self.node_to_connected_view += [j, i]
@@ -272,15 +296,63 @@ class OnlineSLAM:
         whether it ran."""
         if not (self.view_num % self.pgo_every == 0 or force_pgo):
             return False
+        self.wait_pgo()
         if log_intermediate_results:
             self.save_data_all(f"{output_folder}", save_view_graph=False, traj_name_postfix=f"{self.view_num - 1}",
                                save_poses=True, save_images=False, save_scales=True, save_depths=False,
                                save_intrinsics=False, save_confs=False, save_ply=False)
         opt_start = time.time()
+        if self.pgo_background:
+            self._pgo_launch()
+            self.time_dict["pgo"] += time.time() - opt_start
+            return True
         self.pose_graph_optimize()
         self.time_dict["pgo"] += time.time() - opt_start
         torch.cuda.empty_cache()
         return True
+
+    def _pgo_launch(self):
+        """The background form of pose_graph_optimize: its opening messages and optimised set now, loop_related_views
+        cleared now (keyframes inserted before the fold add to the next PGO's set, as after a synchronous PGO), and
+        the optimisation started on a side stream (PoseGraphOpt.start)."""
+        problem = self._pgo_begin()
+        self.loop_related_views = set()
+        if problem is None:
+            _msg("[PoseGraphOpt] ", "Pose graph optimization done.")
+            return
+        graph, args = problem
+        self._pgo_run = (graph.start(*args), problem, [])
+
+    @property
+    def pgo_pending(self):
+        """Whether a background PGO has started and not yet been folded into the graph."""
+        return self._pgo_run is not None
+
+    def wait_pgo(self):
+        """Fold a pending background PGO into the graph, waiting for it to finish if it is still running."""
+        self._pgo_fold(wait=True)
+
+    def _pgo_poll(self):
+        """Fold a pending background PGO if it has finished, or enqueue its next iteration; never waits."""
+        self._pgo_fold(wait=False)
+
+    def _pgo_fold(self, wait):
+        """A finished background PGO into the graph: its poses over the nodes it optimised, the nodes inserted since its
+        launch re-derived from them (sta_graph_replay_nodes), which leaves the graph as a synchronous PGO followed by
+        those insertions would, bit for bit; then the closing message, the flag check and empty_cache."""
+        if self._pgo_run is None:
+            return
+        run, problem, replay = self._pgo_run
+        start = time.time()
+        if wait:
+            run.wait()
+        elif not run.poll():
+            return
+        self._pgo_run = None
+        self._pgo_write(problem, replay)
+        _msg("[PoseGraphOpt] ", "Pose graph optimization done.")
+        torch.cuda.empty_cache()
+        self.time_dict["pgo"] += time.time() - start
 
     # ------------------------------------------------------------------------------------------------ step
     def add_view(self, image, image_shape, view_name):
@@ -298,6 +370,7 @@ class OnlineSLAM:
         self._ensure_graph(image)
         if i == 0:
             self._graph.pose[0].copy_(self._identity)  # slam.py:251-253
+        self._pgo_poll()
         self.time_dict["prepare_data"] += time.time() - prepare_start
 
         enc_start = time.time()
@@ -318,6 +391,7 @@ class OnlineSLAM:
             self.time_dict["decoder"] += time.time() - dec_start
             self._check_flags()
             self._insert_keyframe(i, js, *res)
+        self._pgo_poll()
         self.time_dict["graph_construction"] += time.time() - graph_start
         return self._pgo_if_due(force_pgo, log_intermediate_results, output_folder)
 
@@ -350,6 +424,7 @@ class OnlineSLAM:
         self._ensure_graph(images[0])
         if i0 == 0:
             self._graph.pose[0].copy_(self._identity)
+        self._pgo_poll()
         self.time_dict["prepare_data"] += time.time() - prepare_start
 
         enc_start = time.time()
@@ -375,9 +450,10 @@ class OnlineSLAM:
             self._register_keyframe(v, i, js, res)
             if js:
                 checked = checked and not res[1]
+            self._pgo_poll()
             self.time_dict["graph_construction"] += time.time() - graph_start
             flags.append(self._pgo_if_due(force_pgo and k == n - 1, log_intermediate_results, output_folder))
-            if flags[-1]:
+            if flags[-1] and not self.pgo_background:  # a synchronous PGO's read-backs waited for the graph launches
                 checked = self.num_nodes > 0 and self.num_edges > 0
         if not checked:
             torch.cuda.current_stream().synchronize()
@@ -394,7 +470,9 @@ class OnlineSLAM:
             self._insert_keyframe(i, js, *res)
 
     def pose_graph_optimize(self):
-        """slam.py:108-140 through PoseGraphOpt on the device tables (per-edge weights: DESIGN.md §4)."""
+        """slam.py:108-140 through PoseGraphOpt on the device tables (per-edge weights: DESIGN.md §4).  Runs now, after
+        folding a pending background PGO (wait_pgo), whatever pgo_background says."""
+        self.wait_pgo()
         problem = self._pgo_begin()
         if problem is not None:
             graph, args = problem
@@ -424,10 +502,22 @@ class OnlineSLAM:
         """The second half of a PGO, after the optimisation of _pgo_begin's problem: the poses written back, the
         message, loop_related_views cleared."""
         if problem is not None:
-            self._graph.pose[:self.num_nodes] = problem[0].get_nodes()
-            self._check_flags()
+            self._pgo_write(problem)
         _msg("[PoseGraphOpt] ", "Pose graph optimization done.")
         self.loop_related_views = set()
+
+    def _pgo_write(self, problem, replay=()):
+        """The optimised poses of _pgo_begin's problem into the node table, then the (node, parent, edge) triples of
+        `replay` re-derived in order."""
+        g = self._graph
+        nodes = problem[0].get_nodes()
+        g.pose[:nodes.shape[0]] = nodes
+        if replay:
+            flat = (ctypes.c_int * (3 * len(replay)))(*[x for t in replay for x in t])
+            with torch.cuda.device(g.device):
+                _lib.check(_lib.lib().sta_graph_replay_nodes(g.h, len(replay), flat, _lib.cur_stream()),
+                           "sta_graph_replay_nodes")
+        self._check_flags()
 
     # ------------------------------------------------------------------------------------------------ export
     def _export(self, view0, num_views, cloud):
@@ -461,7 +551,9 @@ class OnlineSLAM:
         return out
 
     def get_view(self, v, filter_outlier=True, return_pose=True, return_depth=True, return_intri=True):
-        """slam.py:299-326."""
+        """slam.py:299-326.  A background PGO is folded first if it has finished; while it runs, the view shows the
+        poses from before it."""
+        self._pgo_poll()
         ex = self._export(v, 1, cloud=False)
         view = View()
         if return_pose:
@@ -486,7 +578,8 @@ class OnlineSLAM:
                       save_depths=True, save_intrinsics=True,
                       save_confs=True, save_ply=True,
                       gt_poses=None, gt_depths=None, gt_intrinsics=None):
-        """slam.py:338-421: the same files, keys, shapes and dtypes."""
+        """slam.py:338-421: the same files, keys, shapes and dtypes.  A pending background PGO is folded first (wait_pgo)."""
+        self.wait_pgo()
         if not os.path.exists(output_folder):
             os.makedirs(output_folder)
         if save_view_graph:
