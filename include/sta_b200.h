@@ -409,8 +409,10 @@ int sta_preprocess_rgb8_many(const uint8_t* rgb_dev, int F, int H, int W, int re
  * and cv2.calcOpticalFlowPyrLK(winSize=(21,21), maxLevel=3, criteria=(EPS|COUNT, 30, 0.01)).  A frame is [H][W] uint8
  * (frame_is_f32 = 0) or the [H][W] fp32 gray in [0,1] that sta_preprocess_rgb8 writes (1), converted as
  * (gray * 255).astype(uint8).  Frame sides must be in [32, 2048]; the size checks come before any CUDA call.
- * A tracker handle owns two pyramids (keyframe and current frame), the keyframe's derivatives and corners, and scratch
- * for one frame size, plus the frame pyramids of its group tracks (below).  One stream at a time: work on a new stream waits for the previous one. ---- */
+ * A tracker handle owns, for one frame size, the keyframe's pyramid, derivatives and corners, corner scratch, the
+ * pyramids of the frames of its group tracks (one from creation on, more allocated on first use for larger groups) and
+ * the LK output and statistics of the groups it leads (16 frames' from creation on).  One stream at a time: work on a
+ * new stream waits for the previous one. ---- */
 enum { STA_FLOW_MAX_CORNERS = 1000 };
 typedef struct StaFlowTracker StaFlowTracker; /* opaque */
 typedef struct StaFlowStats {
@@ -421,37 +423,29 @@ typedef struct StaFlowStats {
 } StaFlowStats;
 int sta_flow_create(int H, int W, StaFlowTracker** out);
 void sta_flow_destroy(StaFlowTracker* t);
-/* initialize_keyframe: builds the frame's pyramid, its Scharr derivatives and its corners (asynchronous). */
-int sta_flow_set_keyframe(StaFlowTracker* t, const void* frame_dev, int frame_is_f32, void* stream);
-/* Builds the current frame's pyramid, tracks the keyframe corners into it and reduces the statistics.  The one host
- * synchronisation of a tracked frame: stats_out (host) is valid on return. */
-int sta_flow_track(StaFlowTracker* t, const void* frame_dev, int frame_is_f32, StaFlowStats* stats_out, void* stream);
-/* The frame of the last sta_flow_track becomes the keyframe (a buffer swap, no rebuild); its derivatives and corners
- * are enqueued asynchronously. */
-int sta_flow_promote(StaFlowTracker* t, void* stream);
-/* Device copies of the keyframe corners: pts_out [STA_FLOW_MAX_CORNERS][2] fp32 (x, y) in selection order, the first
- * *count_out valid; and of the keyframe's level-0 image [H][W] uint8 and derivatives [H][W][2] int16 (either may be
- * NULL). */
-/* Groups: the same over many frames and many trackers (SLAM sessions, or a run of frames of one tracker), with every
- * per-frame result equal to the tracker's own one-frame calls; the calls above are the one-frame case.  All trackers
- * of a group share one frame size; frames are [n][H][W] uint8 or fp32 gray as above.  Refused before any launch: n or
- * F < 1, a null pointer, mixed tracker sizes, and the per-call conditions below.
- * sta_flow_set_keyframe_group: initialize_keyframe of frame i on ts[i] (n distinct trackers); asynchronous.
+/* The tracker works on groups: many frames and many trackers (SLAM sessions, or a run of frames of one tracker), one
+ * frame being a group of one; every per-frame result is independent of the group.  All trackers of a group share one
+ * frame size; frames are [n][H][W] uint8 or fp32 gray as above.  Refused before any launch: n or F < 1, a null pointer,
+ * mixed tracker sizes, and the per-call conditions below.
+ * sta_flow_set_keyframe_group: initialize_keyframe of frame i on ts[i] (n distinct trackers): its pyramid, Scharr
+ * derivatives and corners; asynchronous.
  * sta_flow_track_group: frame f belongs to ts[f]; a tracker's frames are consecutive and in its own order, and every
- * one is tracked against the tracker's current keyframe (which must exist) in one launch per stage, then the one host
- * synchronisation: stats_out [F] (host).  held_host [F] (or NULL: none) marks the frames whose pyramids the tracker
- * still holds from its last group track: the frames after the one sta_flow_promote_group promoted, reused in order
- * as a prefix of its frames here (at most as many as it holds).  frames_dev holds only the other frames, in group
- * order (NULL when there are none).
+ * one is tracked against the tracker's current keyframe (which must exist) in one launch per stage, with the
+ * statistics reduced per frame, then the one host synchronisation: stats_out [F] (host).  held_host [F] (or NULL:
+ * none) marks the frames whose pyramids the tracker still holds from its last group track: the frames after the one
+ * sta_flow_promote_group promoted, reused in order as a prefix of its frames here (at most as many as it holds).
+ * frames_dev holds only the other frames, in group order (NULL when there are none).
  * sta_flow_promote_group: frame frame_host[i] (its index among ts[i]'s frames of its last group track) becomes the
  * keyframe of ts[i] (n distinct trackers) without a rebuild; their derivatives and corners are enqueued as one
- * sequence; asynchronous.  The LK output and statistics of a group are in ts[0]'s buffers; each tracker holds up to
- * its largest group's frame pyramids, allocated on first use. */
+ * sequence; asynchronous.  Refused for a tracker with no group track since its last keyframe. */
 int sta_flow_set_keyframe_group(StaFlowTracker* const* ts, int n, const void* frames_dev, int frames_is_f32,
                                 void* stream);
 int sta_flow_track_group(StaFlowTracker* const* ts, int F, const int* held_host, const void* frames_dev,
                          int frames_is_f32, StaFlowStats* stats_out, void* stream);
 int sta_flow_promote_group(StaFlowTracker* const* ts, int n, const int* frame_host, void* stream);
+/* Device copies of the keyframe corners: pts_out [STA_FLOW_MAX_CORNERS][2] fp32 (x, y) in selection order, the first
+ * *count_out valid; and of the keyframe's level-0 image [H][W] uint8 and derivatives [H][W][2] int16 (either may be
+ * NULL). */
 int sta_flow_keyframe_points(StaFlowTracker* t, float* pts_out_dev, int* count_out_dev, void* stream);
 int sta_flow_keyframe_level0(StaFlowTracker* t, uint8_t* gray_out_dev, int16_t* deriv_out_dev, void* stream);
 /* Op-level entry points (the same kernels).  scratch: a device buffer of sta_flow_scratch_bytes(H, W) bytes (256-byte
@@ -479,40 +473,27 @@ void sta_vocab_destroy(StaVocab* v);
 int sta_loop_create(StaVocab* v, int loop_dist_min, int loop_nms, int loop_cand_thresh_neighbor, StaLoopDetector** out);
 void sta_loop_destroy(StaLoopDetector* d);
 int sta_loop_views(const StaLoopDetector* d);
-/* compute_bow_feat: ORB, transform and append the view's vector (None when ORB finds no keypoint); asynchronous.  The
- * one-frame case of sta_loop_add_frames. */
-int sta_loop_add_frame(StaLoopDetector* d, const void* frame_dev, int frame_is_f32, int H, int W, void* stream);
-/* detect_loop for the newest view i given farthest_neighbor in [0, i]: similarities against every earlier view in one
- * launch, the candidate scan in one thread, and the one host synchronisation: n_out[2] = {candidates, length of view
- * i's vector (-1: None)}; the first `cap` candidates are written to js_out / sims_out (host) in the reference's order
- * (descending similarity, ties in descending j).  The one-row case of sta_loop_detect_many. */
-int sta_loop_detect(StaLoopDetector* d, int farthest_neighbor, int* n_out, int64_t* js_out, double* sims_out, int cap,
-                    void* stream);
-/* Frame batches, every per-frame result equal to the calls above in frame order.  sta_loop_add_frames: compute_bow_feat
- * for F >= 1 frames [F][H][W] of one size (ORB over all frames, one transform, vectors appended in frame order);
- * asynchronous.  sta_loop_detect_many: detect_loop for the newest F views (F at most the frames of the last add call),
- * farthest_host[f] in [0, view index of row f]; one score launch and one detect launch over the F rows, then the one
- * host synchronisation: n_out [2F] = {candidates, length (-1: None)} per row, row f's first cap_per_view candidates at
- * js_out / sims_out + f cap_per_view.  An ORB overflow is reported with the frame's index in the batch.  Afterwards
- * sta_loop_similarities returns the last row (n at most that row's view index). */
-int sta_loop_add_frames(StaLoopDetector* d, const void* frames_dev, int frames_is_f32, int F, int H, int W, void* stream);
-int sta_loop_detect_many(StaLoopDetector* d, int F, const int* farthest_host, int* n_out, int64_t* js_out,
-                         double* sims_out, int cap_per_view, void* stream);
-/* The same over the frames of several detectors (SLAM sessions stepped together).  Frame f belongs to dets[f]; a
- * detector's frames are consecutive and in its own order; all detectors share one StaVocab (refused before any launch
- * otherwise).  Every per-frame result equals the detector's own sta_loop_add_frames / sta_loop_detect_many.
- * sta_loop_add_frames_group: ORB over the F frames, one transform, one build CTA per frame and one append launch into
- * each frame's own database; asynchronous.  sta_loop_detect_group: for the frames of the last group add of dets[0]
- * (the same dets and F, no view added to them since), farthest_host[f] in [0, view index of frame f in its detector];
- * one score and one detect launch over all rows, then the one host synchronisation; outputs as sta_loop_detect_many's.
- * The ORB scratch, staging and result buffers of a group are dets[0]'s.  After a group detect, sta_loop_similarities
- * is refused on its detectors until their own next detect. */
+/* compute_bow_feat and detect_loop over F >= 1 frames [F][H][W] of one size, of one detector or of several that share
+ * one StaVocab (SLAM sessions stepped together; refused before any launch otherwise).  Frame f belongs to dets[f]; a
+ * detector's frames are consecutive and in its own order; one detector's frame is a group of one.  Every per-frame
+ * result is independent of the group.
+ * sta_loop_add_frames_group: compute_bow_feat for every frame: ORB over the F frames, one transform, one build CTA per
+ * frame and one append launch into each frame's own database (a view's vector is None when ORB finds no keypoint);
+ * asynchronous, unless dets[0]'s previous add has had no detect since: then the stream is synchronised first.
+ * sta_loop_detect_group: detect_loop for the frames of the last add of dets[0] (the same dets and F, no view added to
+ * them since), farthest_host[f] in [0, view index of frame f in its detector]: similarities against every earlier view
+ * of its detector in one score launch over all rows, the candidate scan in one thread per row, and the one host
+ * synchronisation: n_out [2F] = {candidates, length of the frame's vector (-1: None)} per row, row f's first
+ * cap_per_view candidates at js_out / sims_out + f cap_per_view (host) in the reference's order (descending
+ * similarity, ties in descending j).  An ORB overflow is reported with the frame's index in the group.  The ORB
+ * scratch, staging and result buffers of a group are dets[0]'s.  Afterwards sta_loop_similarities returns the last
+ * row when every row was dets[0]'s, and is refused on the group's detectors until their own next detect otherwise. */
 int sta_loop_add_frames_group(StaLoopDetector* const* dets, int F, const void* frames_dev, int frames_is_f32,
                               int H, int W, void* stream);
 int sta_loop_detect_group(StaLoopDetector* const* dets, int F, const int* farthest_host, int* n_out,
                           int64_t* js_out, double* sims_out, int cap_per_view, void* stream);
 /* Test read-backs (synchronise): a view's vector (len -1 for None) and the last similarity row of the last detect (NaN
- * where either vector is None). */
+ * where either vector is None; n at most that row's view index). */
 int sta_loop_view(StaLoopDetector* d, int view, int32_t* words_out, double* vals_out, int cap, int* len_out, void* stream);
 int sta_loop_similarities(StaLoopDetector* d, double* sims_out, int n, void* stream);
 /* Op-level entry points (the same kernels).  ORB: scratch of sta_orb_scratch_bytes(H, W) bytes (256-byte aligned; 0 for

@@ -110,7 +110,7 @@ def test_two_runs_are_bit_identical():
             assert (x[2] is None and y[2] is None) or np.array_equal(x[2], y[2])
 
 
-def test_promoted_keyframe_equals_fresh_keyframe():
+def test_group_promoted_keyframe_equals_fresh_keyframe():
     from vista_slam_b200 import _lib
     L = _lib.lib()
     f0, f1 = SEQS["b_192x256"][0], SEQS["b_192x256"][3]
@@ -134,18 +134,20 @@ def test_promoted_keyframe_equals_fresh_keyframe():
         return gray.cpu().numpy(), der.cpu().numpy(), pts[:n].cpu().numpy()
 
     a, b = tracker(), tracker()
+    ta, tb = (ctypes.c_void_p * 1)(a.value), (ctypes.c_void_p * 1)(b.value)
+    frame0 = (ctypes.c_int * 1)(0)
     try:
         stats = _lib.StaFlowStats()
-        _lib.check(L.sta_flow_set_keyframe(a, _lib.ptr(d0), 0, s))
-        _lib.check(L.sta_flow_track(a, _lib.ptr(d1), 0, ctypes.byref(stats), s))
+        _lib.check(L.sta_flow_set_keyframe_group(ta, 1, _lib.ptr(d0), 0, s))
+        _lib.check(L.sta_flow_track_group(ta, 1, None, _lib.ptr(d1), 0, ctypes.byref(stats), s))
         assert stats.n_corners == len(orc.good_features(f0)) and stats.n_tracked >= 10
-        _lib.check(L.sta_flow_promote(a, s))
-        _lib.check(L.sta_flow_set_keyframe(b, _lib.ptr(d1), 0, s))
+        _lib.check(L.sta_flow_promote_group(ta, 1, frame0, s))
+        _lib.check(L.sta_flow_set_keyframe_group(tb, 1, _lib.ptr(d1), 0, s))
         ka, kb = keyframe(a), keyframe(b)
         assert np.array_equal(ka[0], f1) and np.array_equal(ka[0], kb[0])
         assert np.array_equal(ka[1], kb[1]) and np.array_equal(ka[1], orc.scharr(f1))
         assert np.array_equal(ka[2], kb[2]) and np.array_equal(ka[2], orc.good_features(f1).reshape(-1, 2))
-        assert L.sta_flow_promote(a, s) == 2   # nothing tracked since the last promotion
+        assert L.sta_flow_promote_group(ta, 1, frame0, s) == 2   # nothing tracked since the last promotion
     finally:
         L.sta_flow_destroy(a)
         L.sta_flow_destroy(b)

@@ -145,7 +145,7 @@ def test_lk_recovers_an_integer_shift():
     np.testing.assert_allclose(nxt - p[inner], np.broadcast_to(np.float32([-2.0, 3.0]), nxt.shape), atol=0.01)
 
 
-def test_c_abi_refuses_bad_sizes_before_touching_the_gpu():
+def test_c_abi_refuses_bad_sizes_and_null_groups_before_touching_the_gpu():
     from vista_slam_b200 import _lib
     L = _lib.lib()
     h = ctypes.c_void_p()
@@ -156,7 +156,8 @@ def test_c_abi_refuses_bad_sizes_before_touching_the_gpu():
         assert L.sta_op_good_features(None, H, W, None, None, None, None) == 2
         assert L.sta_op_lk_track(None, None, H, W, None, 0, None, None, None, None) == 2
     assert L.sta_flow_scratch_bytes(224, 224) > 2 * (224 + 42) ** 2
-    assert L.sta_flow_track(None, None, 0, None, None) == 2 and L.sta_flow_promote(None, None) == 2
+    assert L.sta_flow_track_group(None, 1, None, None, 0, None, None) == 2
+    assert L.sta_flow_promote_group(None, 1, None, None) == 2
 
 
 def test_flow_tracker_has_no_cpu_path():

@@ -1,7 +1,8 @@
 """GPU: OnlineSLAM.step_many and the frame-batched loop detector against the per-keyframe path.
 
-  * loop detection over frame batches (sta_loop_add_frames / sta_loop_detect_many) is bit-identical to detect_loop on
-    each frame in order, and batched ORB to sta_op_orb per frame;
+  * loop detection over frame batches of one detector (detect_loops, through sta_loop_add_frames_group /
+    sta_loop_detect_group) is bit-identical to detect_loop on each frame in order, and batched ORB to sta_op_orb per
+    frame;
   * with the frontend and loops replayed from the golden stream (as in test_slam_gpu.py), step_many in any chunking
     gives the graph tables, host mirrors, PGO calls and written files of sequential step, bit for bit;
   * with the real frontend at 224 x 224 the batch sizes change the GEMMs' split-K.  test_keyframe_gpu.py bounds one
@@ -117,7 +118,7 @@ def test_batched_orb_equals_per_frame(hw):
             np.testing.assert_array_equal(scratch[f, o:o + pix].cpu().numpy(), r["scratch"][o:o + pix].cpu().numpy())
 
 
-def test_loop_batch_refusals():
+def test_loop_group_of_one_detector_refusals():
     from vista_slam_b200 import _lib
     from vista_slam_b200.loop_detector import LoopDetector
     det = LoopDetector(VOCAB, 40, 40, 5)
@@ -130,14 +131,19 @@ def test_loop_batch_refusals():
     assert det.detect_loops([], []) == [] and len(det.bow_feats) == 0
     L = _lib.lib()
     assert L.sta_loop_views(det._h) == 0
-    assert L.sta_loop_add_frames(det._h, _lib.ptr(a), 0, 0, 64, 64, _lib.cur_stream()) != 0
+
+    def dets(k):
+        return (ctypes.c_void_p * k)(*[det._h.value] * k)
+
+    assert L.sta_loop_add_frames_group(dets(1), 0, _lib.ptr(a), 0, 64, 64, _lib.cur_stream()) != 0
     assert b"frame count" in L.sta_last_error()
-    # the C entry point refuses an out-of-range farthest neighbour before any launch
+    # the C entry point refuses an out-of-range farthest neighbour, or another row count than the last add's, before
+    # any launch
     assert det.detect_loops([a, a], [0, 1]) == [[], []]
-    n = (ctypes.c_int * 4)()
-    rc = L.sta_loop_detect_many(det._h, 2, (ctypes.c_int * 2)(0, 5), n, None, None, 0, _lib.cur_stream())
+    n = (ctypes.c_int * 6)()
+    rc = L.sta_loop_detect_group(dets(2), 2, (ctypes.c_int * 2)(0, 5), n, None, None, 0, _lib.cur_stream())
     assert rc != 0 and b"farthest" in L.sta_last_error()
-    rc = L.sta_loop_detect_many(det._h, 3, (ctypes.c_int * 3)(0, 0, 0), n, None, None, 0, _lib.cur_stream())
+    rc = L.sta_loop_detect_group(dets(3), 3, (ctypes.c_int * 3)(0, 0, 0), n, None, None, 0, _lib.cur_stream())
     assert rc != 0
 
 

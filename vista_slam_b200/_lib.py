@@ -168,9 +168,6 @@ def lib():
     L.sta_flow_create.argtypes = [i, i, POINTER(vp)]
     L.sta_flow_destroy.argtypes = [vp]
     L.sta_flow_destroy.restype = None
-    L.sta_flow_set_keyframe.argtypes = [vp, vp, i, vp]
-    L.sta_flow_track.argtypes = [vp, vp, i, POINTER(StaFlowStats), vp]
-    L.sta_flow_promote.argtypes = [vp, vp]
     L.sta_flow_set_keyframe_group.argtypes = [POINTER(vp), i, vp, i, vp]
     L.sta_flow_track_group.argtypes = [POINTER(vp), i, POINTER(c_int), vp, i, POINTER(StaFlowStats), vp]
     L.sta_flow_promote_group.argtypes = [POINTER(vp), i, POINTER(c_int), vp]
@@ -188,11 +185,6 @@ def lib():
     L.sta_loop_destroy.argtypes = [vp]
     L.sta_loop_destroy.restype = None
     L.sta_loop_views.argtypes = [vp]
-    L.sta_loop_add_frame.argtypes = [vp, vp, i, i, i, vp]
-    L.sta_loop_detect.argtypes = [vp, i, POINTER(c_int), POINTER(c_int64), POINTER(ctypes.c_double), i, vp]
-    L.sta_loop_add_frames.argtypes = [vp, vp, i, i, i, i, vp]
-    L.sta_loop_detect_many.argtypes = [vp, i, POINTER(c_int), POINTER(c_int), POINTER(c_int64), POINTER(ctypes.c_double), i,
-                                       vp]
     L.sta_loop_add_frames_group.argtypes = [POINTER(vp), i, vp, i, i, i, vp]
     L.sta_loop_detect_group.argtypes = [POINTER(vp), i, POINTER(c_int), POINTER(c_int), POINTER(c_int64),
                                         POINTER(ctypes.c_double), i, vp]

@@ -11,15 +11,12 @@
 // are equal, so the order of descriptors does not matter) or set once (addIfNotExist); the L1 norm, the division and the
 // score s += |v - w| - |v| - |w| are sequential fp64 in ascending word id; detect_loop runs in one thread per row.
 //
-// One path serves F >= 1 frames of one size (sta_loop_add_frame / sta_loop_detect are its F = 1 case): ORB with a frame
-// grid dimension, one transform over F x 4096 descriptor slots, one CTA per frame building its vector into a staging
-// slot, an append in frame order, then one score launch and one detect launch over F rows and one host
-// synchronisation: the read-back of the candidate lists.  Every per-frame result is independent of F.
-//
-// A group call (sta_loop_add_frames_group / sta_loop_detect_group) runs that path over the frames of several detectors
-// that share one vocabulary, frame f belonging to dets[f]: ORB, transform and build over all frames in dets[0]'s
-// workspace, then the append, score and detect launches read per row a GroupRow (mapped pinned memory) naming the row's
-// database, view and loop parameters.  Every per-frame result is the one of the detector's own calls.
+// One path serves F >= 1 frames of one size, of one detector or of several that share one vocabulary, frame f belonging
+// to dets[f] (sta_loop_add_frames_group / sta_loop_detect_group; one detector's frame is a group of one): ORB with a
+// frame grid dimension and one transform over F x 4096 descriptor slots in dets[0]'s workspace, one CTA per frame
+// building its vector into a staging slot, then the append, score and detect launches, each reading per row a GroupRow
+// (mapped pinned memory) that names the row's database, view and loop parameters, and one host synchronisation: the
+// read-back of the candidate lists.  Every per-frame result is independent of F and of the other detectors.
 #include "../../include/sta_b200.h"
 #include "common.cuh"
 #include "host_util.h"
@@ -345,7 +342,7 @@ int upload_vocab(const HostVocab& v, const std::vector<int>& order, StaVocab** o
   return 0;
 }
 
-// Row f of a group call: the database of frame f's detector, the view the frame becomes there, the batch index of that
+// Row f of a group: the database of frame f's detector, the view the frame becomes there, the batch index of that
 // detector's first frame, and its detect_loop parameters.
 struct GroupRow {
   int* db_word;
@@ -451,32 +448,24 @@ __device__ long long db_end(const long long* db_start, const int* db_len, int v)
   return db_start[v] + (db_len[v] > 0 ? db_len[v] : 0);
 }
 
-// Appends the F staged vectors to the database in frame order (one CTA per frame); views view0 .. view0 + F - 1.  With
-// rows (a group call), frame f goes to rows[f]'s database as view rows[f].view, after the frames of its detector that
-// precede it in the batch.
-__global__ void append_kernel(const int* stage_word, const double* stage_val, const int* stage_len, int view0,
-                              int* db_word, double* db_val, long long* db_start, int* db_len, const GroupRow* rows) {
+// Appends the F staged vectors, one CTA per frame: frame f goes to rows[f]'s database as view rows[f].view, after the
+// frames of its detector that precede it in the batch.  The CTA reads its row once into shared memory.
+__global__ void append_kernel(const int* stage_word, const double* stage_val, const int* stage_len, const GroupRow* rows) {
   const int f = blockIdx.x;
-  int first = 0;
-  if (rows) {
-    const GroupRow r = rows[f];
-    db_word = r.db_word;
-    db_val = r.db_val;
-    db_start = r.db_start;
-    db_len = r.db_len;
-    first = r.first;
-    view0 = r.view - (f - first);
-  }
-  long long base = view0 > 0 ? db_end(db_start, db_len, view0 - 1) : 0;
-  for (int g = first; g < f; ++g) base += stage_len[g] > 0 ? stage_len[g] : 0;
+  __shared__ GroupRow r;
+  if (threadIdx.x == 0) r = rows[f];
+  __syncthreads();
+  const int view0 = r.view - (f - r.first);  // the view of the detector's first frame in the batch
+  long long base = view0 > 0 ? db_end(r.db_start, r.db_len, view0 - 1) : 0;
+  for (int g = r.first; g < f; ++g) base += stage_len[g] > 0 ? stage_len[g] : 0;
   const int len = stage_len[f];
   for (int k = threadIdx.x; k < len; k += blockDim.x) {
-    db_word[base + k] = stage_word[static_cast<long long>(f) * kOrbMaxKeypoints + k];
-    db_val[base + k] = stage_val[static_cast<long long>(f) * kOrbMaxKeypoints + k];
+    r.db_word[base + k] = stage_word[static_cast<long long>(f) * kOrbMaxKeypoints + k];
+    r.db_val[base + k] = stage_val[static_cast<long long>(f) * kOrbMaxKeypoints + k];
   }
   if (threadIdx.x == 0) {
-    db_start[view0 + f - first] = base;
-    db_len[view0 + f - first] = len;
+    r.db_start[r.view] = base;
+    r.db_len[r.view] = len;
   }
 }
 
@@ -500,29 +489,27 @@ __device__ double l1_score(const int* aw, const double* av, int na, const int* b
   return __ddiv_rn(-s, 2.0);
 }
 
-// Row y = blockIdx.y: query y (length q_len[y], at entry q_start[y] of qw / qv, or 0 without q_start) against views
-// [0, i0 + y), one thread per view, into sims + y stride.  With rows (a group call), row y is view rows[y].view of
-// rows[y]'s database against the earlier views of that database.
-__global__ void score_kernel(const int* qw, const double* qv, const long long* q_start, const int* q_len,
-                             const int* db_word, const double* db_val, const long long* db_start, const int* db_len,
-                             int i0, double* sims, long long stride, const GroupRow* rows) {
+// One thread per view j.  Row y = blockIdx.y of a group detect: view rows[y].view of rows[y]'s database against its
+// earlier views, into sims + y stride.  Without rows (sta_op_bow_score): the query (qw, qv, length *q_len) against views
+// [0, nviews) of the database db_*, into sims.
+__global__ void score_kernel(const int* qw, const double* qv, const int* q_len, const int* db_word, const double* db_val,
+                             const long long* db_start, const int* db_len, int nviews, double* sims, long long stride,
+                             const GroupRow* rows) {
   const int y = blockIdx.y;
   const int j = blockIdx.x * blockDim.x + threadIdx.x;
-  if (rows) {
-    __shared__ GroupRow row;
-    if (threadIdx.x == 0) row = rows[y];
-    __syncthreads();
-    const int i = row.view;
-    if (j >= i) return;
-    const long long* st = row.db_start;
-    const int* ln = row.db_len;
-    sims[y * stride + j] = l1_score(row.db_word + st[i], row.db_val + st[i], ln[i], row.db_word + st[j],
-                                    row.db_val + st[j], ln[j]);
+  if (!rows) {
+    if (j < nviews) sims[j] = l1_score(qw, qv, *q_len, db_word + db_start[j], db_val + db_start[j], db_len[j]);
     return;
   }
-  if (j >= i0 + y) return;
-  const long long qa = q_start ? q_start[y] : 0;
-  sims[y * stride + j] = l1_score(qw + qa, qv + qa, q_len[y], db_word + db_start[j], db_val + db_start[j], db_len[j]);
+  __shared__ GroupRow row;
+  if (threadIdx.x == 0) row = rows[y];
+  __syncthreads();
+  const int i = row.view;
+  if (j >= i) return;
+  const long long* st = row.db_start;
+  const int* ln = row.db_len;
+  sims[y * stride + j] = l1_score(row.db_word + st[i], row.db_val + st[i], ln[i], row.db_word + st[j],
+                                  row.db_val + st[j], ln[j]);
 }
 
 // loop_detector.py:23-50 over the precomputed similarities of view i; out: [0] = count, [1] = length of view i, then
@@ -564,32 +551,18 @@ __device__ void detect_row(const double* sims, const int* db_len, int i, int far
   out[1] = db_len[i];
 }
 
-// One thread per row f (view i0 + f): out row f = {ORB overflow flag of frame f, then detect_row's count, length and
-// pairs}, `out_stride` entries apart; after the gridDim.x rows, the database entries in use.  With rows (a group call),
-// row f is view rows[f].view of rows[f]'s database with that row's parameters, and every row f writes its database's
-// entries in use at gridDim.x out_stride + f.
-__global__ void detect_kernel(const double* sims, long long sims_stride, const long long* db_start, const int* db_len,
-                              int i0, const int* farthest, int dist_min, int nms, int thresh_neighbor, long long* out,
+// One thread per row f: view rows[f].view of rows[f]'s database with that row's parameters.  Out row f = {ORB overflow
+// flag of frame f, then detect_row's count, length and pairs}, `out_stride` entries apart; after the gridDim.x rows,
+// entry gridDim.x out_stride + f holds the entries in use of row f's database.
+__global__ void detect_kernel(const double* sims, long long sims_stride, const int* farthest, long long* out,
                               long long out_stride, const unsigned* overflow, size_t overflow_stride,
                               const GroupRow* rows) {
   const int f = blockIdx.x;
-  int i = i0 + f;
-  if (rows) {
-    const GroupRow r = rows[f];
-    db_start = r.db_start;
-    db_len = r.db_len;
-    i = r.view;
-    dist_min = r.dist_min;
-    nms = r.nms;
-    thresh_neighbor = r.thresh_neighbor;
-  }
+  const GroupRow r = rows[f];
+  out[gridDim.x * out_stride + f] = db_end(r.db_start, r.db_len, r.view);
   long long* row = out + f * out_stride;
-  detect_row(sims + f * sims_stride, db_len, i, farthest[f], dist_min, nms, thresh_neighbor, row + 1);
   row[0] = *reinterpret_cast<const unsigned*>(reinterpret_cast<const char*>(overflow) + f * overflow_stride);
-  if (rows)
-    out[gridDim.x * out_stride + f] = db_end(db_start, db_len, i);
-  else if (f == static_cast<int>(gridDim.x) - 1)
-    out[(f + 1) * out_stride] = db_end(db_start, db_len, i);
+  detect_row(sims + f * sims_stride, r.db_len, r.view, farthest[f], r.dist_min, r.nms, r.thresh_neighbor, row + 1);
 }
 
 }  // namespace
@@ -605,7 +578,6 @@ struct StaLoopDetector {
   void* scratch = nullptr;        // ORB scratch: frame_cap slices of lay.total bytes
   void* kp = nullptr;             // ORB outputs + transform outputs: frame_cap slices of kKpSlice bytes
   int frame_cap = 0, stage_cap = 0;
-  int last_batch = 0;             // frames of the last add call
   int* stage_word = nullptr;      // [stage_cap][kOrbMaxKeypoints] vectors of a batch before the append
   double* stage_val = nullptr;
   int* stage_len = nullptr;       // [stage_cap]
@@ -614,7 +586,7 @@ struct StaLoopDetector {
   long long* result = nullptr;    // its rows and the database entries in use
   long long* pinned = nullptr;    // host copy of result
   long long out_cap = 0;          // entries of sims / result / pinned
-  long long last_row = 0;         // offset in sims of the last detect's last row
+  long long last_row = 0;         // offset in sims of the last row of this detector's last detect of its own rows
   int last_row_len = 0;           // its length (the view index of that row)
   int views = 0, view_cap = 0;
   // Upper bound on the database entries in use, kept on the host: each appended view may add up to kOrbMaxKeypoints
@@ -625,14 +597,14 @@ struct StaLoopDetector {
   double* db_val = nullptr;
   long long* db_start = nullptr;
   int* db_len = nullptr;
-  // Group calls of which this detector is dets[0]: the row table of the last group add (mapped host memory, read by its
-  // append, score and detect launches), that add's detectors per frame and each one's view count after it.
+  // Calls of which this detector is dets[0]: the row table of the last add (mapped host memory, read by its append,
+  // score and detect launches), that add's detectors per frame and each one's view count after it.
   GroupRow* rows_pinned = nullptr;
   int rows_cap = 0;
   std::vector<StaLoopDetector*> group_dets;
   std::vector<int> group_views;
-  bool group_pending = false;   // the last group add's append may still read rows_pinned (no group detect since)
-  bool group_detected = false;  // this detector's last detect was a group detect: sta_loop_similarities is refused
+  bool group_pending = false;   // the last add's append may still read rows_pinned (no detect since)
+  bool group_detected = false;  // this detector's last detect had other detectors' rows: sta_loop_similarities is refused
 };
 
 namespace {
@@ -849,8 +821,8 @@ int sta_op_bow_score(const int32_t* qw, const double* qv, const int32_t* q_len_d
   STA_REQUIRE(nviews >= 0, "bad view count");
   if (nviews)
     score_kernel<<<(nviews + 127) / 128, 128, 0, static_cast<cudaStream_t>(stream)>>>(
-        qw, qv, nullptr, q_len_dev, db_word, db_val, reinterpret_cast<const long long*>(db_start), db_len, nviews,
-        sims_out, 0, nullptr);
+        qw, qv, q_len_dev, db_word, db_val, reinterpret_cast<const long long*>(db_start), db_len, nviews, sims_out, 0,
+        nullptr);
   STA_CHECK_CUDA(cudaGetLastError());
   return 0;
 }
@@ -888,90 +860,11 @@ void sta_loop_destroy(StaLoopDetector* d) {
 
 int sta_loop_views(const StaLoopDetector* d) { return d ? d->views : -1; }
 
-// compute_bow_feat for F frames [F][H][W] of one size: ORB over all frames, one transform, one build CTA per frame and
-// the append in frame order (asynchronous)
-int sta_loop_add_frames(StaLoopDetector* d, const void* frames_dev, int frames_is_f32, int F, int H, int W, void* stream) {
-  STA_REQUIRE(d && frames_dev, "null argument");
-  STA_REQUIRE(F >= 1, "the frame count must be at least 1");
-  STA_REQUIRE(orb_size_ok(H, W), "ORB frame sides must be in [32, 4096]");
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (prepare_frames(d, F, H, W, st) || grow_batch(d, F, st) || reserve(d, st, F)) return 1;
-  KpBufs b = kp_bufs(d->kp, d->frame_cap);
-  OrbOut o = {b.xy, b.level, b.pts, b.angle, b.resp, b.desc, b.count};
-  if (orb_run(d->lay, d->scratch, frames_dev, frames_is_f32, o, st, F)) return 1;
-  if (bow_of_descriptors(d->vocab, b.desc, b.count, 0, b.word, b.weight, st, F)) return 1;
-  build_kernel<<<F, kBuildThreads, 0, st>>>(b.word, b.weight, b.count, 0, d->vocab->weighting, d->stage_word,
-                                            d->stage_val, d->stage_len);
-  append_kernel<<<F, 256, 0, st>>>(d->stage_word, d->stage_val, d->stage_len, d->views, d->db_word, d->db_val,
-                                   d->db_start, d->db_len, nullptr);
-  STA_CHECK_CUDA(cudaGetLastError());
-  d->views += F;
-  d->entries_bound += static_cast<long long>(F) * kOrbMaxKeypoints;
-  d->last_batch = F;
-  d->last_stream = st;
-  return 0;
-}
-
-// compute_bow_feat: the one-frame case of sta_loop_add_frames
-int sta_loop_add_frame(StaLoopDetector* d, const void* frame_dev, int frame_is_f32, int H, int W, void* stream) {
-  return sta_loop_add_frames(d, frame_dev, frame_is_f32, 1, H, W, stream);
-}
-
-// detect_loop for each of the newest F views (the frames of the last sta_loop_add_frames, or fewer of its newest), row
-// f = view views - F + f against every earlier view: one score launch, one detect launch and one read-back, which also
-// brings the database's entry count.  n_out [2F] = {candidates, length (-1: None)} per row; row f's first cap_per_view
-// candidates go to js_out / sims_out + f cap_per_view (host).  Afterwards sta_loop_similarities returns the last row.
-int sta_loop_detect_many(StaLoopDetector* d, int F, const int* farthest_host, int* n_out, int64_t* js_out,
-                         double* sims_out, int cap_per_view, void* stream) {
-  STA_REQUIRE(d && farthest_host && n_out && (cap_per_view == 0 || (js_out && sims_out)), "null argument");
-  STA_REQUIRE(F >= 1 && F <= d->last_batch, "F must be in [1, frames of the last add call]");
-  STA_REQUIRE(cap_per_view >= 0, "bad capacity");
-  const int i0 = d->views - F;
-  for (int f = 0; f < F; ++f)
-    STA_REQUIRE(farthest_host[f] >= 0 && farthest_host[f] <= i0 + f, "farthest_neighbor must be in [0, view index]");
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  d->last_stream = st;
-  const long long sims_stride = d->views, out_stride = 3 + 2LL * d->views;  // out_stride > sims_stride
-  const long long need = F * out_stride + 1;
-  if (grow_results(d, need, st)) return 1;
-  d->group_detected = false;
-  memcpy(d->farthest_pinned, farthest_host, sizeof(int) * F);  // the previous detect has synchronised
-  const int i_last = d->views - 1;
-  if (i_last > 0)
-    score_kernel<<<dim3((i_last + 127) / 128, F), 128, 0, st>>>(d->db_word, d->db_val, d->db_start + i0, d->db_len + i0,
-                                                                 d->db_word, d->db_val, d->db_start, d->db_len, i0,
-                                                                 d->sims, sims_stride, nullptr);
-  const int first_slice = d->last_batch - F;  // scratch slice of row 0
-  detect_kernel<<<F, 1, 0, st>>>(d->sims, sims_stride, d->db_start, d->db_len, i0, d->farthest_pinned, d->dist_min,
-                                 d->nms, d->thresh_neighbor, d->result, out_stride,
-                                 reinterpret_cast<const unsigned*>(static_cast<char*>(d->scratch) +
-                                                                   first_slice * d->lay.total + d->lay.counters +
-                                                                   3 * sizeof(unsigned)),
-                                 d->lay.total, nullptr);
-  STA_CHECK_CUDA(cudaGetLastError());
-  d->last_row = (F - 1) * sims_stride;
-  d->last_row_len = i_last;
-  STA_CHECK_CUDA(cudaMemcpyAsync(d->pinned, d->result, sizeof(long long) * need, cudaMemcpyDeviceToHost, st));
-  STA_CHECK_CUDA(cudaStreamSynchronize(st));
-  d->entries_bound = d->pinned[F * out_stride];
-  if (report_overflow(d->pinned, F, out_stride)) return 1;
-  for (int f = 0; f < F; ++f) copy_row(d->pinned + f * out_stride, f, n_out, js_out, sims_out, cap_per_view);
-  return 0;
-}
-
-// detect_loop for the newest view: the one-row case of sta_loop_detect_many.
-// js_out / sims_out (host) receive up to `cap` candidates; n_out[2] = {number found, length of view i (-1: None)}.
-int sta_loop_detect(StaLoopDetector* d, int farthest_neighbor, int* n_out, int64_t* js_out, double* sims_out, int cap,
-                    void* stream) {
-  STA_REQUIRE(d && d->views > 0, "no view has been added");
-  return sta_loop_detect_many(d, 1, &farthest_neighbor, n_out, js_out, sims_out, cap, stream);
-}
-
-// sta_loop_add_frames over the frames of several detectors: frame f belongs to dets[f], each detector's frames are
+// compute_bow_feat for F frames [F][H][W] of one size: frame f belongs to dets[f], each detector's frames are
 // consecutive, and all share one vocabulary (refused before any launch otherwise).  ORB, transform and build run over
-// all F frames in dets[0]'s workspace; one append launch writes each frame into its own detector's database through
-// dets[0]'s row table.  Asynchronous, unless dets[0]'s previous group add has had no group detect yet: its append may
-// still read the row table, so the stream is synchronised before the table is rewritten.
+// all F frames in dets[0]'s workspace; one append launch writes each frame into its own detector's database, in frame
+// order, through dets[0]'s row table.  Asynchronous, unless dets[0]'s previous add has had no detect yet: its append
+// may still read the row table, so the stream is synchronised before the table is rewritten.
 int sta_loop_add_frames_group(StaLoopDetector* const* dets, int F, const void* frames_dev, int frames_is_f32, int H,
                               int W, void* stream) {
   STA_REQUIRE(dets && frames_dev, "null argument");
@@ -1012,29 +905,27 @@ int sta_loop_add_frames_group(StaLoopDetector* const* dets, int F, const void* f
   if (bow_of_descriptors(d0->vocab, b.desc, b.count, 0, b.word, b.weight, st, F)) return 1;
   build_kernel<<<F, kBuildThreads, 0, st>>>(b.word, b.weight, b.count, 0, d0->vocab->weighting, d0->stage_word,
                                             d0->stage_val, d0->stage_len);
-  append_kernel<<<F, 256, 0, st>>>(d0->stage_word, d0->stage_val, d0->stage_len, 0, nullptr, nullptr, nullptr, nullptr,
-                                   d0->rows_pinned);
+  append_kernel<<<F, 256, 0, st>>>(d0->stage_word, d0->stage_val, d0->stage_len, d0->rows_pinned);
   STA_CHECK_CUDA(cudaGetLastError());
   d0->group_pending = true;
   for (int f = 0; f < F; ++f) {
     StaLoopDetector* d = dets[f];
     d->views++;
     d->entries_bound += kOrbMaxKeypoints;
-    d->last_batch = 0;  // the frames' ORB state is in dets[0]'s scratch: the detector's own detect waits for its own add
     d->last_stream = st;
   }
-  d0->last_batch = 0;
   d0->group_dets.assign(dets, dets + F);
   d0->group_views.resize(F);
   for (int f = 0; f < F; ++f) d0->group_views[f] = dets[f]->views;
   return 0;
 }
 
-// sta_loop_detect_many over the rows of the last sta_loop_add_frames_group of dets[0], with the same dets and F and no
-// view added to any of them since: one score launch and one detect launch over all rows, each against its own
-// database with its own detector's parameters, then one read-back, which also brings every detector's entry count.
-// The outputs are laid out as sta_loop_detect_many's.  Afterwards sta_loop_similarities is refused on these detectors
-// until their own next detect.
+// detect_loop for the rows of the last sta_loop_add_frames_group of dets[0], with the same dets and F and no view added
+// to any of them since: one score launch and one detect launch over all rows, each against its own database with its
+// own detector's parameters, then one read-back, which also brings every detector's entry count.  n_out [2F] =
+// {candidates, length (-1: None)} per row; row f's first cap_per_view candidates go to js_out / sims_out + f
+// cap_per_view (host).  Afterwards sta_loop_similarities returns the last row when every row was dets[0]'s, and is
+// refused on the detectors until their own next detect otherwise.
 int sta_loop_detect_group(StaLoopDetector* const* dets, int F, const int* farthest_host, int* n_out, int64_t* js_out,
                           double* sims_out, int cap_per_view, void* stream) {
   STA_REQUIRE(dets && dets[0] && farthest_host && n_out && (cap_per_view == 0 || (js_out && sims_out)), "null argument");
@@ -1057,10 +948,8 @@ int sta_loop_detect_group(StaLoopDetector* const* dets, int F, const int* farthe
   memcpy(d0->farthest_pinned, farthest_host, sizeof(int) * F);  // every earlier detect has synchronised
   if (max_view > 0)
     score_kernel<<<dim3((max_view + 127) / 128, F), 128, 0, st>>>(nullptr, nullptr, nullptr, nullptr, nullptr, nullptr,
-                                                                   nullptr, nullptr, 0, d0->sims, sims_stride,
-                                                                   d0->rows_pinned);
-  detect_kernel<<<F, 1, 0, st>>>(d0->sims, sims_stride, nullptr, nullptr, 0, d0->farthest_pinned, 0, 0, 0, d0->result,
-                                 out_stride,
+                                                                   nullptr, 0, d0->sims, sims_stride, d0->rows_pinned);
+  detect_kernel<<<F, 1, 0, st>>>(d0->sims, sims_stride, d0->farthest_pinned, d0->result, out_stride,
                                  reinterpret_cast<const unsigned*>(static_cast<char*>(d0->scratch) + d0->lay.counters +
                                                                    3 * sizeof(unsigned)),
                                  d0->lay.total, d0->rows_pinned);
@@ -1068,8 +957,13 @@ int sta_loop_detect_group(StaLoopDetector* const* dets, int F, const int* farthe
   STA_CHECK_CUDA(cudaMemcpyAsync(d0->pinned, d0->result, sizeof(long long) * need, cudaMemcpyDeviceToHost, st));
   STA_CHECK_CUDA(cudaStreamSynchronize(st));
   d0->group_pending = false;
+  const bool own = dets[F - 1] == d0;  // every row is d0's: a detector's frames are consecutive
+  if (own) {
+    d0->last_row = (F - 1) * sims_stride;
+    d0->last_row_len = max_view;
+  }
   for (int f = 0; f < F; ++f) {
-    dets[f]->group_detected = true;
+    dets[f]->group_detected = !own;
     dets[f]->last_stream = st;
     if (f == F - 1 || dets[f + 1] != dets[f]) dets[f]->entries_bound = d0->pinned[F * out_stride + f];
   }
@@ -1100,7 +994,8 @@ int sta_loop_view(StaLoopDetector* d, int view, int32_t* words_out, double* vals
 // Host copy of the last row of the last detect (NaN where a vector is None); n = that row's view index.
 int sta_loop_similarities(StaLoopDetector* d, double* sims_out, int n, void* stream) {
   STA_REQUIRE(d, "null argument");
-  STA_REQUIRE(!d->group_detected, "the detector's last detect was a group detect, whose rows it does not keep");
+  STA_REQUIRE(!d->group_detected,
+              "the detector's last detect was a group detect over several detectors, whose rows it does not keep");
   STA_REQUIRE(n >= 0 && n <= d->last_row_len, "bad count: n must be at most the view index of the last detect");
   if (n == 0) return 0;
   cudaStream_t st = static_cast<cudaStream_t>(stream);

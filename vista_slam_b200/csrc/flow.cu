@@ -10,15 +10,15 @@
 // would otherwise contract to FMA) in the order OpenCV's LKTrackerInvoker uses.  The greedy minimum-distance selection
 // of goodFeaturesToTrack is resolved in rounds inside one CTA (see select_kernel); the result is the sequential one.
 //
-// Buffers (one arena per frame size): two padded pyramids (the keyframe's and the current frame's, swapped when a frame
-// becomes the keyframe), the keyframe's Scharr derivatives, the corner selection scratch, the keyframe corners, the LK
-// output and the statistics the host reads once per tracked frame.  A group track (sta_flow_track_group) adds frame
-// pyramid slots per tracker, and LK output and statistics for every frame of the group.
+// Buffers (one arena per frame size): two padded pyramids (a tracker's keyframe and its first frame slot, swapped when
+// that frame becomes the keyframe), the keyframe's Scharr derivatives, the corner selection scratch and the keyframe
+// corners.  A tracker adds pyramid slots for the frames of its largest group track, and the LK output and statistics of
+// every frame of a group it leads.
 //
 // Every stage runs over a batch: the pyramid kernels over frames, LK and the statistics over (frame, keyframe) items,
 // the derivative and corner kernels over keyframes, each with the batch index in blockIdx.y (one CTA per keyframe in
 // select_kernel, one per item in flow_stats_kernel).  The per-item pointers travel in a __grid_constant__ table of at
-// most kMaxBatch entries; a larger batch is several launches.  The one-frame entry points are batches of one.
+// most kMaxBatch entries; a larger batch is several launches.  One frame is a group of one.
 #include "../../include/sta_b200.h"
 #include "common.cuh"
 #include "host_util.h"
@@ -80,7 +80,7 @@ Levels make_levels(int H, int W) {
 // every buffer the tracker and the op-level entry points use, carved from one arena
 struct Layout {
   Levels lv;
-  size_t pyr[2], deriv, sob, eig, state, cand, acc, counters, corners, ncorners, next_pts, status, stats, total;
+  size_t pyr[2], deriv, sob, eig, state, cand, acc, counters, corners, ncorners, total;
   int acc_cap;
 };
 
@@ -109,9 +109,6 @@ Layout make_layout(int H, int W) {
   s.counters = take(kNumCounters * sizeof(unsigned));
   s.corners = take(kMaxCorners * sizeof(float2));
   s.ncorners = take(sizeof(int));
-  s.next_pts = take(kMaxCorners * sizeof(float2));
-  s.status = take(kMaxCorners);
-  s.stats = take(sizeof(StaFlowStats));
   s.total = off;
   return s;
 }
@@ -717,21 +714,21 @@ struct StaFlowTracker {
   int H = 0, W = 0;
   Layout s;
   void* arena = nullptr;
-  uint8_t* kf_pyr = nullptr;   // the keyframe's pyramid
-  uint8_t* cur_pyr = nullptr;  // the frame of the last sta_flow_track; sta_flow_promote swaps the two
-  bool has_kf = false, has_cur = false;  // a keyframe was set / a frame was tracked since
-  StaFlowStats* pinned = nullptr;      // host copy of the statistics
+  uint8_t* kf_pyr = nullptr;  // the keyframe's pyramid
+  bool has_kf = false;        // a keyframe was set
   cudaStream_t last_stream = nullptr;
   bool has_stream = false;
   cudaEvent_t ev_switch = nullptr;
-  // Group tracks.  Frame pyramid slots, allocated on first use and grown to the most frames this tracker had in one
-  // group: frame j of its last group track is in slots[j] (group_n frames).  A group promotion of frame j swaps
-  // slots[j] with kf_pyr, and the frames after it stay held in slots[held_first, held_first + held_n) for the next
-  // group track to reuse.
+  // Frame pyramid slots: the arena's second pyramid, then more allocated when a group track first needs them, up to the
+  // most frames this tracker had in one group.  Frame j of its last group track is in slots[j] (group_n frames).  A
+  // promotion of frame j swaps slots[j] with kf_pyr, and the frames after it stay held in
+  // slots[held_first, held_first + held_n) for the next group track to reuse.
   std::vector<uint8_t*> slots;
   std::vector<void*> slot_allocs;
   int group_n = 0, held_first = 0, held_n = 0;
-  // when this tracker is the first of a group: LK output and statistics of every frame of the group
+  // when this tracker is the first of a group: LK output and statistics of every frame of the group, allocated at
+  // creation for 16 frames (so a tracker used one frame at a time makes no cudaMalloc, which can stall other streams,
+  // after sta_flow_create) and grown by larger groups
   int gcap = 0;
   void* gbuf = nullptr;  // [gcap][1000] float2 next points, [gcap][1000] uint8 status, [gcap] StaFlowStats
   StaFlowStats* gpinned = nullptr;
@@ -762,9 +759,6 @@ LkItem lk_item(StaFlowTracker* t, const uint8_t* J, float2* next, uint8_t* statu
   return LkItem{t->kf_pyr, at<const short2>(t->arena, t->s.deriv), J, at<const float2>(t->arena, t->s.corners),
                 at<const int>(t->arena, t->s.ncorners), next, status};
 }
-
-// a one-frame call ends whatever group track the tracker was in
-void end_group(StaFlowTracker* t) { t->group_n = t->held_n = 0; }
 
 size_t group_stats_offset(int cap) {
   return (static_cast<size_t>(cap) * kMaxCorners * (sizeof(float2) + 1) + 255) & ~static_cast<size_t>(255);
@@ -828,34 +822,31 @@ int sta_flow_create(int H, int W, StaFlowTracker** out) {
   t->H = H;
   t->W = W;
   t->s = make_layout(H, W);
-  cudaError_t e = cudaMalloc(&t->arena, t->s.total);
-  if (e == cudaSuccess) e = cudaMallocHost(reinterpret_cast<void**>(&t->pinned), sizeof(StaFlowStats));
+  const cudaError_t e = cudaMalloc(&t->arena, t->s.total);
   if (e != cudaSuccess) {
     set_last_error(std::string("sta_flow_create: ") + cudaGetErrorString(e));
     sta_flow_destroy(t);
     return 1;
   }
   t->kf_pyr = at<uint8_t>(t->arena, t->s.pyr[0]);
-  t->cur_pyr = at<uint8_t>(t->arena, t->s.pyr[1]);
+  t->slots.push_back(at<uint8_t>(t->arena, t->s.pyr[1]));
+  if (int rc = ensure_group_buffers(t, 1)) {
+    sta_flow_destroy(t);
+    return rc;
+  }
   *out = t;
   return 0;
 }
 
 void sta_flow_destroy(StaFlowTracker* t) {
   if (!t) return;
-  if (t->arena || t->pinned || t->gbuf || !t->slot_allocs.empty()) cudaDeviceSynchronize();
+  if (t->arena || t->gbuf || !t->slot_allocs.empty()) cudaDeviceSynchronize();
   if (t->arena) cudaFree(t->arena);
   for (void* p : t->slot_allocs) cudaFree(p);
   if (t->gbuf) cudaFree(t->gbuf);
-  if (t->pinned) cudaFreeHost(t->pinned);
   if (t->gpinned) cudaFreeHost(t->gpinned);
   if (t->ev_switch) cudaEventDestroy(t->ev_switch);
   delete t;
-}
-
-int sta_flow_set_keyframe(StaFlowTracker* t, const void* frame_dev, int frame_is_f32, void* stream) {
-  STA_REQUIRE(t != nullptr && frame_dev != nullptr, "null argument");
-  return sta_flow_set_keyframe_group(&t, 1, frame_dev, frame_is_f32, stream);
 }
 
 int sta_flow_set_keyframe_group(StaFlowTracker* const* ts, int n, const void* frames_dev, int frames_is_f32,
@@ -879,27 +870,8 @@ int sta_flow_set_keyframe_group(StaFlowTracker* const* ts, int n, const void* fr
   STA_CHECK_CUDA(cudaGetLastError());
   for (int i = 0; i < n; ++i) {
     ts[i]->has_kf = true;
-    ts[i]->has_cur = false;
-    end_group(ts[i]);
+    ts[i]->group_n = ts[i]->held_n = 0;
   }
-  return 0;
-}
-
-int sta_flow_track(StaFlowTracker* t, const void* frame_dev, int frame_is_f32, StaFlowStats* stats_out, void* stream) {
-  STA_REQUIRE(t != nullptr && frame_dev != nullptr && stats_out != nullptr, "null argument");
-  STA_REQUIRE(t->has_kf, "no keyframe: call sta_flow_set_keyframe first");
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (int rc = bind_stream(t, st)) return rc;
-  const Layout& s = t->s;
-  end_group(t);
-  if (int rc = build_pyramids(s, 1, &frame_dev, frame_is_f32, &t->cur_pyr, st)) return rc;
-  t->has_cur = true;
-  const LkItem item = lk_item(t, t->cur_pyr, at<float2>(t->arena, s.next_pts), at<uint8_t>(t->arena, s.status));
-  StaFlowStats* dstats = at<StaFlowStats>(t->arena, s.stats);
-  if (int rc = track_items(s, 1, &item, 0, dstats, st)) return rc;
-  STA_CHECK_CUDA(cudaMemcpyAsync(t->pinned, dstats, sizeof(StaFlowStats), cudaMemcpyDeviceToHost, st));
-  STA_CHECK_CUDA(cudaStreamSynchronize(st));
-  *stats_out = *t->pinned;
   return 0;
 }
 
@@ -912,7 +884,7 @@ int sta_flow_track_group(StaFlowTracker* const* ts, int F, const int* held_host,
   int n_new = 0;
   for (int f = 0; f < F; ++f) {
     StaFlowTracker* t = ts[f];
-    STA_REQUIRE(t->has_kf, "no keyframe: call sta_flow_set_keyframe first");
+    STA_REQUIRE(t->has_kf, "no keyframe: call sta_flow_set_keyframe_group first");
     j_of[f] = (f > 0 && ts[f - 1] == t) ? j_of[f - 1] + 1 : 0;
     const bool held = held_host && held_host[f];
     if (held) {
@@ -954,7 +926,6 @@ int sta_flow_track_group(StaFlowTracker* const* ts, int F, const int* held_host,
     items[f] = lk_item(t, J, gnext + static_cast<size_t>(f) * kMaxCorners, gstatus + static_cast<size_t>(f) * kMaxCorners);
   }
   for (int f = 0; f < F; ++f) {
-    ts[f]->has_cur = false;
     ts[f]->held_n = 0;
     ts[f]->group_n = j_of[f] + 1;
   }
@@ -964,20 +935,6 @@ int sta_flow_track_group(StaFlowTracker* const* ts, int F, const int* held_host,
   STA_CHECK_CUDA(cudaMemcpyAsync(ts[0]->gpinned, gstats, F * sizeof(StaFlowStats), cudaMemcpyDeviceToHost, st));
   STA_CHECK_CUDA(cudaStreamSynchronize(st));
   for (int f = 0; f < F; ++f) stats_out[f] = ts[0]->gpinned[f];
-  return 0;
-}
-
-int sta_flow_promote(StaFlowTracker* t, void* stream) {
-  STA_REQUIRE(t != nullptr, "null argument");
-  STA_REQUIRE(t->has_cur, "no tracked frame to promote");
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (int rc = bind_stream(t, st)) return rc;
-  std::swap(t->kf_pyr, t->cur_pyr);
-  t->has_cur = false;
-  end_group(t);
-  const KfJob job = kf_job(t);
-  if (int rc = keyframe_products(t->s, 1, &job, true, true, st)) return rc;
-  STA_CHECK_CUDA(cudaGetLastError());
   return 0;
 }
 
@@ -996,7 +953,6 @@ int sta_flow_promote_group(StaFlowTracker* const* ts, int n, const int* frame_ho
     t->held_first = j + 1;
     t->held_n = t->group_n - j - 1;
     t->group_n = 0;
-    t->has_cur = false;
     jobs[i] = kf_job(t);
   }
   if (int rc = keyframe_products(ts[0]->s, n, jobs.data(), true, true, st)) return rc;

@@ -53,13 +53,16 @@ def _as_device_frame(image, device=None):
 
 
 class _Tracker:
-    """Owner of one C tracker handle (one frame size, one device)."""
+    """Owner of one C tracker handle (one frame size, one device), with the one-element tables of its one-frame group
+    calls."""
 
     def __init__(self, H, W, device):
         self.H, self.W, self.device = H, W, device
         h = ctypes.c_void_p()
         _lib.check(_lib.lib().sta_flow_create(H, W, ctypes.byref(h)), "sta_flow_create")
         self.h = h
+        self.group = (ctypes.c_void_p * 1)(h.value)
+        self.frame0 = (ctypes.c_int * 1)(0)
         self.stats = _lib.StaFlowStats()
 
     def __del__(self):
@@ -110,8 +113,8 @@ class FlowTracker:
         frame, is_f32 = _as_device_frame(image)
         t = self._tracker_for(frame)
         with torch.cuda.device(frame.device):
-            _lib.check(_lib.lib().sta_flow_set_keyframe(t.h, _lib.ptr(frame), is_f32, _lib.cur_stream()),
-                       "sta_flow_set_keyframe")
+            _lib.check(_lib.lib().sta_flow_set_keyframe_group(t.group, 1, _lib.ptr(frame), is_f32, _lib.cur_stream()),
+                       "sta_flow_set_keyframe_group")
         self._set_keyframe(image, t)
 
     def _set_keyframe(self, image, t):
@@ -148,8 +151,8 @@ class FlowTracker:
         if tuple(frame.shape) != (t.H, t.W):
             raise ValueError("frame size %s differs from the keyframe's %s" % (tuple(frame.shape), (t.H, t.W)))
         with torch.cuda.device(frame.device):
-            _lib.check(_lib.lib().sta_flow_track(t.h, _lib.ptr(frame), is_f32, ctypes.byref(t.stats), _lib.cur_stream()),
-                       "sta_flow_track")
+            _lib.check(_lib.lib().sta_flow_track_group(t.group, 1, None, _lib.ptr(frame), is_f32, ctypes.byref(t.stats),
+                                                       _lib.cur_stream()), "sta_flow_track_group")
         s = t.stats
         if s.n_corners < MIN_TRACKED or s.n_tracked < MIN_TRACKED:
             self._promote(image, t)
@@ -162,7 +165,7 @@ class FlowTracker:
 
     def _promote(self, image, t):
         with torch.cuda.device(t.device):
-            _lib.check(_lib.lib().sta_flow_promote(t.h, _lib.cur_stream()), "sta_flow_promote")
+            _lib.check(_lib.lib().sta_flow_promote_group(t.group, 1, t.frame0, _lib.cur_stream()), "sta_flow_promote_group")
         self._set_keyframe(image, t)
 
     def compute_disparities(self, frames):

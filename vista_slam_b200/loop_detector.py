@@ -3,9 +3,10 @@
 `detect_loop(image, farthest_neighbor)` returns the reference's [(j, similarity), ...] -- cv2.ORB_create() features,
 the DBoW3 vocabulary transform and L1 scores against the earlier keyframes -- but runs ORB (csrc/orb.cu) and the
 bag-of-words transform, database and scoring (csrc/bow.cu) as CUDA kernels, with one host synchronisation per call: the
-read-back of the candidate list.  `detect_loops(images, farthest_neighbors)` does the same for many frames of one size
-with one host synchronisation for all of them, and `detect_loops_group(detectors, ...)` for the frames of several detectors
-that share one `Vocabulary` (SLAM sessions stepped together).  The frame may stay on the device from
+read-back of the candidate list.  `detect_loops_group(detectors, ...)` does the same for many frames of one size and of
+several detectors that share one `Vocabulary` (SLAM sessions stepped together) with one host synchronisation for all of
+them, and `detect_loops(images, farthest_neighbors)` for many frames of one detector.  All three run one path, a group
+of frames (csrc/bow.cu's sta_loop_add_frames_group / sta_loop_detect_group).  The frame may stay on the device from
 SLAM_image_only.process_image.  There is no CPU path.
 
 The vocabulary is a DBoW3 text file (what the shipped configs name, e.g. pretrains/ORBvoc.txt) or a DBoW3 binary file,
@@ -66,6 +67,7 @@ class LoopDetector:
         _lib.check(_lib.lib().sta_loop_create(self.vocab.h, loop_dist_min, loop_nms, loop_cand_thresh_neighbor,
                                                ctypes.byref(h)), "sta_loop_create")
         self._h = h
+        self._group = (ctypes.c_void_p * 1)(h.value)  # the detector table of its own calls: a group of one
         self._device = torch.device("cuda", torch.cuda.current_device())
 
     def __del__(self):
@@ -86,8 +88,8 @@ class LoopDetector:
         frame, is_f32 = _as_device_frame(image, self._device)
         H, W = frame.shape
         with torch.cuda.device(frame.device):
-            _lib.check(_lib.lib().sta_loop_add_frame(self._h, _lib.ptr(frame), is_f32, H, W, _lib.cur_stream()),
-                       "sta_loop_add_frame")
+            _lib.check(_lib.lib().sta_loop_add_frames_group(self._group, 1, _lib.ptr(frame), is_f32, H, W,
+                                                            _lib.cur_stream()), "sta_loop_add_frames_group")
         return len(self.bow_feats)
 
     def detect_loop(self, image, farthest_neighbor):
@@ -104,8 +106,8 @@ class LoopDetector:
         js = (ctypes.c_int64 * cap)()
         sims = (ctypes.c_double * cap)()
         with torch.cuda.device(self._device):
-            _lib.check(_lib.lib().sta_loop_detect(self._h, farthest_neighbor, n, js, sims, cap, _lib.cur_stream()),
-                       "sta_loop_detect")
+            _lib.check(_lib.lib().sta_loop_detect_group(self._group, 1, ctypes.byref(ctypes.c_int(farthest_neighbor)), n,
+                                                        js, sims, cap, _lib.cur_stream()), "sta_loop_detect_group")
         if n[1] < 0:
             self.bow_feats[i] = None
         return [(int(js[k]), float(sims[k])) for k in range(n[0])]
@@ -115,44 +117,12 @@ class LoopDetector:
         database append over all frames, one score and one detect launch over their rows and ONE host synchronisation.
         Returns the list of candidate lists.  The frames must share one size and type; a refusal comes before any
         launch."""
-        images, far = list(images), [int(f) for f in farthest_neighbors]
-        if len(images) != len(far):
-            raise ValueError("one farthest_neighbor per image")
-        F = len(images)
-        if F == 0:
-            return []
-        i0 = len(self.bow_feats)
-        for f, x in enumerate(far):
-            if not 0 <= x <= i0 + f:
-                raise ValueError("farthest_neighbor of frame %d must be in [0, %d]" % (f, i0 + f))
-        frames = [_as_device_frame(im, self._device) for im in images]
-        if any(t.shape != frames[0][0].shape or k != frames[0][1] for t, k in frames):
-            raise ValueError("all frames of a batch must have the same size and type")
-        batch = torch.stack([t for t, _ in frames]).contiguous() if F > 1 else frames[0][0]
-        is_f32 = frames[0][1]
-        H, W = frames[0][0].shape
-        with torch.cuda.device(batch.device):
-            _lib.check(_lib.lib().sta_loop_add_frames(self._h, _lib.ptr(batch), is_f32, F, H, W, _lib.cur_stream()),
-                       "sta_loop_add_frames")
-        # the views are in the device database from here on, so bow_feats gets their entries even if detection fails
-        self.bow_feats.extend(BowVector(self, i0 + f) for f in range(F))
-        n = (ctypes.c_int * (2 * F))()
-        cap = max(i0 + F - 1, 1)
-        js = (ctypes.c_int64 * (F * cap))()
-        sims = (ctypes.c_double * (F * cap))()
-        with torch.cuda.device(self._device):
-            _lib.check(_lib.lib().sta_loop_detect_many(self._h, F, (ctypes.c_int * F)(*far), n, js, sims, cap,
-                                                        _lib.cur_stream()), "sta_loop_detect_many")
-        out = []
-        for f in range(F):
-            if n[2 * f + 1] < 0:
-                self.bow_feats[i0 + f] = None
-            out.append([(int(js[f * cap + k]), float(sims[f * cap + k])) for k in range(n[2 * f])])
-        return out
+        return detect_loops_group([self], [images], [farthest_neighbors])[0]
 
     def similarities(self):
         """fp64 scores of the newest view against every earlier one from the last detect_loop (NaN where either
-        vector is None).  Refused after a detect_loops_group, until this detector's own next detection."""
+        vector is None).  Refused after a detect_loops_group with other detectors, until this detector's own next
+        detection."""
         i = len(self.bow_feats) - 1
         out = np.zeros(max(i, 0), np.float64)
         if i > 0:
@@ -181,7 +151,7 @@ class LoopDetector:
 
 
 def detect_loops_group(detectors, images_per_detector, farthest_per_detector):
-    """detect_loops on each detector with its own images and farthest neighbours, as one batch over all of them: ORB,
+    """detect_loop on each detector's images in order, with their farthest neighbours, as one batch over all of them: ORB,
     the transform and the appends over every frame, one score and one detect launch over all rows and ONE host
     synchronisation.  The detectors must be distinct and share one Vocabulary, and all frames one size and type; a
     detector may have no frame.  Refusals come before any launch.  Returns, per detector, its list of candidate lists."""
