@@ -534,7 +534,7 @@ int sta_op_bow_score(const int32_t* qw, const double* qv, const int32_t* q_len_d
  * sta_graph_tables: the 12 device pointers in that order (pose, depth, conf, intri, conf mean, node_to_view,
  * node_to_connected_view, best node, best mean, edges, measurements, weights). ---- */
 typedef struct StaGraph StaGraph; /* opaque */
-enum { STA_GRAPH_MAX_KEYFRAME_EDGES = 32, STA_GRAPH_FLAG_NOT_SO3 = 1 };
+enum { STA_GRAPH_MAX_KEYFRAME_EDGES = 32, STA_GRAPH_FLAG_NOT_SO3 = 1, STA_GRAPH_MAX_GROUP_KEYFRAMES = 32 };
 int sta_graph_create(int max_nodes, int max_edges, int max_views, int H, int W, StaGraph** out);
 void sta_graph_destroy(StaGraph* g);
 int sta_graph_tables(const StaGraph* g, void** out12);
@@ -556,6 +556,28 @@ int sta_graph_add_keyframe(StaGraph* g, int view, int n, const int64_t* js_host,
                            const int* first_j_host, int node0, int edge0, int H, int W, const float* pose_dev,
                            const float* pose_conf_dev, const float* confs_dev, const float* depths_dev, const float* intri_dev,
                            const float* conf_mean_dev, void* stream);
+/* One keyframe of sta_graph_add_keyframes: sta_graph_add_keyframe's arguments (js / cand / first_j host arrays of n
+ * entries, the device inputs as there). */
+typedef struct StaGraphKeyframe {
+  StaGraph* graph;
+  int view, n, node0, edge0, H, W;
+  const int64_t* js;
+  const int* cand;
+  const int* first_j;
+  const float *pose, *pose_conf, *confs, *depths, *intri, *conf_mean;
+} StaGraphKeyframe;
+/* Insert count keyframes, of one graph or of several, with two launches in all and no host synchronisation: every
+ * table and the flags end as count consecutive sta_graph_add_keyframe calls in table order would leave them, bit for
+ * bit.  A graph's keyframes go in in table order, and each must continue its graph's previous keyframe in the table
+ * (node0 = previous node0 + 2 n, edge0 = previous edge0 + its scale edges + n); a keyframe's scale edge to a node that
+ * an earlier keyframe of the call inserts reads that keyframe's inputs.  scratch (device, 8-byte aligned) holds the
+ * scale reductions' records: sta_graph_add_keyframes_scratch_bytes(kfs, count) bytes, which is 0 for a table the call
+ * would refuse (the reason is then in sta_last_error), so it also checks a table without launching.  Refused before any launch, with every table untouched: any refusal of
+ * sta_graph_add_keyframe for any keyframe, a keyframe that does not continue its graph's previous one, count outside
+ * [1, STA_GRAPH_MAX_GROUP_KEYFRAMES], a null or too small scratch.  sta_graph_add_keyframe is a group of one over
+ * the same kernels, with the graph's own scratch. */
+size_t sta_graph_add_keyframes_scratch_bytes(const StaGraphKeyframe* kfs, int count);
+int sta_graph_add_keyframes(const StaGraphKeyframe* kfs, int count, void* scratch, size_t scratch_bytes, void* stream);
 /* Re-derive node poses after their parents' poses changed: for t = 0 .. count - 1 in order, with (node, parent, edge) =
  * triples_host[3t .. 3t + 2], pose[node] = pose[parent] * measurement[edge], the Sim(3) product sta_graph_add_keyframe
  * uses when it inserts a node.  Listed in insertion order (a keyframe's first j node before its i node), the triples of

@@ -51,6 +51,7 @@ class StaGemmFp8Desc(Structure):
 
 FLOW_MAX_CORNERS = 1000
 GRAPH_MAX_KEYFRAME_EDGES = 32
+GRAPH_MAX_GROUP_KEYFRAMES = 32  # STA_GRAPH_MAX_GROUP_KEYFRAMES: keyframes per sta_graph_add_keyframes call
 GRAPH_FLAG_NOT_SO3 = 1
 ORB_MAX_KEYPOINTS = 4096
 PG_DENSE_MAX_OPT = 3657  # STA_PG_DENSE_MAX_OPT: above it PoseGraphOpt takes the block-sparse route
@@ -70,6 +71,15 @@ class StaPgSparseStep(Structure):
     _fields_ = [
         ("nodes", c_void_p), ("meas", c_void_p), ("weights", c_void_p), ("nodes_out", c_void_p),
         ("damping", ctypes.c_double), ("active", c_int),
+    ]
+
+
+class StaGraphKeyframe(Structure):
+    _fields_ = [
+        ("graph", c_void_p), ("view", c_int), ("n", c_int), ("node0", c_int), ("edge0", c_int), ("H", c_int),
+        ("W", c_int), ("js", POINTER(c_int64)), ("cand", POINTER(c_int)), ("first_j", POINTER(c_int)),
+        ("pose", c_void_p), ("pose_conf", c_void_p), ("confs", c_void_p), ("depths", c_void_p), ("intri", c_void_p),
+        ("conf_mean", c_void_p),
     ]
 
 
@@ -206,6 +216,9 @@ def lib():
     L.sta_graph_flags.argtypes = [vp, POINTER(c_int)]
     L.sta_graph_add_keyframe.argtypes = [vp, i, i, POINTER(c_int64), POINTER(c_int), POINTER(c_int), i, i, i, i, vp, vp, vp, vp,
                                          vp, vp, vp]
+    L.sta_graph_add_keyframes_scratch_bytes.argtypes = [POINTER(StaGraphKeyframe), i]
+    L.sta_graph_add_keyframes_scratch_bytes.restype = ctypes.c_size_t
+    L.sta_graph_add_keyframes.argtypes = [POINTER(StaGraphKeyframe), i, vp, ctypes.c_size_t, vp]
     L.sta_graph_replay_nodes.argtypes = [vp, i, POINTER(c_int), vp]
     L.sta_graph_export_scratch_bytes.argtypes = [i, i]
     L.sta_graph_export_scratch_bytes.restype = ctypes.c_size_t

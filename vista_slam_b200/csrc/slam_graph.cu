@@ -4,12 +4,15 @@
 // save_data_all / get_view (slam.py:299-412).
 //
 // The reference keeps the maps on the host (pose_graph.py:37) and reads a confidence mean back per node (:41) and per
-// scale edge (slam.py:227); here everything stays on the device and a keyframe costs two launches with no host
-// synchronisation:
-//   graph_ingest_kernel  copies the 2n maps of the n kept edges into the node store and runs the 2n - 1 scale-edge
-//                        reductions (pointmap.cuh, the reduction of sta_depth_scale);
-//   graph_link_kernel    finishes the reductions, then one thread walks the edges in the reference's order: node tables,
-//                        best node (strict > against -100), rotation -> quaternion, node poses and edge records.
+// scale edge (slam.py:227); here everything stays on the device and any number of keyframes, of one graph or of many
+// (up to STA_GRAPH_MAX_GROUP_KEYFRAMES), cost two launches with no host synchronisation:
+//   graph_ingest_kernel  copies the 2n maps of each keyframe's n kept edges into the node store and runs its up to
+//                        2n - 1 scale-edge reductions (pointmap.cuh, the reduction of sta_depth_scale);
+//   graph_link_kernel    one block per graph: for each of its keyframes in order, finishes the reductions, then one
+//                        thread walks the edges in the reference's order: node tables, best node (strict > against
+//                        -100), rotation -> quaternion, node poses and edge records.
+// A scale reduction that reads a node inserted earlier in the same launch reads it from that keyframe's inputs, not
+// from the store the copies are writing (map_of).
 #include <string>
 
 #include "../../include/sta_b200.h"
@@ -31,7 +34,7 @@ struct StaGraph {
   int64_t* edges = nullptr;       // [max_edges][2]
   float* meas = nullptr;          // [max_edges][8]
   float* weight = nullptr;        // [max_edges][7]
-  double* partial = nullptr;      // [STA_GRAPH_MAX_KEYFRAME_EDGES * 2][kStatBlocks][kStatVals]
+  double* partial = nullptr;      // [STA_GRAPH_MAX_KEYFRAME_EDGES * 2][kStatBlocks][kStatVals]: one keyframe's records
   int* flags_host = nullptr;      // mapped host word, written by the link kernel
   int* flags_dev = nullptr;       // its device alias
 };
@@ -40,33 +43,57 @@ namespace sta {
 namespace {
 
 constexpr int kMaxKf = STA_GRAPH_MAX_KEYFRAME_EDGES;
+constexpr int kMaxGroup = STA_GRAPH_MAX_GROUP_KEYFRAMES;
+constexpr long long kPartialDoubles = static_cast<long long>(kStatBlocks) * kStatVals;  // one scale edge's records
 
-struct KfArgs {
-  int n, n_scale, node0, edge0, view;
+// One keyframe of a grouped insertion: its graph's tables, its inputs and its place in the launch.
+struct KfDesc {
+  float *pose, *depth, *conf, *intri, *cmean, *best_mean, *meas, *weight;
+  long long *node_view, *node_cview, *best_node, *edges;
+  int* flags;
+  const float* in_pose;    // [*][4][4]
+  const float* pconf;      // [*]
+  const float* confs;      // [2][n][H][W]
+  const float* depths;     // [2][n][H][W]
+  const float* in_intri;   // [n][3][3]
+  const float* in_cmean;   // [2][n]
   long long hw;
-  int cand[kMaxKf];         // candidate row of edge k in pose / pose_conf
-  long long js[kMaxKf];     // view j of edge k
-  int first_j[kMaxKf];      // first node of view j when edge k is inserted, -1 if it has none
-  const float* pose;        // [*][4][4]
-  const float* pconf;       // [*]
-  const float* confs;       // [2][n][H][W]
-  const float* depths;      // [2][n][H][W]
-  const float* intri;       // [n][3][3]
-  const float* cmean;       // [2][n]
+  int gid;                 // index of its graph among the launch's graphs
+  int n, n_scale, node0, edge0, view;
+  int row0;                // first ingest row (grid y) of the keyframe
+  int s0;                  // first scale-edge record set of the keyframe in the scratch
+  int cand[kMaxKf];        // candidate row of edge k in pose / pose_conf
+  int js[kMaxKf];          // view j of edge k
+  int first_j[kMaxKf];     // first node of view j when edge k is inserted, -1 if it has none
 };
 
-// Map of node `slot`: the keyframe's own nodes node0 + 2k + r are row r of edge k in the inputs, older ones are in
-// the store.
-__device__ __forceinline__ const float* map_of(const KfArgs& a, const float* store, const float* in, int slot) {
-  if (slot >= a.node0) {
-    const int d = slot - a.node0;
-    return in + (static_cast<long long>(d & 1) * a.n + (d >> 1)) * a.hw;
+// The keyframes of one launch pair, in table order; the kernels are instantiated for groups of one and of up to
+// kMaxGroup, so a single keyframe does not pass the large table.  Passed as a __grid_constant__ kernel parameter:
+// no copy of the table precedes the launches.
+template <int N>
+struct KfGroup {
+  int count, graphs;
+  KfDesc k[N];
+};
+static_assert(sizeof(KfGroup<kMaxGroup>) + 64 <= 32764, "the keyframe table must fit the kernel-parameter space");
+
+// Map of node `slot` of keyframe t's graph: a node inserted by keyframe t or by an earlier keyframe of the same graph in
+// this launch is row r of edge k in that keyframe's inputs (slot = node0 + 2k + r); older ones are in the store.  So
+// the scale reductions never read a store slot that this launch's copies write.
+template <int N>
+__device__ __forceinline__ const float* map_of(const KfGroup<N>& p, int t, bool depth, int slot) {
+  const KfDesc& a = p.k[t];
+  for (int u = t; u >= 0; --u) {
+    const KfDesc& b = p.k[u];
+    if (b.gid != a.gid || slot < b.node0 || slot >= b.node0 + 2 * b.n) continue;
+    const int d = slot - b.node0;
+    return (depth ? b.depths : b.confs) + (static_cast<long long>(d & 1) * b.n + (d >> 1)) * b.hw;
   }
-  return store + static_cast<long long>(slot) * a.hw;
+  return (depth ? a.depth : a.conf) + static_cast<long long>(slot) * a.hw;
 }
 
-// Scale edge s of the keyframe, in edge order: (new node, first node of its view).
-__device__ void scale_edge(const KfArgs& a, int s, int* nnew, int* nother) {
+// Scale edge s of a keyframe, in edge order: (new node, first node of its view).
+__device__ void scale_edge(const KfDesc& a, int s, int* nnew, int* nother) {
   int c = 0;
   for (int k = 0; k < a.n; ++k) {
     if (k > 0) {
@@ -78,29 +105,32 @@ __device__ void scale_edge(const KfArgs& a, int s, int* nnew, int* nother) {
   }
 }
 
-// grid (kStatBlocks, n_scale + 2n), 256 threads
-__global__ void __launch_bounds__(256) graph_ingest_kernel(StaGraph g, KfArgs a) {
-  const int y = blockIdx.y;
+// grid (kStatBlocks, sum over keyframes of n_scale + 2n), 256 threads: row y of keyframe t is its scale edge y (y <
+// n_scale, records into the scratch) or the copy of its node node0 + y - n_scale into the store
+template <int N>
+__global__ void __launch_bounds__(256) graph_ingest_kernel(const __grid_constant__ KfGroup<N> p, double* partial) {
+  int t = 0;
+  while (t + 1 < p.count && static_cast<int>(blockIdx.y) >= p.k[t + 1].row0) ++t;
+  const KfDesc& a = p.k[t];
+  const int y = blockIdx.y - a.row0;
   if (y < a.n_scale) {
     int nn = 0, no = 0;
     scale_edge(a, y, &nn, &no);
     // estimate_scale_with_depth_and_confidence(depth, depth_other, conf, conf_other), slam.py:224
-    scale_partial(map_of(a, g.depth, a.depths, nn), map_of(a, g.depth, a.depths, no), map_of(a, g.conf, a.confs, nn),
-                  map_of(a, g.conf, a.confs, no), a.hw, blockIdx.x,
-                  g.partial + (static_cast<long long>(y) * kStatBlocks + blockIdx.x) * kStatVals);
+    scale_partial(map_of(p, t, true, nn), map_of(p, t, true, no), map_of(p, t, false, nn), map_of(p, t, false, no), a.hw,
+                  blockIdx.x, partial + (a.s0 + y) * kPartialDoubles + static_cast<long long>(blockIdx.x) * kStatVals);
     return;
   }
   const int slot = a.node0 + (y - a.n_scale);
-  const float* d = map_of(a, g.depth, a.depths, slot);
-  const float* c = map_of(a, g.conf, a.confs, slot);
-  float* dd = g.depth + static_cast<long long>(slot) * a.hw;
-  float* cd = g.conf + static_cast<long long>(slot) * a.hw;
+  const int d = y - a.n_scale;
+  const long long src = (static_cast<long long>(d & 1) * a.n + (d >> 1)) * a.hw;
+  float* dd = a.depth + static_cast<long long>(slot) * a.hw;
+  float* cd = a.conf + static_cast<long long>(slot) * a.hw;
   for (long long i = static_cast<long long>(blockIdx.x) * 256 + threadIdx.x; i < a.hw; i += kStatBlocks * 256) {
-    dd[i] = d[i];
-    cd[i] = c[i];
+    dd[i] = a.depths[src + i];
+    cd[i] = a.confs[src + i];
   }
-  if (blockIdx.x == 0 && threadIdx.x < 9)
-    g.intri[slot * 9 + threadIdx.x] = a.intri[((slot - a.node0) >> 1) * 9 + threadIdx.x];
+  if (blockIdx.x == 0 && threadIdx.x < 9) a.intri[slot * 9 + threadIdx.x] = a.in_intri[(d >> 1) * 9 + threadIdx.x];
 }
 
 // Sim(3) a * b in the [t | q | s] layout; the quaternion is kept with w >= 0.
@@ -160,52 +190,60 @@ __device__ bool rot_to_quat(const float* M, float* q) {
   return ok;
 }
 
-__device__ void put_edge(const StaGraph& g, int e, long long ni, long long nj, const float* m8, const float* w7) {
+__device__ void put_edge(const KfDesc& g, int e, long long ni, long long nj, const float* m8, const float* w7) {
   g.edges[2 * e] = ni;
   g.edges[2 * e + 1] = nj;
   for (int i = 0; i < 8; ++i) g.meas[e * 8 + i] = m8[i];
   for (int i = 0; i < 7; ++i) g.weight[e * 7 + i] = w7[i];
 }
 
-// one block of 64 threads
-__global__ void graph_link_kernel(StaGraph g, KfArgs a) {
+// grid (graphs), 64 threads: block b walks the keyframes of graph b in table order -- each keyframe's reductions
+// finished, then one thread walks its edges in the reference's order: node tables, best node (strict > against -100),
+// rotation -> quaternion, node poses and edge records
+template <int N>
+__global__ void __launch_bounds__(64) graph_link_kernel(const __grid_constant__ KfGroup<N> p, const double* partial) {
   __shared__ float sc[2 * kMaxKf][2];
-  if (threadIdx.x < a.n_scale)
-    scale_finalize(g.partial + static_cast<long long>(threadIdx.x) * kStatBlocks * kStatVals, a.hw, sc[threadIdx.x]);
-  __syncthreads();
-  if (threadIdx.x != 0) return;
-  int e = a.edge0, s = 0;
-  for (int k = 0; k < a.n; ++k) {
-    for (int r = 0; r < 2; ++r) {  // add_node(i), its scale edge, add_node(j), its scale edge (slam.py:210-232)
-      const int slot = a.node0 + 2 * k + r;
-      const long long v = r ? a.js[k] : a.view;
-      g.node_view[slot] = v;
-      g.node_cview[slot] = r ? a.view : a.js[k];
-      const float m = a.cmean[r * a.n + k];
-      g.cmean[slot] = m;
-      if (m > g.best_mean[v]) {  // pose_graph.py:42: strict, so the first node wins a tie
-        g.best_mean[v] = m;
-        g.best_node[v] = slot;
-      }
-      const int other = r ? a.first_j[k] : (k > 0 ? a.node0 : -1);
-      if (other >= 0) {
-        const float sim3[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 1.f, sc[s][0]};
-        const float w[7] = {2.f, 2.f, 2.f, 2.f, 2.f, 2.f, sc[s][1]};  // PoseGraphEdges.id_pose_conf = 2.0
-        ++s;
-        put_edge(g, e++, slot, other, sim3, w);
-        sim3_mul(g.pose + other * 8, sim3, g.pose + slot * 8);
+  for (int t = 0; t < p.count; ++t) {
+    const KfDesc& a = p.k[t];
+    if (a.gid != static_cast<int>(blockIdx.x)) continue;
+    if (threadIdx.x < a.n_scale) scale_finalize(partial + (a.s0 + threadIdx.x) * kPartialDoubles, a.hw, sc[threadIdx.x]);
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      int e = a.edge0, s = 0;
+      for (int k = 0; k < a.n; ++k) {
+        for (int r = 0; r < 2; ++r) {  // add_node(i), its scale edge, add_node(j), its scale edge (slam.py:210-232)
+          const int slot = a.node0 + 2 * k + r;
+          const long long v = r ? a.js[k] : a.view;
+          a.node_view[slot] = v;
+          a.node_cview[slot] = r ? a.view : a.js[k];
+          const float m = a.in_cmean[r * a.n + k];
+          a.cmean[slot] = m;
+          if (m > a.best_mean[v]) {  // pose_graph.py:42: strict, so the first node wins a tie
+            a.best_mean[v] = m;
+            a.best_node[v] = slot;
+          }
+          const int other = r ? a.first_j[k] : (k > 0 ? a.node0 : -1);
+          if (other >= 0) {
+            const float sim3[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 1.f, sc[s][0]};
+            const float w[7] = {2.f, 2.f, 2.f, 2.f, 2.f, 2.f, sc[s][1]};  // PoseGraphEdges.id_pose_conf = 2.0
+            ++s;
+            put_edge(a, e++, slot, other, sim3, w);
+            sim3_mul(a.pose + other * 8, sim3, a.pose + slot * 8);
+          }
+        }
+        const float* M = a.in_pose + a.cand[k] * 16;
+        float sim3[8] = {M[3], M[7], M[11], 0.f, 0.f, 0.f, 1.f, 1.f};
+        if (!rot_to_quat(M, sim3 + 3)) *reinterpret_cast<volatile int*>(a.flags) |= STA_GRAPH_FLAG_NOT_SO3;
+        const int ni = a.node0 + 2 * k, nj = ni + 1;
+        if (k == 0) sim3_mul(a.pose + nj * 8, sim3, a.pose + ni * 8);  // view i is new at its first node (slam.py:234-236)
+        const float c = a.pconf[a.cand[k]];
+        const float w[7] = {c, c, c, c, c, c, c};
+        put_edge(a, e++, ni, nj, sim3, w);
       }
     }
-    const float* M = a.pose + a.cand[k] * 16;
-    float sim3[8] = {M[3], M[7], M[11], 0.f, 0.f, 0.f, 1.f, 1.f};
-    if (!rot_to_quat(M, sim3 + 3)) *reinterpret_cast<volatile int*>(g.flags_dev) |= STA_GRAPH_FLAG_NOT_SO3;
-    const int ni = a.node0 + 2 * k, nj = ni + 1;
-    if (k == 0) sim3_mul(g.pose + nj * 8, sim3, g.pose + ni * 8);  // view i is new at its first node (slam.py:234-236)
-    const float c = a.pconf[a.cand[k]];
-    const float w[7] = {c, c, c, c, c, c, c};
-    put_edge(g, e++, ni, nj, sim3, w);
+    __syncthreads();  // sc is reused by the graph's next keyframe
   }
-  __threadfence_system();
+  if (threadIdx.x == 0) __threadfence_system();
 }
 
 // Triples (node, parent, edge) of one replay launch: 256 x 12 bytes keeps the parameters under 4 KB.
@@ -400,49 +438,134 @@ int sta_graph_flags(const StaGraph* g, int* flags_out) {
   return 0;
 }
 
+}  // extern "C"
+
+namespace {
+
+// The n_scale of a keyframe: a scale edge for every edge k > 0 (to view i's first node) and for every j with a node.
+int scale_edges_of(const StaGraphKeyframe& f) {
+  int c = 0;
+  for (int k = 0; k < f.n; ++k) c += (k > 0) + (f.first_j[k] >= 0);
+  return c;
+}
+
+// Every refusal of sta_graph_add_keyframes, before any launch; fills the table of the launch pair.
+template <int N>
+int fill_group(const StaGraphKeyframe* kfs, int count, KfGroup<N>* p, int* rows, int* records) {
+  STA_REQUIRE(kfs != nullptr, "null keyframe table");
+  STA_REQUIRE(count >= 1 && count <= N, "1 to STA_GRAPH_MAX_GROUP_KEYFRAMES keyframes per call");
+  const StaGraph* graphs[kMaxGroup];
+  int last[kMaxGroup];  // the graph's previous keyframe in the table
+  p->count = count;
+  p->graphs = 0;
+  *rows = 0;
+  *records = 0;
+  for (int t = 0; t < count; ++t) {
+    const StaGraphKeyframe& f = kfs[t];
+    StaGraph* g = f.graph;
+    const int n = f.n;
+    STA_REQUIRE(g != nullptr && f.js && f.cand && f.first_j, "null argument");
+    STA_REQUIRE(n >= 1 && n <= kMaxKf, "1 to STA_GRAPH_MAX_KEYFRAME_EDGES kept edges per keyframe");
+    STA_REQUIRE(f.H == g->H && f.W == g->W, "map size differs from the graph's");
+    STA_REQUIRE(f.pose && f.pose_conf && f.confs && f.depths && f.intri && f.conf_mean, "null device input");
+    STA_REQUIRE(on_device(f.pose) && on_device(f.pose_conf) && on_device(f.confs) && on_device(f.depths) &&
+                    on_device(f.intri) && on_device(f.conf_mean),
+                "inputs must be device memory");
+    STA_REQUIRE(f.view >= 0 && f.view < g->max_views, "view index out of range");
+    for (int k = 0; k < n; ++k) {
+      STA_REQUIRE(f.js[k] >= 0 && f.js[k] < f.view, "j must be an earlier view");
+      STA_REQUIRE(f.cand[k] >= 0, "negative candidate index");
+      STA_REQUIRE(f.first_j[k] >= -1 && f.first_j[k] < f.node0 + 2 * k, "first node of view j is not in the graph");
+    }
+    const int n_scale = scale_edges_of(f);
+    STA_REQUIRE(f.node0 >= 0 && static_cast<long long>(f.node0) + 2 * n <= g->max_nodes, "node capacity exceeded");
+    STA_REQUIRE(f.edge0 >= 0 && static_cast<long long>(f.edge0) + n_scale + n <= g->max_edges, "edge capacity exceeded");
+    int gid = 0;
+    while (gid < p->graphs && graphs[gid] != g) ++gid;
+    if (gid == p->graphs) {
+      graphs[p->graphs++] = g;
+    } else {
+      const StaGraphKeyframe& q = kfs[last[gid]];
+      STA_REQUIRE(f.node0 == q.node0 + 2 * q.n && f.edge0 == q.edge0 + scale_edges_of(q) + q.n,
+                  "a keyframe's node0 / edge0 do not continue its graph's previous keyframe in the call");
+    }
+    last[gid] = t;
+    KfDesc& a = p->k[t];
+    a = KfDesc{};
+    a.pose = g->pose; a.depth = g->depth; a.conf = g->conf; a.intri = g->intri; a.cmean = g->cmean;
+    a.best_mean = g->best_mean; a.meas = g->meas; a.weight = g->weight;
+    a.node_view = reinterpret_cast<long long*>(g->node_view);
+    a.node_cview = reinterpret_cast<long long*>(g->node_cview);
+    a.best_node = reinterpret_cast<long long*>(g->best_node);
+    a.edges = reinterpret_cast<long long*>(g->edges);
+    a.flags = g->flags_dev;
+    a.in_pose = f.pose; a.pconf = f.pose_conf; a.confs = f.confs; a.depths = f.depths; a.in_intri = f.intri;
+    a.in_cmean = f.conf_mean;
+    a.hw = static_cast<long long>(f.H) * f.W;
+    a.gid = gid;
+    a.n = n; a.n_scale = n_scale; a.node0 = f.node0; a.edge0 = f.edge0; a.view = f.view;
+    a.row0 = *rows;
+    a.s0 = *records;
+    for (int k = 0; k < n; ++k) {
+      a.cand[k] = f.cand[k];
+      a.js[k] = static_cast<int>(f.js[k]);
+      a.first_j[k] = f.first_j[k];
+    }
+    *rows += n_scale + 2 * n;
+    *records += n_scale;
+  }
+  return 0;
+}
+
+template <int N>
+int launch_group(const StaGraphKeyframe* kfs, int count, double* scratch, size_t scratch_bytes, bool own_partial,
+                 cudaStream_t st) {
+  KfGroup<N> p;
+  int rows = 0, records = 0;
+  if (int rc = fill_group(kfs, count, &p, &rows, &records)) return rc;
+  if (own_partial) scratch = kfs[0].graph->partial;
+  STA_REQUIRE(scratch != nullptr, "null scratch");
+  STA_REQUIRE((reinterpret_cast<uintptr_t>(scratch) & 7) == 0, "scratch must be 8-byte aligned");
+  STA_REQUIRE(own_partial || scratch_bytes >= sizeof(double) * kPartialDoubles * (records > 0 ? records : 1),
+              "scratch smaller than sta_graph_add_keyframes_scratch_bytes");
+  graph_ingest_kernel<N><<<dim3(kStatBlocks, rows), 256, 0, st>>>(p, scratch);
+  STA_CHECK_CUDA(cudaGetLastError());
+  graph_link_kernel<N><<<p.graphs, 64, 0, st>>>(p, scratch);
+  STA_CHECK_CUDA(cudaGetLastError());
+  return 0;
+}
+
+}  // namespace
+
+extern "C" {
+
 int sta_graph_add_keyframe(StaGraph* g, int view, int n, const int64_t* js_host, const int* cand_host,
                            const int* first_j_host, int node0, int edge0, int H, int W, const float* pose_dev,
                            const float* pose_conf_dev, const float* confs_dev, const float* depths_dev, const float* intri_dev,
                            const float* conf_mean_dev, void* stream) {
-  STA_REQUIRE(g != nullptr && js_host && cand_host && first_j_host, "null argument");
-  STA_REQUIRE(n >= 1 && n <= kMaxKf, "1 to STA_GRAPH_MAX_KEYFRAME_EDGES kept edges per keyframe");
-  STA_REQUIRE(H == g->H && W == g->W, "map size differs from the graph's");
-  STA_REQUIRE(pose_dev && pose_conf_dev && confs_dev && depths_dev && intri_dev && conf_mean_dev, "null device input");
-  STA_REQUIRE(on_device(pose_dev) && on_device(pose_conf_dev) && on_device(confs_dev) && on_device(depths_dev) &&
-                  on_device(intri_dev) && on_device(conf_mean_dev),
-              "inputs must be device memory");
-  STA_REQUIRE(view >= 0 && view < g->max_views, "view index out of range");
-  KfArgs a = {};
-  a.n = n;
-  a.view = view;
-  a.node0 = node0;
-  a.edge0 = edge0;
-  a.hw = static_cast<long long>(H) * W;
-  int n_scale = 0;
-  for (int k = 0; k < n; ++k) {
-    STA_REQUIRE(js_host[k] >= 0 && js_host[k] < view, "j must be an earlier view");
-    STA_REQUIRE(cand_host[k] >= 0, "negative candidate index");
-    STA_REQUIRE(first_j_host[k] >= -1 && first_j_host[k] < node0 + 2 * k, "first node of view j is not in the graph");
-    a.js[k] = js_host[k];
-    a.cand[k] = cand_host[k];
-    a.first_j[k] = first_j_host[k];
-    n_scale += (k > 0) + (first_j_host[k] >= 0);
+  STA_REQUIRE(g != nullptr, "null argument");
+  const StaGraphKeyframe f = {g, view, n, node0, edge0, H, W, js_host, cand_host, first_j_host,
+                              pose_dev, pose_conf_dev, confs_dev, depths_dev, intri_dev, conf_mean_dev};
+  return launch_group<1>(&f, 1, nullptr, 0, true, static_cast<cudaStream_t>(stream));
+}
+
+size_t sta_graph_add_keyframes_scratch_bytes(const StaGraphKeyframe* kfs, int count) {
+  int rows = 0, records = 0, rc = 0;
+  if (count == 1) {
+    KfGroup<1> p;
+    rc = fill_group(kfs, count, &p, &rows, &records);
+  } else {
+    KfGroup<kMaxGroup> p;
+    rc = fill_group(kfs, count, &p, &rows, &records);
   }
-  a.n_scale = n_scale;
-  STA_REQUIRE(node0 >= 0 && static_cast<long long>(node0) + 2 * n <= g->max_nodes, "node capacity exceeded");
-  STA_REQUIRE(edge0 >= 0 && static_cast<long long>(edge0) + n_scale + n <= g->max_edges, "edge capacity exceeded");
-  a.pose = pose_dev;
-  a.pconf = pose_conf_dev;
-  a.confs = confs_dev;
-  a.depths = depths_dev;
-  a.intri = intri_dev;
-  a.cmean = conf_mean_dev;
+  return rc ? 0 : sizeof(double) * kPartialDoubles * (records > 0 ? records : 1);
+}
+
+int sta_graph_add_keyframes(const StaGraphKeyframe* kfs, int count, void* scratch, size_t scratch_bytes, void* stream) {
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  graph_ingest_kernel<<<dim3(kStatBlocks, n_scale + 2 * n), 256, 0, st>>>(*g, a);
-  STA_CHECK_CUDA(cudaGetLastError());
-  graph_link_kernel<<<1, 64, 0, st>>>(*g, a);
-  STA_CHECK_CUDA(cudaGetLastError());
-  return 0;
+  double* s = static_cast<double*>(scratch);
+  if (count == 1) return launch_group<1>(kfs, count, s, scratch_bytes, false, st);
+  return launch_group<kMaxGroup>(kfs, count, s, scratch_bytes, false, st);
 }
 
 int sta_graph_replay_nodes(StaGraph* g, int count, const int* triples_host, void* stream) {

@@ -231,8 +231,19 @@ class PoseGraphOpt:
     def start(self, edges, poses, weight, steps=20, patience=3, decreasing=1e-4, radius=1e4):
         """optimize() without waiting for it: returns a PoseGraphRun that steps this graph on a side stream, one LM
         iteration per poll().  Same kernels, dampings and accept / plateau decisions as optimize(), so the nodes and the
-        loss history it ends with are optimize()'s, bit for bit.  The row-count refusal of optimize_group applies."""
-        return PoseGraphRun(self, edges, poses, weight, steps, patience, decreasing, radius)
+        loss history it ends with are optimize()'s, bit for bit.  The row-count refusal of optimize_group applies.
+        A group of one (start_group)."""
+        return PoseGraphRun([self], [edges], [poses], [weight], steps, patience, decreasing, radius, single=True)
+
+    @staticmethod
+    @torch.no_grad()
+    def start_group(graphs, edges, poses, weights, steps=20, patience=3, decreasing=1e-4, radius=1e4):
+        """optimize_group() without waiting for it: returns a PoseGraphRun that steps every graph on one side stream,
+        one LM iteration of the group per poll(), with one _Group launch and one pinned copy of the info rows per
+        iteration.  Each graph ends with optimize_group's nodes and loss history, bit for bit, dense, block-sparse or
+        mixed.  The run's losses are the per-graph histories; graph_losses(k) and graph_done(k) report graph k while it
+        runs.  optimize_group's refusals apply, before any launch."""
+        return PoseGraphRun(graphs, edges, poses, weights, steps, patience, decreasing, radius)
 
 
 class _Group:
@@ -268,32 +279,41 @@ class _Group:
 
 
 class PoseGraphRun:
-    """A PoseGraphOpt.optimize() in the background (PoseGraphOpt.start): each LM iteration is enqueued on a non-blocking
-    side stream, its info row copied into pinned host memory and an event recorded.  poll() never waits: when the
-    event has completed it takes the iteration's accept / reject decision and enqueues the next one.  wait() waits on
-    that event until the run is done.
+    """PoseGraphOpt.optimize() (start) or optimize_group() (start_group) in the background: each LM iteration of the
+    group is enqueued on a non-blocking side stream, its info rows copied into pinned host memory and an event recorded.
+    poll() never waits: when the event has completed it takes the iteration's accept / reject decisions and enqueues
+    the next one.  wait() waits on that event until the run is done.
 
     Streams: the side stream starts after the work already queued on the stream that was current at start() (the
-    "main" stream, which holds the PoseGraphOpt's snapshot of the nodes); the main-stream tensors the run reads are
-    recorded on the side stream.  Once done, the main stream is ordered after the run, so graph.nodes can be read
-    there.  A block-sparse plan is built in start(), on the main stream.  Nothing here synchronises the device."""
+    "main" stream, which holds the PoseGraphOpts' snapshots of the nodes); the main-stream tensors the run reads are
+    recorded on the side stream.  Once done, the main stream is ordered after the run, so every graph's nodes can be
+    read there.  Block-sparse plans are built at the start, on the main stream.  Nothing here synchronises the
+    device."""
 
-    def __init__(self, graph, edges, poses, weight, steps, patience, decreasing, radius):
-        _check_group([graph], [edges], [poses], [weight])
-        dev = graph.nodes.device
-        self.graph = graph
+    def __init__(self, graphs, edges, poses, weights, steps, patience, decreasing, radius, single=False):
+        graphs, edges, poses, weights = list(graphs), list(edges), list(poses), list(weights)
+        _check_group(graphs, edges, poses, weights)
+        if not graphs:
+            raise ValueError("a background run needs at least one graph")
+        dev = graphs[0].nodes.device
+        self.graphs, self._single = graphs, single
         self.main = torch.cuda.current_stream(dev)
-        if graph.sparse:
-            graph.plan(edges)  # its one edge-table copy waits only on the main stream's queued work
+        for g, e in zip(graphs, edges):
+            if g.sparse:
+                g.plan(e)  # its one edge-table copy waits only on the main stream's queued work
         self.stream = torch.cuda.Stream(dev)
         self.stream.wait_stream(self.main)
-        for t in (graph.nodes, graph.idxs_opt, edges, poses, weight):
-            t.record_stream(self.stream)  # no-op for memory the caching allocator does not own (the SLAM tables)
-        self.state = _LMState(1, steps, patience, decreasing, radius)
-        self.pinned = torch.empty(1, 4, dtype=torch.float64, pin_memory=True)
+        for g, e, p, w in zip(graphs, edges, poses, weights):
+            for t in (g.nodes, g.idxs_opt, e, p, w):
+                t.record_stream(self.stream)  # no-op for memory the caching allocator does not own (the SLAM tables)
+        self.state = _LMState(len(graphs), steps, patience, decreasing, radius)
+        self.pinned = torch.empty(len(graphs), 4, dtype=torch.float64, pin_memory=True)
         self.event = torch.cuda.Event()
         with torch.cuda.stream(self.stream):
-            self.group = _Group([graph], [edges], [poses], [weight])
+            self.group = _Group(graphs, edges, poses, weights)
+        self.order = self.group.order  # the state machine runs over the graphs in this order, as optimize_group's
+        self._at = {k: t for t, k in enumerate(self.order)}
+        self._ordered = [graphs[k] for k in self.order]
         self._launch()
 
     @property
@@ -302,13 +322,25 @@ class PoseGraphRun:
 
     @property
     def losses(self):
-        """The loss history so far: optimize()'s return value once done."""
-        return self.state.losses[0]
+        """The loss histories so far: once done, optimize()'s return value for a run of start(), optimize_group()'s
+        for a run of start_group()."""
+        if self._single:
+            return self.state.losses[0]
+        return [self.graph_losses(k) for k in range(len(self.graphs))]
+
+    def graph_losses(self, k):
+        """Graph k's loss history so far."""
+        return self.state.losses[self._at[k]]
+
+    def graph_done(self, k):
+        """Whether graph k has left the group (its nodes are final once the run is done)."""
+        return self.state.done or self._at[k] not in self.state.active
 
     def _launch(self):
         if self.state.done:
             self.main.wait_stream(self.stream)
-            self.graph.nodes.record_stream(self.main)
+            for g in self.graphs:
+                g.nodes.record_stream(self.main)
             self.group = self._pending = None
             return
         with torch.cuda.stream(self.stream):
@@ -325,12 +357,12 @@ class PoseGraphRun:
         if not self.event.query():
             return False
         outs, rows, at = self._pending
-        self.state.advance([self.graph], _Group.results(self.pinned[:rows], outs, at))
+        self.state.advance(self._ordered, _Group.results(self.pinned[:rows], outs, at))
         self._launch()
         return self.state.done
 
     def wait(self):
-        """Run to the end, waiting on each iteration's event.  Returns the loss history."""
+        """Run to the end, waiting on each iteration's event.  Returns the loss histories (losses)."""
         while not self.poll():
             self.event.synchronize()
         return self.losses

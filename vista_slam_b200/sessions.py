@@ -10,12 +10,14 @@ keyframes of every named session through one batched frontend pass:
   * the gated edge regression in chunks of at most 16 edges that mix sessions, one read-back per chunk
     (keyframe.regress_keyframes_gated_group).
 
-Graph insertion and PGO stay per session, in the order step_many would run them.  `optimize(ks)` runs the PGO of the
-named sessions now, together: one PoseGraphOpt.optimize_group, whose LM iterations step every session's graph with one
-launch sequence and one read-back.  With pgo_every beyond the sequence length, an evaluation over a scene list ends with
-one `optimize(range(len(scenes)))`, and a live server runs `optimize` on the sessions that are due.  A call leaves every session as
-`for k in sorted(values): sessions[k].step_many(values[k], force_pgo=k in force_pgo, ...)` would: the graph tables,
-host bookkeeping, loop candidates, gate decisions, PGO calls, written files and returned flags.  Frontend floats may
+Graph insertion runs once per edge chunk for all sessions (one sta_graph_add_keyframes), and step's PGOs per session,
+in the order step_many would run them.  `optimize(ks)` runs the PGO of the named sessions now, together: one
+PoseGraphOpt.optimize_group, whose LM iterations step every session's graph with one launch sequence and one
+read-back; `optimize(ks, background=True)` starts the same group on a side stream and returns (INTEGRATION.md §5).
+With pgo_every beyond the sequence length, an evaluation over a scene list ends with one
+`optimize(range(len(scenes)))`, and a live server runs `optimize` on the sessions that are due.  A call leaves every
+session as `for k in sorted(values): sessions[k].step_many(values[k], force_pgo=k in force_pgo, ...)` would: the
+graph tables, host bookkeeping, loop candidates, gate decisions, PGO calls, written files and returned flags.  Frontend floats may
 differ from that loop within rounding, as step_many's differ from step's, because batch sizes change the GEMMs' split-K.
 
 Timing: each session's time_dict gets its share of the batched phases.  The wall time of the encoder calls and of the
@@ -33,12 +35,64 @@ import torch
 from .keyframe import KeyframeFrontend, add_views_group, regress_keyframes_gated_group
 from .loop_detector import Vocabulary, detect_loops_group
 from .pose_graph import PoseGraphOpt
-from .slam import OnlineSLAM
+from .slam import OnlineSLAM, insert_keyframes
 
 
 def _share(sessions, key, seconds):
     for s in sessions:
         s.time_dict[key] += seconds / len(sessions)
+
+
+class _Batch:
+    """PGO problems (PoseGraphOpt, (edges, measurements, weights)) of several sessions, started together as one
+    PoseGraphOpt.start_group run."""
+
+    def __init__(self):
+        self.problems, self.run = [], None
+
+    def start(self):
+        if self.run is None:
+            graphs, args = [g for g, _ in self.problems], [a for _, a in self.problems]
+            self.run = PoseGraphOpt.start_group(graphs, *[[a[i] for a in args] for i in range(3)])
+        return self.run
+
+
+class _SessionRun:
+    """A session's handle on a shared background run (OnlineSLAM._pgo_run[0]): poll() is True once the whole run is
+    done and never waits or starts it; wait() starts the run if it has not started, then waits for it."""
+
+    def __init__(self, batch):
+        self.batch = batch
+
+    @property
+    def stream(self):
+        return self.batch.start().stream
+
+    def poll(self):
+        return self.batch.run is not None and self.batch.run.poll()
+
+    def wait(self):
+        self.batch.start().wait()
+
+
+class _CallGroup:
+    """The background PGOs that fall due during one SLAMSessions.step call: captured at their keyframes (add), then
+    started as one run at the end of the call (start).  Waiting on a captured run starts the group at that point;
+    PGOs captured after that go into a new group."""
+
+    def __init__(self):
+        self.batches = [_Batch()]
+
+    def add(self, graph, args):
+        if self.batches[-1].run is not None:
+            self.batches.append(_Batch())
+        self.batches[-1].problems.append((graph, args))
+        return _SessionRun(self.batches[-1])
+
+    def start(self):
+        for b in self.batches:
+            if b.problems:
+                b.start()
 
 
 class SLAMSessions:
@@ -109,9 +163,11 @@ class SLAMSessions:
         raises ValueError by the end of the call.
 
         Host synchronisations: one for the loop candidates of all sessions, one per edge chunk, one per PGO iteration,
-        and one at the end of the call unless every session's flag has been read since its last graph launch.  A
-        session with pgo_background runs its PGOs on their own side streams (OnlineSLAM.step_many); every session with
-        a pending one is polled after each keyframe of the call."""
+        and one at the end of the call unless every session's flag has been read since its last graph launch.  The
+        kept edges of each edge chunk, of every session, go into the graphs with one sta_graph_add_keyframes.  The
+        PGOs of sessions with pgo_background that fall due during the call are captured at their keyframes and started
+        as one PoseGraphOpt.start_group run at the end of the call (a session due again within the call waits for its
+        run, which starts the group then); every session with a pending PGO is polled after each keyframe."""
         calls = self._calls(values)
         force = {self._index(k) for k in force_pgo}
         flags = {k: [] for k, _ in calls}
@@ -158,30 +214,38 @@ class SLAMSessions:
             for t in chunk:
                 part[t] = members
 
+        chunk_ends = {chunk[-1] for chunk in KeyframeFrontend.edge_chunks([(i, js) for _, i, js in items])}
+        group = _CallGroup()
         checked = [True] * len(calls)
         results = iter(self._regress_keyframes(items))
-        for t, (s, i, js) in enumerate(items):
-            c = owner[t]
-            k, vs = calls[c]
-            m = i - i0[c]
-            dec_start = time.time()
-            res = next(results)  # the first keyframe of an edge chunk runs the chunk: read-back of its gate
-            dt = time.time() - dec_start
-            _share(part[t], "decoder", dt)
-            _share(part[t], "graph_construction", dt)
-            graph_start = time.time()
-            s._check_flags()
-            s._register_keyframe(vs[m], i, js, res)
-            if js:
-                checked[c] = checked[c] and not res[1]
-            for p in self.sessions:
-                if p.pgo_pending:
-                    p._pgo_poll()
-            s.time_dict["graph_construction"] += time.time() - graph_start
-            folder = output_folders.get(k) if output_folders else None
-            flags[k].append(s._pgo_if_due(k in force and m == len(vs) - 1, log_intermediate_results, folder))
-            if flags[k][-1] and not s.pgo_background:
-                checked[c] = s.num_nodes > 0 and s.num_edges > 0
+        try:
+            for t, (s, i, js) in enumerate(items):
+                c = owner[t]
+                k, vs = calls[c]
+                m = i - i0[c]
+                dec_start = time.time()
+                res = next(results)  # the first keyframe of an edge chunk runs the chunk: read-back of its gate
+                dt = time.time() - dec_start
+                _share(part[t], "decoder", dt)
+                _share(part[t], "graph_construction", dt)
+                graph_start = time.time()
+                s._check_flags()
+                s._register_keyframe(vs[m], i, js, res)
+                if js:
+                    checked[c] = checked[c] and not res[1]
+                if t in chunk_ends:  # the chunk's keyframes, of every session, go in with one sta_graph_add_keyframes
+                    insert_keyframes(sess)
+                for p in self.sessions:
+                    if p.pgo_pending:
+                        p._pgo_poll()
+                s.time_dict["graph_construction"] += time.time() - graph_start
+                folder = output_folders.get(k) if output_folders else None
+                flags[k].append(s._pgo_if_due(k in force and m == len(vs) - 1, log_intermediate_results, folder, group))
+                if flags[k][-1] and not s.pgo_background:
+                    checked[c] = s.num_nodes > 0 and s.num_edges > 0
+        finally:  # an exception mid-chunk still leaves every graph as its host bookkeeping says
+            insert_keyframes(sess)
+            group.start()  # the background PGOs that fell due in the call, as one run
         if not all(checked):
             torch.cuda.current_stream().synchronize()
             for s, ok in zip(sess, checked):
@@ -189,14 +253,20 @@ class SLAMSessions:
                     s._check_flags()
         return flags
 
-    def optimize(self, ks):
+    def optimize(self, ks, background=False):
         """Optimise the pose graphs of sessions ks now, together.  Leaves each session as sessions[k].pose_graph_optimize()
         would: the same optimised node set (the window and the loop-related views), the same poses bit for bit,
         loop_related_views cleared and the same messages (every session's opening messages, then the optimisation,
         then every session's closing message); a session without nodes or edges only prints them.  An unknown or
         repeated index raises ValueError before anything runs.  Host synchronisations: one per LM iteration of the
         group, whichever route each session's graph takes (OnlineSLAM.pgo_route).  A pending background PGO of a named
-        session is folded first (OnlineSLAM.wait_pgo)."""
+        session is folded first (OnlineSLAM.wait_pgo).
+
+        background=True does the same up to the optimisation -- folds, opening messages, optimised sets,
+        loop_related_views cleared -- then starts one PoseGraphOpt.start_group run over the named sessions' graphs on
+        a side stream and returns.  Each of those sessions then has a pending PGO (OnlineSLAM.pgo_pending), which its
+        polls fold as they fold its own background PGOs (INTEGRATION.md §5): afterwards it equals optimize(ks) bit
+        for bit.  A session without nodes or edges prints its closing message now."""
         order, seen = [], set()
         for k in ks:
             k = self._index(k)
@@ -211,6 +281,19 @@ class SLAMSessions:
             s.wait_pgo()
         t = time.time()
         problems = [s._pgo_begin() for s in sess]
+        if background:
+            batch = _Batch()
+            for s, p in zip(sess, problems):
+                s.loop_related_views = set()
+                if p is None:
+                    s._pgo_end(None)
+                else:
+                    batch.problems.append(p)
+                    s._pgo_run = (_SessionRun(batch), p, [])
+            if batch.problems:
+                batch.start()
+            _share(sess, "pgo", time.time() - t)
+            return
         run = [p for p in problems if p is not None]
         if run:
             PoseGraphOpt.optimize_group([g for g, _ in run], *[[a[i] for _, a in run] for i in range(3)])

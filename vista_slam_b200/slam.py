@@ -11,8 +11,11 @@ Same constructor (arguments and defaults) and the surface run.py, run_live.py an
   * the device pose graph (csrc/slam_graph.cu, `sta_graph_*`): node / edge tables, the depth / confidence / intrinsics
     store and the per-view best node live in fixed-capacity device arrays sized from the reference's formulas
     (slam.py:33-36).  The map store takes 8 H W max_nodes bytes: 1.44 GB at the defaults (3600 nodes) and 224 x 224.
-    A keyframe's kept edges go in with two launches and no host synchronisation; save_data_all / get_view gather on the
-    device, and the world point cloud is built and compacted there (count, exclusive scan, scatter);
+    Keyframes go in with two launches and no host synchronisation for up to 32 of them (sta_graph_add_keyframes):
+    `step` inserts its keyframe at once; `step_many` and SLAMSessions.step queue the insertions of an edge chunk and
+    launch them together at the chunk's end, and before anything reads the tables (a PGO, the fold of a background
+    one, an export) or a capacity IndexError is raised.  save_data_all / get_view gather on the device, and the world
+    point cloud is built and compacted there (count, exclusive scan, scatter);
   * PoseGraphOpt, working on slices of the node and edge tables.
 
 A step synchronises with the host twice, as the GPU stages need: the loop-candidate read (detect_loop runs first: it
@@ -29,7 +32,9 @@ the call with one read-back, and the gated edge regression in chunks of up to 16
 step and step_many poll it at every keyframe without waiting, and fold it when it is done -- its poses written, the
 nodes inserted since its launch re-derived from them (sta_graph_replay_nodes) -- which leaves the graph bit-identical
 to the synchronous path.  Until the fold, get_view shows the poses from before the PGO; the next due PGO,
-pose_graph_optimize, save_data_all, reset and wait_pgo wait for a pending run (INTEGRATION.md §5).
+pose_graph_optimize, save_data_all, reset and wait_pgo wait for a pending run (INTEGRATION.md §5).  In
+SLAMSessions.step the PGOs that fall due in one call start together as one run (PoseGraphOpt.start_group), and
+SLAMSessions.optimize(ks, background=True) starts one for the named sessions; each session folds its share as above.
 
 Importing this module does not import pypose, munch, colorama or open3d.  `get_view` returns a `View` (attribute and key
 access, as munch.Munch).  The PLY of save_data_all is written here: binary little-endian, float x y z and uchar
@@ -163,6 +168,7 @@ class OnlineSLAM:
         self.pgo_background = False  # run due PGOs on a side stream while step goes on (see the module docstring)
         self._pgo_run = None  # a background PGO not yet folded: (PoseGraphRun, its problem, nodes to replay)
         self._graph = None  # created at the first keyframe, when the map size is known
+        self._kf_queue = []  # keyframe insertions not yet launched (_add_keyframe, insert_keyframes)
         self._reset_host_graph()
 
     @staticmethod
@@ -186,6 +192,7 @@ class OnlineSLAM:
         if self._pgo_run is not None:  # discarded, once its queued work has finished with the tables
             self._pgo_run[0].wait()
             self._pgo_run = None
+        self._kf_queue = []
         if self._graph is not None:
             with torch.cuda.device(self._graph.device):
                 _lib.check(_lib.lib().sta_graph_reset(self._graph.h, _lib.cur_stream()), "sta_graph_reset")
@@ -232,11 +239,13 @@ class OnlineSLAM:
         return self.kf.regress_keyframes_gated(items, self.rel_pose_thres)
 
     def _add_keyframe(self, i, js, keep, batch):
-        """connect_view_i_j (slam.py:191-241) for the kept edges, in order: host integers, then two launches."""
+        """connect_view_i_j (slam.py:191-241) for the kept edges, in order: the host integers now, the launch queued
+        (_kf_queue) for the next insert_keyframes; a capacity IndexError launches the queue first."""
         g = self._graph
         n = len(keep)
         kept_js = [js[k] for k in keep]
         if n > _lib.GRAPH_MAX_KEYFRAME_EDGES:
+            self._insert_queued()
             raise ValueError("at most %d kept edges per keyframe" % _lib.GRAPH_MAX_KEYFRAME_EDGES)
         v2n = {v: list(self.view_to_node.get(v, [])) for v in set(kept_js) | {i}}
         first_j, n_scale = [], n - 1
@@ -246,16 +255,19 @@ class OnlineSLAM:
             n_scale += first_j[-1] >= 0
             v2n[j].append(self.num_nodes + 2 * k + 1)
         if self.num_nodes + 2 * n > g.max_nodes or i >= g.max_views:
+            self._insert_queued()
             raise IndexError("pose graph node capacity (%d) exceeded" % g.max_nodes)
         if self.num_edges + n_scale + n > g.max_edges:
+            self._insert_queued()
             raise IndexError("pose graph edge capacity (%d) exceeded" % g.max_edges)
         H, W = batch["conf"].shape[-2:]
         args = ((ctypes.c_int64 * n)(*kept_js), (ctypes.c_int * n)(*keep), (ctypes.c_int * n)(*first_j))
-        with torch.cuda.device(g.device):
-            _lib.check(_lib.lib().sta_graph_add_keyframe(
-                g.h, i, n, *args, self.num_nodes, self.num_edges, H, W, _lib.ptr(batch["pose"]), _lib.ptr(batch["pose_conf"]),
-                _lib.ptr(batch["conf"]), _lib.ptr(batch["depths"]), _lib.ptr(batch["intri"]), _lib.ptr(batch["conf_mean"]),
-                _lib.cur_stream()), "sta_graph_add_keyframe")
+        kf = _lib.StaGraphKeyframe(g.h, i, n, self.num_nodes, self.num_edges, H, W, *args,
+                                   *[batch[k].data_ptr() for k in ("pose", "pose_conf", "conf", "depths", "intri",
+                                                                   "conf_mean")])
+        if not _lib.lib().sta_graph_add_keyframes_scratch_bytes(ctypes.byref(kf), 1):  # refused: nothing changes
+            _lib.check(1, "sta_graph_add_keyframes")
+        self._kf_queue.append((kf, args, batch))  # the host arrays and the device inputs live until the launch
         if self._pgo_run is not None:  # the nodes a pending background PGO's fold re-derives, in link order
             rec, e = self._pgo_run[2], self.num_edges
             for k in range(n):
@@ -275,6 +287,11 @@ class OnlineSLAM:
         self.num_nodes += 2 * n
         self.num_edges += n_scale + n
 
+    def _insert_queued(self):
+        """Launch this session's queued keyframe insertions (insert_keyframes); called before anything reads the
+        tables."""
+        insert_keyframes([self])
+
     def _insert_keyframe(self, i, js, conf_host, keep, batch):
         """connect_view_i_j (slam.py:191-241) after the gate, for a registered view i: the reject and loop-closure
         messages, loop_related_views, and the kept edges into the graph (_add_keyframe)."""
@@ -291,9 +308,9 @@ class OnlineSLAM:
         if keep:
             self._add_keyframe(i, js, keep, batch)
 
-    def _pgo_if_due(self, force_pgo, log_intermediate_results, output_folder):
+    def _pgo_if_due(self, force_pgo, log_intermediate_results, output_folder, group=None):
         """slam.py:282-297: PGO every pgo_every views or when forced, after logging the trajectory if asked.  Returns
-        whether it ran."""
+        whether it ran.  A background PGO is captured into `group` (SLAMSessions.step) when one is given."""
         if not (self.view_num % self.pgo_every == 0 or force_pgo):
             return False
         self.wait_pgo()
@@ -303,7 +320,7 @@ class OnlineSLAM:
                                save_intrinsics=False, save_confs=False, save_ply=False)
         opt_start = time.time()
         if self.pgo_background:
-            self._pgo_launch()
+            self._pgo_launch(group)
             self.time_dict["pgo"] += time.time() - opt_start
             return True
         self.pose_graph_optimize()
@@ -311,17 +328,18 @@ class OnlineSLAM:
         torch.cuda.empty_cache()
         return True
 
-    def _pgo_launch(self):
+    def _pgo_launch(self, group=None):
         """The background form of pose_graph_optimize: its opening messages and optimised set now, loop_related_views
         cleared now (keyframes inserted before the fold add to the next PGO's set, as after a synchronous PGO), and
-        the optimisation started on a side stream (PoseGraphOpt.start)."""
+        the optimisation started on a side stream (PoseGraphOpt.start), or captured into `group`, which starts it with
+        the other PGOs it holds (group.add returns the run's handle: poll(), wait(), stream)."""
         problem = self._pgo_begin()
         self.loop_related_views = set()
         if problem is None:
             _msg("[PoseGraphOpt] ", "Pose graph optimization done.")
             return
         graph, args = problem
-        self._pgo_run = (graph.start(*args), problem, [])
+        self._pgo_run = (graph.start(*args) if group is None else group.add(graph, args), problem, [])
 
     @property
     def pgo_pending(self):
@@ -391,6 +409,7 @@ class OnlineSLAM:
             self.time_dict["decoder"] += time.time() - dec_start
             self._check_flags()
             self._insert_keyframe(i, js, *res)
+            self._insert_queued()  # a group of one
         self._pgo_poll()
         self.time_dict["graph_construction"] += time.time() - graph_start
         return self._pgo_if_due(force_pgo, log_intermediate_results, output_folder)
@@ -438,23 +457,29 @@ class OnlineSLAM:
         self._check_flags()
 
         items = [(i0 + k, list(range(far[k], i0 + k)) + [j for j, _ in loops[k][:self.loop_edge_num]]) for k in range(n)]
+        chunk_ends = {c[-1] for c in KeyframeFrontend.edge_chunks(items)}
         flags = []
         checked = True
         results = iter(self._regress_keyframes(items))
-        for k, (v, (i, js)) in enumerate(zip(values, items)):
-            graph_start = time.time()
-            dec_start = time.time()
-            res = next(results)  # the first keyframe of an edge chunk runs the chunk: read-back of its gate
-            self.time_dict["decoder"] += time.time() - dec_start
-            self._check_flags()
-            self._register_keyframe(v, i, js, res)
-            if js:
-                checked = checked and not res[1]
-            self._pgo_poll()
-            self.time_dict["graph_construction"] += time.time() - graph_start
-            flags.append(self._pgo_if_due(force_pgo and k == n - 1, log_intermediate_results, output_folder))
-            if flags[-1] and not self.pgo_background:  # a synchronous PGO's read-backs waited for the graph launches
-                checked = self.num_nodes > 0 and self.num_edges > 0
+        try:
+            for k, (v, (i, js)) in enumerate(zip(values, items)):
+                graph_start = time.time()
+                dec_start = time.time()
+                res = next(results)  # the first keyframe of an edge chunk runs the chunk: read-back of its gate
+                self.time_dict["decoder"] += time.time() - dec_start
+                self._check_flags()
+                self._register_keyframe(v, i, js, res)
+                if js:
+                    checked = checked and not res[1]
+                if k in chunk_ends:  # the chunk's keyframes go in with one sta_graph_add_keyframes
+                    self._insert_queued()
+                self._pgo_poll()
+                self.time_dict["graph_construction"] += time.time() - graph_start
+                flags.append(self._pgo_if_due(force_pgo and k == n - 1, log_intermediate_results, output_folder))
+                if flags[-1] and not self.pgo_background:  # a synchronous PGO's read-backs waited for the graph launches
+                    checked = self.num_nodes > 0 and self.num_edges > 0
+        finally:  # an exception mid-chunk still leaves the graph as the host bookkeeping says
+            self._insert_queued()
         if not checked:
             torch.cuda.current_stream().synchronize()
             self._check_flags()
@@ -493,6 +518,7 @@ class OnlineSLAM:
         opt.update(self.loop_related_views)  # view ids, used as node ids (slam.py:120)
         if not (N > 0 and E > 0):
             return None
+        self._insert_queued()
         g = self._graph
         idx = torch.tensor(sorted(opt), dtype=torch.int64).to(self.device)
         graph = PoseGraphOpt(g.pose[:N], to_optimize_idxs=idx, route=self.pgo_route)
@@ -509,6 +535,7 @@ class OnlineSLAM:
     def _pgo_write(self, problem, replay=()):
         """The optimised poses of _pgo_begin's problem into the node table, then the (node, parent, edge) triples of
         `replay` re-derived in order."""
+        self._insert_queued()  # the replayed nodes' insertions come first
         g = self._graph
         nodes = problem[0].get_nodes()
         g.pose[:nodes.shape[0]] = nodes
@@ -525,6 +552,7 @@ class OnlineSLAM:
         for v in range(view0, view0 + num_views):
             if not self.view_to_node.get(v):
                 raise IndexError("view %d has no node in the pose graph" % v)
+        self._insert_queued()
         g = self._graph
         dev = g.device
         H, W = g.H, g.W
@@ -638,6 +666,28 @@ class OnlineSLAM:
         time_dict["graph_construction"] = time_dict["graph_construction"] - time_dict["decoder"]
         time_dict["total"] = sum(time_dict.values())
         return time_dict
+
+
+def insert_keyframes(sessions):
+    """Launch the keyframe insertions the sessions have queued (OnlineSLAM._add_keyframe), every session's in its
+    order: one sta_graph_add_keyframes (two launches, no host synchronisation) per GRAPH_MAX_GROUP_KEYFRAMES
+    keyframes, whichever sessions they belong to.  Nothing is launched when no keyframe is queued."""
+    owners = [s for s in sessions if s._kf_queue]
+    if not owners:
+        return
+    queued = [q for s in owners for q in s._kf_queue]
+    for s in owners:
+        s._kf_queue = []
+    L, M = _lib.lib(), _lib.GRAPH_MAX_GROUP_KEYFRAMES
+    device = owners[0]._graph.device
+    with torch.cuda.device(device):
+        for c0 in range(0, len(queued), M):
+            part = queued[c0:c0 + M]
+            tab = (_lib.StaGraphKeyframe * len(part))(*[kf for kf, _, _ in part])
+            need = int(L.sta_graph_add_keyframes_scratch_bytes(tab, len(part)))
+            scratch = torch.empty((need + 7) // 8, dtype=torch.float64, device=device)
+            _lib.check(L.sta_graph_add_keyframes(tab, len(part), _lib.ptr(scratch), need, _lib.cur_stream()),
+                       "sta_graph_add_keyframes")
 
 
 def write_ply(path, points, colors):
