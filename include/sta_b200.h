@@ -585,6 +585,29 @@ int sta_graph_add_keyframes(const StaGraphKeyframe* kfs, int count, void* scratc
  * poses were written, bit for bit.  One single-thread launch per 256 triples, no host synchronisation.  Refused before
  * any launch: a node or parent outside [0, max_nodes), a node that is its own parent, an edge outside [0, max_edges). */
 int sta_graph_replay_nodes(StaGraph* g, int count, const int* triples_host, void* stream);
+/* Track F frames against the graph without changing it.  Frame f was regressed as the pair (frame, keyframe view k)
+ * (sta_regress_pairs_begin / _finish): pose_dev [F][4][4] its i -> j pose T, depth_dev / conf_dev [F][H][W] its k-side
+ * maps.  anchors_host[f] is the first node of view k.  Per frame:
+ *   s = the scale edge reduction of sta_graph_add_keyframe (depth_k, depth_anchor, conf_k, conf_anchor), same grid;
+ *   T as Sim(3) [t | q | 1] (meas_out [F][8]), s (scale_edge_out [F]), valid_out [F] = 1 unless T's rotation fails
+ *   the orthonormality check that raises STA_GRAPH_FLAG_NOT_SO3 for a keyframe (the flag is not raised here);
+ *   pose = pose[anchor] * Sim3(0, id, s) * Sim3(T): pose_out [F][4][4] with the scale dropped and scale_out [F], as
+ *   sta_graph_export gives keyframes.  This is bit for bit the pose sta_graph_add_keyframe gives node i of a keyframe
+ *   whose first kept edge is (i, k) with the same inputs.
+ * scratch: sta_graph_track_frames_scratch_bytes(F) bytes, 8-byte aligned (0 for F outside the range).  Two launches,
+ * the anchors passed as kernel parameters, no host synchronisation.  Refused before any launch: F outside
+ * [1, STA_GRAPH_MAX_TRACK_FRAMES], a null argument, an anchor outside [0, max_nodes), host memory, a small scratch. */
+enum { STA_GRAPH_MAX_TRACK_FRAMES = 4096 };
+size_t sta_graph_track_frames_scratch_bytes(int num_frames);
+int sta_graph_track_frames(StaGraph* g, int num_frames, const int* anchors_host, const float* pose_dev,
+                           const float* depth_dev, const float* conf_dev, float* meas_out, float* scale_edge_out,
+                           unsigned char* valid_out, float* pose_out, float* scale_out, void* scratch,
+                           size_t scratch_bytes, void* stream);
+/* Recompose F stored frames (meas_dev [F][8] and scale_edge_dev [F] as sta_graph_track_frames wrote them) on their
+ * anchors' current poses, in the same order: pose_out [F][4][4] (scale dropped), scale_out [F].  One launch, no host
+ * synchronisation; refused as sta_graph_track_frames. */
+int sta_graph_frame_poses(StaGraph* g, int num_frames, const int* anchors_host, const float* meas_dev,
+                          const float* scale_edge_dev, float* pose_out, float* scale_out, void* stream);
 /* Per view v in [view0, view0 + num_views), through its best node (every view must have one): pose_out [V][4][4] (rotation
  * and translation, scale dropped), scale_out [V], depth_out / conf_out [V][H][W] (unscaled), intri_out [V][3][3].
  * With points_out: the world point cloud of save_data_all -- depth s unprojected with K^-1, then R p + t, points with

@@ -53,6 +53,7 @@ FLOW_MAX_CORNERS = 1000
 GRAPH_MAX_KEYFRAME_EDGES = 32
 GRAPH_MAX_GROUP_KEYFRAMES = 32  # STA_GRAPH_MAX_GROUP_KEYFRAMES: keyframes per sta_graph_add_keyframes call
 GRAPH_FLAG_NOT_SO3 = 1
+GRAPH_MAX_TRACK_FRAMES = 4096  # STA_GRAPH_MAX_TRACK_FRAMES: frames per sta_graph_track_frames / _frame_poses call
 ORB_MAX_KEYPOINTS = 4096
 PG_DENSE_MAX_OPT = 3657  # STA_PG_DENSE_MAX_OPT: above it PoseGraphOpt takes the block-sparse route
 PG_GROUP_MAX = 16  # STA_PG_GROUP_MAX: graphs per sta_pose_graph_lm_step_group call or sta_pg_group_plan
@@ -220,6 +221,10 @@ def lib():
     L.sta_graph_add_keyframes_scratch_bytes.restype = ctypes.c_size_t
     L.sta_graph_add_keyframes.argtypes = [POINTER(StaGraphKeyframe), i, vp, ctypes.c_size_t, vp]
     L.sta_graph_replay_nodes.argtypes = [vp, i, POINTER(c_int), vp]
+    L.sta_graph_track_frames_scratch_bytes.argtypes = [i]
+    L.sta_graph_track_frames_scratch_bytes.restype = ctypes.c_size_t
+    L.sta_graph_track_frames.argtypes = [vp, i, POINTER(c_int), vp, vp, vp, vp, vp, vp, vp, vp, vp, ctypes.c_size_t, vp]
+    L.sta_graph_frame_poses.argtypes = [vp, i, POINTER(c_int), vp, vp, vp, vp, vp]
     L.sta_graph_export_scratch_bytes.argtypes = [i, i]
     L.sta_graph_export_scratch_bytes.restype = ctypes.c_size_t
     L.sta_graph_export.argtypes = [vp, i, i, c_float, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]

@@ -13,12 +13,18 @@
 //                        -100), rotation -> quaternion, node poses and edge records.
 // A scale reduction that reads a node inserted earlier in the same launch reads it from that keyframe's inputs, not
 // from the store the copies are writing (map_of).
+//
+// Tracked frames (OnlineSLAM.track) read the graph and never write it: track_reduce_kernel runs each frame's scale
+// reduction against its anchor node in the store, and track_link_kernel composes the frame's pose with the Sim(3)
+// algebra of sim3.cuh in the order graph_link_kernel would use for a keyframe with that single edge.
+// frame_poses_kernel recomposes stored frames on their anchors' current poses.
 #include <string>
 
 #include "../../include/sta_b200.h"
 #include "cloud.cuh"
 #include "host_util.h"
 #include "pointmap.cuh"
+#include "sim3.cuh"
 
 struct StaGraph {
   int max_nodes = 0, max_edges = 0, max_views = 0, H = 0, W = 0;
@@ -131,63 +137,6 @@ __global__ void __launch_bounds__(256) graph_ingest_kernel(const __grid_constant
     cd[i] = a.confs[src + i];
   }
   if (blockIdx.x == 0 && threadIdx.x < 9) a.intri[slot * 9 + threadIdx.x] = a.in_intri[(d >> 1) * 9 + threadIdx.x];
-}
-
-// Sim(3) a * b in the [t | q | s] layout; the quaternion is kept with w >= 0.
-__device__ void sim3_mul(const float* a, const float* b, float* o) {
-  const float ax = a[3], ay = a[4], az = a[5], aw = a[6];
-  const float bx = b[3], by = b[4], bz = b[5], bw = b[6];
-  // t = t_a + s_a R_a t_b, with R_a t_b = t_b + 2 w (u x t_b) + 2 u x (u x t_b)
-  const float tx = b[0], ty = b[1], tz = b[2];
-  const float cx = ay * tz - az * ty, cy = az * tx - ax * tz, cz = ax * ty - ay * tx;
-  const float rx = tx + 2.f * (aw * cx + ay * cz - az * cy);
-  const float ry = ty + 2.f * (aw * cy + az * cx - ax * cz);
-  const float rz = tz + 2.f * (aw * cz + ax * cy - ay * cx);
-  float q[4] = {aw * bx + ax * bw + ay * bz - az * by, aw * by - ax * bz + ay * bw + az * bx,
-                aw * bz + ax * by - ay * bx + az * bw, aw * bw - ax * bx - ay * by - az * bz};
-  const float sg = q[3] < 0.f ? -1.f : 1.f;
-  o[0] = a[0] + a[7] * rx;
-  o[1] = a[1] + a[7] * ry;
-  o[2] = a[2] + a[7] * rz;
-  for (int i = 0; i < 4; ++i) o[3 + i] = sg * q[i];
-  o[7] = a[7] * b[7];
-}
-
-// Rotation (row-major 3x3 inside a 4x4) -> unit quaternion (x, y, z, w), w >= 0 (Shepperd's method, fp64).
-// Returns false when R is not orthonormal with det +1 to 1e-3 (what pp.mat2SE3(atol=1e-3) refuses).
-__device__ bool rot_to_quat(const float* M, float* q) {
-  double R[3][3];
-  for (int r = 0; r < 3; ++r)
-    for (int c = 0; c < 3; ++c) R[r][c] = M[r * 4 + c];
-  bool ok = true;
-  for (int r = 0; r < 3; ++r)
-    for (int c = 0; c < 3; ++c) {
-      const double d = R[r][0] * R[c][0] + R[r][1] * R[c][1] + R[r][2] * R[c][2] - (r == c ? 1.0 : 0.0);
-      ok = ok && fabs(d) <= 1e-3;
-    }
-  const double det = R[0][0] * (R[1][1] * R[2][2] - R[1][2] * R[2][1]) - R[0][1] * (R[1][0] * R[2][2] - R[1][2] * R[2][0]) +
-                     R[0][2] * (R[1][0] * R[2][1] - R[1][1] * R[2][0]);
-  ok = ok && fabs(det - 1.0) <= 1e-3;
-  double x[4];
-  const double t = R[0][0] + R[1][1] + R[2][2];
-  if (t > 0) {
-    const double s = sqrt(t + 1.0) * 2;
-    x[0] = (R[2][1] - R[1][2]) / s; x[1] = (R[0][2] - R[2][0]) / s; x[2] = (R[1][0] - R[0][1]) / s; x[3] = 0.25 * s;
-  } else {
-    int i = 0;
-    if (R[1][1] > R[i][i]) i = 1;
-    if (R[2][2] > R[i][i]) i = 2;
-    const int j = (i + 1) % 3, k = (i + 2) % 3;
-    const double s = sqrt(1.0 + R[i][i] - R[j][j] - R[k][k]) * 2;
-    x[i] = 0.25 * s;
-    x[j] = (R[j][i] + R[i][j]) / s;
-    x[k] = (R[k][i] + R[i][k]) / s;
-    x[3] = (R[k][j] - R[j][k]) / s;
-  }
-  const double sg = x[3] < 0 ? -1.0 : 1.0;
-  const double nrm = sqrt(x[0] * x[0] + x[1] * x[1] + x[2] * x[2] + x[3] * x[3]);
-  for (int e = 0; e < 4; ++e) q[e] = static_cast<float>(sg * x[e] / nrm);
-  return ok;
 }
 
 __device__ void put_edge(const KfDesc& g, int e, long long ni, long long nj, const float* m8, const float* w7) {
@@ -312,18 +261,7 @@ export_gather_kernel(StaGraph g, int view0, float thres, float* pose_out, float*
     if (threadIdx.x == 0) counts[static_cast<long long>(v) * g.H + row] = t;
   }
   if (row == 0 && threadIdx.x == 0) {
-    const float* p = g.pose + b * 8;
-    const float x = p[3], y = p[4], z = p[5], w = p[6];  // LieTensor.rotation().matrix()
-    const float R[9] = {1 - 2 * (y * y + z * z), 2 * (x * y - z * w), 2 * (x * z + y * w),
-                        2 * (x * y + z * w), 1 - 2 * (x * x + z * z), 2 * (y * z - x * w),
-                        2 * (x * z - y * w), 2 * (y * z + x * w), 1 - 2 * (x * x + y * y)};
-    float* P = pose_out + v * 16;
-    for (int r = 0; r < 3; ++r) {
-      for (int c = 0; c < 3; ++c) P[r * 4 + c] = R[r * 3 + c];
-      P[r * 4 + 3] = p[r];
-    }
-    P[12] = 0.f; P[13] = 0.f; P[14] = 0.f; P[15] = 1.f;
-    scale_out[v] = p[7];
+    scale_out[v] = sim3_to_pose44(g.pose + b * 8, pose_out + v * 16);
     for (int i = 0; i < 9; ++i) intri_out[v * 9 + i] = g.intri[b * 9 + i];
   }
 }
@@ -348,6 +286,76 @@ export_scatter_kernel(StaGraph g, float thres, const float* pose_out, const floa
                     for (int c = 0; c < 3; ++c)
                       colors[o * 3 + c] = (imgs[(static_cast<long long>(v) * 3 + c) * hw + static_cast<long long>(row) * W + x] + 1.f) / 2.f;
                   });
+}
+
+// ---- tracked frames ----
+
+// Host anchors of a track or frame-pose launch, passed as a __grid_constant__ kernel parameter: one launch for up to
+// STA_GRAPH_MAX_TRACK_FRAMES frames with no copy before it.  Instantiated for up to kTrackSmall frames and for the
+// maximum, so that a few frames do not pass the large table.
+constexpr int kTrackSmall = 64;
+constexpr int kMaxTrack = STA_GRAPH_MAX_TRACK_FRAMES;
+template <int N>
+struct TrackArgs {
+  int count;
+  int anchor[N];
+};
+static_assert(sizeof(TrackArgs<kMaxTrack>) + 128 <= 32764, "the anchor table must fit the kernel-parameter space");
+
+// grid (kStatBlocks, F), 256 threads: frame f's scale reduction against its anchor in the store, with the argument
+// order of the scale edge a new node of the keyframe view gets (estimate_scale_with_depth_and_confidence(depth,
+// depth_other, conf, conf_other), slam.py:224): the frame pair's keyframe-side maps first.
+template <int N>
+__global__ void __launch_bounds__(256) track_reduce_kernel(const __grid_constant__ TrackArgs<N> p, const float* gdepth,
+                                                          const float* gconf, const float* depth, const float* conf,
+                                                          long long hw, double* partial) {
+  const int f = blockIdx.y;
+  const long long a = p.anchor[f];
+  scale_partial(depth + f * hw, gdepth + a * hw, conf + f * hw, gconf + a * hw, hw, blockIdx.x,
+                partial + f * kPartialDoubles + static_cast<long long>(blockIdx.x) * kStatVals);
+}
+
+// pose[anchor] * Sim3(0, id, s) * Sim3(T): the product graph_link_kernel gives node i of a keyframe whose first kept
+// edge is (i, k) -- the scale edge's node of k from the anchor, then the pose edge -- as [t | q | s].
+__device__ void track_compose(const float* anchor_pose, float s, const float* T, float* out) {
+  const float S[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 1.f, s};
+  float j[8];
+  sim3_mul(anchor_pose, S, j);
+  sim3_mul(j, T, out);
+}
+
+// one thread per frame: the reduction finished, T_fk -> [t | q | 1] (a failed SO(3) check clears valid and raises no
+// graph flag), the composed pose as 4x4 (scale dropped) and its scale
+template <int N>
+__global__ void __launch_bounds__(64) track_link_kernel(const __grid_constant__ TrackArgs<N> p, const float* gpose,
+                                                        const double* partial, long long hw, const float* pose_in,
+                                                        float* meas_out, float* s_out, unsigned char* valid_out,
+                                                        float* pose_out, float* scale_out) {
+  const int f = blockIdx.x * blockDim.x + threadIdx.x;
+  if (f >= p.count) return;
+  float sc[2];
+  scale_finalize(partial + f * kPartialDoubles, hw, sc);
+  const float* M = pose_in + f * 16;
+  float T[8] = {M[3], M[7], M[11], 0.f, 0.f, 0.f, 1.f, 1.f};
+  const bool ok = rot_to_quat(M, T + 3);
+  for (int i = 0; i < 8; ++i) meas_out[f * 8 + i] = T[i];
+  s_out[f] = sc[0];
+  valid_out[f] = ok ? 1 : 0;
+  float P[8];
+  track_compose(gpose + static_cast<long long>(p.anchor[f]) * 8, sc[0], T, P);
+  scale_out[f] = sim3_to_pose44(P, pose_out + f * 16);
+}
+
+// one thread per frame: a stored frame recomposed on its anchor's current pose
+template <int N>
+__global__ void __launch_bounds__(64) frame_poses_kernel(const __grid_constant__ TrackArgs<N> p, const float* gpose,
+                                                         const float* meas, const float* s, float* pose_out,
+                                                         float* scale_out) {
+  const int f = blockIdx.x * blockDim.x + threadIdx.x;
+  if (f >= p.count) return;
+  float P[8];
+  track_compose(gpose + static_cast<long long>(p.anchor[f]) * 8, s[f], meas + f * 8, P);
+  scale_out[f] = sim3_to_pose44(P, pose_out + f * 16);
 }
 
 }  // namespace
@@ -625,6 +633,94 @@ int sta_graph_export(StaGraph* g, int view0, int num_views, float conf_thres, co
                                                                imgs_dev, offsets, points_out, colors_out);
   STA_CHECK_CUDA(cudaGetLastError());
   return 0;
+}
+
+}  // extern "C"
+
+namespace {
+
+// The refusals shared by sta_graph_track_frames and sta_graph_frame_poses, before any launch.
+int check_frames(const StaGraph* g, int F, const int* anchors_host) {
+  STA_REQUIRE(F >= 1 && F <= kMaxTrack, "1 to STA_GRAPH_MAX_TRACK_FRAMES frames per call");
+  STA_REQUIRE(g != nullptr && anchors_host != nullptr, "null argument");
+  for (int f = 0; f < F; ++f)
+    STA_REQUIRE(anchors_host[f] >= 0 && anchors_host[f] < g->max_nodes, "anchor node out of the graph's capacity");
+  return 0;
+}
+
+template <int N>
+TrackArgs<N> track_args(int F, const int* anchors_host) {
+  TrackArgs<N> p;
+  p.count = F;
+  for (int f = 0; f < F; ++f) p.anchor[f] = anchors_host[f];
+  return p;
+}
+
+template <int N>
+int launch_track(StaGraph* g, int F, const int* anchors_host, const float* pose_dev, const float* depth_dev,
+                 const float* conf_dev, float* meas_out, float* s_out, unsigned char* valid_out, float* pose_out,
+                 float* scale_out, double* partial, cudaStream_t st) {
+  const TrackArgs<N> p = track_args<N>(F, anchors_host);
+  const long long hw = static_cast<long long>(g->H) * g->W;
+  track_reduce_kernel<N><<<dim3(kStatBlocks, F), 256, 0, st>>>(p, g->depth, g->conf, depth_dev, conf_dev, hw, partial);
+  STA_CHECK_CUDA(cudaGetLastError());
+  track_link_kernel<N><<<(F + 63) / 64, 64, 0, st>>>(p, g->pose, partial, hw, pose_dev, meas_out, s_out, valid_out,
+                                                    pose_out, scale_out);
+  STA_CHECK_CUDA(cudaGetLastError());
+  return 0;
+}
+
+template <int N>
+int launch_frame_poses(StaGraph* g, int F, const int* anchors_host, const float* meas_dev, const float* s_dev,
+                       float* pose_out, float* scale_out, cudaStream_t st) {
+  frame_poses_kernel<N><<<(F + 63) / 64, 64, 0, st>>>(track_args<N>(F, anchors_host), g->pose, meas_dev, s_dev, pose_out,
+                                                      scale_out);
+  STA_CHECK_CUDA(cudaGetLastError());
+  return 0;
+}
+
+}  // namespace
+
+extern "C" {
+
+size_t sta_graph_track_frames_scratch_bytes(int num_frames) {
+  if (num_frames < 1 || num_frames > kMaxTrack) return 0;
+  return sizeof(double) * kPartialDoubles * num_frames;
+}
+
+int sta_graph_track_frames(StaGraph* g, int num_frames, const int* anchors_host, const float* pose_dev,
+                           const float* depth_dev, const float* conf_dev, float* meas_out, float* scale_edge_out,
+                           unsigned char* valid_out, float* pose_out, float* scale_out, void* scratch,
+                           size_t scratch_bytes, void* stream) {
+  const int F = num_frames;
+  if (int rc = check_frames(g, F, anchors_host)) return rc;
+  STA_REQUIRE(pose_dev && depth_dev && conf_dev, "null device input");
+  STA_REQUIRE(meas_out && scale_edge_out && valid_out && pose_out && scale_out, "null output");
+  STA_REQUIRE(scratch != nullptr && (reinterpret_cast<uintptr_t>(scratch) & 7) == 0, "null or misaligned scratch");
+  STA_REQUIRE(scratch_bytes >= sta_graph_track_frames_scratch_bytes(F), "scratch smaller than sta_graph_track_frames_scratch_bytes");
+  STA_REQUIRE(on_device(pose_dev) && on_device(depth_dev) && on_device(conf_dev) && on_device(meas_out) &&
+                  on_device(scale_edge_out) && on_device(valid_out) && on_device(pose_out) && on_device(scale_out) &&
+                  on_device(scratch),
+              "inputs and outputs must be device memory");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  double* partial = static_cast<double*>(scratch);
+  if (F <= kTrackSmall)
+    return launch_track<kTrackSmall>(g, F, anchors_host, pose_dev, depth_dev, conf_dev, meas_out, scale_edge_out,
+                                     valid_out, pose_out, scale_out, partial, st);
+  return launch_track<kMaxTrack>(g, F, anchors_host, pose_dev, depth_dev, conf_dev, meas_out, scale_edge_out, valid_out,
+                                 pose_out, scale_out, partial, st);
+}
+
+int sta_graph_frame_poses(StaGraph* g, int num_frames, const int* anchors_host, const float* meas_dev,
+                          const float* scale_edge_dev, float* pose_out, float* scale_out, void* stream) {
+  const int F = num_frames;
+  if (int rc = check_frames(g, F, anchors_host)) return rc;
+  STA_REQUIRE(meas_dev && scale_edge_dev && pose_out && scale_out, "null device argument");
+  STA_REQUIRE(on_device(meas_dev) && on_device(scale_edge_dev) && on_device(pose_out) && on_device(scale_out),
+              "inputs and outputs must be device memory");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (F <= kTrackSmall) return launch_frame_poses<kTrackSmall>(g, F, anchors_host, meas_dev, scale_edge_dev, pose_out, scale_out, st);
+  return launch_frame_poses<kMaxTrack>(g, F, anchors_host, meas_dev, scale_edge_dev, pose_out, scale_out, st);
 }
 
 }  // extern "C"

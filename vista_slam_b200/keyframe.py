@@ -17,7 +17,10 @@ ones within rounding, not bit for bit.
 
 Across caches (SLAMSessions): `add_views_group` encodes the new views of several caches that share one STA in the same
 calls, and `regress_keyframes_gated_group` runs the gated step over keyframes of several caches, a chunk's edges mixing
-caches.  One cache through them launches exactly what add_views / regress_keyframes_gated launch."""
+caches.  One cache through them launches exactly what add_views / regress_keyframes_gated launch.
+
+Tracked frames (OnlineSLAM.track): `encode_views` encodes frames without caching them and `regress_frames` regresses
+each (frame, keyframe) pair through `regress_pairs`, the chunk regression the keyframe path runs, with no gate."""
 import ctypes
 
 import torch
@@ -98,27 +101,12 @@ class KeyframeFrontend:
             raise ValueError("all views of a batch must have the same size")
         fi = torch.cat([c.enc_features[i] for c, i, _ in run], dim=0)
         fj = torch.cat([c.enc_features[j] for c, _, j in run], dim=0)
-        L = self.frontend._ready(fi)
-        dev = fi.device
 
-        def f32(*shape):
-            return torch.empty(*shape, device=dev, dtype=torch.float32)
+        def gate(conf_host):
+            return [e for e, (_, i, j) in enumerate(edges) if not (conf_host[e] < rel_pose_thres and i - j != 1)]
 
-        pose, pconf = f32(2, K, 4, 4), f32(2, K)
-        m = self.frontend
-        with torch.cuda.device(dev):
-            _lib.check(L.sta_regress_pairs_begin(m._handle, _lib.ptr(fi), _lib.ptr(fj), K, H, W, _lib.ptr(pose),
-                                                 _lib.ptr(pconf), _lib.cur_stream()), "sta_regress_pairs_begin")
-            conf_host = self._read_confs(pconf[0, :len(edges)])  # the one host synchronisation of the chunk
-            keep = [e for e, (_, i, j) in enumerate(edges) if not (conf_host[e] < rel_pose_thres and i - j != 1)]
-            n = len(keep)
-            if n:
-                conf, depth = f32(2, n, H, W), f32(2, n, H, W)
-                pts, intri, cmean = f32(2, n, H, W, 3), f32(n, 3, 3), f32(2, n)
-                idx = (ctypes.c_int * n)(*keep)
-                _lib.check(L.sta_regress_pairs_finish(m._handle, idx, n, _lib.ptr(pts), _lib.ptr(conf), _lib.ptr(intri),
-                                                      _lib.ptr(depth), _lib.ptr(cmean), _lib.ptr(_scratch_for(dev, 2 * n)),
-                                                      _lib.cur_stream()), "sta_regress_pairs_finish")
+        pose, pconf, conf_host, keep, maps = regress_pairs(self.frontend, fi, fj, H, W, len(edges), gate,
+                                                           self._read_confs)
         e0 = p0 = 0
         for _, i, js in items:
             e1 = e0 + len(js)
@@ -126,6 +114,7 @@ class KeyframeFrontend:
             p1 = p0 + len(kf_keep)
             batch = {"pose": pose[0, e0:e1], "pose_conf": pconf[0, e0:e1]}
             if kf_keep:
+                conf, depth, intri, cmean = maps
                 batch.update(conf=conf[:, p0:p1].contiguous(), depths=depth[:, p0:p1].contiguous(), intri=intri[p0:p1],
                              conf_mean=cmean[:, p0:p1].contiguous())
             yield conf_host[e0:e1], kf_keep, batch
@@ -200,10 +189,29 @@ class KeyframeFrontend:
 
 
 @torch.no_grad()
+def encode_views(sta, images, shapes):
+    """The encoder features (1, N, 1024) of images (1, 3, H, W) of one size, in order, from B at a time with
+    B N <= GRAPH_MAX_TOKENS (N = H W / 256 tokens; 41 views at 224 x 224), so every call is replayed as a CUDA graph."""
+    if not images:
+        return []
+    H, W = int(images[0].shape[-2]), int(images[0].shape[-1])
+    if any(tuple(im.shape[-2:]) != (H, W) for im in images):
+        raise ValueError("all views of a batch must have the same size")
+    B = max(1, GRAPH_MAX_TOKENS // ((H // 16) * (W // 16)))
+    feats = []
+    for c0 in range(0, len(images), B):
+        chunk = images[c0:c0 + B]
+        x = torch.cat([im.reshape(1, *im.shape[-3:]) for im in chunk]) if len(chunk) > 1 else chunk[0]
+        feat, _ = sta._encode_image(x, shapes[c0], normalize=False)
+        feats += [feat[b:b + 1] for b in range(len(chunk))]
+    return feats
+
+
+@torch.no_grad()
 def add_views_group(caches, images_per_cache, shapes_per_cache=None):
     """KeyframeFrontend.add_views for several caches that share one STA, as one sequence of encoder calls: the new views
-    of all caches in order (cache by cache), all of one size, B at a time as add_views chunks them, each feature
-    appended to its own cache.  Returns each cache's new view indices."""
+    of all caches in order (cache by cache), all of one size, B at a time as add_views chunks them (encode_views), each
+    feature appended to its own cache.  Returns each cache's new view indices."""
     caches = list(caches)
     images = [list(x) for x in images_per_cache]
     shapes = [[None] * len(x) for x in images] if shapes_per_cache is None else [list(x) for x in shapes_per_cache]
@@ -212,18 +220,71 @@ def add_views_group(caches, images_per_cache, shapes_per_cache=None):
     flat = [(c, im, sh) for c, ims, shs in zip(caches, images, shapes) for im, sh in zip(ims, shs)]
     firsts = [c.view_num for c in caches]
     if flat:
+        feats = encode_views(caches[0].frontend, [im for _, im, _ in flat], [sh for _, _, sh in flat])
         H, W = int(flat[0][1].shape[-2]), int(flat[0][1].shape[-1])
-        if any(tuple(im.shape[-2:]) != (H, W) for _, im, _ in flat):
-            raise ValueError("all views of a batch must have the same size")
-        B = max(1, GRAPH_MAX_TOKENS // ((H // 16) * (W // 16)))
-        for c0 in range(0, len(flat), B):
-            chunk = flat[c0:c0 + B]
-            x = torch.cat([im.reshape(1, *im.shape[-3:]) for _, im, _ in chunk]) if len(chunk) > 1 else chunk[0][1]
-            feat, _ = caches[0].frontend._encode_image(x, chunk[0][2], normalize=False)
-            for b, (c, _, _) in enumerate(chunk):
-                c.enc_features.append(feat[b:b + 1])
-                c.img_shapes.append((H, W))
+        for (c, _, _), feat in zip(flat, feats):
+            c.enc_features.append(feat)
+            c.img_shapes.append((H, W))
     return [list(range(f, c.view_num)) for f, c in zip(firsts, caches)]
+
+
+@torch.no_grad()
+def regress_pairs(sta, fi, fj, H, W, n, gate=None, read_confs=None):
+    """The edge regression of one chunk, shared by keyframes and tracked frames: the feature pairs fi / fj [K, N, 1024]
+    (edges 0 .. n - 1 real, the rest padding) through ONE sta_regress_pairs_begin, then ONE sta_regress_pairs_finish
+    over the kept edges.  With a gate, the kept edges are gate(conf_host), conf_host being the n pose confidences read
+    back once (read_confs); without one, all n edges are kept and nothing is read back.
+
+    Returns (pose [2,K,4,4], pose_conf [2,K], conf_host or None, keep, maps), maps = (conf, depths [2,n',H,W],
+    intri [n',3,3], conf_mean [2,n']) over the n' kept edges ([0] = i side, [1] = j side), or None when none is kept."""
+    K = fi.shape[0]
+    L = sta._ready(fi)
+    dev = fi.device
+
+    def f32(*shape):
+        return torch.empty(*shape, device=dev, dtype=torch.float32)
+
+    pose, pconf = f32(2, K, 4, 4), f32(2, K)
+    maps = conf_host = None
+    with torch.cuda.device(dev):
+        _lib.check(L.sta_regress_pairs_begin(sta._handle, _lib.ptr(fi), _lib.ptr(fj), K, H, W, _lib.ptr(pose),
+                                             _lib.ptr(pconf), _lib.cur_stream()), "sta_regress_pairs_begin")
+        if gate is None:
+            keep = list(range(n))
+        else:
+            conf_host = read_confs(pconf[0, :n])  # the one host synchronisation of the chunk
+            keep = gate(conf_host)
+        m = len(keep)
+        if m:
+            conf, depth = f32(2, m, H, W), f32(2, m, H, W)
+            pts, intri, cmean = f32(2, m, H, W, 3), f32(m, 3, 3), f32(2, m)
+            idx = (ctypes.c_int * m)(*keep)
+            _lib.check(L.sta_regress_pairs_finish(sta._handle, idx, m, _lib.ptr(pts), _lib.ptr(conf), _lib.ptr(intri),
+                                                  _lib.ptr(depth), _lib.ptr(cmean), _lib.ptr(_scratch_for(dev, 2 * m)),
+                                                  _lib.cur_stream()), "sta_regress_pairs_finish")
+            maps = (conf, depth, intri, cmean)
+    return pose, pconf, conf_host, keep, maps
+
+
+def regress_frames(sta, pairs, H, W):
+    """The ungated regression of tracked frames: pairs = [(frame feature, keyframe feature), ...] (each (1, N, 1024),
+    one image size H x W) as the edges (i = frame, j = keyframe view), in chunks of at most MAX_EDGES with the padding
+    rule of regress_keyframes_gated_group (every chunk padded to MAX_EDGES when there is more than one), each chunk
+    through regress_pairs with no gate and no read-back.  Returns, over all pairs in order, (pose [F,4,4] of i -> j,
+    pose_conf [F], depth [F,H,W] and conf [F,H,W] of the keyframe side)."""
+    pad = len(pairs) > MAX_EDGES
+    parts = []
+    for c0 in range(0, len(pairs), MAX_EDGES):
+        run = pairs[c0:c0 + MAX_EDGES]
+        n = len(run)
+        run = run + [run[-1]] * ((MAX_EDGES if pad else n) - n)
+        fi = torch.cat([f for f, _ in run], dim=0)
+        fj = torch.cat([k for _, k in run], dim=0)
+        pose, pconf, _, _, (conf, depth, _, _) = regress_pairs(sta, fi, fj, H, W, n)
+        parts.append((pose[0, :n], pconf[0, :n], depth[1], conf[1]))
+    if len(parts) == 1:
+        return parts[0]
+    return tuple(torch.cat(x) for x in zip(*parts))
 
 
 def regress_keyframes_gated_group(items, rel_pose_thres):

@@ -14,6 +14,8 @@ Graph insertion runs once per edge chunk for all sessions (one sta_graph_add_key
 in the order step_many would run them.  `optimize(ks)` runs the PGO of the named sessions now, together: one
 PoseGraphOpt.optimize_group, whose LM iterations step every session's graph with one launch sequence and one
 read-back; `optimize(ks, background=True)` starts the same group on a side stream and returns (INTEGRATION.md §5).
+`track({k: [value, ...]})` gives frames that are not keyframes a pose against
+a keyframe of their session, all sessions' frames through one encode and one regression pass (OnlineSLAM.track).
 With pgo_every beyond the sequence length, an evaluation over a scene list ends with one
 `optimize(range(len(scenes)))`, and a live server runs `optimize` on the sessions that are due.  A call leaves every
 session as `for k in sorted(values): sessions[k].step_many(values[k], force_pgo=k in force_pgo, ...)` would: the
@@ -35,7 +37,7 @@ import torch
 from .keyframe import KeyframeFrontend, add_views_group, regress_keyframes_gated_group
 from .loop_detector import Vocabulary, detect_loops_group
 from .pose_graph import PoseGraphOpt
-from .slam import OnlineSLAM, insert_keyframes
+from .slam import OnlineSLAM, insert_keyframes, track_frames
 
 
 def _share(sessions, key, seconds):
@@ -301,3 +303,17 @@ class SLAMSessions:
             s._pgo_end(p)
         _share(sess, "pgo", time.time() - t)
         torch.cuda.empty_cache()
+
+    def track(self, values, kfs=None):
+        """Track frames in several sessions at once: values = {k: [value, ...], ...} (or (k, [value, ...]) pairs) names
+        any subset of the sessions, kfs = {k: keyframe view} (default: each session's last stepped view).  One
+        transient encode of all frames, one regression whose edge chunks mix sessions, one sta_graph_track_frames per
+        session (slam.track_frames).  Returns {k: result of OnlineSLAM.track}.  Refused with ValueError before any
+        launch, with no session changed: an unknown or repeated session, a kfs entry for a session not in values,
+        frames of different sizes within the call, and every refusal of OnlineSLAM.track."""
+        calls = self._calls(values)
+        kfs = {} if kfs is None else {self._index(k): kf for k, kf in (kfs.items() if hasattr(kfs, "items") else kfs)}
+        if set(kfs) - {k for k, _ in calls}:
+            raise ValueError("kfs names sessions that track no frames: %s" % sorted(set(kfs) - {k for k, _ in calls}))
+        res = track_frames([(self.sessions[k], vs, kfs.get(k)) for k, vs in calls])
+        return {k: r for (k, _), r in zip(calls, res)}

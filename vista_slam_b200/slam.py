@@ -36,10 +36,17 @@ pose_graph_optimize, save_data_all, reset and wait_pgo wait for a pending run (I
 SLAMSessions.step the PGOs that fall due in one call start together as one run (PoseGraphOpt.start_group), and
 SLAMSessions.optimize(ks, background=True) starts one for the named sessions; each session folds its share as above.
 
+`track(values, kf)` gives frames that are not keyframes a pose against a keyframe view without changing the session:
+one transient encode, the keyframe path's regression launches for the pairs (frame, kf) with no gate, and
+sta_graph_track_frames, which composes each pose from the first node of kf as a keyframe with that one edge would get
+it.  frame_trajectory() recomposes every tracked frame on the current graph, so tracked frames follow their keyframes
+through PGOs (track_frames; DESIGN.md §5).
+
 Importing this module does not import pypose, munch, colorama or open3d.  `get_view` returns a `View` (attribute and key
 access, as munch.Munch).  The PLY of save_data_all is written here: binary little-endian, float x y z and uchar
 red green blue (colours rounded from [0, 1]); whether that is byte-identical to open3d's writer is not checked."""
 import ctypes
+import operator
 import os
 import time
 
@@ -49,7 +56,7 @@ from tqdm import tqdm
 
 from . import _lib
 from .flow_tracker import FlowTracker
-from .keyframe import KeyframeFrontend
+from .keyframe import KeyframeFrontend, encode_views, regress_frames
 from .loop_detector import LoopDetector
 from .pose_graph import PoseGraphOpt
 
@@ -169,6 +176,7 @@ class OnlineSLAM:
         self._pgo_run = None  # a background PGO not yet folded: (PoseGraphRun, its problem, nodes to replay)
         self._graph = None  # created at the first keyframe, when the map size is known
         self._kf_queue = []  # keyframe insertions not yet launched (_add_keyframe, insert_keyframes)
+        self._tracked = []  # one record per track call and session (_track_store), in tracking order
         self._reset_host_graph()
 
     @staticmethod
@@ -193,6 +201,7 @@ class OnlineSLAM:
             self._pgo_run[0].wait()
             self._pgo_run = None
         self._kf_queue = []
+        self._tracked = []
         if self._graph is not None:
             with torch.cuda.device(self._graph.device):
                 _lib.check(_lib.lib().sta_graph_reset(self._graph.h, _lib.cur_stream()), "sta_graph_reset")
@@ -667,6 +676,99 @@ class OnlineSLAM:
         time_dict["total"] = sum(time_dict.values())
         return time_dict
 
+    # ------------------------------------------------------------------------------------------------ tracked frames
+    def track(self, values, kf=None):
+        """Poses for frames that are not keyframes: each frame of values (step-style dicts: rgb, shape, view_name; gray
+        is ignored), all of the views' size, is tracked against keyframe view kf (default: the last stepped view),
+        which must have a node.  Returns device tensors {pose [F,4,4] (scale dropped, as get_view), scale [F],
+        pose_conf [F], valid [F] uint8}; no host synchronisation.  See track_frames for the semantics; ValueError,
+        before any launch and with nothing changed, for a frame of another size or a kf out of range or without a
+        node."""
+        return track_frames([(self, list(values), kf)])[0]
+
+    def _track_check(self, values, kf):
+        """The refusals of track for this session; returns the keyframe view."""
+        if self.view_num == 0 or self._graph is None:
+            raise ValueError("nothing to track against: no view has been stepped")
+        kf = self.view_num - 1 if kf is None else operator.index(kf)
+        if not 0 <= kf < self.view_num:
+            raise ValueError("keyframe view %d out of range (%d views)" % (kf, self.view_num))
+        if not self.view_to_node.get(kf):
+            raise ValueError("view %d has no node in the pose graph yet" % kf)
+        size = tuple(self.kf.img_shapes[0])
+        if any(tuple(v["rgb"].shape[-2:]) != size for v in values):
+            raise ValueError("tracked frames must have the size of the session's views %s" % (size,))
+        return kf
+
+    def _track_store(self, kf, names, pose, pconf, depth, conf):
+        """sta_graph_track_frames over this session's frames of a track call (regressed against view kf), recorded for
+        frame_trajectory; returns track's result."""
+        g = self._graph
+        F = len(names)
+        anchor = self.view_to_node[kf][0]
+        dev = g.device
+
+        def f32(*shape):
+            return torch.empty(*shape, dtype=torch.float32, device=dev)
+
+        meas, s_edge, pose_out, scale = f32(F, 8), f32(F), f32(F, 4, 4), f32(F)
+        valid = torch.empty(F, dtype=torch.uint8, device=dev)
+        L, M = _lib.lib(), _lib.GRAPH_MAX_TRACK_FRAMES
+        with torch.cuda.device(dev):
+            for a in range(0, F, M):
+                b = min(F, a + M)
+                need = int(L.sta_graph_track_frames_scratch_bytes(b - a))
+                scratch = torch.empty((need + 7) // 8, dtype=torch.float64, device=dev)
+                _lib.check(L.sta_graph_track_frames(
+                    g.h, b - a, (ctypes.c_int * (b - a))(*[anchor] * (b - a)), _lib.ptr(pose[a:b]), _lib.ptr(depth[a:b]),
+                    _lib.ptr(conf[a:b]), _lib.ptr(meas[a:b]), _lib.ptr(s_edge[a:b]), _lib.ptr(valid[a:b]),
+                    _lib.ptr(pose_out[a:b]), _lib.ptr(scale[a:b]), _lib.ptr(scratch), need, _lib.cur_stream()),
+                    "sta_graph_track_frames")
+        self._tracked.append({"names": list(names), "kf": [kf] * F, "anchor": [anchor] * F, "meas": meas,
+                              "scale_edge": s_edge, "pose_conf": pconf, "valid": valid})
+        return {"pose": pose_out, "scale": scale, "pose_conf": pconf, "valid": valid}
+
+    def frame_trajectory(self):
+        """Every tracked frame, in tracking order, recomposed on the current graph with one sta_graph_frame_poses per
+        GRAPH_MAX_TRACK_FRAMES frames: {names, kf (host lists), pose [F,4,4] (scale dropped), scale [F], pose_conf [F],
+        valid [F]} and the stored values it is composed from: anchor (host list), meas [F,8] (T_fk as [t | q | s]),
+        scale_edge [F].  A background PGO is folded first if it has finished (as get_view); no host synchronisation."""
+        self._pgo_poll()
+        self._insert_queued()
+        recs = self._tracked
+        out = {k: [x for r in recs for x in r[k]] for k in ("names", "kf", "anchor")}
+        dev = self.device if self._graph is None else self._graph.device
+        F = len(out["names"])
+        for k, shape, dt in (("meas", (0, 8), torch.float32), ("scale_edge", (0,), torch.float32),
+                             ("pose_conf", (0,), torch.float32), ("valid", (0,), torch.uint8)):
+            out[k] = torch.cat([r[k] for r in recs]) if recs else torch.empty(shape, dtype=dt, device=dev)
+        out["pose"] = torch.empty(F, 4, 4, dtype=torch.float32, device=dev)
+        out["scale"] = torch.empty(F, dtype=torch.float32, device=dev)
+        L, M = _lib.lib(), _lib.GRAPH_MAX_TRACK_FRAMES
+        with torch.cuda.device(dev):
+            for a in range(0, F, M):
+                b = min(F, a + M)
+                _lib.check(L.sta_graph_frame_poses(
+                    self._graph.h, b - a, (ctypes.c_int * (b - a))(*out["anchor"][a:b]), _lib.ptr(out["meas"][a:b]),
+                    _lib.ptr(out["scale_edge"][a:b]), _lib.ptr(out["pose"][a:b]), _lib.ptr(out["scale"][a:b]),
+                    _lib.cur_stream()), "sta_graph_frame_poses")
+        return out
+
+    def save_frame_trajectory(self, output_folder, traj_name_postfix=None):
+        """frame_trajectory() into output_folder, in save_data_all's style: frame_trajectory{_postfix}.npy [F,4,4],
+        frame_scales{_postfix}.npy [F] and frame_info{_postfix}.npz (names, kf, pose_conf, valid).  A pending
+        background PGO is folded first (wait_pgo), as save_data_all does."""
+        self.wait_pgo()
+        if not os.path.exists(output_folder):
+            os.makedirs(output_folder)
+        t = self.frame_trajectory()
+        postfix = f"_{traj_name_postfix}" if traj_name_postfix is not None else ""
+        np.save(f"{output_folder}/frame_trajectory{postfix}.npy", t["pose"].cpu().numpy())
+        np.save(f"{output_folder}/frame_scales{postfix}.npy", t["scale"].cpu().numpy())
+        np.savez(f"{output_folder}/frame_info{postfix}.npz", names=np.array(t["names"]),
+                 kf=np.array(t["kf"], dtype=np.int64), pose_conf=t["pose_conf"].cpu().numpy(),
+                 valid=t["valid"].cpu().numpy())
+
 
 def insert_keyframes(sessions):
     """Launch the keyframe insertions the sessions have queued (OnlineSLAM._add_keyframe), every session's in its
@@ -688,6 +790,54 @@ def insert_keyframes(sessions):
             scratch = torch.empty((need + 7) // 8, dtype=torch.float64, device=device)
             _lib.check(L.sta_graph_add_keyframes(tab, len(part), _lib.ptr(scratch), need, _lib.cur_stream()),
                        "sta_graph_add_keyframes")
+
+
+def track_frames(calls):
+    """Track frames in several sessions that share one STA: calls = [(session, [value, ...], kf or None), ...].
+    Every refusal comes first (OnlineSLAM._track_check; all frames of the call must have one size), then each session's
+    queued keyframe insertions are launched (the anchors' maps must be in the store), then one transient encode of all
+    frames (encode_views: nothing is cached), one regression of the pairs (frame, kf) in edge chunks that mix sessions
+    (regress_frames: the launches of the keyframe path, no gate, no read-back), and one sta_graph_track_frames per
+    session.  Returns each call's track result, in order.
+
+    Frame f tracked against view k, a = the first node of k: s is the scale edge a new node of k would get from a
+    (estimate_scale_with_depth_and_confidence(depth_k, depth_a, conf_k, conf_a) over the pair's k-side maps), and
+    pose_f = pose[a] * Sim3(0, id, s) * Sim3(T_fk), the pose node i of a keyframe whose first kept edge is (i, k) gets,
+    bit for bit.  No gate: valid = 0 only where T_fk's rotation is not orthonormal (no graph flag is raised).  Nothing
+    of the session changes but its record of tracked frames: not the graph, its host mirror, the views, the encoder
+    cache, the loop detector, the flow tracker or time_dict, and a background PGO is neither polled nor waited for."""
+    calls = [(s, list(vs), kf) for s, vs, kf in calls]
+    kfs = [s._track_check(vs, kf) for s, vs, kf in calls]
+    images = [v["rgb"] for _, vs, _ in calls for v in vs]
+    if any(tuple(x.shape[-2:]) != tuple(images[0].shape[-2:]) for x in images):
+        raise ValueError("all frames of a track call must have the same image size")
+    if any(s.frontend is not calls[0][0].frontend for s, _, _ in calls):
+        raise ValueError("the sessions of a track call must share one STA")
+    for s, _, _ in calls:
+        s._insert_queued()
+    out = []
+    if images:
+        H, W = int(images[0].shape[-2]), int(images[0].shape[-1])
+        feats = encode_views(calls[0][0].frontend, images, [v["shape"] for _, vs, _ in calls for v in vs])
+        pairs = [(f, None) for f in feats]
+        t = 0
+        for (s, vs, _), kf in zip(calls, kfs):
+            for m in range(len(vs)):
+                pairs[t + m] = (feats[t + m], s.kf.enc_features[kf])
+            t += len(vs)
+        pose, pconf, depth, conf = regress_frames(calls[0][0].frontend, pairs, H, W)
+    t = 0
+    for (s, vs, _), kf in zip(calls, kfs):
+        F = len(vs)
+        if F:
+            out.append(s._track_store(kf, [v["view_name"] for v in vs], pose[t:t + F], pconf[t:t + F],
+                                      depth[t:t + F], conf[t:t + F]))
+        else:
+            dev = s._graph.device
+            out.append({"pose": torch.empty(0, 4, 4, device=dev), "scale": torch.empty(0, device=dev),
+                        "pose_conf": torch.empty(0, device=dev), "valid": torch.empty(0, dtype=torch.uint8, device=dev)})
+        t += F
+    return out
 
 
 def write_ply(path, points, colors):
