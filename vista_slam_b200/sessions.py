@@ -11,7 +11,9 @@ keyframes of every named session through one batched frontend pass:
     (keyframe.regress_keyframes_gated_group).
 
 Graph insertion runs once per edge chunk for all sessions (one sta_graph_add_keyframes), and step's PGOs per session,
-in the order step_many would run them.  `optimize(ks)` runs the PGO of the named sessions now, together: one
+in the order step_many would run them.  The keyframe loop is slam.step_keyframes, which OnlineSLAM.step_many runs over
+one session; this class adds the group hooks (detection and regression across sessions, due background PGOs started
+together at the end of the call).  `optimize(ks)` runs the PGO of the named sessions now, together: one
 PoseGraphOpt.optimize_group, whose LM iterations step every session's graph with one launch sequence and one
 read-back; `optimize(ks, background=True)` starts the same group on a side stream and returns (INTEGRATION.md §5).
 `track({k: [value, ...]})` gives frames that are not keyframes a pose against
@@ -34,15 +36,10 @@ import time
 
 import torch
 
-from .keyframe import KeyframeFrontend, add_views_group, regress_keyframes_gated_group
+from .keyframe import regress_keyframes_gated_group
 from .loop_detector import Vocabulary, detect_loops_group
 from .pose_graph import PoseGraphOpt
-from .slam import OnlineSLAM, insert_keyframes, track_frames
-
-
-def _share(sessions, key, seconds):
-    for s in sessions:
-        s.time_dict[key] += seconds / len(sessions)
+from .slam import OnlineSLAM, _share, step_keyframes, track_frames
 
 
 class _Batch:
@@ -169,91 +166,15 @@ class SLAMSessions:
         kept edges of each edge chunk, of every session, go into the graphs with one sta_graph_add_keyframes.  The
         PGOs of sessions with pgo_background that fall due during the call are captured at their keyframes and started
         as one PoseGraphOpt.start_group run at the end of the call (a session due again within the call waits for its
-        run, which starts the group then); every session with a pending PGO is polled after each keyframe."""
+        run, which starts the group then).  Each session of the call is polled before its first keyframe, and every
+        session with a pending PGO after each keyframe (slam.step_keyframes, the loop step_many runs)."""
         calls = self._calls(values)
         force = {self._index(k) for k in force_pgo}
-        flags = {k: [] for k, _ in calls}
-        calls = [(k, vs) for k, vs in calls if vs]
-        if not calls:
-            return flags
-        size = tuple(calls[0][1][0]["rgb"].shape[-2:])
-        for k, vs in calls:
-            if any(tuple(v["rgb"].shape[-2:]) != size for v in vs):
-                raise ValueError("all keyframes of a call must have the same image size")
-            kf = self.sessions[k].kf
-            if kf.img_shapes and tuple(kf.img_shapes[0]) != size:
-                raise ValueError("the keyframes of session %d must have the size of its views" % k)
-        sess = [self.sessions[k] for k, _ in calls]
-        i0 = [s.view_num for s in sess]
-        for s, (_, vs) in zip(sess, calls):
-            t = time.time()
-            s._ensure_graph(vs[0]["rgb"])
-            if s.view_num == 0:
-                s._graph.pose[0].copy_(s._identity)
-            s.time_dict["prepare_data"] += time.time() - t
-
-        t = time.time()
-        add_views_group([s.kf for s in sess], [[v["rgb"] for v in vs] for _, vs in calls],
-                        [[v["shape"] for v in vs] for _, vs in calls])
-        _share(sess, "encoder", time.time() - t)
-
-        fars = [[max(0, i + m - s.neighbor_edge_num) for m in range(len(vs))] for s, i, (_, vs) in zip(sess, i0, calls)]
-        t = time.time()
-        loops = self._detect_loops(sess, [[v["gray"] for v in vs] for _, vs in calls], fars)  # read-back: candidates
-        _share(sess, "lc", time.time() - t)
-        for s in sess:
-            s._check_flags()
-
-        items, owner = [], []
-        for c, (s, i, (_, vs)) in enumerate(zip(sess, i0, calls)):
-            for m in range(len(vs)):
-                items.append((s, i + m, list(range(fars[c][m], i + m)) + [j for j, _ in loops[c][m][:s.loop_edge_num]]))
-                owner.append(c)
-        # the sessions of each item's edge chunk, which share the chunk's regression time
-        part = [[sess[c]] for c in owner]
-        for chunk in KeyframeFrontend.edge_chunks([(i, js) for _, i, js in items]):
-            members = [sess[c] for c in sorted({owner[t] for t in chunk})]
-            for t in chunk:
-                part[t] = members
-
-        chunk_ends = {chunk[-1] for chunk in KeyframeFrontend.edge_chunks([(i, js) for _, i, js in items])}
-        group = _CallGroup()
-        checked = [True] * len(calls)
-        results = iter(self._regress_keyframes(items))
-        try:
-            for t, (s, i, js) in enumerate(items):
-                c = owner[t]
-                k, vs = calls[c]
-                m = i - i0[c]
-                dec_start = time.time()
-                res = next(results)  # the first keyframe of an edge chunk runs the chunk: read-back of its gate
-                dt = time.time() - dec_start
-                _share(part[t], "decoder", dt)
-                _share(part[t], "graph_construction", dt)
-                graph_start = time.time()
-                s._check_flags()
-                s._register_keyframe(vs[m], i, js, res)
-                if js:
-                    checked[c] = checked[c] and not res[1]
-                if t in chunk_ends:  # the chunk's keyframes, of every session, go in with one sta_graph_add_keyframes
-                    insert_keyframes(sess)
-                for p in self.sessions:
-                    if p.pgo_pending:
-                        p._pgo_poll()
-                s.time_dict["graph_construction"] += time.time() - graph_start
-                folder = output_folders.get(k) if output_folders else None
-                flags[k].append(s._pgo_if_due(k in force and m == len(vs) - 1, log_intermediate_results, folder, group))
-                if flags[k][-1] and not s.pgo_background:
-                    checked[c] = s.num_nodes > 0 and s.num_edges > 0
-        finally:  # an exception mid-chunk still leaves every graph as its host bookkeeping says
-            insert_keyframes(sess)
-            group.start()  # the background PGOs that fell due in the call, as one run
-        if not all(checked):
-            torch.cuda.current_stream().synchronize()
-            for s, ok in zip(sess, checked):
-                if not ok:
-                    s._check_flags()
-        return flags
+        folders = [output_folders.get(k) if output_folders else None for k, _ in calls]
+        flags = step_keyframes([(self.sessions[k], vs) for k, vs in calls], [k in force for k, _ in calls],
+                               log_intermediate_results, folders, detect=self._detect_loops,
+                               regress=self._regress_keyframes, group=_CallGroup(), polled=self.sessions)
+        return {k: f for (k, _), f in zip(calls, flags)}
 
     def optimize(self, ks, background=False):
         """Optimise the pose graphs of sessions ks now, together.  Leaves each session as sessions[k].pose_graph_optimize()

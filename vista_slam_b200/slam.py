@@ -26,7 +26,9 @@ of those read-backs and raises ValueError there.
 `step_many(values)` steps through many keyframes of one size in one call, with the graph, the PGO calls and the host
 bookkeeping of calling `step` on each in order.  The frontend work does not depend on the pose graph, so it runs across
 keyframes at real batch sizes: the encoder over up to 41 views per call at 224 x 224, loop detection over all frames of
-the call with one read-back, and the gated edge regression in chunks of up to 16 edges with one read-back each.
+the call with one read-back, and the gated edge regression in chunks of up to 16 edges with one read-back each.  Its
+keyframe loop is step_keyframes, which SLAMSessions.step runs over several sessions; `step` keeps its own
+one-keyframe path, the reference step_many is tested against.
 
 `pgo_background = True` (default False) runs each due PGO on a side stream while step goes on (PoseGraphOpt.start):
 step and step_many poll it at every keyframe without waiting, and fold it when it is done -- its poses written, the
@@ -56,7 +58,7 @@ from tqdm import tqdm
 
 from . import _lib
 from .flow_tracker import FlowTracker
-from .keyframe import KeyframeFrontend, encode_views, regress_frames
+from .keyframe import KeyframeFrontend, add_views_group, encode_views, regress_frames
 from .loop_detector import LoopDetector
 from .pose_graph import PoseGraphOpt
 
@@ -436,63 +438,12 @@ class OnlineSLAM:
         views of the call.  A non-orthonormal rotation raises ValueError by the end of the call.
 
         Host synchronisations: one for the loop candidates, one per edge chunk, one per PGO iteration, and one at the
-        end of the call unless a PGO ran last (reading the rotation flag)."""
-        values = list(values)
-        if not values:
-            return []
-        prepare_start = time.time()
-        images = [v["rgb"] for v in values]
-        size = tuple(images[0].shape[-2:])
-        if any(tuple(x.shape[-2:]) != size for x in images):
-            raise ValueError("all keyframes of a step_many call must have the same image size")
-        if self.kf.img_shapes and tuple(self.kf.img_shapes[0]) != size:
-            raise ValueError("the keyframes must have the size of the views already in the graph")
-        i0 = self.view_num
-        n = len(values)
-        self._ensure_graph(images[0])
-        if i0 == 0:
-            self._graph.pose[0].copy_(self._identity)
-        self._pgo_poll()
-        self.time_dict["prepare_data"] += time.time() - prepare_start
-
-        enc_start = time.time()
-        self.kf.add_views(images, [v["shape"] for v in values])
-        self.time_dict["encoder"] += time.time() - enc_start
-
-        far = [max(0, i0 + k - self.neighbor_edge_num) for k in range(n)]
-        loop_start = time.time()
-        loops = self.lc_detector.detect_loops([v["gray"] for v in values], far)  # read-back: candidates
-        self.time_dict["lc"] += time.time() - loop_start
-        self._check_flags()
-
-        items = [(i0 + k, list(range(far[k], i0 + k)) + [j for j, _ in loops[k][:self.loop_edge_num]]) for k in range(n)]
-        chunk_ends = {c[-1] for c in KeyframeFrontend.edge_chunks(items)}
-        flags = []
-        checked = True
-        results = iter(self._regress_keyframes(items))
-        try:
-            for k, (v, (i, js)) in enumerate(zip(values, items)):
-                graph_start = time.time()
-                dec_start = time.time()
-                res = next(results)  # the first keyframe of an edge chunk runs the chunk: read-back of its gate
-                self.time_dict["decoder"] += time.time() - dec_start
-                self._check_flags()
-                self._register_keyframe(v, i, js, res)
-                if js:
-                    checked = checked and not res[1]
-                if k in chunk_ends:  # the chunk's keyframes go in with one sta_graph_add_keyframes
-                    self._insert_queued()
-                self._pgo_poll()
-                self.time_dict["graph_construction"] += time.time() - graph_start
-                flags.append(self._pgo_if_due(force_pgo and k == n - 1, log_intermediate_results, output_folder))
-                if flags[-1] and not self.pgo_background:  # a synchronous PGO's read-backs waited for the graph launches
-                    checked = self.num_nodes > 0 and self.num_edges > 0
-        finally:  # an exception mid-chunk still leaves the graph as the host bookkeeping says
-            self._insert_queued()
-        if not checked:
-            torch.cuda.current_stream().synchronize()
-            self._check_flags()
-        return flags
+        end of the call unless a PGO ran last (reading the rotation flag).  This is step_keyframes over this session
+        alone; a background PGO that falls due starts at its keyframe."""
+        return step_keyframes([(self, list(values))], [force_pgo], log_intermediate_results, [output_folder],
+                              detect=lambda sessions, grays, fars: [self.lc_detector.detect_loops(grays[0], fars[0])],
+                              regress=lambda items: self._regress_keyframes([(i, js) for _, i, js in items]),
+                              group=None, polled=[self])[0]
 
     def _register_keyframe(self, v, i, js, res):
         """Keyframe i of step_many after its gate: the view's host lists, then its kept edges (_insert_keyframe)."""
@@ -790,6 +741,103 @@ def insert_keyframes(sessions):
             scratch = torch.empty((need + 7) // 8, dtype=torch.float64, device=device)
             _lib.check(L.sta_graph_add_keyframes(tab, len(part), _lib.ptr(scratch), need, _lib.cur_stream()),
                        "sta_graph_add_keyframes")
+
+
+def _share(sessions, key, seconds):
+    for s in sessions:
+        s.time_dict[key] += seconds / len(sessions)
+
+
+def step_keyframes(calls, force, log_intermediate_results, output_folders, *, detect, regress, group, polled):
+    """The keyframe loop of OnlineSLAM.step_many and SLAMSessions.step, over distinct sessions that share one STA:
+    calls = [(session, [value, ...]), ...], force[c] whether call c's last keyframe forces a PGO, output_folders[c] its
+    folder for log_intermediate_results.  Returns each call's is_optimized flags ([] for a call without keyframes).
+
+    The callers differ only in these arguments: detect(sessions, grays, fars) gives each session's loop candidates with
+    one read-back; regress([(session, i, js), ...]) yields, per keyframe, what OnlineSLAM._regress_keyframe returns or
+    None; a due background PGO is captured into `group`, which starts it with the others at the end of the call, or is
+    started at its keyframe when group is None; `polled` are the sessions polled after every keyframe (each session of
+    the call is also polled before its first).  Order, refusals, host synchronisations and time buckets: see
+    SLAMSessions.step and the sessions module."""
+    flags = [[] for _ in calls]
+    live = [(s, vs, f, d, out) for (s, vs), f, d, out in zip(calls, force, output_folders, flags) if vs]
+    if not live:
+        return flags
+    sess, vals, force, folders, out = zip(*live)
+    size = tuple(vals[0][0]["rgb"].shape[-2:])
+    for s, vs in zip(sess, vals):
+        if any(tuple(v["rgb"].shape[-2:]) != size for v in vs):
+            raise ValueError("all keyframes of a call must have the same image size")
+        if s.kf.img_shapes and tuple(s.kf.img_shapes[0]) != size:
+            raise ValueError("the keyframes of a session must have the size of its views %s" % (s.kf.img_shapes[0],))
+    i0 = [s.view_num for s in sess]
+    for s, vs in zip(sess, vals):
+        t = time.time()
+        s._ensure_graph(vs[0]["rgb"])
+        if s.view_num == 0:
+            s._graph.pose[0].copy_(s._identity)  # slam.py:251-253
+        s._pgo_poll()
+        s.time_dict["prepare_data"] += time.time() - t
+
+    t = time.time()
+    add_views_group([s.kf for s in sess], [[v["rgb"] for v in vs] for vs in vals],
+                    [[v["shape"] for v in vs] for vs in vals])
+    _share(sess, "encoder", time.time() - t)
+
+    fars = [[max(0, i + m - s.neighbor_edge_num) for m in range(len(vs))] for s, i, vs in zip(sess, i0, vals)]
+    t = time.time()
+    loops = detect(sess, [[v["gray"] for v in vs] for vs in vals], fars)  # read-back: candidates
+    _share(sess, "lc", time.time() - t)
+    for s in sess:
+        s._check_flags()
+
+    items, owner = [], []
+    for c, (s, i, vs) in enumerate(zip(sess, i0, vals)):
+        for m in range(len(vs)):
+            items.append((s, i + m, list(range(fars[c][m], i + m)) + [j for j, _ in loops[c][m][:s.loop_edge_num]]))
+            owner.append(c)
+    chunks = KeyframeFrontend.edge_chunks([(i, js) for _, i, js in items])
+    part = [[sess[c]] for c in owner]  # the sessions of each item's edge chunk, which share the chunk's regression time
+    for chunk in chunks:
+        members = [sess[c] for c in sorted({owner[t] for t in chunk})]
+        for t in chunk:
+            part[t] = members
+    chunk_ends = {chunk[-1] for chunk in chunks}
+    checked = [True] * len(sess)
+    results = iter(regress(items))
+    try:
+        for t, (s, i, js) in enumerate(items):
+            c = owner[t]
+            m = i - i0[c]
+            dec_start = time.time()
+            res = next(results)  # the first keyframe of an edge chunk runs the chunk: read-back of its gate
+            dt = time.time() - dec_start
+            _share(part[t], "decoder", dt)
+            _share(part[t], "graph_construction", dt)
+            graph_start = time.time()
+            s._check_flags()
+            s._register_keyframe(vals[c][m], i, js, res)
+            if js:
+                checked[c] = checked[c] and not res[1]
+            if t in chunk_ends:  # the chunk's keyframes, of every session, go in with one sta_graph_add_keyframes
+                insert_keyframes(sess)
+            for p in polled:
+                p._pgo_poll()
+            s.time_dict["graph_construction"] += time.time() - graph_start
+            last = m == len(vals[c]) - 1
+            out[c].append(s._pgo_if_due(force[c] and last, log_intermediate_results, folders[c], group))
+            if out[c][-1] and not s.pgo_background:  # a synchronous PGO's read-backs waited for the graph launches
+                checked[c] = s.num_nodes > 0 and s.num_edges > 0
+    finally:  # an exception mid-chunk still leaves every graph as its host bookkeeping says
+        insert_keyframes(sess)
+        if group is not None:
+            group.start()  # the background PGOs that fell due in the call, as one run
+    if not all(checked):
+        torch.cuda.current_stream().synchronize()
+        for s, ok in zip(sess, checked):
+            if not ok:
+                s._check_flags()
+    return flags
 
 
 def track_frames(calls):
