@@ -222,9 +222,6 @@ int sta_op_patch_im2col(const void* img, int img_is_bf16, int B, int H, int W, v
 int sta_op_upsample2x(const void* in_bf16, void* out_bf16, int nimg, int H, int W, int C, void* stream);
 int sta_op_im2col_3x3_s2(const void* in_bf16, void* out_bf16, int nimg, int H, int W, int C, void* stream);
 int sta_op_cast_f32_bf16(const float* in, void* out_bf16, int64_t rows, int C, int drop_first_of, void* stream);
-/* In-place 2-D RoPE on tokens [B][N][H][64] bf16 with int64 positions [B][N][2]: the contract of
- * curope.rope_2d (pos_embed/curope/curope.cpp:49-65, kernels.cu:84-108), base 100, F0 = 1. */
-int sta_op_rope2d(void* tokens_bf16, const int64_t* pos, int B, int N, int H, void* stream);
 
 
 /* ---- keyframe step (SURVEY.md 8(f) rank 1): OnlineSLAM.regress_two_views (vista_slam/slam.py:153-189) for K edges

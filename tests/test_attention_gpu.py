@@ -185,7 +185,8 @@ _CASES += [
     ("wide_heads2to5_ldo_pad", 2, 4, 200, 200, 1, _wide, None),
     ("k_v_apart", 3, 2, 300, 129, 2, _apart, None),
 ]
-# every shape of tools/bringup.py::group_attention
+# both query-tile sizes with ragged last query and key tiles, cross-sample K / V (shift), a single row; and the
+# online-softmax rescale under growing row maxima, at 64-row (3 heads) and 128-row tiles (16 heads)
 _CASES += [("bringup_b%d_h%d_n%d_s%d" % (b, h, n, s), b, h, n, n, s, _self, None)
            for b, h, n, s in ((2, 3, 128, 0), (2, 3, 196, 0), (2, 12, 769, 0), (4, 12, 769, 2), (3, 16, 768, 0),
                               (2, 12, 197, 0), (2, 3, 130, 0), (2, 3, 257, 1), (3, 2, 1, 0), (2, 2, 901, 1))]

@@ -12,7 +12,7 @@ import torch
 
 pytestmark = pytest.mark.gpu
 
-import tools.bringup as bu  # noqa: E402  (descriptor helpers)
+from test_layers_gpu import gemm_desc, run_gemm  # noqa: E402
 from vista_slam_b200._lib import EPI_BF16, EPI_F32, EPI_GELU, EPI_ROPE  # noqa: E402
 
 DEV = "cuda"
@@ -42,8 +42,8 @@ def _run(epi, M, N, K, tile_n, seed, f32_in_place=True, relu=0, bias=True):
         out = torch.full((M + PAD_ROWS, ldo), float("nan"), device=DEV, dtype=torch.bfloat16)
     if epi == EPI_ROPE:
         kw.update(pos=pos, rope_cols=2 * N // 3)
-    bu.run_gemm(bu.gemm_desc(epi=epi, A=A, lda=K, W=W, ldw=K, M=M, N=N, K=K, bias=b, out=out, ldo=ldo,
-                             relu_main=relu, tile_n=tile_n, **kw))
+    run_gemm(gemm_desc(epi=epi, A=A, lda=K, W=W, ldw=K, M=M, N=N, K=K, bias=b, out=out, ldo=ldo,
+                       relu_main=relu, tile_n=tile_n, **kw))
     torch.cuda.synchronize()
     return out
 

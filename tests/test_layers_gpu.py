@@ -1,9 +1,11 @@
 """GPU: every bf16 GEMM and implicit-GEMM convolution launch the model makes, at the model's shapes, against float64 with a
 bound on every output element, against planted integer answers bit for bit, and with NaN canaries around every output;
-plus the DPT's bandwidth kernels (bilinear upsample, stride-2 im2col, LayerNorm, fp32 -> bf16 cast) at the same sizes.
+plus the bandwidth kernels (patch im2col, bilinear upsample, stride-2 im2col, LayerNorm, fp32 -> bf16 cast) at the same
+sizes.
 
 The launch list is layer_catalogue(): it restates run_encoder (runtime.cu:892-920), run_decoder (runtime.cu:927-1002) and
 run_dpt (runtime.cu:1029-1106) one launch at a time.  A layer added to runtime.cu gets its line there.
+off_model_layers() runs the same checks on launches the model does not make: other shapes and epilogue combinations.
 
 Float64 check.  Random operands (weights scaled by 1/sqrt(K) as the model's are), the reference is the float64 product of
 exactly the bf16 operands the kernel reads (cuBLAS DGEMM; convolutions as F.unfold + matmul).  Per element:
@@ -49,12 +51,14 @@ from vista_slam_b200._lib import EPI_BF16, EPI_F32, EPI_GELU, EPI_HEAD, EPI_PIXS
 pytestmark = pytest.mark.gpu
 
 TAU_STEP = 2.0 ** -22
-# Largest err / bound of the float64 checks, H100 80GB HBM3 (700 W power limit), all three sizes:
-#   fp32-output layers, where the tau term dominates: 0.027 (dec.proj at cfg-2), so tau is a worst case ~37x above what
-#   the tensor cores show on random operands;
+# Largest err / bound of the float64 checks, H100 80GB HBM3 (700 W power limit), all three sizes and the off-model
+# layers:
+#   fp32-output layers, where the tau term dominates: 0.027 in the catalogue (dec.proj at cfg-2), 0.042 off the model
+#   (f32_inplace_M24576_N1024_K256): tau grows with K / 16 while random roundings grow with its square root, so K = 256
+#   comes closest; tau is a worst case ~24x above what the tensor cores show on random operands;
 #   bf16 outputs: 0.994 -- the output rounding, which u_out = 2^-8 covers exactly, with little room left;
 #   x3: 0.27; EPI_HEAD: 0.0017; planted EPI_HEAD against its 2^-20 post-process bound: 0.18.
-MEASURED_RATIO = {"f32_out": 0.027, "bf16_out": 0.994, "x3": 0.27, "head": 0.0017, "head_planted": 0.18}
+MEASURED_RATIO = {"f32_out": 0.042, "bf16_out": 0.994, "x3": 0.27, "head": 0.0017, "head_planted": 0.18}
 GELU_SLOPE = 1.1289
 SPLITK_BYTES = 48 << 20  # StaModel::kSplitKBytes (runtime.cu): the model's split-K workspace
 
@@ -76,15 +80,17 @@ class Layer:
     K: int = 0                # logical reduction length
     conv: tuple = None        # (nimg, H, W, Cin): 3x3 implicit-GEMM convolution, padding 1
     bias: bool = True
-    resid: str = ""           # "" | "inplace" (fp32 residual stream, out += ...) | "skip" (bf16 skip tensor)
+    resid: str = ""           # "" | "inplace" (fp32 residual stream, out += ...) | "skip" (a tensor of the out type)
     resid2: bool = False
     relu_main: int = 0
     relu_copy: bool = False
     rope_cols: int = 0
     pos_grid: tuple = None    # RoPE positions: (samples, h, w, with_pose_token) as launch_make_positions builds them
+    pos_rand: int = 0         # RoPE positions without a grid: uniform in [-1, pos_rand) on each axis
     rowmap_n: int = 0
     ps: tuple = None          # EPI_PIXSHUF: (k, cout, nimg, h, w)
     taps: int = 1             # K = taps x channels (act3c reads stride-2 im2col rows): x3 splits each tap
+    splitk: bool = True       # pass the model's split-K workspace
 
 
 def layer_catalogue(h, w, nimg, pairs, dpt_nimg):
@@ -139,6 +145,53 @@ def layer_catalogue(h, w, nimg, pairs, dpt_nimg):
     L += [Layer("dpt.head.0", EPI_BF16, N=128, K=2304, conv=(m, 8 * h, 8 * w, 256)),
           Layer("dpt.head.2", EPI_HEAD, N=128, K=1152, conv=(m, 16 * h, 16 * w, 128))]
     return L
+
+
+def off_model_layers():
+    """sta_op_gemm launches the model does not make: ragged and other shapes, tile counts from one CTA to many waves,
+    epilogue combinations the catalogue lacks (two skip tensors on a linear layer, relu on a linear layer's output, an
+    fp32 output with its own skip tensor, the in-place fp32 update without a split-K workspace), RoPE at random
+    positions, partly past the shared-memory table, and small convolutions, pixel shuffles and a head."""
+    L = [Layer("linear_M%d_N%d_K%d" % s, EPI_BF16, *s)
+         for s in ((128, 256, 64), (300, 512, 192), (128, 256, 1024), (8192, 1024, 1024), (1000, 384, 768),
+                   (24608, 768, 768), (777, 512, 256), (4096, 768, 768), (300, 384, 192))]
+    L += [Layer("f32_inplace_M%d_N%d_K%d" % s, EPI_F32, *s, resid="inplace")
+          for s in ((777, 512, 256), (4096, 768, 768), (300, 384, 192), (777, 320, 256), (5000, 1024, 256),
+                    (24576, 1024, 256))]
+    L += [Layer("f32_inplace_M196_N1024_K1024_no_splitk_ws", EPI_F32, 196, 1024, 1024, resid="inplace", splitk=False),
+          Layer("f32_M777_N512_K256", EPI_F32, 777, 512, 256),
+          Layer("f32_M196_N1024_K1024", EPI_F32, 196, 1024, 1024),
+          Layer("f32_skip_M777_N512_K256", EPI_F32, 777, 512, 256, resid="skip"),
+          Layer("f32_rowmap_7x111_N512_K256", EPI_F32, 777, 512, 256, rowmap_n=111),
+          Layer("skip2_relu_copy_M777_N512_K256", EPI_BF16, 777, 512, 256, resid="skip", resid2=True, relu_copy=True),
+          Layer("skip2_relu_copy_M500_N256_K256", EPI_BF16, 500, 256, 256, resid="skip", resid2=True, relu_copy=True),
+          Layer("relu_main_M777_N512_K256", EPI_BF16, 777, 512, 256, relu_main=1),
+          Layer("no_bias_M777_N384_K256", EPI_BF16, 777, 384, 256, bias=False),
+          Layer("gelu_M777_N512_K256", EPI_GELU, 777, 512, 256),
+          Layer("gelu_M4096_N768_K768", EPI_GELU, 4096, 768, 768),
+          Layer("gelu_M196_N1024_K1024", EPI_GELU, 196, 1024, 1024),
+          Layer("gelu_M5000_N1024_K256", EPI_GELU, 5000, 1024, 256),
+          Layer("rope_M777_N768_K256", EPI_ROPE, 777, 768, 256, rope_cols=512, pos_rand=40),
+          Layer("rope_M500_N768_K256", EPI_ROPE, 500, 768, 256, rope_cols=512, pos_rand=70),
+          Layer("rope_M196_N1024_K1024", EPI_ROPE, 196, 1024, 1024, rope_cols=768, pos_rand=14),
+          Layer("rope_M5000_N1024_K256", EPI_ROPE, 5000, 1024, 256, rope_cols=768, pos_rand=70),
+          Layer("pixshuf_k2_C128_64_2x5x7", EPI_PIXSHUF, 70, 256, 128, ps=(2, 64, 2, 5, 7)),
+          Layer("pixshuf_k2_C192_192_2x6x10", EPI_PIXSHUF, 120, 768, 192, ps=(2, 192, 2, 6, 10))]
+    L += [Layer("conv_%dx%dx%d_C%d_%d_skip_relu_copy" % g, EPI_BF16, N=g[4], K=9 * g[3], conv=g[:4], resid="skip",
+                relu_copy=True)
+          for g in ((2, 8, 16, 64, 256), (3, 14, 14, 128, 256), (2, 24, 32, 256, 256), (1, 20, 36, 256, 128))]
+    L += [Layer("conv_2x14x18_C128_256_skip", EPI_BF16, N=256, K=1152, conv=(2, 14, 18, 128), resid="skip"),
+          Layer("conv_2x14x18_C256_256_no_bias_relu_main", EPI_BF16, N=256, K=2304, conv=(2, 14, 18, 256), bias=False,
+                relu_main=1),
+          Layer("head_2x32x48", EPI_HEAD, N=128, K=1152, conv=(2, 32, 48, 128))]
+    return L
+
+
+# the off-model layers also checked in the split-precision (x3) parity mode
+OFF_MODEL_X3 = {"linear_M777_N512_K256", "linear_M4096_N768_K768", "linear_M300_N384_K192",
+                "f32_inplace_M777_N512_K256", "f32_inplace_M4096_N768_K768", "f32_inplace_M300_N384_K192",
+                "skip2_relu_copy_M500_N256_K256", "gelu_M777_N512_K256", "gelu_M4096_N768_K768", "rope_M500_N768_K256",
+                "pixshuf_k2_C192_192_2x6x10", "conv_2x14x18_C128_256_skip"}
 
 
 # (id, h, w, trunk images, pairs, DPT images, x3 checked)
@@ -357,7 +410,9 @@ def make_operands(e, kind, seed, dev="cuda"):
             o["head_w"] = torch.randn(4, 128, generator=g, device=dev) / math.sqrt(128)
             o["head_b"] = torch.randn(4, generator=g, device=dev) * 0.1
     if e.rope_cols:
-        o["pos"] = (torch.zeros(e.M, 2, dtype=torch.int32, device=dev) if planted else positions(e.pos_grid, dev))
+        o["pos"] = (torch.zeros(e.M, 2, dtype=torch.int32, device=dev) if planted else
+                    positions(e.pos_grid, dev) if e.pos_grid else
+                    torch.randint(-1, e.pos_rand, (e.M, 2), generator=g, device=dev, dtype=torch.int32))
     return o
 
 
@@ -390,6 +445,19 @@ def _bits(t):
     return t.view(torch.int16) if t.element_size() == 2 else t.view(torch.int32)
 
 
+def gemm_desc(**kw):
+    """StaGemmDesc with the given fields; tensors stand for their data pointers"""
+    d = StaGemmDesc()
+    for k, v in kw.items():
+        setattr(d, k, v.data_ptr() if isinstance(v, torch.Tensor) else v)
+    return d
+
+
+def run_gemm(d, what="sta_op_gemm"):
+    from vista_slam_b200._lib import check, cur_stream, lib
+    check(lib().sta_op_gemm(ctypes.byref(d), cur_stream()), what)
+
+
 def run_layer(e, o, split):
     """Launch layer e on the physical form of operands o (bf16, or the x3 layout when split).  Every output sits in a
     NaN-filled buffer with trailing rows / a trailing image and padding columns; the unaddressed part must keep its
@@ -408,7 +476,8 @@ def run_layer(e, o, split):
     d.W, d.ldw = Wp.data_ptr(), Kp
     d.N, d.K = e.N, Kp
     d.split_precision = int(split)
-    d.splitk_ws, d.splitk_ws_bytes = _splitk_ws().data_ptr(), SPLITK_BYTES
+    if e.splitk:
+        d.splitk_ws, d.splitk_ws_bytes = _splitk_ws().data_ptr(), SPLITK_BYTES
     keep = [A, Wp]
     if conv:
         nimg, H, W, Cin = e.conv
@@ -466,8 +535,8 @@ def run_layer(e, o, split):
         checks.append((out, out.clone(), mo))
         for key in ("resid", "resid2"):
             if key in o and e.resid == "skip":
-                s = _nan(shape, torch.bfloat16)
-                s[addr] = _phys(o[key], split)
+                s = _nan(shape, out.dtype)
+                s[addr] = o[key] if f32 else _phys(o[key], split)
                 keep.append(s)
                 setattr(d, key, s.data_ptr())
                 o[key + "_phys"] = s[addr]
@@ -479,8 +548,7 @@ def run_layer(e, o, split):
         d.rowmap_n = e.rowmap_n
     if e.rope_cols:
         d.pos, d.rope_cols = o["pos"].data_ptr(), e.rope_cols
-    from vista_slam_b200._lib import check, cur_stream, lib
-    check(lib().sta_op_gemm(ctypes.byref(d), cur_stream()), "sta_op_gemm " + e.name)
+    run_gemm(d, "sta_op_gemm " + e.name)
     torch.cuda.synchronize()
     for buf, before, mask in checks:
         assert torch.equal(_bits(buf)[~mask], _bits(before)[~mask]), "%s: wrote outside the addressed output" % e.name
@@ -581,9 +649,10 @@ def reference(e, o, A, Wp, split, images=None):
 # ---------------------------------------------------------------------------------------------------------------------
 
 def _cases(x3_only):
-    return [pytest.param(sid, e, id="%s-%s" % (sid, e.name))
-            for sid, h, w, nimg, pairs, dn, x3 in SIZES if x3 or not x3_only
-            for e in layer_catalogue(h, w, nimg, pairs, dn)]
+    cases = [(sid, e) for sid, h, w, nimg, pairs, dn, x3 in SIZES if x3 or not x3_only
+             for e in layer_catalogue(h, w, nimg, pairs, dn)]
+    cases += [("off_model", e) for e in off_model_layers() if e.name in OFF_MODEL_X3 or not x3_only]
+    return [pytest.param(sid, e, id="%s-%s" % (sid, e.name)) for sid, e in cases]
 
 
 def _seed(sid, e, salt):
@@ -659,6 +728,8 @@ def _upsample_shapes():
         out += [(sid, dn, h, w, 256), (sid, dn, 2 * h, 2 * w, 256), (sid, dn, 4 * h, 4 * w, 256),
                 (sid, dn, 8 * h, 8 * w, 128)]
     out += [("ragged", 2, 5, 33, 256), ("ragged", 1, 3, 37, 128), ("ragged", 2, 1, 1, 256)]
+    out += [("off_model", 2, 7, 9, 64), ("off_model", 1, 12, 16, 256), ("off_model", 3, 5, 3, 128),
+            ("off_model", 2, 24, 32, 128), ("off_model", 1, 1, 40, 64)]
     return out
 
 
@@ -688,7 +759,7 @@ def test_upsample2x_within_float64_bound(sid, nimg, H, W, C):
 
 
 @pytest.mark.parametrize("nimg,H,W,C", [(1, 14, 14, 768), (2, 3, 5, 768), (16, 24, 32, 768), (2, 7, 9, 768),
-                                        (2, 3, 5, 2304), (1, 1, 1, 768)])
+                                        (2, 3, 5, 2304), (1, 1, 1, 768), (2, 7, 10, 64)])
 def test_im2col_3x3_s2_is_exact(nimg, H, W, C):
     """act3c's input: a pure copy of channel vectors, so it must equal the unfold of the input exactly"""
     from vista_slam_b200._lib import check, cur_stream, lib
@@ -705,6 +776,28 @@ def test_im2col_3x3_s2_is_exact(nimg, H, W, C):
     check_exact("im2col s2 %dx%dx%dx%d" % (nimg, H, W, C), out[:rows], conv_cols(x, stride=2))
 
 
+@pytest.mark.parametrize("src", ["fp32", "bf16"])
+@pytest.mark.parametrize("sid,B,H,W", [(sid, nimg, 16 * h, 16 * w) for sid, h, w, nimg, _, _, _ in SIZES] +
+                         [("off_model", 2, 32, 48)])
+def test_patch_im2col_is_exact(sid, B, H, W, src):
+    """patch_embed's input: the 16 x 16 patches of a [B][3][H][W] image as rows [B h w][768] in F.unfold's (c, ky, kx)
+    order.  A bf16 image is copied exactly, an fp32 one rounded to the nearest bf16."""
+    from vista_slam_b200._lib import check, cur_stream, lib
+    g = torch.Generator(device="cuda").manual_seed(B * H + W)
+    img = torch.rand(B, 3, H, W, generator=g, device="cuda") * 2 - 1
+    if src == "bf16":
+        img = img.bfloat16()
+    rows = B * (H // 16) * (W // 16)
+    out = _nan((rows + 3, 768), torch.bfloat16)
+    before = out.clone()
+    check(lib().sta_op_patch_im2col(ctypes.c_void_p(img.data_ptr()), int(src == "bf16"), B, H, W,
+                                    ctypes.c_void_p(out.data_ptr()), cur_stream()))
+    torch.cuda.synchronize()
+    assert torch.equal(_bits(out[rows:]), _bits(before[rows:]))
+    want = F.unfold(img.float(), 16, stride=16).transpose(1, 2).reshape(-1, 768).bfloat16()
+    assert torch.equal(_bits(out[:rows]), _bits(want))
+
+
 def _ln_cases():
     out = []
     for sid, h, w, nimg, pairs, dn, _ in SIZES:
@@ -712,7 +805,7 @@ def _ln_cases():
         S = 2 * pairs
         out += [(sid + "-enc", nimg * n, 1024, "single", 0), (sid + "-dec_norm1|norm_y", S * (n + 1), 768, "dual", 0),
                 (sid + "-dec_norm_drop_pose", S * (n + 1), 768, "single", n + 1)]
-    return out
+    return out + [("off_model-dual_C1024", 1000, 1024, "dual", 0)]
 
 
 @pytest.mark.parametrize("sid,rows,C,form,drop", _ln_cases())

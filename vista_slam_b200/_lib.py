@@ -144,7 +144,6 @@ def lib():
     L.sta_op_upsample2x.argtypes = [vp, vp, i, i, i, i, vp]
     L.sta_op_im2col_3x3_s2.argtypes = [vp, vp, i, i, i, i, vp]
     L.sta_op_cast_f32_bf16.argtypes = [vp, vp, i64, i, i, vp]
-    L.sta_op_rope2d.argtypes = [vp, vp, i, i, i, vp]
     L.sta_preprocess_shape.argtypes = [i, i, i, i, i, i, POINTER(c_int)]
     L.sta_preprocess_geometry.argtypes = [i, i, i, i, i, i, POINTER(c_int)]
     L.sta_preprocess_coeffs.argtypes = [i, i, POINTER(c_int), POINTER(c_int), POINTER(c_int), i64]

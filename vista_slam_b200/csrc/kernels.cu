@@ -780,50 +780,6 @@ int launch_pose_head(const float* x, long long sample_stride, int samples, int a
 }
 
 // ---------------------------------------------------------------------------
-// Stand-alone in-place 2-D RoPE on tokens [B][N][H][64] bf16 with int64 positions
-// [B][N][2]: the contract of curope.rope_2d (curope/curope.cpp:49-65, kernels.cu:17-108).
-// The model itself never launches this: RoPE is fused into the QKV GEMM epilogue.
-// One thread rotates one (token, head, axis) group of 32 features.
-// ---------------------------------------------------------------------------
-__global__ void __launch_bounds__(256)
-rope2d_kernel(__nv_bfloat16* __restrict__ tok, const long long* __restrict__ pos, long long ntok, int H,
-              const float* __restrict__ tab, int max_pos) {
-  const long long idx = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
-  if (idx >= ntok * H * 2) return;
-  const int axis = static_cast<int>(idx & 1);
-  const long long th = idx >> 1;
-  const long long t = th / H;
-  const long long p = pos[2 * t + axis];
-  if (p < -1 || p > max_pos) device_fatal("token position outside the RoPE table");
-  __nv_bfloat16* v = tok + th * 64 + axis * 32;
-  const float2* tb = reinterpret_cast<const float2*>(tab) + (p + 1) * 16;
-  float u[32];
-#pragma unroll
-  for (int i = 0; i < 32; ++i) u[i] = __bfloat162float(v[i]);
-#pragma unroll
-  for (int i = 0; i < 16; ++i) {
-    const float2 cs = __ldg(tb + i);
-    v[i] = __float2bfloat16(u[i] * cs.x - u[i + 16] * cs.y);
-    v[i + 16] = __float2bfloat16(u[i + 16] * cs.x + u[i] * cs.y);
-  }
-}
-const float* rope_table(int* max_pos);
-int launch_rope2d(bf16* tokens, const long long* pos, int B, int N, int H, cudaStream_t stream) {
-  int max_pos = 0;
-  const float* tab = rope_table(&max_pos);
-  if (!tab) {
-    set_last_error("failed to build the RoPE table");
-    return 1;
-  }
-  const long long total = static_cast<long long>(B) * N * H * 2;
-  if (total == 0) return 0;
-  rope2d_kernel<<<static_cast<int>((total + 255) / 256), 256, 0, stream>>>(tokens, pos, static_cast<long long>(B) * N, H,
-                                                                           tab, max_pos);
-  STA_CHECK_CUDA(cudaGetLastError());
-  return 0;
-}
-
-// ---------------------------------------------------------------------------
 // RoPE table: tab[(pos + 1) * 16 + i] = (cos, sin)(pos * 100^(-i/16)), pos in [-1, 1023]
 // (pos_embed.py:128-146 with base = 100, F0 = 1, D/4 = 16 frequencies per axis).
 // Built once per device in fp32 exactly like the reference (inv_freq = 1 / base^(i/16)).

@@ -67,7 +67,6 @@ int launch_fill_pose_token(float* x, const float* tok, int samples, int tokens_p
                            cudaStream_t stream);
 int launch_upsample2x(const bf16* in, bf16* out, int nimg, int H, int W, int C, int OH, int OW, cudaStream_t stream,
                       int split = 0);
-int launch_rope2d(bf16* tokens, const long long* pos, int B, int N, int H, cudaStream_t stream);
 // preprocess.cu: SLAM_image_only.process_image on the device (PIL-exact Lanczos resize + ToTensor/Normalize/Grayscale),
 // F same-size frames per launch pair
 int launch_preprocess_rgb8(const uint8_t* rgb_dev, int F, int H, int W, int res_w, int res_h, int w_edge, int h_edge,

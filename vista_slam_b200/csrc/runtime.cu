@@ -1901,10 +1901,6 @@ int sta_op_cast_f32_bf16(const float* in, void* out_bf16, int64_t rows, int C, i
   return launch_cast_f32_bf16(in, static_cast<bf16*>(out_bf16), rows, C, drop_first_of,
                               static_cast<cudaStream_t>(stream));
 }
-int sta_op_rope2d(void* tokens_bf16, const int64_t* pos, int B, int N, int H, void* stream) {
-  return launch_rope2d(static_cast<bf16*>(tokens_bf16), reinterpret_cast<const long long*>(pos), B, N, H,
-                       static_cast<cudaStream_t>(stream));
-}
 
 // ---------------------------------------------------------------------------
 // pointmap consumers (pointmap.cu)
