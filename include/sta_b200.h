@@ -125,6 +125,23 @@ int64_t sta_device_bytes(StaModel* m);
 int sta_profile(StaModel* m, int enable);
 int sta_profile_read(StaModel* m, double* ms4, int64_t* counts4, double* flops4);
 
+/* Buffer taps (tests): read a forward's intermediate buffers launch by launch.  After each launch of run_encoder,
+ * run_decoder, decode_with_poses, run_dpt and forward_chunk whose tap name is set, the runtime enqueues a
+ * device-to-device copy of that launch's output, in its physical layout (bf16 rows 3x wide in the x3 mode; FP8 codes
+ * and scales as two taps, ".q" and ".s"), on the call's stream to dst + written (bytes), then advances `written` and
+ * increments `fired`.  Repeated firings within a call append.  A null dst only counts.  A copy past `capacity` fails the
+ * entry point with sta_last_error naming the tap.  The caller owns the array, zeroes written / fired, and keeps it
+ * alive until n = 0 clears the taps.  While any tap is set the graphed entry points run eagerly; the copies are not
+ * counted by sta_launch_count.  The names are listed in tests/test_forward_taps_gpu.py (TAP_PATTERNS). */
+typedef struct {
+  const char* name;
+  void* dst;
+  int64_t capacity;
+  int64_t written;
+  int32_t fired;
+} StaTap;
+int sta_set_taps(StaModel* m, StaTap* taps, int n);
+
 /* ---- op-level entry points (used by the parity tests; same kernels the model uses) ---- */
 
 enum { STA_EPI_BF16 = 0, STA_EPI_GELU = 1, STA_EPI_F32 = 2, STA_EPI_ROPE = 3, STA_EPI_PIXSHUF = 4, STA_EPI_HEAD = 5,

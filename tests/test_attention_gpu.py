@@ -151,6 +151,7 @@ def _check_bound(name, kernel, out, seen, shift):
     ratio = ((out - ref).abs() / bound).max().item()
     print("attention bound %-28s %-4s worst err / bound = %.3f" % (name, kernel, ratio), flush=True)
     assert ratio <= 1.0, "%s %s: err / bound = %.3f" % (name, kernel, ratio)
+    return ratio
 
 
 def _random_qkv(B, H, nq, nk, seed):

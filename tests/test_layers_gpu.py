@@ -808,6 +808,18 @@ def _ln_cases():
     return out + [("off_model-dual_C1024", 1000, 1024, "dual", 0)]
 
 
+def layernorm64(x, g, b, eps=1e-6):
+    """float64 LayerNorm of fp32 rows x with gain g and bias b, and the bound of the kernel's fp32 arithmetic,
+    2^-16 (|g| (|z| + max|x_row| / std) + |b|), without the output rounding"""
+    x64 = x.double()
+    mu = x64.mean(1, keepdim=True)
+    std = (x64.var(1, unbiased=False, keepdim=True) + eps).sqrt()
+    z = (x64 - mu) / std
+    xmax = x64.abs().max(1, keepdim=True).values / std
+    gg, bb = g.double(), b.double()
+    return z * gg + bb, 2.0 ** -16 * (gg.abs() * (z.abs() + xmax) + bb.abs())
+
+
 @pytest.mark.parametrize("sid,rows,C,form,drop", _ln_cases())
 def test_layernorm_within_float64_bound(sid, rows, C, form, drop):
     """|got - ref| <= 2^-8 |ref| + 2^-16 (|g| (|z| + max|x_row| / std) + |b|), z the float64 normalised value: the bf16
@@ -826,18 +838,11 @@ def test_layernorm_within_float64_bound(sid, rows, C, form, drop):
                                  P(params[2]) if dual else None, P(params[3]) if dual else None,
                                  P(outs[1]) if dual else None, drop, cur_stream()))
     torch.cuda.synchronize()
-    x64 = x.double()
-    mu = x64.mean(1, keepdim=True)
-    std = (x64.var(1, unbiased=False, keepdim=True) + 1e-6).sqrt()
-    z = (x64 - mu) / std
-    xmax = x64.abs().max(1, keepdim=True).values / std
-    if drop:
-        keep = (torch.arange(rows, device="cuda") % drop) != 0
-        z, xmax = z[keep], xmax[keep]
+    keep = (torch.arange(rows, device="cuda") % drop) != 0 if drop else slice(None)
     for i, o in enumerate(outs):
-        gg, bb = params[2 * i].double(), params[2 * i + 1].double()
-        ref = z * gg + bb
-        bound = 2.0 ** -8 * ref.abs() + 2.0 ** -16 * (gg.abs() * (z.abs() + xmax) + bb.abs())
+        ref, b32 = layernorm64(x, params[2 * i], params[2 * i + 1])
+        ref, b32 = ref[keep], b32[keep]
+        bound = 2.0 ** -8 * ref.abs() + b32
         assert torch.equal(_bits(o[out_rows:]), _bits(befores[i][out_rows:]))
         check_bound("layernorm %s out%d" % (sid, i + 1), o[:out_rows], ref, bound)
 

@@ -32,12 +32,15 @@ def _gam(K):
     return (K / 32 + 8) * 2.0 ** -24
 
 
-def head_pose64(sd, tok):
+def head_pose64(sd, tok, tok_err=None):
     """float64 head_pose_s of dec_norm-ed tokens [B][768] from the fp32 weights, with first-order bounds on the fp32
-    kernel's fc_t / fc_rot / fc_conf outputs"""
+    kernel's fc_t / fc_rot / fc_conf outputs; tok_err [B][768]: a bound on the error of the tokens the kernel starts
+    from (its own fp32 dec_norm), zero if not given"""
     P = lambda k: sd[PFX + k].to(tok.device).double()  # noqa: E731
     x = tok.double()
-    err = torch.zeros(x.shape[0], device=x.device, dtype=torch.float64)  # 2-norm of the error of the layer input
+    # 2-norm of the error of the layer input
+    err = (torch.zeros(x.shape[0], device=x.device, dtype=torch.float64) if tok_err is None else
+           tok_err.double().norm(dim=1))
     for i in (0, 2, 4):
         W, b = P("mlp.%d.weight" % i), P("mlp.%d.bias" % i)
         y = x @ W.t() + b

@@ -84,6 +84,10 @@ class StaGraphKeyframe(Structure):
     ]
 
 
+class StaTap(Structure):
+    _fields_ = [("name", c_char_p), ("dst", c_void_p), ("capacity", c_int64), ("written", c_int64), ("fired", c_int32)]
+
+
 class StaFlowStats(Structure):
     _fields_ = [("n_corners", c_int32), ("n_tracked", c_int32), ("abs_sum", ctypes.c_double),
                 ("mean_disparity", ctypes.c_double)]
@@ -133,6 +137,7 @@ def lib():
     L.sta_device_bytes.restype = i64
     L.sta_profile.argtypes = [vp, i]
     L.sta_profile_read.argtypes = [vp, POINTER(ctypes.c_double), POINTER(c_int64), POINTER(ctypes.c_double)]
+    L.sta_set_taps.argtypes = [vp, POINTER(StaTap), i]
     L.sta_op_gemm.argtypes = [POINTER(StaGemmDesc), vp]
     L.sta_op_gemm_fp8.argtypes = [POINTER(StaGemmFp8Desc), vp]
     L.sta_op_layernorm_fp8.argtypes = [vp, i, i, c_float, vp, vp, vp, vp, vp, vp, vp, vp, vp]

@@ -297,6 +297,8 @@ struct StaModel {
   double prof_ms[4] = {0, 0, 0, 0};
   int64_t prof_cnt[4] = {0, 0, 0, 0};
   double prof_flops[4] = {0, 0, 0, 0};
+  // ---- buffer taps of the tests (sta_set_taps): name -> the caller's StaTap ----
+  std::unordered_map<std::string, StaTap*> taps;
   cudaEvent_t prof_event() {
     cudaEvent_t e;
     if (!prof_pool.empty()) {
@@ -657,6 +659,37 @@ int attn(const Ctx& c, const bf16* q, long long ldq, int qc, const bf16* k, long
   return launch_attention(a, c.st);
 }
 
+// Buffer taps (sta_set_taps): after the launch named fmt % i, copy `bytes` of its output at src to the tap of that name.
+// The name is only formatted while taps are set.
+int tap(const Ctx& c, const void* src, size_t bytes, const char* fmt, int i = 0) {
+  StaModel* m = c.m;
+  if (m->taps.empty()) return 0;
+  char name[48];
+  snprintf(name, sizeof(name), fmt, i);
+  const auto it = m->taps.find(name);
+  if (it == m->taps.end()) return 0;
+  StaTap* t = it->second;
+  if (t->dst) {
+    if (t->written + static_cast<int64_t>(bytes) > t->capacity) {
+      set_last_error(std::string("tap ") + name + ": capacity too small");
+      return 2;
+    }
+    STA_CHECK_CUDA(cudaMemcpyAsync(static_cast<char*>(t->dst) + t->written, src, bytes, cudaMemcpyDeviceToDevice, c.st));
+  }
+  t->written += static_cast<int64_t>(bytes);
+  t->fired++;
+  return 0;
+}
+// bf16 activation rows of n logical elements, in bytes
+size_t bf_bytes(const Ctx& c, size_t n) { return n * c.m->bmul() * sizeof(bf16); }
+// FP8 activation rows: codes as fmt.q, scales as fmt.s
+int tap_fp8(const Ctx& c, const Fp8Act& a, size_t rows, int C, const char* fmt, int i) {
+  if (c.m->taps.empty()) return 0;
+  const std::string f(fmt);
+  RUN(tap(c, a.q, rows * C, (f + ".q").c_str(), i));
+  return tap(c, a.s, rows * (C / 128) * sizeof(float), (f + ".s").c_str(), i);
+}
+
 // ---------------------------------------------------------------------------
 // workspace: every entry point carves its buffers with the take functions below before its first launch, and
 // ws_need sizes the allocation by a dry run of the same functions
@@ -842,7 +875,8 @@ void drop_graphs(StaModel* m) {
 
 template <typename Body>
 int run_graphed(StaModel* m, cudaStream_t st, bool graphed, const std::vector<long long>& key, Body&& body) {
-  if (!graphed || m->prof_on) return body(Ctx{m, st});  // per-kernel timing events need eager launches
+  // per-kernel timing events and buffer taps need eager launches
+  if (!graphed || m->prof_on || !m->taps.empty()) return body(Ctx{m, st});
   StaModel::GraphEntry* ent = nullptr;
   for (auto& g : m->graphs)
     if (g.key == key) ent = &g;
@@ -892,29 +926,46 @@ int run_graphed(StaModel* m, cudaStream_t st, bool graphed, const std::vector<lo
 int run_encoder(const Ctx& c, int nimg, int N, float* x, EncBufs& e) {
   StaModel* m = c.m;
   const int T = nimg * N;
+  const size_t xb = static_cast<size_t>(T) * kEncDim * sizeof(float);
   RUN(linear(c, EPI_F32, e.patches, T, m->patch, x));
+  RUN(tap(c, x, xb, "enc.embed"));
   for (int l = 0; l < 24; ++l) {
     const EncBlock& b = m->enc[l];
     if (m->fp8) {
       RUN(ln_fp8(c, x, T, kEncDim, b.n1, e.ln8));
+      RUN(tap_fp8(c, e.ln8, T, kEncDim, "enc.%d.ln1", l));
       RUN(linear_fp8(c, EPI_ROPE, e.ln8, T, b.qkv, e.qkv, e.pos, 2 * kEncDim));
+      RUN(tap(c, e.qkv, bf_bytes(c, T * 3 * kEncDim), "enc.%d.qkv", l));
       RUN(attn(c, e.qkv, 3 * kEncDim, 0, e.qkv, 3 * kEncDim, kEncDim, e.qkv, 3 * kEncDim, 2 * kEncDim, e.att, kEncDim,
                nimg, kEncHeads, N, N, 0));
+      RUN(tap(c, e.att, bf_bytes(c, T * kEncDim), "enc.%d.att", l));
       RUN(quant_fp8(c, e.att, T, kEncDim, e.att8));
+      RUN(tap_fp8(c, e.att8, T, kEncDim, "enc.%d.att8", l));
       RUN(linear_fp8(c, EPI_F32, e.att8, T, b.proj, x));
+      RUN(tap(c, x, xb, "enc.%d.x_attn", l));
       RUN(ln_fp8(c, x, T, kEncDim, b.n2, e.ln8));
+      RUN(tap_fp8(c, e.ln8, T, kEncDim, "enc.%d.ln2", l));
       RUN(linear_fp8(c, EPI_GELU_FP8, e.ln8, T, b.fc1, nullptr, nullptr, 0, &e.hid8));
+      RUN(tap_fp8(c, e.hid8, T, 4 * kEncDim, "enc.%d.hid", l));
       RUN(linear_fp8(c, EPI_F32, e.hid8, T, b.fc2, x));
+      RUN(tap(c, x, xb, "enc.%d.x", l));
       continue;
     }
     RUN(ln(c, x, T, kEncDim, b.n1, e.lnb));
+    RUN(tap(c, e.lnb, bf_bytes(c, T * kEncDim), "enc.%d.ln1", l));
     RUN(linear(c, EPI_ROPE, e.lnb, T, b.qkv, e.qkv, nullptr, e.pos, 2 * kEncDim));
+    RUN(tap(c, e.qkv, bf_bytes(c, T * 3 * kEncDim), "enc.%d.qkv", l));
     RUN(attn(c, e.qkv, 3 * kEncDim, 0, e.qkv, 3 * kEncDim, kEncDim, e.qkv, 3 * kEncDim, 2 * kEncDim, e.att, kEncDim,
              nimg, kEncHeads, N, N, 0));
+    RUN(tap(c, e.att, bf_bytes(c, T * kEncDim), "enc.%d.att", l));
     RUN(linear(c, EPI_F32, e.att, T, b.proj, x, x));
+    RUN(tap(c, x, xb, "enc.%d.x_attn", l));
     RUN(ln(c, x, T, kEncDim, b.n2, e.lnb));
+    RUN(tap(c, e.lnb, bf_bytes(c, T * kEncDim), "enc.%d.ln2", l));
     RUN(linear(c, EPI_GELU, e.lnb, T, b.fc1, e.hid));
+    RUN(tap(c, e.hid, bf_bytes(c, T * 4 * kEncDim), "enc.%d.hid", l));
     RUN(linear(c, EPI_F32, e.hid, T, b.fc2, x, x));
+    RUN(tap(c, x, xb, "enc.%d.x", l));
   }
   return 0;
 }
@@ -928,61 +979,105 @@ int run_decoder(const Ctx& c, int B, int N, DecBufs& d, float* const* out1, floa
   StaModel* m = c.m;
   const int S = 2 * B, M = N + 1, T = S * N, Td = S * M;
   const long long half = static_cast<long long>(B) * M * kDecDim;
+  const size_t xb = static_cast<size_t>(Td) * kDecDim * sizeof(float);
+  const size_t hb = bf_bytes(c, static_cast<size_t>(T) * kDecDim);  // a decoder hook: the pose rows dropped
   auto emit = [&](int idx) -> int {
-    if (out1 && out1[idx]) { m->launches++; RUN(launch_copy_f32(d.xd, out1[idx], half, c.st)); }
-    if (out2 && out2[idx]) { m->launches++; RUN(launch_copy_f32(d.xd + half, out2[idx], half, c.st)); }
+    if (out1 && out1[idx]) {
+      m->launches++;
+      RUN(launch_copy_f32(d.xd, out1[idx], half, c.st));
+      RUN(tap(c, out1[idx], half * sizeof(float), "dec.out"));
+    }
+    if (out2 && out2[idx]) {
+      m->launches++;
+      RUN(launch_copy_f32(d.xd + half, out2[idx], half, c.st));
+      RUN(tap(c, out2[idx], half * sizeof(float), "dec.out"));
+    }
     return 0;
   };
   RUN(linear(c, EPI_F32, d.hook[0], T, m->dec_embed, d.xd, nullptr, nullptr, 0, N));
+  RUN(tap(c, d.xd, xb, "dec.embed"));
   m->launches++;
   RUN(launch_fill_pose_token(d.xd, m->pose_tok, S, M, kDecDim, c.st));
+  RUN(tap(c, d.xd, xb, "dec.pose_tok"));
   RUN(emit(0));
   for (int l = 0; l < 12; ++l) {
     const DecBlock& b = m->dec[l];
+    const size_t lnb = bf_bytes(c, static_cast<size_t>(Td) * kDecDim);
     if (m->fp8) {  // the same sequence with e4m3 operands for every linear
       RUN(ln_fp8(c, d.xd, Td, kDecDim, b.n1, d.ln8, &b.ny, &d.lny8));
+      RUN(tap_fp8(c, d.ln8, Td, kDecDim, "dec.%d.ln1", l));
+      RUN(tap_fp8(c, d.lny8, Td, kDecDim, "dec.%d.lny", l));
       RUN(linear_fp8(c, EPI_ROPE, d.ln8, Td, b.qkv, d.qkv, d.pos, 2 * kDecDim));
+      RUN(tap(c, d.qkv, 3 * lnb, "dec.%d.qkv", l));
       RUN(attn(c, d.qkv, 3 * kDecDim, 0, d.qkv, 3 * kDecDim, kDecDim, d.qkv, 3 * kDecDim, 2 * kDecDim, d.att, kDecDim, S,
                kDecHeads, M, M, 0));
+      RUN(tap(c, d.att, lnb, "dec.%d.att", l));
       RUN(quant_fp8(c, d.att, Td, kDecDim, d.att8));
+      RUN(tap_fp8(c, d.att8, Td, kDecDim, "dec.%d.att8", l));
       RUN(linear_fp8(c, EPI_F32, d.att8, Td, b.proj, d.xd));
+      RUN(tap(c, d.xd, xb, "dec.%d.x_self", l));
       RUN(linear_fp8(c, EPI_ROPE, d.lny8, Td, b.ckv, d.kvc, d.pos, kDecDim));
+      RUN(tap(c, d.kvc, 2 * lnb, "dec.%d.kvc", l));
       RUN(ln_fp8(c, d.xd, Td, kDecDim, b.n2, d.ln8));
+      RUN(tap_fp8(c, d.ln8, Td, kDecDim, "dec.%d.ln2", l));
       RUN(linear_fp8(c, EPI_ROPE, d.ln8, Td, b.cq, d.qc, d.pos, kDecDim));
+      RUN(tap(c, d.qc, lnb, "dec.%d.qc", l));
       RUN(attn(c, d.qc, kDecDim, 0, d.kvc, 2 * kDecDim, 0, d.kvc, 2 * kDecDim, kDecDim, d.att, kDecDim, S, kDecHeads, M,
                M, B));
+      RUN(tap(c, d.att, lnb, "dec.%d.catt", l));
       RUN(quant_fp8(c, d.att, Td, kDecDim, d.att8));
+      RUN(tap_fp8(c, d.att8, Td, kDecDim, "dec.%d.catt8", l));
       RUN(linear_fp8(c, EPI_F32, d.att8, Td, b.cproj, d.xd));
+      RUN(tap(c, d.xd, xb, "dec.%d.x_cross", l));
       RUN(ln_fp8(c, d.xd, Td, kDecDim, b.n3, d.ln8));
+      RUN(tap_fp8(c, d.ln8, Td, kDecDim, "dec.%d.ln3", l));
       RUN(linear_fp8(c, EPI_GELU_FP8, d.ln8, Td, b.fc1, nullptr, nullptr, 0, &d.hid8));
+      RUN(tap_fp8(c, d.hid8, Td, 4 * kDecDim, "dec.%d.hid", l));
       RUN(linear_fp8(c, EPI_F32, d.hid8, Td, b.fc2, d.xd));
+      RUN(tap(c, d.xd, xb, "dec.%d.x", l));
     } else {
     // self-attention on norm1(x); norm_y(x) is what the partner view cross-attends to
     RUN(ln(c, d.xd, Td, kDecDim, b.n1, d.ln1, &b.ny, d.lny));
+    RUN(tap(c, d.ln1, lnb, "dec.%d.ln1", l));
+    RUN(tap(c, d.lny, lnb, "dec.%d.lny", l));
     RUN(linear(c, EPI_ROPE, d.ln1, Td, b.qkv, d.qkv, nullptr, d.pos, 2 * kDecDim));
+    RUN(tap(c, d.qkv, 3 * lnb, "dec.%d.qkv", l));
     RUN(attn(c, d.qkv, 3 * kDecDim, 0, d.qkv, 3 * kDecDim, kDecDim, d.qkv, 3 * kDecDim, 2 * kDecDim, d.att, kDecDim, S,
              kDecHeads, M, M, 0));
+    RUN(tap(c, d.att, lnb, "dec.%d.att", l));
     RUN(linear(c, EPI_F32, d.att, Td, b.proj, d.xd, d.xd));
+    RUN(tap(c, d.xd, xb, "dec.%d.x_self", l));
     // cross-attention: q from norm2(x), k/v from norm_y(partner input) -- kv sample = (s + B) % 2B
     RUN(linear(c, EPI_ROPE, d.lny, Td, b.ckv, d.kvc, nullptr, d.pos, kDecDim));
+    RUN(tap(c, d.kvc, 2 * lnb, "dec.%d.kvc", l));
     RUN(ln(c, d.xd, Td, kDecDim, b.n2, d.ln1));
+    RUN(tap(c, d.ln1, lnb, "dec.%d.ln2", l));
     RUN(linear(c, EPI_ROPE, d.ln1, Td, b.cq, d.qc, nullptr, d.pos, kDecDim));
+    RUN(tap(c, d.qc, lnb, "dec.%d.qc", l));
     RUN(attn(c, d.qc, kDecDim, 0, d.kvc, 2 * kDecDim, 0, d.kvc, 2 * kDecDim, kDecDim, d.att, kDecDim, S, kDecHeads, M, M,
              B));
+    RUN(tap(c, d.att, lnb, "dec.%d.catt", l));
     RUN(linear(c, EPI_F32, d.att, Td, b.cproj, d.xd, d.xd));
+    RUN(tap(c, d.xd, xb, "dec.%d.x_cross", l));
     // MLP
     RUN(ln(c, d.xd, Td, kDecDim, b.n3, d.ln1));
+    RUN(tap(c, d.ln1, lnb, "dec.%d.ln3", l));
     RUN(linear(c, EPI_GELU, d.ln1, Td, b.fc1, d.hid));
+    RUN(tap(c, d.hid, 4 * lnb, "dec.%d.hid", l));
     RUN(linear(c, EPI_F32, d.hid, Td, b.fc2, d.xd, d.xd));
+    RUN(tap(c, d.xd, xb, "dec.%d.x", l));
     }
     if (l + 1 == 6 || l + 1 == 9) {  // DPT hooks [0, 7, 10, 13] -> decoder outputs 6, 9, 12 (dpt_head.py:112)
+      const int q = l + 1 == 6 ? 1 : 2;
       m->launches++;
-      RUN(launch_cast_f32_bf16(d.xd, d.hook[l + 1 == 6 ? 1 : 2], Td, kDecDim, M, c.st, m->split));
+      RUN(launch_cast_f32_bf16(d.xd, d.hook[q], Td, kDecDim, M, c.st, m->split));
+      RUN(tap(c, d.hook[q], hb, "dec.hook%d", q));
     }
     if (l + 1 < 12) RUN(emit(l + 1));
   }
   // dec_norm on the last output; bf16 copy without the pose token feeds the DPT head
   RUN(ln(c, d.xd, Td, kDecDim, m->dec_norm, d.hook[3], nullptr, nullptr, M));
+  RUN(tap(c, d.hook[3], hb, "dec.hook3"));
   if ((out1 && out1[12]) || (out2 && out2[12])) {
     // compat path: fp32 LayerNorm-ed last layer
     const int rows_half = B * M;
@@ -990,11 +1085,13 @@ int run_decoder(const Ctx& c, int B, int N, DecBufs& d, float* const* out1, floa
       m->launches++;
       layernorm_f32_kernel<<<(rows_half + 7) / 8, 256, 0, c.st>>>(d.xd, rows_half, kDecDim, kLnEps, m->dec_norm.g,
                                                                   m->dec_norm.b, out1[12]);
+      RUN(tap(c, out1[12], half * sizeof(float), "dec.out"));
     }
     if (out2 && out2[12]) {
       m->launches++;
       layernorm_f32_kernel<<<(rows_half + 7) / 8, 256, 0, c.st>>>(d.xd + half, rows_half, kDecDim, kLnEps,
                                                                   m->dec_norm.g, m->dec_norm.b, out2[12]);
+      RUN(tap(c, out2[12], half * sizeof(float), "dec.out"));
     }
     STA_CHECK_CUDA(cudaGetLastError());
   }
@@ -1006,7 +1103,9 @@ int cast_features(const Ctx& c, const float* feat1, const float* feat2, int B, i
   const long long T = static_cast<long long>(B) * N;
   c.m->launches += 2;
   RUN(launch_cast_f32_bf16(feat1, d.hook[0], T, kEncDim, 0, c.st, c.m->split));
-  return launch_cast_f32_bf16(feat2, d.hook[0] + T * kEncDim * c.m->bmul(), T, kEncDim, 0, c.st, c.m->split);
+  RUN(tap(c, d.hook[0], bf_bytes(c, T * kEncDim), "dec.hook0"));
+  RUN(launch_cast_f32_bf16(feat2, d.hook[0] + T * kEncDim * c.m->bmul(), T, kEncDim, 0, c.st, c.m->split));
+  return tap(c, d.hook[0] + T * kEncDim * c.m->bmul(), bf_bytes(c, T * kEncDim), "dec.hook0");
 }
 
 // Decoder positions, the symmetric decoder over 2B samples (d.hook[0] must be filled) and the pose heads on the
@@ -1016,10 +1115,16 @@ int decode_with_poses(const Ctx& c, int B, int h, int w, DecBufs& d, float* pose
   const long long rows = static_cast<long long>(h * w + 1) * kDecDim;  // decoder rows of one sample
   m->launches += 3;
   RUN(launch_make_positions(d.pos, 2 * B, h, w, 1, c.st));
+  RUN(tap(c, d.pos, 2 * static_cast<size_t>(B) * (h * w + 1) * 2 * sizeof(int), "pos.dec"));
   RUN(run_decoder(c, B, h * w, d, nullptr, nullptr));
-  RUN(launch_pose_head(d.xd, rows, B, 1, kLnEps, m->pose, pose, pose_conf, c.st));
-  return launch_pose_head(d.xd + B * rows, rows, B, 1, kLnEps, m->pose, pose + static_cast<long long>(view_stride) * 16,
-                          pose_conf + view_stride, c.st);
+  for (int v = 0; v < 2; ++v) {
+    float* p = pose + static_cast<long long>(v) * view_stride * 16;
+    float* pc = pose_conf + static_cast<long long>(v) * view_stride;
+    RUN(launch_pose_head(d.xd + v * B * rows, rows, B, 1, kLnEps, m->pose, p, pc, c.st));
+    RUN(tap(c, p, static_cast<size_t>(B) * 16 * sizeof(float), "pose"));
+    RUN(tap(c, pc, static_cast<size_t>(B) * sizeof(float), "pose_conf"));
+  }
+  return 0;
 }
 
 // ---------------------------------------------------------------------------
@@ -1037,34 +1142,48 @@ int run_dpt(const Ctx& c, const DptBufs& b, int h, int w, const bf16* const hook
              *hook3 = hook[3] + tok0 * 768;
 
   // ---- act_postprocess (dpt_block.py:356-410) ----
+  const size_t T4 = static_cast<size_t>(nimg) * h4 * w4;
   RUN(linear(c, EPI_BF16, hook0, T, m->act0, b.a0));
+  RUN(tap(c, b.a0, bf_bytes(c, static_cast<size_t>(T) * 128), "dpt.a0"));
   {
     GemmParams p = {};
     p.M = T; p.out = b.l1; p.ps_k = 4; p.ps_cout = 128; p.ps_h = h; p.ps_w = w;
     RUN(gemm(c, A_LINEAR, EPI_PIXSHUF, b.a0, m->act0T.K, m->act0T, p));
+    RUN(tap(c, b.l1, bf_bytes(c, static_cast<size_t>(T) * 16 * 128), "dpt.l1"));
   }
   RUN(linear(c, EPI_BF16, hook1, T, m->act1, b.a1));
+  RUN(tap(c, b.a1, bf_bytes(c, static_cast<size_t>(T) * 192), "dpt.a1"));
   {
     GemmParams p = {};
     p.M = T; p.out = b.l2; p.ps_k = 2; p.ps_cout = 192; p.ps_h = h; p.ps_w = w;
     RUN(gemm(c, A_LINEAR, EPI_PIXSHUF, b.a1, m->act1T.K, m->act1T, p));
+    RUN(tap(c, b.l2, bf_bytes(c, static_cast<size_t>(T) * 4 * 192), "dpt.l2"));
   }
   RUN(linear(c, EPI_BF16, hook2, T, m->act2, b.l3));
+  RUN(tap(c, b.l3, bf_bytes(c, static_cast<size_t>(T) * 384), "dpt.l3"));
   RUN(linear(c, EPI_BF16, hook3, T, m->act3, b.a3));
+  RUN(tap(c, b.a3, bf_bytes(c, static_cast<size_t>(T) * 768), "dpt.a3"));
   m->launches++;
   RUN(launch_im2col_3x3_s2(b.a3, b.col4, nimg, h, w, 768 * m->bmul(), c.st));  // pure channel-vector copy
+  RUN(tap(c, b.col4, bf_bytes(c, T4 * 9 * 768), "dpt.col4"));
   RUN(linear(c, EPI_BF16, b.col4, nimg * h4 * w4, m->act3c, b.l4));
+  RUN(tap(c, b.l4, bf_bytes(c, T4 * 768), "dpt.l4"));
   // ---- layer_rn: 3x3 conv to 256 channels, no bias (dpt_block.py:33-75); raw + relu copies ----
   const bf16* lin[4] = {b.l1, b.l2, b.l3, b.l4};
   const int lc[4] = {128, 192, 384, 768};
-  for (int i = 0; i < 4; ++i)
+  for (int i = 0; i < 4; ++i) {
     RUN(conv3(c, lin[i], nimg, LH[i], LW[i], lc[i], m->rn[i], b.r_raw[i], b.r_relu[i], nullptr, nullptr, 0));
+    const size_t rb = bf_bytes(c, static_cast<size_t>(nimg) * LH[i] * LW[i] * 256);
+    RUN(tap(c, b.r_raw[i], rb, "dpt.rn%d.raw", i));
+    RUN(tap(c, b.r_relu[i], rb, "dpt.rn%d.relu", i));
+  }
 
   // ---- refinenet4 .. refinenet1 (dpt_block.py:189-218, dpt_head.py:58-61) ----
   const bf16* path = nullptr;  // output of the previous (coarser) fusion block at this level's resolution
   for (int lvl = 3; lvl >= 0; --lvl) {
     const Refine& r = m->ref[lvl];
     const int Hh = LH[lvl], Ww = LW[lvl];
+    const size_t lb = bf_bytes(c, static_cast<size_t>(nimg) * Hh * Ww * 256);  // one 256-channel map of this level
     const bf16* s_raw;
     const bf16* s_relu;
     if (lvl == 3) {
@@ -1073,13 +1192,18 @@ int run_dpt(const Ctx& c, const DptBufs& b, int h, int w, const bf16* const hook
     } else {
       // res = RCU1(layer); s = path + res
       RUN(conv3(c, b.r_relu[lvl], nimg, Hh, Ww, 256, r.r1.c1, b.t1, nullptr, nullptr, nullptr, 1));
+      RUN(tap(c, b.t1, lb, "dpt.ref%d.t1", lvl));
       RUN(conv3(c, b.t1, nimg, Hh, Ww, 256, r.r1.c2, b.s_raw, b.s_relu, b.r_raw[lvl], path, 0));
+      RUN(tap(c, b.s_raw, lb, "dpt.ref%d.s_raw", lvl));
+      RUN(tap(c, b.s_relu, lb, "dpt.ref%d.s_relu", lvl));
       s_raw = b.s_raw;
       s_relu = b.s_relu;
     }
     // out = RCU2(s)
     RUN(conv3(c, s_relu, nimg, Hh, Ww, 256, r.r2.c1, b.t2, nullptr, nullptr, nullptr, 1));
+    RUN(tap(c, b.t2, lb, "dpt.ref%d.t2", lvl));
     RUN(conv3(c, b.t2, nimg, Hh, Ww, 256, r.r2.c2, b.o, nullptr, s_raw, nullptr, 0));
+    RUN(tap(c, b.o, lb, "dpt.ref%d.o", lvl));
     // bilinear x2 (align_corners=True), cropped to the next level's size for refinenet4 (dpt_head.py:58)
     // The reference applies out_conv (1x1) AFTER the upsample (dpt_block.py:215-217).  Both are linear and the
     // bilinear weights sum to one, so conv1x1(up(x)) == up(conv1x1(x)) exactly in real arithmetic; doing the
@@ -1087,20 +1211,27 @@ int run_dpt(const Ctx& c, const DptBufs& b, int h, int w, const bf16* const hook
     int OH = 2 * Hh, OW = 2 * Ww;
     if (lvl == 3) { OH = LH[2]; OW = LW[2]; }
     RUN(linear(c, EPI_BF16, b.o, nimg * Hh * Ww, r.out, b.up));
+    RUN(tap(c, b.up, lb, "dpt.ref%d.up", lvl));
     m->launches++;
     RUN(launch_upsample2x(b.up, b.path, nimg, Hh, Ww, 256, OH, OW, c.st, m->split));
+    RUN(tap(c, b.path, bf_bytes(c, static_cast<size_t>(nimg) * OH * OW * 256), "dpt.ref%d.path", lvl));
     path = b.path;
   }
   // ---- head (dpt_block.py:318-324) + postprocess (postprocess.py:10-62) ----
   const int H8 = 8 * h, W8 = 8 * w;
+  const size_t px8 = static_cast<size_t>(nimg) * H8 * W8;
   RUN(conv3(c, b.path, nimg, H8, W8, 256, m->head0, b.hc1, nullptr, nullptr, nullptr, 0));
+  RUN(tap(c, b.hc1, bf_bytes(c, px8 * 128), "dpt.hc1"));
   m->launches++;
   RUN(launch_upsample2x(b.hc1, b.hup, nimg, H8, W8, 128, 2 * H8, 2 * W8, c.st, m->split));
+  RUN(tap(c, b.hup, bf_bytes(c, 4 * px8 * 128), "dpt.hup"));
   {
     GemmParams p = {};
     p.nimg = nimg; p.H = 2 * H8; p.W = 2 * W8; p.Cin = 128 * m->bmul();
     p.head_w = m->head4_w; p.head_b = m->head4_b; p.pts3d = pts3d; p.conf = conf;
     RUN(gemm(c, A_CONV3, EPI_HEAD, b.hup, 0, m->head2, p));
+    RUN(tap(c, pts3d, 4 * px8 * 3 * sizeof(float), "dpt.pts3d"));
+    RUN(tap(c, conf, 4 * px8 * sizeof(float), "dpt.conf"));
   }
   return 0;
 }
@@ -1181,12 +1312,17 @@ int forward_chunk(const Ctx& c, const void* img1, const void* img2, int img_is_b
   // encode both views as one batch of 2B images: [view 1 batch ; view 2 batch]
   m->launches += 3;
   const size_t bm = m->bmul();  // physical / logical width of the bf16 activation rows
+  const size_t pb = bf_bytes(c, static_cast<size_t>(B) * N * 768);  // one view's patches
   RUN(launch_patch_im2col(img1, img_is_bf16, B, H, W, e.patches, c.st, m->split));
+  RUN(tap(c, e.patches, pb, "patches"));
   RUN(launch_patch_im2col(img2, img_is_bf16, B, H, W, e.patches + static_cast<size_t>(B) * N * 768 * bm, c.st, m->split));
+  RUN(tap(c, e.patches + static_cast<size_t>(B) * N * 768 * bm, pb, "patches"));
   RUN(launch_make_positions(e.pos, S, h, w, 0, c.st));
+  RUN(tap(c, e.pos, static_cast<size_t>(S) * N * 2 * sizeof(int), "pos.enc"));
   RUN(run_encoder(c, S, N, x, e));
   m->launches += 1;
   RUN(launch_cast_f32_bf16(x, d.hook[0], static_cast<long long>(S) * N, kEncDim, 0, c.st, m->split));
+  RUN(tap(c, d.hook[0], bf_bytes(c, static_cast<size_t>(S) * N * kEncDim), "dec.hook0"));
   // pose outputs are laid out [2][B_total]: view 1 block then view 2 block
   RUN(decode_with_poses(c, B, h, w, d, pose, pose_conf, B_total));
   // DPT heads: view 1 images then view 2 images (outputs are [2][B_total] blocks).  The host entry point passes events:
@@ -1342,6 +1478,22 @@ int sta_profile_read(StaModel* m, double* ms4, int64_t* counts4, double* flops4)
   }
   return 0;
 }
+int sta_set_taps(StaModel* m, StaTap* taps, int n) {
+  if (!m || n < 0 || (n > 0 && !taps)) {
+    set_last_error("sta_set_taps: null model, or n > 0 taps at a null array");
+    return 2;
+  }
+  m->taps.clear();
+  for (int i = 0; i < n; ++i) {
+    if (!taps[i].name || m->taps.count(taps[i].name)) {
+      set_last_error("sta_set_taps: a tap without a name, or two taps with one name");
+      m->taps.clear();
+      return 2;
+    }
+    m->taps[taps[i].name] = &taps[i];
+  }
+  return 0;
+}
 int sta_weight_arena(StaModel* m, void** ptr, int64_t* bytes) {
   if (!m || !ptr || !bytes) {
     set_last_error("sta_weight_arena: null argument");
@@ -1473,9 +1625,11 @@ int sta_encode(StaModel* m, const void* img_dev, int img_is_bf16, int B, int H, 
   RUN(check_ws(m->ws));
   m->launches += 1;
   RUN(launch_patch_im2col(img_dev, img_is_bf16, B, H, W, e.patches, c.st, m->split));
+  RUN(tap(c, e.patches, bf_bytes(c, static_cast<size_t>(B) * N * 768), "patches"));
   auto body = [&](const Ctx& cc) -> int {
     m->launches += 1;
     RUN(launch_make_positions(e.pos, B, h, w, 0, cc.st));
+    RUN(tap(cc, e.pos, static_cast<size_t>(B) * N * 2 * sizeof(int), "pos.enc"));
     return run_encoder(cc, B, N, x, e);
   };
   RUN(run_graphed(m, c.st, graphed, {1, B, H, W}, body));
