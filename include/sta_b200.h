@@ -633,6 +633,28 @@ int sta_graph_export(StaGraph* g, int view0, int num_views, float conf_thres, co
                      float* scale_out, float* depth_out, float* conf_out, float* intri_out, float* points_out,
                      float* colors_out, int64_t* count_out, void* scratch, void* stream);
 
+/* ---- map rendering (OnlineSLAM.render, tools/render_video.py) ---- */
+enum { STA_RENDER_MAX_RADIUS = 4 };
+/* Render a map from C cameras into a z-buffer.  The map is sta_graph_export's output without the cloud: depth / conf
+ * [V][H][W] (unscaled), pose44 [V][4][4] (scale dropped), scale [V], intri [V][3][3], and imgs [V][3][H][W] in [-1, 1].
+ * Every pixel with conf > conf_thres becomes the PLY's world point (K^-1 from the fp64 adjugate, then
+ * P (K^-1 [col row 1]^T depth s) in fp32); segs [L][2][3] are world-space line segments coloured seg_colors [L][3].
+ * Cameras: w2c [C][4][4] world-to-camera, K [C][3][3].  A point with camera z >= near covers the (2 radius + 1)^2
+ * pixels centred on floor(u / w + 0.5), floor(v / w + 0.5); a segment is clipped to z >= near and to the image and
+ * drawn by DDA with perspective-correct z.  Each pixel keeps the smallest key (float bits of z << 32) | id, id =
+ * v H W + row W + col for a point and V H W + l for segment l, so ties go to the lower id and the result does not depend
+ * on scheduling.  Outputs per camera: rgb_out [C][Ho][Wo][3] ((img + 1) / 2, the segment's colour, or background, a
+ * host float[3]), depth_out [C][Ho][Wo] (the winner's camera z, or 0), index_out [C][Ho][Wo] (its id, or -1).
+ * scratch: sta_render_scratch_bytes(C, Ho, Wo), 8-byte aligned.  Four launches (clear, points, segments, resolve), no
+ * host synchronisation.  Refused before any launch: C, Ho or Wo outside [1, 8192], radius outside
+ * [0, STA_RENDER_MAX_RADIUS], near <= 0, V outside [0, 65535], V H W + L >= 2^32 - 1, a null input or output, a small
+ * or misaligned scratch, host memory. */
+size_t sta_render_scratch_bytes(int num_cams, int Ho, int Wo);
+int sta_render(const float* depth, const float* conf, const float* pose44, const float* scale, const float* intri,
+               const float* imgs, int V, int H, int W, float conf_thres, const float* w2c, const float* K, int C, int Ho,
+               int Wo, int radius, float near, const float* segs, const float* seg_colors, int L, const float* background,
+               void* scratch, size_t scratch_bytes, float* rgb_out, float* depth_out, int64_t* index_out, void* stream);
+
 /* ---- reconstruction evaluation (vista_slam/eval/eval_recon.py:108-206): world clouds, open3d's voxel_down_sample, the
  * moments of open3d's point-to-point ICP and the nearest-neighbour distances of the Chamfer metric.  Points are fp64
  * [n][3] device arrays.  Every reduction runs in a fixed order without floating-point atomics, so repeated runs are

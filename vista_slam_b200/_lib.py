@@ -57,6 +57,8 @@ GRAPH_MAX_TRACK_FRAMES = 4096  # STA_GRAPH_MAX_TRACK_FRAMES: frames per sta_grap
 ORB_MAX_KEYPOINTS = 4096
 PG_DENSE_MAX_OPT = 3657  # STA_PG_DENSE_MAX_OPT: above it PoseGraphOpt takes the block-sparse route
 PG_GROUP_MAX = 16  # STA_PG_GROUP_MAX: graphs per sta_pose_graph_lm_step_group call or sta_pg_group_plan
+RENDER_MAX_RADIUS = 4  # STA_RENDER_MAX_RADIUS: largest point radius of sta_render
+RENDER_MAX_SIDE = 8192  # cameras per sta_render call and output rows / columns
 
 
 class StaPgGraph(Structure):
@@ -233,6 +235,10 @@ def lib():
     L.sta_graph_export_scratch_bytes.restype = ctypes.c_size_t
     L.sta_graph_export.argtypes = [vp, i, i, c_float, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]
     f64, sz = ctypes.c_double, ctypes.c_size_t
+    L.sta_render_scratch_bytes.argtypes = [i, i, i]
+    L.sta_render_scratch_bytes.restype = sz
+    L.sta_render.argtypes = [vp, vp, vp, vp, vp, vp, i, i, i, c_float, vp, vp, i, i, i, i, c_float, vp, vp, i,
+                             POINTER(c_float), vp, sz, vp, vp, vp, vp]
     L.sta_sort_scratch_bytes.argtypes = [i64]
     L.sta_sort_scratch_bytes.restype = sz
     L.sta_op_radix_sort.argtypes = [vp, vp, i64, i, vp, vp, vp, vp]

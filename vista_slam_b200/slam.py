@@ -556,6 +556,33 @@ class OnlineSLAM:
             view["intri"] = ex["intri"][0].cpu()
         return view
 
+    def render(self, poses, K, size, point_radius=0, views=None, lines=None, background=(1.0, 1.0, 1.0)):
+        """Images of the map of `views` (a range; default: every view with a node) from cameras poses [C,4,4]
+        (camera-to-world) with intrinsics K, drawn on the device by render.render_views: the confident points of
+        save_data_all's PLY, z-buffered, and `lines` (render.camera_frusta, render.graph_segments) depth-tested with
+        them.  Returns {rgb, depth, index} device tensors without a host synchronisation.  A background PGO is folded
+        first if it has finished, never waited for (as get_view).  IndexError for a view without a node; nothing in
+        the session changes."""
+        from .render import render_views
+        self._pgo_poll()
+        if views is None:
+            n = 0
+            while self.view_to_node.get(n):
+                n += 1
+            views = range(n)
+        if not isinstance(views, range) or views.step != 1:
+            raise ValueError("views must be a range with step 1")
+        if len(views) == 0:
+            dev = self.device if self._graph is None else self._graph.device
+            maps = {k: torch.empty(s, dtype=torch.float32, device=dev)
+                    for k, s in (("pose", (0, 4, 4)), ("scale", (0, 1)), ("depth", (0, 1, 1)), ("conf", (0, 1, 1)),
+                                 ("intri", (0, 3, 3)), ("images", (0, 3, 1, 1)))}
+        else:
+            maps = self._export(views.start, len(views), cloud=False)
+            maps["images"] = torch.stack(list(list.__iter__(self.imgs))[views.start:views.stop]).to(torch.float32)
+        return render_views(maps, self.conf_thres, poses, K, size, point_radius=point_radius, lines=lines,
+                            background=background)
+
     def get_view_graph(self):
         """slam.py:328-336."""
         return {v: [self.node_to_connected_view[u] for u in self.view_to_node.get(v, [])] for v in range(self.view_num)}
