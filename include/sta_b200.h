@@ -655,6 +655,53 @@ int sta_render(const float* depth, const float* conf, const float* pose44, const
                int Wo, int radius, float near, const float* segs, const float* seg_colors, int L, const float* background,
                void* scratch, size_t scratch_bytes, float* rgb_out, float* depth_out, int64_t* index_out, void* stream);
 
+/* ---- TSDF fusion and meshing of the map (fusion.fuse_views, OnlineSLAM.extract_mesh) ---- */
+enum { STA_FUSION_BRICK = 8, STA_FUSION_BRICK_BITS = 21, STA_FUSION_MAX_BRICKS = 1 << 20 };
+/* The map is sta_render's (depth / conf [V][H][W] unscaled, pose44 [V][4][4], scale [V], intri [V][3][3], imgs
+ * [V][3][H][W] in [-1, 1]).  Samples sit at (i v, j v, k v), each coordinate float(i) * v in fp32, in bricks of
+ * STA_FUSION_BRICK^3; brick (bx, by, bz) = floor(i / 8) per axis, each in [-2^20, 2^20 - 1], has the 63-bit key
+ * (bz + 2^20) << 42 | (by + 2^20) << 21 | (bx + 2^20).  A pixel is used when conf > conf_thres and d = depth scale > 0.
+ *
+ * sta_fusion_bricks: the sorted distinct keys of the bricks that the cube [p - trunc, p + trunc] of some used pixel's
+ * PLY point p touches (floor((p -+ trunc) / 8v) per axis); a point with a non-finite coordinate or a brick outside
+ * the range is skipped.  Two calls: with key_capacity 0 it writes counts_out[0] = the number of (tile, brick) keys
+ * (an upper bound of the brick count); with key_capacity = that count it writes the keys to keys_out [key_capacity]
+ * and counts_out[1] = the brick count B.  scratch: sta_fusion_bricks_scratch_bytes(V, H, W, key_capacity), 16-byte
+ * aligned.  No host synchronisation.
+ *
+ * sta_fusion_integrate: KinectFusion's projective TSDF with unit weights of every view, in increasing index, into the
+ * B bricks of keys: for sample x and view v, c = w2c[v] x (fp32); skipped unless c_z > 0, the pixel
+ * (floor(u + 0.5), floor(r + 0.5)) of intri[v] c / c_z is inside the image and used, and sdf = d - c_z >= -trunc;
+ * then T <- (T W + min(1, sdf / trunc)) / (W + 1), rgb alike with (img + 1) / 2, W <- W + 1.  Outputs tsdf_out,
+ * weight_out [B][8][8][8] ([b][z][y][x]) and color_out [B][8][8][8][3]; unobserved samples are 0.  Views are culled
+ * per brick conservatively, and there are no floating-point atomics, so the result is the same bit for bit on every
+ * call.  scratch: sta_fusion_integrate_scratch_bytes(B, V), 16-byte aligned.
+ *
+ * sta_fusion_mesh: marching cubes (mc_table.h) over every cube whose 8 samples exist with weight >= min_weight; inside
+ * is T < 0.  One vertex per crossing lattice edge used by an emitted face, at a + T_a / (T_a - T_b) (b - a) with its
+ * colour interpolated alike, in (brick, sample, axis) order; faces in (brick, cube, triangle) order, counter-clockwise
+ * seen from T > 0.  Two calls: with zero capacities it writes counts_out[0] = vertices, counts_out[1] = faces; with
+ * capacities at least those it also writes vertices_out / vertex_colors_out [Nv][3] and faces_out [Nf][3].
+ * scratch: sta_fusion_mesh_scratch_bytes(B), 16-byte aligned.
+ *
+ * Refused before any CUDA call: sizes outside [1, 65535], voxel <= 0 or not finite, trunc outside (0, 4 voxel],
+ * min_weight < 1, B outside [0, STA_FUSION_MAX_BRICKS], a key capacity outside [0, 2^31), a null input or output, a
+ * small or misaligned scratch, host memory. */
+size_t sta_fusion_bricks_scratch_bytes(int V, int H, int W, int64_t key_capacity);
+int sta_fusion_bricks(const float* depth, const float* conf, const float* pose44, const float* scale, const float* intri,
+                      int V, int H, int W, float conf_thres, float voxel, float trunc, int64_t key_capacity,
+                      void* scratch, size_t scratch_bytes, int64_t* keys_out, int64_t* counts_out, void* stream);
+size_t sta_fusion_integrate_scratch_bytes(int64_t num_bricks, int V);
+int sta_fusion_integrate(const float* depth, const float* conf, const float* scale, const float* intri, const float* imgs,
+                         const float* w2c, int V, int H, int W, float conf_thres, const int64_t* keys, int64_t num_bricks,
+                         float voxel, float trunc, void* scratch, size_t scratch_bytes, float* tsdf_out,
+                         float* weight_out, float* color_out, void* stream);
+size_t sta_fusion_mesh_scratch_bytes(int64_t num_bricks);
+int sta_fusion_mesh(const int64_t* keys, int64_t num_bricks, const float* tsdf, const float* weight, const float* color,
+                    float voxel, float min_weight, int64_t max_vertices, int64_t max_faces, void* scratch,
+                    size_t scratch_bytes, float* vertices_out, float* vertex_colors_out, int32_t* faces_out,
+                    int64_t* counts_out, void* stream);
+
 /* ---- reconstruction evaluation (vista_slam/eval/eval_recon.py:108-206): world clouds, open3d's voxel_down_sample, the
  * moments of open3d's point-to-point ICP and the nearest-neighbour distances of the Chamfer metric.  Points are fp64
  * [n][3] device arrays.  Every reduction runs in a fixed order without floating-point atomics, so repeated runs are

@@ -59,6 +59,10 @@ PG_DENSE_MAX_OPT = 3657  # STA_PG_DENSE_MAX_OPT: above it PoseGraphOpt takes the
 PG_GROUP_MAX = 16  # STA_PG_GROUP_MAX: graphs per sta_pose_graph_lm_step_group call or sta_pg_group_plan
 RENDER_MAX_RADIUS = 4  # STA_RENDER_MAX_RADIUS: largest point radius of sta_render
 RENDER_MAX_SIDE = 8192  # cameras per sta_render call and output rows / columns
+FUSION_BRICK = 8  # STA_FUSION_BRICK: samples per brick side
+FUSION_BRICK_BITS = 21  # STA_FUSION_BRICK_BITS: bits per brick coordinate in a key
+FUSION_MAX_BRICKS = 1 << 20  # STA_FUSION_MAX_BRICKS: bricks per sta_fusion_integrate / sta_fusion_mesh call
+FUSION_MAX_SIDE = 65535  # views, rows and columns per sta_fusion_bricks / sta_fusion_integrate call
 
 
 class StaPgGraph(Structure):
@@ -239,6 +243,16 @@ def lib():
     L.sta_render_scratch_bytes.restype = sz
     L.sta_render.argtypes = [vp, vp, vp, vp, vp, vp, i, i, i, c_float, vp, vp, i, i, i, i, c_float, vp, vp, i,
                              POINTER(c_float), vp, sz, vp, vp, vp, vp]
+    L.sta_fusion_bricks_scratch_bytes.argtypes = [i, i, i, i64]
+    L.sta_fusion_bricks_scratch_bytes.restype = sz
+    L.sta_fusion_bricks.argtypes = [vp, vp, vp, vp, vp, i, i, i, c_float, c_float, c_float, i64, vp, sz, vp, vp, vp]
+    L.sta_fusion_integrate_scratch_bytes.argtypes = [i64, i]
+    L.sta_fusion_integrate_scratch_bytes.restype = sz
+    L.sta_fusion_integrate.argtypes = [vp, vp, vp, vp, vp, vp, i, i, i, c_float, vp, i64, c_float, c_float, vp, sz, vp,
+                                       vp, vp, vp]
+    L.sta_fusion_mesh_scratch_bytes.argtypes = [i64]
+    L.sta_fusion_mesh_scratch_bytes.restype = sz
+    L.sta_fusion_mesh.argtypes = [vp, i64, vp, vp, vp, c_float, c_float, i64, i64, vp, sz, vp, vp, vp, vp, vp]
     L.sta_sort_scratch_bytes.argtypes = [i64]
     L.sta_sort_scratch_bytes.restype = sz
     L.sta_op_radix_sort.argtypes = [vp, vp, i64, i, vp, vp, vp, vp]

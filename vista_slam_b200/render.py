@@ -48,15 +48,9 @@ def _w2c(poses):
     return torch.stack(rows + [last], dim=1).to(torch.float32).contiguous()
 
 
-def render_views(maps, conf_thres, poses, K, size, point_radius=0, near=1e-3, lines=None, background=(1.0, 1.0, 1.0)):
-    """Render `maps` (module docstring; every array float32 on one CUDA device) from C cameras.
-
-    poses [C,4,4]: camera-to-world (the convention of trajectory.npy, get_view().pose and frame_trajectory()["pose"]),
-    host or device, inverted on the map's device in float64.  K: [C,3,3] or one [3,3] for all.  size: (Ho, Wo).
-    lines: (segs [L,2,3] world endpoints, colors [L,3]) or None.  A point or segment is drawn where its camera-frame z
-    is at least near.  Returns {rgb [C,Ho,Wo,3] float32, depth [C,Ho,Wo] float32 (camera z, 0 where empty), index
-    [C,Ho,Wo] int64 (v H W + row W + col of the point drawn, V H W + l for segment l, -1 where empty)} on the map's
-    device, with no host synchronisation.  Shapes, dtypes, devices and ranges are checked first (ValueError)."""
+def _check_maps(maps):
+    """The arrays of a `maps` dict (module docstring) as tensors, and V, H, W; ValueError for a missing key, a shape
+    or a dtype other than float32.  Devices are the caller's to check."""
     if not isinstance(maps, dict) or any(k not in maps for k in _MAP_KEYS):
         raise ValueError("maps must be a dict with keys %s" % (_MAP_KEYS,))
     m = {k: _tensor(maps[k], "maps[%r]" % k) for k in _MAP_KEYS}
@@ -71,6 +65,19 @@ def render_views(maps, conf_thres, poses, K, size, point_radius=0, near=1e-3, li
             raise ValueError("maps[%r] must be %s, got %s" % (k, shape, got))
         if m[k].dtype != torch.float32:
             raise ValueError("maps[%r] must be float32, not %s" % (k, m[k].dtype))
+    return m, V, H, W
+
+
+def render_views(maps, conf_thres, poses, K, size, point_radius=0, near=1e-3, lines=None, background=(1.0, 1.0, 1.0)):
+    """Render `maps` (module docstring; every array float32 on one CUDA device) from C cameras.
+
+    poses [C,4,4]: camera-to-world (the convention of trajectory.npy, get_view().pose and frame_trajectory()["pose"]),
+    host or device, inverted on the map's device in float64.  K: [C,3,3] or one [3,3] for all.  size: (Ho, Wo).
+    lines: (segs [L,2,3] world endpoints, colors [L,3]) or None.  A point or segment is drawn where its camera-frame z
+    is at least near.  Returns {rgb [C,Ho,Wo,3] float32, depth [C,Ho,Wo] float32 (camera z, 0 where empty), index
+    [C,Ho,Wo] int64 (v H W + row W + col of the point drawn, V H W + l for segment l, -1 where empty)} on the map's
+    device, with no host synchronisation.  Shapes, dtypes, devices and ranges are checked first (ValueError)."""
+    m, V, H, W = _check_maps(maps)
     if not (isinstance(size, (tuple, list)) and len(size) == 2 and all(isinstance(s, numbers.Integral) for s in size)):
         raise ValueError("size must be (Ho, Wo)")
     Ho, Wo = int(size[0]), int(size[1])

@@ -564,6 +564,12 @@ class OnlineSLAM:
         first if it has finished, never waited for (as get_view).  IndexError for a view without a node; nothing in
         the session changes."""
         from .render import render_views
+        return render_views(self._view_maps(views), self.conf_thres, poses, K, size, point_radius=point_radius,
+                            lines=lines, background=background)
+
+    def _view_maps(self, views):
+        """The `maps` dict of render_views and fuse_views for `views` (a range; default: every view with a node), after
+        folding a background PGO that has finished (never waiting for one).  IndexError for a view without a node."""
         self._pgo_poll()
         if views is None:
             n = 0
@@ -574,14 +580,33 @@ class OnlineSLAM:
             raise ValueError("views must be a range with step 1")
         if len(views) == 0:
             dev = self.device if self._graph is None else self._graph.device
-            maps = {k: torch.empty(s, dtype=torch.float32, device=dev)
+            return {k: torch.empty(s, dtype=torch.float32, device=dev)
                     for k, s in (("pose", (0, 4, 4)), ("scale", (0, 1)), ("depth", (0, 1, 1)), ("conf", (0, 1, 1)),
                                  ("intri", (0, 3, 3)), ("images", (0, 3, 1, 1)))}
-        else:
-            maps = self._export(views.start, len(views), cloud=False)
-            maps["images"] = torch.stack(list(list.__iter__(self.imgs))[views.start:views.stop]).to(torch.float32)
-        return render_views(maps, self.conf_thres, poses, K, size, point_radius=point_radius, lines=lines,
-                            background=background)
+        maps = self._export(views.start, len(views), cloud=False)
+        maps["images"] = torch.stack(list(list.__iter__(self.imgs))[views.start:views.stop]).to(torch.float32)
+        return maps
+
+    def extract_mesh(self, voxel_size, trunc=None, min_weight=1, views=None):
+        """The map of `views` (a range; default: every view with a node) fused into a TSDF volume and meshed on the
+        device by fusion.fuse_views: {bricks, tsdf, weight, color, vertices, vertex_colors, faces} device tensors.
+        voxel_size in world units; trunc in (0, 4 voxel_size], default 4 voxel_size; min_weight: the views every
+        corner of a meshed cube needs.  The volume is rebuilt from the current poses on every call, so it follows each
+        PGO.  A background PGO is folded first if it has finished, never waited for (as render).  IndexError for a
+        view without a node; nothing in the session changes."""
+        from .fusion import fuse_views
+        return fuse_views(self._view_maps(views), self.conf_thres, voxel_size, trunc=trunc, min_weight=min_weight)
+
+    def save_mesh(self, output_folder, voxel_size, trunc=None, min_weight=1, views=None):
+        """extract_mesh written to output_folder/mesh.ply (write_mesh_ply).  A pending background PGO is folded first
+        (wait_pgo), as save_data_all does.  Returns the mesh's path."""
+        self.wait_pgo()
+        mesh = self.extract_mesh(voxel_size, trunc=trunc, min_weight=min_weight, views=views)
+        os.makedirs(output_folder, exist_ok=True)
+        path = os.path.join(output_folder, "mesh.ply")
+        write_mesh_ply(path, mesh["vertices"].cpu().numpy(), mesh["vertex_colors"].cpu().numpy(),
+                       mesh["faces"].cpu().numpy())
+        return path
 
     def get_view_graph(self):
         """slam.py:328-336."""
@@ -929,6 +954,46 @@ def write_ply(path, points, colors):
     with open(path, "wb") as f:
         f.write(header.encode("ascii"))
         f.write(rec.tobytes())
+
+
+def write_mesh_ply(path, vertices, colors, faces):
+    """Binary little-endian PLY of a triangle mesh: float x y z and uchar red green blue per vertex (colours in [0, 1],
+    rounded to 8 bits, as write_ply), then per face `property list uchar int vertex_indices` of 3."""
+    vertices, faces = np.asarray(vertices), np.asarray(faces)
+    n, m = len(vertices), len(faces)
+    rec = np.empty(n, dtype=[("x", "<f4"), ("y", "<f4"), ("z", "<f4"), ("r", "u1"), ("g", "u1"), ("b", "u1")])
+    for k, name in enumerate("xyz"):
+        rec[name] = vertices[:, k]
+    rgb = np.rint(np.clip(np.asarray(colors, np.float64), 0.0, 1.0) * 255.0).astype(np.uint8)
+    for k, name in enumerate("rgb"):
+        rec[name] = rgb[:, k]
+    frec = np.empty(m, dtype=[("n", "u1"), ("v", "<i4", (3,))])
+    frec["n"] = 3
+    frec["v"] = faces.reshape(m, 3)
+    header = ("ply\nformat binary_little_endian 1.0\nelement vertex %d\nproperty float x\nproperty float y\n"
+              "property float z\nproperty uchar red\nproperty uchar green\nproperty uchar blue\nelement face %d\n"
+              "property list uchar int vertex_indices\nend_header\n" % (n, m))
+    with open(path, "wb") as f:
+        f.write(header.encode("ascii"))
+        f.write(rec.tobytes())
+        f.write(frec.tobytes())
+
+
+def read_mesh_ply(path):
+    """(vertices [N,3] fp32, colours [N,3] uint8, faces [M,3] int32) of a file write_mesh_ply wrote."""
+    with open(path, "rb") as f:
+        data = f.read()
+    end = data.index(b"end_header\n") + len(b"end_header\n")
+    head = data[:end].decode().splitlines()
+    n = int([ln for ln in head if ln.startswith("element vertex")][0].split()[-1])
+    m = int([ln for ln in head if ln.startswith("element face")][0].split()[-1])
+    vdt = np.dtype([("x", "<f4"), ("y", "<f4"), ("z", "<f4"), ("r", "u1"), ("g", "u1"), ("b", "u1")])
+    rec = np.frombuffer(data, dtype=vdt, count=n, offset=end)
+    frec = np.frombuffer(data, dtype=[("n", "u1"), ("v", "<i4", (3,))], count=m, offset=end + n * vdt.itemsize)
+    if m and not (frec["n"] == 3).all():
+        raise ValueError("%s: not a triangle mesh" % path)
+    return (np.stack([rec["x"], rec["y"], rec["z"]], -1), np.stack([rec["r"], rec["g"], rec["b"]], -1),
+            frec["v"].astype(np.int32).reshape(m, 3))
 
 
 def read_ply(path):
