@@ -702,6 +702,18 @@ int sta_fusion_mesh(const int64_t* keys, int64_t num_bricks, const float* tsdf, 
                     size_t scratch_bytes, float* vertices_out, float* vertex_colors_out, int32_t* faces_out,
                     int64_t* counts_out, void* stream);
 
+/* ---- multi-view depth consistency of the map (slam_utils.view_consistency_check, OnlineSLAM.view_consistency) ---- */
+/* vista_slam/utils/slam_utils.py:346-419 for n views: depth [n][H][W], intri [n][3][3], pose44 [n][4][4]
+ * camera-to-world, all fp32.  count_out [n][H][W] (device int32): for pixel (x, y) of view i, the number of views j in
+ * [max(0, i - 4), min(n - 1, i + 4)], j != i, for which |sample - z| < threshold and z > 0, where p = T_i (K_i^-1
+ * [x y 1]^T d_i), c = T_j^-1 p, z = max(c_z, 1e-6), (u, v) = (K_j c)_xy / (K_j c)_z with the unclamped c, and sample is
+ * depth j bilinearly at (u, v) with zero padding (grid_sample, align_corners=True).  A non-finite coordinate never
+ * agrees; a finite one outside the image samples 0.  One launch, no atomics (the same bits on every call), no host
+ * synchronisation.  Refused before any launch: n outside [1, 65535], H or W < 2, n H W >= 2^31, a non-finite threshold,
+ * a null pointer, host memory. */
+int sta_view_consistency(const float* depth, const float* intri, const float* pose44, int n, int H, int W,
+                         float threshold, int32_t* count_out, void* stream);
+
 /* ---- reconstruction evaluation (vista_slam/eval/eval_recon.py:108-206): world clouds, open3d's voxel_down_sample, the
  * moments of open3d's point-to-point ICP and the nearest-neighbour distances of the Chamfer metric.  Points are fp64
  * [n][3] device arrays.  Every reduction runs in a fixed order without floating-point atomics, so repeated runs are

@@ -253,6 +253,7 @@ def lib():
     L.sta_fusion_mesh_scratch_bytes.argtypes = [i64]
     L.sta_fusion_mesh_scratch_bytes.restype = sz
     L.sta_fusion_mesh.argtypes = [vp, i64, vp, vp, vp, c_float, c_float, i64, i64, vp, sz, vp, vp, vp, vp, vp]
+    L.sta_view_consistency.argtypes = [vp, vp, vp, i, i, i, c_float, vp, vp]
     L.sta_sort_scratch_bytes.argtypes = [i64]
     L.sta_sort_scratch_bytes.restype = sz
     L.sta_op_radix_sort.argtypes = [vp, vp, i64, i, vp, vp, vp, vp]

@@ -62,6 +62,16 @@ from .keyframe import KeyframeFrontend, add_views_group, encode_views, regress_f
 from .loop_detector import LoopDetector
 from .pose_graph import PoseGraphOpt
 
+def _min_consistent_views(k):
+    """min_consistent_views of render, extract_mesh, save_mesh and save_data_all: None or an integer in [0, 8] (the
+    most neighbours view_consistency counts); ValueError otherwise."""
+    if k is None:
+        return 0
+    if isinstance(k, bool) or not isinstance(k, (int, np.integer)) or not 0 <= k <= 8:
+        raise ValueError("min_consistent_views must be None or an integer in [0, 8], got %r" % (k,))
+    return int(k)
+
+
 def _msg(prefix, text):
     """print_msg (utils/slam_utils.py:448-450) without colours."""
     tqdm.write(prefix + text)
@@ -175,6 +185,7 @@ class OnlineSLAM:
         self.pgo_window_size = 2 * pgo_every
         self.pgo_route = None  # PoseGraphOpt's route: None (by size), "sparse" or "dense"
         self.pgo_background = False  # run due PGOs on a side stream while step goes on (see the module docstring)
+        self.consistency_thres = 0.05  # view_consistency's depth agreement threshold, in world units of the map
         self._pgo_run = None  # a background PGO not yet folded: (PoseGraphRun, its problem, nodes to replay)
         self._graph = None  # created at the first keyframe, when the map size is known
         self._kf_queue = []  # keyframe insertions not yet launched (_add_keyframe, insert_keyframes)
@@ -556,20 +567,46 @@ class OnlineSLAM:
             view["intri"] = ex["intri"][0].cpu()
         return view
 
-    def render(self, poses, K, size, point_radius=0, views=None, lines=None, background=(1.0, 1.0, 1.0)):
+    def render(self, poses, K, size, point_radius=0, views=None, lines=None, background=(1.0, 1.0, 1.0),
+               min_consistent_views=None):
         """Images of the map of `views` (a range; default: every view with a node) from cameras poses [C,4,4]
         (camera-to-world) with intrinsics K, drawn on the device by render.render_views: the confident points of
         save_data_all's PLY, z-buffered, and `lines` (render.camera_frusta, render.graph_segments) depth-tested with
         them.  Returns {rgb, depth, index} device tensors without a host synchronisation.  A background PGO is folded
         first if it has finished, never waited for (as get_view).  IndexError for a view without a node; nothing in
-        the session changes."""
+        the session changes.  min_consistent_views=k in [0, 8] keeps only the pixels whose view_consistency count
+        over `views` is at least k (None or 0: every confident pixel)."""
         from .render import render_views
-        return render_views(self._view_maps(views), self.conf_thres, poses, K, size, point_radius=point_radius,
-                            lines=lines, background=background)
+        k = _min_consistent_views(min_consistent_views)
+        maps = self._consistent_maps(self._view_maps(views), k)
+        return render_views(maps, self.conf_thres, poses, K, size, point_radius=point_radius, lines=lines,
+                            background=background)
 
-    def _view_maps(self, views):
+    def view_consistency(self, views=None):
+        """Multi-view depth consistency of the map of `views` (a range; default: every view with a node): int32
+        [len(views),H,W], per pixel the number of views of the range within 4 indices whose depth agrees with the
+        pixel's reprojection within consistency_thres -- utils.slam_utils.view_consistency_check of get_view's
+        depth (scaled, zero where conf < conf_thres), intri and pose of those views, bit for bit.  The window is
+        clipped at the range's ends.  No host synchronisation; a background PGO is folded first if it has finished,
+        never waited for (as render).  IndexError for a view without a node; nothing in the session changes."""
+        return self._consistency(self._view_maps(views, images=False))
+
+    def _consistency(self, maps):
+        """view_consistency of an exported `maps` dict; depth * scale is get_view's single float32 multiply."""
+        from .utils.slam_utils import view_consistency_check
+        depth = (maps["depth"] * maps["scale"][:, :, None]).masked_fill(maps["conf"] < self.conf_thres, 0.0)
+        return view_consistency_check(depth, maps["intri"], maps["pose"], self.consistency_thres)
+
+    def _consistent_maps(self, maps, k):
+        """maps with conf set to -inf where the view_consistency count is below k (maps unchanged for k = 0)."""
+        if k:
+            maps["conf"] = maps["conf"].masked_fill(self._consistency(maps) < k, float("-inf"))
+        return maps
+
+    def _view_maps(self, views, images=True):
         """The `maps` dict of render_views and fuse_views for `views` (a range; default: every view with a node), after
-        folding a background PGO that has finished (never waiting for one).  IndexError for a view without a node."""
+        folding a background PGO that has finished (never waiting for one).  IndexError for a view without a node.
+        images=False leaves the images out."""
         self._pgo_poll()
         if views is None:
             n = 0
@@ -584,24 +621,29 @@ class OnlineSLAM:
                     for k, s in (("pose", (0, 4, 4)), ("scale", (0, 1)), ("depth", (0, 1, 1)), ("conf", (0, 1, 1)),
                                  ("intri", (0, 3, 3)), ("images", (0, 3, 1, 1)))}
         maps = self._export(views.start, len(views), cloud=False)
-        maps["images"] = torch.stack(list(list.__iter__(self.imgs))[views.start:views.stop]).to(torch.float32)
+        if images:
+            maps["images"] = torch.stack(list(list.__iter__(self.imgs))[views.start:views.stop]).to(torch.float32)
         return maps
 
-    def extract_mesh(self, voxel_size, trunc=None, min_weight=1, views=None):
+    def extract_mesh(self, voxel_size, trunc=None, min_weight=1, views=None, min_consistent_views=None):
         """The map of `views` (a range; default: every view with a node) fused into a TSDF volume and meshed on the
         device by fusion.fuse_views: {bricks, tsdf, weight, color, vertices, vertex_colors, faces} device tensors.
         voxel_size in world units; trunc in (0, 4 voxel_size], default 4 voxel_size; min_weight: the views every
         corner of a meshed cube needs.  The volume is rebuilt from the current poses on every call, so it follows each
         PGO.  A background PGO is folded first if it has finished, never waited for (as render).  IndexError for a
-        view without a node; nothing in the session changes."""
+        view without a node; nothing in the session changes.  min_consistent_views as in render."""
         from .fusion import fuse_views
-        return fuse_views(self._view_maps(views), self.conf_thres, voxel_size, trunc=trunc, min_weight=min_weight)
+        k = _min_consistent_views(min_consistent_views)
+        maps = self._consistent_maps(self._view_maps(views), k)
+        return fuse_views(maps, self.conf_thres, voxel_size, trunc=trunc, min_weight=min_weight)
 
-    def save_mesh(self, output_folder, voxel_size, trunc=None, min_weight=1, views=None):
+    def save_mesh(self, output_folder, voxel_size, trunc=None, min_weight=1, views=None, min_consistent_views=None):
         """extract_mesh written to output_folder/mesh.ply (write_mesh_ply).  A pending background PGO is folded first
         (wait_pgo), as save_data_all does.  Returns the mesh's path."""
+        _min_consistent_views(min_consistent_views)
         self.wait_pgo()
-        mesh = self.extract_mesh(voxel_size, trunc=trunc, min_weight=min_weight, views=views)
+        mesh = self.extract_mesh(voxel_size, trunc=trunc, min_weight=min_weight, views=views,
+                                 min_consistent_views=min_consistent_views)
         os.makedirs(output_folder, exist_ok=True)
         path = os.path.join(output_folder, "mesh.ply")
         write_mesh_ply(path, mesh["vertices"].cpu().numpy(), mesh["vertex_colors"].cpu().numpy(),
@@ -617,8 +659,11 @@ class OnlineSLAM:
                       save_poses=True, save_images=True, save_scales=True,
                       save_depths=True, save_intrinsics=True,
                       save_confs=True, save_ply=True,
-                      gt_poses=None, gt_depths=None, gt_intrinsics=None):
-        """slam.py:338-421: the same files, keys, shapes and dtypes.  A pending background PGO is folded first (wait_pgo)."""
+                      gt_poses=None, gt_depths=None, gt_intrinsics=None, min_consistent_views=None):
+        """slam.py:338-421: the same files, keys, shapes and dtypes.  A pending background PGO is folded first (wait_pgo).
+        min_consistent_views=k in [0, 8] keeps in pointcloud.ply only the points whose view_consistency count over all
+        views is at least k, in the same order (None or 0: every point); the other files do not change."""
+        k = _min_consistent_views(min_consistent_views)
         self.wait_pgo()
         if not os.path.exists(output_folder):
             os.makedirs(output_folder)
@@ -644,7 +689,11 @@ class OnlineSLAM:
             np.save(f"{output_folder}/intrinsics.npy", ex["intri"].cpu().numpy())
         if save_ply:
             n = int(ex["count"].cpu())
-            write_ply(f"{output_folder}/pointcloud.ply", ex["points"][:n].cpu().numpy(), ex["colors"][:n].cpu().numpy())
+            points, colors = ex["points"][:n], ex["colors"][:n]
+            if k:  # the cloud is the conf > conf_thres pixels in (view, row, column) order
+                keep = self._consistency(ex)[ex["conf"] > self.conf_thres] >= k
+                points, colors = points[keep], colors[keep]
+            write_ply(f"{output_folder}/pointcloud.ply", points.cpu().numpy(), colors.cpu().numpy())
         if gt_poses is not None:
             np.save(f"{output_folder}/gt_poses.npy", np.array(gt_poses).astype(np.float32))
         if gt_depths is not None:

@@ -3,6 +3,8 @@ functions OnlineSLAM calls on the head outputs right after the STA boundary (SUR
 
     estimate_intrinsic_from_pts3d               slam_utils.py:8-79    (slam.py:184)
     estimate_scale_with_depth_and_confidence    slam_utils.py:168-190 (slam.py:224)
+    view_consistency_check                      slam_utils.py:346-419 (the map's multi-view depth consistency;
+                                                OnlineSLAM.view_consistency and min_consistent_views)
 
 plus `pointmap_consumers`, the fused form of slam.py:181-185 + pose_graph.py:41 (intrinsics, depth maps and the
 per-view confidence mean in ONE pass over the pointmaps, no host synchronisation), and `scale_and_confidence`
@@ -70,3 +72,29 @@ def scale_and_confidence(Di, Dj, ci, cj):
 def estimate_scale_with_depth_and_confidence(Di, Dj, ci, cj):
     """Drop-in for slam_utils.py:168-190: scalar s with Dj ~ s * Di."""
     return scale_and_confidence(Di, Dj, ci, cj)[0]
+
+
+def view_consistency_check(depth, intrinsics, poses, threshold=0.05):
+    """Drop-in for slam_utils.py:346-419: depth [n,H,W], intrinsics [n,3,3], poses [n,4,4] camera-to-world ->
+    int32 [n,H,W], per pixel the number of views within 4 indices whose depth agrees with the pixel's reprojection
+    within `threshold` (absolute).  Computed in float32 (inputs are cast) by one kernel launch (csrc/consistency.cu),
+    with the reference's quirks: a point projecting outside a neighbour samples 0 there, a non-finite projection never
+    agrees, and the window is clipped at the ends of the sequence.  No host synchronisation."""
+    depth = _f32_cuda(depth, "depth")
+    intrinsics = _f32_cuda(intrinsics, "intrinsics")
+    poses = _f32_cuda(poses, "poses")
+    if depth.dim() != 3:
+        raise RuntimeError("expected depth [n,H,W], got %s" % (tuple(depth.shape),))
+    n, H, W = depth.shape
+    if tuple(intrinsics.shape) != (n, 3, 3) or tuple(poses.shape) != (n, 4, 4):
+        raise RuntimeError("expected intrinsics [n,3,3] and poses [n,4,4] for depth [n,H,W]")
+    if intrinsics.device != depth.device or poses.device != depth.device:
+        raise RuntimeError("depth, intrinsics and poses must be on one device")
+    count = torch.empty((n, H, W), dtype=torch.int32, device=depth.device)
+    if n == 0:
+        return count
+    with torch.cuda.device(depth.device):
+        _lib.check(_lib.lib().sta_view_consistency(_lib.ptr(depth), _lib.ptr(intrinsics), _lib.ptr(poses), n, H, W,
+                                                   float(threshold), _lib.ptr(count), _lib.cur_stream()),
+                   "sta_view_consistency")
+    return count
