@@ -702,6 +702,29 @@ int sta_fusion_mesh(const int64_t* keys, int64_t num_bricks, const float* tsdf, 
                     size_t scratch_bytes, float* vertices_out, float* vertex_colors_out, int32_t* faces_out,
                     int64_t* counts_out, void* stream);
 
+/* ---- ray casting of the fused volume (fusion.raycast, OnlineSLAM.render_surface) ---- */
+/* Ray-cast a volume exactly as sta_fusion_integrate returns it -- keys [B] (sorted, distinct), tsdf / weight
+ * [B][8][8][8] ([b][z][y][x]) and color [B][8][8][8][3], samples at (float(i) v, float(j) v, float(k) v) -- from C
+ * cameras: c2w [C][4][4] camera-to-world, K [C][3][3] (fx = K[0], cx = K[2], fy = K[4], cy = K[5]).  Pixel (col, row)
+ * is the ray o + z R ((col - cx) / fx, (row - cy) / fy, 1), z the camera depth.  A point lies in cell floor(p / v);
+ * a cell is valid when its 8 corner samples exist with weight >= min_weight (sta_fusion_mesh's rule), and there the
+ * field and colour are the trilinear interpolants.  The march covers the ray's overlap with the bricks' bounding box
+ * (computed on the device) from z >= near, in steps of half a voxel of world length, and jumps over absent bricks.
+ * The hit is the first pair of consecutive valid samples with T > 0 then T <= 0 (surfaces seen from behind are passed
+ * through), refined by 16 bisection steps and a final secant.  Outputs per pixel: depth_out [C][Ho][Wo] (the hit's z, 0 on
+ * a miss), normal_out [C][Ho][Wo][3] (normalised gradient of the interpolant, world frame, 0 on a miss), color_out
+ * [C][Ho][Wo][3] (the interpolated colour) and rgb_out [C][Ho][Wo][3] (color (0.3 + 0.7 max(0, -n . r)), r the unit ray
+ * direction), both background (a host float[3]) on a miss.  One thread per pixel, no atomics in the march: the same
+ * bits on every call and for a camera alone or among others.  scratch: sta_raycast_scratch_bytes(B), 16-byte aligned.
+ * Two launches (the box, the march), no host synchronisation.  Refused before any launch: C, Ho or Wo outside
+ * [1, 8192], B outside [0, STA_FUSION_MAX_BRICKS], voxel <= 0 or not finite, min_weight < 1, near <= 0 or not finite,
+ * a null input or output, a small or misaligned scratch, host memory. */
+size_t sta_raycast_scratch_bytes(int64_t num_bricks);
+int sta_raycast(const int64_t* keys, int64_t num_bricks, const float* tsdf, const float* weight, const float* color,
+                float voxel, float min_weight, const float* c2w, const float* K, int C, int Ho, int Wo, float near,
+                const float* background, void* scratch, size_t scratch_bytes, float* rgb_out, float* color_out,
+                float* depth_out, float* normal_out, void* stream);
+
 /* ---- multi-view depth consistency of the map (slam_utils.view_consistency_check, OnlineSLAM.view_consistency) ---- */
 /* vista_slam/utils/slam_utils.py:346-419 for n views: depth [n][H][W], intri [n][3][3], pose44 [n][4][4]
  * camera-to-world, all fp32.  count_out [n][H][W] (device int32): for pixel (x, y) of view i, the number of views j in

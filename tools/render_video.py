@@ -1,6 +1,7 @@
 """The frames of the reference's scripts/video.py, drawn on the GPU by the map renderer (vista_slam_b200/render.py).
 
     python tools/render_video.py FOLDER --out DIR [--size 480x720] [--radius 0] [--follow] [--camera w2c.npy]
+                                 [--surface VOXEL [--min-weight N]]
 
 FOLDER holds what OnlineSLAM.save_data_all and log_intermediate_results write: trajectory{_k}.npy, scales{_k}.npy,
 depths.npy, confs.npz, intrinsics.npy, images.npy and view_graph.npz.  Frame v shows views 0..v with the poses of the
@@ -10,6 +11,9 @@ an extra frame v_pgo shows the new trajectory.  Cameras: --follow is video.py's 
 [0, 0.3, 5]) composed with the current view's world-to-camera; --camera is a fixed 4x4 world-to-camera; by default a
 fixed camera above the camera centres looks along their mean up axis (-y of the poses), backed off until every centre
 is in frame.  Colours are the images' (not video.py's /1.5 shading); frames are PNG when cv2 imports, .npy otherwise.
+With --surface VOXEL each frame draws, instead of point splats, the map fused into a TSDF volume of that voxel size
+and ray-cast with a headlight (fusion.fuse_volume, fusion.raycast; min_weight --min-weight); the lines are drawn by
+render_views over the same map with every point masked out and kept where they are nearer than the surface.
 Prints each frame's render time (device time, the call synchronised)."""
 import argparse
 import glob
@@ -22,6 +26,7 @@ import torch
 
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), ".."))
 
+from vista_slam_b200.fusion import fuse_volume, raycast  # noqa: E402
 from vista_slam_b200.render import camera_frusta, concat_lines, graph_segments, render_views  # noqa: E402
 
 CAMERA_COLOR = (0.6, 0.8, 1.0)
@@ -59,6 +64,18 @@ def overhead_w2c(traj, K, Ho, Wo):
     return w2c
 
 
+def surface_frame(maps, thres, c2w, K, size, lines, voxel, min_weight):
+    """The fused surface of maps ray-cast from c2w [1,4,4], with lines drawn by render_views over the same map with
+    every point masked out (conf -inf), each pixel taking the nearer of the two."""
+    vol = fuse_volume(maps, thres, voxel)
+    surf = raycast(vol["bricks"], vol["tsdf"], vol["weight"], vol["color"], voxel, c2w, K, size, min_weight=min_weight)
+    bare = dict(maps, conf=torch.full_like(maps["conf"], float("-inf")))
+    ln = render_views(bare, thres, c2w, K, size, lines=lines)
+    front = (ln["depth"] > 0) & ((surf["depth"] == 0) | (ln["depth"] < surf["depth"]))
+    return {"rgb": torch.where(front[..., None], ln["rgb"], surf["rgb"]),
+            "depth": torch.where(front, ln["depth"], surf["depth"])}
+
+
 def main(argv=None):
     ap = argparse.ArgumentParser()
     ap.add_argument("folder")
@@ -67,6 +84,8 @@ def main(argv=None):
     ap.add_argument("--radius", type=int, default=0)
     ap.add_argument("--follow", action="store_true")
     ap.add_argument("--camera", default=None)
+    ap.add_argument("--surface", type=float, default=None, metavar="VOXEL")
+    ap.add_argument("--min-weight", type=float, default=1.0)
     a = ap.parse_args(argv)
     Ho, Wo = (int(x) for x in a.size.lower().split("x"))
     F = a.folder
@@ -126,8 +145,11 @@ def main(argv=None):
             w2c = overhead
         torch.cuda.synchronize()
         t0 = time.perf_counter()
-        out = render_views(maps, thres, np.linalg.inv(w2c)[None], K, (Ho, Wo), point_radius=a.radius,
-                           lines=concat_lines(*parts))
+        c2w = np.linalg.inv(w2c)[None]
+        if a.surface is None:
+            out = render_views(maps, thres, c2w, K, (Ho, Wo), point_radius=a.radius, lines=concat_lines(*parts))
+        else:
+            out = surface_frame(maps, thres, c2w, K, (Ho, Wo), concat_lines(*parts), a.surface, a.min_weight)
         torch.cuda.synchronize()
         ms = (time.perf_counter() - t0) * 1e3
         rgb = out["rgb"][0].cpu().numpy()

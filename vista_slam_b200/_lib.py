@@ -253,6 +253,10 @@ def lib():
     L.sta_fusion_mesh_scratch_bytes.argtypes = [i64]
     L.sta_fusion_mesh_scratch_bytes.restype = sz
     L.sta_fusion_mesh.argtypes = [vp, i64, vp, vp, vp, c_float, c_float, i64, i64, vp, sz, vp, vp, vp, vp, vp]
+    L.sta_raycast_scratch_bytes.argtypes = [i64]
+    L.sta_raycast_scratch_bytes.restype = sz
+    L.sta_raycast.argtypes = [vp, i64, vp, vp, vp, c_float, c_float, vp, vp, i, i, i, c_float, POINTER(c_float), vp, sz,
+                              vp, vp, vp, vp, vp]
     L.sta_view_consistency.argtypes = [vp, vp, vp, i, i, i, c_float, vp, vp]
     L.sta_sort_scratch_bytes.argtypes = [i64]
     L.sta_sort_scratch_bytes.restype = sz

@@ -18,7 +18,7 @@ OBJDIR = os.path.join(CSRC, "build")
 STAMP = os.path.join(OBJDIR, "nvcc_flags.txt")
 SOURCES = ["host_util.cu", "gemm.cu", "attention.cu", "kernels.cu", "pointmap.cu", "preprocess.cu", "pose_graph.cu",
            "pose_graph_sparse.cu", "flow.cu", "orb.cu", "bow.cu", "slam_graph.cu", "recon.cu", "render.cu", "fusion.cu",
-           "consistency.cu", "runtime.cu"]
+           "raycast.cu", "consistency.cu", "runtime.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
     "-std=c++17", "-O3", "-lineinfo",

@@ -5,7 +5,7 @@
 //              point p (cloud.cuh); the bricks floor((p -+ tau) / 8v) per axis that the cube [p - tau, p + tau] touches
 //              (at most 2 per axis since tau <= 4v) are deduplicated in a shared-memory hash per 256-pixel tile, counted,
 //              scanned over the tiles and written; then recon.cu's radix sort (sta_op_radix_sort) and a unique pass.
-//              A key is the three brick coordinates biased by 2^20 in 21 bits each, z above y above x.
+//              A key is the three brick coordinates biased by 2^20 in 21 bits each, z above y above x (brick.cuh).
 //   integrate  brick_views_kernel: one bit per (brick, view) for the views whose frustum and depth range can reach
 //              the brick, tested on the brick's box grown by one voxel (conservative: it never drops a view that
 //              reaches a sample); integrate_kernel: one CTA per brick, one thread per sample, the brick's views in
@@ -20,6 +20,7 @@
 #include <stdint.h>
 
 #include "../../include/sta_b200.h"
+#include "brick.cuh"
 #include "cloud.cuh"
 #include "host_util.h"
 #define STA_MC_SPACE __constant__
@@ -28,23 +29,10 @@
 namespace sta {
 namespace {
 
-constexpr int kBrick = STA_FUSION_BRICK;
-constexpr int kSamples = kBrick * kBrick * kBrick;  // 512
-constexpr int kBias = 1 << 20;                      // brick coordinates lie in [-2^20, 2^20 - 1]
+constexpr int kSamples = kBrickSamples;            // 512
 constexpr int kTileSlots = 4096;                    // hash slots per 256-pixel tile: 8 keys per pixel at most
 constexpr int kUniqueChunk = 2048;                  // sorted keys per unique block
 constexpr unsigned long long kEmptyKey = ~0ull;     // above every 63-bit key
-
-__host__ __device__ __forceinline__ unsigned long long brick_key(int bx, int by, int bz) {
-  return (static_cast<unsigned long long>(bz + kBias) << 42) | (static_cast<unsigned long long>(by + kBias) << 21) |
-         static_cast<unsigned long long>(bx + kBias);
-}
-
-__device__ __forceinline__ void key_brick(unsigned long long k, int& bx, int& by, int& bz) {
-  bx = static_cast<int>(k & 0x1fffff) - kBias;
-  by = static_cast<int>((k >> 21) & 0x1fffff) - kBias;
-  bz = static_cast<int>((k >> 42) & 0x1fffff) - kBias;
-}
 
 struct MapArgs {
   const float *depth, *conf, *pose, *scale, *intri, *imgs, *w2c;
@@ -286,17 +274,6 @@ struct MeshArgs {
   const float *tsdf, *weight, *color;
   float vox, min_weight;
 };
-
-// index of key k in the sorted keys, or -1
-__device__ __forceinline__ int find_brick(const int64_t* keys, long long B, long long k) {
-  long long lo = 0, hi = B;
-  while (lo < hi) {
-    const long long mid = (lo + hi) >> 1;
-    if (keys[mid] < k) lo = mid + 1;
-    else hi = mid;
-  }
-  return lo < B && keys[lo] == k ? static_cast<int>(lo) : -1;
-}
 
 // threads 0..7 of the block: nb[o] = the brick at offset (o & 1, o >> 1 & 1, o >> 2) from brick b, or -1
 __device__ __forceinline__ void load_neighbours(const MeshArgs& a, int b, int* nb) {

@@ -637,6 +637,26 @@ class OnlineSLAM:
         maps = self._consistent_maps(self._view_maps(views), k)
         return fuse_views(maps, self.conf_thres, voxel_size, trunc=trunc, min_weight=min_weight)
 
+    def render_surface(self, poses, K, size, voxel_size, trunc=None, min_weight=1, views=None, min_consistent_views=None,
+                       background=(1.0, 1.0, 1.0)):
+        """Images of the fused surface of `views` (a range; default: every view with a node) from cameras poses
+        [C,4,4] (camera-to-world) with intrinsics K ([3,3] or [C,3,3]) at size (Ho, Wo): the map fused as
+        extract_mesh fuses it (fusion.fuse_volume) and ray-cast on the device (fusion.raycast), without meshing.
+        Returns {rgb, color [C,Ho,Wo,3], depth [C,Ho,Wo], normal [C,Ho,Wo,3]} device tensors.  The only host
+        synchronisations are fusion's two counts.  voxel_size, trunc, min_weight and min_consistent_views as in
+        extract_mesh; a background PGO is folded first if it has finished, never waited for (as render).  IndexError
+        for a view without a node; nothing in the session changes.  Arguments are checked before any work
+        (ValueError)."""
+        from .fusion import _check_cameras, _fuse, _min_weight, _raycast, _voxel_args
+        k = _min_consistent_views(min_consistent_views)
+        _voxel_args(voxel_size, trunc)
+        mw = _min_weight(min_weight)
+        dev = self.device if self._graph is None else self._graph.device
+        cams = _check_cameras(poses, K, size, 1e-3, background, dev)
+        maps = self._consistent_maps(self._view_maps(views), k)
+        vol, keys, vox = _fuse(maps, self.conf_thres, voxel_size, trunc, 2 ** 20, mw)
+        return _raycast(keys, vol["tsdf"], vol["weight"], vol["color"], vox, mw, *cams)
+
     def save_mesh(self, output_folder, voxel_size, trunc=None, min_weight=1, views=None, min_consistent_views=None):
         """extract_mesh written to output_folder/mesh.ply (write_mesh_ply).  A pending background PGO is folded first
         (wait_pgo), as save_data_all does.  Returns the mesh's path."""
